@@ -12,10 +12,16 @@ once, outside the timed region - the regime of the reference's own harness, demo
 edges/sec = (2 * E) / step time: every layer pass streams all E input edges (appended self loops are NOT counted).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--config headline|cfg1..cfg5] [--scale S]
+                    [--dump-outputs DIR]
 
 --config selects one of BASELINE.json's configs (default: headline = the configuration the metric is quoted on); every
 config prints the same JSON contract with its own roofline.  --gpus N > 1 (under torchrun) runs the headline step
 destination-partitioned over N GPUs through the same tfg.layers calls; cfg5 (papers100M shape) needs 8 GPUs.
+
+--dump-outputs DIR writes what the last timed step returned as DIR/<name>.npy, float32: the whole array when it is small,
+else the same seeded sample of rows on every run (60 MiB in all at most).  The inputs depend only on the arguments, so two
+builds can be compared output for output.  Only the single-GPU path dumps: the flag is refused with --impl reference, with
+several GPUs and with cfg5.
 
 --impl reference times the reference's op sequence on the host CPU cores (oracle/torch_cpu_port.py; TensorFlow and
 tf_sparse cannot be installed offline) on a bounded sample of the same workload.
@@ -73,7 +79,16 @@ def parse_args():
                     help="reference arm: graph scaled down by this factor (0 = auto: about two minutes of CPU work in total)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-e2e", action="store_true")
-    return ap.parse_args()
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step as DIR/<name>.npy (float32; a seeded row sample past 60 MiB in all)")
+    args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
+    if args.dump_outputs and (args.impl != "ours" or args.gpus > 1 or int(os.environ.get("WORLD_SIZE", "1")) > 1
+                              or CONFIGS[args.config]["kind"] == "gcn_partitioned"):
+        ap.error("--dump-outputs writes the outputs of the single-GPU path: it needs --impl ours, one GPU and a config "
+                 "other than cfg5")
+    return args
 
 
 # ---- synthetic workload --------------------------------------------------------------------------------------------
@@ -101,8 +116,8 @@ def glorot(shape, seed):
 
 
 class ClockSampler(object):
-    """SM clock / throttle reasons sampled DURING the timed region (B200_PROFILING.md): NVML in a background thread every
-    ~2 ms (nvidia-smi -lms cannot resolve a 50 ms region); falls back to one nvidia-smi query if NVML is unavailable."""
+    """SM clock / throttle reasons sampled DURING the timed region: NVML in a background thread every ~2 ms (nvidia-smi -lms
+    cannot resolve a 50 ms region); reports "nvml unavailable" when pynvml cannot be imported."""
 
     def __init__(self, index):
         self.index = index
@@ -170,7 +185,7 @@ def measured_peak_gbs():
             return float(json.load(open(path))["hbm_gbs"]), "MEASURED_PEAKS.json hbm_gbs"
         except Exception:
             pass
-    return 6650.0, "fallback 6.65 TB/s (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet: 3.35 TB/s HBM3 (not measured)"
 
 
 # ---- reference arm (CPU) ---------------------------------------------------------------------------------------------
@@ -338,7 +353,7 @@ def workload_config(args, world):
                        "warm graph.cache".format(cfg["what"], n, e, cfg["features"]),
            "name": args.config, "nodes": n, "edges": e, "features": cfg["features"], "units": UNITS, "heads": HEADS,
            "edges_per_step": passes * e, "parallelism": "single GPU" if world == 1 else "dst-partitioned x{}".format(world),
-           "l2_policy": "working set (gathered rows + CSR, GBs) exceeds the 126 MB L2; no explicit flush"}
+           "l2_policy": "working set (gathered rows + CSR, GBs) exceeds the 50 MB L2; no explicit flush"}
     if cfg["kind"] == "gcn2":
         out["l2_policy"] = "Cora-sized working set fits in L2: this config is latency/launch bound by construction"
     return out
@@ -406,9 +421,7 @@ def run_e2e(args, device, x_host, step_fn, n_out_rows, edges_per_layer, barrier=
 
 
 TIMED_CALLS = ("tfgk_gat_fused_f32", "tfgk_spmm_f32", "tfgk_gemm_f32", "tfgk_gemm_proj_f32")
-# dram__bytes_read.sum + dram__bytes_write.sum per launch from the committed `ncu --set full` capture of round 2 (constants, NOT
-# live counters): profiles/r2_ncu_full_headline_kernels.json; only valid for the full-size products-shape graph
-NCU_TRAFFIC = {"gat": 128185916000, "spmm_d128": 63372534000}
+DUMP_BYTES = 60 << 20                                     # whole dump, .npy headers aside: under 64 MB
 
 
 def build_workload(args, tfg, device):
@@ -432,22 +445,23 @@ def build_workload(args, tfg, device):
     gat_bytes = e_loop * (4 * UNITS + 4 * UNITS + 4) + n * (4 * UNITS + 4 * UNITS + 8)       # DESIGN.md K3
     proj_bytes = lambda cols: n * F * 4 + n * cols * 4                                       # noqa: E731
     kernels = {}
+    names = []                                             # one name per array the step returns (--dump-outputs)
     if kind in ("gcn+gat", "gcn", "gat"):
         layers = []
         if "gcn" in kind:
             gcn = tfg.layers.GCN(UNITS, activation=tfg.nn.relu, seed=2)
             gcn.build_cache_for_graph(graph)                   # normalised adjacency + CSR (one-off, untimed)
             layers.append(lambda xd: gcn([xd, graph.edge_index, graph.edge_weight], cache=graph.cache))
-            kernels["gcn_spmm"] = ("tfgk_spmm_f32", spmm_bytes(UNITS, e_loop, True), "spmm_gather4_kernel<0,3> (tfgk_spmm_f32)",
-                                   NCU_TRAFFIC["spmm_d128"] if args.config == "headline" and args.scale == 1.0 else None)
-            kernels["gcn_projection"] = ("tfgk_gemm_f32", proj_bytes(UNITS), "gemm_proj_ts_kernel<STAGES> reached through tfgk_gemm_f32", None)
+            kernels["gcn_spmm"] = ("tfgk_spmm_f32", spmm_bytes(UNITS, e_loop, True), "spmm_tma4_kernel<false,3> (tfgk_spmm_f32)", None)
+            kernels["gcn_projection"] = ("tfgk_gemm_f32", proj_bytes(UNITS), "gemm_proj_kernel<STAGES> reached through tfgk_gemm_f32", None)
+            names.append("gcn")
         if "gat" in kind:
             gat = tfg.layers.GAT(UNITS, num_heads=HEADS, activation=tfg.nn.relu, seed=3)
             layers.append(lambda xd: gat([xd, graph.edge_index], cache=graph.cache))
-            kernels["gat_fused"] = ("tfgk_gat_fused_f32", gat_bytes, "gat_gather4_kernel<2> (tfgk_gat_fused_f32)",
-                                    NCU_TRAFFIC["gat"] if args.config == "headline" and args.scale == 1.0 else None)
+            kernels["gat_fused"] = ("tfgk_gat_fused_f32", gat_bytes, "gat_tma4_kernel<2> (tfgk_gat_fused_f32)", None)
             kernels["gat_projections"] = ("tfgk_gemm_proj_f32", proj_bytes(3 * UNITS),
-                                          "gemm_proj_ts_kernel<STAGES>, Q|K|V in one launch (tfgk_gemm_proj_f32)", None)
+                                          "gemm_proj_kernel<STAGES>, Q|K|V in one launch (tfgk_gemm_proj_f32)", None)
+            names.append("gat")
         step = lambda xd: tuple(f(xd) for f in layers)     # noqa: E731
         passes = len(layers)
     elif kind == "gcn2":
@@ -463,6 +477,7 @@ def build_workload(args, tfg, device):
         l1.build_cache_for_graph(graph)
         step = lambda xd: (l2([l1([pattern.with_value(xd), graph.edge_index, graph.edge_weight], cache=graph.cache),     # noqa: E731
                                graph.edge_index, graph.edge_weight], cache=graph.cache),)
+        names = ["gcn2"]
         nnz = int(x_host.numel())
         kernels["gcn_spmm"] = ("tfgk_spmm_f32", spmm_bytes(16, e_loop, True) + spmm_bytes(7, e_loop, True)
                                + nnz * (4 * 16 + 8) + n * (4 * 16 + 8),
@@ -479,6 +494,7 @@ def build_workload(args, tfg, device):
             loss = (out * g).sum()
             loss.backward()
             return (loss.detach().reshape(1), xg.grad)
+        names = ["loss", "x_grad"]
         # forward mean aggregation (unweighted) + backward aggregation on the transposed CSR (weights 1/deg)
         kernels["sage_spmm"] = ("tfgk_spmm_f32", spmm_bytes(F, E, False) + spmm_bytes(F, E, True),
                                 "spmm kernels at D=100, forward + transposed backward (tfgk_spmm_f32)", None)
@@ -486,7 +502,23 @@ def build_workload(args, tfg, device):
         passes = 1
     else:
         raise ValueError(kind)
-    return {"x_host": x_host, "x": x, "step": step, "E": E, "n": n, "passes": passes, "kernels": kernels, "graph": graph}
+    return {"x_host": x_host, "x": x, "step": step, "E": E, "n": n, "passes": passes, "kernels": kernels, "graph": graph,
+            "names": names}
+
+
+def dump_outputs(directory, names, outputs):
+    """Writes each output of a step as <directory>/<name>.npy in float32.  An output larger than its share of DUMP_BYTES is
+    cut to a sample of rows drawn with a fixed seed (sorted, the same rows on every run of the same configuration)."""
+    os.makedirs(directory, exist_ok=True)
+    share = DUMP_BYTES // max(len(outputs), 1)
+    for name, out in zip(names, outputs):
+        t = out.detach().float()
+        if t.numel() * 4 > share:
+            row_bytes = 4 * (t.numel() // t.shape[0])
+            keep = max(1, share // row_bytes)
+            rows = np.sort(np.random.RandomState(0).choice(t.shape[0], size=keep, replace=False))
+            t = t[torch.from_numpy(rows).to(t.device)]
+        np.save(os.path.join(directory, name + ".npy"), t.cpu().numpy().astype(np.float32))
 
 
 def run_ours(args, rank, world, local_rank):
@@ -531,13 +563,16 @@ def run_ours(args, rank, world, local_rank):
     torch.cuda.synchronize()
     ev[0].record()
     for _ in range(args.steps):
-        step(x)
+        outputs = step(x)
     ev[1].record()
     torch.cuda.synchronize()
     clocks = sampler.stop()
     _ffi.set_trace(None)
     ms_step = ev[0].elapsed_time(ev[1]) / args.steps
     value = wl["passes"] * E / (ms_step * 1e-3)
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, wl["names"], outputs)
+    del outputs
 
     call_ms = {name: float(np.sum(trace.elapsed_ms(name))) / args.steps for name in TIMED_CALLS}
     call_n = {name: trace.counts.get(name, 0) / args.steps for name in TIMED_CALLS}
@@ -555,8 +590,7 @@ def run_ours(args, rank, world, local_rank):
     d = fams[dominant]
     roofline = {"bound": "hbm", "kernel": d["kernel"], "achieved": d["achieved"], "peak": peak, "unit": "GB/s",
                 "frac": d["frac"], "traffic": d["traffic"],
-                "traffic_source": ("constant copied from the committed ncu --set full capture of round 2 "
-                                   "(profiles/r2_ncu_full_headline_kernels.json), not measured in this run") if d["traffic"] else None,
+                "traffic_source": None,
                 "peak_source": peak_src, "algorithmic_bytes": d["algorithmic_bytes_per_step"] / max(d["launches_per_step"], 1),
                 "kernel_ms": d["ms_per_step"] / max(d["launches_per_step"], 1),
                 "launches_per_step": d["launches_per_step"],

@@ -1,9 +1,9 @@
 /*
- * tfgk.h - C ABI of the B200 (sm_100a) message-passing kernel backend for tf_geometric's hot path.
+ * tfgk.h - C ABI of the H100 (sm_90a) message-passing kernel backend for tf_geometric's hot path.
  *
  * The reference (CrawlScript/tf_geometric @4539f11) has NO native FFI: its "operator API" for this path is a set
  * of Python functions built on stock TensorFlow ops and the tf_sparse package.  Each entry point below therefore
- * cites the reference Python interface (file:line, relative to /root/reference/tf_geometric) whose arithmetic it
+ * cites the reference Python interface (file:line, relative to tf_geometric/ of the reference, CrawlScript/tf_geometric) whose arithmetic it
  * replaces; INTEGRATION.md shows the ctypes binding a tf_geometric maintainer would add at each of those sites.
  *
  * Conventions
@@ -47,7 +47,7 @@ enum tfgk_sample_padding { TFGK_SAMPLE_NO_PADDING = 0, TFGK_SAMPLE_PADDING = 1, 
 
 int tfgk_version(void);
 const char *tfgk_last_error(void);
-/* SM count and compute capability of the current device (used by the host side to refuse non-sm_100 parts). */
+/* SM count and compute capability of the current device. */
 int tfgk_device_info(int *sm_count, int *cc_major, int *cc_minor);
 
 /* ---- integer edge preprocessing (bit-exact) ------------------------------------------------------------------ */
@@ -178,7 +178,7 @@ int tfgk_gemm_f32(const float *A, int64_t lda, int transA, const float *B, int64
 /* Several projections of the same input in ONE launch (round 2): for every column block b < n_blocks
  *   C_b[M, ncols_b] = act_b( A[M, K] @ B_b[K, ncols_b] + bias_b ),   ncols_b <= 128, n_blocks <= 4,
  * e.g. the three projections of gat.py:52,61,70 (Q | K | V) or gcn.py:272 next to them; A is read from HBM once.
- * Same 3xTF32 tcgen05 arithmetic as tfgk_gemm_f32's tensor-core path (bit-identical results).
+ * Same 3xTF32 wgmma arithmetic as tfgk_gemm_f32's tensor-core path (bit-identical results).
  * A may live in n_parts <= 8 row blocks of part_rows rows each (a multiple of 128 when n_parts > 1), part i at
  * A_parts[i]: with the other ranks' buffers mapped through tfgk_peer_open this is the fused all-gather -> GEMM of the
  * partitioned path (rows are pulled over NVLink tile by tile while earlier tiles are multiplied); the walk starts at
@@ -215,8 +215,8 @@ int tfgk_peer_export(void *ptr, void *handle_out);
 int tfgk_peer_open(const void *handle, void **ptr);
 int tfgk_peer_close(void *ptr);
 /* Copies `bytes` (a multiple of 16, both pointers 16-byte aligned) from a peer-mapped buffer into local memory.
- * max_ctas > 0: copy kernel with that many CTAs (wide contiguous loads; ~7.5 GB/s per CTA, 663 GB/s from 148 CTAs on);
- * max_ctas = 0: the kernel on 148 CTAs;  max_ctas < 0: the copy engine (cudaMemcpyAsync on `stream`, 741 GB/s, no SMs). */
+ * max_ctas > 0: copy kernel with that many CTAs (wide contiguous loads);  max_ctas = 0: the copy kernel on one CTA per SM
+ * of the current device;  max_ctas < 0: the copy engine (cudaMemcpyAsync on `stream`; takes no SMs). */
 int tfgk_peer_pull(const void *src, void *dst, int64_t bytes, int32_t max_ctas, void *stream);
 int tfgk_peer_barrier(uint32_t *const *flags, int32_t rank, int32_t world, uint32_t value, int32_t timeout_ms, void *stream);
 

@@ -8,7 +8,7 @@
  * Parity status: "unpinned" for TensorFlow/tf_sparse kernel internals (see the header of tfg_oracle.py);
  * tests/test_oracle.py checks this file bit-for-bit against the numpy restatement.
  *
- * References (relative to /root/reference/tf_geometric):
+ * References (relative to tf_geometric/ of the reference, CrawlScript/tf_geometric):
  *   nn/kernel/map_reduce.py:15-16,27-28,38-42,45-73   nn/kernel/segment.py:26-33   nn/conv/gcn.py:221-222
  *   nn/conv/gat.py:73-114
  */

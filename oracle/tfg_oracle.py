@@ -7,9 +7,9 @@ CPU ORACLE (numpy) for the tf_geometric message-passing hot path.
   ``bench.py`` use it, and only as the checker / the timed CPU arm.
 
 PARITY PINNING STATUS
-  The reference (/root/reference, CrawlScript/tf_geometric @4539f11) ships *no* tests and no golden vectors for
+  The reference (CrawlScript/tf_geometric @4539f11) ships *no* tests and no golden vectors for
   this path, and neither TensorFlow nor the un-vendored dependency ``tf_sparse`` (setup.py:25, ">= 0.0.17") can be
-  imported in the authoring container.  The oracle is pinned two ways (see tests/golden/README.md):
+  imported here.  The oracle is pinned two ways (see tests/golden/README.md):
     (1) tests/golden/ref_exec_*.npz - the reference's OWN Python functions (nn/kernel/*.py, nn/conv/{gcn,gat,
         graph_sage,appnp}.py, utils/graph_utils.py) executed here over a numpy shim of the TF ops they call
         (tools/gen_golden_from_reference.py).  That pins call order, quirks and the in-repo arithmetic; it does
@@ -27,7 +27,7 @@ TF op semantics restated here (TensorFlow 2.x CPU kernels):
   * tf.unique                                   -> first-occurrence order, plus inverse index
 
 All floating point arithmetic is float32, indices int32 (data/graph.py:22-23,58-66).
-Every function cites the reference file:line it restates (paths relative to /root/reference/tf_geometric).
+Every function cites the reference file:line it restates (paths relative to tf_geometric/ of the reference, CrawlScript/tf_geometric).
 """
 import numpy as np
 
@@ -304,7 +304,7 @@ def csr_build(row, col, num_rows):
 
 
 # --------------------------------------------------------------------------------------------------------------
-# tf_sparse.SparseMatrix  [UNVERIFIED restatement - the package is not under /root/reference]
+# tf_sparse.SparseMatrix  [UNVERIFIED restatement - the package is not part of the reference]
 # --------------------------------------------------------------------------------------------------------------
 
 class SparseMatrix(object):

@@ -65,3 +65,12 @@ def test_gpu_arm_refuses_to_run_without_a_gpu():
     out = subprocess.run([sys.executable, "bench.py", "--steps", "1", "--warmup", "1"], cwd=ROOT, capture_output=True,
                          text=True, timeout=300)
     assert out.returncode != 0 and out.stdout.strip() == "" and "no CPU fallback" in out.stderr
+
+
+def test_dump_outputs_is_refused_where_it_cannot_be_honoured():
+    """--dump-outputs writes the single-GPU path's outputs; the CPU arm, several GPUs and cfg5 refuse it instead of ignoring it."""
+    for extra in (["--impl", "reference"], ["--gpus", "2"], ["--config", "cfg5"]):
+        out = subprocess.run([sys.executable, "bench.py", "--steps", "1", "--dump-outputs", "unused_dir"] + extra, cwd=ROOT,
+                             capture_output=True, text=True, timeout=300)
+        assert out.returncode != 0 and out.stdout.strip() == "" and "--dump-outputs" in out.stderr, extra
+        assert not os.path.exists(os.path.join(ROOT, "unused_dir"))

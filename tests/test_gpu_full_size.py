@@ -1,7 +1,7 @@
 # coding=utf-8
 """Parity at BASELINE.json's full size (synthetic ogbn-products shape: 2,449,029 nodes, 123,718,280 edges, D=128)
 through size-independent properties plus bit-exact spot checks of sampled destination rows against the oracle's
-arithmetic (sequential fp32 in edge order), so the whole thing runs in seconds on the GPU box."""
+arithmetic (sequential fp32 in edge order), so the whole thing runs in seconds on the GPU."""
 import numpy as np
 import pytest
 import torch

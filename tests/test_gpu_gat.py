@@ -131,7 +131,7 @@ def test_gat_hub_rows_sliced_softmax_merge():
 
 @pytest.mark.parametrize("stages", ["2", "3", "4"])
 def test_gat_tma_gather4_variant_is_bit_identical(stages, monkeypatch):
-    """K3 with the K|V rows of four neighbours fetched by one TMA tile::gather4 per round: same bits as the cp.async ring,
+    """K3 with the K|V rows of four neighbours fetched by four TMA bulk copies per round: same bits as the cp.async ring,
     ragged rows, a hub row cut into slices, with and without the training statistics."""
     rs = np.random.RandomState(5)
     n, heads, a = 3000, 8, 128
@@ -143,7 +143,7 @@ def test_gat_tma_gather4_variant_is_bit_identical(stages, monkeypatch):
     bias = dev(rs.randn(a).astype(np.float32))
     monkeypatch.setenv("TFGK_GAT_IMPL", "async")
     want = ops.gat_fused(csr, q, kv[:, :a], kv[:, a:], heads, bias=bias, act=ops.ACT_RELU)
-    monkeypatch.setenv("TFGK_GAT_IMPL", "gather4:" + stages)
+    monkeypatch.setenv("TFGK_GAT_IMPL", "tma:" + stages)
     got = ops.gat_fused(csr, q, kv[:, :a], kv[:, a:], heads, bias=bias, act=ops.ACT_RELU)
     assert torch.equal(got, want)
     sep_k, sep_v = kv[:, :a].contiguous(), kv[:, a:].contiguous()          # separate buffers: falls back to the cp.async ring

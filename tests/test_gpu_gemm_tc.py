@@ -1,5 +1,5 @@
 # coding=utf-8
-"""K4 tensor-core path (tcgen05, 3xTF32 split): fp32-level accuracy against float64, far inside the 1e-4 gate that a
+"""K4 tensor-core path (wgmma, 3xTF32 split): fp32-level accuracy against float64, far inside the 1e-4 gate that a
 single TF32 pass would miss.  Shapes cover the projections of the hot path and the ragged edges (M, N, K tails)."""
 import os
 

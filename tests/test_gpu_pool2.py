@@ -168,7 +168,7 @@ def test_pools_over_few_large_graphs_use_edge_sized_tasks():
     x = rs.randn(n, d).astype(np.float32)
     from tf_geometric_b200 import _structure
     seg = _structure.csr_for_segment_ids(dev(gi), graphs)
-    if torch.cuda.is_available():
+    if seg.rowptr.is_cuda:             # the real kernels (the host-logic tests replay this body on CPU tensors, without a plan)
         assert seg.plan is not None and seg.plan.n_hubs == 0 and seg.plan.n_tasks >= graphs
     for name in ("mean_pool", "sum_pool", "max_pool", "min_pool"):
         got = host(getattr(tfg.nn, name)(dev(x), dev(gi), graphs))

@@ -175,8 +175,8 @@ def test_hub_rows_are_sliced_and_merged_deterministically(d):
 @pytest.mark.parametrize("d", [128, 100, 64, 32, 256, 200])
 @pytest.mark.parametrize("stages", ["2", "4", "8"])
 def test_tma_gather4_variant_is_bit_identical(d, stages, monkeypatch):
-    """K1 through TMA tile::gather4 (one instruction fetches four neighbour rows into the warp's ring): same bits as the
-    default cp.async ring for weighted sum, mean and max, ragged rows, empty rows and a hub row cut into slices."""
+    """K1 through the TMA ring (four 1-D bulk copies fetch four neighbour rows into the warp's ring): same bits as the
+    cp.async ring for weighted sum, mean and max, ragged rows, empty rows and a hub row cut into slices."""
     rs = np.random.RandomState(d)
     n = 3000
     ei = random_graph(n, 40000, seed=d, isolated=7, hub=(11, 9000))
@@ -187,7 +187,7 @@ def test_tma_gather4_variant_is_bit_identical(d, stages, monkeypatch):
     for reduce, weights in (("sum", w), ("mean", None), ("max", w)):
         monkeypatch.setenv("TFGK_SPMM_IMPL", "async")
         want = ops.spmm(csr, weights, h, reduce=reduce, bias=bias, act=ops.ACT_RELU)
-        monkeypatch.setenv("TFGK_SPMM_IMPL", "gather4")
-        monkeypatch.setenv("TFGK_SPMM_GATHER4_STAGES", stages)
+        monkeypatch.setenv("TFGK_SPMM_IMPL", "tma")
+        monkeypatch.setenv("TFGK_SPMM_TMA_STAGES", stages)
         got = ops.spmm(csr, weights, h, reduce=reduce, bias=bias, act=ops.ACT_RELU)
-        assert torch.equal(got, want), "gather4 changed bits (D={}, reduce={})".format(d, reduce)
+        assert torch.equal(got, want), "TMA ring changed bits (D={}, reduce={})".format(d, reduce)

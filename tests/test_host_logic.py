@@ -1,7 +1,7 @@
 # coding=utf-8
 """Host-side logic of the reference-facing API, exercised on CPU through a test double of the kernel layer
 (tests/fake_backend.py): argument plumbing, graph.cache, quirks, layer wiring, weight names, casting rules.
-The SAME test bodies run against the real kernels in the test_gpu_*.py modules on the B200."""
+The SAME test bodies run against the real kernels in the test_gpu_*.py modules on the H100."""
 import numpy as np
 import pytest
 import torch

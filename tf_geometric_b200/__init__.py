@@ -1,5 +1,5 @@
 # coding=utf-8
-"""tf_geometric_b200 - a B200 (sm_100a) message-passing backend behind tf_geometric's own API surface.
+"""tf_geometric_b200 - an H100 (sm_90a) message-passing backend behind tf_geometric's own API surface.
 
     import tf_geometric_b200 as tfg
     graph = tfg.Graph(x, edge_index).to_device()

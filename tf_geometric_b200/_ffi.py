@@ -1,5 +1,5 @@
 # coding=utf-8
-"""ctypes binding of include/tfgk.h (libtfgk.so, sm_100a).
+"""ctypes binding of include/tfgk.h (libtfgk.so, sm_90a).
 
 There is deliberately NO fallback: if the shared library is missing, or a call fails, an exception is raised.
 PyTorch is only the owner of device memory and streams; every pointer handed to the library is `tensor.data_ptr()`.

@@ -1,7 +1,7 @@
 # coding=utf-8
 """Memoisation of destination-sorted CSR structures.
 
-The reference rebuilds nothing per call because tf.gather/unsorted_segment_sum need no preprocessing; the B200 path
+The reference rebuilds nothing per call because tf.gather/unsorted_segment_sum need no preprocessing; the CUDA path
 needs a dst-sorted CSR, built once per edge list and reused by every forward ("warm cache", the same regime as
 `graph.cache` in demo/demo_gcn.py:47,99-105).  Keys are tensor identities (weakref + in-place version counter), so a
 stale hit is impossible; a user-supplied `cache` dict (the `graph.cache` convention) takes precedence.

@@ -1,10 +1,11 @@
-// Shared helpers for the tfgk kernels (sm_100a only).
+// Shared helpers for the tfgk kernels (sm_90a, H100).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
 #include <stdarg.h>
 #include <float.h>
+#include <atomic>
 #include <mutex>
 #include "tfgk.h"
 
@@ -58,6 +59,21 @@ inline cudaError_t ensure_dynamic_smem(Kernel kernel, size_t bytes) {
         ++used;
     }
     return err;
+}
+
+// SM count of the current device (132 on an H100 SXM, 114 on an H100 PCIe), queried once per device.  It sizes the
+// grid-stride grids, the split-K and column-sum decisions and the copy kernel's default grid.
+inline int sm_count() {
+    static std::atomic<int> cache[64];       // zero-initialised: static storage
+    int dev = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) dev = -1;
+    int n = dev >= 0 ? cache[dev].load(std::memory_order_relaxed) : 0;
+    if (n == 0) {
+        if (dev < 0 || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0)
+            return 132;                      // no device to ask: the launch that follows reports the error
+        cache[dev].store(n, std::memory_order_relaxed);
+    }
+    return n;
 }
 
 inline bool aligned16(const void *p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }

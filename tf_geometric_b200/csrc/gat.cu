@@ -469,13 +469,11 @@ __global__ void __launch_bounds__(kGatAsyncWarps * 32) gat_async_kernel(const Ga
     while (r < r1) finalize_row();
 }
 
-// ---- the same kernel with the neighbour rows fetched by TMA tile::gather4 (north_star: "staged through TMA") ------------------
-// K and V are projected into ONE [N, 2A] buffer (nn/conv/gat.py), so a tensor map over that buffer with a box of 2A columns x 1
-// row lets ONE cp.async.bulk.tensor...tile::gather4 fetch the key AND the value rows of four neighbours (4 x 2A x 4 bytes = 4 KB
-// at A = 128) into the warp's ring stage, completing its mbarrier with the transaction bytes.  Arithmetic, edge order and the
-// online softmax are those of gat_async_kernel: same bits.  Requires V == K + A columns in the same buffer (ldk == ldv).
-struct alignas(64) GatTensorMap { uint64_t opaque[16]; };
-
+// ---- the same kernel with the neighbour rows fetched by the TMA unit (north_star: "staged through TMA") ------------------------
+// K and V are projected into ONE [N, 2A] buffer (nn/conv/gat.py), so the key AND the value row of a neighbour are one contiguous
+// 2A x 4 byte span (1 KB at A = 128): lanes 0-3 each issue one 1-D cp.async.bulk of such a span per round of four edges into
+// the warp's ring stage, completing its mbarrier with the transaction bytes.  Arithmetic, edge order and the online softmax are
+// those of gat_async_kernel: same bits.  Requires V == K + A columns in the same buffer (ldk == ldv).
 __device__ __forceinline__ void gat_mbar_wait(uint32_t bar, uint32_t parity) {
     uint32_t done = 0;
     for (uint32_t spin = 0; !done; ++spin) {
@@ -489,15 +487,14 @@ __device__ __forceinline__ void gat_mbar_wait(uint32_t bar, uint32_t parity) {
 }
 
 template <int S>
-__global__ void __launch_bounds__(kGatAsyncWarps * 32) gat_gather4_kernel(const GatParams p, const __grid_constant__ GatTensorMap tmap) {
+__global__ void __launch_bounds__(kGatAsyncWarps * 32) gat_tma4_kernel(const GatParams p) {
     constexpr int U = 4, RPC = 32 / U;
     static_assert(S <= RPC, "index chunk refill assumes the prologue stays inside chunk 0");
     extern __shared__ __align__(128) uint8_t gat_g4_ring[];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int A = p.H * p.dqk;
     const uint32_t edge_bytes = 2u * (uint32_t)A * 4u;            // [K row | V row] of one neighbour, contiguous in the KV buffer
-    const uint32_t tx_bytes = U * edge_bytes;
-    const uint32_t stage_bytes = (tx_bytes + 127u) & ~127u;
+    const uint32_t stage_bytes = (U * edge_bytes + 127u) & ~127u;
     uint8_t *my_ring = gat_g4_ring + (size_t)warp * S * stage_bytes;
     const uint32_t ring_addr = (uint32_t)__cvta_generic_to_shared(my_ring);
     uint64_t *bars = reinterpret_cast<uint64_t *>(gat_g4_ring + (size_t)kGatAsyncWarps * S * stage_bytes) + warp * S;
@@ -571,20 +568,15 @@ __global__ void __launch_bounds__(kGatAsyncWarps * 32) gat_gather4_kernel(const 
         if (g < n_rounds) {
             const int base = (g % RPC) * U;
             const int valid = min(U, n_edges - g * U);
-            const int c0 = __shfl_sync(0xffffffffu, ci, base);
-            int c1 = __shfl_sync(0xffffffffu, ci, base + 1), c2 = __shfl_sync(0xffffffffu, ci, base + 2);
-            int c3 = __shfl_sync(0xffffffffu, ci, base + 3);
-            if (valid < 2) c1 = c0;
-            if (valid < 3) c2 = c0;
-            if (valid < 4) c3 = c0;
-            if (lane == 0) {
-                const uint32_t bar = bar0 + 8 * (uint32_t)(g % S);
-                asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(tx_bytes) : "memory");
-                asm volatile(
-                    "cp.async.bulk.tensor.2d.shared::cta.global.tile::gather4.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4, %5, %6}], [%7];"
-                    ::"r"(ring_addr + (uint32_t)(g % S) * stage_bytes), "l"(&tmap), "r"(0), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(bar)
-                    : "memory");
-            }
+            const int c = __shfl_sync(0xffffffffu, ci, base + (lane < U ? lane : 0));
+            const uint32_t bar = bar0 + 8 * (uint32_t)(g % S);
+            if (lane == 0)
+                asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"((uint32_t)valid * edge_bytes)
+                             : "memory");
+            if (lane < valid)
+                asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+                             ::"r"(ring_addr + (uint32_t)(g % S) * stage_bytes + (uint32_t)lane * edge_bytes),
+                             "l"(p.K + (int64_t)c * p.ldk), "r"(edge_bytes), "r"(bar) : "memory");
         }
     };
 
@@ -694,34 +686,18 @@ static int launch_gat_async(const GatParams &p, cudaStream_t st) {
     return TFGK_OK;
 }
 
-typedef int (*GatEncodeTiledFn)(void *map, int dtype, uint32_t rank, void *base, const uint64_t *dims, const uint64_t *strides,
-                                const uint32_t *box, const uint32_t *elem_strides, int interleave, int swizzle, int l2promo,
-                                int oob_fill);
-
 template <int S>
-static int launch_gat_gather4(const GatParams &p, cudaStream_t st) {
+static int launch_gat_tma4(const GatParams &p, cudaStream_t st) {
     const int A = p.H * p.dqk;
-    if (p.V != p.K + A || p.ldk != p.ldv || 2 * A > 256 || (p.ldk % 4) != 0) return TFGK_ERR_UNSUPPORTED;
-    static GatEncodeTiledFn encode = nullptr;
-    if (encode == nullptr) {
-        void *fn = nullptr;
-        cudaDriverEntryPointQueryResult qres;
-        TFGK_CUDA(cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres));
-        if (fn == nullptr || qres != cudaDriverEntryPointSuccess) return TFGK_ERR_UNSUPPORTED;
-        encode = reinterpret_cast<GatEncodeTiledFn>(fn);
-    }
-    GatTensorMap tmap;
-    const uint64_t dims[2] = {(uint64_t)(2 * A), (uint64_t)1 << 31};      // rows are bounded by the int32 column ids
-    const uint64_t strides[1] = {(uint64_t)p.ldk * sizeof(float)};
-    const uint32_t box[2] = {(uint32_t)(2 * A), 1u};
-    const uint32_t elem[2] = {1u, 1u};
-    if (encode(&tmap, 7, 2, const_cast<float *>(p.K), dims, strides, box, elem, 0, 0, 2, 0) != 0) return TFGK_ERR_UNSUPPORTED;
+    // one bulk copy per neighbour: the [K | V] span must be 16-byte aligned and a multiple of 16 bytes
+    if (p.V != p.K + A || p.ldk != p.ldv || 2 * A > 256 || (p.ldk % 4) != 0 || (A % 2) != 0 || !aligned16(p.K))
+        return TFGK_ERR_UNSUPPORTED;
     const size_t stage_pitch = ((size_t)4 * 2 * A * 4 + 127) & ~(size_t)127;
     const size_t smem = (size_t)kGatAsyncWarps * S * stage_pitch + (size_t)kGatAsyncWarps * S * 8;
-    TFGK_CUDA(ensure_dynamic_smem(gat_gather4_kernel<S>, smem));
+    TFGK_CUDA(ensure_dynamic_smem(gat_tma4_kernel<S>, smem));
     const int64_t n_tasks = p.task_row ? p.n_tasks : ceil_div64(p.N, kGatAsyncRows);
     const unsigned blocks = (unsigned)ceil_div64(n_tasks, kGatAsyncWarps);
-    gat_gather4_kernel<S><<<blocks, kGatAsyncWarps * 32, smem, st>>>(p, tmap);
+    gat_tma4_kernel<S><<<blocks, kGatAsyncWarps * 32, smem, st>>>(p);
     TFGK_LAUNCH_CHECK();
     if (p.task_row && p.n_hubs > 0) {
         gat_hub_fixup_kernel<<<(unsigned)ceil_div64(p.n_hubs, 8), 256, 0, st>>>(p);
@@ -731,15 +707,14 @@ static int launch_gat_gather4(const GatParams &p, cudaStream_t st) {
 }
 
 static int dispatch_gat_async(const GatParams &p, cudaStream_t st) {
-    // default: TMA tile::gather4 ring with two stages whenever K and V sit side by side in one buffer (the layers project them
-    // that way): 18.74 ms against 19.97 ms for the cp.async ring at the products shape, three / four stages lose resident warps
-    // (22.1 / 26.3 ms; profiles/r2_kernel_variants_final.json).  TFGK_GAT_IMPL=async keeps the cp.async ring; "gather4:S" sets S.
+    // default: the TMA ring with two stages whenever K and V sit side by side in one buffer (the layers project them that way).
+    // TFGK_GAT_IMPL=async selects the cp.async ring; "tma:S" sets the depth S of the TMA ring (2, 3 or 4).
     const char *g4 = getenv("TFGK_GAT_IMPL");
     if (!(g4 && g4[0] == 'a')) {
         const char *colon = g4 ? strchr(g4, ':') : nullptr;
         const int stages = colon ? atoi(colon + 1) : 2;
-        const int rc = stages == 2 ? launch_gat_gather4<2>(p, st) : stages == 4 ? launch_gat_gather4<4>(p, st)
-                                                                              : launch_gat_gather4<3>(p, st);
+        const int rc = stages == 2 ? launch_gat_tma4<2>(p, st) : stages == 4 ? launch_gat_tma4<4>(p, st)
+                                                                           : launch_gat_tma4<3>(p, st);
         if (rc != TFGK_ERR_UNSUPPORTED) return rc;
     }
     const char *cfg = getenv("TFGK_GAT_ASYNC_CFG");        // "UxS"; default 2x3
@@ -950,10 +925,11 @@ static int gat_fused_impl(const int64_t *rowptr, const int32_t *col,
                       ldv % 4 == 0 && ldo % 4 == 0 && aligned16(Q) && aligned16(K) && aligned16(V) && aligned16(out) &&
                       (!bias || aligned16(bias));
     const char *impl = getenv("TFGK_GAT_IMPL");          // "twopass" forces the reference-order kernel
-    if (fast && dqk == dv && A <= 128 && !write_att && (stats != nullptr || !(impl && (impl[0] == 't' || impl[0] == 'o'))))
+    const bool twopass = impl && strncmp(impl, "twopass", 7) == 0, online = impl && strncmp(impl, "online", 6) == 0;
+    if (fast && dqk == dv && A <= 128 && !write_att && (stats != nullptr || !(twopass || online)))
         return dispatch_gat_async(p, st);                    // "online" forces the register-staged single-pass kernel
     if (stats != nullptr) return TFGK_ERR_UNSUPPORTED;      // only the streaming kernel keeps (max, denominator)
-    if (fast && dqk == dv && !(impl && impl[0] == 't')) {
+    if (fast && dqk == dv && !twopass) {
         switch ((A + 127) / 128) {
             case 1: return launch_gat_online<1>(p, st);
             case 2: return launch_gat_online<2>(p, st);

@@ -1,6 +1,6 @@
 // K4 (SIMT path): C = act(op(A) @ op(B) + bias + beta*C) in exact fp32 (FFMA), 128x128x8 tiles, 8x8 micro-tiles.
 // This is the general fallback (any transpose, any shape, split-K for tall-skinny weight-gradient reductions).
-// The forward projections x@W of the hot path go through the tcgen05 kernel in gemm_tc.cu when it applies.
+// The forward projections x@W of the hot path go through the wgmma kernel in gemm_proj.cu when it applies.
 #include "common.cuh"
 #include <algorithm>
 
@@ -119,8 +119,9 @@ __global__ void splitk_reduce_kernel(const GemmParams p, int S) {
 
 static int choose_splits(int M, int N, int K) {
     const int64_t tiles = ceil_div64(M, BM) * ceil_div64(N, BN);
-    if (tiles >= 148 || K < 4096) return 1;
-    int64_t s = (148 * 2) / tiles;
+    const int sms = sm_count();
+    if (tiles >= sms || K < 4096) return 1;
+    int64_t s = (sms * 2) / tiles;
     const int64_t by_k = ceil_div64(K, 1024);
     if (s > by_k) s = by_k;
     return (int)(s < 1 ? 1 : s);
@@ -178,7 +179,7 @@ using namespace tfgk;
 
 static int colsum_blocks(int64_t n_rows) {
     int64_t b = ceil_div64(n_rows, 512);
-    if (b > 148 * 8) b = 148 * 8;
+    if (b > sm_count() * 8) b = sm_count() * 8;
     return (int)(b < 1 ? 1 : b);
 }
 
@@ -204,11 +205,6 @@ extern "C" int tfgk_colsum_f32(const float *x, int64_t ldx, int64_t n_rows, int3
     return TFGK_OK;
 }
 
-namespace tfgk {
-}  // namespace tfgk
-
-using namespace tfgk;
-
 extern "C" int tfgk_gemm_workspace_bytes(int32_t M, int32_t N, int32_t K, size_t *out_bytes) {
     TFGK_CHECK_ARG(out_bytes != nullptr, "gemm_workspace_bytes: null output");
     TFGK_CHECK_ARG(M >= 0 && N >= 0 && K >= 0, "gemm_workspace_bytes: negative size");
@@ -216,10 +212,6 @@ extern "C" int tfgk_gemm_workspace_bytes(int32_t M, int32_t N, int32_t K, size_t
     *out_bytes = s > 1 ? (size_t)s * M * N * sizeof(float) : 0;
     return TFGK_OK;
 }
-
-// tensor-core path (gemm_tc.cu); returns TFGK_ERR_UNSUPPORTED when the shape/layout does not qualify
-extern "C" int tfgk_gemm_tc_f32(const float *A, int64_t lda, const float *B, int64_t ldb, const float *bias, int act,
-                                int32_t M, int32_t N, int32_t K, float *C, int64_t ldc, void *stream);
 
 extern "C" int tfgk_gemm_f32(const float *A, int64_t lda, int transA, const float *B, int64_t ldb, int transB,
                              const float *bias, int act, float beta, int32_t M, int32_t N, int32_t K,
@@ -233,8 +225,8 @@ extern "C" int tfgk_gemm_f32(const float *A, int64_t lda, int transA, const floa
     cudaStream_t st = as_stream(stream);
 
     if (!transA && beta == 0.0f && K > 0) {
-        // tall projections (and dX = dY W^T with transB): the multi-block tcgen05 kernel (gemm_proj.cu), N cut into blocks
-        // of <= 128 columns
+        // tall projections (and dX = dY W^T with transB): the multi-block wgmma kernel (gemm_proj.cu), N cut into blocks
+        // of <= 128 columns; TFGK_GEMM_TC=0 forces the exact-fp32 SIMT kernel
         const char *env = getenv("TFGK_GEMM_TC");
         const bool tc_on = !(env != nullptr && env[0] == '0');
         if (tc_on && N <= 512 && (int64_t)M * K >= (1 << 14)) {
@@ -250,10 +242,6 @@ extern "C" int tfgk_gemm_f32(const float *A, int64_t lda, int transA, const floa
             const float *parts[1] = {A};
             const int rcp = tfgk_gemm_proj_f32(parts, 1, 0, lda, M, K, blocks, nb, 0, 0, stream);
             if (rcp != TFGK_ERR_UNSUPPORTED) return rcp;
-        }
-        if (!transB) {
-            const int rc = tfgk_gemm_tc_f32(A, lda, B, ldb, bias, act, M, N, K, C, ldc, stream);
-            if (rc != TFGK_ERR_UNSUPPORTED) return rc;
         }
     }
 
@@ -272,7 +260,7 @@ extern "C" int tfgk_gemm_f32(const float *A, int64_t lda, int transA, const floa
     else                  sgemm_kernel<false, false><<<grid, kGemmThreads, 0, st>>>(p);
     TFGK_LAUNCH_CHECK();
     if (S > 1) {
-        splitk_reduce_kernel<<<(unsigned)std::min<int64_t>(ceil_div64((int64_t)M * N, 256), 148 * 8), 256, 0, st>>>(p, S);
+        splitk_reduce_kernel<<<(unsigned)std::min<int64_t>(ceil_div64((int64_t)M * N, 256), (int64_t)sm_count() * 8), 256, 0, st>>>(p, S);
         TFGK_LAUNCH_CHECK();
     }
     return TFGK_OK;

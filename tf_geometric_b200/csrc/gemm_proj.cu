@@ -1,652 +1,273 @@
-// K4 (round 2): the dense projections of the hot path as ONE launch over several column blocks, optionally with the A
-// operand gathered tile by tile from other GPUs' memory (fused all-gather -> GEMM over NVLink peer mappings, K5).
+// K4: the dense projections of the hot path on the Hopper tensor cores (wgmma), as ONE launch over several column blocks,
+// optionally with the A operand gathered tile by tile from other GPUs' memory (fused all-gather -> GEMM over NVLink peer
+// mappings, K5).
 //
 //   C_b[M, n_b] = act_b(A[M, K] @ W_b[K, n_b] + bias_b)     for b in 0..nb-1  (n_b <= 128, nb <= 4)
 //
-// replaces x@W at nn/conv/gcn.py:272 and the three projections x@Wq, x@Wk, x@W of nn/conv/gat.py:52,61,70, which the
-// round-1 path ran as three launches that each re-read x.  Differences from gemm_tc.cu (same 3xTF32 arithmetic, same bits):
-//   * column blocks: CTA b handles block b % nb for the row tiles of its group b / nb; the nb CTAs of a group walk the
-//     same tiles in the same order, so x is read from HBM once and from L2 nb-1 times (A traffic is 4(MK), not 4 nb MK);
-//   * W_b (hi | lo) resident in shared memory for K rounded up to 8 (not 32), the MMA issuer skips the UMMA_K steps
-//     beyond K and the producers skip the 16-byte chunks beyond it: K = 100 costs 13 k-steps instead of 16;
-//   * epilogue through shared memory: tcgen05.ld 32 columns per round trip -> +bias -> act -> per-warp staging tile ->
-//     full 128-byte row segments per store instruction (the round-1 epilogue wrote 16 bytes per row per instruction);
+// replaces x@W at nn/conv/gcn.py:272 and the three projections x@Wq, x@Wk, x@W of nn/conv/gat.py:52,61,70, which would
+// otherwise be three launches that each re-read x.  tfgk_gemm_f32 sends every tall projection here as well.
+//
+// Arithmetic: 3xTF32.  a = a_hi + a_lo and w = w_hi + w_lo with x_hi = cvt.rna.tf32(x), and per k-step of 8
+//     acc += a_lo * w_hi;  acc += a_hi * w_lo;  acc += a_hi * w_hi        (wgmma.m64n128k8.f32.tf32.tf32, fp32 accumulators)
+// which keeps the error at the fp32 level (tests/test_gpu_gemm_tc.py: < 5e-6 relative up to K = 512), where a single TF32
+// pass is off by ~1e-3.  The result of a row depends only on that row, the weights and K: the same bits whatever the
+// number of blocks, the grid or the part layout of A.
+//
+// Layout (one CTA = 128 output rows x one column block of <= 128 columns, 256 threads = two warpgroups of 64 rows):
+//   * W_b (hi | lo) resident in shared memory for the whole kernel, K rounded up to 8, in the K-major no-swizzle layout of
+//     the wgmma descriptors: 8 x 16-byte core matrices, LBO = 128 B along K, SBO = 32 * Kpad bytes along N;
+//   * A streams through a cp.async ring of BK = 32 columns per stage (rows padded to 36 floats: the fragment loads hit 32
+//     distinct banks); each thread splits its own A fragment into hi / lo in registers, so A never goes back to shared memory
+//     and the wgmma reads A from registers and W through the descriptors.  The fragments live in two register sets, so the
+//     wait for the MMAs of k-block j comes after k-block j + 1 has been loaded and split into the other set (ptxas adds
+//     warpgroup.arrive fences around the register operands; measured, this is 3-4 % faster than waiting after every
+//     k-block, DESIGN.md section 4);
+//   * persistent CTAs: CTA b handles block b % nb for the row tiles of its group b / nb; the nb CTAs of a group walk the
+//     same tiles in the same order, so x is read from HBM once and from L2 nb-1 times.  The ring runs across tile
+//     boundaries, so the loads of the next tile overlap the epilogue of the current one;
 //   * A may be split into `n_parts` row blocks living at different base pointers (the other ranks' copies of x, mapped
-//     through CUDA IPC): the producers' cp.async then read straight over NVLink, tile by tile, while the tensor core
-//     works on the previous tiles - no halo buffer for x, no separate exchange step.  Tiles are walked starting at part
-//     `first_part` so that every rank pulls from a different peer at any moment.
+//     through CUDA IPC): the cp.async then read straight over NVLink, tile by tile.  Tiles are walked starting at the tile
+//     of part `first_part`, so that every rank pulls from a different peer at any moment.
 #include "common.cuh"
-#include "tfgk_tc.cuh"
-#include <stdlib.h>
+#include <type_traits>
 
 namespace tfgk {
 namespace proj {
 
-using namespace tc;
-
+constexpr int BM = 128;                  // rows per tile (two warpgroups x 64)
+constexpr int BK = 32;                   // A columns per ring stage
+constexpr int kUN = 128;                 // output columns per CTA
+constexpr int kThreads = 256;
+constexpr int kApitch = BK + 4;          // floats per A row in a stage
+constexpr int kStageBytes = BM * kApitch * 4;
 constexpr int kMaxBlocks = 4;
 constexpr int kMaxParts = 8;
-// warp roles: 0-3 converters (lo = a - trunc(a) on landed k-blocks), 4-11 epilogue (TMEM lane quarter = warp % 4, two
-// warps per quarter split the columns), 12 MMA issuer, 13-14 loaders (cp.async into the ring as soon as a stage is free)
-constexpr int kProducerWarps = 4, kEpilogueWarps = 8, kLoaderWarps = 2;
-constexpr int kLoaderWarp0 = kProducerWarps + kEpilogueWarps + 1;
-constexpr int kThreadsProj = (kProducerWarps + kEpilogueWarps + 1 + kLoaderWarps) * 32;      // 480
-constexpr int kBarrierBytes = 192;
-constexpr int kUN = 128;                 // accumulator columns per buffer
-constexpr int kTmemColsProj = 256;       // 2 accumulator buffers
-constexpr int kPassCols = 16;             // accumulator columns per TMEM round trip of an epilogue warp
-constexpr int kStageRowBytes = 80;       // 16 floats + 16 B pad: conflict-free row-wise STS.128, segment-wise LDS.128
-constexpr int kStageBytes = 32 * kStageRowBytes;
 
 struct Params {
     const float *A[kMaxParts];
     int64_t lda, part_rows;
-    int n_parts, first_tile, local_part;
-    int M, K, nb, tiles_m, n_groups;
-    int dbg;           // measurement switches (TFGK_PROJ_DEBUG): 1 no lo conversion, 2 hi*hi MMA only, 4 no stores, 8 no loads,
-                       // 16 no TMEM reads, 32 no staging / stores after the TMEM read, 64 epilogue stores straight from registers
+    int first_tile;
+    int M, K, kpad, nb, tiles_m, n_groups;
     const float *B[kMaxBlocks]; int64_t ldb[kMaxBlocks];
     const float *bias[kMaxBlocks]; int act[kMaxBlocks]; int ncols[kMaxBlocks]; int transb[kMaxBlocks];
     float *C[kMaxBlocks]; int64_t ldc[kMaxBlocks];
 };
 
+// shared memory: W hi | W lo | bias | ring of A stages
 struct Plan {
-    uint32_t kpad8, b_bytes, a_stage_bytes, stages, total;
-    __host__ __device__ explicit Plan(int K) {
-        kpad8 = (uint32_t)((K + 7) / 8) * 8;
-        b_bytes = (uint32_t)kUN * kpad8 * 4u;
-        a_stage_bytes = 2u * BM * BK * 4u;
-        const uint32_t fixed = 2u * b_bytes + kEpilogueWarps * kStageBytes + kBarrierBytes + kUN * 4u;
+    uint32_t kpad, b_bytes, ring_off, stages, total;
+    explicit Plan(int K) {
+        kpad = (uint32_t)((K + 7) / 8) * 8;
+        b_bytes = (uint32_t)kUN * kpad * 4u;
+        ring_off = 2u * b_bytes + kUN * 4u;
         const uint32_t budget = 227u * 1024u;
         stages = 0;
         for (uint32_t st = 4; st >= 2; --st)
-            if (fixed + st * a_stage_bytes <= budget) { stages = st; break; }
-        total = fixed + stages * a_stage_bytes;
+            if (ring_off + st * kStageBytes <= budget) { stages = st; break; }
+        total = ring_off + stages * kStageBytes;
     }
 };
 
-__device__ __forceinline__ bool elect_one() {
-    uint32_t pred;
-    asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(pred));
-    return pred != 0;
+__device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
+
+// byte offset of W[k][n] in the K-major core-matrix layout (8 rows of n x 16 bytes of k per core matrix)
+__device__ __forceinline__ uint32_t w_offset(int n, int k, int kpad) {
+    return (uint32_t)(n >> 3) * (uint32_t)(kpad * 32) + (uint32_t)(k >> 2) * 128u + (uint32_t)(n & 7) * 16u + (uint32_t)(k & 3) * 4u;
 }
 
-// ---- epilogue shared by both kernels: TMEM -> registers -> per-warp staging tile -> full row segments per store ----------
+// wgmma shared-memory descriptor: K-major, no swizzle, LBO = 128 B (next core matrix along K), SBO (next 8 rows along N)
+__device__ __forceinline__ uint64_t make_desc(uint32_t saddr, uint32_t sbo_bytes) {
+    uint64_t d = 0;
+    d |= (uint64_t)((saddr & 0x3FFFFu) >> 4);          // start address,       bits [0,14)
+    d |= (uint64_t)(128u >> 4) << 16;                  // leading byte offset, bits [16,30)
+    d |= (uint64_t)(sbo_bytes >> 4) << 32;             // stride byte offset,  bits [32,46)
+    return d;                                          // base offset 0, layout type 0 (no swizzle)
+}
+
+__device__ __forceinline__ void split_tf32(float a, uint32_t &hi, uint32_t &lo) {
+    asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(hi) : "f"(a));
+    lo = __float_as_uint(a - __uint_as_float(hi));
+}
+
+__device__ __forceinline__ void cp_async16_zfill(uint32_t dst, const void *src, uint32_t src_bytes) {
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(src_bytes) : "memory");
+}
+
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+
+// D[64 x 128] (+)= A[64 x 8] (registers, tf32) * B[8 x 128] (shared memory descriptor, tf32); accumulate == 0 overwrites D
+__device__ __forceinline__ void wgmma_m64n128k8(float (&d)[64], const uint32_t (&a)[4], uint64_t b_desc, uint32_t accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %69, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+        "{%64, %65, %66, %67}, %68, p, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+          "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+          "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+          "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+          "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "r"(accumulate)
+        : "memory");
+}
+
 __device__ __forceinline__ int tile_index(const Params &p, int group, int it) {
     int tl = group + it * p.n_groups + p.first_tile;
     return tl >= p.tiles_m ? tl - p.tiles_m : tl;
 }
 
-__device__ __forceinline__ void epilogue_loop(const Params &p, int cb, int group, int un, int ncols, uint32_t tmem_base,
-                                              uint8_t *stage_base, const float *s_bias, uint64_t *acc_full, uint64_t *acc_empty,
-                                              int my_tiles, int warp, int lane) {
-    auto tile_of = [&](int it) { return tile_index(p, group, it); };
-        const int ew = warp - kProducerWarps;                 // 0..7
-        const int q = warp & 3, half = ew >> 2;               // TMEM lane quarter (= warp % 4) and column half of this warp
-        uint8_t *stg = stage_base + ew * kStageBytes;
-        const uint32_t stg_addr = smem_u32(stg);
-        float *__restrict__ Cb = p.C[cb];
-        const int64_t ldc = p.ldc[cb];
-        const int act = p.act[cb];
-        const bool vec_ok = (ldc % 4 == 0) && ((reinterpret_cast<uintptr_t>(Cb) & 15) == 0);
-        const int seg_row = lane >> 2, seg_chunk = lane & 3;  // store phase: 8 rows x 64 bytes per instruction
-        const int n_pass = un / kPassCols;
-        const int pass0 = half == 0 ? 0 : (n_pass + 1) / 2, pass1 = half == 0 ? (n_pass + 1) / 2 : n_pass;
-        for (int it = 0; it < my_tiles; ++it) {
-            const int buf = it & 1;
-            const int tile = tile_of(it);
-            mbar_wait(&acc_full[buf], (uint32_t)((it >> 1) & 1));
-            tc_fence_after();
-            const int64_t row0 = (int64_t)tile * BM + q * 32;
-            if (pass0 >= pass1) {                             // nothing to read (a single pass belongs to the other half)
-                tc_fence_before();
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&acc_empty[buf]);
-            }
-            if (p.dbg & 64) {
-                // direct variant: every thread stores the 16 columns of its own row straight from registers (64 contiguous
-                // bytes per row in four 16-byte stores), the tensor-memory read of the next pass is issued before the stores
-                // of this one - no staging tile, no warp barriers on the path
-                uint32_t ra[16], rb[16];
-                auto ldtm = [&](int ps, uint32_t (&r)[16]) {
-                    const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(buf * kUN + ps * kPassCols);
-                    asm volatile(
-                        "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-                        "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-                        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-                          "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-                        : "r"(taddr));
-                };
-                auto store = [&](int ps, const uint32_t (&r)[16]) {
-                    const int c0 = ps * kPassCols;
-                    const int64_t row = row0 + lane;
-                    if (row >= p.M || (p.dbg & 4)) return;
-                    float *dst = Cb + row * ldc + c0;
-#pragma unroll
-                    for (int j = 0; j < 16; j += 4) {
-                        float4 v;
-                        v.x = apply_act(__uint_as_float(r[j]) + s_bias[c0 + j], act);
-                        v.y = apply_act(__uint_as_float(r[j + 1]) + s_bias[c0 + j + 1], act);
-                        v.z = apply_act(__uint_as_float(r[j + 2]) + s_bias[c0 + j + 2], act);
-                        v.w = apply_act(__uint_as_float(r[j + 3]) + s_bias[c0 + j + 3], act);
-                        if (vec_ok && c0 + j + 4 <= ncols) {
-                            *reinterpret_cast<float4 *>(dst + j) = v;
-                        } else {
-                            if (c0 + j < ncols) dst[j] = v.x;
-                            if (c0 + j + 1 < ncols) dst[j + 1] = v.y;
-                            if (c0 + j + 2 < ncols) dst[j + 2] = v.z;
-                            if (c0 + j + 3 < ncols) dst[j + 3] = v.w;
-                        }
-                    }
-                };
-                if (pass0 < pass1) ldtm(pass0, ra);
-                for (int ps = pass0; ps < pass1; ps += 2) {
-                    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-                    if (ps + 1 < pass1) ldtm(ps + 1, rb);
-                    else { tc_fence_before(); __syncwarp(); if (lane == 0) mbar_arrive(&acc_empty[buf]); }
-                    store(ps, ra);
-                    if (ps + 1 < pass1) {
-                        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-                        if (ps + 2 < pass1) ldtm(ps + 2, ra);
-                        else { tc_fence_before(); __syncwarp(); if (lane == 0) mbar_arrive(&acc_empty[buf]); }
-                        store(ps + 1, rb);
-                    }
-                }
-                continue;
-            }
-            for (int ps = pass0; ps < pass1; ++ps) {
-                const int c0 = ps * kPassCols;
-                uint32_t r[16];
-                const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(buf * kUN + c0);
-                if (p.dbg & 16) {
-#pragma unroll
-                    for (int j = 0; j < 16; ++j) r[j] = 0;
-                } else
-                asm volatile(
-                    "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-                    "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-                    : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-                      "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-                    : "r"(taddr));
-                asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-                if (ps + 1 == pass1) {                        // this warp's share is drained: one arrive per warp frees the buffer
-                    tc_fence_before();
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive(&acc_empty[buf]);
-                }
-                if (p.dbg & 32) continue;
-#pragma unroll
-                for (int j = 0; j < 16; j += 4) {
-                    const float v0 = apply_act(__uint_as_float(r[j]) + s_bias[c0 + j], act);
-                    const float v1 = apply_act(__uint_as_float(r[j + 1]) + s_bias[c0 + j + 1], act);
-                    const float v2 = apply_act(__uint_as_float(r[j + 2]) + s_bias[c0 + j + 2], act);
-                    const float v3 = apply_act(__uint_as_float(r[j + 3]) + s_bias[c0 + j + 3], act);
-                    st_shared_v4(stg_addr + (uint32_t)lane * kStageRowBytes + (uint32_t)j * 4u, v0, v1, v2, v3);
-                }
-                __syncwarp();
-                const int col = c0 + seg_chunk * 4;
-#pragma unroll
-                for (int j = 0; j < 4; ++j) {
-                    const int rl = j * 8 + seg_row;
-                    const int64_t row = row0 + rl;
-                    const float4 v = *reinterpret_cast<const float4 *>(stg + rl * kStageRowBytes + seg_chunk * 16);
-                    if (row < p.M && !(p.dbg & 4)) {
-                        float *dst = Cb + row * ldc + col;
-                        if (vec_ok && col + 4 <= ncols) {
-                            *reinterpret_cast<float4 *>(dst) = v;
-                        } else {
-                            if (col < ncols) dst[0] = v.x;
-                            if (col + 1 < ncols) dst[1] = v.y;
-                            if (col + 2 < ncols) dst[2] = v.z;
-                            if (col + 3 < ncols) dst[3] = v.w;
-                        }
-                    }
-                }
-                __syncwarp();
-            }
-        }
-}
-
 template <int STAGES>
-__global__ void __launch_bounds__(kThreadsProj, 1) gemm_proj_kernel(const Params p) {
-    extern __shared__ __align__(1024) uint8_t smem[];
-    const Plan L(p.K);
-    uint8_t *b_hi_ptr = smem, *b_lo_ptr = smem + L.b_bytes;
-    uint8_t *a_ring = smem + 2 * L.b_bytes;
-    uint8_t *stage_base = a_ring + STAGES * L.a_stage_bytes;
-    uint64_t *full = reinterpret_cast<uint64_t *>(stage_base + kEpilogueWarps * kStageBytes);
-    uint64_t *empty = full + STAGES, *landed = empty + STAGES, *acc_full = landed + STAGES, *acc_empty = acc_full + 2;
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(acc_empty + 2);
-    float *s_bias = reinterpret_cast<float *>(reinterpret_cast<uint8_t *>(full) + kBarrierBytes);
-    const int t = threadIdx.x, warp = t >> 5, lane = t & 31;
-    const int cb = (int)blockIdx.x % p.nb, group = (int)blockIdx.x / p.nb;
-    const int ncols = p.ncols[cb];
-    const int un = ((ncols + 15) / 16) * 16;
-    const float *__restrict__ Bm = p.B[cb];
-    const int64_t ldb = p.ldb[cb];
-    const bool tb = p.transb[cb] != 0;
+__global__ void __launch_bounds__(kThreads, 1) gemm_proj_kernel(const Params p) {
+    extern __shared__ __align__(128) uint8_t smem[];
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int cb = blockIdx.x % p.nb, group = blockIdx.x / p.nb;
+    const int kpad = p.kpad;
+    const uint32_t b_bytes = (uint32_t)kUN * kpad * 4u;
+    uint8_t *w_hi = smem, *w_lo = smem + b_bytes;
+    float *s_bias = reinterpret_cast<float *>(smem + 2 * b_bytes);
+    uint8_t *ring = smem + 2 * b_bytes + kUN * 4;
+    const uint32_t ring_addr = smem_u32(ring);
 
-    for (int i = t; i < kUN; i += kThreadsProj) s_bias[i] = (p.bias[cb] != nullptr && i < ncols) ? __ldg(p.bias[cb] + i) : 0.0f;
-    if (t == 0) {
-        for (int i = 0; i < STAGES; ++i) {
-            mbar_init(&full[i], kProducerWarps); mbar_init(&empty[i], 1); mbar_init(&landed[i], kLoaderWarps * 32);
-        }
-        for (int i = 0; i < 2; ++i) { mbar_init(&acc_full[i], 1); mbar_init(&acc_empty[i], kEpilogueWarps); }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 0) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(kTmemColsProj) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    {   // W_b: transpose + RNA split into the K-major core-matrix layout, once per CTA
-        const int kchunks = (int)L.kpad8 / 4;
-        const int total = un * kchunks;
-        const uint32_t bh = smem_u32(b_hi_ptr), bl = smem_u32(b_lo_ptr);
-        for (int c = t; c < total; c += kThreadsProj) {
-            const int n8 = c & 7, kc = (c >> 3) % kchunks, ng = (c >> 3) / kchunks;
-            const int n = ng * 8 + n8, k = kc * 4;
-            float w[4] = {0.f, 0.f, 0.f, 0.f}, h[4], l[4];
-            if (n < ncols) {
+    const int ncols = p.ncols[cb];
+    const int my_tiles = group < p.tiles_m ? (p.tiles_m - group + p.n_groups - 1) / p.n_groups : 0;
+    const int kb_per_tile = (p.K + BK - 1) / BK;
+    const int total = my_tiles * kb_per_tile;
+
+    // A k-block j of this CTA (tile j / kb_per_tile) -> ring stage j % STAGES; rows beyond M and columns beyond K are zeros
+    // (a tile never straddles two parts: part_rows is a multiple of BM)
+    auto load_stage = [&](int j) {
+        if (j < total) {
+            const int64_t row0 = (int64_t)tile_index(p, group, j / kb_per_tile) * BM;
+            const int part = (int)(row0 / p.part_rows);
+            const float *a_tile = p.A[part] + (row0 - (int64_t)part * p.part_rows) * p.lda;
+            const int rows = (int)min((int64_t)BM, (int64_t)p.M - row0);
+            const int k0 = (j % kb_per_tile) * BK;
+            const uint32_t dst0 = ring_addr + (uint32_t)(j % STAGES) * kStageBytes;
+            const int ch = tid & 7, gk = k0 + ch * 4;
+            const uint32_t bytes = gk < p.K ? (uint32_t)min(16, (p.K - gk) * 4) : 0u;
 #pragma unroll
-                for (int i = 0; i < 4; ++i)
-                    if (k + i < p.K) w[i] = __ldg(tb ? Bm + (int64_t)n * ldb + (k + i) : Bm + (int64_t)(k + i) * ldb + n);
+            for (int i = 0; i < (BM * BK / 4) / kThreads; ++i) {
+                const int r = (tid >> 3) + i * (kThreads / 8);
+                const bool ok = r < rows && bytes != 0;
+                cp_async16_zfill(dst0 + (uint32_t)(r * kApitch + ch * 4) * 4u, ok ? a_tile + (int64_t)r * p.lda + gk : p.A[0],
+                                 ok ? bytes : 0u);
             }
-#pragma unroll
-            for (int i = 0; i < 4; ++i) split_tf32(w[i], h[i], l[i]);
-            st_shared_v4(bh + c * 16, h[0], h[1], h[2], h[3]);
-            st_shared_v4(bl + c * 16, l[0], l[1], l[2], l[3]);
         }
-    }
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-    const int nkb = (int)(L.kpad8 + BK - 1) / BK;
-    const int last_steps = ((int)L.kpad8 - (nkb - 1) * BK) / UMMA_K;
-    const int my_tiles = group < p.tiles_m ? (p.tiles_m - 1 - group) / p.n_groups + 1 : 0;
-    const int total_kb = my_tiles * nkb;
-    // logical tile i of this group -> physical row tile (rotated so that ranks start on different parts)
-    auto tile_of = [&](int it) {
-        int tl = group + it * p.n_groups + p.first_tile;
-        return tl >= p.tiles_m ? tl - p.tiles_m : tl;
+        asm volatile("cp.async.commit_group;" ::: "memory");
     };
 
-    if (warp >= kLoaderWarp0) {
-        // ===================== loaders: cp.async A (possibly from a peer GPU) straight into the UMMA layout =====================
-        // The round-1 kernel (and the first version of this one) let the same threads load AND convert: a k-block could only be
-        // published after the thread had blocked on the stage for a later load, so producer, tensor core and the commit
-        // round trip (~1000 cycles, measured with the TFGK_PROJ_DEBUG switches) ran one after the other.  Here every
-        // role blocks only on its own dependency: loaders on `empty`, converters on `landed`, the MMA issuer on `full`.
-        const int tl = t - kLoaderWarp0 * 32;                                // 0..63
-        const uint32_t a_ring_addr = smem_u32(a_ring);
-        constexpr int kChunks = (BM * BK / 4) / (kLoaderWarps * 32);        // 16 per thread per k-block
-        const int r8 = tl & 7, kc = (tl >> 3) & 7;                          // chunk c = tl + 64 i: rows i * 8 + r8
-        // L2 prefetch of whole row tiles kPrefetchTiles ahead (one bulk-prefetch instruction per tile, issued by the group's
-        // first column block).  Peer-mapped parts are not prefetched (remote data bypasses the local L2).
-        constexpr int kPrefetchTiles = 4;
-        const bool can_prefetch = (cb == 0) && (tl == 0) && p.lda <= 2 * (int64_t)p.K;
-        auto prefetch_tile = [&](int it) {
-            if (!can_prefetch || it >= my_tiles) return;
-            const int64_t m0 = (int64_t)tile_of(it) * BM;
-            const int part = p.n_parts > 1 ? (int)(m0 / p.part_rows) : 0;
-            if (p.n_parts > 1 && part != p.local_part) return;
-            const int64_t rows = min((int64_t)BM, (int64_t)p.M - m0);
-            const float *src = p.A[part] + (m0 - (int64_t)part * p.part_rows) * p.lda;
-            const uint32_t bytes = (uint32_t)(rows * p.lda * 4);
-            asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(src), "r"(bytes) : "memory");
-        };
-        for (int i = 0; i < kPrefetchTiles; ++i) prefetch_tile(i);
-        for (int G = 0; G < total_kb; ++G) {
-            const int stage = G % STAGES;
-            mbar_wait(&empty[stage], (uint32_t)(((G / STAGES) & 1) ^ 1));      // MMAs of k-block G - STAGES retired
-            const int tile = tile_of(G / nkb), kb = G % nkb;
-            if (kb == 0) prefetch_tile(G / nkb + kPrefetchTiles);
-            const int k = kb * BK + kc * 4;
-            if (k < (int)L.kpad8 && !(p.dbg & 8)) {
-                const int64_t m0 = (int64_t)tile * BM;
-                const int part = p.n_parts > 1 ? (int)(m0 / p.part_rows) : 0;
-                const float *base = p.A[part] + (m0 - (int64_t)part * p.part_rows) * p.lda + k;
-                const uint32_t kbytes = k < p.K ? (uint32_t)min(4, p.K - k) * 4u : 0u;
-                const uint32_t dst0 = a_ring_addr + stage * L.a_stage_bytes + (uint32_t)tl * 16u;
 #pragma unroll
-                for (int i = 0; i < kChunks; ++i) {
-                    const int rl = i * 8 + r8;
-                    const bool ok = m0 + rl < p.M;
-                    cp_async16_zfill(dst0 + (uint32_t)i * 1024u, ok ? base + (int64_t)rl * p.lda : p.A[0], ok ? kbytes : 0u);
-                }
-            }
-            // the stage's `landed` barrier completes when the copies of all 64 loader threads have arrived
-            asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(smem_u32(&landed[stage])) : "memory");
+    for (int s = 0; s < STAGES - 1; ++s) load_stage(s);
+
+    {   // W_b: split into hi / lo, once per CTA; columns beyond n_b and rows beyond K are zeros
+        const float *B = p.B[cb];
+        const int64_t ldb = p.ldb[cb];
+        const bool tb = p.transb[cb] != 0;
+        for (int idx = tid; idx < kUN * kpad; idx += kThreads) {
+            int n, k;
+            if (tb) { n = idx / kpad; k = idx % kpad; } else { k = idx / kUN; n = idx % kUN; }     // coalesced reads of B
+            const float w = (n < ncols && k < p.K) ? (tb ? B[(int64_t)n * ldb + k] : B[(int64_t)k * ldb + n]) : 0.0f;
+            uint32_t hi, lo;
+            split_tf32(w, hi, lo);
+            const uint32_t off = w_offset(n, k, kpad);
+            *reinterpret_cast<uint32_t *>(w_hi + off) = hi;
+            *reinterpret_cast<uint32_t *>(w_lo + off) = lo;
         }
-    } else if (warp < kProducerWarps) {
-        // ===================== converters: lo = a - trunc_tf32(a) for every landed k-block =====================
-        constexpr int kChunks = (BM * BK / 4) / (kProducerWarps * 32);      // 8 per thread per k-block
-        const int kc = (t >> 3) & 7;                                        // chunk c = t + 128 i
-        for (int G = 0; G < total_kb; ++G) {
-            const int stage = G % STAGES, kb = G % nkb;
-            mbar_wait(&landed[stage], (uint32_t)((G / STAGES) & 1));
-            if (kb * BK + kc * 4 < (int)L.kpad8 && !(p.dbg & 1)) {
-                uint8_t *sraw = a_ring + stage * L.a_stage_bytes + t * 16;
+        if (tid < kUN) s_bias[tid] = (p.bias[cb] != nullptr && tid < ncols) ? p.bias[cb][tid] : 0.0f;
+    }
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");      // generic-proxy stores of W -> visible to wgmma
+    __syncthreads();
+
+    const uint32_t w_hi_addr = smem_u32(w_hi), w_lo_addr = smem_u32(w_lo), sbo = (uint32_t)kpad * 32u;
+    // fragment coordinates: warpgroup wg owns rows [64 wg, 64 wg + 64), warp w of it rows 16 w .. 16 w + 15
+    const int frag_row = (warp >> 2) * 64 + (warp & 3) * 16 + (lane >> 2);
+    const int frag_col = lane & 3;
+    const int act = p.act[cb];
+    float *C = p.C[cb];
+    const int64_t ldc = p.ldc[cb];
+    const bool vec2 = (ldc % 2) == 0 && (reinterpret_cast<uintptr_t>(C) & 7u) == 0;     // (col, col + 1) as one 8-byte store
+    float acc[64];
 #pragma unroll
-                for (int i = 0; i < kChunks; ++i) {
-                    const float4 v = *reinterpret_cast<const float4 *>(sraw + i * 2048);
-                    float4 l;
-                    l.x = v.x - __uint_as_float(__float_as_uint(v.x) & 0xFFFFE000u);
-                    l.y = v.y - __uint_as_float(__float_as_uint(v.y) & 0xFFFFE000u);
-                    l.z = v.z - __uint_as_float(__float_as_uint(v.z) & 0xFFFFE000u);
-                    l.w = v.w - __uint_as_float(__float_as_uint(v.w) & 0xFFFFE000u);
-                    *reinterpret_cast<float4 *>(sraw + BM * BK * 4 + i * 2048) = l;
-                }
-            }
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&full[stage]);
+    for (int i = 0; i < 64; ++i) acc[i] = 0.0f;
+
+    // A fragments (m16n8k8 layout per warp) of the stage's four k-steps, split into hi / lo, in two register sets: the MMAs of
+    // stage j - 1 read one set while stage j loads and splits into the other, and are waited for only then
+    uint32_t ah[2][BK / 8][4], al[2][BK / 8][4];
+    auto stage = [&](auto parity, int j) {
+        constexpr int P = decltype(parity)::value;
+        asm volatile("cp.async.wait_group %0;" ::"n"(STAGES - 2) : "memory");
+        __syncthreads();                          // stage j landed for every thread; stage j - 1 is no longer read
+        load_stage(j + STAGES - 1);
+        const int kb = j % kb_per_tile;
+        const float *As = reinterpret_cast<const float *>(ring + (size_t)(j % STAGES) * kStageBytes);
+#pragma unroll
+        for (int ks = 0; ks < BK / 8; ++ks) {
+            const float *a_r0 = As + frag_row * kApitch + ks * 8 + frag_col;
+            const float *a_r8 = a_r0 + 8 * kApitch;
+            split_tf32(a_r0[0], ah[P][ks][0], al[P][ks][0]);
+            split_tf32(a_r8[0], ah[P][ks][1], al[P][ks][1]);
+            split_tf32(a_r0[4], ah[P][ks][2], al[P][ks][2]);
+            split_tf32(a_r8[4], ah[P][ks][3], al[P][ks][3]);
         }
-    } else if (warp == kProducerWarps + kEpilogueWarps) {
-        // ===================== MMA issuer (warp-uniform loop, one elected lane issues; see the TS kernel) =====================
-        const uint32_t idesc = make_idesc(un);
-        const uint32_t sbo_b = (L.kpad8 / 4) * 128u;
-        const uint64_t dbh0 = make_desc_sbo(smem_u32(b_hi_ptr), sbo_b), dbl0 = make_desc_sbo(smem_u32(b_lo_ptr), sbo_b);
-        const uint32_t a_ring0 = smem_u32(a_ring);
-        int stage = 0, kb = 0, it = 0;
-        uint32_t stage_phase = 0;
-        for (int G = 0; G < total_kb; ++G) {
-            const int buf = it & 1;
-            if (kb == 0) mbar_wait(&acc_empty[buf], (uint32_t)(((it >> 1) & 1) ^ 1));
-            mbar_wait(&full[stage], stage_phase);
-            tc_fence_after();
-            const uint32_t d_tmem = tmem_base + (uint32_t)(buf * kUN);
-            const uint32_t a_raw = a_ring0 + (uint32_t)stage * L.a_stage_bytes;
-            const uint64_t dah0 = make_desc_sbo(a_raw, 1024u), dal0 = make_desc_sbo(a_raw + BM * BK * 4, 1024u);
-            const uint64_t dbh = dbh0 + (uint64_t)(kb * 64), dbl = dbl0 + (uint64_t)(kb * 64);
-            const int steps = kb == nkb - 1 ? last_steps : BK / UMMA_K;
-            if (elect_one()) {
+        wgmma_wait_all();                         // the MMAs of stage j - 1 (the other register set) have retired
+        wgmma_fence();                            // wgmma may only read registers written before the fence
 #pragma unroll
-                for (int j = 0; j < BK / UMMA_K; ++j) {
-                    if (j < steps) {
-                        const uint64_t o = (uint64_t)(j * 16);
-                        if (p.dbg & 2) { umma_tf32(d_tmem, dah0 + o, dbh + o, idesc, (kb | j) != 0); continue; }
-                        umma_tf32(d_tmem, dal0 + o, dbh + o, idesc, (kb | j) != 0);
-                        umma_tf32(d_tmem, dah0 + o, dbl + o, idesc, 1u);
-                        umma_tf32(d_tmem, dah0 + o, dbh + o, idesc, 1u);
+        for (int ks = 0; ks < BK / 8; ++ks) {
+            const int kg = kb * BK + ks * 8;
+            if (kg < kpad) {                      // block-uniform: skips the k-steps beyond K rounded up to 8
+                const uint32_t koff = (uint32_t)(kg >> 2) * 128u;
+                const uint64_t dh = make_desc(w_hi_addr + koff, sbo), dl = make_desc(w_lo_addr + koff, sbo);
+                wgmma_m64n128k8(acc, al[P][ks], dh, (kb | ks) != 0);
+                wgmma_m64n128k8(acc, ah[P][ks], dl, 1u);
+                wgmma_m64n128k8(acc, ah[P][ks], dh, 1u);
+            }
+        }
+        wgmma_commit();
+        if (kb == kb_per_tile - 1) {              // epilogue of the tile: + bias -> act -> C
+            wgmma_wait_all();
+            const int64_t row0 = (int64_t)tile_index(p, group, j / kb_per_tile) * BM + frag_row;
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int64_t row = row0 + 8 * h;
+                if (row < p.M) {
+                    float *crow = C + row * ldc;
+#pragma unroll
+                    for (int nb8 = 0; nb8 < kUN / 8; ++nb8) {
+                        const int col = nb8 * 8 + 2 * frag_col;
+                        const float v0 = apply_act(acc[4 * nb8 + 2 * h] + s_bias[col], act);
+                        const float v1 = apply_act(acc[4 * nb8 + 2 * h + 1] + s_bias[col + 1], act);
+                        if (vec2 && col + 1 < ncols) {
+                            *reinterpret_cast<float2 *>(crow + col) = make_float2(v0, v1);
+                        } else {
+                            if (col < ncols) crow[col] = v0;
+                            if (col + 1 < ncols) crow[col + 1] = v1;
+                        }
                     }
                 }
-                umma_commit(&empty[stage]);
-                if (kb == nkb - 1) umma_commit(&acc_full[buf]);
             }
-            __syncwarp();
-            if (++stage == STAGES) { stage = 0; stage_phase ^= 1u; }
-            if (++kb == nkb) { kb = 0; ++it; }
         }
-    } else {
-        epilogue_loop(p, cb, group, un, ncols, tmem_base, stage_base, s_bias, acc_full, acc_empty, my_tiles, warp, lane);
+    };
+    for (int j = 0; j < total; j += 2) {
+        stage(std::integral_constant<int, 0>(), j);
+        if (j + 1 < total) stage(std::integral_constant<int, 1>(), j + 1);
     }
-    __syncthreads();
-    if (warp == 0) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(kTmemColsProj) : "memory");
-    }
-}
-
-// ---- variant with the A operands in tensor memory ("TS" form of tcgen05.mma) -----------------------------------------------
-// Measured on the kernel above (TFGK_PROJ_DEBUG switches, profiles/r2_notes.md): a ring stage makes one trip
-// free -> load -> convert -> MMA -> commit -> free in ~3000 cycles whatever its size, and next to the resident W the ring
-// holds raw + lo tiles for only 96 K-columns - less than one 128 x 104 row tile - so a row tile costs about one full trip
-// (4.3 us) where its 39 MMAs need 1.3 us.  Here the ring in shared memory holds RAW k-blocks only (16 KB per 32 columns,
-// up to six stages) and the split operands live in TENSOR MEMORY: the converter warps read their own row of a landed
-// k-block, compute hi = trunc_tf32(a) and lo = a - hi in registers and store both with tcgen05.st into a 4-slot ring
-// (2 x 32 columns per slot) next to the two accumulators: 256 + 256 = all 512 TMEM columns.  The MMAs then take A from
-// tensor memory and only W from shared memory, which also halves their shared-memory traffic.  Twice the K-columns in
-// flight in shared memory plus four k-blocks in tensor memory cover the trip latency.
-constexpr int kTsSlots = 4;
-constexpr int kTsTmemCols = 512;
-constexpr int kTsBarrierBytes = 256;
-constexpr int kTsAcol0 = 2 * kUN;                 // first TMEM column of the A ring
-
-struct PlanTS {
-    uint32_t kpad8, b_bytes, raw_bytes, stages, total;
-    __host__ __device__ explicit PlanTS(int K) {
-        kpad8 = (uint32_t)((K + 7) / 8) * 8;
-        b_bytes = (uint32_t)kUN * kpad8 * 4u;
-        raw_bytes = BM * BK * 4u;
-        const uint32_t fixed = 2u * b_bytes + kEpilogueWarps * kStageBytes + kTsBarrierBytes + kUN * 4u;
-        const uint32_t budget = 227u * 1024u;
-        stages = 0;
-        for (uint32_t st = 6; st >= 2; --st)
-            if (fixed + st * raw_bytes <= budget) { stages = st; break; }
-        total = fixed + stages * raw_bytes;
-    }
-};
-
-__device__ __forceinline__ void umma_tf32_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %2, %3, p;\n\t}"
-        ::"r"(d_tmem), "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate) : "memory");
-}
-
-#define TFGK_ST32(taddr, v)                                                                                                    \
-    asm volatile("tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "                                                              \
-                 "{%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,"                                                   \
-                 "%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32};"                                          \
-                 ::"r"(taddr), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]),         \
-                   "r"(v[8]), "r"(v[9]), "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15]),               \
-                   "r"(v[16]), "r"(v[17]), "r"(v[18]), "r"(v[19]), "r"(v[20]), "r"(v[21]), "r"(v[22]), "r"(v[23]),             \
-                   "r"(v[24]), "r"(v[25]), "r"(v[26]), "r"(v[27]), "r"(v[28]), "r"(v[29]), "r"(v[30]), "r"(v[31]) : "memory")
-
-template <int STAGES>
-__global__ void __launch_bounds__(kThreadsProj, 1) gemm_proj_ts_kernel(const Params p) {
-    extern __shared__ __align__(1024) uint8_t smem[];
-    const PlanTS L(p.K);
-    uint8_t *b_hi_ptr = smem, *b_lo_ptr = smem + L.b_bytes;
-    uint8_t *raw_ring = smem + 2 * L.b_bytes;
-    uint8_t *stage_base = raw_ring + STAGES * L.raw_bytes;
-    uint64_t *landed = reinterpret_cast<uint64_t *>(stage_base + kEpilogueWarps * kStageBytes);
-    uint64_t *smem_free = landed + STAGES, *full_t = smem_free + STAGES, *tmem_free = full_t + kTsSlots;
-    uint64_t *acc_full = tmem_free + kTsSlots, *acc_empty = acc_full + 2;
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(acc_empty + 2);
-    float *s_bias = reinterpret_cast<float *>(reinterpret_cast<uint8_t *>(landed) + kTsBarrierBytes);
-    const int t = threadIdx.x, warp = t >> 5, lane = t & 31;
-    const int cb = (int)blockIdx.x % p.nb, group = (int)blockIdx.x / p.nb;
-    const int ncols = p.ncols[cb];
-    const int un = ((ncols + 15) / 16) * 16;
-    const float *__restrict__ Bm = p.B[cb];
-    const int64_t ldb = p.ldb[cb];
-    const bool tb = p.transb[cb] != 0;
-
-    for (int i = t; i < kUN; i += kThreadsProj) s_bias[i] = (p.bias[cb] != nullptr && i < ncols) ? __ldg(p.bias[cb] + i) : 0.0f;
-    if (t == 0) {
-        for (int i = 0; i < STAGES; ++i) { mbar_init(&landed[i], kLoaderWarps * 32); mbar_init(&smem_free[i], kProducerWarps); }
-        for (int i = 0; i < kTsSlots; ++i) { mbar_init(&full_t[i], kProducerWarps); mbar_init(&tmem_free[i], 1); }
-        for (int i = 0; i < 2; ++i) { mbar_init(&acc_full[i], 1); mbar_init(&acc_empty[i], kEpilogueWarps); }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 0) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(kTsTmemCols) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    {   // W_b: transpose + RNA split into the K-major core-matrix layout, once per CTA
-        const int kchunks = (int)L.kpad8 / 4;
-        const int total = un * kchunks;
-        const uint32_t bh = smem_u32(b_hi_ptr), bl = smem_u32(b_lo_ptr);
-        for (int c = t; c < total; c += kThreadsProj) {
-            const int n8 = c & 7, kc = (c >> 3) % kchunks, ng = (c >> 3) / kchunks;
-            const int n = ng * 8 + n8, k = kc * 4;
-            float w[4] = {0.f, 0.f, 0.f, 0.f}, h[4], l[4];
-            if (n < ncols) {
-#pragma unroll
-                for (int i = 0; i < 4; ++i)
-                    if (k + i < p.K) w[i] = __ldg(tb ? Bm + (int64_t)n * ldb + (k + i) : Bm + (int64_t)(k + i) * ldb + n);
-            }
-#pragma unroll
-            for (int i = 0; i < 4; ++i) split_tf32(w[i], h[i], l[i]);
-            st_shared_v4(bh + c * 16, h[0], h[1], h[2], h[3]);
-            st_shared_v4(bl + c * 16, l[0], l[1], l[2], l[3]);
-        }
-    }
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-    const int nkb = (int)(L.kpad8 + BK - 1) / BK;
-    const int last_steps = ((int)L.kpad8 - (nkb - 1) * BK) / UMMA_K;
-    const int my_tiles = group < p.tiles_m ? (p.tiles_m - 1 - group) / p.n_groups + 1 : 0;
-    const int total_kb = my_tiles * nkb;
-
-    if (warp >= kLoaderWarp0) {
-        // ===================== loaders: raw k-blocks, row-major with the 16-byte chunks XOR-swizzled by row =====================
-        const int tl = t - kLoaderWarp0 * 32;                                // 0..63
-        const uint32_t ring_addr = smem_u32(raw_ring);
-        const int kc = tl & 7, rsub = tl >> 3;                               // a warp covers 4 rows x 128 contiguous bytes
-        constexpr int kPrefetchTiles = 4;
-        const bool can_prefetch = (cb == 0) && (tl == 0) && p.lda <= 2 * (int64_t)p.K;
-        auto prefetch_tile = [&](int it) {
-            if (!can_prefetch || it >= my_tiles) return;
-            const int64_t m0 = (int64_t)tile_index(p, group, it) * BM;
-            const int part = p.n_parts > 1 ? (int)(m0 / p.part_rows) : 0;
-            if (p.n_parts > 1 && part != p.local_part) return;
-            const int64_t rows = min((int64_t)BM, (int64_t)p.M - m0);
-            const float *src = p.A[part] + (m0 - (int64_t)part * p.part_rows) * p.lda;
-            asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(src), "r"((uint32_t)(rows * p.lda * 4)) : "memory");
-        };
-        for (int i = 0; i < kPrefetchTiles; ++i) prefetch_tile(i);
-        for (int G = 0; G < total_kb; ++G) {
-            const int stage = G % STAGES;
-            mbar_wait(&smem_free[stage], (uint32_t)(((G / STAGES) & 1) ^ 1));
-            const int tile = tile_index(p, group, G / nkb), kb = G % nkb;
-            if (kb == 0) prefetch_tile(G / nkb + kPrefetchTiles);
-            const int k = kb * BK + kc * 4;
-            if (k < (int)L.kpad8 && !(p.dbg & 8)) {
-                const int64_t m0 = (int64_t)tile * BM;
-                const int part = p.n_parts > 1 ? (int)(m0 / p.part_rows) : 0;
-                const float *base = p.A[part] + (m0 - (int64_t)part * p.part_rows) * p.lda + k;
-                const uint32_t kbytes = k < p.K ? (uint32_t)min(4, p.K - k) * 4u : 0u;
-                const uint32_t dst0 = ring_addr + stage * L.raw_bytes;
-#pragma unroll
-                for (int i = 0; i < 16; ++i) {
-                    const int rl = i * 8 + rsub;
-                    const bool ok = m0 + rl < p.M;
-                    cp_async16_zfill(dst0 + (uint32_t)rl * 128u + (uint32_t)((kc ^ (rl & 7)) * 16),
-                                     ok ? base + (int64_t)rl * p.lda : p.A[0], ok ? kbytes : 0u);
-                }
-            }
-            asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(smem_u32(&landed[stage])) : "memory");
-        }
-    } else if (warp < kProducerWarps) {
-        // ===================== converters: own row of a landed k-block -> (hi, lo) -> tensor memory =====================
-        const uint32_t lane_field = (uint32_t)(warp * 32) << 16;             // this warp's TMEM lane quarter
-        // software pipelined: the tensor-memory stores of k-block G are issued, and only after the shared-memory reads and
-        // the split of k-block G+1 does the warp wait for them and publish G (tcgen05.wait::st latency off the critical path)
-        int prev_slot = -1, prev_stage = -1;
-        auto publish_prev = [&]() {
-            if (prev_slot < 0) return;
-            asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) { mbar_arrive(&full_t[prev_slot]); mbar_arrive(&smem_free[prev_stage]); }
-        };
-        for (int G = 0; G < total_kb; ++G) {
-            const int stage = G % STAGES, slot = G % kTsSlots, kb = G % nkb;
-            mbar_wait(&landed[stage], (uint32_t)((G / STAGES) & 1));
-            uint32_t hi[32], lo[32];
-            const uint8_t *row = raw_ring + stage * L.raw_bytes + t * 128;
-#pragma unroll
-            for (int c = 0; c < 8; ++c) {
-                float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-                if (kb * BK + c * 4 < (int)L.kpad8 && !(p.dbg & 1)) v = *reinterpret_cast<const float4 *>(row + ((c ^ (t & 7)) * 16));
-                const float a[4] = {v.x, v.y, v.z, v.w};
-#pragma unroll
-                for (int e = 0; e < 4; ++e) {
-                    const uint32_t h = __float_as_uint(a[e]) & 0xFFFFE000u;
-                    hi[c * 4 + e] = h;
-                    lo[c * 4 + e] = __float_as_uint(a[e] - __uint_as_float(h));
-                }
-            }
-            publish_prev();
-            mbar_wait(&tmem_free[slot], (uint32_t)(((G / kTsSlots) & 1) ^ 1));      // MMAs of k-block G - 4 retired
-            tc_fence_after();
-            const uint32_t taddr = tmem_base + lane_field + (uint32_t)(kTsAcol0 + slot * 64);
-            TFGK_ST32(taddr, hi);
-            TFGK_ST32(taddr + 32u, lo);
-            prev_slot = slot; prev_stage = stage;
-        }
-        publish_prev();
-    } else if (warp == kProducerWarps + kEpilogueWarps) {
-        // ===================== MMA issuer: A from tensor memory, W from shared memory =====================
-        // The whole warp walks the loop with warp-uniform values and one elected lane issues: written as `if (lane == 0)`
-        // the compiler wrapped every tcgen05.mma in an ELECT / BRA.U.ANY sequence and rebuilt both descriptors with integer
-        // divisions per k-block - ~130 issue cycles per MMA against the 64 cycles the tensor core needs for it, which made
-        // this single thread the critical path of the kernel (profiles/r2_notes.md).  Counters are carried, the W descriptors
-        // advance by constants (the address field counts 16-byte units).
-        const uint32_t idesc = make_idesc(un);
-        const uint32_t sbo_b = (L.kpad8 / 4) * 128u;
-        const uint64_t dbh0 = make_desc_sbo(smem_u32(b_hi_ptr), sbo_b), dbl0 = make_desc_sbo(smem_u32(b_lo_ptr), sbo_b);
-        const uint32_t a_ring0 = tmem_base + (uint32_t)kTsAcol0;
-        int slot = 0, kb = 0, it = 0;
-        uint32_t slot_phase = 0;
-        for (int G = 0; G < total_kb; ++G) {
-            const int buf = it & 1;
-            if (kb == 0) mbar_wait(&acc_empty[buf], (uint32_t)(((it >> 1) & 1) ^ 1));
-            mbar_wait(&full_t[slot], slot_phase);
-            tc_fence_after();
-            const uint32_t d_tmem = tmem_base + (uint32_t)(buf * kUN);
-            const uint32_t a_hi = a_ring0 + (uint32_t)(slot * 64);
-            const uint64_t dbh = dbh0 + (uint64_t)(kb * 64), dbl = dbl0 + (uint64_t)(kb * 64);      // + kb * 1024 bytes
-            const int steps = kb == nkb - 1 ? last_steps : BK / UMMA_K;
-            if (elect_one()) {
-#pragma unroll
-                for (int j = 0; j < BK / UMMA_K; ++j) {
-                    if (j < steps) {
-                        const uint64_t bh = dbh + (uint64_t)(j * 16), bl = dbl + (uint64_t)(j * 16);           // + j * 256 bytes
-                        const uint32_t ah = a_hi + (uint32_t)(j * UMMA_K), al = ah + 32u;
-                        if (p.dbg & 2) { umma_tf32_ts(d_tmem, ah, bh, idesc, (kb | j) != 0); continue; }
-                        umma_tf32_ts(d_tmem, al, bh, idesc, (kb | j) != 0);
-                        umma_tf32_ts(d_tmem, ah, bl, idesc, 1u);
-                        umma_tf32_ts(d_tmem, ah, bh, idesc, 1u);
-                    }
-                }
-                umma_commit(&tmem_free[slot]);
-                if (kb == nkb - 1) umma_commit(&acc_full[buf]);
-            }
-            __syncwarp();
-            if (++slot == kTsSlots) { slot = 0; slot_phase ^= 1u; }
-            if (++kb == nkb) { kb = 0; ++it; }
-        }
-    } else {
-        epilogue_loop(p, cb, group, un, ncols, tmem_base, stage_base, s_bias, acc_full, acc_empty, my_tiles, warp, lane);
-    }
-    __syncthreads();
-    if (warp == 0) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(kTsTmemCols) : "memory");
-    }
-}
-
-template <int STAGES>
-static int launch_ts(const Params &p, int grid, uint32_t smem_bytes, cudaStream_t st) {
-    static int configured[16] = {0};
-    int dev = 0;
-    TFGK_CUDA(cudaGetDevice(&dev));
-    if (dev < 0 || dev >= 16 || configured[dev] < (int)smem_bytes) {
-        TFGK_CUDA(cudaFuncSetAttribute(gemm_proj_ts_kernel<STAGES>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes));
-        if (dev >= 0 && dev < 16) configured[dev] = (int)smem_bytes;
-    }
-    gemm_proj_ts_kernel<STAGES><<<grid, kThreadsProj, smem_bytes, st>>>(p);
-    TFGK_LAUNCH_CHECK();
-    return TFGK_OK;
+    wgmma_wait_all();
+    asm volatile("cp.async.wait_group 0;" ::: "memory");
 }
 
 template <int STAGES>
 static int launch(const Params &p, int grid, uint32_t smem_bytes, cudaStream_t st) {
-    static int configured[16] = {0};       // cudaFuncSetAttribute once per device, not per call
-    int dev = 0;
-    TFGK_CUDA(cudaGetDevice(&dev));
-    if (dev < 0 || dev >= 16 || configured[dev] < (int)smem_bytes) {
-        TFGK_CUDA(cudaFuncSetAttribute(gemm_proj_kernel<STAGES>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes));
-        if (dev >= 0 && dev < 16) configured[dev] = (int)smem_bytes;
-    }
-    gemm_proj_kernel<STAGES><<<grid, kThreadsProj, smem_bytes, st>>>(p);
+    TFGK_CUDA(ensure_dynamic_smem(gemm_proj_kernel<STAGES>, smem_bytes));
+    gemm_proj_kernel<STAGES><<<grid, kThreads, smem_bytes, st>>>(p);
     TFGK_LAUNCH_CHECK();
     return TFGK_OK;
 }
@@ -666,21 +287,20 @@ extern "C" int tfgk_gemm_proj_f32(const float *const *A_parts, int32_t n_parts, 
     TFGK_CHECK_ARG(first_part >= 0 && first_part < n_parts, "gemm_proj: first_part=%d out of range", first_part);
     if (M == 0) return TFGK_OK;
     if (n_parts > 1)
-        TFGK_CHECK_ARG(part_rows > 0 && part_rows % tc::BM == 0 && (int64_t)n_parts * part_rows >= M,
-                       "gemm_proj: part_rows=%lld must be a positive multiple of %d covering M=%d", (long long)part_rows, tc::BM, M);
-    if (K > 512 || (lda % 4) != 0 || lda < K) return TFGK_ERR_UNSUPPORTED;        // same accuracy bound as gemm_tc.cu
+        TFGK_CHECK_ARG(part_rows > 0 && part_rows % proj::BM == 0 && (int64_t)n_parts * part_rows >= M,
+                       "gemm_proj: part_rows=%lld must be a positive multiple of %d covering M=%d", (long long)part_rows, proj::BM, M);
+    // K <= 512: tensor-core accumulation truncates, so the error grows with K; up to K = 512 it stays below 5e-6 relative
+    if (K > 512 || (lda % 4) != 0 || lda < K) return TFGK_ERR_UNSUPPORTED;
     proj::Params p;
     for (int i = 0; i < proj::kMaxParts; ++i) {
         p.A[i] = A_parts[i < n_parts ? i : 0];
         if (!aligned16(p.A[i]) || p.A[i] == nullptr) return i < n_parts && A_parts[i] == nullptr
             ? set_error(TFGK_ERR_INVALID_ARGUMENT, "gemm_proj: A part %d is null", i) : TFGK_ERR_UNSUPPORTED;
     }
-    p.lda = lda; p.part_rows = n_parts > 1 ? part_rows : (int64_t)1 << 40; p.n_parts = n_parts;
+    p.lda = lda; p.part_rows = n_parts > 1 ? part_rows : (int64_t)1 << 40;
     p.M = M; p.K = K; p.nb = n_blocks;
-    { const char *d = getenv("TFGK_PROJ_DEBUG"); p.dbg = d ? atoi(d) : 0; }
-    p.tiles_m = (int)ceil_div64(M, tc::BM);
-    p.first_tile = n_parts > 1 ? (int)((int64_t)first_part * part_rows / tc::BM) : 0;
-    p.local_part = n_parts > 1 ? (first_part + n_parts - 1) % n_parts : 0;      // the walk starts one past the caller's own part
+    p.tiles_m = (int)ceil_div64(M, proj::BM);
+    p.first_tile = n_parts > 1 ? (int)((int64_t)first_part * part_rows / proj::BM) : 0;
     if (p.first_tile >= p.tiles_m) p.first_tile = 0;
     for (int b = 0; b < proj::kMaxBlocks; ++b) {
         const tfgk_proj_block &blk = blocks[b < n_blocks ? b : 0];
@@ -696,7 +316,8 @@ extern "C" int tfgk_gemm_proj_f32(const float *const *A_parts, int32_t n_parts, 
         p.C[b] = blk.C; p.ldc[b] = blk.ldc;
     }
     const proj::Plan L(K);
-    if (L.stages == 0) return TFGK_ERR_UNSUPPORTED;
+    if (L.stages == 0) return TFGK_ERR_UNSUPPORTED;     // W (hi | lo) does not fit next to two A stages
+    p.kpad = (int)L.kpad;
     int dev = 0, sms = 0;
     TFGK_CUDA(cudaGetDevice(&dev));
     TFGK_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
@@ -707,19 +328,6 @@ extern "C" int tfgk_gemm_proj_f32(const float *const *A_parts, int32_t n_parts, 
     p.n_groups = n_groups;
     const int grid = n_groups * n_blocks;
     cudaStream_t st = as_stream(stream);
-    {   // A operands through tensor memory (TFGK_PROJ_IMPL=ss selects the all-shared-memory kernel)
-        const char *impl = getenv("TFGK_PROJ_IMPL");
-        const proj::PlanTS LT(K);
-        if (!(impl != nullptr && impl[0] == 's') && LT.stages >= 2) {
-            switch (LT.stages) {
-                case 6: return proj::launch_ts<6>(p, grid, LT.total, st);
-                case 5: return proj::launch_ts<5>(p, grid, LT.total, st);
-                case 4: return proj::launch_ts<4>(p, grid, LT.total, st);
-                case 3: return proj::launch_ts<3>(p, grid, LT.total, st);
-                default: return proj::launch_ts<2>(p, grid, LT.total, st);
-            }
-        }
-    }
     if (L.stages >= 4) return proj::launch<4>(p, grid, L.total, st);
     if (L.stages == 3) return proj::launch<3>(p, grid, L.total, st);
     return proj::launch<2>(p, grid, L.total, st);

@@ -57,14 +57,13 @@ extern "C" int tfgk_peer_pull(const void *src, void *dst, int64_t bytes, int32_t
     TFGK_CHECK_ARG(src != nullptr && dst != nullptr && bytes % 16 == 0 && aligned16(src) && aligned16(dst),
                    "peer_pull: buffers must be 16-byte aligned and a multiple of 16 bytes");
     if (max_ctas < 0) {
-        // copy engine: measured 741 GB/s against 663 GB/s for the kernel on >= 148 CTAs (profiles/r2_peer_pull.json) and it
-        // leaves every SM to the projection GEMM that runs beside it
+        // copy engine: it leaves every SM to the projection GEMM that runs beside it
         TFGK_CUDA(cudaMemcpyAsync(dst, src, (size_t)bytes, cudaMemcpyDeviceToDevice, as_stream(stream)));
         return TFGK_OK;
     }
     const int64_t n_vec = bytes / 16;
     int64_t blocks = ceil_div64(n_vec, 256 * 8);
-    const int cap = max_ctas > 0 ? max_ctas : 148;
+    const int cap = max_ctas > 0 ? max_ctas : sm_count();
     if (blocks > cap) blocks = cap;
     peer_pull_kernel<<<(unsigned)blocks, 256, 0, as_stream(stream)>>>(static_cast<const uint4 *>(src), static_cast<uint4 *>(dst), n_vec);
     TFGK_LAUNCH_CHECK();

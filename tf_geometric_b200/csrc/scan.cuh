@@ -110,7 +110,7 @@ static inline size_t align_up(size_t x, size_t a = 256) { return (x + a - 1) / a
 static inline unsigned grid_for(int64_t n, int threads = 256) {
     int64_t b = ceil_div64(n, threads);
     if (b < 1) b = 1;
-    if (b > 148 * 32) b = 148 * 32;   // grid-stride loops: 32 CTAs of 256 threads per SM is plenty
+    if (b > sm_count() * 32) b = sm_count() * 32;   // grid-stride loops: 32 CTAs of 256 threads per SM is plenty
     return (unsigned)b;
 }
 

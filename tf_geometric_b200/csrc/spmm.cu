@@ -473,7 +473,7 @@ static int dispatch_spmm_stream(const SpmmParams &p, cudaStream_t st) {
 // ------------------------------------------------------------------------------------------------------------
 // cp.async variant.  Register double-buffering cannot overlap two gather rounds: a warp has six counting scoreboard
 // slots, ptxas puts the loads of both rounds on the same slots, and the first use of round g then also waits for
-// round g+1 (decoded from SASS, profiles/r1_notes.md).  LDGSTS copies are tracked by commit groups instead, so a
+// round g+1 (visible in the SASS).  LDGSTS copies are tracked by commit groups instead, so a
 // per-warp shared-memory ring of S stages x U rows keeps (S-1)*U rows in flight per warp with no register cost.
 // Each lane copies - and later reads back - only its own 16-byte slices: shared memory is used as an asynchronous
 // extension of the register file, no cross-lane traffic, no barriers.  Edge streaming as above: a warp owns
@@ -653,33 +653,25 @@ __global__ void __launch_bounds__(kAsyncWarps * 32) spmm_async_kernel(const Spmm
 }
 
 // ------------------------------------------------------------------------------------------------------------
-// TMA tile::gather4 variant (north_star: "staged through TMA into shared memory").  Same edge streaming, ring and
-// arithmetic as spmm_async_kernel, but a round of U = 4 edges is ONE instruction
-//     cp.async.bulk.tensor.2d.shared::cta.global.tile::gather4 [ring stage], [tensor map of h, {0, c0, c1, c2, c3}], [mbarrier]
-// issued by one lane: the TMA unit fetches the four neighbour rows (box = D columns x 1 row each) and completes the
-// stage's mbarrier with 4 * row_bytes transaction bytes.  That is a quarter of the TMA issue rate that sank the 1-D
-// cp.async.bulk variant (one 512-byte copy per row, spmm_bulk_kernel) and frees the 4 LDGSTS issue slots per lane and
-// round of the cp.async ring.  Each warp owns S mbarriers; a stage is re-armed only after every lane has read it
-// (__syncwarp before the elected lane issues).  Rows beyond the edge range repeat a valid row id (the bytes still count
-// towards the stage's transaction total) and are ignored by the consumer.  Same rounding and order => same bits.
+// TMA ring variant (north_star: "staged through TMA into shared memory").  Same edge streaming, ring and arithmetic as
+// spmm_async_kernel, but the neighbour rows of a round of U = 4 edges are fetched by the TMA unit: lane 0 arms the
+// stage's mbarrier with the round's transaction bytes and lanes 0-3 each issue one 1-D cp.async.bulk of a whole row
+// (row_bytes = 4 D), which leaves the LSU issue slots of the cp.async ring to the consumer.  Each warp owns S mbarriers;
+// a stage is re-armed only after every lane has read it (__syncwarp before the copies are issued).  A short last round
+// copies only its valid rows.  Same rounding and order => same bits.
 // ------------------------------------------------------------------------------------------------------------
-struct alignas(64) TensorMap { uint64_t opaque[16]; };      // CUtensorMap (128 bytes), filled by the driver on the host
-
-__device__ __forceinline__ void tma_gather4(uint32_t dst, const TensorMap *map, int c0, int c1, int c2, int c3, uint32_t bar) {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.shared::cta.global.tile::gather4.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4, %5, %6}], [%7];"
-        ::"r"(dst), "l"(map), "r"(0), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(bar) : "memory");
+__device__ __forceinline__ void tma_row(uint32_t dst, const float *src, uint32_t bytes, uint32_t bar) {
+    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+                 ::"r"(dst), "l"(src), "r"(bytes), "r"(bar) : "memory");
 }
 
 template <bool IS_MAX, int S>
-__global__ void __launch_bounds__(kAsyncWarps * 32) spmm_gather4_kernel(const SpmmParams p, uint32_t row_bytes,
-                                                                          const __grid_constant__ TensorMap tmap) {
+__global__ void __launch_bounds__(kAsyncWarps * 32) spmm_tma4_kernel(const SpmmParams p, uint32_t row_bytes) {
     constexpr int U = 4, RPC = 32 / U;
     static_assert(S <= 2 * RPC, "weight look-ahead registers would be overwritten before they are consumed");
     extern __shared__ __align__(128) uint8_t g4_ring[];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const uint32_t tx_bytes = U * row_bytes;
-    const uint32_t stage_bytes = (tx_bytes + 127u) & ~127u;      // TMA destinations are 128-byte aligned
+    const uint32_t stage_bytes = (U * row_bytes + 127u) & ~127u;
     uint8_t *my_ring = g4_ring + (size_t)warp * S * stage_bytes;
     const uint32_t ring_addr = (uint32_t)__cvta_generic_to_shared(my_ring);
     uint64_t *bars = reinterpret_cast<uint64_t *>(g4_ring + (size_t)kAsyncWarps * S * stage_bytes) + warp * S;
@@ -762,22 +754,19 @@ __global__ void __launch_bounds__(kAsyncWarps * 32) spmm_gather4_kernel(const Sp
             if (weighted) wi = ld_stream_f32(p.w + e_begin + e);
         }
     };
-    // round g (edges [4g, 4g+4)) -> ring stage g % S: one gather4, armed and issued by lane 0
+    // round g (edges [4g, 4g+4)) -> ring stage g % S: armed by lane 0, one row copy from each of lanes 0 .. valid-1
     auto issue = [&](int g, int ci) {
         if (g < n_rounds) {
             const int base = (g % RPC) * U;
             const int valid = min(U, n_edges - g * U);
-            const int c0 = __shfl_sync(0xffffffffu, ci, base);
-            int c1 = __shfl_sync(0xffffffffu, ci, base + 1), c2 = __shfl_sync(0xffffffffu, ci, base + 2);
-            int c3 = __shfl_sync(0xffffffffu, ci, base + 3);
-            if (valid < 2) c1 = c0;
-            if (valid < 3) c2 = c0;
-            if (valid < 4) c3 = c0;
-            if (lane == 0) {
-                const uint32_t bar = bar0 + 8 * (uint32_t)(g % S);
-                asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(tx_bytes) : "memory");
-                tma_gather4(ring_addr + (uint32_t)(g % S) * stage_bytes, &tmap, c0, c1, c2, c3, bar);
-            }
+            const int c = __shfl_sync(0xffffffffu, ci, base + (lane < U ? lane : 0));
+            const uint32_t bar = bar0 + 8 * (uint32_t)(g % S);
+            if (lane == 0)
+                asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"((uint32_t)valid * row_bytes)
+                             : "memory");
+            if (lane < valid)
+                tma_row(ring_addr + (uint32_t)(g % S) * stage_bytes + (uint32_t)lane * row_bytes, p.h + (int64_t)c * p.ldh,
+                        row_bytes, bar);
         }
     };
 
@@ -893,49 +882,22 @@ static int launch_spmm_async(const SpmmParams &p, cudaStream_t st) {
     return TFGK_OK;
 }
 
-// cuTensorMapEncodeTiled through the runtime's driver entry point (no link-time dependency on libcuda)
-typedef int (*EncodeTiledFn)(void *map, int dtype, uint32_t rank, void *base, const uint64_t *dims, const uint64_t *strides,
-                             const uint32_t *box, const uint32_t *elem_strides, int interleave, int swizzle, int l2promo,
-                             int oob_fill);
-
-static int make_row_tensor_map(TensorMap *out, const float *h, int64_t ldh, int64_t n_rows, int32_t D) {
-    static EncodeTiledFn encode = nullptr;
-    if (encode == nullptr) {
-        void *fn = nullptr;
-        cudaDriverEntryPointQueryResult qres;
-        TFGK_CUDA(cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres));
-        if (fn == nullptr || qres != cudaDriverEntryPointSuccess)
-            return set_error(TFGK_ERR_UNSUPPORTED, "cuTensorMapEncodeTiled is not available from this driver");
-        encode = reinterpret_cast<EncodeTiledFn>(fn);
-    }
-    const uint64_t dims[2] = {(uint64_t)D, (uint64_t)n_rows};
-    const uint64_t strides[1] = {(uint64_t)ldh * sizeof(float)};          // byte stride of dimension 1 (rows)
-    const uint32_t box[2] = {(uint32_t)D, 1u};                            // gather4: 1 in the gathered dimension
-    const uint32_t elem[2] = {1u, 1u};
-    // CU_TENSOR_MAP_DATA_TYPE_FLOAT32 = 7, INTERLEAVE_NONE = 0, SWIZZLE_NONE = 0, L2_PROMOTION_L2_128B = 2, OOB_FILL_NONE = 0
-    const int rc = encode(out, 7, 2, const_cast<float *>(h), dims, strides, box, elem, 0, 0, 2, 0);
-    if (rc != 0) return set_error(TFGK_ERR_UNSUPPORTED, "cuTensorMapEncodeTiled failed with CUresult %d", rc);
-    return TFGK_OK;
-}
-
 template <int S>
-static int launch_spmm_gather4(const SpmmParams &p, int64_t h_rows, cudaStream_t st) {
-    if (p.D > 256 || p.D % 4 != 0 || p.ldh % 4 != 0) return TFGK_ERR_UNSUPPORTED;
+static int launch_spmm_tma4(const SpmmParams &p, cudaStream_t st) {
+    // cp.async.bulk wants 16-byte aligned rows: D, ldh multiples of 4 floats and an aligned base
+    if (p.D > 256 || p.D % 4 != 0 || p.ldh % 4 != 0 || !aligned16(p.h)) return TFGK_ERR_UNSUPPORTED;
     const uint32_t row_bytes = (uint32_t)p.D * 4u;
     const size_t stage_pitch = ((size_t)4 * row_bytes + 127) & ~(size_t)127;
     const size_t smem = (size_t)kAsyncWarps * S * stage_pitch + (size_t)kAsyncWarps * S * 8;
     if (smem > 200 * 1024) return TFGK_ERR_UNSUPPORTED;
-    TensorMap tmap;
-    const int rc = make_row_tensor_map(&tmap, p.h, p.ldh, h_rows, p.D);
-    if (rc != TFGK_OK) return rc;
     const int64_t n_tasks = p.task_row ? p.n_tasks : ceil_div64(p.n_dst, kAsyncRows);
     const unsigned blocks = (unsigned)ceil_div64(n_tasks, kAsyncWarps);
     if (p.reduce == TFGK_REDUCE_MAX) {
-        TFGK_CUDA(ensure_dynamic_smem(spmm_gather4_kernel<true, S>, smem));
-        spmm_gather4_kernel<true, S><<<blocks, kAsyncWarps * 32, smem, st>>>(p, row_bytes, tmap);
+        TFGK_CUDA(ensure_dynamic_smem(spmm_tma4_kernel<true, S>, smem));
+        spmm_tma4_kernel<true, S><<<blocks, kAsyncWarps * 32, smem, st>>>(p, row_bytes);
     } else {
-        TFGK_CUDA(ensure_dynamic_smem(spmm_gather4_kernel<false, S>, smem));
-        spmm_gather4_kernel<false, S><<<blocks, kAsyncWarps * 32, smem, st>>>(p, row_bytes, tmap);
+        TFGK_CUDA(ensure_dynamic_smem(spmm_tma4_kernel<false, S>, smem));
+        spmm_tma4_kernel<false, S><<<blocks, kAsyncWarps * 32, smem, st>>>(p, row_bytes);
     }
     TFGK_LAUNCH_CHECK();
     if (p.task_row && p.n_hubs > 0) {
@@ -959,28 +921,26 @@ static int dispatch_spmm_async(const SpmmParams &p, cudaStream_t st) {
         if (cfg && cfg[0] == '4' && cfg[2] == '6') return launch_spmm_async<1, 4, 6>(p, st);
         if (cfg && cfg[0] == '2' && cfg[2] == '6') return launch_spmm_async<1, 2, 6>(p, st);
         if (cfg && cfg[0] == '2' && cfg[2] == '4') return launch_spmm_async<1, 2, 4>(p, st);
-        return launch_spmm_async<1, 4, 3>(p, st);      // 99% of the measured HBM peak at D=128 (profiles/r1_kernel_variants_spmm_async.json)
+        return launch_spmm_async<1, 4, 3>(p, st);      // default: four rows per round, three stages
     }
     if (lanes <= 64) return launch_spmm_async<2, 4, 4>(p, st);
     if (lanes <= 96) return launch_spmm_async<3, 4, 3>(p, st);
     return launch_spmm_async<4, 2, 4>(p, st);
 }
 
-// Default kernel: the TMA tile::gather4 ring with three stages for every float4-aligned width up to 256 columns
-// (profiles/r2_kernel_variants_final.json: D = 128 9.55 ms against 9.87 ms for the cp.async ring, D = 100 9.51 against 10.24;
-// three stages beat four, six and eight, which cost resident warps).  TFGK_SPMM_IMPL=async keeps the cp.async ring, which is also
-// the fallback when the driver entry point for tensor maps is unavailable.
-static bool spmm_prefers_gather4(int D) { return D >= 32 && D <= 256; }
+// Default kernel: the TMA row-copy ring with three stages for every float4-aligned width up to 256 columns.
+// TFGK_SPMM_IMPL=async selects the cp.async ring; TFGK_SPMM_TMA_STAGES sets the depth of the TMA ring (2, 3, 4, 6 or 8).
+static bool spmm_prefers_tma4(int D) { return D >= 32 && D <= 256; }
 
 static int spmm_impl_choice() {
     // 0 = register-staged LDG gather, 1 = TMA bulk gather.  TFGK_SPMM_IMPL overrides (read per call: cheap).
     const char *e = getenv("TFGK_SPMM_IMPL");
     if (e && e[0] == 'b') return 1;
     if (e && e[0] == 's') return 2;
-    if (e && (e[0] == 'g' || e[0] == 't')) return 4;      // "gather4" / "tma": TMA tile::gather4 ring
+    if (e && e[0] == 't') return 4;      // "tma": TMA row-copy ring
     if (e && e[0] == 'l') return 0;
     if (e && e[0] == 'a') return 3;      // "async": the cp.async ring for every shape
-    return 5;                            // default: by row shape (spmm_prefers_gather4); "ldg" / "stream" / "bulk" are the measured alternatives
+    return 5;                            // default: by row shape (spmm_prefers_tma4); "ldg" / "stream" / "bulk" are the alternatives
 }
 
 template <int NC>
@@ -1083,17 +1043,15 @@ extern "C" int tfgk_spmm_f32(const int64_t *rowptr, const int32_t *col, const fl
             p.hub_nslots = plan->hub_nslots; p.scratch = plan->scratch;
         }
         const int lanes = (p.D + vec - 1) / vec;
-        const int choice = spmm_impl_choice() == 5 ? (spmm_prefers_gather4(p.D) ? 4 : 3) : spmm_impl_choice();
+        const int choice = spmm_impl_choice() == 5 ? (spmm_prefers_tma4(p.D) ? 4 : 3) : spmm_impl_choice();
         if (vec4 && p.D >= 32 && choice == 4) {
-            // the ABI does not carry the number of source rows: the tensor map is bounded by the index type instead
-            // (column ids were validated against n_cols when the CSR was built)
-            const char *cfg = getenv("TFGK_SPMM_GATHER4_STAGES");
+            const char *cfg = getenv("TFGK_SPMM_TMA_STAGES");
             const int st = cfg ? atoi(cfg) : 3;
-            const int rcg = st == 2 ? launch_spmm_gather4<2>(p, (int64_t)1 << 31, as_stream(stream))
-                          : st == 3 ? launch_spmm_gather4<3>(p, (int64_t)1 << 31, as_stream(stream))
-                          : st == 6 ? launch_spmm_gather4<6>(p, (int64_t)1 << 31, as_stream(stream))
-                          : st == 8 ? launch_spmm_gather4<8>(p, (int64_t)1 << 31, as_stream(stream))
-                                    : launch_spmm_gather4<4>(p, (int64_t)1 << 31, as_stream(stream));
+            const int rcg = st == 2 ? launch_spmm_tma4<2>(p, as_stream(stream))
+                          : st == 3 ? launch_spmm_tma4<3>(p, as_stream(stream))
+                          : st == 6 ? launch_spmm_tma4<6>(p, as_stream(stream))
+                          : st == 8 ? launch_spmm_tma4<8>(p, as_stream(stream))
+                                    : launch_spmm_tma4<4>(p, as_stream(stream));
             if (rcg != TFGK_ERR_UNSUPPORTED) { if (rcg != TFGK_OK) return rcg; continue; }
         }
         if (vec4 && p.D >= 32 && (choice == 3 || choice == 4)) {

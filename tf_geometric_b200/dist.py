@@ -7,7 +7,7 @@ tf.distribute.MirroredStrategy, demo/demo_distributed_gcn.py:37-57); this is the
   * rank r owns destination rows [r*B, min((r+1)*B, N)), B = ceil(N / R), all their in-edges and the same rows of x;
   * dense projections are row-local (weights replicated);
   * each aggregation needs the projected rows of every SOURCE: one all-gather (torch.distributed, NCCL over
-    NVLink/NVSwitch on the GPU box, gloo in the CPU tests) into a [R*B, D] buffer indexed by global node id;
+    NVLink/NVSwitch between GPUs, gloo in the CPU tests) into a [R*B, D] buffer indexed by global node id;
   * softmax / mean / max are per destination, so nothing is reduced across ranks; the GCN normalisation exchanges only
     the [N] vector of deg^-1/2.
 Per-row edge order is the caller's order, so every output row is bit-identical to the single-GPU result.
@@ -76,8 +76,8 @@ class PartitionedGraph(object):
         self._pull_stream = None
         self._work = {}                             # persistent exchange buffers (no per-step allocation of the [N, width] tables)
         self.pull_events = []                       # (start, end) CUDA events around the pulls of each exchange (for bench.py)
-        # peer pulls: copy engine (-1, default: 741 GB/s and no SMs taken from the GEMM running beside it) or the copy kernel
-        # on this many CTAs (TFGK_DIST_PULL_CTAS > 0; 663 GB/s from 148 CTAs on)
+        # peer pulls: copy engine (-1, default: no SMs taken from the GEMM running beside it) or the copy kernel on this many
+        # CTAs (TFGK_DIST_PULL_CTAS > 0)
         self.pull_ctas = int(os.environ.get("TFGK_DIST_PULL_CTAS", "-1"))
         self.nvlink_bytes = 0                       # bytes pulled from / received from peers so far (accounting)
 
@@ -215,8 +215,8 @@ class PartitionedGraph(object):
                 c0 += wd
             return outs
         if self.exchange == "p2p_fused":
-            # measured alternative: the GEMM's producers read the owners' rows in place (tfgk_gemm_proj_f32 a_parts).  Peer
-            # reads bypass the local L2, so every column block re-reads the remote tile, in 64-byte pieces: 54-160 GB/s.
+            # alternative: the GEMM's loads read the owners' rows in place (tfgk_gemm_proj_f32 a_parts).  Peer reads bypass
+            # the local L2, so every column block re-reads the remote tile.
             ex = self._row_exchange(x_local.shape[1], dev)
             slot = ex.publish(x_local)
             outs = [torch.empty((p.padded_nodes, wd), dtype=torch.float32, device=dev) for wd in widths]
@@ -627,7 +627,7 @@ def bench_papers(args, rank, world, device, metric, config):
                 "steps": args.steps, "warmup": max(args.warmup, 3), "ms_per_step": ms_step, "higher_is_better": True,
                 "scaling": "weak", "vs_baseline": None, "dtype": "f32", "data": "synthetic", "config": config,
                 "clocks": clocks, "e2e": None, "gpu_launches": launches,
-                "roofline": {"bound": "hbm", "kernel": "spmm_gather4_kernel<0,3> (tfgk_spmm_f32), rank 0 partition",
+                "roofline": {"bound": "hbm", "kernel": "spmm_tma4_kernel<false,3> (tfgk_spmm_f32), rank 0 partition",
                              "achieved": spmm_bytes / (spmm_ms * 1e-3) / 1e9, "peak": peak, "unit": "GB/s",
                              "frac": spmm_bytes / (spmm_ms * 1e-3) / 1e9 / peak, "traffic": None, "peak_source": peak_src,
                              "algorithmic_bytes": spmm_bytes, "kernel_ms": spmm_ms},
@@ -749,7 +749,7 @@ def bench_partitioned(args, rank, world, device, metric, config):
                 "steps": args.steps, "warmup": max(args.warmup, 3), "ms_per_step": ms_step, "higher_is_better": True,
                 "scaling": "strong", "vs_baseline": None, "dtype": "f32", "data": "synthetic", "config": config,
                 "clocks": clocks, "e2e": e2e, "gpu_launches": launches,
-                "roofline": {"bound": "hbm", "kernel": "gat_gather4_kernel<2> (tfgk_gat_fused_f32), rank 0 partition",
+                "roofline": {"bound": "hbm", "kernel": "gat_tma4_kernel<2> (tfgk_gat_fused_f32), rank 0 partition",
                              "achieved": gat_bytes / (gat_ms * 1e-3) / 1e9, "peak": peak, "unit": "GB/s",
                              "frac": gat_bytes / (gat_ms * 1e-3) / 1e9 / peak, "traffic": None, "peak_source": peak_src,
                              "algorithmic_bytes": gat_bytes, "kernel_ms": gat_ms},

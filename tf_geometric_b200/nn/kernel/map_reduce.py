@@ -1,5 +1,5 @@
 # coding=utf-8
-"""The message-passing primitive of tf_geometric (nn/kernel/map_reduce.py) on the B200 kernels.
+"""The message-passing primitive of tf_geometric (nn/kernel/map_reduce.py) on the CUDA kernels.
 
 `aggregate_neighbors` keeps the reference's mapper / reducer / updater protocol.  When the three callables are the
 stock ones below, the whole gather -> map -> reduce -> update chain is ONE launch of tfgk_spmm_f32 (no [E, D]

@@ -19,7 +19,7 @@ _REDUCE_CODES = {"sum": REDUCE_SUM, "mean": REDUCE_MEAN, "max": REDUCE_MAX}
 
 def _require_cuda():
     if not torch.cuda.is_available():
-        raise RuntimeError("tf_geometric_b200 needs a CUDA device (B200 / sm_100a); there is no CPU fallback")
+        raise RuntimeError("tf_geometric_b200 needs a CUDA device (H100 / sm_90a); there is no CPU fallback")
 
 
 def default_device():

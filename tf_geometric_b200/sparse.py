@@ -1,7 +1,7 @@
 # coding=utf-8
 """SparseMatrix: the subset of tf_sparse.SparseMatrix that tf_geometric's hot path calls
 (nn/conv/gcn.py:56,72-119,262,280; gat.py:83-89; appnp.py:51-55,86; data/graph.py:208-210), backed by the
-destination-sorted CSR + sm_100a kernels instead of tf.gather / tf.math.unsorted_segment_sum.
+destination-sorted CSR + sm_90a kernels instead of tf.gather / tf.math.unsorted_segment_sum.
 
 COO semantics are kept on the outside: `index` int32 [2, nnz] (row = aggregation target), `value` float32 [nnz]
 in the caller's edge order, no sorting or merging is visible.  The CSR (stable sort by row) and the CSR-ordered

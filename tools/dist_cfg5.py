@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 # coding=utf-8
 """BASELINE config 5 (GCN fwd, ogbn-papers100M shape: 111,059,956 nodes / 1,615,685,872 edges / 128 features, destination-
-partitioned over 8 B200s) at an arbitrary rank count with the SAME per-GPU load: every rank owns 13.9 M destination rows and
+partitioned over 8 GPUs) at an arbitrary rank count with the SAME per-GPU load: every rank owns 13.9 M destination rows and
 generates its own ~202 M in-edges on the device (seed 1000 + rank; the global graph is never materialised), x is generated
 per owner rank.  sym=False is not needed here: the GCN normalisation uses row degrees locally and the all-gathered deg^-1/2.
 Run:  torchrun --nproc-per-node R tools/dist_cfg5.py        (R = 8 is the real config; R = 2 keeps the per-GPU sizes)

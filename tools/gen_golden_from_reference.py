@@ -1,8 +1,8 @@
 #!/usr/bin/env python
 # coding=utf-8
-"""Generate tests/golden/ref_exec_*.npz by EXECUTING the reference's own Python (read-only /root/reference) over the
-numpy shims in tools/ref_shim.  Runs only in the authoring container (the reference does not travel to the GPU box);
-the resulting small fixtures are committed.  Re-run:  python tools/gen_golden_from_reference.py
+"""Generate tests/golden/ref_exec_*.npz by EXECUTING the reference's own Python (a read-only checkout of
+CrawlScript/tf_geometric named by $TFG_REFERENCE) over the numpy shims in tools/ref_shim.  The tests never need the
+reference: the resulting small fixtures are committed.  Re-run:  TFG_REFERENCE=<checkout> python tools/gen_golden_from_reference.py
 """
 import importlib
 import os
@@ -13,7 +13,9 @@ import numpy as np
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tools"))
-REFERENCE = os.environ.get("TFG_REFERENCE", "/root/reference")
+REFERENCE = os.environ.get("TFG_REFERENCE")
+if not REFERENCE:
+    raise SystemExit("set TFG_REFERENCE to a checkout of CrawlScript/tf_geometric")
 OUT = os.path.join(ROOT, "tests", "golden")
 
 import ref_shim  # noqa: E402

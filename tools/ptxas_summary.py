@@ -2,7 +2,7 @@
 """Summarise `-Xptxas -v` logs under tf_geometric_b200/csrc/build: registers / spills per kernel."""
 import re, subprocess, sys, glob, os
 root = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "tf_geometric_b200", "csrc", "build")
-pat = re.compile(r"Compiling entry function '(\S+)' for 'sm_100a'\n.*\n\s+(\d+) bytes stack frame, (\d+) bytes spill stores.*\n.*Used (\d+) registers")
+pat = re.compile(r"Compiling entry function '(\S+)' for 'sm_90a'\n.*\n\s+(\d+) bytes stack frame, (\d+) bytes spill stores.*\n.*Used (\d+) registers")
 flt = sys.argv[1] if len(sys.argv) > 1 else None
 for f in sorted(glob.glob(os.path.join(root, "*.ptxas.log"))):
     items = pat.findall(open(f).read())
