@@ -267,7 +267,9 @@ int tfgk_gat_softmax_bwd_f32(const int64_t *rowptr, const int32_t *col, const fl
  *   _dst    : dQ[r] = (1/scale) sum_{e in row r} ds_e K[col_e]                     forward CSR
  *   _src    : dK[c] = (1/scale) sum ds_e Q[row_e],  dV[c] = sum a_e G[row_e]       transposed CSR (rows = sources)
  * with a_e = exp(<Q_r, K_c>/scale - max_r) / den_r and ds_e = a_e (<G_r, V_c> - delta_r) per head.  Replaces TensorFlow
- * autodiff over gat.py:73-114.  TFGK_ERR_UNSUPPORTED for H > 8, non power-of-two head sizes or unaligned operands. */
+ * autodiff over gat.py:73-114.  The forward and the three backward entry points take the same (H, dqk): H a power of two
+ * <= 8, dqk / 4 a power of two, H * dqk <= 128; TFGK_ERR_UNSUPPORTED for any other shape or unaligned operands, and the
+ * caller keeps the coefficient table instead. */
 int tfgk_gat_fused_stats_f32(const int64_t *rowptr, const int32_t *col,
                              const float *Q, int64_t ldq, const float *K, int64_t ldk, const float *V, int64_t ldv,
                              int32_t N, int32_t H, int32_t dqk, int32_t dv, float scale,

@@ -44,6 +44,26 @@ def gcn_forward(x, row, col, normed_value, kernel, bias, relu=True):
     return torch.relu(h) if relu else h
 
 
+def gat_attention(Q, K, V, row, col, num_rows, num_heads, scale=None, bias=None, relu=False):
+    """The attention core of nn/conv/gat.py:73-120 with the heads split and concatenated, on given Q [n_dst, A],
+    K [n_src, A] and V [n_src, H * dv]: per head, a_e = segment_softmax(<Q[row_e], K[col_e]> / scale) over the edges of
+    each destination row, out[r] = sum_e a_e V[col_e], then act(out + bias).  Rows without edges get act(bias).
+    scale defaults to sqrt(A / H) (gat.py:78; set2set.py passes 1).  Differentiable w.r.t. Q, K, V and bias: in float64
+    it is the reference the GAT backward kernels are checked against."""
+    H = int(num_heads)
+    E, A = row.shape[0], Q.shape[1]
+    dqk, dv = A // H, V.shape[1] // H
+    if scale is None:
+        scale = dqk ** 0.5
+    score = (Q.index_select(0, row).reshape(E, H, dqk) * K.index_select(0, col).reshape(E, H, dqk)).sum(-1) / scale
+    att = segment_softmax(score, row, num_rows)                                          # [E, H]
+    msg = (V.index_select(0, col).reshape(E, H, dv) * att.unsqueeze(-1)).reshape(E, H * dv)
+    out = _segment_sum(msg, row, num_rows)
+    if bias is not None:
+        out = out + bias
+    return torch.relu(out) if relu else out
+
+
 def gat_forward(x, row, col, wq, bq, wk, bk, wv, bias, num_heads, relu=True, split_value_heads=True, att_scale=None):
     """nn/conv/gat.py:43-120; row/col already hold the appended self loops (gat.py:43).
     att_scale: optional [num_heads * E'] multiplier standing in for tf.nn.dropout on the attention values (gat.py:85),

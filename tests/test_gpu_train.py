@@ -11,7 +11,7 @@ import pytest
 import torch
 
 import tf_geometric_b200 as tfg
-from tf_geometric_b200 import ops, _structure
+from tf_geometric_b200 import ops, _structure, _ffi
 from oracle import tfg_oracle as o
 from oracle import torch_cpu_port as port
 from conftest import random_graph, assert_close, glorot
@@ -97,18 +97,31 @@ def test_gat_softmax_bwd_matches_restatement(H, dv, split, rate):
 def _port_gat(x, ei_loops, params, H, relu, split, att_scale=None):
     t = [torch.tensor(np.asarray(p, np.float64), requires_grad=True) for p in params]
     row, col = torch.from_numpy(ei_loops[0].astype(np.int64)), torch.from_numpy(ei_loops[1].astype(np.int64))
-    y = port.gat_forward(torch.tensor(x.astype(np.float64)), row, col, t[0], t[1], t[2], t[3], t[4], t[5], H, relu=relu,
+    x64 = torch.tensor(x.astype(np.float64), requires_grad=True)
+    y = port.gat_forward(x64, row, col, t[0], t[1], t[2], t[3], t[4], t[5], H, relu=relu,
                          split_value_heads=split, att_scale=None if att_scale is None else torch.tensor(att_scale))
-    return y, t
+    return y, t, x64
 
 
-@pytest.mark.parametrize("f,a,u,H,split,relu,rate", [
-    (24, 64, 128, 8, True, True, 0.0), (24, 64, 128, 8, True, True, 0.4), (10, 12, 20, 4, True, False, 0.0),
-    (10, 12, 6, 3, False, True, 0.0), (10, 12, 6, 3, False, False, 0.3)])
-def test_gat_gradients_match_reference_autodiff(f, a, u, H, split, relu, rate):
+# path: "recompute" = stats forward + tfgk_gat_bwd_* (heads split, V as wide as Q/K, no dropout, no hub row, H <= 8);
+#       "table"     = coefficient table + tfgk_gat_softmax_bwd_f32 + spmm_heads (everything else)
+# the first five rows keep the ids they had before `hub` and `path` were parameters
+@pytest.mark.parametrize("f,a,u,H,split,relu,rate,hub,path", [
+    pytest.param(24, 64, 128, 8, True, True, 0.0, False, "table", id="24-64-128-8-True-True-0.0"),   # V wider than Q/K
+    pytest.param(24, 64, 128, 8, True, True, 0.4, False, "table", id="24-64-128-8-True-True-0.4"),   # attention dropout
+    pytest.param(10, 12, 20, 4, True, False, 0.0, False, "table", id="10-12-20-4-True-False-0.0"),
+    pytest.param(10, 12, 6, 3, False, True, 0.0, False, "table", id="10-12-6-3-False-True-0.0"),      # averaged heads
+    pytest.param(10, 12, 6, 3, False, False, 0.3, False, "table", id="10-12-6-3-False-False-0.3"),
+    (24, 64, 64, 8, True, True, 0.0, False, "recompute"),      # GAT(64, num_heads=8), attention_units = units
+    (24, 128, 128, 8, True, True, 0.0, False, "recompute"),    # GAT(128, num_heads=8)
+    (16, 32, 32, 4, True, False, 0.0, False, "recompute"),     # no output activation
+    (16, 32, 32, 4, True, True, 0.0, True, "table"),           # a hub destination row: the forward has a hub plan
+    (24, 64, 64, 16, True, True, 0.0, False, "table"),         # GAT(64, num_heads=16): more heads than the backward packs
+    (24, 128, 128, 32, True, True, 0.0, False, "table")])      # GAT(128, num_heads=32)
+def test_gat_gradients_match_reference_autodiff(f, a, u, H, split, relu, rate, hub, path):
     rs = np.random.RandomState(f + a + u)
     n = 350
-    ei = random_graph(n, 2600, seed=a, symmetric=True, isolated=2)
+    ei = random_graph(n, 2600, seed=a, symmetric=True, isolated=2, hub=(5, ops.HUB_THRESHOLD + 100) if hub else None)
     x = rs.randn(n, f).astype(np.float32)
     v_units = u if split else u * H
     params = [glorot(rs, f, a), rs.randn(a).astype(np.float32) * .1, glorot(rs, f, a), rs.randn(a).astype(np.float32) * .1,
@@ -118,10 +131,23 @@ def test_gat_gradients_match_reference_autodiff(f, a, u, H, split, relu, rate):
 
     ei_dev = dev(ei, torch.int32)
     tp = [dev(p).requires_grad_(True) for p in params]
-    y = tfg.nn.gat(dev(x), ei_dev, tp[0], tp[1], tfg.nn.relu, tp[2], tp[3], tfg.nn.relu, tp[4], tp[5],
-                   tfg.nn.relu if relu else None, num_heads=H, split_value_heads=split, edge_drop_rate=rate,
-                   training=True, seed=seed)
-    (y * dev(gout)).sum().backward()
+    xd = dev(x).requires_grad_(True)
+    trace = _ffi.CallTrace()
+    prev = _ffi.set_trace(trace)
+    try:
+        y = tfg.nn.gat(xd, ei_dev, tp[0], tp[1], tfg.nn.relu, tp[2], tp[3], tfg.nn.relu, tp[4], tp[5],
+                       tfg.nn.relu if relu else None, num_heads=H, split_value_heads=split, edge_drop_rate=rate,
+                       training=True, seed=seed)
+        (y * dev(gout)).sum().backward()
+    finally:
+        _ffi.set_trace(prev)
+    recompute, table = trace.counts.get("tfgk_gat_bwd_dst_f32", 0), trace.counts.get("tfgk_gat_softmax_bwd_f32", 0)
+    if path == "recompute":
+        assert recompute == 1 and table == 0, trace.counts
+    elif path == "table":
+        assert table == 1 and recompute == 0, trace.counts
+    else:
+        assert path is None and not trace.counts          # host-logic tests: fake kernels that never reach the C ABI
 
     ei_loops = o.add_self_loop_edge(ei, n)[0]
     att_scale = None
@@ -133,11 +159,12 @@ def test_gat_gradients_match_reference_autodiff(f, a, u, H, split, relu, rate):
         mult = np.empty_like(mult_csr)
         mult[perm] = mult_csr
         att_scale = mult.T.reshape(-1).astype(np.float64)
-    y_ref, t = _port_gat(x, ei_loops, params, H, relu, split, att_scale)
+    y_ref, t, x64 = _port_gat(x, ei_loops, params, H, relu, split, att_scale)
     (y_ref * torch.tensor(gout.astype(np.float64))).sum().backward()
 
     assert_close(host(y), y_ref.detach().numpy(), what="gat training forward")
-    for name, mine, ref in zip(("query_kernel", "query_bias", "key_kernel", "key_bias", "kernel", "bias"), tp, t):
+    for name, mine, ref in zip(("query_kernel", "query_bias", "key_kernel", "key_bias", "kernel", "bias", "x"), tp + [xd],
+                               t + [x64]):
         assert mine.grad is not None, name
         assert_close(host(mine.grad), ref.grad.numpy(), rtol=1e-3, atol_scale=2e-4, what="d loss / d " + name)
 

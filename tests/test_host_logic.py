@@ -114,10 +114,12 @@ def test_training_extras_and_samplers(fake):
     """dropout / GAT backward / drop_edge / samplers: host logic over the numpy restatements of the kernels."""
     test_gpu_train.test_dropout_mask_bit_exact(4099, 0.9)
     test_gpu_train.test_spmm_heads_bit_exact(3, 5, "split", True, 0.0)
-    test_gpu_train.test_gat_gradients_match_reference_autodiff(24, 64, 128, 8, True, True, 0.4)
-    test_gpu_train.test_gat_gradients_match_reference_autodiff(10, 12, 20, 4, True, False, 0.0)
-    test_gpu_train.test_gat_gradients_match_reference_autodiff(10, 12, 6, 3, False, True, 0.0)
-    test_gpu_train.test_gat_gradients_match_reference_autodiff(10, 12, 6, 3, False, False, 0.3)
+    # the fake kernels bypass the C ABI, so there are no call counts to say which backward ran (path=None)
+    test_gpu_train.test_gat_gradients_match_reference_autodiff(24, 64, 128, 8, True, True, 0.4, False, None)
+    test_gpu_train.test_gat_gradients_match_reference_autodiff(10, 12, 20, 4, True, False, 0.0, False, None)
+    test_gpu_train.test_gat_gradients_match_reference_autodiff(10, 12, 6, 3, False, True, 0.0, False, None)
+    test_gpu_train.test_gat_gradients_match_reference_autodiff(10, 12, 6, 3, False, False, 0.3, False, None)
+    test_gpu_train.test_gat_gradients_match_reference_autodiff(16, 32, 32, 4, True, True, 0.0, True, None)
     test_gpu_train.test_gcn_edge_dropout_forward_and_gradients()
     test_gpu_train.test_appnp_training_gradients_and_dense_dropout()
     test_gpu_train.test_drop_edge_matches_oracle(False)

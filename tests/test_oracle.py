@@ -197,6 +197,42 @@ def test_c_gat_core_matches_numpy_gat():
         np.testing.assert_allclose(att_c, att, rtol=1e-5, atol=1e-8)
 
 
+def test_gat_attention_reference_matches_c_oracle_and_port():
+    """port.gat_attention, the float64 reference of tests/test_gpu_gat_backward.py: its forward is the C oracle's attention
+    core and the core of port.gat_forward, it takes destination rows without edges and fewer destinations than sources
+    (the set2set layout), and its autograd gradients agree with finite differences."""
+    import torch
+    from oracle import torch_cpu_port as port
+    rs = np.random.RandomState(11)
+    n, f = 90, 10
+    full, _ = o.add_self_loop_edge(random_graph(n, 700, seed=12, isolated=3), n)
+    row, col = torch.from_numpy(full[0].astype(np.int64)), torch.from_numpy(full[1].astype(np.int64))
+    t = lambda a: torch.from_numpy(np.asarray(a, np.float64))       # noqa: E731
+    for heads, a, u in ((8, 32, 32), (4, 16, 24), (1, 8, 8)):
+        x = rs.randn(n, f).astype(np.float32)
+        wq, wk, wv = glorot(rs, f, a), glorot(rs, f, a), glorot(rs, f, u)
+        bq, bk, bias = (rs.randn(k).astype(np.float32) * .1 for k in (a, a, u))
+        q = o.relu((x @ wq + bq).astype(np.float32))
+        k = o.relu((x @ wk + bk).astype(np.float32))
+        v = (x @ wv).astype(np.float32)
+        got = port.gat_attention(t(q), t(k), t(v), row, col, n, heads).numpy()
+        assert_close(got, c_oracle.gat_core(full[0], full[1], q, k, v, heads), rtol=1e-5, atol_scale=1e-6,
+                     what="gat_attention vs C gat core")
+        x64 = t(x)
+        want = port.gat_forward(x64, row, col, t(wq), t(bq), t(wk), t(bk), t(wv), t(bias), heads, relu=True)
+        got = port.gat_attention(torch.relu(x64 @ t(wq) + t(bq)), torch.relu(x64 @ t(wk) + t(bk)), x64 @ t(wv), row, col, n,
+                                 heads, bias=t(bias), relu=True)
+        np.testing.assert_allclose(got.numpy(), want.numpy(), rtol=1e-12, atol=1e-12)
+
+    # 4 destinations over 7 sources, destination 2 without edges, source 6 never gathered; H = 2, dqk = 2, dv = 3
+    row = torch.tensor([0, 0, 1, 1, 1, 3, 3, 3, 0])
+    col = torch.tensor([0, 3, 1, 2, 5, 4, 0, 3, 3])
+    args = tuple(torch.tensor(rs.randn(*s), requires_grad=True) for s in ((4, 4), (7, 4), (7, 6), (6,)))
+    out = port.gat_attention(*args[:3], row, col, 4, 2, bias=args[3]).detach().numpy()
+    np.testing.assert_allclose(out[2], args[3].detach().numpy(), rtol=0, atol=0)
+    torch.autograd.gradcheck(lambda Q, K, V, b: port.gat_attention(Q, K, V, row, col, 4, 2, scale=0.7, bias=b), args)
+
+
 def test_graph_sage_quirks():
     rs = np.random.RandomState(1)
     n, f, u = 20, 6, 4

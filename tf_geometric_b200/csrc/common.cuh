@@ -78,6 +78,16 @@ inline int sm_count() {
 
 inline bool aligned16(const void *p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
 
+inline bool is_pow2(int x) { return x > 0 && (x & (x - 1)) == 0; }
+
+// (H, dqk) of the GAT training path without the [E, H] coefficient table.  The forward that keeps (max, denominator)
+// per (row, head) (tfgk_gat_fused_stats_f32) exists only to feed the backward that recomputes the coefficients
+// (tfgk_gat_bwd_*_f32), so both take exactly these shapes: dqk / 4 lanes per head, A = H * dqk <= 128 (one float4 per
+// lane), H <= 8 (the backward packs [m | den | delta] per row in 8-float slots).  Any other shape keeps the table.
+inline bool gat_recompute_shape(int H, int dqk) {
+    return is_pow2(H) && H <= 8 && dqk % 4 == 0 && is_pow2(dqk / 4) && H * dqk <= 128;
+}
+
 // activation applied in every fused epilogue
 __device__ __forceinline__ float apply_act(float v, int act) {
     return act == TFGK_ACT_RELU ? fmaxf(v, 0.0f) : v;

@@ -841,8 +841,6 @@ __global__ void __launch_bounds__(kGatThreads) segment_softmax_kernel(const int6
     }
 }
 
-static inline bool is_pow2(int x) { return x > 0 && (x & (x - 1)) == 0; }
-
 template <int NC>
 static int launch_gat_online(const GatParams &p, cudaStream_t st) {
     constexpr int U = NC == 1 ? 4 : 2;
@@ -894,6 +892,8 @@ static int gat_fused_impl(const int64_t *rowptr, const int32_t *col,
     TFGK_CHECK_ARG(N >= 0 && H >= 1 && dqk >= 1 && dv >= 1, "gat: bad size (N=%d H=%d dqk=%d dv=%d)", N, H, dqk, dv);
     TFGK_CHECK_ARG(act == TFGK_ACT_NONE || act == TFGK_ACT_RELU, "gat: unknown activation %d", act);
     TFGK_CHECK_ARG(scale > 0.0f, "gat: scale must be positive");
+    // a forward that keeps (max, denominator) is only useful with a backward that reads them
+    if (stats != nullptr && !gat_recompute_shape(H, dqk)) return TFGK_ERR_UNSUPPORTED;
     if (N == 0) return TFGK_OK;
     TFGK_CHECK_ARG(rowptr && col && Q && K && V && out, "gat: null pointer");
     TFGK_CHECK_ARG(att != nullptr || (!write_att), "gat: write_att needs an attention buffer");

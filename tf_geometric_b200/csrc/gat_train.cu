@@ -17,7 +17,7 @@
 // [G (A floats) | m (8) | den (8) | delta (8) | pad (8)] per row so that pass 2 fetches everything it needs about a
 // destination with one 640-byte gather.  Both passes reuse the edge-streaming cp.async ring of the forward kernels.
 // Limits of this path (the caller falls back to the coefficient-table path otherwise): heads concatenated, dqk == dv,
-// A = H * dqk <= 128, H <= 8, no hub-row plan.
+// A = H * dqk <= 128, H <= 8 (gat_recompute_shape in common.cuh, which the stats forward checks too), no hub-row plan.
 #include "common.cuh"
 
 namespace tfgk {
@@ -64,7 +64,9 @@ __global__ void __launch_bounds__(256) gat_bwd_prepare_kernel(const float *__res
             g.x = y.x > 0.0f ? g.x : 0.0f; g.y = y.y > 0.0f ? g.y : 0.0f;
             g.z = y.z > 0.0f ? g.z : 0.0f; g.w = y.w > 0.0f ? g.w : 0.0f;
         }
-        // aggregate before bias: out = y - b wherever the gradient survives (relu passes y = out + b > 0 through unchanged)
+        // aggregate before bias: out = y - b wherever the gradient survives (relu passes y = out + b > 0 through unchanged).
+        // y - b is exact, but y = fl(out + b) kept out only to 2^-24 |y|: about 24 - log2(|b| / |out|) bits of out survive
+        // (17 at |b| = 100 |out|, checked in tests/test_gpu_gat_backward.py)
         d = g.x * (y.x - b.x) + g.y * (y.y - b.y) + g.z * (y.z - b.z) + g.w * (y.w - b.w);
         *reinterpret_cast<float4 *>(GS + r * ldgs + ccol) = g;
     }
@@ -250,11 +252,9 @@ static int launch_gat_bwd(const GatBwdParams &p, cudaStream_t st) {
     return TFGK_OK;
 }
 
-static inline bool pow2(int x) { return x > 0 && (x & (x - 1)) == 0; }
-
 static int check_bwd_shape(int32_t N, int32_t H, int32_t dqk) {
     if (N < 0 || H < 1 || dqk < 1) return set_error(TFGK_ERR_INVALID_ARGUMENT, "gat_bwd: bad size (N=%d H=%d dqk=%d)", N, H, dqk);
-    if (H > 8 || !pow2(H) || dqk % 4 != 0 || !pow2(dqk / 4) || H * dqk > 128) return TFGK_ERR_UNSUPPORTED;
+    if (!gat_recompute_shape(H, dqk)) return TFGK_ERR_UNSUPPORTED;
     return TFGK_OK;
 }
 
