@@ -26,7 +26,7 @@
 extern "C" {
 #endif
 
-#define TFGK_ABI_VERSION 5
+#define TFGK_ABI_VERSION 6
 
 enum tfgk_status {
     TFGK_OK = 0,
@@ -327,6 +327,41 @@ int tfgk_neighbor_sample_count(const int64_t *rowptr, int32_t n_rows, int32_t k,
 int tfgk_neighbor_sample_fill(const int64_t *rowptr, int32_t n_rows, int32_t k, double ratio, int padding,
                               uint64_t seed, uint32_t rng_stream, const int64_t *out_rowptr,
                               int32_t *out_row, int32_t *out_pos, void *stream);
+
+/* ---- link prediction (SURVEY.md 8(f)5, demo/demo_gae.py) -------------------------------------------------------- */
+
+/* K6, predict_edge of demo/demo_gae.py:53-60: out[e] = sum_d h[row_e, d] * h[col_e, d] in fp32, COO order.
+ * h is [N, D] with leading dimension ldh.  An edge's result depends only on that edge and h (same bits whatever E,
+ * the launch or the edge's position); an id outside [0, N) gives NaN and is never read.  Asynchronous.
+ * Algorithmic bytes: E * (8 D + 12). */
+int tfgk_edge_dot_f32(const float *h, int64_t ldh, int32_t N, const int32_t *row, const int32_t *col, int64_t E, int32_t D,
+                      float *out, void *stream);
+
+/* Exact negative sampling over an implicit candidate list (utils/graph_utils.py:369-452).  The caller passes a CSR
+ * (rowptr int64 [N+1], col int32) whose row i holds X_i, the sorted DISTINCT columns row i must not pair with:
+ *   TFGK_NEG_UPPER  X_i = upper neighbours j > i of the undirected edge set; row i's candidates are the j in (i, N) not
+ *                   in X_i, and the rows concatenated are np.nonzero(np.triu(adj, 1)) of the reference (row-major);
+ *   TFGK_NEG_START  X_a = out-neighbours of a together with a itself; a's candidates are [0, N) minus X_a.
+ * _offsets: offsets[i] = candidates before row i (int64 prefix sum), *total_host = C (synchronises `stream`).
+ * _draw: k[s] = random_below64(seed, rng_stream, round << 32 | s, C) for s = index[t] (index NULL: s = t < n).
+ * _dup_flags: flag[order[p]] = 1 when k[order[p]] == k[order[p-1]] (order = a stable argsort of k: later duplicates).
+ * _decode: candidate k[s] -> (out_row[s], out_col[s]) by two binary searches; k outside [0, C) gives (-1, -1).
+ * _sample_start: out_col[s] = candidate random_below64(seed, rng_stream, s, count) of row start[s] (TFGK_NEG_START
+ *                structure); -1 for a start id outside [0, N) or a row without candidates. */
+enum tfgk_neg_mode { TFGK_NEG_UPPER = 0, TFGK_NEG_START = 1 };
+int tfgk_neg_offsets_workspace_bytes(int32_t N, size_t *out_bytes);
+int tfgk_neg_offsets(const int64_t *rowptr, int32_t N, int mode, int64_t *offsets, int64_t *total_host, void *workspace,
+                     size_t workspace_bytes, void *stream);
+int tfgk_neg_draw(int64_t C, const int32_t *index, int64_t n, uint64_t seed, uint32_t rng_stream, int32_t round, int64_t *k,
+                  void *stream);
+int tfgk_neg_dup_flags(const int64_t *k, const int32_t *order, int64_t S, int32_t *flag, void *stream);
+int tfgk_neg_decode(const int64_t *rowptr, const int32_t *col, const int64_t *offsets, int32_t N, int mode, const int64_t *k,
+                    int64_t S, int32_t *out_row, int32_t *out_col, void *stream);
+int tfgk_neg_sample_start(const int64_t *rowptr, const int32_t *col, int32_t N, const int32_t *start, int64_t S,
+                          uint64_t seed, uint32_t rng_stream, int32_t *out_col, void *stream);
+/* np.random.randint(0, N, [2, S]) with the counter-based generator: out[0, s] = random_below(seed, rng_stream, 2 s, N),
+ * out[1, s] = random_below(seed, rng_stream, 2 s + 1, N)  (negative_sampling without edge_index, graph_utils.py:384-386). */
+int tfgk_random_pairs_i32(int32_t N, int64_t S, uint64_t seed, uint32_t rng_stream, int32_t *out, void *stream);
 
 #ifdef __cplusplus
 }

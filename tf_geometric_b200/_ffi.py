@@ -12,7 +12,7 @@ _LIB_PATH = os.path.join(os.path.dirname(os.path.abspath(__file__)), "lib", "lib
 _lock = threading.Lock()
 _lib = None
 
-ABI_VERSION = 5
+ABI_VERSION = 6
 
 OK = 0
 ERR_INVALID_ARGUMENT, ERR_CUDA, ERR_WORKSPACE, ERR_UNSUPPORTED, ERR_INDEX_OUT_OF_RANGE = 1, 2, 3, 4, 5
@@ -23,6 +23,7 @@ HEADS_SPLIT, HEADS_BROADCAST, HEADS_REDUCE = 0, 1, 2
 FLAG_ALL, FLAG_UPPER, FLAG_MAPPED = 0, 1, 2
 BERNOULLI_NONE, BERNOULLI_DROPOUT, BERNOULLI_KEEP = 0, 1, 2
 SAMPLE_NO_PADDING, SAMPLE_PADDING, SAMPLE_HEAD = 0, 1, 2
+NEG_UPPER, NEG_START = 0, 1
 
 _i32, _i64, _f32, _int = ctypes.c_int32, ctypes.c_int64, ctypes.c_float, ctypes.c_int
 _ptr, _size = ctypes.c_void_p, ctypes.c_size_t
@@ -90,6 +91,14 @@ SIGNATURES = {
     "tfgk_neighbor_sample_workspace_bytes": [_i32, ctypes.POINTER(_size)],
     "tfgk_neighbor_sample_count": [_ptr, _i32, _i32, _f64, _int, _ptr, ctypes.POINTER(_i64), _ptr, _size, _ptr],
     "tfgk_neighbor_sample_fill": [_ptr, _i32, _i32, _f64, _int, _u64, _u32, _ptr, _ptr, _ptr, _ptr],
+    "tfgk_edge_dot_f32": [_ptr, _i64, _i32, _ptr, _ptr, _i64, _i32, _ptr, _ptr],
+    "tfgk_neg_offsets_workspace_bytes": [_i32, ctypes.POINTER(_size)],
+    "tfgk_neg_offsets": [_ptr, _i32, _int, _ptr, ctypes.POINTER(_i64), _ptr, _size, _ptr],
+    "tfgk_neg_draw": [_i64, _ptr, _i64, _u64, _u32, _i32, _ptr, _ptr],
+    "tfgk_neg_dup_flags": [_ptr, _ptr, _i64, _ptr, _ptr],
+    "tfgk_neg_decode": [_ptr, _ptr, _ptr, _i32, _int, _ptr, _i64, _ptr, _ptr, _ptr],
+    "tfgk_neg_sample_start": [_ptr, _ptr, _i32, _ptr, _i64, _u64, _u32, _ptr, _ptr],
+    "tfgk_random_pairs_i32": [_i32, _i64, _u64, _u32, _ptr, _ptr],
 }
 
 

@@ -356,5 +356,39 @@ class SagePair(torch.autograd.Function):
         return grad_x, grad_ws, grad_wn, grad_b, None, None, None, None, None
 
 
+def _half_edge_csr(edge_index, num_nodes):
+    """CSR of the 2E half-edges of a query edge list: keys [row || col], partners [col || row].  Memoised on the edge
+    tensor."""
+    tag = ("half_edges", int(num_nodes))
+    hit = _structure._lookup(edge_index, tag)
+    if hit is None:
+        row, col = edge_index[0].contiguous(), edge_index[1].contiguous()
+        hit = _structure._store(edge_index, tag, ops.csr_build(torch.cat([row, col]), torch.cat([col, row]), num_nodes,
+                                                               num_nodes))
+    return hit
+
+
+class EdgeDot(torch.autograd.Function):
+    """logits[e] = <h[row_e], h[col_e]> (predict_edge of demo/demo_gae.py:53-60) through K6, differentiable w.r.t. h.
+    Backward: dh[u] = sum_{e: row_e = u} g_e h[col_e] + sum_{e: col_e = u} g_e h[row_e], ONE tfgk_spmm_f32 over the CSR
+    of the 2E half-edges with g permuted into its order: no atomics, run-to-run identical, hub rows through the work
+    plan, and a self-loop query counted twice (as autodiff does)."""
+
+    @staticmethod
+    def forward(ctx, h, edge_index):
+        hd = h.detach()
+        ctx.save_for_backward(hd)
+        ctx.edge_index = edge_index
+        return ops.edge_dot(hd, edge_index[0].contiguous(), edge_index[1].contiguous())
+
+    @staticmethod
+    def backward(ctx, grad_logits):
+        (h,) = ctx.saved_tensors
+        csr = _half_edge_csr(ctx.edge_index, h.shape[0])
+        g = grad_logits.to(torch.float32).reshape(-1)
+        w = ops.permute(torch.cat([g, g]).contiguous(), csr.perm)
+        return ops.spmm(csr, w, h, reduce="sum"), None
+
+
 def needs_grad(*tensors):
     return torch.is_grad_enabled() and any(torch.is_tensor(t) and t.requires_grad for t in tensors)

@@ -52,4 +52,18 @@ __host__ __device__ __forceinline__ uint32_t random_below(uint64_t seed, uint32_
     return (uint32_t)(((uint64_t)random_u32(seed, stream, idx) * (uint64_t)n) >> 32);
 }
 
+// 64-bit integer in [0, n): u = random_u32(2 idx) | random_u32(2 idx + 1) << 32 (two lanes of one Philox block),
+// k = high 64 bits of u * n
+__host__ __device__ __forceinline__ uint64_t random_below64(uint64_t seed, uint32_t stream, uint64_t idx, uint64_t n) {
+    const uint64_t blk = idx >> 1;
+    const Philox4 r = philox4x32_10((uint32_t)blk, (uint32_t)(blk >> 32), stream, 0u, (uint32_t)seed, (uint32_t)(seed >> 32));
+    const int l = (int)(idx & 1) * 2;
+    const uint64_t u = (uint64_t)r.v[l] | ((uint64_t)r.v[l + 1] << 32);
+#ifdef __CUDA_ARCH__
+    return __umul64hi(u, n);
+#else
+    return (uint64_t)(((unsigned __int128)u * n) >> 64);
+#endif
+}
+
 }  // namespace tfgk

@@ -1,7 +1,7 @@
 # coding=utf-8
 """Functional API: the names a tf_geometric user finds under `tfg.nn`, resolved from this package's own modules
 (message-passing hot path and the rows of SURVEY.md section 8f)."""
-from . import conv, kernel, pool, sampling
+from . import conv, kernel, link, pool, sampling
 from ..ops import relu
 
 _EXPORTS = {
@@ -18,6 +18,7 @@ _EXPORTS = {
     pool.topk_pool: ("topk_pool",),
     pool.score_pool: ("sag_pool", "sort_pool"),
     sampling.drop_edge: ("drop_edge",),
+    link.predict_edge: ("predict_edge",),
 }
 for _module, _names in _EXPORTS.items():
     for _name in _names:

@@ -12,7 +12,8 @@ import torch
 from . import _ffi
 from ._ffi import (REDUCE_SUM, REDUCE_MEAN, REDUCE_MAX, ACT_NONE, ACT_RELU, POW_INV_SQRT, POW_INV,  # noqa: F401
                    HEADS_SPLIT, HEADS_BROADCAST, HEADS_REDUCE, FLAG_ALL, FLAG_UPPER, FLAG_MAPPED,
-                   BERNOULLI_NONE, BERNOULLI_DROPOUT, BERNOULLI_KEEP, SAMPLE_NO_PADDING, SAMPLE_PADDING, SAMPLE_HEAD)
+                   BERNOULLI_NONE, BERNOULLI_DROPOUT, BERNOULLI_KEEP, SAMPLE_NO_PADDING, SAMPLE_PADDING, SAMPLE_HEAD,
+                   NEG_UPPER, NEG_START)
 
 _REDUCE_CODES = {"sum": REDUCE_SUM, "mean": REDUCE_MEAN, "max": REDUCE_MAX}
 
@@ -402,7 +403,8 @@ def gat_backward_recompute(csr, csr_t, Q, K, V, G, Y, bias, act, stats, num_head
 
 # ---- training-mode extras: dropout, per-head aggregation, GAT softmax backward -----------------------------------
 
-RNG_STREAM_DROPOUT, RNG_STREAM_SAMPLER = 0, 1      # rng_stream ids: independent draws for the same (seed, element)
+# rng_stream ids: independent draws for the same (seed, element); LINK = negative sampling and the edge split
+RNG_STREAM_DROPOUT, RNG_STREAM_SAMPLER, RNG_STREAM_LINK = 0, 1, 2
 
 
 def dropout(x, rate, seed, rng_stream=RNG_STREAM_DROPOUT, out=None):
@@ -535,6 +537,83 @@ def neighbor_sample(csr, k=None, ratio=None, padding=False, seed=0, rng_stream=R
         _ffi.call("tfgk_neighbor_sample_fill", _p(csr.rowptr), csr.n_rows, kk, rr, padding, int(seed),
                   int(rng_stream), _p(out_rowptr), _p(out_row), _p(out_pos), _stream(out_rowptr))
     return out_row, out_pos, out_rowptr
+
+
+# ---- link prediction: K6 edge scoring, negative sampling ----------------------------------------------------------
+
+def edge_dot(h, row, col, out=None):
+    """out[e] = <h[row_e], h[col_e]> in fp32 (K6, tfgk_edge_dot_f32); an id outside [0, N) gives NaN."""
+    if not (h.is_cuda and h.dtype == torch.float32 and h.dim() == 2):
+        raise TypeError("h must be a 2-D float32 CUDA tensor")
+    _check(row, torch.int32, "row")
+    _check(col, torch.int32, "col")
+    E = row.numel()
+    if col.numel() != E:
+        raise ValueError("edge_dot: row and col differ in length")
+    if out is None:
+        out = torch.empty((E,), dtype=torch.float32, device=h.device)
+    _ffi.call("tfgk_edge_dot_f32", _p(h), _row_major_2d(h, "h"), h.shape[0], _p(row), _p(col), E, h.shape[1], _p(out),
+              _stream(h))
+    return out
+
+
+def neg_offsets(csr, mode):
+    """(offsets int64 [N+1], C): candidates before each row of the implicit negative list (tfgk_neg_offsets)."""
+    dev = csr.rowptr.device
+    need = ctypes.c_size_t()
+    _ffi.call("tfgk_neg_offsets_workspace_bytes", csr.n_rows, ctypes.byref(need))
+    ws = torch.empty((max(need.value, 1),), dtype=torch.uint8, device=dev)
+    offsets = torch.empty((csr.n_rows + 1,), dtype=torch.int64, device=dev)
+    total = ctypes.c_int64()
+    _ffi.call("tfgk_neg_offsets", _p(csr.rowptr), csr.n_rows, int(mode), _p(offsets), ctypes.byref(total), _p(ws),
+              need.value, _stream(offsets))
+    return offsets, total.value
+
+
+def neg_draw(C, n, seed, round=0, index=None, out=None, device=None, rng_stream=RNG_STREAM_LINK):
+    """k[s] = random_below64(seed, rng_stream, round << 32 | s, C) for s < n, or only for s in `index` (into `out`)."""
+    if index is not None:
+        _check(index, torch.int32, "index")
+    k = out if out is not None else torch.empty((n,), dtype=torch.int64, device=device)
+    count = n if index is None else index.numel()
+    if count:
+        _ffi.call("tfgk_neg_draw", int(C), _p(index), count, int(seed), int(rng_stream), int(round), _p(k), _stream(k))
+    return k
+
+
+def neg_dup_flags(k, order):
+    """int32 flags of the later duplicates of k, given a stable argsort `order` of k."""
+    _check(k, torch.int64, "k")
+    _check(order, torch.int32, "order")
+    flag = torch.empty((k.numel(),), dtype=torch.int32, device=k.device)
+    _ffi.call("tfgk_neg_dup_flags", _p(k), _p(order), k.numel(), _p(flag), _stream(k))
+    return flag
+
+
+def neg_decode(csr, offsets, mode, k):
+    """Candidate indices k (int64) -> int32 [2, S] node pairs of the implicit negative list (tfgk_neg_decode)."""
+    _check(k, torch.int64, "k")
+    S = k.numel()
+    out = torch.empty((2, S), dtype=torch.int32, device=k.device)
+    _ffi.call("tfgk_neg_decode", _p(csr.rowptr), _p(csr.col), _p(offsets), csr.n_rows, int(mode), _p(k), S, _p(out[0]),
+              _p(out[1]), _stream(k))
+    return out
+
+
+def neg_sample_start(csr, start, seed, rng_stream=RNG_STREAM_LINK):
+    """One uniform candidate per start node over a TFGK_NEG_START structure (tfgk_neg_sample_start); -1 where none."""
+    _check(start, torch.int32, "start")
+    out = torch.empty((start.numel(),), dtype=torch.int32, device=start.device)
+    _ffi.call("tfgk_neg_sample_start", _p(csr.rowptr), _p(csr.col), csr.n_rows, _p(start), start.numel(), int(seed),
+              int(rng_stream), _p(out), _stream(start))
+    return out
+
+
+def random_pairs(num_nodes, num_samples, seed, device, rng_stream=RNG_STREAM_LINK):
+    """int32 [2, S] uniform node ids (np.random.randint(0, N, [2, S]) with the counter-based generator)."""
+    out = torch.empty((2, num_samples), dtype=torch.int32, device=device)
+    _ffi.call("tfgk_random_pairs_i32", int(num_nodes), int(num_samples), int(seed), int(rng_stream), _p(out), _stream(out))
+    return out
 
 
 # ---- K4 ----------------------------------------------------------------------------------------------------------

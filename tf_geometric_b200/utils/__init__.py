@@ -2,5 +2,6 @@
 from . import graph_utils
 from .graph_utils import (add_self_loop_edge, remove_self_loop_edge, convert_edge_to_directed, merge_duplicated_edge,
                           convert_edge_to_upper, convert_edge_index_to_edge_hash, convert_edge_hash_to_edge_index,
-                          adj_norm_edge, compute_num_or_size_splits)
+                          adj_norm_edge, compute_num_or_size_splits, negative_sampling,
+                          negative_sampling_with_start_node, edge_train_test_split)
 from .sampling import RandomNeighborSampler, UniformNeighborSampler

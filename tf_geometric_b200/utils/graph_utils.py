@@ -6,10 +6,13 @@ Device inputs (torch CUDA tensors) run on the GPU kernels - including the hash/u
 with tf.unique's first-occurrence order) - and return device tensors.  numpy / list inputs are processed with numpy and
 return numpy, exactly like the reference does for non-tensor inputs (its eager host path).
 """
+import math
+import warnings
+
 import numpy as np
 import torch
 
-from .. import ops
+from .. import ops, _rng, _structure
 
 
 def _is_device(x):
@@ -240,6 +243,202 @@ def compute_num_or_size_splits(num_h_features, num_splits):
         raise Exception("cannot split H of shape [None, {}] into {} matrices, please provide a valid num_splits"
                         .format(num_h_features, num_splits))
     return sizes
+
+
+# ---- link prediction: negative sampling and the edge split (reference :369-452, :488-535) ---------------------------
+# One implementation for every container: numpy inputs are copied to the device and the results back (the draws come
+# from the counter-based generator of csrc/rng.cuh, so they cannot follow numpy's global generator anyway).
+
+_MASK64 = (1 << 64) - 1
+
+
+def _batch_seed(seed, b):
+    """Key of draw b of a batch: independent Philox keys for the same base seed."""
+    return (seed + b * 0x9E3779B97F4A7C15) & _MASK64
+
+
+def _check_ids(ids, num_nodes, what):
+    if ids.numel():
+        lo, hi = torch.aminmax(ids)
+        if int(lo) < 0 or int(hi) >= num_nodes:
+            raise ValueError("{} holds node ids outside [0, {})".format(what, num_nodes))
+
+
+def _excluded_structure(edge_index, num_nodes, mode):
+    """(csr, offsets, C): row i of csr holds the sorted distinct columns row i may not pair with (tfgk.h tfgk_neg_*):
+    NEG_UPPER - the upper neighbours j > i of the undirected edge set (self loops are never candidates anyway);
+    NEG_START - the out-neighbours of i and i itself.  Memoised on the edge tensor."""
+    tag = ("neg", int(num_nodes), int(mode))
+    hit = _structure._lookup(edge_index, tag)
+    if hit is not None:
+        return hit
+    row, col = edge_index[0].contiguous(), edge_index[1].contiguous()
+    if mode == ops.NEG_UPPER:
+        lo, hi = torch.minimum(row, col).contiguous(), torch.maximum(row, col).contiguous()
+        keep = ops.select_flagged(ops.edge_flags(lo, hi, lo.numel(), mode=ops.FLAG_UPPER))
+        lo, hi = ops.gather_i32(lo, keep), ops.gather_i32(hi, keep)
+    else:
+        loops = torch.arange(num_nodes, dtype=torch.int32, device=row.device)
+        lo, hi = torch.cat([row, loops]), torch.cat([col, loops])
+    if lo.numel():
+        uniq, _ = ops.edge_unique(lo, hi, num_nodes)
+        lo, hi = uniq[0].contiguous(), uniq[1].contiguous()
+        by_col = ops.stable_argsort(hi, key_bits=max(1, (num_nodes - 1).bit_length()))
+        lo, hi = ops.gather_i32(lo, by_col), ops.gather_i32(hi, by_col)
+    csr = ops.csr_build(lo, hi, num_nodes, num_nodes)           # stable by row: columns stay ascending within a row
+    offsets, C = ops.neg_offsets(csr, mode)
+    return _structure._store(edge_index, tag, (csr, offsets, C))
+
+
+def _words(k):
+    """(low, high) 32-bit halves of an int64 vector, as int32 vectors."""
+    halves = k.view(torch.int32).view(-1, 2)
+    return halves[:, 0].contiguous(), halves[:, 1].contiguous()
+
+
+def _random_keys(n, seed, device):
+    """n independent 32-bit keys (the high word of a 64-bit draw below 2^32 is zero)."""
+    return _words(ops.neg_draw(1 << 32, n, seed, device=device))[0]
+
+
+def _argsort_i64(k, C):
+    """Stable argsort of int64 values in [0, C): LSD passes over the low, then the high 32-bit word."""
+    bits = max(1, (C - 1).bit_length())
+    lo, hi = _words(k)
+    order = ops.stable_argsort(lo, key_bits=min(bits, 32))
+    if bits > 32:
+        order = ops.gather_i32(order, ops.stable_argsort(ops.gather_i32(hi, order), key_bits=bits - 32))
+    return order
+
+
+def _draw_candidates(C, S, replace, seed, device):
+    """S candidate indices in [0, C) as int64: independent draws, or S distinct ones."""
+    if replace:
+        return ops.neg_draw(C, S, seed, device=device)
+    if 2 * S > C:               # dense: shuffle the whole range and take a prefix (work O(C) <= O(2 S))
+        perm = ops.stable_argsort(_random_keys(C, seed, device))
+        return perm[:S].to(torch.int64)
+    k = ops.neg_draw(C, S, seed, device=device)
+    rnd = 0
+    while True:                 # redraw the later duplicates; draw s of round r has the counter (s, r)
+        dup = ops.select_flagged(ops.neg_dup_flags(k, _argsort_i64(k, C)))
+        if dup.numel() == 0:
+            return k
+        rnd += 1
+        ops.neg_draw(C, S, seed, round=rnd, index=dup, out=k)
+
+
+def negative_sampling(num_samples, num_nodes, edge_index=None, replace=True, mode="undirected", batch_size=None,
+                      seed=None):
+    """Node pairs that are not edges (reference :369-412), drawn exactly from the implicit candidate list.
+
+    :param num_samples: pairs per draw
+    :param num_nodes: number of nodes
+    :param edge_index: optional positive edges.  Given: the candidates are the pairs i < j that are not in
+        convert_edge_to_upper(edge_index), in the reference's row-major order, and no dense N x N matrix is built.
+        None: both ends are uniform in [0, num_nodes) (self loops and positives included, like np.random.randint).
+    :param replace: with edge_index, whether the same pair may be drawn twice
+    :param mode: only "undirected" (the reference raises NotImplementedError otherwise)
+    :param batch_size: None -> one int32 [2, num_samples] edge index; else a list of batch_size independent draws
+    :param seed: optional 64-bit key pinning the draws
+    :return: device tensors for device (and for absent) edge_index, numpy arrays for numpy edge_index
+    """
+    seed = _rng.resolve(seed)
+    num_samples, num_nodes = int(num_samples), int(num_nodes)
+    n_batches = 1 if batch_size is None else int(batch_size)
+    if num_samples < 0 or num_nodes < 0:
+        raise ValueError("num_samples and num_nodes must be non-negative")
+    if edge_index is None:
+        if num_samples and num_nodes == 0:
+            raise ValueError("cannot sample node pairs from an empty graph")
+        dev = ops.default_device()
+        out = [ops.random_pairs(num_nodes, num_samples, _batch_seed(seed, b), dev) for b in range(n_batches)]
+        return out[0] if batch_size is None else out
+    if mode != "undirected":
+        raise NotImplementedError()
+    on_device = _is_device(edge_index)
+    ei = ops.as_device(edge_index, torch.int32)
+    _check_ids(ei, num_nodes, "edge_index")
+    csr, offsets, C = _excluded_structure(ei, num_nodes, ops.NEG_UPPER)
+    if num_samples and C == 0:
+        raise ValueError("no candidate pair: every pair i < j of the {} nodes is an edge".format(num_nodes))
+    if not replace and num_samples > C:
+        raise ValueError("cannot draw {} distinct pairs without replacement from {} candidates".format(num_samples, C))
+    out = []
+    for b in range(n_batches):
+        k = _draw_candidates(C, num_samples, replace, _batch_seed(seed, b), ei.device) if num_samples else \
+            torch.empty((0,), dtype=torch.int64, device=ei.device)
+        pairs = ops.neg_decode(csr, offsets, ops.NEG_UPPER, k)
+        out.append(pairs if on_device else pairs.cpu().numpy())
+    return out[0] if batch_size is None else out
+
+
+def negative_sampling_with_start_node(start_node_index, num_nodes, edge_index=None, seed=None):
+    """One negative partner per start node (reference :415-452): b != a with (a, b) not in edge_index (directed),
+    uniform over the candidates.  A start node adjacent to every other node raises ValueError (the reference loops
+    forever).  Without edge_index b is uniform in [0, num_nodes).  Returns int32 [2, S] in the container of
+    start_node_index."""
+    seed = _rng.resolve(seed)
+    num_nodes = int(num_nodes)
+    on_device = _is_device(start_node_index)
+    dev = edge_index.device if _is_device(edge_index) else None
+    start = ops.as_device(start_node_index, torch.int32, device=dev).reshape(-1).contiguous()
+    _check_ids(start, num_nodes, "start_node_index")
+    if edge_index is None:
+        end = ops.random_pairs(num_nodes, start.numel(), seed, start.device)[1]
+    else:
+        ei = ops.as_device(edge_index, torch.int32, device=start.device)
+        _check_ids(ei, num_nodes, "edge_index")
+        csr, offsets, _ = _excluded_structure(ei, num_nodes, ops.NEG_START)
+        if start.numel():
+            s = start.to(torch.int64)
+            if bool(((offsets[s + 1] - offsets[s]) == 0).any()):
+                raise ValueError("a start node is adjacent to every other node: it has no negative partner")
+        end = ops.neg_sample_start(csr, start, seed)
+    out = torch.stack([start, end])
+    return out if on_device else out.cpu().numpy()
+
+
+def edge_train_test_split(edge_index, test_size, edge_weight=None, mode="undirected", seed=None, **kwargs):
+    """Split the undirected edges into train and test sets (reference :488-535).
+
+    The edges are merged into convert_edge_to_upper(edge_index, [edge_weight], merge_modes=["max"]) and permuted by
+    random keys; with n merged edges, n_test = ceil(test_size * n) for a float test_size and test_size for an int
+    (sklearn's sizes), test = the first n_test of the permutation and train = the rest.  Weights follow their edges.
+    :return: (train_edge_index, test_edge_index, train_edge_weight, test_edge_weight), each in the container of its
+        input (weights None without edge_weight)
+    """
+    if "num_nodes" in kwargs:
+        warnings.warn("argument \"num_nodes\" is deprecated for the method \"edge_train_test_split\", you can remove it")
+    if mode != "undirected":
+        raise NotImplementedError()
+    seed = _rng.resolve(seed)
+    ei = ops.as_device(edge_index, torch.int32)
+    w = None if edge_weight is None else ops.as_device(edge_weight, torch.float32, device=ei.device).reshape(-1)
+    upper, props = convert_edge_to_upper(ei, None if w is None else [w], None if w is None else ["max"])
+    n = upper.shape[1]
+    if isinstance(test_size, (float, np.floating)):
+        if not 0.0 < test_size < 1.0:
+            raise ValueError("test_size={} should be in (0, 1) as a fraction".format(test_size))
+        n_test = int(math.ceil(test_size * n))
+    else:
+        n_test = int(test_size)
+    n_train = n - n_test
+    if n_test <= 0 or n_train <= 0:
+        raise ValueError("with n_samples={} and test_size={} the train or the test set would be empty".format(n, test_size))
+    perm = ops.stable_argsort(_random_keys(n, seed, ei.device))
+    row, col = upper[0].contiguous(), upper[1].contiguous()
+    parts = []
+    for idx in (perm[n_test:].contiguous(), perm[:n_test].contiguous()):
+        part = torch.stack([ops.gather_i32(row, idx), ops.gather_i32(col, idx)])
+        parts.append(part if _is_device(edge_index) else part.cpu().numpy())
+    weights = [None, None]
+    if w is not None:
+        upw = props[0].contiguous()
+        weights = [ops.permute(upw, idx) for idx in (perm[n_test:].contiguous(), perm[:n_test].contiguous())]
+        if not _is_device(edge_weight):
+            weights = [x.cpu().numpy() for x in weights]
+    return parts[0], parts[1], weights[0], weights[1]
 
 
 # samplers live in utils/sampling.py; re-exported here because the reference defines them in this module (:630-846)

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 # coding=utf-8
-"""Generate tests/golden/ref_exec_*.npz by EXECUTING the reference's own Python (a read-only checkout of
+"""Generate tests/golden/ref_exec_*.npz and link_exec.npz by EXECUTING the reference's own Python (a read-only checkout of
 CrawlScript/tf_geometric named by $TFG_REFERENCE) over the numpy shims in tools/ref_shim.  The tests never need the
 reference: the resulting small fixtures are committed.  Re-run:  TFG_REFERENCE=<checkout> python tools/gen_golden_from_reference.py
 """
@@ -325,6 +325,40 @@ def main():
     out.update(batch_x=bg.x, batch_ei=bg.edge_index, batch_w=bg.edge_weight, batch_y=bg.y, batch_gi=bg.node_graph_index,
                batch_egi=bg.edge_graph_index)
     save("graph", **out)
+
+    # ---- link prediction: negative_sampling, edge_train_test_split, negative_sampling_with_start_node ------------------
+    # tests/golden/link_exec.npz: the reference's full negative candidate list in its own order, the split sizes with the
+    # merged upper edges and their max weights, and start-node samples (whose draws only allow property checks).
+    # Own RandomState (and np.random seeds of its own), so adding this section leaves every fixture above unchanged.
+    lrs = np.random.RandomState(2024)
+    n = 30
+    ei = graph(n, 150, 61, True)
+    ei = np.concatenate([ei, np.array([[4, 9, 9], [4, 2, 2]], np.int32)], axis=1)     # a self loop and a duplicate
+    w = lrs.rand(ei.shape[1]).astype(np.float32)
+    up, _ = gu.convert_edge_to_upper(ei)
+    num_cand = n * (n - 1) // 2 - int(len(set(zip(up[0][up[0] < up[1]].tolist(), up[1][up[0] < up[1]].tolist()))))
+    # replace=False with num_samples = C draws a permutation of the candidate list with np.random.choice; replaying
+    # the seeded choice recovers the list in the reference's own (row-major np.nonzero) order
+    np.random.seed(11)
+    neg = gu.negative_sampling(num_cand, n, ei, replace=False)
+    np.random.seed(11)
+    p = np.random.choice(list(range(num_cand)), num_cand, replace=False)
+    cand = np.empty_like(neg)
+    cand[:, p] = neg
+    out = {"n": n, "ei": ei, "w": w, "candidates": cand}
+    np.random.seed(12)
+    tr_i, te_i, tr_w, te_w = gu.edge_train_test_split(ei, 0.2, edge_weight=w)
+    out.update(split_train_index=tr_i, split_test_index=te_i, split_train_w=tr_w, split_test_w=te_w)
+    np.random.seed(13)
+    tr_i, te_i, _, _ = gu.edge_train_test_split(ei, 7)
+    out.update(split7_train_index=tr_i, split7_test_index=te_i)
+    start = lrs.randint(0, n, 40).astype(np.int32)
+    np.random.seed(14)
+    out.update(start=start, start_sample=gu.negative_sampling_with_start_node(start, n, ei))
+    # named apart from ref_exec_*: those are replayed case by case through tests/golden_cases.py, while this one is read
+    # by tests/test_link_host.py and tests/test_gpu_link.py
+    np.savez_compressed(os.path.join(OUT, "link_exec.npz"), **{k: np.asarray(v) for k, v in out.items()})
+    print("wrote link_exec.npz: {}".format(", ".join(sorted(out))))
 
 
 if __name__ == "__main__":
