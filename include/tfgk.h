@@ -26,7 +26,7 @@
 extern "C" {
 #endif
 
-#define TFGK_ABI_VERSION 6
+#define TFGK_ABI_VERSION 7
 
 enum tfgk_status {
     TFGK_OK = 0,
@@ -362,6 +362,21 @@ int tfgk_neg_sample_start(const int64_t *rowptr, const int32_t *col, int32_t N, 
 /* np.random.randint(0, N, [2, S]) with the counter-based generator: out[0, s] = random_below(seed, rng_stream, 2 s, N),
  * out[1, s] = random_below(seed, rng_stream, 2 s + 1, N)  (negative_sampling without edge_index, graph_utils.py:384-386). */
 int tfgk_random_pairs_i32(int32_t N, int64_t S, uint64_t seed, uint32_t rng_stream, int32_t *out, void *stream);
+
+/* ---- edge-weight gradients ------------------------------------------------------------------------------------ */
+
+/* K7, sampled dense-dense product over a destination-sorted CSR: for every slot p of every row r,
+ *     out[perm ? perm[p] : p] = (alpha * row_scale[r]) * sum_d G[r, d] * X[col[p], d]
+ * (row_scale NULL: 1).  It is the gradient of K1's output with respect to its edge weights: G = d loss / d out, X the
+ * aggregated rows, row_scale = 1 / max(cnt, 1) for the mean reducer; with perm (the CSR's slot -> edge map) the result
+ * lands in the caller's edge order.  G is [N_rows, D] with leading dimension ldg, X [*, D] with ldx; column slices are
+ * fine.  The slots are cut into warp tasks of equal size (TFGK_SDDMM_TASK_EDGES, default 512), so a hub row is spread
+ * over several warps; each output is one edge, written once, without atomics.  An edge's bits depend only on G[r],
+ * X[col[p]], row_scale[r] and alpha (not on the task size, the grid or perm).  Asynchronous.
+ * Algorithmic bytes: E * (4 D + 12) + N_rows * (4 D + 8). */
+int tfgk_sddmm_csr_f32(const int64_t *rowptr, const int32_t *col, const int32_t *perm, int32_t N_rows,
+                       const float *G, int64_t ldg, const float *X, int64_t ldx, int32_t D,
+                       const float *row_scale, float alpha, float *out, void *stream);
 
 #ifdef __cplusplus
 }

@@ -12,7 +12,7 @@ _LIB_PATH = os.path.join(os.path.dirname(os.path.abspath(__file__)), "lib", "lib
 _lock = threading.Lock()
 _lib = None
 
-ABI_VERSION = 6
+ABI_VERSION = 7
 
 OK = 0
 ERR_INVALID_ARGUMENT, ERR_CUDA, ERR_WORKSPACE, ERR_UNSUPPORTED, ERR_INDEX_OUT_OF_RANGE = 1, 2, 3, 4, 5
@@ -99,6 +99,7 @@ SIGNATURES = {
     "tfgk_neg_decode": [_ptr, _ptr, _ptr, _i32, _int, _ptr, _i64, _ptr, _ptr, _ptr],
     "tfgk_neg_sample_start": [_ptr, _ptr, _i32, _ptr, _i64, _u64, _u32, _ptr, _ptr],
     "tfgk_random_pairs_i32": [_i32, _i64, _u64, _u32, _ptr, _ptr],
+    "tfgk_sddmm_csr_f32": [_ptr, _ptr, _ptr, _i32, _ptr, _i64, _ptr, _i64, _i32, _ptr, _f32, _ptr, _ptr],
 }
 
 

@@ -48,21 +48,32 @@ def _transposed_structure(edge_index, num_nodes, edge_weight, mean, csr):
 
 
 class NeighborAggregate(torch.autograd.Function):
-    """agg = REDUCE_{e: row_e = r} w_e x[col_e]  (sum | mean), differentiable w.r.t. x."""
+    """agg = REDUCE_{e: row_e = r} w_e x[col_e]  (sum | mean), differentiable w.r.t. x and the edge weights.
+    d w_e = <dagg[row_e], x[col_e]> (/ max(cnt[row_e], 1) for mean) is K7 over the forward CSR, written in edge order."""
 
     @staticmethod
     def forward(ctx, x, edge_index, edge_weight, reduce, num_nodes):
         csr, _ = _structure.csr_for_edge_index(edge_index, num_nodes)
         w_csr = None if edge_weight is None else _structure.weights_in_csr_order(edge_weight, csr)
         ctx.saved = (edge_index, edge_weight, reduce, num_nodes, csr)
+        ctx.save_for_backward(x.detach() if edge_weight is not None and edge_weight.requires_grad else None)
         return ops.spmm(csr, w_csr, x.detach(), reduce=reduce)
 
     @staticmethod
     def backward(ctx, grad_out):
         edge_index, edge_weight, reduce, num_nodes, csr = ctx.saved
-        csr_t, w_t = _transposed_structure(edge_index, num_nodes, edge_weight, reduce == "mean", csr)
-        grad_x = ops.spmm(csr_t, w_t, grad_out.contiguous(), reduce="sum")
-        return grad_x, None, None, None, None
+        (x,) = ctx.saved_tensors
+        g = grad_out.contiguous()
+        grad_x = grad_w = None
+        if ctx.needs_input_grad[0]:
+            csr_t, w_t = _transposed_structure(edge_index, num_nodes, edge_weight, reduce == "mean", csr)
+            grad_x = ops.spmm(csr_t, w_t, g, reduce="sum")
+        if ctx.needs_input_grad[2]:
+            scale = None
+            if reduce == "mean":
+                scale = torch.reciprocal((csr.rowptr[1:] - csr.rowptr[:-1]).clamp(min=1).to(torch.float32))
+            grad_w = ops.sddmm_csr(csr, g, x, row_scale=scale)
+        return grad_x, None, grad_w, None, None
 
 
 class Dense(torch.autograd.Function):
@@ -93,35 +104,100 @@ class Dense(torch.autograd.Function):
 
 
 class SparseMatmul(torch.autograd.Function):
-    """y = act(A @ h + b) for a cached SparseMatrix A (gcn.py:280-288), differentiable w.r.t. h and b.
-    dh = A^T dz runs the same kernel on the transposed structure of A (built once per matrix, values permuted into it);
-    dz = dy * (y > 0) for relu."""
+    """y = act(A @ h + b) for a cached SparseMatrix A (gcn.py:280-288), differentiable w.r.t. h, b and, when they are
+    passed as the trailing input, the values of A (COO order; tf_sparse products are differentiable in their values).
+    dz = dy * (y > 0) for relu; dh = A^T dz runs the same kernel on the transposed structure of A (built once per
+    matrix, values permuted into it); d value_e = <dz[row_e], h[col_e]> is K7 over A's CSR, written in COO order."""
 
     @staticmethod
-    def forward(ctx, h, bias, adj, act_code):
+    def forward(ctx, h, bias, adj, act_code, value=None):
         y = ops.spmm(adj.csr, adj.value_csr, h.detach(), reduce="sum", bias=None if bias is None else bias.detach(),
                      act=act_code)
         ctx.adj = adj
         ctx.act_code = act_code
         ctx.has_bias = bias is not None
-        ctx.save_for_backward(y if act_code == ops.ACT_RELU else None)
+        ctx.save_for_backward(y if act_code == ops.ACT_RELU else None,
+                              h.detach() if value is not None and value.requires_grad else None)
         return y
 
     @staticmethod
     def backward(ctx, grad_y):
-        (y,) = ctx.saved_tensors
+        y, h = ctx.saved_tensors
         g = grad_y.contiguous()
         if ctx.act_code == ops.ACT_RELU:
             g = _relu_grad(g, y)
         adj = ctx.adj
-        csr_t = adj._transposed_csr()
-        if getattr(adj, "_value_csc", None) is None:
-            adj._value_csc = ops.permute(adj.value, csr_t.perm)
-        grad_h = ops.spmm(csr_t, adj._value_csc, g, reduce="sum") if ctx.needs_input_grad[0] else None
-        grad_b = None
+        grad_h = grad_b = grad_value = None
+        if ctx.needs_input_grad[0]:
+            csr_t = adj._transposed_csr()
+            if getattr(adj, "_value_csc", None) is None:
+                adj._value_csc = ops.permute(adj.value.detach(), csr_t.perm)
+            grad_h = ops.spmm(csr_t, adj._value_csc, g, reduce="sum")
         if ctx.has_bias and ctx.needs_input_grad[1]:
             grad_b = ops.colsum(g)
-        return grad_h, grad_b, None, None
+        if len(ctx.needs_input_grad) > 4 and ctx.needs_input_grad[4]:        # four-argument calls pass no values
+            grad_value = ops.sddmm_csr(adj.csr, g, h)
+        return grad_h, grad_b, None, None, grad_value
+
+
+def _gather(values, index):
+    """values[index] for a float32 per-node vector and an int32 index vector (tfgk_permute_f32)."""
+    return ops.permute(values.contiguous(), index)
+
+
+def _segment_sums(csr, per_edge):
+    """Sum of a per-edge float32 vector (the order of the edge list `csr` was built from) over every CSR row:
+    tfgk_spmm_f32 with D = 1 gathering through csr.perm; deterministic."""
+    return ops.spmm(csr, None, per_edge.contiguous().unsqueeze(1), reduce="sum", col=csr.perm).squeeze(1)
+
+
+class GcnNormValues(torch.autograd.Function):
+    """The values of gcn_norm_adj(A) (nn/conv/gcn.py) as a function of A's values w, differentiable.
+
+    The forward receives the values the normalisation kernels already produced (the caller runs exactly the kernels of the
+    non-differentiable path, so requires_grad never changes a bit) and returns them.  `aux` holds what the backward needs:
+    the matrix A' whose row / column sums are the degrees (A, plus the self loops appended before normalising), its
+    normalised values v, and the degree factors.  With g = dL/dv and R_i = sum_{row_e = i} g_e v_e, C_j = sum_{col_e = j}
+    g_e v_e over the entries of A' (two deterministic D = 1 segment sums, over A's CSR and CSC):
+        both, sym   : v = a_r w a_c, a = deg^-1/2         dw = g a_r a_c - 1/2 a_r^2 (R_r + C_r)
+        both, !sym  : v = a_r w b_c, b = coldeg^-1/2      dw = g a_r b_c - 1/2 a_r^2 R_r - 1/2 b_c^2 C_c
+        left        : v = p_r w, p = 1/deg                dw = (g - R_r) p_r
+        right       : v = w q_c, q = 1/rowdeg             dw = g q_c - q_r C_r
+    A degree <= 0 has its factor forced to 0 (_remove_inf_and_nan), and so has its derivative.  Self loops (appended
+    before or after normalising) carry constant fill weights: they enter the degrees and get no gradient.  Entries past
+    A' (loops appended after normalising) are constants."""
+
+    @staticmethod
+    def forward(ctx, w, normed_value, aux):
+        ctx.aux = aux
+        ctx.n_w = w.shape[0]
+        return normed_value
+
+    @staticmethod
+    def backward(ctx, grad_value):
+        kind, adj, v, f_row, f_col = ctx.aux
+        n_prime = v.shape[0]
+        g = grad_value.contiguous()[:n_prime].contiguous()
+        row, col = adj.index[0].contiguous(), adj.index[1].contiguous()
+        gv = g * v
+        if kind == "left":
+            R = _segment_sums(adj.csr, gv)
+            dw = (g - _gather(R, row)) * _gather(f_row, row)
+        elif kind == "right":
+            C = _segment_sums(adj._transposed_csr(), gv)
+            if C.shape[0] < f_row.shape[0]:               # q is indexed by row ids, C by column ids
+                C = torch.cat([C, C.new_zeros(f_row.shape[0] - C.shape[0])])
+            dw = g * _gather(f_row, col) - _gather(f_row * C[:f_row.shape[0]], row)
+        else:
+            R = _segment_sums(adj.csr, gv)
+            C = _segment_sums(adj._transposed_csr(), gv)
+            a_r = _gather(f_row, row)
+            if kind == "both_sym":
+                dw = g * a_r * _gather(f_row, col) - _gather(0.5 * f_row * f_row * (R + C), row)
+            else:
+                dw = g * a_r * _gather(f_col, col) - _gather(0.5 * f_row * f_row * R, row) \
+                    - _gather(0.5 * f_col * f_col * C, col)
+        return dw[:ctx.n_w], None, None
 
 
 def _transposed_of_csr(csr, edge_index_used):
@@ -247,8 +323,8 @@ def dense(x, weight, bias=None, activation=None):
 
 
 def propagate(adj, h, bias=None, act_code=ops.ACT_NONE):
-    """Differentiable act(A @ h + b) for a SparseMatrix A (gradient w.r.t. h and b)."""
-    return SparseMatmul.apply(h, bias, adj, act_code)
+    """Differentiable act(A @ h + b) for a SparseMatrix A (gradient w.r.t. h, b and A's values)."""
+    return SparseMatmul.apply(h, bias, adj, act_code, adj.value)
 
 
 class SegmentReduce(torch.autograd.Function):

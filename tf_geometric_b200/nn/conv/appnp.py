@@ -25,7 +25,7 @@ def appnp(x, edge_index, edge_weight, kernels, biases,
     num_nodes = x.shape[0]
     normed = gcn_norm_adj(SparseMatrix(edge_index, edge_weight, [num_nodes, num_nodes]), cache=cache)
     normed = normed.dropout(edge_drop_rate, training=training)                          # appnp.py:54-55
-    with_grad = autograd.needs_grad(x, *[t for t in list(kernels) + list(biases) if t is not None])
+    with_grad = autograd.needs_grad(x, normed.value, *[t for t in list(kernels) + list(biases) if t is not None])
 
     h = x
     num_dense = len(kernels)
@@ -44,7 +44,7 @@ def appnp(x, edge_index, edge_weight, kernels, biases,
         # the teleport mix is elementwise
         out = h
         for _ in range(k):
-            out = autograd.SparseMatmul.apply(out, None, normed, ops.ACT_NONE) * (1.0 - alpha) + h * alpha
+            out = autograd.propagate(normed, out) * (1.0 - alpha) + h * alpha
         if act_code != ops.ACT_NONE:
             out = torch.relu(out)
         return leftover(out) if leftover is not None else out

@@ -40,6 +40,21 @@ def gcn_norm_adj(sparse_adj, norm="both", add_self_loop=True, sym=True, renorm=T
                 return cached
             return SparseMatrix(cached[0], cached[1], cached[2])      # a reference-style (index, value, shape) triple
 
+    w = sparse_adj.value
+    normed, aux = _normalize(sparse_adj, norm, add_self_loop, sym, renorm, improved)
+    if cache is not None:
+        normed.csr, normed.value_csr    # build the CSR now: cached objects are always warm
+        cache[cache_key] = normed       # the cached matrix carries no gradient: a warm call returns it as is
+    if autograd.needs_grad(w):
+        # differentiable in the edge weights (tf.GradientTape sees through the reference's normalisation): same values,
+        # same CSR, with a backward to w
+        normed = normed.with_value(autograd.GcnNormValues.apply(w, normed.value, aux))
+    return normed
+
+
+def _normalize(sparse_adj, norm, add_self_loop, sym, renorm, improved):
+    """(normed SparseMatrix, aux): the kernels of reference gcn.py:32-130, and what GcnNormValues' backward needs
+    (kind, A' = the matrix whose sums are the degrees, its normalised values, the row and column factors)."""
     fill_weight = 2.0 if improved else 1.0
     if sparse_adj.shape[0] != sparse_adj.shape[1]:
         if add_self_loop:
@@ -58,23 +73,22 @@ def gcn_norm_adj(sparse_adj, norm="both", add_self_loop=True, sym=True, renorm=T
         value = ops.scale_edges(sparse_adj.index[0].contiguous(), sparse_adj.index[1].contiguous(), sparse_adj.value,
                                 dl=row_dis, dr=col_dis)
         normed = sparse_adj.with_value(value)
+        aux = ("both_sym" if sym else "both", sparse_adj, value, row_dis, col_dis)
         if add_self_loop and not renorm:
             normed = normed.add_diag(fill_weight)
     elif norm == "left":
         row_inv = ops.deg_inv(sparse_adj.segment_sum(axis=-1), ops.POW_INV)
         normed = sparse_adj.with_value(ops.scale_edges(sparse_adj.index[0].contiguous(), None, sparse_adj.value,
                                                        dl=row_inv))
+        aux = ("left", sparse_adj, normed.value, row_inv, None)
     elif norm == "right":
         col_inv = ops.deg_inv(sparse_adj.segment_sum(axis=-1), ops.POW_INV)     # row sums, literally as gcn.py:113
         normed = sparse_adj.with_value(ops.scale_edges(None, sparse_adj.index[1].contiguous(), sparse_adj.value,
                                                        dr=col_inv))
+        aux = ("right", sparse_adj, normed.value, col_inv, None)
     else:
         raise Exception("wrong GCN norm type: {}".format(norm))
-
-    if cache is not None:
-        normed.csr, normed.value_csr    # build the CSR now: cached objects are always warm
-        cache[cache_key] = normed
-    return normed
+    return normed, aux
 
 
 def gcn_build_cache_by_adj(sparse_adj, norm="both", add_self_loop=True, sym=True, renorm=True, improved=False,
@@ -128,20 +142,21 @@ def gcn(x, sparse_adj, kernel, bias=None, activation=None,
     if x_sparse is not None:                   # tf.SparseTensor features (gcn.py:269-272): sparse x dense projection
         if kernel is None:
             raise ValueError("a sparse feature matrix needs a kernel (reference gcn.py:266-272)")
-        if autograd.needs_grad(kernel, bias):
-            # training (demo/demo_gcn.py:60-75): dW = x^T dH is the same kernel over the transposed pattern of x
+        if autograd.needs_grad(kernel, bias, x_sparse.value, normed.value):
+            # training (demo/demo_gcn.py:60-75): dW = x^T dH is the same kernel over the transposed pattern of x; learnable
+            # edge weights reach normed.value through the normalisation
             h = autograd.propagate(x_sparse, ops.as_device(kernel, torch.float32, device=dev))
-            h = autograd.SparseMatmul.apply(h, bias, normed, act_code)
+            h = autograd.propagate(normed, h, bias, act_code)
             return leftover(h) if leftover is not None else h
         h = project_features(x_sparse, kernel)
         h = normed.matmul(h, num_or_size_splits=num_or_size_splits, bias=bias, act=act_code)
         return leftover(h) if leftover is not None else h
     x = ops.as_device(x, torch.float32, device=dev)
-    if autograd.needs_grad(x, kernel, bias):
+    if autograd.needs_grad(x, kernel, bias, normed.value):
         # training path (demo/demo_gcn.py:60-75 uses tf.GradientTape): same kernels behind autograd Functions
         h = x if kernel is None else autograd.Dense.apply(x, ops.as_device(kernel, torch.float32, device=dev), None,
                                                          ops.ACT_NONE)
-        h = autograd.SparseMatmul.apply(h, bias, normed, act_code)
+        h = autograd.propagate(normed, h, bias, act_code)
         return leftover(h) if leftover is not None else h
     h = x if kernel is None else ops.gemm(x, ops.as_device(kernel, torch.float32, device=dev))
     h = normed.matmul(h, num_or_size_splits=num_or_size_splits, bias=bias, act=act_code)

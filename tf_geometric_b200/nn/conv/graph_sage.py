@@ -69,7 +69,7 @@ def _plain_sage(reduce, x, edge_index, edge_weight, self_kernel, neighbor_kernel
     dev = edge_index.device
     x = ops.as_device(x, torch.float32, device=dev)
     num_nodes = x.shape[0]
-    if autograd.needs_grad(x, self_kernel, neighbor_kernel, bias):
+    if autograd.needs_grad(x, self_kernel, neighbor_kernel, bias, edge_weight):
         ew = None if edge_weight is None else ops.as_device(edge_weight, torch.float32, device=dev)
         return _plain_sage_autograd(reduce, x, edge_index, ew, ops.as_device(self_kernel, torch.float32, device=dev),
                                     ops.as_device(neighbor_kernel, torch.float32, device=dev),

@@ -22,7 +22,7 @@ def sgc(x, edge_index, edge_weight, k, kernel, bias=None, activation=None, renor
     normed = gcn_norm_adj(SparseMatrix(edge_index, edge_weight, [n, n]), renorm=renorm, improved=improved, cache=cache)
     act_code, leftover = ops.activation_code(activation)
     b = _f32(bias, dev)
-    with_grad = autograd.needs_grad(x, kernel, bias)       # training: the same kernels behind autograd Functions
+    with_grad = autograd.needs_grad(x, kernel, bias, normed.value)     # training: the same kernels behind autograd
     h = autograd.dense(x, _f32(kernel, dev)) if with_grad else ops.gemm(x, _f32(kernel, dev))
     for i in range(k):
         last = i == k - 1
@@ -49,7 +49,7 @@ def ssgc(x, edge_index, edge_weight, kernels=None, biases=None, k=10, alpha=0.1,
     n = h.shape[0]
     normed = gcn_norm_adj(SparseMatrix(edge_index, edge_weight, [n, n]), cache=cache)
     normed = normed.dropout(edge_drop_rate, training=training)                          # ssgc.py:60-61
-    with_grad = autograd.needs_grad(h, *[t for t in list(kernels or []) + list(biases or []) if t is not None])
+    with_grad = autograd.needs_grad(h, normed.value, *[t for t in list(kernels or []) + list(biases or []) if t is not None])
     if kernels is not None:
         num_dense = len(kernels)
         for i, (kern, b) in enumerate(zip(kernels, biases)):
@@ -79,7 +79,7 @@ def tagcn(x, edge_index, edge_weight, k, kernel, bias=None, activation=None, ren
     x = _f32(x, dev)
     n, f = x.shape
     normed = gcn_norm_adj(SparseMatrix(edge_index, edge_weight, [n, n]), renorm=renorm, improved=improved, cache=cache)
-    if autograd.needs_grad(x, kernel, bias):
+    if autograd.needs_grad(x, kernel, bias, normed.value):
         terms = [x]
         for _ in range(k):
             terms.append(autograd.propagate(normed, terms[-1]))
@@ -124,7 +124,7 @@ def le_conv(x, edge_index, edge_weight, self_kernel, self_bias, aggr_self_kernel
     x = _f32(x, dev)
     n = x.shape[0]
     if autograd.needs_grad(x, self_kernel, self_bias, aggr_self_kernel, aggr_self_bias, aggr_neighbor_kernel,
-                           aggr_neighbor_bias):
+                           aggr_neighbor_bias, edge_weight):
         self_h = autograd.dense(x, _f32(self_kernel, dev), _f32(self_bias, dev))
         diff = autograd.dense(x, _f32(aggr_self_kernel, dev), _f32(aggr_self_bias, dev)) \
             - autograd.dense(x, _f32(aggr_neighbor_kernel, dev), _f32(aggr_neighbor_bias, dev))

@@ -616,6 +616,32 @@ def random_pairs(num_nodes, num_samples, seed, device, rng_stream=RNG_STREAM_LIN
     return out
 
 
+# ---- K7: edge-weight gradients ----------------------------------------------------------------------------------
+
+def sddmm_csr(csr, G, X, row_scale=None, alpha=1.0, edge_order=True, out=None):
+    """out[e] = alpha * row_scale[r] * <G[r], X[col_e]> for every CSR slot of row r (K7, tfgk_sddmm_csr_f32): the gradient
+    of K1's output with respect to its edge weights.  edge_order=True writes slot p to out[csr.perm[p]], the order of
+    the edge list (or SparseMatrix values) the CSR was built from; False keeps CSR order.  G: [n_rows, D], X: [*, D]
+    (column slices are fine); row_scale: float32 [n_rows] or None."""
+    for t, n in ((G, "G"), (X, "X")):
+        if not (t.is_cuda and t.dtype == torch.float32 and t.dim() == 2):
+            raise TypeError("{} must be a 2-D float32 CUDA tensor".format(n))
+    D = G.shape[1]
+    if X.shape[1] != D or G.shape[0] != csr.n_rows:
+        raise ValueError("sddmm_csr: G is {} and X is {} for a CSR of {} rows".format(tuple(G.shape), tuple(X.shape),
+                                                                                  csr.n_rows))
+    if row_scale is not None:
+        _check(row_scale, torch.float32, "row_scale")
+    if out is None:
+        out = torch.empty((csr.nnz,), dtype=torch.float32, device=G.device)
+    _check(out, torch.float32, "out")
+    if csr.nnz:
+        _ffi.call("tfgk_sddmm_csr_f32", _p(csr.rowptr), _p(csr.col), _p(csr.perm) if edge_order else None, csr.n_rows,
+                  _p(G), _row_major_2d(G, "G"), _p(X), _row_major_2d(X, "X"), D, _p(row_scale), float(alpha), _p(out),
+                  _stream(G))
+    return out
+
+
 # ---- K4 ----------------------------------------------------------------------------------------------------------
 
 def gemm(a, b, bias=None, act=ACT_NONE, trans_a=False, trans_b=False, beta=0.0, out=None):

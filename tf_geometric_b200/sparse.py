@@ -105,7 +105,12 @@ class SparseMatrix(object):
         become explicit zeros and the kept ones are scaled by 1/(1-rate).  `seed` (an extension) pins the mask."""
         if not training or rate <= 0.0:
             return self
-        out = SparseMatrix(self.index, ops.dropout(self.value, rate, _rng.resolve(seed)), self._shape, _csr=self._csr)
+        from . import autograd
+        seed = _rng.resolve(seed)
+        # differentiable values (learnable edge weights) take the gradient through the same regenerated mask
+        value = autograd.Dropout.apply(self.value, rate, seed) if autograd.needs_grad(self.value) else \
+            ops.dropout(self.value, rate, seed)
+        out = SparseMatrix(self.index, value, self._shape, _csr=self._csr)
         out._pattern_of = self            # the transposed structure (backward) is built once, on the cached parent
         return out
 
@@ -116,9 +121,10 @@ class SparseMatrix(object):
         same bits with or without it."""
         h = ops.as_device(h, torch.float32, device=self.index.device)
         from . import autograd
-        if autograd.needs_grad(h, epilogue.get("bias")):
-            # `A @ h` inside a user's training loop (tf_sparse products are differentiable under tf.GradientTape): the same
-            # kernel behind autograd (dh = A^T g over the transposed structure); column chunks change no bit, so none here
+        if autograd.needs_grad(h, epilogue.get("bias"), self.value):
+            # `A @ h` inside a user's training loop (tf_sparse products are differentiable under tf.GradientTape, in h and
+            # in A's values): the same kernel behind autograd (dh = A^T g over the transposed structure, d value by K7);
+            # column chunks change no bit, so none here
             if h.dim() != 2 or set(epilogue) - {"bias", "act"}:
                 raise NotImplementedError("SparseMatrix.matmul: gradients are built for act(A @ h + bias) with a 2-D h")
             return autograd.propagate(self, h, epilogue.get("bias"), epilogue.get("act", ops.ACT_NONE))
