@@ -378,6 +378,32 @@ int tfgk_sddmm_csr_f32(const int64_t *rowptr, const int32_t *col, const int32_t 
                        const float *G, int64_t ldg, const float *X, int64_t ldx, int32_t D,
                        const float *row_scale, float alpha, float *out, void *stream);
 
+/* ---- DiffPool / MinCutPool: per-graph dense algebra (nn/pool/cluster_pool.py:32-44) -------------------------------
+ * A batch of G graphs whose nodes are each assigned to C clusters of their own graph; block layout: row g*C + c of a
+ * [G*C, *] matrix belongs to cluster c of graph g. */
+
+/* K8a, per-graph transposed product: out[g*C + c, d] = sum_{n in graph g} S[n, c] * Y[n, d], fp32, for c < C, d < D.
+ * Graph g's nodes are the node-list positions p in [gptr[g], gptr[g+1]), node id gnodes[p] (gnodes NULL: p itself, i.e.
+ * graph-major nodes).  S is [N, C] (lds), Y [N, D] (ldy), out [G*C, D] (ldo); column slices are fine.  S^T X, S^T (A S)
+ * and S^T S are one launch each.  Every graph is cut into chunks of 1024 positions; a graph with several chunks sums
+ * them into the workspace and a fix-up adds the partial blocks in chunk order.  Within a chunk the rows are summed in
+ * node-list order with fmaf, so a graph's bits depend only on its own rows (not on G, the grid or the other graphs); no
+ * atomics.  A node id outside [0, N), or a graph whose positions reach past N, makes its graph's block NaN.  Asynchronous (the chunk plan is computed on the device).
+ * Algorithmic bytes: N * 4 (C + D) + G * C * D * 4 + G * 8. */
+int tfgk_graph_tmm_workspace_bytes(int32_t G, int32_t N, int32_t C, int32_t D, size_t *out_bytes);
+int tfgk_graph_tmm_f32(const float *S, int64_t lds, const float *Y, int64_t ldy, int32_t N, int32_t C, int32_t D,
+                       const int64_t *gptr, const int32_t *gnodes, int32_t G, float *out, int64_t ldo, void *workspace,
+                       size_t workspace_bytes, void *stream);
+
+/* K8b, row times its graph's block: with g = node_graph[n] and B [G*C, K] (ldb) in block layout,
+ *   trans = 0: out[n, k] = beta * out[n, k] + sum_{c < C} Y[n, c] * B[g*C + c, k]     Y [N, C], out [N, K]
+ *   trans = 1: out[n, c] = beta * out[n, c] + sum_{k < K} Y[n, k] * B[g*C + c, k]     Y [N, K], out [N, C]
+ * (beta = 0 never reads out).  The backward of K8a and of S^T A S: dX = S dP, dS = X dP^T + T dQ^T + U dQ, and S dQ for
+ * the edge-weight gradient.  One output element per thread, summed in ascending order with fmaf: bits independent of the
+ * grid.  A graph id outside [0, G) gives NaN.  Asynchronous.  Algorithmic bytes: N * 4 (C + K + 1) + G * C * K * 4. */
+int tfgk_graph_rmm_f32(const float *Y, int64_t ldy, const int32_t *node_graph, int32_t N, const float *B, int64_t ldb,
+                       int32_t G, int32_t C, int32_t K, int trans, float beta, float *out, int64_t ldo, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

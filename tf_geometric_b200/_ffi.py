@@ -100,6 +100,9 @@ SIGNATURES = {
     "tfgk_neg_sample_start": [_ptr, _ptr, _i32, _ptr, _i64, _u64, _u32, _ptr, _ptr],
     "tfgk_random_pairs_i32": [_i32, _i64, _u64, _u32, _ptr, _ptr],
     "tfgk_sddmm_csr_f32": [_ptr, _ptr, _ptr, _i32, _ptr, _i64, _ptr, _i64, _i32, _ptr, _f32, _ptr, _ptr],
+    "tfgk_graph_tmm_workspace_bytes": [_i32, _i32, _i32, _i32, ctypes.POINTER(_size)],
+    "tfgk_graph_tmm_f32": [_ptr, _i64, _ptr, _i64, _i32, _i32, _i32, _ptr, _ptr, _i32, _ptr, _i64, _ptr, _size, _ptr],
+    "tfgk_graph_rmm_f32": [_ptr, _i64, _ptr, _i32, _ptr, _i64, _i32, _i32, _i32, _int, _f32, _ptr, _i64, _ptr],
 }
 
 

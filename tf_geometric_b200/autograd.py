@@ -372,8 +372,10 @@ class TakeRows(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, grad_out):
-        csr = _structure.csr_for_segment_ids(ctx.index, ctx.n)
         g = grad_out.contiguous()
+        if ctx.index.numel() == 0:                     # nothing was taken (e.g. a pooled graph without edges)
+            return g.new_zeros((ctx.n,) + tuple(g.shape[1:])), None
+        csr = _structure.csr_for_segment_ids(ctx.index, ctx.n)
         flat = g if g.dim() == 2 else g.unsqueeze(1)
         res = ops.spmm(csr, None, flat, reduce="sum", col=csr.perm)
         return (res if g.dim() == 2 else res.squeeze(1)), None
@@ -464,6 +466,70 @@ class EdgeDot(torch.autograd.Function):
         g = grad_logits.to(torch.float32).reshape(-1)
         w = ops.permute(torch.cat([g, g]).contiguous(), csr.perm)
         return ops.spmm(csr, w, h, reduce="sum"), None
+
+
+class ClusterPool(torch.autograd.Function):
+    """DiffPool / MinCutPool coarsening (nn/pool/cluster_pool.py:32-44) per graph g, in block layout:
+        P[g*C + c] = (S_g^T X_g)[c]          Q[g*C + c, c'] = (S_g^T A_g S_g)[c, c'],   A[row_e, col_e] += w_e
+    without the dense [G*C, N] assignment or N x N adjacency of the reference.  `layout` (nn/pool/cluster_pool.py) holds
+    the edge CSR, the graph pointer / node list and node -> graph ids.  x may be None (then P is [G*C, 0]).
+    Forward: T = A S (K1), Q = K8a(S, T), P = K8a(S, X); T is kept for the backward (N * C floats).
+    Backward, with U = A^T S (K1 over the transposed CSR):
+        dX = S dP            dS = X dP^T + T dQ^T + U dQ          (K8b)
+        dw_e = <(S dQ)[row_e], S[col_e]>                          (K8b, then K7)
+    The forward runs the same kernels whatever requires grad, so gradients change no forward bit."""
+
+    @staticmethod
+    def forward(ctx, x, s, edge_weight, layout):
+        sd = s.detach()
+        xd = torch.empty((sd.shape[0], 0), dtype=torch.float32, device=sd.device) if x is None else x.detach()
+        w_csr = _structure.weights_in_csr_order(edge_weight.detach(), layout.csr)
+        t = ops.spmm(layout.csr, w_csr, sd, reduce="sum")
+        q = ops.graph_tmm(sd, t, layout.gptr, layout.num_graphs, gnodes=layout.gnodes)
+        p = ops.graph_tmm(sd, xd, layout.gptr, layout.num_graphs, gnodes=layout.gnodes)
+        ctx.layout = layout
+        ctx.edge_weight = edge_weight.detach()
+        ctx.save_for_backward(xd, sd, t)
+        return p, q
+
+    @staticmethod
+    def backward(ctx, grad_p, grad_q):
+        x, s, t = ctx.saved_tensors
+        lay = ctx.layout
+        C, ng = lay.num_clusters, lay.node_graph
+        dp, dq = grad_p.contiguous(), grad_q.contiguous()
+        grad_x = grad_s = grad_w = None
+        if ctx.needs_input_grad[0]:
+            grad_x = ops.graph_rmm(s, dp, ng, C)
+        if ctx.needs_input_grad[1]:
+            grad_s = ops.graph_rmm(t, dq, ng, C, trans=True)
+            if x.shape[1]:
+                ops.graph_rmm(x, dp, ng, C, trans=True, beta=1.0, out=grad_s)
+            csr_t, w_t = _transposed_structure(lay.edge_index, lay.num_nodes, ctx.edge_weight, False, lay.csr)
+            u = ops.spmm(csr_t, w_t, s, reduce="sum")
+            ops.graph_rmm(u, dq, ng, C, beta=1.0, out=grad_s)
+        if ctx.needs_input_grad[2]:
+            grad_w = ops.sddmm_csr(lay.csr, ops.graph_rmm(s, dq, ng, C), s)
+        return grad_x, grad_s, grad_w, None
+
+
+class AssignGram(torch.autograd.Function):
+    """M[g*C + c, c'] = (S_g^T S_g)[c, c'] (the S^T S of min_cut_pool.py:85-93) through K8a; dS = S dM + S dM^T (K8b)."""
+
+    @staticmethod
+    def forward(ctx, s, layout):
+        sd = s.detach()
+        ctx.layout = layout
+        ctx.save_for_backward(sd)
+        return ops.graph_tmm(sd, sd, layout.gptr, layout.num_graphs, gnodes=layout.gnodes)
+
+    @staticmethod
+    def backward(ctx, grad_m):
+        (s,) = ctx.saved_tensors
+        lay = ctx.layout
+        g = grad_m.contiguous()
+        out = ops.graph_rmm(s, g, lay.node_graph, lay.num_clusters)
+        return ops.graph_rmm(s, g, lay.node_graph, lay.num_clusters, trans=True, beta=1.0, out=out), None
 
 
 def needs_grad(*tensors):

@@ -17,6 +17,8 @@ _EXPORTS = {
     pool.set2set: ("set2set",),
     pool.topk_pool: ("topk_pool",),
     pool.score_pool: ("sag_pool", "sort_pool"),
+    pool.diff_pool: ("diff_pool", "diff_pool_coarsen"),
+    pool.min_cut_pool: ("min_cut_pool", "min_cut_pool_coarsen", "min_cut_pool_compute_losses"),
     sampling.drop_edge: ("drop_edge",),
     link.predict_edge: ("predict_edge",),
 }

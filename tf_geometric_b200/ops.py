@@ -642,6 +642,68 @@ def sddmm_csr(csr, G, X, row_scale=None, alpha=1.0, edge_order=True, out=None):
     return out
 
 
+# ---- K8: per-graph dense algebra of DiffPool / MinCutPool ----------------------------------------------------------
+
+def _float_2d(t, name):
+    if not (torch.is_tensor(t) and t.is_cuda and t.dtype == torch.float32 and t.dim() == 2):
+        raise TypeError("{} must be a 2-D float32 CUDA tensor".format(name))
+    return _row_major_2d(t, name)
+
+
+def graph_tmm(S, Y, gptr, num_graphs, gnodes=None, out=None):
+    """out[g*C + c] = sum_{n in graph g} S[n, c] * Y[n] (K8a, tfgk_graph_tmm_f32): the per-graph S_g^T Y_g in block
+    layout [G*C, D].  gptr int64 [G+1] delimits the node-list positions of every graph, gnodes int32 [N] maps positions to
+    node ids (None: positions are node ids, i.e. graph-major nodes).  S: [N, C], Y: [N, D]; column slices are fine."""
+    lds, ldy = _float_2d(S, "S"), _float_2d(Y, "Y")
+    N, C = S.shape
+    D = Y.shape[1]
+    G = int(num_graphs)
+    if Y.shape[0] != N:
+        raise ValueError("graph_tmm: S has {} rows and Y {}".format(N, Y.shape[0]))
+    if C < 1:
+        raise ValueError("graph_tmm: S needs at least one cluster column")
+    _check(gptr, torch.int64, "gptr")
+    if gptr.numel() != G + 1:
+        raise ValueError("graph_tmm: gptr has {} entries for {} graphs".format(gptr.numel(), G))
+    if gnodes is not None:
+        _check(gnodes, torch.int32, "gnodes")
+    if out is None:
+        out = torch.empty((G * C, D), dtype=torch.float32, device=S.device)
+    ldo = _float_2d(out, "out")
+    need = ctypes.c_size_t()
+    _ffi.call("tfgk_graph_tmm_workspace_bytes", G, N, C, D, ctypes.byref(need))
+    ws = torch.empty((max(need.value, 1),), dtype=torch.uint8, device=S.device)
+    _ffi.call("tfgk_graph_tmm_f32", _p(S), lds, _p(Y), ldy, N, C, D, _p(gptr), _p(gnodes), G, _p(out), ldo, _p(ws),
+              need.value, _stream(S))
+    return out
+
+
+def graph_rmm(Y, B, node_graph, num_clusters, trans=False, beta=0.0, out=None):
+    """Every row times its graph's [C, K] block of the block-layout matrix B [G*C, K] (K8b, tfgk_graph_rmm_f32):
+    trans=False: out[n] = beta * out[n] + Y[n, :C] @ B_g          (out [N, K])
+    trans=True : out[n] = beta * out[n] + Y[n, :K] @ B_g^T        (out [N, C])
+    with g = node_graph[n] (int32 [N])."""
+    ldy, ldb = _float_2d(Y, "Y"), _float_2d(B, "B")
+    C = int(num_clusters)
+    N = Y.shape[0]
+    if C < 1 or B.shape[0] % C:
+        raise ValueError("graph_rmm: B has {} rows, not a multiple of {} clusters".format(B.shape[0], C))
+    G, K = B.shape[0] // C, B.shape[1]
+    if Y.shape[1] != (K if trans else C):
+        raise ValueError("graph_rmm: Y has {} columns, {} expected".format(Y.shape[1], K if trans else C))
+    _check(node_graph, torch.int32, "node_graph")
+    if node_graph.numel() != N:
+        raise ValueError("graph_rmm: node_graph has {} entries for {} rows".format(node_graph.numel(), N))
+    if out is None:
+        if beta != 0.0:
+            raise ValueError("graph_rmm: beta != 0 needs `out`")
+        out = torch.empty((N, C if trans else K), dtype=torch.float32, device=Y.device)
+    ldo = _float_2d(out, "out")
+    _ffi.call("tfgk_graph_rmm_f32", _p(Y), ldy, _p(node_graph), N, _p(B), ldb, G, C, K, 1 if trans else 0, float(beta),
+              _p(out), ldo, _stream(Y))
+    return out
+
+
 # ---- K4 ----------------------------------------------------------------------------------------------------------
 
 def gemm(a, b, bias=None, act=ACT_NONE, trans_a=False, trans_b=False, beta=0.0, out=None):

@@ -181,7 +181,19 @@ def convert_edge_to_directed(edge_index, edge_props=None, merge_modes=None):
 
 
 def remove_self_loop_edge(edge_index, edge_weight=None):
-    """reference :252-269."""
+    """reference :252-269.  Device tensors stay on the device: the kept positions come from tfgk_select_flagged_i32 and
+    the kept weights are a differentiable gather (the same bits as the host path, and the weights' autograd graph is
+    kept, which MinCutPool's pooled weights need)."""
+    if _is_device(edge_index):
+        from .. import autograd
+        ei = (edge_index if edge_index.dtype == torch.int32 else edge_index.to(torch.int32)).contiguous()
+        row, col = ei[0].contiguous(), ei[1].contiguous()
+        keep = ops.select_flagged((row != col).to(torch.int32))
+        out_index = torch.stack([ops.gather_i32(row, keep), ops.gather_i32(col, keep)])
+        out_w = None
+        if edge_weight is not None:
+            out_w = autograd.TakeRows.apply(ops.as_device(edge_weight, torch.float32, device=ei.device).reshape(-1), keep)
+        return out_index, out_w
     ei = _to_numpy(edge_index)
     mask = ei[0] != ei[1]
     out_w = None
@@ -213,20 +225,68 @@ def add_self_loop_edge(edge_index, num_nodes, edge_weight=None, fill_weight=1.0)
 
 
 def adj_norm_edge(edge_index, num_nodes, edge_weight=None, add_self_loop=False, cache=None):
-    """D^-1/2 A D^-1/2 on the edge list with ROW degrees on both sides (reference :914-943)."""
+    """D^-1/2 A D^-1/2 on the edge list with ROW degrees on both sides (reference :914-943).  Differentiable in
+    edge_weight (GcnNormValues, kind "both_sym"); the forward runs the same kernels either way.  A warm cache hit returns
+    the cached constant, as gcn_norm_adj does."""
     cache_key = "adj_normed_edge"
     if cache is not None and cache.get(cache_key) is not None:
         return cache[cache_key]
+    from .. import autograd
     from ..sparse import SparseMatrix
     ei = ops.as_device(edge_index, torch.int32)
     adj = SparseMatrix(ei, edge_weight, [num_nodes, num_nodes])
+    w = adj.value
     if add_self_loop:
         adj = adj.add_diag(1.0)
     dis = ops.deg_inv(adj.segment_sum(axis=-1), ops.POW_INV_SQRT)
-    normed = ops.scale_edges(adj.index[0].contiguous(), adj.index[1].contiguous(), adj.value, dl=dis, dr=dis)
+    normed = ops.scale_edges(adj.index[0].contiguous(), adj.index[1].contiguous(), adj.value.detach(), dl=dis, dr=dis)
     if cache is not None:
         cache[cache_key] = adj.index, normed
+    if autograd.needs_grad(w):
+        normed = autograd.GcnNormValues.apply(w, normed, ("both_sym", adj, normed, dis, dis))
     return adj.index, normed
+
+
+def convert_dense_adj_to_edge(dense_adj):
+    """The non-zero entries of a dense [M, M] matrix as an edge list, row-major (reference :272-285): entries != 0 are
+    kept, so NaN is.  Device tensors: positions from tfgk_select_flagged_i32, weights a differentiable gather."""
+    if _is_device(dense_adj):
+        from .. import autograd
+        m = dense_adj.shape[0]
+        flat = dense_adj.reshape(-1)
+        if flat.dtype != torch.float32:
+            flat = flat.to(torch.float32)
+        k = ops.select_flagged((flat != 0).to(torch.int32))
+        k64 = k.to(torch.int64)
+        edge_index = torch.stack([k64 // m, k64 % m]).to(torch.int32)
+        return edge_index, autograd.TakeRows.apply(flat.contiguous(), k)
+    a = _to_numpy(dense_adj)
+    row, col = np.nonzero(a != 0)
+    return np.stack([row, col]).astype(np.int32), a[row, col]
+
+
+def convert_dense_assign_to_edge(dense_assign, node_graph_index=None, num_nodes=None, num_clusters=None):
+    """Assignment matrix [N, C] -> (edge_index [2, N*C], edge_weight [N*C]) with edge (n, C * graph(n) + c) for entry
+    (n, c), row-major (reference :288-322).  Device tensors stay on the device and the weights are a differentiable
+    view of the matrix."""
+    if _is_device(dense_assign):
+        n = int(dense_assign.shape[0] if num_nodes is None else num_nodes)
+        c = int(dense_assign.shape[1] if num_clusters is None else num_clusters)
+        dev = dense_assign.device
+        row = torch.arange(n, dtype=torch.int32, device=dev).repeat_interleave(c)
+        col = torch.arange(c, dtype=torch.int32, device=dev).repeat(n)
+        if node_graph_index is not None:
+            ngi = ops.as_device(node_graph_index, torch.int32, device=dev)
+            col = col + ngi.repeat_interleave(c) * c
+        return torch.stack([row, col]), dense_assign.reshape(-1)
+    a = _to_numpy(dense_assign)
+    n = a.shape[0] if num_nodes is None else int(num_nodes)
+    c = a.shape[1] if num_clusters is None else int(num_clusters)
+    row = np.repeat(np.arange(n, dtype=np.int32), c)
+    col = np.tile(np.arange(c, dtype=np.int32), n)
+    if node_graph_index is not None:
+        col = col + np.repeat(_to_numpy(node_graph_index).astype(np.int32), c) * c
+    return np.stack([row, col]).astype(np.int32), a.reshape(-1)
 
 
 def compute_num_or_size_splits(num_h_features, num_splits):

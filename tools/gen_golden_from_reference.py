@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 # coding=utf-8
-"""Generate tests/golden/ref_exec_*.npz and link_exec.npz by EXECUTING the reference's own Python (a read-only checkout of
+"""Generate tests/golden/ref_exec_*.npz, link_exec.npz and cluster_pool_exec.npz by EXECUTING the reference's own Python (a read-only checkout of
 CrawlScript/tf_geometric named by $TFG_REFERENCE) over the numpy shims in tools/ref_shim.  The tests never need the
 reference: the resulting small fixtures are committed.  Re-run:  TFG_REFERENCE=<checkout> python tools/gen_golden_from_reference.py
 """
@@ -359,6 +359,80 @@ def main():
     # by tests/test_link_host.py and tests/test_gpu_link.py
     np.savez_compressed(os.path.join(OUT, "link_exec.npz"), **{k: np.asarray(v) for k, v in out.items()})
     print("wrote link_exec.npz: {}".format(", ".join(sorted(out))))
+
+    # ---- DiffPool / MinCutPool: nn/pool/{cluster_pool,diff_pool,min_cut_pool}.py and utils convert_dense_* -----------
+    # tests/golden/cluster_pool_exec.npz (read by tests/test_cluster_pool_host.py and tests/test_gpu_cluster_pool.py).  The
+    # sub-GNNs are arguments of the reference functions: simple deterministic callables, restated in
+    # tests/cluster_pool_ref.py.  Own RandomState, so the fixtures above are unchanged.
+    cluster_pool_fixture()
+
+
+def golden_gnn(weight, mix):
+    """[x, edge_index, edge_weight] -> x W + sum_{e: row_e = r} w_e (x M)[col_e], then tanh when it is a feature GNN."""
+    def gnn(inputs, training=None, cache=None):
+        x, ei, w = (np.asarray(a) for a in inputs)
+        h, m = (x @ weight).astype(np.float32), (x @ mix).astype(np.float32)
+        agg = np.zeros_like(m)
+        for e in range(ei.shape[1]):
+            agg[ei[0, e]] = agg[ei[0, e]] + w[e] * m[ei[1, e]]
+        return T((h + agg).astype(np.float32))
+    return gnn
+
+
+def cluster_pool_fixture():
+    diff_m = importlib.import_module("tf_geometric.nn.pool.diff_pool")
+    mc_m = importlib.import_module("tf_geometric.nn.pool.min_cut_pool")
+    crs = np.random.RandomState(77)
+    sizes = [6, 3, 8, 5]                                       # graph 1 has no edge
+    rows, cols, base = [], [], 0
+    for g, size in enumerate(sizes):
+        if g != 1:
+            half = 2 * size
+            u, v = crs.randint(0, size, half), crs.randint(0, size, half)
+            keep = u != v
+            rows += list(base + u[keep]) + list(base + v[keep])
+            cols += list(base + v[keep]) + list(base + u[keep])
+        base += size
+    rows += [rows[0], 0, 10]                                   # a duplicate of edge 0 and two self loops
+    cols += [cols[0], 0, 10]
+    n = base
+    gi_sorted = np.repeat(np.arange(len(sizes)), sizes).astype(np.int32)
+    perm = crs.permutation(n)                                  # node p of the batch is sorted node perm[p]: unsorted gi
+    inv = np.empty_like(perm)
+    inv[perm] = np.arange(n)
+    ei = inv[np.array([rows, cols])].astype(np.int32)
+    gi = gi_sorted[perm].astype(np.int32)
+    w = (crs.rand(ei.shape[1]) + 0.3).astype(np.float32)
+    f_in, f_out = 4, 5
+    x = crs.randn(n, f_in).astype(np.float32)
+    out = {"x": x, "ei": ei, "w": w, "gi": gi}
+    for c in (3, 1):
+        wf, mf = glorot(crs, f_in, f_out), glorot(crs, f_in, f_out)
+        wa, ma = glorot(crs, f_in, c), glorot(crs, f_in, c)
+        bias = (crs.randn(f_out) * 0.1).astype(np.float32)
+        out.update({"wf_c%d" % c: wf, "mf_c%d" % c: mf, "wa_c%d" % c: wa, "ma_c%d" % c: ma, "bias_c%d" % c: bias})
+        feat, assign = golden_gnn(wf, mf), golden_gnn(wa, ma)
+        relu = tf.nn.relu
+        cases = {"diff": lambda ew: diff_m.diff_pool(T(x), T(ei), ew, T(gi), feat, assign, c, bias=T(bias), activation=relu)}
+        for tag, ew in (("w", T(w)), ("none", None)):
+            px, pei, pw, pgi = cases["diff"](ew)
+            out.update({"diff_%s_c%d_%s" % (tag, c, k): v for k, v in zip(("x", "ei", "w", "gi"), (px, pei, pw, pgi))})
+        for tag, normed in (("normed", True), ("raw", False)):
+            (px, pei, pw, pgi), (cut, orth) = mc_m.min_cut_pool(T(x), T(ei), T(w), T(gi), feat, assign, c, bias=T(bias),
+                                                                 activation=relu, gnn_use_normed_edge=normed,
+                                                                 return_losses=True)
+            out.update({"mincut_%s_c%d_%s" % (tag, c, k): v
+                        for k, v in zip(("x", "ei", "w", "gi", "cut", "orth"), (px, pei, pw, pgi, cut, orth))})
+    dense = crs.randn(5, 5).astype(np.float32)
+    dense[dense < 0.2] = 0.0
+    dense[1, 3] = np.nan
+    out["dense_adj"] = dense
+    out["dense_adj_ei"], out["dense_adj_w"] = gu.convert_dense_adj_to_edge(T(dense))
+    assign = crs.rand(n, 3).astype(np.float32)
+    out["dense_assign"] = assign
+    out["dense_assign_ei"], out["dense_assign_w"] = gu.convert_dense_assign_to_edge(T(assign), T(gi))
+    np.savez_compressed(os.path.join(OUT, "cluster_pool_exec.npz"), **{k: np.asarray(v) for k, v in out.items()})
+    print("wrote cluster_pool_exec.npz: {}".format(", ".join(sorted(out))))
 
 
 if __name__ == "__main__":

@@ -1,6 +1,7 @@
 # coding=utf-8
 """numpy stand-ins for `tensorflow` and `tf_sparse`, just large enough to EXECUTE the reference's own Python files
 for the message-passing hot path (nn/kernel/*.py, nn/conv/{gcn,gat,graph_sage,appnp}.py, utils/graph_utils.py)
+and the cluster pooling (nn/pool/{cluster_pool,diff_pool,min_cut_pool}.py)
 in a container that has neither package.  Used ONLY by tools/gen_golden_from_reference.py to produce
 tests/golden/ref_exec_*.npz.  What this pins: the reference's control flow, call order, quirks and in-repo arithmetic.
 What it cannot pin: TensorFlow's / tf_sparse's own kernels - their semantics are restated here from the public docs
@@ -206,15 +207,98 @@ def build_tensorflow():
     nn = types.ModuleType("tensorflow.nn")
     nn.relu = lambda x: T(np.maximum(np.asarray(x), np.float32(0)))
     nn.l2_normalize = lambda x, axis=-1: T(_l2_normalize_last_axis(x))
+
+    def softmax(logits, axis=-1):
+        x = np.asarray(logits, dtype=np.float32)
+        e = np.exp(x - np.max(x, axis=axis, keepdims=True)).astype(np.float32)
+        return T((e / np.sum(e, axis=axis, keepdims=True, dtype=np.float32)).astype(np.float32))
+    nn.softmax = softmax
     nn.__getattr__ = lambda name: _unsupported("tf.nn." + name)
     tf.nn = nn
+
+    tf.sqrt = lambda x: (T(np.sqrt(np.asarray(x))) if np.ndim(x) else np.sqrt(np.float32(x)))
+    tf.transpose = lambda x, perm=None: T(np.transpose(np.asarray(x), perm))
+    tf.tile = lambda x, multiples: T(np.tile(np.asarray(x), [int(m) for m in multiples]))
+
+    def eye(num_rows, num_columns=None, batch_shape=None, dtype=np.float32):
+        m = np.eye(int(num_rows), int(num_rows if num_columns is None else num_columns), dtype=dtype)
+        if batch_shape is not None:
+            m = np.tile(m, [int(b) for b in batch_shape] + [1, 1])
+        return T(m)
+    tf.eye = eye
+
+    def norm(x, ord="euclidean", axis=None, keepdims=False):
+        # tf.norm(ord="euclidean", axis=[-2, -1]): the Frobenius norm of every matrix, sqrt of the sum of squares in float32
+        assert ord == "euclidean" and axis is not None and [int(a) for a in axis] == [-2, -1]
+        x = np.asarray(x, dtype=np.float32)
+        out = np.zeros(x.shape[:-2], dtype=np.float32)
+        for b in np.ndindex(*x.shape[:-2]):
+            acc = np.float32(0)
+            for v in x[b].reshape(-1):
+                acc = np.float32(acc + v * v)
+            out[b] = np.sqrt(acc)
+        return T(out.reshape(x.shape[:-2] + (1, 1)) if keepdims else out)
+    tf.norm = norm
 
     sparse = types.ModuleType("tensorflow.sparse")
 
     class SparseTensor(object):
-        pass
+        """tf.SparseTensor of rank 2: indices [nnz, 2] int64, values [nnz], dense_shape; no implicit ordering."""
+
+        def __init__(self, indices, values, dense_shape):
+            self.indices = np.asarray(indices, dtype=np.int64).reshape(-1, 2)
+            self.values = np.asarray(values)
+            self.dense_shape = [int(d) for d in np.asarray([int(v) for v in dense_shape])]
+
+        def __mul__(self, other):
+            # SparseTensor * dense: the dense operand is read at the stored positions only (sparse_dense_cwise_mul)
+            d = np.asarray(other)
+            vals = np.empty_like(self.values)
+            for k in range(self.indices.shape[0]):
+                i, j = self.indices[k]
+                vals[k] = self.values[k] * d[i, j]
+            return SparseTensor(self.indices, vals, self.dense_shape)
+
+    def reorder(sp):
+        """tf.sparse.reorder: canonical row-major order of the indices (stable for repeated indices)."""
+        order = sorted(range(sp.indices.shape[0]), key=lambda k: (int(sp.indices[k, 0]), int(sp.indices[k, 1])))
+        return SparseTensor(sp.indices[order], sp.values[order], sp.dense_shape)
+
+    def to_dense(sp):
+        # repeated indices add up here, like tf_sparse's SparseMatrix.to_dense (scatter-add); tf.sparse.to_dense's default
+        # validate_indices would reject them instead, so an adjacency with duplicate edges pins the summing semantics
+        out = np.zeros(sp.dense_shape, dtype=sp.values.dtype)
+        for k in range(sp.indices.shape[0]):
+            i, j = sp.indices[k]
+            out[i, j] = out[i, j] + sp.values[k]
+        return T(out)
+
+    def transpose(sp, perm=None):
+        assert perm is None or [int(p) for p in perm] == [1, 0]
+        return reorder(SparseTensor(sp.indices[:, ::-1], sp.values, sp.dense_shape[::-1]))
+
+    def sparse_dense_matmul(sp, dense):
+        d = np.asarray(dense)
+        out = np.zeros((sp.dense_shape[0], d.shape[1]), dtype=np.result_type(sp.values.dtype, d.dtype))
+        for k in range(sp.indices.shape[0]):              # accumulated entry by entry in index order
+            i, j = sp.indices[k]
+            out[i] = out[i] + sp.values[k] * d[j]
+        return T(out)
+
+    def sparse_reduce_sum(sp, axis=None):
+        assert axis is not None and int(axis) in (-1, 1), "only the row sums are restated"
+        out = np.zeros(sp.dense_shape[0], dtype=sp.values.dtype)
+        for k in range(sp.indices.shape[0]):
+            out[sp.indices[k, 0]] = out[sp.indices[k, 0]] + sp.values[k]
+        return T(out)
+
     sparse.SparseTensor = SparseTensor
     tf.SparseTensor = SparseTensor
+    sparse.reorder = reorder
+    sparse.to_dense = to_dense
+    sparse.transpose = transpose
+    sparse.sparse_dense_matmul = sparse_dense_matmul
+    sparse.reduce_sum = sparse_reduce_sum
 
     class Variable(object):
         pass
@@ -305,10 +389,36 @@ def build_tf_sparse():
             msg = (_gather0(h, np.asarray(self.index[1])) * np.asarray(self.value)[:, None]).astype(np.float32)
             return T(_segment_sum(msg, np.asarray(self.index[0]), self.shape[0]))
 
+        __array_ufunc__ = None                            # dense @ SparseMatrix must reach __rmatmul__
+
+        def to_dense(self):
+            # scatter-add of the entries: duplicates add up
+            out = np.zeros(self.shape, dtype=np.float32)
+            idx, val = np.asarray(self.index), np.asarray(self.value)
+            for k in range(idx.shape[1]):
+                out[idx[0, k], idx[1, k]] = out[idx[0, k], idx[1, k]] + val[k]
+            return T(out)
+
+        def transpose(self):
+            return SparseMatrix(np.asarray(self.index)[::-1], self.value, self.shape[::-1])
+
         def __matmul__(self, other):
             if isinstance(other, DiagMatrix):             # A @ diags(d) : scale columns
                 return SparseMatrix(self.index, T(np.asarray(self.value) * other.d[np.asarray(self.index[1])]), self.shape)
+            if isinstance(other, SparseMatrix):           # sparse @ sparse: the non-zero entries of the product, row-major
+                prod = np.asarray(self.matmul(other.to_dense()))
+                r, c = np.nonzero(prod)
+                return SparseMatrix(np.stack([r, c]), prod[r, c], [self.shape[0], other.shape[1]])
             return self.matmul(other)
+
+        def __rmatmul__(self, other):
+            # dense @ sparse: out[:, j] += dense[:, i] * v for every entry (i, j, v) in stored order
+            d = np.asarray(other, dtype=np.float32)
+            out = np.zeros((d.shape[0], self.shape[1]), dtype=np.float32)
+            idx, val = np.asarray(self.index), np.asarray(self.value)
+            for k in range(idx.shape[1]):
+                out[:, idx[1, k]] = out[:, idx[1, k]] + d[:, idx[0, k]] * val[k]
+            return T(out)
 
     tfs.SparseMatrix = SparseMatrix
     tfs.diags = lambda d: DiagMatrix(d)
