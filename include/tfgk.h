@@ -404,6 +404,29 @@ int tfgk_graph_tmm_f32(const float *S, int64_t lds, const float *Y, int64_t ldy,
 int tfgk_graph_rmm_f32(const float *Y, int64_t ldy, const int32_t *node_graph, int32_t N, const float *B, int64_t ldb,
                        int32_t G, int32_t C, int32_t K, int trans, float beta, float *out, int64_t ldo, void *stream);
 
+/* ---- K9: padded row gather (nn/conv/graph_sage.py:319-337 lstm_graph_sage, utils/graph_utils.py:215-249
+ * convert_x_to_3d): the rows of every CSR row r, in slot order, zero-padded to a width of K --------------------------- */
+
+enum tfgk_pad_layout { TFGK_PAD_ROW_MAJOR = 0, TFGK_PAD_STEP_MAJOR = 1 };
+
+/* out[r, j, :] = X[src[rowptr[r] + j], :] for j < min(deg r, K), zeros for every other j < K; r < R, D columns.
+ * layout TFGK_PAD_ROW_MAJOR: out is [R, K, D]; TFGK_PAD_STEP_MAJOR: out is [K, R, D] (the input order of a sequence-major
+ * recurrence).  out is dense (leading dimension D); X is [NX, D] with leading dimension ldx (column slices are fine).
+ * src is csr.col (neighbour rows) or csr.perm (the data rows of a segment-id CSR).  A padded slot is never read; a src
+ * id outside [0, NX) gives its output row NaN.  slot_out (may be NULL) receives, for every slot p of row r with
+ * j = p - rowptr[r], the flat output row of that slot: r * K + j (row-major) or j * R + r (step-major), -1 for j >= K;
+ * it needs K * R < 2^31.  A pure copy: bit-exact.  16-byte loads and stores when X, ldx, D and out are aligned, scalar
+ * otherwise.  Asynchronous.  Algorithmic bytes: R * K * D * 4 written, kept * (4 D + 4) read, R * 8 for rowptr. */
+int tfgk_pad_rows_f32(const int64_t *rowptr, const int32_t *src, int32_t R, int32_t K, int layout, const float *X,
+                      int64_t ldx, int32_t NX, int32_t D, float *out, int32_t *slot_out, void *stream);
+
+/* Backward of the convert_x_to_3d case (src = perm): for every slot p of row r, j = p - rowptr[r],
+ *   out[perm[p], :] = j < K ? G[r * K + j, :] : 0          G [R, K, D] row-major, out [nnz, D], both dense.
+ * Every output row whose index appears in perm is written exactly once (truncated rows become 0); no atomics.  A perm
+ * entry outside [0, n_out) is skipped.  Asynchronous.  Algorithmic bytes: kept * 8 D + (nnz - kept) * 4 D + nnz * 4. */
+int tfgk_unpad_rows_f32(const int64_t *rowptr, const int32_t *perm, int32_t R, int32_t K, const float *G, int32_t D,
+                        float *out, int64_t n_out, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

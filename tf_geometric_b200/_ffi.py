@@ -24,6 +24,7 @@ FLAG_ALL, FLAG_UPPER, FLAG_MAPPED = 0, 1, 2
 BERNOULLI_NONE, BERNOULLI_DROPOUT, BERNOULLI_KEEP = 0, 1, 2
 SAMPLE_NO_PADDING, SAMPLE_PADDING, SAMPLE_HEAD = 0, 1, 2
 NEG_UPPER, NEG_START = 0, 1
+PAD_ROW_MAJOR, PAD_STEP_MAJOR = 0, 1
 
 _i32, _i64, _f32, _int = ctypes.c_int32, ctypes.c_int64, ctypes.c_float, ctypes.c_int
 _ptr, _size = ctypes.c_void_p, ctypes.c_size_t
@@ -103,6 +104,8 @@ SIGNATURES = {
     "tfgk_graph_tmm_workspace_bytes": [_i32, _i32, _i32, _i32, ctypes.POINTER(_size)],
     "tfgk_graph_tmm_f32": [_ptr, _i64, _ptr, _i64, _i32, _i32, _i32, _ptr, _ptr, _i32, _ptr, _i64, _ptr, _size, _ptr],
     "tfgk_graph_rmm_f32": [_ptr, _i64, _ptr, _i32, _ptr, _i64, _i32, _i32, _i32, _int, _f32, _ptr, _i64, _ptr],
+    "tfgk_pad_rows_f32": [_ptr, _ptr, _i32, _i32, _int, _ptr, _i64, _i32, _i32, _ptr, _ptr, _ptr],
+    "tfgk_unpad_rows_f32": [_ptr, _ptr, _i32, _i32, _ptr, _i32, _ptr, _i64, _ptr],
 }
 
 

@@ -381,6 +381,88 @@ class TakeRows(torch.autograd.Function):
         return (res if g.dim() == 2 else res.squeeze(1)), None
 
 
+class PadRows(torch.autograd.Function):
+    """out[r, j] = x[src[rowptr[r] + j]] zero-padded to K (K9; nn/conv/graph_sage.py:319-337, utils/graph_utils.py:215-249),
+    differentiable w.r.t. x.
+      edge_index None : src = csr.perm of a segment-id CSR (convert_x_to_3d), row-major; backward = unpad_rows (every
+                        row of x is written once, truncated rows get 0).
+      edge_index given: src = csr.col of that edge list's CSR (lstm_graph_sage); every padded slot comes from one edge,
+                        so dx[c] = sum_{e: col_e = c} dout[slot(e)]: K1 over the transposed CSR whose column override is
+                        the flat slot index of each edge (K9's slot output, permuted with gather_i32).  No atomics.
+    The forward runs the same kernel whatever requires grad (the slot output does not change the padded values)."""
+
+    @staticmethod
+    def forward(ctx, x, csr, K, step_major, edge_index):
+        xd = x.detach()
+        by_col = edge_index is not None
+        want_slots = by_col and ctx.needs_input_grad[0]
+        res = ops.pad_rows(csr, xd, K, src=csr.col if by_col else csr.perm, step_major=step_major, slot_index=want_slots)
+        out, slot = res if want_slots else (res, None)
+        ctx.csr, ctx.edge_index, ctx.slot, ctx.n = csr, edge_index, slot, x.shape[0]
+        return out
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        g = grad_out.contiguous()
+        if ctx.edge_index is None:
+            return ops.unpad_rows(ctx.csr, g), None, None, None, None
+        D = g.shape[-1]
+        csr_t, emap = _transposed_of_csr(ctx.csr, ctx.edge_index)
+        slot_col = ops.gather_i32(ctx.slot, emap)
+        return ops.spmm(csr_t, None, g.view(-1, D), reduce="sum", col=slot_col), None, None, None, None
+
+
+class Fp32Recurrence(torch.autograd.Function):
+    """seq = module(inputs)[0] for a torch.nn.LSTM with cuDNN's TF32 math off in the forward AND the backward: cuDNN
+    reads `torch.backends.cudnn.allow_tf32` (default True) when it builds the RNN descriptor of each pass, so a context
+    manager around the call alone would leave the backward on TF32.  The module's graph is built inside the forward and
+    differentiated in the backward under the same setting; the parameters are passed as inputs so that they get their
+    gradients through this node."""
+
+    @staticmethod
+    def forward(ctx, module, inputs, *params):
+        with torch.enable_grad(), _cudnn_fp32():
+            leaf = inputs.detach().requires_grad_(ctx.needs_input_grad[1])
+            seq = module(leaf)[0]
+        ctx.inner = (leaf, seq, params)
+        return seq.detach()
+
+    @staticmethod
+    def backward(ctx, grad_seq):
+        leaf, seq, params = ctx.inner
+        wanted = [(i, t) for i, t in enumerate((leaf,) + tuple(params)) if ctx.needs_input_grad[i + 1]]
+        grads = [None] * (1 + len(params))
+        if wanted:
+            with _cudnn_fp32():
+                got = torch.autograd.grad(seq, [t for _, t in wanted], grad_seq, allow_unused=True)
+            for (i, _), gi in zip(wanted, got):
+                grads[i] = gi
+        ctx.inner = None
+        return (None,) + tuple(grads)
+
+
+class _cudnn_fp32(object):
+    """Context manager: cuDNN without TF32 (restores the caller's setting)."""
+
+    def __enter__(self):
+        self.prev = torch.backends.cudnn.allow_tf32
+        torch.backends.cudnn.allow_tf32 = False
+
+    def __exit__(self, *exc):
+        torch.backends.cudnn.allow_tf32 = self.prev
+        return False
+
+
+def run_lstm_fp32(module, inputs):
+    """Output sequence of a torch.nn.LSTM module with cuDNN's TF32 off in the forward and, when gradients flow, the
+    backward (Fp32Recurrence)."""
+    params = tuple(module.parameters())
+    if needs_grad(inputs, *params):
+        return Fp32Recurrence.apply(module, inputs, *params)
+    with _cudnn_fp32():
+        return module(inputs)[0]
+
+
 class SagePair(torch.autograd.Function):
     """mean / sum GraphSAGE (nn/conv/graph_sage.py:9-115) as ONE differentiable op:
         out = act([x Ws || agg Wn] + b)   (or x Ws + agg Wn + b),   agg = REDUCE_{e: row_e = r} w_e x[col_e].

@@ -10,7 +10,8 @@ _EXPORTS = {
     kernel.segment: ("segment_softmax", "segment_count"),
     conv.gcn: ("gcn", "gcn_norm_adj", "gcn_norm_edge", "gcn_build_cache_by_adj", "gcn_build_cache_for_graph", "compute_cache_key"),
     conv.gat: ("gat",),
-    conv.graph_sage: ("mean_graph_sage", "sum_graph_sage", "gcn_graph_sage", "mean_pool_graph_sage", "max_pool_graph_sage"),
+    conv.graph_sage: ("mean_graph_sage", "sum_graph_sage", "gcn_graph_sage", "mean_pool_graph_sage", "max_pool_graph_sage",
+                        "lstm_graph_sage"),
     conv.appnp: ("appnp",),
     conv.propagation: ("sgc", "ssgc", "tagcn", "gin", "gin_updater", "le_conv", "chebynet", "chebynet_norm_edge", "get_laplacian"),
     pool.common_pool: ("mean_pool", "sum_pool", "max_pool", "min_pool"),

@@ -174,3 +174,39 @@ def max_pool_graph_sage(x, edge_index, edge_weight, self_kernel, neighbor_mlp_ke
     """Max-pooling aggregator (reference graph_sage.py:228-287); nodes without in-edges get float32 lowest."""
     return _pool_sage("max", x, edge_index, edge_weight, self_kernel, neighbor_mlp_kernel, neighbor_kernel,
                       neighbor_mlp_bias, bias, activation, concat, normalize)
+
+
+def _lstm_sage(x, edge_index, reduce_steps, step_major, self_kernel, neighbor_kernel, bias, activation, concat,
+               normalize):
+    """Shared body of lstm_graph_sage and LSTMGraphSage: pad the neighbour rows (K9), `reduce_steps(padded)` -> [N, U]
+    (the recurrence and the mean over all K steps), then the pair projection."""
+    edge_index = ops.as_device(edge_index, torch.int32)
+    dev = edge_index.device
+    x = ops.as_device(x, torch.float32, device=dev)
+    num_nodes, num_edges = x.shape[0], edge_index.shape[1]
+    if num_edges == 0:
+        raise ValueError("lstm_graph_sage needs at least one edge (the reference would run the LSTM over zero steps)")
+    csr, _ = _structure.csr_for_edge_index(edge_index, num_nodes)
+    K = int(csr.degree_i64().max())                                  # graph_sage.py:325 reduce_max(degree)
+    if K * num_nodes >= 2 ** 31:
+        raise ValueError("lstm_graph_sage: max in-degree {} times {} nodes reaches 2^31 padded slots, beyond the int32 "
+                         "slot index of the backward".format(K, num_nodes))
+    padded = autograd.PadRows.apply(x, csr, K, step_major, edge_index)
+    reduced = reduce_steps(padded)
+    dev_f32 = lambda t: None if t is None else ops.as_device(t, torch.float32, device=dev)     # noqa: E731
+    if autograd.needs_grad(x, self_kernel, neighbor_kernel, bias, reduced):
+        return _project_pair_autograd(x, reduced, dev_f32(self_kernel), dev_f32(neighbor_kernel), dev_f32(bias),
+                                      activation, concat, normalize)
+    return _project_pair(x, reduced, self_kernel, neighbor_kernel, bias, activation, concat, normalize)
+
+
+def lstm_graph_sage(x, edge_index, lstm, self_kernel, neighbor_kernel, bias=None, activation=None, concat=True,
+                    normalize=False, training=False):
+    """LSTM aggregator (reference graph_sage.py:290-356): every node's in-neighbours x[col], in edge order (stable by
+    edge_index[0]), zero-padded to the maximum in-degree K, go through `lstm` - any callable with the Keras
+    return_sequences=True convention, lstm([N, K, F], training=...) -> [N, K, U] - whose outputs are averaged over all K
+    steps (padded steps included, divided by K, as the reference does); then [x Ws || mean Wn] (+ b, act, l2) with
+    neighbor_kernel [U, U].  Differentiable in x, the kernels, the bias and the callable's parameters.  An edgeless graph
+    raises ValueError; so does K * N >= 2^31."""
+    return _lstm_sage(x, edge_index, lambda padded: lstm(padded, training=training).mean(dim=1), False, self_kernel,
+                      neighbor_kernel, bias, activation, concat, normalize)

@@ -13,7 +13,7 @@ from . import _ffi
 from ._ffi import (REDUCE_SUM, REDUCE_MEAN, REDUCE_MAX, ACT_NONE, ACT_RELU, POW_INV_SQRT, POW_INV,  # noqa: F401
                    HEADS_SPLIT, HEADS_BROADCAST, HEADS_REDUCE, FLAG_ALL, FLAG_UPPER, FLAG_MAPPED,
                    BERNOULLI_NONE, BERNOULLI_DROPOUT, BERNOULLI_KEEP, SAMPLE_NO_PADDING, SAMPLE_PADDING, SAMPLE_HEAD,
-                   NEG_UPPER, NEG_START)
+                   NEG_UPPER, NEG_START, PAD_ROW_MAJOR, PAD_STEP_MAJOR)
 
 _REDUCE_CODES = {"sum": REDUCE_SUM, "mean": REDUCE_MEAN, "max": REDUCE_MAX}
 
@@ -701,6 +701,47 @@ def graph_rmm(Y, B, node_graph, num_clusters, trans=False, beta=0.0, out=None):
     ldo = _float_2d(out, "out")
     _ffi.call("tfgk_graph_rmm_f32", _p(Y), ldy, _p(node_graph), N, _p(B), ldb, G, C, K, 1 if trans else 0, float(beta),
               _p(out), ldo, _stream(Y))
+    return out
+
+
+# ---- K9: padded row gather of lstm_graph_sage / convert_x_to_3d -------------------------------------------------------
+
+def pad_rows(csr, X, K, src=None, step_major=False, slot_index=False, out=None):
+    """out[r, j] = X[src[rowptr[r] + j]] for j < min(deg r, K), zeros up to K (K9, tfgk_pad_rows_f32): [R, K, D], or
+    [K, R, D] with step_major.  src is csr.col (default: neighbour rows) or csr.perm (the data rows of a segment-id CSR).
+    slot_index=True also returns, per CSR slot, its flat output row (r*K + j, or j*R + r step-major; -1 past K), which
+    needs K * R < 2^31.  X: [NX, D], column slices are fine."""
+    ldx = _float_2d(X, "X")
+    R, K, D = csr.n_rows, int(K), X.shape[1]
+    src = csr.col if src is None else src
+    _check(src, torch.int32, "src")
+    if slot_index and K * R >= 2 ** 31:
+        raise ValueError("pad_rows: K * R = {} does not fit the int32 slot index".format(K * R))
+    shape = (K, R, D) if step_major else (R, K, D)
+    if out is None:
+        out = torch.empty(shape, dtype=torch.float32, device=X.device)
+    elif tuple(out.shape) != shape or not out.is_contiguous() or out.dtype != torch.float32:
+        raise ValueError("pad_rows: out must be a contiguous float32 tensor of shape {}".format(shape))
+    slot = torch.empty((csr.nnz,), dtype=torch.int32, device=X.device) if slot_index else None
+    _ffi.call("tfgk_pad_rows_f32", _p(csr.rowptr), _p(src), R, K, PAD_STEP_MAJOR if step_major else PAD_ROW_MAJOR,
+              _p(X), ldx, X.shape[0], D, _p(out), _p(slot), _stream(X))
+    return (out, slot) if slot_index else out
+
+
+def unpad_rows(csr, G, out=None):
+    """Backward of pad_rows with src = csr.perm (row-major): out[perm[p]] = G[r, j] for j = p - rowptr[r] < K, else 0
+    (tfgk_unpad_rows_f32).  G: dense [R, K, D]; out: [csr.nnz, D], every row written."""
+    if not (torch.is_tensor(G) and G.is_cuda and G.dtype == torch.float32 and G.dim() == 3 and G.is_contiguous()):
+        raise TypeError("G must be a contiguous 3-D float32 CUDA tensor")
+    R, K, D = G.shape
+    if R != csr.n_rows:
+        raise ValueError("unpad_rows: G has {} groups, the CSR {} rows".format(R, csr.n_rows))
+    n = csr.nnz
+    if out is None:
+        out = torch.empty((n, D), dtype=torch.float32, device=G.device)
+    elif tuple(out.shape) != (n, D) or not out.is_contiguous() or out.dtype != torch.float32:
+        raise ValueError("unpad_rows: out must be a contiguous float32 tensor of shape {}".format((n, D)))
+    _ffi.call("tfgk_unpad_rows_f32", _p(csr.rowptr), _p(csr.perm), R, K, _p(G), D, _p(out), n, _stream(G))
     return out
 
 

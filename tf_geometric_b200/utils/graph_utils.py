@@ -12,7 +12,7 @@ import warnings
 import numpy as np
 import torch
 
-from .. import ops, _rng, _structure
+from .. import ops, _rng, _structure, autograd
 
 
 def _is_device(x):
@@ -499,6 +499,32 @@ def edge_train_test_split(edge_index, test_size, edge_weight=None, mode="undirec
         if not _is_device(edge_weight):
             weights = [x.cpu().numpy() for x in weights]
     return parts[0], parts[1], weights[0], weights[1]
+
+
+def convert_x_to_3d(x, source_index, k=None, pad=True):
+    """Group the rows of x by source_index into a zero-padded [num_sources, k, D] tensor (reference :215-249): row j of
+    group s is the j-th row of x with id s, in input order (stable); num_sources = max(source_index) + 1, so ids that do
+    not appear give all-zero groups.  k=None takes the largest group; a k above it keeps its width with pad=True and
+    shrinks to it with pad=False; a k below it keeps each group's first k rows.  One K9 launch (pad_rows over the
+    segment-id CSR); differentiable in x.  Tensors or numpy in, a device tensor out.  A length mismatch between x and
+    source_index, a negative id or an empty input raises ValueError."""
+    sid = ops.as_device(source_index, torch.int32).reshape(-1)
+    dev = sid.device
+    x = ops.as_device(x, torch.float32, device=dev)
+    if x.dim() != 2:
+        raise ValueError("convert_x_to_3d: x must be 2-D, got shape {}".format(tuple(x.shape)))
+    if x.shape[0] != sid.numel():
+        raise ValueError("convert_x_to_3d: x has {} rows but source_index {} entries".format(x.shape[0], sid.numel()))
+    if sid.numel() == 0:
+        raise ValueError("convert_x_to_3d: empty input")
+    lo, hi = (int(v) for v in torch.stack([sid.min(), sid.max()]).cpu())
+    if lo < 0:
+        raise ValueError("convert_x_to_3d: negative source id {}".format(lo))
+    csr = _structure.csr_for_segment_ids(sid, hi + 1)
+    largest = int(csr.degree_i64().max())
+    if k is None or (int(k) > largest and not pad):
+        k = largest
+    return autograd.PadRows.apply(x, csr, int(k), False, None)
 
 
 # samplers live in utils/sampling.py; re-exported here because the reference defines them in this module (:630-846)

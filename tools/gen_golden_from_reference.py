@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 # coding=utf-8
-"""Generate tests/golden/ref_exec_*.npz, link_exec.npz and cluster_pool_exec.npz by EXECUTING the reference's own Python (a read-only checkout of
+"""Generate tests/golden/ref_exec_*.npz, link_exec.npz, cluster_pool_exec.npz and padded_exec.npz by EXECUTING the reference's own Python (a read-only checkout of
 CrawlScript/tf_geometric named by $TFG_REFERENCE) over the numpy shims in tools/ref_shim.  The tests never need the
 reference: the resulting small fixtures are committed.  Re-run:  TFG_REFERENCE=<checkout> python tools/gen_golden_from_reference.py
 """
@@ -365,6 +365,48 @@ def main():
     # sub-GNNs are arguments of the reference functions: simple deterministic callables, restated in
     # tests/cluster_pool_ref.py.  Own RandomState, so the fixtures above are unchanged.
     cluster_pool_fixture()
+
+    # ---- convert_x_to_3d and lstm_graph_sage: utils/graph_utils.py:215-249, nn/conv/graph_sage.py:290-356 -----------
+    # tests/golden/padded_exec.npz (read by tests/test_padded_host.py and tests/test_gpu_padded.py).  Own RandomState.
+    padded_fixture()
+
+
+def padded_fixture():
+    prs = np.random.RandomState(99)
+    out = {}
+    # unsorted source ids with a gap (id 2 never appears): groups of sizes 3, 1, 0, 4, 2
+    sid = prs.permutation(np.repeat(np.array([0, 1, 3, 4], np.int32), [3, 1, 4, 2])).astype(np.int32)
+    x3 = prs.randn(sid.shape[0], 3).astype(np.float32)
+    out.update(x3d_x=x3, x3d_sid=sid)
+    for tag, kw in (("none", {}), ("k2", {"k": 2}), ("k6_pad", {"k": 6, "pad": True}), ("k6_nopad", {"k": 6, "pad": False})):
+        out["x3d_" + tag] = gu.convert_x_to_3d(T(x3), T(sid), **kw)
+    # a graph with an isolated node (0), a duplicate edge and a self loop; the LSTM is oracle.numpy_lstm behind the Keras
+    # return_sequences=True convention with a zero initial state
+    from oracle import tfg_oracle as oracle_mod
+    n, f, u = 12, 5, 4
+    ei = prs.randint(1, n, (2, 30)).astype(np.int32)
+    ei = np.concatenate([ei, ei[:, :1], np.array([[5], [5]], np.int32)], axis=1)
+    x = prs.randn(n, f).astype(np.float32)
+    w = prs.rand(ei.shape[1]).astype(np.float32)
+    lstm_k, lstm_r = glorot(prs, f, 4 * u), glorot(prs, u, 4 * u)
+    lstm_b = (prs.randn(4 * u) * 0.1).astype(np.float32)
+    np_lstm = oracle_mod.numpy_lstm(lstm_k, lstm_r, lstm_b)
+
+    def keras_lstm(inputs, training=None):
+        zeros = np.zeros((np.shape(inputs)[0], u), np.float32)
+        return T(np_lstm(np.asarray(inputs), [zeros, zeros], training)[0])
+    out.update(lstm_ei=ei, lstm_x=x, lstm_w=w, lstm_k=lstm_k, lstm_r=lstm_r, lstm_b=lstm_b)
+    for concat in (True, False):
+        ws, wn = glorot(prs, f, u), glorot(prs, u, u)
+        bias = (prs.randn(2 * u if concat else u) * 0.1).astype(np.float32)
+        tag = "concat" if concat else "sum"
+        out.update({"lstm_%s_ws" % tag: ws, "lstm_%s_wn" % tag: wn, "lstm_%s_bias" % tag: bias})
+        out["lstm_%s_relu" % tag] = sage_m.lstm_graph_sage(T(x), T(ei), keras_lstm, T(ws), T(wn), bias=T(bias),
+                                                           activation=tf.nn.relu, concat=concat)
+        out["lstm_%s_l2" % tag] = sage_m.lstm_graph_sage(T(x), T(ei), keras_lstm, T(ws), T(wn), bias=T(bias),
+                                                         concat=concat, normalize=True)
+    np.savez_compressed(os.path.join(OUT, "padded_exec.npz"), **{k: np.asarray(v) for k, v in out.items()})
+    print("wrote padded_exec.npz: {}".format(", ".join(sorted(out))))
 
 
 def golden_gnn(weight, mix):
