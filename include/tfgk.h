@@ -427,6 +427,42 @@ int tfgk_pad_rows_f32(const int64_t *rowptr, const int32_t *src, int32_t R, int3
 int tfgk_unpad_rows_f32(const int64_t *rowptr, const int32_t *perm, int32_t R, int32_t K, const float *G, int32_t D,
                         float *out, int64_t n_out, void *stream);
 
+/* ---- K10: sparse x sparse product C = A B of two CSR matrices (nn/pool/cluster_pool.py:32-34, S^T A S) --------------
+ * A is [M, K] and B [K, Ncol], both CSR (rowptr int64, col int32, val f32; columns in any order, duplicates allowed).
+ * C is CSR with ascending columns in every row, duplicates merged, every structurally present entry kept (exact zeros
+ * too).  C[i, j] is the fp32 sum of the products a_ik * b_kj in production order (A's row i left to right, then B's row k
+ * left to right): ((p_0 + p_1) + p_2) + ..., no fused multiply-add, no atomics, so the bits depend only on the inputs
+ * (not on the grid, the chunking or the tier).  One CTA per row expands the products, sorts them stably by column and
+ * sums every run.  A row with more than TFGK_SPGEMM_SHARED_PRODUCTS products is "big": its expansion goes to the caller's
+ * workspace instead of shared memory.
+ *   _plan      prod_ptr[M+1] = exclusive scan of the products per row, big_ptr[M+1] = the same over big rows only (0 for
+ *              the others); both are also copied to the host arrays.  Synchronises once.  A column id of A outside
+ *              [0, K) or of B outside [0, Ncol) returns TFGK_ERR_INDEX_OUT_OF_RANGE (nothing is read through it); a row
+ *              with 2^31 or more products TFGK_ERR_UNSUPPORTED.
+ *   _count     c_count[i] = distinct columns of C's row i for the rows [row0, row1).  Asynchronous.
+ *   _rowptr    c_rowptr[M+1] = exclusive scan of c_count; *nnz_host = nnz(C).  Synchronises once.
+ *   _fill_f32  C's columns and values of the rows [row0, row1).  Asynchronous.
+ * _count and _fill_f32 take the big-row products of their row range, big_products = big_ptr[row1] - big_ptr[row0], and a
+ * workspace of tfgk_spgemm_rows_workspace_bytes(big_products); the caller cuts the rows into ranges whose expansion fits
+ * its budget (a single row larger than the budget is a range on its own).
+ * Algorithmic bytes of _fill_f32: A (8 per row, 8 per entry) + B's row offsets (16 per A entry) + B's column and value
+ * (8 per product) + C (8 per row read, 8 per entry written). */
+#define TFGK_SPGEMM_SHARED_PRODUCTS 2048
+int tfgk_spgemm_plan_workspace_bytes(int32_t M, size_t *out_bytes);
+int tfgk_spgemm_plan(const int64_t *a_rowptr, const int32_t *a_col, int32_t M, int32_t K, const int64_t *b_rowptr,
+                     const int32_t *b_col, int32_t Ncol, int64_t *prod_ptr, int64_t *big_ptr, int64_t *prod_ptr_host,
+                     int64_t *big_ptr_host, void *workspace, size_t workspace_bytes, void *stream);
+int tfgk_spgemm_rows_workspace_bytes(int64_t big_products, size_t *out_bytes);
+int tfgk_spgemm_count(const int64_t *a_rowptr, const int32_t *a_col, const int64_t *b_rowptr, const int32_t *b_col,
+                      int32_t row0, int32_t row1, const int64_t *prod_ptr, const int64_t *big_ptr, int64_t big_products,
+                      int64_t *c_count, void *workspace, size_t workspace_bytes, void *stream);
+int tfgk_spgemm_rowptr(const int64_t *c_count, int32_t M, int64_t *c_rowptr, int64_t *nnz_host, void *workspace,
+                       size_t workspace_bytes, void *stream);
+int tfgk_spgemm_fill_f32(const int64_t *a_rowptr, const int32_t *a_col, const float *a_val, const int64_t *b_rowptr,
+                         const int32_t *b_col, const float *b_val, int32_t row0, int32_t row1, const int64_t *prod_ptr,
+                         const int64_t *big_ptr, int64_t big_products, const int64_t *c_rowptr, int32_t *c_col,
+                         float *c_val, void *workspace, size_t workspace_bytes, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -106,6 +106,13 @@ SIGNATURES = {
     "tfgk_graph_rmm_f32": [_ptr, _i64, _ptr, _i32, _ptr, _i64, _i32, _i32, _i32, _int, _f32, _ptr, _i64, _ptr],
     "tfgk_pad_rows_f32": [_ptr, _ptr, _i32, _i32, _int, _ptr, _i64, _i32, _i32, _ptr, _ptr, _ptr],
     "tfgk_unpad_rows_f32": [_ptr, _ptr, _i32, _i32, _ptr, _i32, _ptr, _i64, _ptr],
+    "tfgk_spgemm_plan_workspace_bytes": [_i32, ctypes.POINTER(_size)],
+    "tfgk_spgemm_plan": [_ptr, _ptr, _i32, _i32, _ptr, _ptr, _i32, _ptr, _ptr, _ptr, _ptr, _ptr, _size, _ptr],
+    "tfgk_spgemm_rows_workspace_bytes": [_i64, ctypes.POINTER(_size)],
+    "tfgk_spgemm_count": [_ptr, _ptr, _ptr, _ptr, _i32, _i32, _ptr, _ptr, _i64, _ptr, _ptr, _size, _ptr],
+    "tfgk_spgemm_rowptr": [_ptr, _i32, _ptr, ctypes.POINTER(_i64), _ptr, _size, _ptr],
+    "tfgk_spgemm_fill_f32": [_ptr, _ptr, _ptr, _ptr, _ptr, _ptr, _i32, _i32, _ptr, _ptr, _i64, _ptr, _ptr, _ptr, _ptr, _size,
+                             _ptr],
 }
 
 

@@ -361,6 +361,38 @@ class SegmentReduce(torch.autograd.Function):
         return ops.permute(g / n_selected, ids) * selected, None, None, None
 
 
+def segment_softmax_forward(data, ids, num_segments):
+    """exp(d - max_seg) / (sum_seg + 1e-8) per segment of a plain id vector, [E] or [E, C]: K3's segment softmax over the
+    segment CSR, in and out of its order by permutation."""
+    csr = _structure.csr_for_segment_ids(ids, int(num_segments))
+    soft_csr = ops.segment_softmax_csr(csr, ops.permute(data.contiguous(), csr.perm))
+    return ops.permute(soft_csr, csr.perm, inverse=True)
+
+
+class SegmentSoftmax(torch.autograd.Function):
+    """segment_softmax (nn/kernel/segment.py:26-33) differentiable w.r.t. the scores.  The forward is the kernel of the
+    non-differentiable path (same bits).  Backward: ds = a * (g - segsum(a * g)[seg]), the segment sums through the
+    segment CSR (K1 gathering by perm, no atomics).  Like tfgk_gat_softmax_bwd_f32 it drops the 1e-8 of the denominator,
+    whose derivative is about 1e-8 relative."""
+
+    @staticmethod
+    def forward(ctx, data, ids, num_segments):
+        a = segment_softmax_forward(data.detach(), ids, num_segments)
+        ctx.ids, ctx.num_segments = ids, int(num_segments)
+        ctx.save_for_backward(a)
+        return a
+
+    @staticmethod
+    def backward(ctx, grad_a):
+        (a,) = ctx.saved_tensors
+        csr = _structure.csr_for_segment_ids(ctx.ids, ctx.num_segments)
+        ag = a * grad_a
+        flat = ag if ag.dim() == 2 else ag.unsqueeze(1)
+        seg = ops.spmm(csr, None, flat.contiguous(), reduce="sum", col=csr.perm)
+        back = ops.permute(seg, ctx.ids)
+        return a * (grad_a - (back if ag.dim() == 2 else back.squeeze(1))), None, None
+
+
 class TakeRows(torch.autograd.Function):
     """data[index] (tf.gather along axis 0) through the gather kernel; backward = segment sum of the upstream rows by
     index (a deterministic scatter-add on the CSR kernel)."""
@@ -612,6 +644,21 @@ class AssignGram(torch.autograd.Function):
         g = grad_m.contiguous()
         out = ops.graph_rmm(s, g, lay.node_graph, lay.num_clusters)
         return ops.graph_rmm(s, g, lay.node_graph, lay.num_clusters, trans=True, beta=1.0, out=out), None
+
+
+class RefusedPooledWeights(torch.autograd.Function):
+    """The pooled edge weights of cluster_pool (the entries of S^T A S) as a function of A's and S's values.  The forward
+    returns the weights K10 computed; their backward is not built, so it raises instead of returning no gradient."""
+
+    @staticmethod
+    def forward(ctx, pooled_weight, edge_weight, assign_edge_weight):
+        return pooled_weight
+
+    @staticmethod
+    def backward(ctx, grad):
+        raise RuntimeError("cluster_pool: the gradient of the pooled edge weights with respect to edge_weight and "
+                           "assign_edge_weight is not implemented; detach those weights (ASAP detaches its assignment) or "
+                           "keep the pooled weights out of the loss")
 
 
 def needs_grad(*tensors):

@@ -8,5 +8,6 @@ from .conv.appnp import APPNP
 from .conv.propagation import SGC, SSGC, TAGCN, GIN, LEConv, ChebyNet
 from .pool.pool import MeanPool, SumPool, MaxPool, MinPool, Set2Set, SAGPool, SortPool
 from .pool.cluster_pool import DiffPool, MinCutPool
+from .pool.asap import ASAP
 from .sampling import DropEdge
 from .kernel import MapReduceGNN

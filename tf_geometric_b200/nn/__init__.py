@@ -20,6 +20,8 @@ _EXPORTS = {
     pool.score_pool: ("sag_pool", "sort_pool"),
     pool.diff_pool: ("diff_pool", "diff_pool_coarsen"),
     pool.min_cut_pool: ("min_cut_pool", "min_cut_pool_coarsen", "min_cut_pool_compute_losses"),
+    pool.cluster_pool: ("cluster_pool",),
+    pool.asap: ("asap",),
     sampling.drop_edge: ("drop_edge",),
     link.predict_edge: ("predict_edge",),
 }

@@ -3,16 +3,17 @@
 CSR kernels (tfgk_segment_softmax_f32, tfgk_segment_count_i32)."""
 import torch
 
-from ... import ops, _structure
+from ... import ops, autograd
 
 
 def segment_softmax(data, segment_ids, num_segments):
-    """exp(d - max_seg) / (sum_seg + 1e-8) per segment (reference segment.py:26-33).  `data` is [E] or [E, C]."""
+    """exp(d - max_seg) / (sum_seg + 1e-8) per segment (reference segment.py:26-33).  `data` is [E] or [E, C];
+    differentiable w.r.t. `data` (autograd.SegmentSoftmax) with the same forward bits."""
     segment_ids = ops.as_device(segment_ids, torch.int32)
     data = ops.as_device(data, torch.float32, device=segment_ids.device)
-    csr = _structure.csr_for_segment_ids(segment_ids, int(num_segments))
-    soft_csr = ops.segment_softmax_csr(csr, ops.permute(data, csr.perm))
-    return ops.permute(soft_csr, csr.perm, inverse=True)
+    if autograd.needs_grad(data):
+        return autograd.SegmentSoftmax.apply(data, segment_ids, int(num_segments))
+    return autograd.segment_softmax_forward(data, segment_ids, num_segments)
 
 
 def segment_count(index, num_segments=None):

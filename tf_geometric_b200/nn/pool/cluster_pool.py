@@ -1,6 +1,11 @@
 # coding=utf-8
-"""Shared coarsening step of DiffPool and MinCutPool (reference nn/pool/cluster_pool.py), restricted to what both use: a
-dense [N, C] assignment in which every node belongs to the C clusters of its own graph.
+"""cluster_pool with a sparse assignment (reference nn/pool/cluster_pool.py:9-44), and the shared coarsening step of DiffPool
+and MinCutPool, restricted to what both use: a dense [N, C] assignment in which every node belongs to the C clusters of
+its own graph.
+
+cluster_pool computes the reference's S^T A S without the dense N x N adjacency: T = S^T A, then P = T S, two launches of
+K10 (csrc/spgemm.cu, the reference's left-to-right association).  Its pooled edges are P's entries != 0 in row-major
+order, which is the order of the reference's tf.where over the dense [K, K] matrix.
 
 The reference builds the [G*C, N] assignment as a sparse matrix, densifies the N x N adjacency and multiplies
 S^T A S over [G*C]^2.  Here the pooled blocks are computed per graph by K8 (csrc/cluster_pool.cu): P = S_g^T X_g and
@@ -13,6 +18,60 @@ import weakref
 import torch
 
 from ... import ops, autograd, _structure
+from ...sparse import SparseMatrix
+
+
+def _weights(weight, n, dev):
+    if weight is None:
+        return torch.ones((n,), dtype=torch.float32, device=dev)
+    return ops.as_device(weight, torch.float32, device=dev).reshape(-1)
+
+
+def cluster_pool(x, edge_index, edge_weight, assign_edge_index, assign_edge_weight, num_clusters, num_nodes=None):
+    """
+    Coarsen a graph by a sparse assignment of nodes to clusters (reference nn/pool/cluster_pool.py:9-44).
+
+    :param x: [num_nodes, num_features] or None
+    :param edge_index: [2, num_edges]; edge_weight: [num_edges] or None (ones)
+    :param assign_edge_index: [2, num_assignments] as [node, cluster]: entry e puts node assign_edge_index[0, e] in cluster
+        assign_edge_index[1, e] with weight assign_edge_weight[e] (None: ones).  Duplicate entries, in the assignment or in
+        the edges, add up.
+    :param num_clusters: K
+    :param num_nodes: required when x is None
+    :return: [pooled_x (S^T x, or None), pooled_edge_index int32 [2, P], pooled_edge_weight [P]]: the entries != 0 of
+        S^T A S (NaN kept) in row-major order.  pooled_x is differentiable in x and assign_edge_weight; the pooled edge
+        weights have no gradient with respect to edge_weight or assign_edge_weight, and a backward that reaches them while
+        either requires grad raises RuntimeError.
+    """
+    if num_nodes is None:
+        if x is None:
+            raise Exception("Please provide num_nodes if x is None")
+        num_nodes = x.shape[0]
+    N, K = int(num_nodes), int(num_clusters)
+    ei = ops.as_device(edge_index, torch.int32).reshape(2, -1)
+    dev = ei.device
+    aei = ops.as_device(assign_edge_index, torch.int32, device=dev).reshape(2, -1)
+    w = _weights(edge_weight, ei.shape[1], dev)
+    aw = _weights(assign_edge_weight, aei.shape[1], dev)
+    node, cluster = aei[0].contiguous(), aei[1].contiguous()
+    a_csr, _ = _structure.csr_for_edge_index(ei, N)
+    s_csr = ops.csr_build(node, cluster, N, K)                 # S by node, stable: the assignment order within a node
+    st_csr = ops.csr_build(cluster, node, K, N)                # S^T by cluster
+    awd = aw.detach()
+    t = ops.spgemm(st_csr.rowptr, st_csr.col, ops.permute(awd, st_csr.perm), a_csr.rowptr, a_csr.col,
+                   ops.permute(w.detach(), a_csr.perm), N)
+    rowptr, col, val = ops.spgemm(*t, s_csr.rowptr, s_csr.col, ops.permute(awd, s_csr.perm), K)
+    keep = ops.select_flagged((val != 0).to(torch.int32))      # != 0 keeps NaN, like convert_dense_adj_to_edge
+    rows = torch.repeat_interleave(torch.arange(K, dtype=torch.int32, device=dev), rowptr[1:] - rowptr[:-1])
+    pooled_edge_index = torch.stack([ops.gather_i32(rows, keep), ops.gather_i32(col, keep)])
+    pooled_edge_weight = ops.permute(val, keep)
+    if autograd.needs_grad(w, aw):
+        pooled_edge_weight = autograd.RefusedPooledWeights.apply(pooled_edge_weight, w, aw)
+    pooled_x = None
+    if x is not None:
+        st = SparseMatrix(torch.stack([cluster, node]), aw, [K, N], _csr=st_csr)
+        pooled_x = st @ ops.as_device(x, torch.float32, device=dev)
+    return pooled_x, pooled_edge_index, pooled_edge_weight
 
 
 class ClusterLayout(object):

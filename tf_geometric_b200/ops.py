@@ -745,6 +745,66 @@ def unpad_rows(csr, G, out=None):
     return out
 
 
+# ---- K10: CSR x CSR product -----------------------------------------------------------------------------------------
+
+SPGEMM_BUDGET = 1 << 24    # products expanded per launch; the big rows among them need 24 bytes of workspace each
+
+
+def _spgemm_chunks(prod_ptr, budget):
+    """Row ranges [r0, r1) whose products fit `budget` (a row with more products is a range on its own)."""
+    M = len(prod_ptr) - 1
+    chunks, r0 = [], 0
+    while r0 < M:
+        r1 = int(np.searchsorted(prod_ptr, prod_ptr[r0] + budget, side="right")) - 1
+        r1 = min(max(r1, r0 + 1), M)
+        chunks.append((r0, r1))
+        r0 = r1
+    return chunks
+
+
+def spgemm(a_rowptr, a_col, a_val, b_rowptr, b_col, b_val, n_cols, budget=SPGEMM_BUDGET):
+    """C = A B for two CSR matrices (K10, tfgk_spgemm_*): A [M, K] and B [K, n_cols] as (rowptr int64, col int32,
+    val float32).  Returns C's (rowptr int64 [M+1], col int32, val float32) with ascending columns per row; every entry is
+    the fp32 sum of its products in Gustavson order, so the bits do not depend on `budget`, which bounds the products
+    expanded per launch (and with it the workspace of the rows too large for shared memory)."""
+    for t, n, dt in ((a_rowptr, "a_rowptr", torch.int64), (a_col, "a_col", torch.int32), (a_val, "a_val", torch.float32),
+                     (b_rowptr, "b_rowptr", torch.int64), (b_col, "b_col", torch.int32), (b_val, "b_val", torch.float32)):
+        _check(t, dt, n)
+    if a_col.numel() != a_val.numel() or b_col.numel() != b_val.numel():
+        raise ValueError("spgemm: column and value arrays differ in length")
+    M, K = a_rowptr.numel() - 1, b_rowptr.numel() - 1
+    dev, st = a_rowptr.device, _stream(a_rowptr)
+    need = ctypes.c_size_t()
+    _ffi.call("tfgk_spgemm_plan_workspace_bytes", M, ctypes.byref(need))
+    ws = torch.empty((need.value,), dtype=torch.uint8, device=dev)
+    prod_ptr = torch.empty((M + 1,), dtype=torch.int64, device=dev)
+    big_ptr = torch.empty((M + 1,), dtype=torch.int64, device=dev)
+    prod_host = np.empty((M + 1,), np.int64)
+    big_host = np.empty((M + 1,), np.int64)
+    _ffi.call("tfgk_spgemm_plan", _p(a_rowptr), _p(a_col), M, K, _p(b_rowptr), _p(b_col), int(n_cols), _p(prod_ptr),
+              _p(big_ptr), prod_host.ctypes.data_as(ctypes.c_void_p), big_host.ctypes.data_as(ctypes.c_void_p), _p(ws),
+              need.value, st)
+    chunks = _spgemm_chunks(prod_host, max(int(budget), 0))
+    big = [int(big_host[r1] - big_host[r0]) for r0, r1 in chunks]
+    rows_ws = ctypes.c_size_t()
+    _ffi.call("tfgk_spgemm_rows_workspace_bytes", max(big, default=0), ctypes.byref(rows_ws))
+    rws = torch.empty((max(rows_ws.value, 1),), dtype=torch.uint8, device=dev)
+    c_count = torch.empty((max(M, 1),), dtype=torch.int64, device=dev)
+    for (r0, r1), nb in zip(chunks, big):
+        _ffi.call("tfgk_spgemm_count", _p(a_rowptr), _p(a_col), _p(b_rowptr), _p(b_col), r0, r1, _p(prod_ptr),
+                  _p(big_ptr), nb, _p(c_count), _p(rws), rows_ws.value, st)
+    c_rowptr = torch.empty((M + 1,), dtype=torch.int64, device=dev)
+    nnz = ctypes.c_int64()
+    _ffi.call("tfgk_spgemm_rowptr", _p(c_count), M, _p(c_rowptr), ctypes.byref(nnz), _p(ws), need.value, st)
+    c_col = torch.empty((nnz.value,), dtype=torch.int32, device=dev)
+    c_val = torch.empty((nnz.value,), dtype=torch.float32, device=dev)
+    if nnz.value:
+        for (r0, r1), nb in zip(chunks, big):
+            _ffi.call("tfgk_spgemm_fill_f32", _p(a_rowptr), _p(a_col), _p(a_val), _p(b_rowptr), _p(b_col), _p(b_val), r0,
+                      r1, _p(prod_ptr), _p(big_ptr), nb, _p(c_rowptr), _p(c_col), _p(c_val), _p(rws), rows_ws.value, st)
+    return c_rowptr, c_col, c_val
+
+
 # ---- K4 ----------------------------------------------------------------------------------------------------------
 
 def gemm(a, b, bias=None, act=ACT_NONE, trans_a=False, trans_b=False, beta=0.0, out=None):

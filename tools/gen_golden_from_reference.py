@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 # coding=utf-8
-"""Generate tests/golden/ref_exec_*.npz, link_exec.npz, cluster_pool_exec.npz and padded_exec.npz by EXECUTING the reference's own Python (a read-only checkout of
+"""Generate tests/golden/ref_exec_*.npz, link_exec.npz, cluster_pool_exec.npz, padded_exec.npz and asap_exec.npz by EXECUTING the reference's own Python (a read-only checkout of
 CrawlScript/tf_geometric named by $TFG_REFERENCE) over the numpy shims in tools/ref_shim.  The tests never need the
 reference: the resulting small fixtures are committed.  Re-run:  TFG_REFERENCE=<checkout> python tools/gen_golden_from_reference.py
 """
@@ -369,6 +369,70 @@ def main():
     # ---- convert_x_to_3d and lstm_graph_sage: utils/graph_utils.py:215-249, nn/conv/graph_sage.py:290-356 -----------
     # tests/golden/padded_exec.npz (read by tests/test_padded_host.py and tests/test_gpu_padded.py).  Own RandomState.
     padded_fixture()
+
+    # ---- cluster_pool with a sparse assignment and ASAP: nn/pool/cluster_pool.py, nn/pool/asap.py ------------------------
+    # tests/golden/asap_exec.npz (read by tests/test_asap_host.py and tests/test_gpu_asap.py).  Own RandomState.
+    asap_fixture()
+
+
+def asap_fixture():
+    cp_m = importlib.import_module("tf_geometric.nn.pool.cluster_pool")
+    sys.modules["tf_geometric.nn"].max_pool = pool_m.max_pool           # asap.py: from tf_geometric.nn import max_pool
+    asap_m = importlib.import_module("tf_geometric.nn.pool.asap")
+    ars = np.random.RandomState(321)
+    out = {}
+    # cluster_pool, assignment [node, cluster]: duplicates in S ((2, 1) twice) and in A ((2, 3) twice), node 6 in no
+    # cluster, cluster 3 empty, a self loop (3, 3), and the zero-weight edge (3, 5) whose pooled entry (1, 2) is exactly 0
+    ei = np.array([[0, 1, 2, 2, 3, 3, 4, 5, 1], [1, 2, 3, 3, 3, 5, 0, 4, 0]], np.int32)
+    w = np.array([1.0, 0.5, 2.0, 2.0, 1.5, 0.0, 0.75, 1.25, -1.0], np.float32)
+    aei = np.array([[0, 1, 2, 2, 3, 4, 5, 0], [0, 0, 1, 1, 1, 2, 2, 2]], np.int32)
+    aw = ars.uniform(0.1, 2.0, aei.shape[1]).astype(np.float32)
+    x = ars.randn(7, 3).astype(np.float32)
+    out.update(cp_ei=ei, cp_w=w, cp_aei=aei, cp_aw=aw, cp_x=x)
+    for tag, ew, aew in (("w", T(w), T(aw)), ("none", None, None)):
+        px, pei, pw = cp_m.cluster_pool(T(x), T(ei), ew, T(aei), aew, 4)
+        out.update({"cp_%s_%s" % (tag, k): v for k, v in zip(("x", "ei", "w"), (px, pei, pw))})
+
+    # asap.py with its two call sites read the one way that runs (DESIGN.md section 5 (9)):
+    #   adapter 1: gcn(x, edge_index, edge_weight, kernel, bias) (asap.py:54) is the edge-list GCN, as layers/conv/gcn.py
+    #              reads [x, edge_index, edge_weight] inputs;
+    #   adapter 2: the assignment stacked as [cluster, node] (asap.py:107-115) reaches cluster_pool as [node, cluster].
+    asap_m.gcn = lambda x_, ei_, ew_, k_, b_=None, cache=None: gcn_m.gcn(
+        x_, tfs.SparseMatrix(ei_, ew_, [np.shape(x_)[0]] * 2), k_, b_, cache=cache)
+
+    def cluster_pool_node_cluster(x_, ei_, ew_, aei_, aew_, k_, num_nodes=None):
+        return cp_m.cluster_pool(x_, ei_, ew_, T(np.asarray(aei_)[::-1].copy()), aew_, k_, num_nodes=num_nodes)
+    asap_m.cluster_pool = cluster_pool_node_cluster
+
+    # graphs of 7, 1 (edgeless), 9 and 5 nodes, relabelled so that node_graph_index is unsorted; duplicates, self loops
+    sizes, f = [7, 1, 9, 5], 4
+    rows, cols, base = [], [], 0
+    for size in sizes:
+        if size > 1:
+            e = ars.randint(0, size, (2, 3 * size))
+            rows += list(base + e[0]) + [base + e[0, 0]]
+            cols += list(base + e[1]) + [base + e[1, 0]]
+        base += size
+    n = base
+    perm = ars.permutation(n)
+    inv = np.empty_like(perm)
+    inv[perm] = np.arange(n)
+    ei = inv[np.array([rows, cols])].astype(np.int32)
+    gi = np.repeat(np.arange(len(sizes)), sizes)[perm].astype(np.int32)
+    w = ars.uniform(0.5, 1.5, ei.shape[1]).astype(np.float32)
+    x = ars.randn(n, f).astype(np.float32)
+    names = ("attention_gcn_kernel", "attention_gcn_bias", "attention_query_kernel", "attention_query_bias",
+             "attention_score_kernel", "attention_score_bias", "le_conv_self_kernel", "le_conv_self_bias",
+             "le_conv_aggr_self_kernel", "le_conv_aggr_self_bias", "le_conv_aggr_neighbor_kernel")
+    shapes = ((f, f), (f,), (f, f), (f,), (2 * f, 1), (1,), (f, 1), (1,), (f, 1), (1,), (f, 1))
+    params = [glorot(ars, *s) if len(s) == 2 else (ars.randn(*s) * 0.1).astype(np.float32) for s in shapes]
+    out.update(asap_ei=ei, asap_w=w, asap_x=x, asap_gi=gi, **{"asap_p_" + k: v for k, v in zip(names, params)})
+    for tag, ew, kw in (("r50_w", T(w), {"ratio": 0.5}), ("r50_none", None, {"ratio": 0.5}), ("k2_w", T(w), {"k": 2}),
+                        ("k3_none", None, {"k": 3})):
+        res = asap_m.asap(T(x), T(ei), ew, T(gi), *[T(p) for p in params], None, training=False, **kw)
+        out.update({"asap_%s_%s" % (tag, k): v for k, v in zip(("x", "ei", "w", "gi"), res)})
+    np.savez_compressed(os.path.join(OUT, "asap_exec.npz"), **{k: np.asarray(v) for k, v in out.items()})
+    print("wrote asap_exec.npz: {}".format(", ".join(sorted(out))))
 
 
 def padded_fixture():

@@ -213,6 +213,9 @@ def build_tensorflow():
         e = np.exp(x - np.max(x, axis=axis, keepdims=True)).astype(np.float32)
         return T((e / np.sum(e, axis=axis, keepdims=True, dtype=np.float32)).astype(np.float32))
     nn.softmax = softmax
+    nn.leaky_relu = lambda x, alpha=0.2: T(np.where(np.asarray(x) > 0, np.asarray(x),
+                                                    np.float32(alpha) * np.asarray(x)).astype(np.float32))
+    nn.sigmoid = lambda x: T((1 / (1 + np.exp(-np.asarray(x, np.float32)))).astype(np.float32))
     nn.__getattr__ = lambda name: _unsupported("tf.nn." + name)
     tf.nn = nn
 
