@@ -183,8 +183,9 @@ int tfgk_gemm_f32(const float *A, int64_t lda, int transA, const float *B, int64
  * A_parts[i]: with the other ranks' buffers mapped through tfgk_peer_open this is the fused all-gather -> GEMM of the
  * partitioned path (rows are pulled over NVLink tile by tile while earlier tiles are multiplied); the walk starts at
  * part first_part so that concurrent ranks read from different peers.  max_ctas > 0 bounds the grid (to share the GPU
- * with a kernel on another stream).  Returns TFGK_ERR_UNSUPPORTED when the shape does not qualify (K > 512, unaligned A,
- * W too large for shared memory): the caller then uses tfgk_gemm_f32 per block. */
+ * with a kernel on another stream).  Returns TFGK_ERR_UNSUPPORTED when the shape does not qualify (K > 184, where W no
+ * longer fits in shared memory; lda not a multiple of 4 or A not 16-byte aligned; ncols > 128): the caller then uses
+ * tfgk_gemm_f32 per block. */
 typedef struct tfgk_proj_block {
     const float *B; int64_t ldb;       /* [K, ncols] row-major weights ([ncols, K] row-major when transB != 0) */
     int32_t ncols;

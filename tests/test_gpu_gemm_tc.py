@@ -19,8 +19,8 @@ def dev(a):
 
 
 @pytest.mark.parametrize("m,n,k", [
-    (128, 128, 32), (128, 16, 8), (4096, 128, 100), (5000, 128, 128), (2708, 16, 512), (3000, 7, 16),
-    (1000, 64, 20), (777, 200, 333), (130000, 128, 100), (300, 256, 64), (129, 48, 5)])
+    (128, 128, 32), (128, 16, 8), (4096, 128, 100), (5000, 128, 128), (2708, 16, 184), (3000, 7, 16),
+    (1000, 64, 20), (777, 200, 160), (130000, 128, 100), (300, 256, 64), (129, 48, 5)])
 def test_gemm_tc_matches_float64(m, n, k):
     rs = np.random.RandomState(m + n + k)
     a = rs.randn(m, k).astype(np.float32)
@@ -32,6 +32,27 @@ def test_gemm_tc_matches_float64(m, n, k):
     assert err < 5e-6, "3xTF32 relative error {:.2e} (single-pass TF32 would be ~1e-3)".format(err)
     got = ops.gemm(dev(a), dev(b), bias=dev(bias), act=ops.ACT_RELU).cpu().numpy()
     assert_close(got, np.maximum(want + bias, 0), rtol=1e-5, atol_scale=5e-6, what="tc gemm + bias + relu")
+
+
+@pytest.mark.parametrize("m,n,k", [(2708, 16, 512), (777, 200, 333)])
+def test_gemm_wide_k_runs_simt_and_matches_float64(monkeypatch, m, n, k):
+    """K above ops.GEMM_PROJ_MAX_K: W (hi | lo) does not fit in shared memory next to the A ring, so the exact-fp32 SIMT
+    kernel runs (the same bits as with the tensor-core route switched off)."""
+    assert k > ops.GEMM_PROJ_MAX_K
+    rs = np.random.RandomState(m + n + k)
+    a = rs.randn(m, k).astype(np.float32)
+    b = (rs.randn(k, n) / np.sqrt(k)).astype(np.float32)
+    bias = rs.randn(n).astype(np.float32)
+    want = a.astype(np.float64) @ b.astype(np.float64)
+    got = ops.gemm(dev(a), dev(b))
+    with monkeypatch.context() as mp:
+        mp.setenv("TFGK_GEMM_TC", "0")
+        assert torch.equal(got, ops.gemm(dev(a), dev(b)))
+    got = got.cpu().numpy()
+    err = np.abs(got - want).max() / np.abs(want).max()
+    assert err < 5e-6, "SIMT relative error {:.2e}".format(err)
+    got = ops.gemm(dev(a), dev(b), bias=dev(bias), act=ops.ACT_RELU).cpu().numpy()
+    assert_close(got, np.maximum(want + bias, 0), rtol=1e-5, atol_scale=5e-6, what="SIMT gemm + bias + relu")
 
 
 def test_gemm_tc_strided_operands_and_output_slices():

@@ -7,11 +7,12 @@
 // replaces x@W at nn/conv/gcn.py:272 and the three projections x@Wq, x@Wk, x@W of nn/conv/gat.py:52,61,70, which would
 // otherwise be three launches that each re-read x.  tfgk_gemm_f32 sends every tall projection here as well.
 //
-// Arithmetic: 3xTF32.  a = a_hi + a_lo and w = w_hi + w_lo with x_hi = cvt.rna.tf32(x), and per k-step of 8
+// Arithmetic: 3xTF32.  a = a_hi + a_lo and w = w_hi + w_lo with x_hi = rna_tf32(x) kept finite, and per k-step of 8
 //     acc += a_lo * w_hi;  acc += a_hi * w_lo;  acc += a_hi * w_hi        (wgmma.m64n128k8.f32.tf32.tf32, fp32 accumulators)
-// which keeps the error at the fp32 level (tests/test_gpu_gemm_tc.py: < 5e-6 relative up to K = 512), where a single TF32
-// pass is off by ~1e-3.  The result of a row depends only on that row, the weights and K: the same bits whatever the
-// number of blocks, the grid or the part layout of A.
+// which keeps the error at the fp32 level, where a single TF32 pass is off by ~1e-3: every entry is within
+// (K 2^-23 + 2^-19) S + 2^-23 |ref| of float64, S = |A| |W| + |bias| (tests/test_gpu_gemm_contract.py, every K up to the
+// limit of 184 set by the shared-memory plan below).  The result of a row depends only on that row, the weights and K: the
+// same bits whatever the number of blocks, the grid or the part layout of A.
 //
 // Layout (one CTA = 128 output rows x one column block of <= 128 columns, 256 threads = two warpgroups of 64 rows):
 //   * W_b (hi | lo) resident in shared memory for the whole kernel, K rounded up to 8, in the K-major no-swizzle layout of
@@ -53,7 +54,8 @@ struct Params {
     float *C[kMaxBlocks]; int64_t ldc[kMaxBlocks];
 };
 
-// shared memory: W hi | W lo | bias | ring of A stages
+// shared memory: W hi | W lo | bias | ring of A stages.  With 1024 bytes of W per K (rounded up to 8), 18 432 per A stage
+// and 227 KB in all: 4 stages for K <= 152, 3 for K 153..168, 2 for K 169..184, none (unsupported) from K = 185 on
 struct Plan {
     uint32_t kpad, b_bytes, ring_off, stages, total;
     explicit Plan(int K) {
@@ -84,8 +86,15 @@ __device__ __forceinline__ uint64_t make_desc(uint32_t saddr, uint32_t sbo_bytes
     return d;                                          // base offset 0, layout type 0 (no swizzle)
 }
 
+// hi = rna_tf32(a) (round half away from zero to 10 mantissa bits: add half a TF32 ulp to the magnitude bits, truncate),
+// of a first clamped to +-0x7F7FEFFF, the largest magnitude that rounds to a finite TF32 number (2 - 2^-10) 2^127.  Without
+// the clamp |a| >= (2 - 2^-11) 2^127 would round to inf and a = +-inf would give lo = inf - inf = NaN.  With it,
+// lo = a - hi is finite for every finite a, +-inf for a = +-inf and NaN for a NaN (fmaxf takes the number), so the
+// products give the IEEE result.  Every a below the threshold gets the bits of cvt.rna.tf32.f32, in as many instructions
+// (two FMNMX instead of the inf test and select that cvt.rna, or .satfinite on top of it, compiles to).
 __device__ __forceinline__ void split_tf32(float a, uint32_t &hi, uint32_t &lo) {
-    asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(hi) : "f"(a));
+    const float lim = __uint_as_float(0x7F7FEFFFu);
+    hi = (__float_as_uint(fminf(fmaxf(a, -lim), lim)) + 0x1000u) & 0xFFFFE000u;
     lo = __float_as_uint(a - __uint_as_float(hi));
 }
 
@@ -289,7 +298,8 @@ extern "C" int tfgk_gemm_proj_f32(const float *const *A_parts, int32_t n_parts, 
     if (n_parts > 1)
         TFGK_CHECK_ARG(part_rows > 0 && part_rows % proj::BM == 0 && (int64_t)n_parts * part_rows >= M,
                        "gemm_proj: part_rows=%lld must be a positive multiple of %d covering M=%d", (long long)part_rows, proj::BM, M);
-    // K <= 512: tensor-core accumulation truncates, so the error grows with K; up to K = 512 it stays below 5e-6 relative
+    // K > 512 never fits (Plan below stops at K = 184, ops.GEMM_PROJ_MAX_K); refusing it here keeps Plan's byte counts
+    // far from overflowing 32 bits
     if (K > 512 || (lda % 4) != 0 || lda < K) return TFGK_ERR_UNSUPPORTED;
     proj::Params p;
     for (int i = 0; i < proj::kMaxParts; ++i) {

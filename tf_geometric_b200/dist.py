@@ -199,7 +199,7 @@ class PartitionedGraph(object):
         widths = [sum(int(w.shape[1]) for w, _, _ in g) for g in groups]
         fused_ok = x_local.is_cuda and x_local.shape[1] % 4 == 0 and sum(widths) % 4 == 0        # 16-byte rows for the pulls
         if self.exchange == "p2p_fused":
-            fused_ok = fused_ok and x_local.shape[1] <= 512                                         # tfgk_gemm_proj_f32 limit
+            fused_ok = fused_ok and x_local.shape[1] <= ops.GEMM_PROJ_MAX_K                         # tfgk_gemm_proj_f32 limit
         if p.world_size == 1 or self.exchange not in ("p2p", "p2p_fused") or not fused_ok \
                 or self._row_exchange(x_local.shape[1], dev) is None:
             send = torch.empty((p.block, sum(widths)), dtype=torch.float32, device=dev)

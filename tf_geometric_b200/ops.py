@@ -807,6 +807,10 @@ def spgemm(a_rowptr, a_col, a_val, b_rowptr, b_col, b_val, n_cols, budget=SPGEMM
 
 # ---- K4 ----------------------------------------------------------------------------------------------------------
 
+# Largest K that tfgk_gemm_proj_f32 (the tensor-core kernel) accepts: W (hi | lo, 1024 bytes per K rounded up to 8) has to
+# fit in shared memory next to at least two A stages.  Larger K goes to the exact-fp32 SIMT kernel.
+GEMM_PROJ_MAX_K = 184
+
 def gemm(a, b, bias=None, act=ACT_NONE, trans_a=False, trans_b=False, beta=0.0, out=None):
     """act(op(a) @ op(b) + bias + beta*out) in fp32."""
     for t, n in ((a, "a"), (b, "b")):
