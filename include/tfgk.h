@@ -44,6 +44,8 @@ enum tfgk_heads_mode { TFGK_HEADS_SPLIT = 0, TFGK_HEADS_BROADCAST = 1, TFGK_HEAD
 enum tfgk_edge_flag { TFGK_FLAG_ALL = 0, TFGK_FLAG_UPPER = 1, TFGK_FLAG_MAPPED = 2 };
 enum tfgk_bernoulli { TFGK_BERNOULLI_NONE = 0, TFGK_BERNOULLI_DROPOUT = 1, TFGK_BERNOULLI_KEEP = 2 };
 enum tfgk_sample_padding { TFGK_SAMPLE_NO_PADDING = 0, TFGK_SAMPLE_PADDING = 1, TFGK_SAMPLE_HEAD = 2 };
+/* element type of a bf16-capable buffer; bf16 data is passed as its 16-bit patterns (uint16_t) */
+enum tfgk_dtype { TFGK_DTYPE_F32 = 0, TFGK_DTYPE_BF16 = 1 };
 
 int tfgk_version(void);
 const char *tfgk_last_error(void);
@@ -145,6 +147,19 @@ int tfgk_spmm_f32(const int64_t *rowptr, const int32_t *col, const float *w,
                   float alpha, const float *addend, int64_t ld_addend, float beta,
                   const float *bias, int act,
                   float *out, int64_t ldo, const tfgk_plan *plan, void *stream);
+/* The same with bf16 rows h (w, addend, bias, the accumulators and out stay fp32).  Bf16 -> fp32 widening is exact, and
+ * the kernels widen each element and run the fp32 arithmetic in the same order with the same plan, so the output is
+ * bit-identical to tfgk_spmm_f32 over the widened table with the same leading dimension and alignment in elements.  Rows
+ * with D % 8 == 0, 32 <= D <= 256 and 16-byte aligned rows take the TMA ring (2 D bytes per row); D % 4 == 0 up to 512
+ * with 8-byte aligned rows a cp.async ring; both use the plan, as tfgk_spmm_f32 does for 16-byte aligned fp32 rows.  Any
+ * other D or leading dimension takes a scalar path without the plan (hub rows summed strictly in order), as in fp32: a
+ * dense widened copy of such a view would take the plan, so callers comparing against one pass a dense copy of h
+ * (ops.spmm does when the plan has hub rows).  Algorithmic bytes: E*(2*D + 4 [+4 weighted]) + N*(4*D + 8). */
+int tfgk_spmm_bf16(const int64_t *rowptr, const int32_t *col, const float *w,
+                   const uint16_t *h, int64_t ldh, int32_t n_dst, int32_t D, int reduce,
+                   float alpha, const float *addend, int64_t ld_addend, float beta,
+                   const float *bias, int act,
+                   float *out, int64_t ldo, const tfgk_plan *plan, void *stream);
 
 /* ---- K3: edge softmax and fused GAT ------------------------------------------------------------------------- */
 
@@ -165,6 +180,18 @@ int tfgk_gat_fused_f32(const int64_t *rowptr, const int32_t *col,
                        int32_t N, int32_t H, int32_t dqk, int32_t dv, float scale, int split_value_heads,
                        const float *bias, int act, float *att, int write_att, float *out, int64_t ldo,
                        const tfgk_plan *plan, void *stream);
+/* The same with bf16 K and V (Q, bias, att and out fp32), inference only: write_att != 0 returns TFGK_ERR_UNSUPPORTED.
+ * Heads concatenated with dqk == dv, H * dqk <= 128 and V == K + H*dqk in one [N, 2A] buffer (ldk == ldv, a multiple of 8,
+ * 16-byte aligned) take the TMA ring, one bulk copy of 4A bytes per neighbour; other shapes with heads concatenated,
+ * dqk == dv and A <= 512 (8-byte aligned rows) the register-staged single-pass kernel.  Both give the output of
+ * tfgk_gat_fused_f32 over the widened K and V where it runs the same kernel.  Every other shape (averaged heads, dqk != dv)
+ * takes the two-pass generic kernel, which needs att ([E, H] scratch).  Only the TMA ring reads K and V faster than fp32 does;
+ * the single-pass kernel with bf16 rows is latency-bound and slower than with fp32 rows (DESIGN.md section 4). */
+int tfgk_gat_fused_bf16(const int64_t *rowptr, const int32_t *col,
+                        const float *Q, int64_t ldq, const uint16_t *K, int64_t ldk, const uint16_t *V, int64_t ldv,
+                        int32_t N, int32_t H, int32_t dqk, int32_t dv, float scale, int split_value_heads,
+                        const float *bias, int act, float *att, int write_att, float *out, int64_t ldo,
+                        const tfgk_plan *plan, void *stream);
 
 /* ---- K4: dense projections (gcn.py:272, gat.py:52,61,70, graph_sage.py:43-44, appnp.py:69) ------------------- */
 
@@ -197,6 +224,25 @@ typedef struct tfgk_proj_block {
 int tfgk_gemm_proj_f32(const float *const *A_parts, int32_t n_parts, int64_t part_rows, int64_t lda,
                        int32_t M, int32_t K, const tfgk_proj_block *blocks, int32_t n_blocks,
                        int32_t first_part, int32_t max_ctas, void *stream);
+/* tfgk_gemm_proj_f32 with a per-block output type: a TFGK_DTYPE_BF16 block stores the fp32 result of its epilogue
+ * (bias, activation) rounded to nearest even, bit-identical to rounding tfgk_gemm_proj_f32's output (inf and NaN stay
+ * inf and NaN, finite values beyond the bf16 range become inf).  GAT's fp32 Q and bf16 K | V thus still come from one
+ * launch that reads x once.  Only n_parts == 1 (TFGK_ERR_UNSUPPORTED otherwise); the other shape limits are those of
+ * tfgk_gemm_proj_f32, and tfgk_round_bf16 rounds the output of tfgk_gemm_f32 for the shapes it refuses. */
+typedef struct tfgk_proj_block_out {
+    const float *B; int64_t ldb;       /* as in tfgk_proj_block */
+    int32_t ncols;
+    int32_t transB;
+    const float *bias;
+    int act;
+    void *C; int64_t ldc;              /* [M, ncols] output of type c_dtype (may be a column slice) */
+    int32_t c_dtype;                   /* tfgk_dtype */
+} tfgk_proj_block_out;
+int tfgk_gemm_proj_mixed(const float *const *A_parts, int32_t n_parts, int64_t part_rows, int64_t lda,
+                         int32_t M, int32_t K, const tfgk_proj_block_out *blocks, int32_t n_blocks,
+                         int32_t first_part, int32_t max_ctas, void *stream);
+/* dst[r, c] = bf16(src[r, c]) rounded to nearest even, r < rows, c < cols. */
+int tfgk_round_bf16(const float *src, int64_t lds, int32_t rows, int32_t cols, uint16_t *dst, int64_t ldd, void *stream);
 
 /* ---- K5: peer memory for the partitioned path (SURVEY.md 8e) ---------------------------------------------------
  * The ONE exception to "the library never allocates": buffers that other ranks on the same node read over NVLink

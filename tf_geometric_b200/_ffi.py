@@ -25,6 +25,7 @@ BERNOULLI_NONE, BERNOULLI_DROPOUT, BERNOULLI_KEEP = 0, 1, 2
 SAMPLE_NO_PADDING, SAMPLE_PADDING, SAMPLE_HEAD = 0, 1, 2
 NEG_UPPER, NEG_START = 0, 1
 PAD_ROW_MAJOR, PAD_STEP_MAJOR = 0, 1
+DTYPE_F32, DTYPE_BF16 = 0, 1
 
 _i32, _i64, _f32, _int = ctypes.c_int32, ctypes.c_int64, ctypes.c_float, ctypes.c_int
 _ptr, _size = ctypes.c_void_p, ctypes.c_size_t
@@ -54,13 +55,19 @@ SIGNATURES = {
     "tfgk_scale_edges_f32": [_ptr, _ptr, _ptr, _i64, _ptr, _ptr, _ptr, _ptr],
     "tfgk_spmm_f32": [_ptr, _ptr, _ptr, _ptr, _i64, _i32, _i32, _int, _f32, _ptr, _i64, _f32, _ptr, _int, _ptr, _i64,
                       _ptr, _ptr],
+    "tfgk_spmm_bf16": [_ptr, _ptr, _ptr, _ptr, _i64, _i32, _i32, _int, _f32, _ptr, _i64, _f32, _ptr, _int, _ptr, _i64,
+                       _ptr, _ptr],
     "tfgk_segment_softmax_f32": [_ptr, _ptr, _i32, _i32, _ptr, _ptr],
     "tfgk_gat_fused_f32": [_ptr, _ptr, _ptr, _i64, _ptr, _i64, _ptr, _i64, _i32, _i32, _i32, _i32, _f32, _int, _ptr,
                            _int, _ptr, _int, _ptr, _i64, _ptr, _ptr],
+    "tfgk_gat_fused_bf16": [_ptr, _ptr, _ptr, _i64, _ptr, _i64, _ptr, _i64, _i32, _i32, _i32, _i32, _f32, _int, _ptr,
+                            _int, _ptr, _int, _ptr, _i64, _ptr, _ptr],
     "tfgk_gemm_workspace_bytes": [_i32, _i32, _i32, ctypes.POINTER(_size)],
     "tfgk_gemm_f32": [_ptr, _i64, _int, _ptr, _i64, _int, _ptr, _int, _f32, _i32, _i32, _i32, _ptr, _i64, _ptr, _size,
                       _ptr],
     "tfgk_gemm_proj_f32": [_ptr, _i32, _i64, _i64, _i32, _i32, _ptr, _i32, _i32, _i32, _ptr],
+    "tfgk_gemm_proj_mixed": [_ptr, _i32, _i64, _i64, _i32, _i32, _ptr, _i32, _i32, _i32, _ptr],
+    "tfgk_round_bf16": [_ptr, _i64, _i32, _i32, _ptr, _i64, _ptr],
     "tfgk_peer_alloc": [_size, ctypes.POINTER(_ptr)],
     "tfgk_peer_free": [_ptr],
     "tfgk_peer_export": [_ptr, _ptr],
@@ -127,6 +134,11 @@ class ProjBlock(ctypes.Structure):
     """struct tfgk_proj_block of include/tfgk.h."""
     _fields_ = [("B", _ptr), ("ldb", _i64), ("ncols", _i32), ("transB", _i32), ("bias", _ptr), ("act", _int), ("C", _ptr),
                 ("ldc", _i64)]
+
+
+class ProjBlockOut(ctypes.Structure):
+    """struct tfgk_proj_block_out of include/tfgk.h."""
+    _fields_ = ProjBlock._fields_ + [("c_dtype", _i32)]
 
 
 PEER_HANDLE_BYTES = 64

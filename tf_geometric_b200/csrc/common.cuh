@@ -105,4 +105,23 @@ __device__ __forceinline__ float ld_stream_f32(const float *p) {
     return v;
 }
 
+// bf16 message rows are stored as their 16-bit patterns (uint16_t); widening to fp32 is exact (the pattern is the upper
+// half of the fp32 one), so a kernel that widens each element and then runs the fp32 arithmetic computes exactly what the
+// fp32 kernel computes over the widened table.
+__device__ __forceinline__ float bf16_to_f32(uint32_t bits) { return __uint_as_float(bits << 16); }
+
+// four consecutive row elements at `p` (shared or global memory), widened to fp32: one 16-byte load for fp32 rows, one
+// 8-byte load for bf16 rows (p aligned accordingly)
+template <typename T> __device__ __forceinline__ float4 load_row4(const uint8_t *p);
+template <> __device__ __forceinline__ float4 load_row4<float>(const uint8_t *p) {
+    return *reinterpret_cast<const float4 *>(p);
+}
+template <> __device__ __forceinline__ float4 load_row4<uint16_t>(const uint8_t *p) {
+    const uint2 t = *reinterpret_cast<const uint2 *>(p);
+    return make_float4(__uint_as_float(t.x << 16), __uint_as_float(t.x & 0xFFFF0000u), __uint_as_float(t.y << 16),
+                       __uint_as_float(t.y & 0xFFFF0000u));
+}
+
+inline bool aligned8(const void *p) { return (reinterpret_cast<uintptr_t>(p) & 7u) == 0; }
+
 }  // namespace tfgk

@@ -20,6 +20,12 @@ constexpr int kGatWarps = kGatThreads / 32;
 constexpr int kMaxHeadsFast = 32;
 
 __device__ __forceinline__ float4 ldg4(const float *p) { return __ldg(reinterpret_cast<const float4 *>(p)); }
+// four consecutive row elements from global memory, widened to fp32 (16-byte fp32 or 8-byte bf16 load)
+__device__ __forceinline__ float4 ldg_row4(const float *p) { return ldg4(p); }
+__device__ __forceinline__ float4 ldg_row4(const uint16_t *p) {
+    const uint2 t = __ldg(reinterpret_cast<const uint2 *>(p));
+    return make_float4(bf16_to_f32(t.x & 0xFFFFu), bf16_to_f32(t.x >> 16), bf16_to_f32(t.y & 0xFFFFu), bf16_to_f32(t.y >> 16));
+}
 
 struct GatParams {
     const int64_t *rowptr;
@@ -27,6 +33,7 @@ struct GatParams {
     const float *Q; int64_t ldq;
     const float *K; int64_t ldk;
     const float *V; int64_t ldv;
+    const uint16_t *Kb, *Vb;   // bf16 K and V (tfgk_gat_fused_bf16), leading dimensions ldk / ldv
     int32_t N, H, dqk, dv;
     float scale;
     int split;
@@ -206,8 +213,10 @@ __global__ void __launch_bounds__(kGatThreads) gat_fast_kernel(const GatParams p
 // [N, A+U] buffer (V == K + A, same leading dimension) the two 16-byte loads of a lane hit the same 1 KB DRAM
 // burst.  No score scratch is touched unless the attention coefficients are requested.  The result differs from the
 // reference's max -> exp -> sum -> divide order only by the rounding of the rescales (<= 1e-6 relative).
-template <int NC, int U>
+template <int NC, int U, typename T>
 __global__ void __launch_bounds__(kGatThreads) gat_online_kernel(const GatParams p) {
+    const T *Kt = sizeof(T) == 4 ? (const T *)p.K : (const T *)p.Kb;
+    const T *Vt = sizeof(T) == 4 ? (const T *)p.V : (const T *)p.Vb;
     __shared__ float s_max[kGatWarps][kMaxHeadsFast];
     __shared__ float s_den[kGatWarps][kMaxHeadsFast];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -245,13 +254,13 @@ __global__ void __launch_bounds__(kGatThreads) gat_online_kernel(const GatParams
 #pragma unroll
             for (int u = 0; u < U; ++u) {
                 const int c = __shfl_sync(0xffffffffu, my_c, j + u);
-                const float *krow = p.K + (int64_t)c * p.ldk;
-                const float *vrow = p.V + (int64_t)c * p.ldv;
+                const T *krow = Kt + (int64_t)c * p.ldk;
+                const T *vrow = Vt + (int64_t)c * p.ldv;
 #pragma unroll
                 for (int k = 0; k < NC; ++k)
                     if (j + u < nb && cok[k]) {
-                        kk[u][k] = ldg4(krow + ccol[k]);
-                        vv[u][k] = ldg4(vrow + ccol[k]);
+                        kk[u][k] = ldg_row4(krow + ccol[k]);
+                        vv[u][k] = ldg_row4(vrow + ccol[k]);
                     }
             }
             float sc[U][NC];
@@ -486,14 +495,14 @@ __device__ __forceinline__ void gat_mbar_wait(uint32_t bar, uint32_t parity) {
     }
 }
 
-template <int S>
+template <int S, typename T>
 __global__ void __launch_bounds__(kGatAsyncWarps * 32) gat_tma4_kernel(const GatParams p) {
     constexpr int U = 4, RPC = 32 / U;
     static_assert(S <= RPC, "index chunk refill assumes the prologue stays inside chunk 0");
     extern __shared__ __align__(128) uint8_t gat_g4_ring[];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int A = p.H * p.dqk;
-    const uint32_t edge_bytes = 2u * (uint32_t)A * 4u;            // [K row | V row] of one neighbour, contiguous in the KV buffer
+    const uint32_t edge_bytes = 2u * (uint32_t)A * (uint32_t)sizeof(T);   // [K row | V row] of one neighbour, contiguous
     const uint32_t stage_bytes = (U * edge_bytes + 127u) & ~127u;
     uint8_t *my_ring = gat_g4_ring + (size_t)warp * S * stage_bytes;
     const uint32_t ring_addr = (uint32_t)__cvta_generic_to_shared(my_ring);
@@ -528,7 +537,8 @@ __global__ void __launch_bounds__(kGatAsyncWarps * 32) gat_tma4_kernel(const Gat
     const int lanes_per_head = p.dqk >> 2;
     const int ccol = lane * 4;
     const bool cok = ccol < A;
-    const uint32_t row_bytes = (uint32_t)A * 4u;
+    const uint32_t row_bytes = (uint32_t)A * (uint32_t)sizeof(T);
+    const T *kv = sizeof(T) == 4 ? (const T *)p.K : (const T *)p.Kb;
 
     int64_t r = r0;
     int row_end = slot >= 0 ? 0x7fffffff : (int)(__shfl_sync(0xffffffffu, rp_hi, 0) - e_begin);
@@ -576,7 +586,7 @@ __global__ void __launch_bounds__(kGatAsyncWarps * 32) gat_tma4_kernel(const Gat
             if (lane < valid)
                 asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
                              ::"r"(ring_addr + (uint32_t)(g % S) * stage_bytes + (uint32_t)lane * edge_bytes),
-                             "l"(p.K + (int64_t)c * p.ldk), "r"(edge_bytes), "r"(bar) : "memory");
+                             "l"(kv + (int64_t)c * p.ldk), "r"(edge_bytes), "r"(bar) : "memory");
         }
     };
 
@@ -599,8 +609,8 @@ __global__ void __launch_bounds__(kGatAsyncWarps * 32) gat_tma4_kernel(const Gat
                 while (e == row_end) finalize_row();
                 float4 kk = make_float4(0.f, 0.f, 0.f, 0.f), vv = kk;
                 if (cok) {
-                    kk = *reinterpret_cast<const float4 *>(sbuf + (size_t)u * edge_bytes + ccol * 4);
-                    vv = *reinterpret_cast<const float4 *>(sbuf + (size_t)u * edge_bytes + row_bytes + ccol * 4);
+                    kk = load_row4<T>(sbuf + (size_t)u * edge_bytes + ccol * sizeof(T));
+                    vv = load_row4<T>(sbuf + (size_t)u * edge_bytes + row_bytes + ccol * sizeof(T));
                 }
                 float d = q.x * kk.x + q.y * kk.y + q.z * kk.z + q.w * kk.w;
                 for (int off = 1; off < lanes_per_head; off <<= 1) d += __shfl_xor_sync(0xffffffffu, d, off);
@@ -686,18 +696,21 @@ static int launch_gat_async(const GatParams &p, cudaStream_t st) {
     return TFGK_OK;
 }
 
-template <int S>
+template <int S, typename T = float>
 static int launch_gat_tma4(const GatParams &p, cudaStream_t st) {
     const int A = p.H * p.dqk;
     // one bulk copy per neighbour: the [K | V] span must be 16-byte aligned and a multiple of 16 bytes
-    if (p.V != p.K + A || p.ldk != p.ldv || 2 * A > 256 || (p.ldk % 4) != 0 || (A % 2) != 0 || !aligned16(p.K))
+    constexpr int kPer16 = 16 / (int)sizeof(T);
+    const bool adjacent = sizeof(T) == 4 ? p.V == p.K + A : p.Vb == p.Kb + A;
+    const void *base = sizeof(T) == 4 ? (const void *)p.K : (const void *)p.Kb;
+    if (!adjacent || p.ldk != p.ldv || 2 * A > 256 || (p.ldk % kPer16) != 0 || (2 * A) % kPer16 != 0 || !aligned16(base))
         return TFGK_ERR_UNSUPPORTED;
-    const size_t stage_pitch = ((size_t)4 * 2 * A * 4 + 127) & ~(size_t)127;
+    const size_t stage_pitch = ((size_t)4 * 2 * A * sizeof(T) + 127) & ~(size_t)127;
     const size_t smem = (size_t)kGatAsyncWarps * S * stage_pitch + (size_t)kGatAsyncWarps * S * 8;
-    TFGK_CUDA(ensure_dynamic_smem(gat_tma4_kernel<S>, smem));
+    TFGK_CUDA(ensure_dynamic_smem(gat_tma4_kernel<S, T>, smem));
     const int64_t n_tasks = p.task_row ? p.n_tasks : ceil_div64(p.N, kGatAsyncRows);
     const unsigned blocks = (unsigned)ceil_div64(n_tasks, kGatAsyncWarps);
-    gat_tma4_kernel<S><<<blocks, kGatAsyncWarps * 32, smem, st>>>(p);
+    gat_tma4_kernel<S, T><<<blocks, kGatAsyncWarps * 32, smem, st>>>(p);
     TFGK_LAUNCH_CHECK();
     if (p.task_row && p.n_hubs > 0) {
         gat_hub_fixup_kernel<<<(unsigned)ceil_div64(p.n_hubs, 8), 256, 0, st>>>(p);
@@ -738,7 +751,13 @@ __device__ __forceinline__ float warp_max(float v) {
     return v;
 }
 
+__device__ __forceinline__ float ld_elem(const float *p) { return *p; }
+__device__ __forceinline__ float ld_elem(const uint16_t *p) { return bf16_to_f32(*p); }
+
+template <typename T>
 __global__ void __launch_bounds__(kGatThreads) gat_generic_kernel(const GatParams p) {
+    const T *Kt = sizeof(T) == 4 ? (const T *)p.K : (const T *)p.Kb;
+    const T *Vt = sizeof(T) == 4 ? (const T *)p.V : (const T *)p.Vb;
     extern __shared__ float smem[];   // [warps][2][H]
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int64_t r = (int64_t)blockIdx.x * kGatWarps + warp;
@@ -754,11 +773,11 @@ __global__ void __launch_bounds__(kGatThreads) gat_generic_kernel(const GatParam
     for (int h = lane; h < H; h += 32) s_max[h] = -FLT_MAX;
     __syncwarp();
     for (int e = 0; e < deg; ++e) {
-        const float *krow = p.K + (int64_t)col[e] * p.ldk;
+        const T *krow = Kt + (int64_t)col[e] * p.ldk;
         const float *qrow = p.Q + r * p.ldq;
         for (int h = 0; h < H; ++h) {
             float d = 0.0f;
-            for (int j = lane; j < p.dqk; j += 32) d += qrow[h * p.dqk + j] * krow[h * p.dqk + j];
+            for (int j = lane; j < p.dqk; j += 32) d += qrow[h * p.dqk + j] * ld_elem(krow + h * p.dqk + j);
             d = warp_sum(d);
             if (lane == 0) {
                 const float s = __fdiv_rn(d, p.scale);
@@ -787,7 +806,7 @@ __global__ void __launch_bounds__(kGatThreads) gat_generic_kernel(const GatParam
             float acc = 0.0f;
             for (int e = 0; e < deg; ++e) {
                 const float a = __fdiv_rn(att[(int64_t)e * H + hv], dn);
-                acc = __fadd_rn(acc, __fmul_rn(p.V[(int64_t)col[e] * p.ldv + c], a));
+                acc = __fadd_rn(acc, __fmul_rn(ld_elem(Vt + (int64_t)col[e] * p.ldv + c), a));
             }
             if (p.bias) acc += p.bias[c];
             p.out[r * p.ldo + c] = apply_act(acc, p.act);
@@ -800,7 +819,7 @@ __global__ void __launch_bounds__(kGatThreads) gat_generic_kernel(const GatParam
                 float acc = 0.0f;
                 for (int e = 0; e < deg; ++e) {
                     const float a = __fdiv_rn(att[(int64_t)e * H + h], dn);
-                    acc = __fadd_rn(acc, __fmul_rn(p.V[(int64_t)col[e] * p.ldv + h * p.dv + u], a));
+                    acc = __fadd_rn(acc, __fmul_rn(ld_elem(Vt + (int64_t)col[e] * p.ldv + h * p.dv + u), a));
                 }
                 tot = h == 0 ? acc : __fadd_rn(tot, acc);     // tf.add_n over heads
             }
@@ -841,11 +860,11 @@ __global__ void __launch_bounds__(kGatThreads) segment_softmax_kernel(const int6
     }
 }
 
-template <int NC>
+template <int NC, typename T = float>
 static int launch_gat_online(const GatParams &p, cudaStream_t st) {
     constexpr int U = NC == 1 ? 4 : 2;
     const unsigned blocks = (unsigned)ceil_div64(p.N, kGatWarps);
-    gat_online_kernel<NC, U><<<blocks, kGatThreads, 0, st>>>(p);
+    gat_online_kernel<NC, U, T><<<blocks, kGatThreads, 0, st>>>(p);
     TFGK_LAUNCH_CHECK();
     return TFGK_OK;
 }
@@ -903,7 +922,7 @@ static int gat_fused_impl(const int64_t *rowptr, const int32_t *col,
 
     GatParams p;
     p.rowptr = rowptr; p.col = col;
-    p.Q = Q; p.ldq = ldq; p.K = K; p.ldk = ldk; p.V = V; p.ldv = ldv;
+    p.Q = Q; p.ldq = ldq; p.K = K; p.ldk = ldk; p.V = V; p.ldv = ldv; p.Kb = nullptr; p.Vb = nullptr;
     p.N = N; p.H = H; p.dqk = dqk; p.dv = dv; p.scale = scale; p.split = split_value_heads;
     p.bias = bias; p.act = act; p.att = att; p.write_att = write_att; p.out = out; p.ldo = ldo;
     p.n_tasks = 0; p.task_row = nullptr; p.task_nrows = nullptr; p.task_e0 = nullptr; p.task_e1 = nullptr;
@@ -949,7 +968,7 @@ static int gat_fused_impl(const int64_t *rowptr, const int32_t *col,
     }
     const size_t smem = (size_t)kGatWarps * 2 * H * sizeof(float);
     TFGK_CHECK_ARG(smem <= 48 * 1024, "gat: too many heads for the generic path (H=%d)", H);
-    gat_generic_kernel<<<(unsigned)ceil_div64(N, kGatWarps), kGatThreads, smem, st>>>(p);
+    gat_generic_kernel<float><<<(unsigned)ceil_div64(N, kGatWarps), kGatThreads, smem, st>>>(p);
     TFGK_LAUNCH_CHECK();
     return TFGK_OK;
 }
@@ -971,4 +990,69 @@ extern "C" int tfgk_gat_fused_stats_f32(const int64_t *rowptr, const int32_t *co
     TFGK_CHECK_ARG(stats != nullptr, "gat_fused_stats: stats buffer is required");
     return gat_fused_impl(rowptr, col, Q, ldq, K, ldk, V, ldv, N, H, dqk, dv, scale, 1, bias, act, nullptr, 0, out, ldo, plan,
                           stats, stream);
+}
+
+// bf16 K and V (inference): each element is widened on its way out of shared memory (TMA ring) or global memory (the
+// single-pass and generic kernels), then the fp32 arithmetic of the same kernel runs unchanged; Q, the softmax, the
+// accumulators and the output stay fp32.  The TMA ring (A <= 128, K | V adjacent) and the single-pass kernel (heads
+// concatenated, dqk == dv, A <= 512) keep the fp32 lane-to-column mapping, so their output equals tfgk_gat_fused_f32's
+// over the widened K and V when it takes the same kernel; the generic path takes every other shape (averaged heads, dqk !=
+// dv, ...) and needs the [E, H] score scratch.
+extern "C" int tfgk_gat_fused_bf16(const int64_t *rowptr, const int32_t *col,
+                                   const float *Q, int64_t ldq, const uint16_t *K, int64_t ldk, const uint16_t *V, int64_t ldv,
+                                   int32_t N, int32_t H, int32_t dqk, int32_t dv, float scale, int split_value_heads,
+                                   const float *bias, int act, float *att, int write_att, float *out, int64_t ldo,
+                                   const tfgk_plan *plan, void *stream) {
+    TFGK_CHECK_ARG(N >= 0 && H >= 1 && dqk >= 1 && dv >= 1, "gat: bad size (N=%d H=%d dqk=%d dv=%d)", N, H, dqk, dv);
+    TFGK_CHECK_ARG(act == TFGK_ACT_NONE || act == TFGK_ACT_RELU, "gat: unknown activation %d", act);
+    TFGK_CHECK_ARG(scale > 0.0f, "gat: scale must be positive");
+    if (write_att) return set_error(TFGK_ERR_UNSUPPORTED, "gat_fused_bf16: the attention coefficients are not returned");
+    if (N == 0) return TFGK_OK;
+    TFGK_CHECK_ARG(rowptr && col && Q && K && V && out, "gat: null pointer");
+    const int A = H * dqk, VW = H * dv;
+    const int out_w = split_value_heads ? VW : dv;
+    TFGK_CHECK_ARG(ldq >= A && ldk >= A && ldv >= VW && ldo >= out_w, "gat: leading dimension too small");
+
+    GatParams p;
+    p.rowptr = rowptr; p.col = col;
+    p.Q = Q; p.ldq = ldq; p.K = nullptr; p.ldk = ldk; p.V = nullptr; p.ldv = ldv; p.Kb = K; p.Vb = V;
+    p.N = N; p.H = H; p.dqk = dqk; p.dv = dv; p.scale = scale; p.split = split_value_heads;
+    p.bias = bias; p.act = act; p.att = att; p.write_att = 0; p.out = out; p.ldo = ldo;
+    p.n_tasks = 0; p.task_row = nullptr; p.task_nrows = nullptr; p.task_e0 = nullptr; p.task_e1 = nullptr;
+    p.task_slot = nullptr; p.n_hubs = 0; p.hub_row = nullptr; p.hub_slot0 = nullptr; p.hub_nslots = nullptr; p.scratch = nullptr;
+    p.stats = nullptr;
+    if (plan != nullptr && plan->n_tasks > 0) {
+        if (plan->n_hubs > 0)
+            TFGK_CHECK_ARG(plan->scratch != nullptr && plan->scratch_bytes >= (size_t)plan->n_slots * (VW + 64) * sizeof(float),
+                           "gat: plan scratch too small (need %zu bytes)", (size_t)plan->n_slots * (VW + 64) * sizeof(float));
+        p.n_tasks = plan->n_tasks; p.task_row = plan->task_row; p.task_nrows = plan->task_nrows;
+        p.task_e0 = plan->task_e0; p.task_e1 = plan->task_e1; p.task_slot = plan->task_slot;
+        p.n_hubs = plan->n_hubs; p.hub_row = plan->hub_row; p.hub_slot0 = plan->hub_slot0;
+        p.hub_nslots = plan->hub_nslots; p.scratch = plan->scratch;
+    }
+    cudaStream_t st = as_stream(stream);
+    // the shapes of the fp32 single-pass kernels (four consecutive columns per lane), with 8-byte aligned bf16 rows
+    const bool fast = split_value_heads && is_pow2(H) && H <= kMaxHeadsFast && dqk == dv && dqk % 4 == 0 &&
+                      is_pow2(dqk / 4) && dqk <= 128 && A <= 512 && ldq % 4 == 0 && ldk % 4 == 0 && ldv % 4 == 0 &&
+                      ldo % 4 == 0 && aligned16(Q) && aligned8(K) && aligned8(V) && aligned16(out) &&
+                      (!bias || aligned16(bias));
+    if (fast && A <= 128) {
+        // 512-byte [K | V] spans at A = 128: three stages keep two rounds of four neighbours in flight per warp
+        const int rc = launch_gat_tma4<3, uint16_t>(p, st);      // TFGK_ERR_UNSUPPORTED unless K | V are adjacent
+        if (rc != TFGK_ERR_UNSUPPORTED) return rc;
+    }
+    if (fast) {                                                  // the register-staged single-pass kernel
+        switch ((A + 127) / 128) {
+            case 1: return launch_gat_online<1, uint16_t>(p, st);
+            case 2: return launch_gat_online<2, uint16_t>(p, st);
+            case 3: return launch_gat_online<3, uint16_t>(p, st);
+            default: return launch_gat_online<4, uint16_t>(p, st);
+        }
+    }
+    if (att == nullptr) return set_error(TFGK_ERR_WORKSPACE, "gat: this shape needs the [E,H] attention scratch buffer");
+    const size_t smem = (size_t)kGatWarps * 2 * H * sizeof(float);
+    TFGK_CHECK_ARG(smem <= 48 * 1024, "gat: too many heads for the generic path (H=%d)", H);
+    gat_generic_kernel<uint16_t><<<(unsigned)ceil_div64(N, kGatWarps), kGatThreads, smem, st>>>(p);
+    TFGK_LAUNCH_CHECK();
+    return TFGK_OK;
 }

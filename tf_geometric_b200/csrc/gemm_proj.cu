@@ -30,6 +30,7 @@
 //     through CUDA IPC): the cp.async then read straight over NVLink, tile by tile.  Tiles are walked starting at the tile
 //     of part `first_part`, so that every rank pulls from a different peer at any moment.
 #include "common.cuh"
+#include <cuda_bf16.h>
 #include <type_traits>
 
 namespace tfgk {
@@ -51,7 +52,7 @@ struct Params {
     int M, K, kpad, nb, tiles_m, n_groups;
     const float *B[kMaxBlocks]; int64_t ldb[kMaxBlocks];
     const float *bias[kMaxBlocks]; int act[kMaxBlocks]; int ncols[kMaxBlocks]; int transb[kMaxBlocks];
-    float *C[kMaxBlocks]; int64_t ldc[kMaxBlocks];
+    void *C[kMaxBlocks]; int64_t ldc[kMaxBlocks]; int c_bf16[kMaxBlocks];   // c_bf16: C holds bf16, rounded to nearest even
 };
 
 // shared memory: W hi | W lo | bias | ring of A stages.  With 1024 bytes of W per K (rounded up to 8), 18 432 per A stage
@@ -201,9 +202,12 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_proj_kernel(const Params p) 
     const int frag_row = (warp >> 2) * 64 + (warp & 3) * 16 + (lane >> 2);
     const int frag_col = lane & 3;
     const int act = p.act[cb];
-    float *C = p.C[cb];
+    float *C = static_cast<float *>(p.C[cb]);
+    __nv_bfloat16 *Cb = static_cast<__nv_bfloat16 *>(p.C[cb]);
+    const bool c_bf16 = p.c_bf16[cb] != 0;
     const int64_t ldc = p.ldc[cb];
-    const bool vec2 = (ldc % 2) == 0 && (reinterpret_cast<uintptr_t>(C) & 7u) == 0;     // (col, col + 1) as one 8-byte store
+    // (col, col + 1) as one 8-byte store (fp32) or one 4-byte store (bf16)
+    const bool vec2 = (ldc % 2) == 0 && (reinterpret_cast<uintptr_t>(p.C[cb]) & (c_bf16 ? 3u : 7u)) == 0;
     float acc[64];
 #pragma unroll
     for (int i = 0; i < 64; ++i) acc[i] = 0.0f;
@@ -247,7 +251,21 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_proj_kernel(const Params p) 
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
                 const int64_t row = row0 + 8 * h;
-                if (row < p.M) {
+                if (row < p.M && c_bf16) {        // block-uniform: the fp32 value, rounded once
+                    __nv_bfloat16 *crow = Cb + row * ldc;
+#pragma unroll
+                    for (int nb8 = 0; nb8 < kUN / 8; ++nb8) {
+                        const int col = nb8 * 8 + 2 * frag_col;
+                        const float v0 = apply_act(acc[4 * nb8 + 2 * h] + s_bias[col], act);
+                        const float v1 = apply_act(acc[4 * nb8 + 2 * h + 1] + s_bias[col + 1], act);
+                        if (vec2 && col + 1 < ncols) {
+                            *reinterpret_cast<__nv_bfloat162 *>(crow + col) = __floats2bfloat162_rn(v0, v1);
+                        } else {
+                            if (col < ncols) crow[col] = __float2bfloat16_rn(v0);
+                            if (col + 1 < ncols) crow[col + 1] = __float2bfloat16_rn(v1);
+                        }
+                    }
+                } else if (row < p.M) {
                     float *crow = C + row * ldc;
 #pragma unroll
                     for (int nb8 = 0; nb8 < kUN / 8; ++nb8) {
@@ -281,14 +299,25 @@ static int launch(const Params &p, int grid, uint32_t smem_bytes, cudaStream_t s
     return TFGK_OK;
 }
 
+// dst = bf16(src), round to nearest even, for the projections tfgk_gemm_proj_mixed cannot take (fp32 GEMM, then this)
+__global__ void __launch_bounds__(256) round_bf16_kernel(const float *src, int64_t lds, int32_t rows, int32_t cols,
+                                                         __nv_bfloat16 *dst, int64_t ldd) {
+    const int64_t n = (int64_t)rows * cols;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t r = i / cols, c = i % cols;
+        dst[r * ldd + c] = __float2bfloat16_rn(src[r * lds + c]);
+    }
+}
+
 }  // namespace proj
 }  // namespace tfgk
 
 using namespace tfgk;
 
-extern "C" int tfgk_gemm_proj_f32(const float *const *A_parts, int32_t n_parts, int64_t part_rows, int64_t lda,
-                                  int32_t M, int32_t K, const tfgk_proj_block *blocks, int32_t n_blocks,
-                                  int32_t first_part, int32_t max_ctas, void *stream) {
+// blocks: n_blocks entries (read only when blocks != nullptr); c_bf16[b] != 0 marks a bf16 output block
+static int gemm_proj_impl(const float *const *A_parts, int32_t n_parts, int64_t part_rows, int64_t lda, int32_t M, int32_t K,
+                          const tfgk_proj_block *blocks, const int *c_bf16, int32_t n_blocks, int32_t first_part,
+                          int32_t max_ctas, void *stream) {
     TFGK_CHECK_ARG(A_parts != nullptr && blocks != nullptr, "gemm_proj: null argument");
     TFGK_CHECK_ARG(n_parts >= 1 && n_parts <= proj::kMaxParts, "gemm_proj: n_parts=%d not in [1, %d]", n_parts, proj::kMaxParts);
     TFGK_CHECK_ARG(n_blocks >= 1 && n_blocks <= proj::kMaxBlocks, "gemm_proj: n_blocks=%d not in [1, %d]", n_blocks, proj::kMaxBlocks);
@@ -323,7 +352,7 @@ extern "C" int tfgk_gemm_proj_f32(const float *const *A_parts, int32_t n_parts, 
         }
         p.B[b] = blk.B; p.ldb[b] = blk.ldb; p.bias[b] = blk.bias; p.act[b] = blk.act; p.ncols[b] = blk.ncols;
         p.transb[b] = blk.transB;
-        p.C[b] = blk.C; p.ldc[b] = blk.ldc;
+        p.C[b] = blk.C; p.ldc[b] = blk.ldc; p.c_bf16[b] = b < n_blocks ? c_bf16[b] : 0;
     }
     const proj::Plan L(K);
     if (L.stages == 0) return TFGK_ERR_UNSUPPORTED;     // W (hi | lo) does not fit next to two A stages
@@ -341,4 +370,46 @@ extern "C" int tfgk_gemm_proj_f32(const float *const *A_parts, int32_t n_parts, 
     if (L.stages >= 4) return proj::launch<4>(p, grid, L.total, st);
     if (L.stages == 3) return proj::launch<3>(p, grid, L.total, st);
     return proj::launch<2>(p, grid, L.total, st);
+}
+
+extern "C" int tfgk_gemm_proj_f32(const float *const *A_parts, int32_t n_parts, int64_t part_rows, int64_t lda,
+                                  int32_t M, int32_t K, const tfgk_proj_block *blocks, int32_t n_blocks,
+                                  int32_t first_part, int32_t max_ctas, void *stream) {
+    const int all_f32[proj::kMaxBlocks] = {0, 0, 0, 0};
+    return gemm_proj_impl(A_parts, n_parts, part_rows, lda, M, K, blocks, all_f32, n_blocks, first_part, max_ctas, stream);
+}
+
+extern "C" int tfgk_gemm_proj_mixed(const float *const *A_parts, int32_t n_parts, int64_t part_rows, int64_t lda,
+                                    int32_t M, int32_t K, const tfgk_proj_block_out *blocks, int32_t n_blocks,
+                                    int32_t first_part, int32_t max_ctas, void *stream) {
+    TFGK_CHECK_ARG(A_parts != nullptr && blocks != nullptr, "gemm_proj: null argument");
+    TFGK_CHECK_ARG(n_blocks >= 1 && n_blocks <= proj::kMaxBlocks, "gemm_proj: n_blocks=%d not in [1, %d]", n_blocks, proj::kMaxBlocks);
+    tfgk_proj_block plain[proj::kMaxBlocks];
+    int c_bf16[proj::kMaxBlocks];
+    for (int b = 0; b < n_blocks; ++b) {
+        const tfgk_proj_block_out &o = blocks[b];
+        TFGK_CHECK_ARG(o.c_dtype == TFGK_DTYPE_F32 || o.c_dtype == TFGK_DTYPE_BF16, "gemm_proj: block %d has unknown dtype %d",
+                       b, o.c_dtype);
+        if (o.c_dtype == TFGK_DTYPE_BF16)
+            TFGK_CHECK_ARG((reinterpret_cast<uintptr_t>(o.C) & 1u) == 0, "gemm_proj: block %d: bf16 output not 2-byte aligned", b);
+        plain[b].B = o.B; plain[b].ldb = o.ldb; plain[b].ncols = o.ncols; plain[b].transB = o.transB;
+        plain[b].bias = o.bias; plain[b].act = o.act; plain[b].C = static_cast<float *>(o.C); plain[b].ldc = o.ldc;
+        c_bf16[b] = o.c_dtype == TFGK_DTYPE_BF16;
+    }
+    if (n_parts != 1) return set_error(TFGK_ERR_UNSUPPORTED, "gemm_proj_mixed: only a single-part A is supported (n_parts=%d)", n_parts);
+    return gemm_proj_impl(A_parts, n_parts, part_rows, lda, M, K, plain, c_bf16, n_blocks, first_part, max_ctas, stream);
+}
+
+extern "C" int tfgk_round_bf16(const float *src, int64_t lds, int32_t rows, int32_t cols, uint16_t *dst, int64_t ldd,
+                               void *stream) {
+    TFGK_CHECK_ARG(rows >= 0 && cols >= 0, "round_bf16: negative size (rows=%d, cols=%d)", rows, cols);
+    if (rows == 0 || cols == 0) return TFGK_OK;
+    TFGK_CHECK_ARG(src != nullptr && dst != nullptr, "round_bf16: null pointer");
+    TFGK_CHECK_ARG(lds >= cols && ldd >= cols, "round_bf16: leading dimension < cols");
+    const int64_t n = (int64_t)rows * cols;
+    const unsigned grid = (unsigned)(ceil_div64(n, 256) < 4 * sm_count() ? ceil_div64(n, 256) : 4 * sm_count());
+    proj::round_bf16_kernel<<<grid, 256, 0, as_stream(stream)>>>(src, lds, rows, cols, reinterpret_cast<__nv_bfloat16 *>(dst),
+                                                                 ldd);
+    TFGK_LAUNCH_CHECK();
+    return TFGK_OK;
 }

@@ -29,6 +29,13 @@ __device__ __forceinline__ void load_vec(const float *p, float (&v)[VEC]) {
     }
 }
 
+// bf16 rows (scalar path only): one widened element
+template <int VEC>
+__device__ __forceinline__ void load_vec(const uint16_t *p, float (&v)[VEC]) {
+    static_assert(VEC == 1, "bf16 rows take the scalar path");
+    v[0] = bf16_to_f32(__ldg(p));
+}
+
 template <int VEC>
 __device__ __forceinline__ void store_vec(float *p, const float (&v)[VEC]) {
     if constexpr (VEC == 4) {
@@ -43,6 +50,7 @@ struct SpmmParams {
     const int32_t *col;
     const float *w;
     const float *h;
+    const uint16_t *hb;    // bf16 rows (tfgk_spmm_bf16); the kernels instantiated for uint16_t read this one
     int64_t ldh;
     int32_t n_dst;
     int32_t D;
@@ -65,10 +73,15 @@ struct SpmmParams {
     float *scratch;
 };
 
+// the message rows of a kernel instantiated for element type T (float or bf16 bits)
+template <typename T> __device__ __forceinline__ const T *rows_of(const SpmmParams &p);
+template <> __device__ __forceinline__ const float *rows_of<float>(const SpmmParams &p) { return p.h; }
+template <> __device__ __forceinline__ const uint16_t *rows_of<uint16_t>(const SpmmParams &p) { return p.hb; }
+
 constexpr int kSpmmThreads = 256;
 
 // G: lanes per row (power of two), NC: vectors per lane, IS_MAX: max-reduce instead of sum/mean, U: rows in flight
-template <int VEC, int G, int NC, bool IS_MAX, int U>
+template <int VEC, int G, int NC, bool IS_MAX, int U, typename T>
 __global__ void __launch_bounds__(kSpmmThreads) spmm_kernel(const SpmmParams p) {
     constexpr int RPW = 32 / G;   // rows per warp
     const int lane = threadIdx.x & 31;
@@ -105,7 +118,7 @@ __global__ void __launch_bounds__(kSpmmThreads) spmm_kernel(const SpmmParams p) 
         for (int v = 0; v < VEC; ++v) acc[k][v] = IS_MAX ? -FLT_MAX : 0.0f;
 
     const bool weighted = p.w != nullptr;
-    const float *__restrict__ h = p.h;
+    const T *__restrict__ h = rows_of<T>(p);
 
     for (int t = 0; t < deg_max; t += G) {
         // coalesced read of up to G (col, w) pairs of this row
@@ -127,7 +140,7 @@ __global__ void __launch_bounds__(kSpmmThreads) spmm_kernel(const SpmmParams p) 
                 const int c = __shfl_sync(0xffffffffu, my_c, src, G);
                 ww[u] = __shfl_sync(0xffffffffu, my_w, src, G);
                 const bool ok = src < nb;
-                const float *rowp = h + (int64_t)c * p.ldh;
+                const T *rowp = h + (int64_t)c * p.ldh;
 #pragma unroll
                 for (int k = 0; k < NC; ++k) {
                     if (ok && cok[k]) load_vec<VEC>(rowp + coff[k], v[u][k]);
@@ -488,8 +501,13 @@ __device__ __forceinline__ void cp_async16(uint32_t dst, const void *src) {
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 template <int N>
 __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
+// one lane's slice of a row: four elements, 16 bytes of fp32 or 8 bytes of bf16
+__device__ __forceinline__ void cp_async_slice(uint32_t dst, const float *src) { cp_async16(dst, src); }
+__device__ __forceinline__ void cp_async_slice(uint32_t dst, const uint16_t *src) {
+    asm volatile("cp.async.ca.shared.global [%0], [%1], 8;" ::"r"(dst), "l"(src) : "memory");
+}
 
-template <int NC, bool IS_MAX, int U, int S>
+template <int NC, bool IS_MAX, int U, int S, typename T>
 __global__ void __launch_bounds__(kAsyncWarps * 32) spmm_async_kernel(const SpmmParams p, uint32_t row_bytes) {
     static_assert(32 % U == 0, "a round must not straddle an index chunk");
     constexpr int RPC = 32 / U;
@@ -580,10 +598,10 @@ __global__ void __launch_bounds__(kAsyncWarps * 32) spmm_async_kernel(const Spmm
             for (int u = 0; u < U; ++u) {
                 const int c = __shfl_sync(0xffffffffu, ci, base + u);
                 if (g * U + u < n_edges) {
-                    const float *rowp = p.h + (int64_t)c * p.ldh;
+                    const T *rowp = rows_of<T>(p) + (int64_t)c * p.ldh;
 #pragma unroll
                     for (int k = 0; k < NC; ++k)
-                        if (cok[k]) cp_async16(dst0 + u * row_bytes + coff[k] * 4, rowp + coff[k]);
+                        if (cok[k]) cp_async_slice(dst0 + u * row_bytes + coff[k] * (uint32_t)sizeof(T), rowp + coff[k]);
                 }
             }
         }
@@ -623,7 +641,7 @@ __global__ void __launch_bounds__(kAsyncWarps * 32) spmm_async_kernel(const Spmm
 #pragma unroll
                 for (int k = 0; k < NC; ++k) {
                     if (cok[k]) {
-                        const float4 v = *reinterpret_cast<const float4 *>(sbuf + (size_t)u * row_bytes + coff[k] * 4);
+                        const float4 v = load_row4<T>(sbuf + (size_t)u * row_bytes + coff[k] * sizeof(T));
                         const float m0 = __fmul_rn(v.x, we), m1 = __fmul_rn(v.y, we), m2 = __fmul_rn(v.z, we), m3 = __fmul_rn(v.w, we);
                         acc[k][0] = IS_MAX ? fmaxf(acc[k][0], m0) : __fadd_rn(acc[k][0], m0);
                         acc[k][1] = IS_MAX ? fmaxf(acc[k][1], m1) : __fadd_rn(acc[k][1], m1);
@@ -660,12 +678,12 @@ __global__ void __launch_bounds__(kAsyncWarps * 32) spmm_async_kernel(const Spmm
 // a stage is re-armed only after every lane has read it (__syncwarp before the copies are issued).  A short last round
 // copies only its valid rows.  Same rounding and order => same bits.
 // ------------------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tma_row(uint32_t dst, const float *src, uint32_t bytes, uint32_t bar) {
+__device__ __forceinline__ void tma_row(uint32_t dst, const void *src, uint32_t bytes, uint32_t bar) {
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
                  ::"r"(dst), "l"(src), "r"(bytes), "r"(bar) : "memory");
 }
 
-template <bool IS_MAX, int S>
+template <bool IS_MAX, int S, typename T>
 __global__ void __launch_bounds__(kAsyncWarps * 32) spmm_tma4_kernel(const SpmmParams p, uint32_t row_bytes) {
     constexpr int U = 4, RPC = 32 / U;
     static_assert(S <= 2 * RPC, "weight look-ahead registers would be overwritten before they are consumed");
@@ -765,8 +783,8 @@ __global__ void __launch_bounds__(kAsyncWarps * 32) spmm_tma4_kernel(const SpmmP
                 asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"((uint32_t)valid * row_bytes)
                              : "memory");
             if (lane < valid)
-                tma_row(ring_addr + (uint32_t)(g % S) * stage_bytes + (uint32_t)lane * row_bytes, p.h + (int64_t)c * p.ldh,
-                        row_bytes, bar);
+                tma_row(ring_addr + (uint32_t)(g % S) * stage_bytes + (uint32_t)lane * row_bytes,
+                        rows_of<T>(p) + (int64_t)c * p.ldh, row_bytes, bar);
         }
     };
 
@@ -798,7 +816,7 @@ __global__ void __launch_bounds__(kAsyncWarps * 32) spmm_tma4_kernel(const SpmmP
 #pragma unroll
                 for (int k = 0; k < NCX; ++k) {
                     if (cok[k]) {
-                        const float4 v = *reinterpret_cast<const float4 *>(sbuf + (size_t)u * row_bytes + coff[k] * 4);
+                        const float4 v = load_row4<T>(sbuf + (size_t)u * row_bytes + coff[k] * sizeof(T));
                         const float m0 = __fmul_rn(v.x, we), m1 = __fmul_rn(v.y, we), m2 = __fmul_rn(v.z, we), m3 = __fmul_rn(v.w, we);
                         acc[k][0] = IS_MAX ? fmaxf(acc[k][0], m0) : __fadd_rn(acc[k][0], m0);
                         acc[k][1] = IS_MAX ? fmaxf(acc[k][1], m1) : __fadd_rn(acc[k][1], m1);
@@ -858,19 +876,19 @@ __global__ void __launch_bounds__(256) spmm_hub_fixup_kernel(const SpmmParams p)
     }
 }
 
-template <int NC, int U, int S>
+template <int NC, int U, int S, typename T = float>
 static int launch_spmm_async(const SpmmParams &p, cudaStream_t st) {
-    const uint32_t row_bytes = (uint32_t)p.D * 4u;
+    const uint32_t row_bytes = (uint32_t)(p.D * sizeof(T));
     const size_t smem = (size_t)kAsyncWarps * S * U * row_bytes;
     if (smem > 200 * 1024) return TFGK_ERR_UNSUPPORTED;
     const int64_t n_tasks = p.task_row ? p.n_tasks : ceil_div64(p.n_dst, kAsyncRows);
     const unsigned blocks = (unsigned)ceil_div64(n_tasks, kAsyncWarps);
     if (p.reduce == TFGK_REDUCE_MAX) {
-        TFGK_CUDA(ensure_dynamic_smem(spmm_async_kernel<NC, true, U, S>, smem));
-        spmm_async_kernel<NC, true, U, S><<<blocks, kAsyncWarps * 32, smem, st>>>(p, row_bytes);
+        TFGK_CUDA(ensure_dynamic_smem(spmm_async_kernel<NC, true, U, S, T>, smem));
+        spmm_async_kernel<NC, true, U, S, T><<<blocks, kAsyncWarps * 32, smem, st>>>(p, row_bytes);
     } else {
-        TFGK_CUDA(ensure_dynamic_smem(spmm_async_kernel<NC, false, U, S>, smem));
-        spmm_async_kernel<NC, false, U, S><<<blocks, kAsyncWarps * 32, smem, st>>>(p, row_bytes);
+        TFGK_CUDA(ensure_dynamic_smem(spmm_async_kernel<NC, false, U, S, T>, smem));
+        spmm_async_kernel<NC, false, U, S, T><<<blocks, kAsyncWarps * 32, smem, st>>>(p, row_bytes);
     }
     TFGK_LAUNCH_CHECK();
     if (p.task_row && p.n_hubs > 0) {
@@ -882,22 +900,24 @@ static int launch_spmm_async(const SpmmParams &p, cudaStream_t st) {
     return TFGK_OK;
 }
 
-template <int S>
+template <int S, typename T = float>
 static int launch_spmm_tma4(const SpmmParams &p, cudaStream_t st) {
-    // cp.async.bulk wants 16-byte aligned rows: D, ldh multiples of 4 floats and an aligned base
-    if (p.D > 256 || p.D % 4 != 0 || p.ldh % 4 != 0 || !aligned16(p.h)) return TFGK_ERR_UNSUPPORTED;
-    const uint32_t row_bytes = (uint32_t)p.D * 4u;
+    // cp.async.bulk wants 16-byte aligned rows: D, ldh multiples of 16 bytes' worth of elements and an aligned base
+    constexpr int kPer16 = 16 / (int)sizeof(T);
+    const void *base = sizeof(T) == 4 ? (const void *)p.h : (const void *)p.hb;
+    if (p.D > 256 || p.D % kPer16 != 0 || p.ldh % kPer16 != 0 || !aligned16(base)) return TFGK_ERR_UNSUPPORTED;
+    const uint32_t row_bytes = (uint32_t)(p.D * sizeof(T));
     const size_t stage_pitch = ((size_t)4 * row_bytes + 127) & ~(size_t)127;
     const size_t smem = (size_t)kAsyncWarps * S * stage_pitch + (size_t)kAsyncWarps * S * 8;
     if (smem > 200 * 1024) return TFGK_ERR_UNSUPPORTED;
     const int64_t n_tasks = p.task_row ? p.n_tasks : ceil_div64(p.n_dst, kAsyncRows);
     const unsigned blocks = (unsigned)ceil_div64(n_tasks, kAsyncWarps);
     if (p.reduce == TFGK_REDUCE_MAX) {
-        TFGK_CUDA(ensure_dynamic_smem(spmm_tma4_kernel<true, S>, smem));
-        spmm_tma4_kernel<true, S><<<blocks, kAsyncWarps * 32, smem, st>>>(p, row_bytes);
+        TFGK_CUDA(ensure_dynamic_smem(spmm_tma4_kernel<true, S, T>, smem));
+        spmm_tma4_kernel<true, S, T><<<blocks, kAsyncWarps * 32, smem, st>>>(p, row_bytes);
     } else {
-        TFGK_CUDA(ensure_dynamic_smem(spmm_tma4_kernel<false, S>, smem));
-        spmm_tma4_kernel<false, S><<<blocks, kAsyncWarps * 32, smem, st>>>(p, row_bytes);
+        TFGK_CUDA(ensure_dynamic_smem(spmm_tma4_kernel<false, S, T>, smem));
+        spmm_tma4_kernel<false, S, T><<<blocks, kAsyncWarps * 32, smem, st>>>(p, row_bytes);
     }
     TFGK_LAUNCH_CHECK();
     if (p.task_row && p.n_hubs > 0) {
@@ -972,30 +992,73 @@ static int dispatch_spmm_bulk(const SpmmParams &p, cudaStream_t st) {
     return launch_spmm_bulk<4>(p, st);
 }
 
-template <int VEC, int G, int NC, int U>
+template <int VEC, int G, int NC, int U, typename T>
 static int launch_spmm(const SpmmParams &p, cudaStream_t st) {
     constexpr int rows_per_block = (kSpmmThreads / 32) * (32 / G);
     const int64_t blocks = ceil_div64(p.n_dst, rows_per_block);
     if (p.reduce == TFGK_REDUCE_MAX)
-        spmm_kernel<VEC, G, NC, true, U><<<(unsigned)blocks, kSpmmThreads, 0, st>>>(p);
+        spmm_kernel<VEC, G, NC, true, U, T><<<(unsigned)blocks, kSpmmThreads, 0, st>>>(p);
     else
-        spmm_kernel<VEC, G, NC, false, U><<<(unsigned)blocks, kSpmmThreads, 0, st>>>(p);
+        spmm_kernel<VEC, G, NC, false, U, T><<<(unsigned)blocks, kSpmmThreads, 0, st>>>(p);
     TFGK_LAUNCH_CHECK();
     return TFGK_OK;
 }
 
-template <int VEC>
+template <int VEC, typename T = float>
 static int dispatch_spmm(const SpmmParams &p, int lanes, cudaStream_t st) {
     // lanes = number of VEC-wide vectors in a row (<= 128)
-    if (lanes <= 1) return launch_spmm<VEC, 1, 1, 8>(p, st);
-    if (lanes <= 2) return launch_spmm<VEC, 2, 1, 8>(p, st);
-    if (lanes <= 4) return launch_spmm<VEC, 4, 1, 8>(p, st);
-    if (lanes <= 8) return launch_spmm<VEC, 8, 1, 8>(p, st);
-    if (lanes <= 16) return launch_spmm<VEC, 16, 1, 8>(p, st);
-    if (lanes <= 32) return launch_spmm<VEC, 32, 1, 8>(p, st);
-    if (lanes <= 64) return launch_spmm<VEC, 32, 2, 4>(p, st);
-    if (lanes <= 96) return launch_spmm<VEC, 32, 3, 2>(p, st);
-    return launch_spmm<VEC, 32, 4, 2>(p, st);
+    if (lanes <= 1) return launch_spmm<VEC, 1, 1, 8, T>(p, st);
+    if (lanes <= 2) return launch_spmm<VEC, 2, 1, 8, T>(p, st);
+    if (lanes <= 4) return launch_spmm<VEC, 4, 1, 8, T>(p, st);
+    if (lanes <= 8) return launch_spmm<VEC, 8, 1, 8, T>(p, st);
+    if (lanes <= 16) return launch_spmm<VEC, 16, 1, 8, T>(p, st);
+    if (lanes <= 32) return launch_spmm<VEC, 32, 1, 8, T>(p, st);
+    if (lanes <= 64) return launch_spmm<VEC, 32, 2, 4, T>(p, st);
+    if (lanes <= 96) return launch_spmm<VEC, 32, 3, 2, T>(p, st);
+    return launch_spmm<VEC, 32, 4, 2, T>(p, st);
+}
+
+// argument checks shared by the fp32 and bf16 entry points: TFGK_OK to go on (with *nothing_to_do set for an empty
+// launch), or the error status
+static int spmm_validate(const int64_t *rowptr, const void *h, int64_t ldh, int32_t n_dst, int32_t D, int reduce,
+                         const float *addend, int64_t ld_addend, int act, const float *out, int64_t ldo,
+                         const tfgk_plan *plan, bool *nothing_to_do) {
+    *nothing_to_do = true;
+    TFGK_CHECK_ARG(n_dst >= 0 && D >= 0, "spmm: negative size (n_dst=%d, D=%d)", n_dst, D);
+    if (plan != nullptr && plan->n_hubs > 0)
+        TFGK_CHECK_ARG(plan->scratch != nullptr && plan->scratch_bytes >= (size_t)plan->n_slots * D * sizeof(float),
+                       "spmm: plan scratch too small (need %zu bytes)", (size_t)plan->n_slots * D * sizeof(float));
+    TFGK_CHECK_ARG(reduce >= TFGK_REDUCE_SUM && reduce <= TFGK_REDUCE_MAX, "spmm: unknown reduce %d", reduce);
+    TFGK_CHECK_ARG(act == TFGK_ACT_NONE || act == TFGK_ACT_RELU, "spmm: unknown activation %d", act);
+    if (n_dst == 0 || D == 0) return TFGK_OK;
+    TFGK_CHECK_ARG(rowptr && out && h, "spmm: null pointer");
+    TFGK_CHECK_ARG(ldh >= D && ldo >= D && (!addend || ld_addend >= D), "spmm: leading dimension < D");
+    *nothing_to_do = false;
+    return TFGK_OK;
+}
+
+static SpmmParams spmm_params(const int64_t *rowptr, const int32_t *col, const float *w, int64_t ldh, int32_t n_dst,
+                              int reduce, float alpha, const float *addend, int64_t ld_addend, float beta,
+                              const float *bias, int act, float *out, int64_t ldo, int c0, int width) {
+    SpmmParams p;
+    p.rowptr = rowptr; p.col = col; p.w = w;
+    p.h = nullptr; p.hb = nullptr; p.ldh = ldh; p.n_dst = n_dst;
+    p.D = width;
+    p.reduce = reduce; p.alpha = alpha;
+    p.addend = addend ? addend + c0 : nullptr; p.ld_addend = ld_addend; p.beta = beta;
+    p.bias = bias ? bias + c0 : nullptr; p.act = act;
+    p.out = out + c0; p.ldo = ldo;
+    p.n_tasks = 0; p.task_row = nullptr; p.task_nrows = nullptr; p.task_e0 = nullptr; p.task_e1 = nullptr;
+    p.task_slot = nullptr; p.n_hubs = 0; p.hub_row = nullptr; p.hub_slot0 = nullptr; p.hub_nslots = nullptr;
+    p.scratch = nullptr;
+    return p;
+}
+
+static void spmm_use_plan(SpmmParams &p, const tfgk_plan *plan) {
+    p.n_tasks = plan->n_tasks; p.task_row = plan->task_row; p.task_nrows = plan->task_nrows;
+    p.task_e0 = plan->task_e0; p.task_e1 = plan->task_e1; p.task_slot = plan->task_slot;
+    p.n_hubs = plan->n_hubs; p.hub_row = plan->hub_row; p.hub_slot0 = plan->hub_slot0;
+    p.hub_nslots = plan->hub_nslots; p.scratch = plan->scratch;
 }
 
 }  // namespace tfgk
@@ -1007,41 +1070,22 @@ extern "C" int tfgk_spmm_f32(const int64_t *rowptr, const int32_t *col, const fl
                              float alpha, const float *addend, int64_t ld_addend, float beta,
                              const float *bias, int act,
                              float *out, int64_t ldo, const tfgk_plan *plan, void *stream) {
-    TFGK_CHECK_ARG(n_dst >= 0 && D >= 0, "spmm: negative size (n_dst=%d, D=%d)", n_dst, D);
-    if (plan != nullptr && plan->n_hubs > 0)
-        TFGK_CHECK_ARG(plan->scratch != nullptr && plan->scratch_bytes >= (size_t)plan->n_slots * D * sizeof(float),
-                       "spmm: plan scratch too small (need %zu bytes)", (size_t)plan->n_slots * D * sizeof(float));
-    TFGK_CHECK_ARG(reduce >= TFGK_REDUCE_SUM && reduce <= TFGK_REDUCE_MAX, "spmm: unknown reduce %d", reduce);
-    TFGK_CHECK_ARG(act == TFGK_ACT_NONE || act == TFGK_ACT_RELU, "spmm: unknown activation %d", act);
-    if (n_dst == 0 || D == 0) return TFGK_OK;
-    TFGK_CHECK_ARG(rowptr && out && h, "spmm: null pointer");
-    TFGK_CHECK_ARG(ldh >= D && ldo >= D && (!addend || ld_addend >= D), "spmm: leading dimension < D");
+    bool nothing_to_do = true;
+    const int vrc = spmm_validate(rowptr, h, ldh, n_dst, D, reduce, addend, ld_addend, act, out, ldo, plan, &nothing_to_do);
+    if (vrc != TFGK_OK || nothing_to_do) return vrc;
 
     const bool vec4 = (D % 4 == 0) && (ldh % 4 == 0) && (ldo % 4 == 0) && aligned16(h) && aligned16(out) &&
                       (!addend || ((ld_addend % 4 == 0) && aligned16(addend))) && (!bias || aligned16(bias));
     const int vec = vec4 ? 4 : 1;
     const int cols_per_launch = 128 * vec;   // 32 lanes x NC<=4 vectors
     for (int c0 = 0; c0 < D; c0 += cols_per_launch) {
-        SpmmParams p;
-        p.rowptr = rowptr; p.col = col; p.w = w;
-        p.h = h + c0; p.ldh = ldh; p.n_dst = n_dst;
-        p.D = (D - c0 < cols_per_launch) ? D - c0 : cols_per_launch;
-        p.reduce = reduce; p.alpha = alpha;
-        p.addend = addend ? addend + c0 : nullptr; p.ld_addend = ld_addend; p.beta = beta;
-        p.bias = bias ? bias + c0 : nullptr; p.act = act;
-        p.out = out + c0; p.ldo = ldo;
-        p.n_tasks = 0; p.task_row = nullptr; p.task_nrows = nullptr; p.task_e0 = nullptr; p.task_e1 = nullptr;
-        p.task_slot = nullptr; p.n_hubs = 0; p.hub_row = nullptr; p.hub_slot0 = nullptr; p.hub_nslots = nullptr;
-        p.scratch = nullptr;
+        SpmmParams p = spmm_params(rowptr, col, w, ldh, n_dst, reduce, alpha, addend, ld_addend, beta, bias, act, out, ldo,
+                                   c0, (D - c0 < cols_per_launch) ? D - c0 : cols_per_launch);
+        p.h = h + c0;
         // the plan applies when the whole width runs in one launch of the streaming kernel (scratch rows are D wide)
         const bool use_plan = plan != nullptr && plan->n_tasks > 0 && vec4 && D >= 32 && D <= cols_per_launch &&
                               (spmm_impl_choice() >= 3);
-        if (use_plan) {
-            p.n_tasks = plan->n_tasks; p.task_row = plan->task_row; p.task_nrows = plan->task_nrows;
-            p.task_e0 = plan->task_e0; p.task_e1 = plan->task_e1; p.task_slot = plan->task_slot;
-            p.n_hubs = plan->n_hubs; p.hub_row = plan->hub_row; p.hub_slot0 = plan->hub_slot0;
-            p.hub_nslots = plan->hub_nslots; p.scratch = plan->scratch;
-        }
+        if (use_plan) spmm_use_plan(p, plan);
         const int lanes = (p.D + vec - 1) / vec;
         const int choice = spmm_impl_choice() == 5 ? (spmm_prefers_tma4(p.D) ? 4 : 3) : spmm_impl_choice();
         if (vec4 && p.D >= 32 && choice == 4) {
@@ -1067,6 +1111,49 @@ extern "C" int tfgk_spmm_f32(const int64_t *rowptr, const int32_t *col, const fl
             if (rcb != TFGK_ERR_UNSUPPORTED) { if (rcb != TFGK_OK) return rcb; continue; }
         }
         const int rc = vec4 ? dispatch_spmm<4>(p, lanes, as_stream(stream)) : dispatch_spmm<1>(p, lanes, as_stream(stream));
+        if (rc != TFGK_OK) return rc;
+    }
+    return TFGK_OK;
+}
+
+// bf16 rows.  The kernels are the fp32 ones with each element widened on the way from shared memory (or from global
+// memory on the scalar path), with the same lane-to-column mapping, plan and order of operations: the output is the
+// fp32 kernel's output over a widened table with the same leading dimension, bit for bit.  The rings (and the plan) need
+// 8-byte aligned rows of D % 4 == 0 elements, 32 <= D <= 512, where the fp32 kernel needs 16-byte aligned ones: the two
+// layouts correspond element for element, so both take the plan for the same shapes.
+extern "C" int tfgk_spmm_bf16(const int64_t *rowptr, const int32_t *col, const float *w,
+                              const uint16_t *h, int64_t ldh, int32_t n_dst, int32_t D, int reduce,
+                              float alpha, const float *addend, int64_t ld_addend, float beta,
+                              const float *bias, int act,
+                              float *out, int64_t ldo, const tfgk_plan *plan, void *stream) {
+    bool nothing_to_do = true;
+    const int vrc = spmm_validate(rowptr, h, ldh, n_dst, D, reduce, addend, ld_addend, act, out, ldo, plan, &nothing_to_do);
+    if (vrc != TFGK_OK || nothing_to_do) return vrc;
+
+    // rows4: every lane moves four consecutive columns (8 bytes of h, 16 bytes of out / addend / bias)
+    const bool rows4 = (D % 4 == 0) && (ldh % 4 == 0) && aligned8(h) && (ldo % 4 == 0) && aligned16(out) &&
+                       (!addend || ((ld_addend % 4 == 0) && aligned16(addend))) && (!bias || aligned16(bias));
+    cudaStream_t st = as_stream(stream);
+    if (rows4 && D >= 32 && D <= 512) {                // the ring kernels: one launch over the whole width
+        SpmmParams p = spmm_params(rowptr, col, w, ldh, n_dst, reduce, alpha, addend, ld_addend, beta, bias, act, out, ldo,
+                                   0, D);
+        p.hb = h;
+        // the plan is taken exactly when the fp32 entry point takes it for the same shape (TFGK_SPMM_IMPL included)
+        if (plan != nullptr && plan->n_tasks > 0 && spmm_impl_choice() >= 3) spmm_use_plan(p, plan);
+        // 256-byte rows at D = 128: six ring stages keep as many bytes in flight per warp as three stages of fp32 rows
+        const int rc = launch_spmm_tma4<6, uint16_t>(p, st);        // TFGK_ERR_UNSUPPORTED unless 16-byte rows, D <= 256
+        if (rc != TFGK_ERR_UNSUPPORTED) return rc;
+        const int lanes = (D + 3) / 4;
+        return lanes <= 32 ? launch_spmm_async<1, 4, 3, uint16_t>(p, st)
+             : lanes <= 64 ? launch_spmm_async<2, 4, 4, uint16_t>(p, st)
+             : lanes <= 96 ? launch_spmm_async<3, 4, 3, uint16_t>(p, st)
+                           : launch_spmm_async<4, 2, 4, uint16_t>(p, st);
+    }
+    for (int c0 = 0; c0 < D; c0 += 128) {               // scalar path: 32 lanes x 4 single columns per launch
+        SpmmParams p = spmm_params(rowptr, col, w, ldh, n_dst, reduce, alpha, addend, ld_addend, beta, bias, act, out, ldo,
+                                   c0, D - c0 < 128 ? D - c0 : 128);
+        p.hb = h + c0;
+        const int rc = dispatch_spmm<1, uint16_t>(p, p.D, st);
         if (rc != TFGK_OK) return rc;
     }
     return TFGK_OK;

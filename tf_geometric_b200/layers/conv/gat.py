@@ -16,15 +16,18 @@ class GAT(Layer):
 
     def __init__(self, units, attention_units=None, activation=None, use_bias=True, num_heads=1,
                  split_value_heads=True, query_activation=ops.relu, key_activation=ops.relu, edge_drop_rate=0.0,
-                 kernel_regularizer=None, bias_regularizer=None, *args, **kwargs):
+                 kernel_regularizer=None, bias_regularizer=None, *args, message_dtype=None, **kwargs):
         """
         :param units: output width
         :param attention_units: width of the query / key projections (default: units); must divide by num_heads
         :param num_heads: attention heads; split_value_heads=True concatenates per-head slices of the values,
             False lets every head see full-width values and averages the heads
         :param edge_drop_rate: dropout on the attention coefficients while training
+        :param message_dtype: None / torch.float32, or torch.bfloat16 for inference with bf16 keys and values (nn.gat)
         """
         super().__init__(*args, **kwargs)
+        ops.message_dtype(message_dtype)          # ValueError for anything but fp32 / bf16
+        self.message_dtype = message_dtype
         for slot in _WEIGHT_SLOTS:                  # declared up front like the reference, created lazily in build()
             setattr(self, slot, None)
         self.units, self.num_heads, self.split_value_heads = units, num_heads, split_value_heads
@@ -55,6 +58,8 @@ class GAT(Layer):
         several GPUs [x_local, partitioned_graph] (tf_geometric_b200.dist.PartitionedGraph)."""
         if hasattr(inputs[1], "part") and hasattr(inputs[1], "project_all_rows"):
             from ... import dist as tdist
+            if ops.message_dtype(self.message_dtype) is not None:
+                raise NotImplementedError("message_dtype=bfloat16 is not implemented for partitioned graphs")
             if not self.split_value_heads:
                 raise NotImplementedError("partitioned GAT concatenates the heads (split_value_heads=True)")
             return tdist.gat_partitioned(inputs[1], inputs[0], self.query_kernel, self.query_bias, self.query_activation,
@@ -63,4 +68,4 @@ class GAT(Layer):
         return gat(inputs[0], inputs[1], self.query_kernel, self.query_bias, self.query_activation, self.key_kernel,
                    self.key_bias, self.key_activation, self.kernel, self.bias, self.activation, num_heads=self.num_heads,
                    split_value_heads=self.split_value_heads, edge_drop_rate=self.edge_drop_rate, training=bool(training),
-                   cache=cache)
+                   cache=cache, message_dtype=self.message_dtype)

@@ -26,7 +26,8 @@ def gat(x, edge_index,
         query_kernel, query_bias, query_activation,
         key_kernel, key_bias, key_activation,
         kernel, bias=None, activation=None, num_heads=1,
-        split_value_heads=True, edge_drop_rate=0.0, training=False, cache=None, return_attention=False, seed=None):
+        split_value_heads=True, edge_drop_rate=0.0, training=False, cache=None, return_attention=False, seed=None,
+        message_dtype=None):
     """
     :param x: [num_nodes, num_features]
     :param edge_index: [2, num_edges]; self loops are appended (never de-duplicated), reference gat.py:43
@@ -38,8 +39,19 @@ def gat(x, edge_index,
     :param edge_drop_rate: dropout on the attention coefficients while training (gat.py:85)
     :param cache: optional dict (e.g. graph.cache) memoising the self-looped CSR; an extension of the reference API
     :param seed: optional 64-bit key pinning the dropout mask (extension; default: a fresh key per call)
+    :param message_dtype: None / torch.float32 (default), or torch.bfloat16: inference with K and V stored in bf16 (rounded
+        once, to nearest even, by the projection that also writes the fp32 Q) and read from half the bytes; scores,
+        softmax, accumulation and output stay fp32.  An extension of the reference API
     :return: [num_nodes, units]
     """
+    bf16 = ops.message_dtype(message_dtype) is not None
+    if bf16:
+        if as_sparse_features(x) is not None:
+            raise NotImplementedError("message_dtype=bfloat16 takes a dense x")
+        if training and edge_drop_rate > 0.0:
+            raise NotImplementedError("message_dtype=bfloat16 is for inference: attention dropout is not applied in bf16")
+        if return_attention:
+            raise NotImplementedError("message_dtype=bfloat16 does not return attention coefficients")
     edge_index = ops.as_device(edge_index, torch.int32)
     dev = edge_index.device
     x_sparse = as_sparse_features(x)             # tf.SparseTensor features (reference gat.py:45-70)
@@ -70,6 +82,8 @@ def gat(x, edge_index,
         h = leftover(h) if leftover is not None else h
         return (h, ops.permute(att, csr.perm, inverse=True)) if return_attention else h
     if drop_rate > 0.0 or autograd.needs_grad(x, query_kernel, query_bias, key_kernel, key_bias, kernel, bias):
+        if bf16:
+            raise NotImplementedError("message_dtype=bfloat16 is for inference: no operand may require grad")
         if return_attention:
             raise NotImplementedError("return_attention is an inference-path extension")
         return _gat_training(x, csr, edge_index_used, query_kernel, query_bias, query_activation, key_kernel, key_bias,
@@ -85,15 +99,21 @@ def gat(x, edge_index,
     wv = ops.as_device(kernel, torch.float32, device=dev)
     a_units = wk.shape[1]
     Q = torch.empty((num_nodes, wq.shape[1]), dtype=torch.float32, device=dev)
-    kv = torch.empty((num_nodes, a_units + wv.shape[1]), dtype=torch.float32, device=dev)
+    # bf16 messages: the projection rounds K | V in its epilogue; Q stays fp32
+    kv = torch.empty((num_nodes, a_units + wv.shape[1]), dtype=torch.bfloat16 if bf16 else torch.float32, device=dev)
     K, V = kv[:, :a_units], kv[:, a_units:]
+    # a key activation the projection cannot fuse is applied in fp32 before the keys are rounded
+    K_f32 = torch.empty((num_nodes, a_units), dtype=torch.float32, device=dev) if bf16 and k_left is not None else K
     project(x, [(wq, ops.as_device(query_bias, torch.float32, device=dev), q_act, Q),
-                (wk, ops.as_device(key_bias, torch.float32, device=dev), k_act, K),
+                (wk, ops.as_device(key_bias, torch.float32, device=dev), k_act, K_f32),
                 (wv, None, ops.ACT_NONE, V)])
     if q_left is not None:
         Q = q_left(Q)
     if k_left is not None:
-        K.copy_(k_left(K))
+        if K_f32 is K:
+            K.copy_(k_left(K))
+        else:
+            ops.round_bf16(k_left(K_f32), out=K)
 
     act_code, leftover = ops.activation_code(activation)
     bias = None if bias is None else ops.as_device(bias, torch.float32, device=dev)

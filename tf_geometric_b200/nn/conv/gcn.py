@@ -119,7 +119,7 @@ def gcn_norm_edge(edge_index, num_nodes, edge_weight=None, renorm=True, improved
 
 def gcn(x, sparse_adj, kernel, bias=None, activation=None,
         norm="both", add_self_loop=True, sym=True, renorm=True, improved=False, edge_drop_rate=0.0,
-        num_or_size_splits=None, training=False, cache=None):
+        num_or_size_splits=None, training=False, cache=None, message_dtype=None):
     """
     Functional GCN layer (reference gcn.py:225-290).
 
@@ -130,8 +130,14 @@ def gcn(x, sparse_adj, kernel, bias=None, activation=None,
     :param activation: callable or None; relu is fused into the aggregation epilogue
     :param num_or_size_splits: column chunks of the propagation (gcn.py:274-280): one launch per chunk into slices of one
         output, same bits (the fused kernel has no [E, D] temporary to bound, so this is an API-parity feature)
+    :param message_dtype: None / torch.float32 (default), or torch.bfloat16: inference with x W stored in bf16 (rounded
+        once, to nearest even, by the projection) and aggregated from half the bytes in fp32; the output is fp32.  An
+        extension of the reference API
     :return: [num_nodes, units]
     """
+    if ops.message_dtype(message_dtype) is not None:
+        return _gcn_bf16(x, sparse_adj, kernel, bias, activation, norm, add_self_loop, sym, renorm, improved, edge_drop_rate,
+                         num_or_size_splits, training, cache)
     normed = gcn_norm_adj(sparse_adj, norm=norm, add_self_loop=add_self_loop, sym=sym, renorm=renorm,
                           improved=improved, cache=cache)
     normed = normed.dropout(edge_drop_rate, training=training)
@@ -163,3 +169,29 @@ def gcn(x, sparse_adj, kernel, bias=None, activation=None,
     if leftover is not None:
         h = leftover(h)
     return h
+
+
+def _gcn_bf16(x, sparse_adj, kernel, bias, activation, norm, add_self_loop, sym, renorm, improved, edge_drop_rate,
+              num_or_size_splits, training, cache):
+    """gcn() with bf16 message rows: act(norm(A) @ bf16(x W) + b), the product over the widened rows in fp32."""
+    from .gat import project
+    if as_sparse_features(x) is not None:
+        raise NotImplementedError("message_dtype=bfloat16 takes a dense x")
+    if training and edge_drop_rate > 0.0:
+        raise NotImplementedError("message_dtype=bfloat16 is for inference: edge dropout is not applied in bf16")
+    normed = gcn_norm_adj(sparse_adj, norm=norm, add_self_loop=add_self_loop, sym=sym, renorm=renorm,
+                          improved=improved, cache=cache)
+    dev = normed.index.device
+    x = ops.as_device(x, torch.float32, device=dev)
+    if autograd.needs_grad(x, kernel, bias, normed.value):
+        raise NotImplementedError("message_dtype=bfloat16 is for inference: no operand may require grad")
+    act_code, leftover = ops.activation_code(activation)
+    bias = None if bias is None else ops.as_device(bias, torch.float32, device=dev)
+    if kernel is None:
+        h = ops.round_bf16(x)
+    else:
+        kernel = ops.as_device(kernel, torch.float32, device=dev)
+        h = torch.empty((x.shape[0], kernel.shape[1]), dtype=torch.bfloat16, device=dev)
+        project(x, [(kernel, None, ops.ACT_NONE, h)])
+    h = normed.matmul(h, num_or_size_splits=num_or_size_splits, bias=bias, act=act_code)
+    return leftover(h) if leftover is not None else h

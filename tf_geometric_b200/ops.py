@@ -269,13 +269,25 @@ def scale_edges(row, col, w, dl=None, dr=None):
 
 # ---- K1 ----------------------------------------------------------------------------------------------------------
 
-def spmm(csr, w_csr, h, reduce="sum", alpha=1.0, addend=None, beta=0.0, bias=None, act=ACT_NONE, out=None, col=None):
+def spmm(csr, w_csr, h, reduce="sum", alpha=1.0, addend=None, beta=0.0, bias=None, act=ACT_NONE, out=None, col=None,
+         keep_layout=False):
     """out = epilogue(REDUCE_{e in row} w[e] * h[col[e]]); see tfgk_spmm_f32.  `col` overrides csr.col (used by the
-    generic reducers, which gather message rows through csr.perm)."""
-    if h.dtype != torch.float32 or not h.is_cuda:
-        raise TypeError("h must be a float32 CUDA tensor")
+    generic reducers, which gather message rows through csr.perm).  h may be bfloat16 (tfgk_spmm_bf16): the output is
+    fp32 and bit-identical to the product over h.float(), also for strided or unaligned views of h.  With keep_layout=True
+    a bf16 view is read in place, and the result is instead that of the fp32 product over a widened view with the same
+    layout (the column chunks of SparseMatrix.matmul)."""
+    if h.dtype not in (torch.float32, torch.bfloat16) or not h.is_cuda:
+        raise TypeError("h must be a float32 or bfloat16 CUDA tensor")
     ldh = _row_major_2d(h, "h")
     n_dst, D = csr.n_rows, h.shape[1]
+    plan = getattr(csr, "plan", None)
+    if h.dtype == torch.bfloat16 and not keep_layout and plan is not None and plan.n_hubs > 0 and D % 4 == 0 and \
+            32 <= D <= 512 and (ldh % 4 or h.data_ptr() % 8):
+        # rows that are not 8-byte aligned take tfgk_spmm_bf16's scalar path, which sums hub rows strictly in order; the
+        # fp32 kernel over h.float() (contiguous) slices them through the plan.  A dense copy takes the ring with the plan,
+        # so that the result stays bit-identical to the product over h.float()
+        h = h.clone(memory_format=torch.contiguous_format)
+        ldh = _row_major_2d(h, "h")
     if out is None:
         out = torch.empty((n_dst, D), dtype=torch.float32, device=h.device)
     ldo = _row_major_2d(out, "out")
@@ -287,9 +299,9 @@ def spmm(csr, w_csr, h, reduce="sum", alpha=1.0, addend=None, beta=0.0, bias=Non
     if bias is not None:
         _check(bias, torch.float32, "bias")
     code = _REDUCE_CODES[reduce] if isinstance(reduce, str) else reduce
-    plan = getattr(csr, "plan", None)
     plan_struct = plan.struct(D, h.device) if plan is not None else None
-    _ffi.call("tfgk_spmm_f32", _p(csr.rowptr), _p(csr.col if col is None else col), _p(w_csr), _p(h), ldh, n_dst, D,
+    _ffi.call("tfgk_spmm_bf16" if h.dtype == torch.bfloat16 else "tfgk_spmm_f32", _p(csr.rowptr),
+              _p(csr.col if col is None else col), _p(w_csr), _p(h), ldh, n_dst, D,
               code, float(alpha), _p(addend), lda, float(beta), _p(bias), act, _p(out), ldo,
               ctypes.byref(plan_struct) if plan_struct is not None else None, _stream(h))
     return out
@@ -308,9 +320,15 @@ def segment_softmax_csr(csr, score_csr):
 
 def gat_fused(csr, Q, K, V, num_heads, split_value_heads=True, bias=None, act=ACT_NONE, return_attention=False,
               att_buffer=None, out=None, scale=None):
-    for t, n in ((Q, "Q"), (K, "K"), (V, "V")):
-        if not (t.is_cuda and t.dtype == torch.float32):
-            raise TypeError("{} must be a float32 CUDA tensor".format(n))
+    """Fused GAT attention (tfgk_gat_fused_f32).  K and V may both be bfloat16 (tfgk_gat_fused_bf16, inference only:
+    no return_attention); Q and the output stay float32."""
+    bf16 = K.dtype == torch.bfloat16
+    for t, n, dt in ((Q, "Q", torch.float32), (K, "K", K.dtype), (V, "V", K.dtype)):
+        if not (t.is_cuda and t.dtype == dt and dt in (torch.float32, torch.bfloat16)):
+            raise TypeError("{} must be a {} CUDA tensor (Q float32; K and V both float32 or both bfloat16)".format(
+                n, "float32" if n == "Q" else "float32 or bfloat16"))
+    if bf16 and return_attention:
+        raise NotImplementedError("gat_fused: bfloat16 K and V are an inference mode without attention coefficients")
     N = csr.n_rows
     H = int(num_heads)
     A, VW = Q.shape[1], V.shape[1]
@@ -334,7 +352,8 @@ def gat_fused(csr, Q, K, V, num_heads, split_value_heads=True, bias=None, act=AC
     plan_struct = plan.struct(VW + 64, Q.device) if plan is not None else None
 
     def launch(att_buf):
-        _ffi.call("tfgk_gat_fused_f32", _p(csr.rowptr), _p(csr.col), _p(Q), _row_major_2d(Q, "Q"), _p(K),
+        _ffi.call("tfgk_gat_fused_bf16" if bf16 else "tfgk_gat_fused_f32", _p(csr.rowptr), _p(csr.col), _p(Q),
+                  _row_major_2d(Q, "Q"), _p(K),
                   _row_major_2d(K, "K"), _p(V), _row_major_2d(V, "V"), N, H, dqk, dv, scale,
                   1 if split_value_heads else 0, _p(bias), act, _p(att_buf), 1 if return_attention else 0, _p(out),
                   _row_major_2d(out, "out"), ctypes.byref(plan_struct) if plan_struct is not None else None, _stream(Q))
@@ -838,7 +857,8 @@ def gemm(a, b, bias=None, act=ACT_NONE, trans_a=False, trans_b=False, beta=0.0, 
 
 def gemm_proj(a, blocks, a_parts=None, part_rows=0, first_part=0, max_ctas=0, num_rows=None):
     """Several projections of the same rows in ONE launch (tfgk_gemm_proj_f32): `blocks` is a list of
-    (weight [K, n<=128], bias or None, act code, out [M, n] view); returns the list of outputs.
+    (weight [K, n<=128], bias or None, act code, out [M, n] view); returns the list of outputs.  An `out` may be bfloat16
+    (tfgk_gemm_proj_mixed, single-part input): it receives the fp32 result rounded to nearest even.
     With `a_parts` (device pointers of the row blocks of A, `part_rows` rows each, e.g. the other ranks' copies of x
     mapped through peer memory) the rows are pulled from where they live; `a` then only supplies lda / K / the stream.
     Shapes the tensor-core kernel does not take fall back to one tfgk_gemm_f32 per block (single-part input only)."""
@@ -847,7 +867,7 @@ def gemm_proj(a, blocks, a_parts=None, part_rows=0, first_part=0, max_ctas=0, nu
     lda = _row_major_2d(a, "a")
     M = int(a.shape[0] if num_rows is None else num_rows)
     K = a.shape[1]
-    structs = (_ffi.ProjBlock * len(blocks))()
+    fields = []
     outs = []
     for i, blk in enumerate(blocks):
         w, bias, act, out = blk[:4]
@@ -858,12 +878,22 @@ def gemm_proj(a, blocks, a_parts=None, part_rows=0, first_part=0, max_ctas=0, nu
         n_cols = w.shape[n_dim]
         if out is None:
             out = torch.empty((M, n_cols), dtype=torch.float32, device=a.device)
+        if not (out.is_cuda and out.dtype in (torch.float32, torch.bfloat16)):
+            raise TypeError("gemm_proj: out {} must be a float32 or bfloat16 CUDA tensor".format(i))
         if bias is not None:
             _check(bias, torch.float32, "bias")
-        structs[i] = _ffi.ProjBlock(w.data_ptr(), _row_major_2d(w, "weight"), n_cols, 1 if trans_b else 0,
-                                    None if bias is None else bias.data_ptr(), int(act), out.data_ptr(),
-                                    _row_major_2d(out, "out"))
+        fields.append((w.data_ptr(), _row_major_2d(w, "weight"), n_cols, 1 if trans_b else 0,
+                       None if bias is None else bias.data_ptr(), int(act), out.data_ptr(), _row_major_2d(out, "out")))
         outs.append(out)
+    mixed = any(out.dtype == torch.bfloat16 for out in outs)
+    if mixed:
+        if a_parts is not None:
+            raise ValueError("gemm_proj: bfloat16 outputs need a single-part input")
+        structs = (_ffi.ProjBlockOut * len(blocks))(*[
+            _ffi.ProjBlockOut(*(f + (_ffi.DTYPE_BF16 if out.dtype == torch.bfloat16 else _ffi.DTYPE_F32,)))
+            for f, out in zip(fields, outs)])
+    else:
+        structs = (_ffi.ProjBlock * len(blocks))(*[_ffi.ProjBlock(*f) for f in fields])
     if a_parts is None:
         parts = (ctypes.c_void_p * 1)(a.data_ptr())
         n_parts = 1
@@ -871,14 +901,41 @@ def gemm_proj(a, blocks, a_parts=None, part_rows=0, first_part=0, max_ctas=0, nu
         parts = (ctypes.c_void_p * len(a_parts))(*[int(q) for q in a_parts])
         n_parts = len(a_parts)
     try:
-        _ffi.call("tfgk_gemm_proj_f32", parts, n_parts, int(part_rows), lda, M, K, structs, len(blocks), int(first_part),
-                  int(max_ctas), _stream(a))
+        _ffi.call("tfgk_gemm_proj_mixed" if mixed else "tfgk_gemm_proj_f32", parts, n_parts, int(part_rows), lda, M, K,
+                  structs, len(blocks), int(first_part), int(max_ctas), _stream(a))
     except _ffi.TfgkError as err:
         if err.code != _ffi.ERR_UNSUPPORTED or n_parts != 1:
             raise
         for blk, out in zip(blocks, outs):
-            gemm(a[:M], blk[0], bias=blk[1], act=blk[2], trans_b=bool(blk[4]) if len(blk) > 4 else False, out=out)
+            tb = bool(blk[4]) if len(blk) > 4 else False
+            if out.dtype == torch.bfloat16:     # the fp32 product, then rounded to nearest even
+                round_bf16(gemm(a[:M], blk[0], bias=blk[1], act=blk[2], trans_b=tb), out=out)
+            else:
+                gemm(a[:M], blk[0], bias=blk[1], act=blk[2], trans_b=tb, out=out)
     return outs
+
+
+def round_bf16(src, out=None):
+    """bfloat16 copy of a 2-D float32 CUDA tensor, rounded to nearest even (tfgk_round_bf16); `out` may be a view."""
+    if not (src.is_cuda and src.dtype == torch.float32 and src.dim() == 2):
+        raise TypeError("round_bf16: src must be a 2-D float32 CUDA tensor")
+    if out is None:
+        out = torch.empty(tuple(src.shape), dtype=torch.bfloat16, device=src.device)
+    if not (out.is_cuda and out.dtype == torch.bfloat16 and tuple(out.shape) == tuple(src.shape)):
+        raise TypeError("round_bf16: out must be a bfloat16 CUDA tensor of shape {}".format(tuple(src.shape)))
+    _ffi.call("tfgk_round_bf16", _p(src), _row_major_2d(src, "src"), src.shape[0], src.shape[1], _p(out),
+              _row_major_2d(out, "out"), _stream(src))
+    return out
+
+
+def message_dtype(value):
+    """Storage type of the rows a layer gathers along edges: None / torch.float32 -> None (fp32, the default path),
+    torch.bfloat16 / "bfloat16" -> torch.bfloat16; anything else raises ValueError."""
+    if value is None or value is torch.float32 or value == "float32":
+        return None
+    if value is torch.bfloat16 or value == "bfloat16":
+        return torch.bfloat16
+    raise ValueError("message_dtype must be None, torch.float32 or torch.bfloat16 (got {!r})".format(value))
 
 
 def colsum(x):

@@ -118,9 +118,15 @@ class SparseMatrix(object):
         """A @ h (gcn.py:280).  `num_or_size_splits` (tf.split semantics: a count of equal column chunks or a list of
         chunk widths, utils/tf_sparse_utils.py:71-90) runs one launch per column chunk into slices of one output, like the
         reference's split -> matmul -> concat; the fused kernel has no [E, D] temporary to bound, so the results are the
-        same bits with or without it."""
-        h = ops.as_device(h, torch.float32, device=self.index.device)
+        same bits with or without it.  A bfloat16 h stays bfloat16 and is gathered as such (tfgk_spmm_bf16) when no operand
+        (h, bias, the values) needs a gradient: the float32 result is bit-identical to the product over h.float(), from
+        half the row bytes."""
         from . import autograd
+        # the differentiable route below works in fp32 (its backward products take fp32 operands): a bf16 h is widened
+        # for it, as it always was
+        keep_bf16 = torch.is_tensor(h) and h.dtype == torch.bfloat16 and \
+            not autograd.needs_grad(h, epilogue.get("bias"), self.value)
+        h = ops.as_device(h, torch.bfloat16 if keep_bf16 else torch.float32, device=self.index.device)
         if autograd.needs_grad(h, epilogue.get("bias"), self.value):
             # `A @ h` inside a user's training loop (tf_sparse products are differentiable under tf.GradientTape, in h and
             # in A's values): the same kernel behind autograd (dh = A^T g over the transposed structure, d value by K7);
@@ -143,6 +149,9 @@ class SparseMatrix(object):
         if out is None:
             out = torch.empty((self._shape[0], d), dtype=torch.float32, device=h.device)
         bias, addend = epilogue.pop("bias", None), epilogue.pop("addend", None)
+        if h.dtype == torch.bfloat16:
+            # each chunk is read in place, so it matches the fp32 chunk of h.float() (same layout, same use of the plan)
+            epilogue["keep_layout"] = True
         c0 = 0
         for width in sizes:
             c1 = c0 + width
