@@ -160,6 +160,22 @@ int tfgk_spmm_bf16(const int64_t *rowptr, const int32_t *col, const float *w,
                    float alpha, const float *addend, int64_t ld_addend, float beta,
                    const float *bias, int act,
                    float *out, int64_t ldo, const tfgk_plan *plan, void *stream);
+/* tfgk_spmm_bf16 that stores its fp32 result (after alpha / addend / bias / activation) in `out` and/or, rounded to
+ * nearest even, in the bf16 table `out_bf16` ([n_dst, D], leading dimension ldob): either may be NULL, not both.  `out`
+ * is bit-identical to what tfgk_spmm_bf16 writes with the same arguments, and out_bf16 to tfgk_round_bf16 of it (inf and
+ * NaN stay inf and NaN, finite values beyond the bf16 range become inf); with out == NULL, to tfgk_spmm_bf16 into a dense
+ * fp32 out.  A multi-hop chain thus writes its intermediate hops as 2 bytes per element, ready for the next gather.
+ * Padded tables: rows 16-byte aligned with ldh % 8 == 0 and ldh >= D rounded up to 8 (8-byte aligned, ldh >= D rounded
+ * up to 4) may be read with their pad columns, so that the TMA (cp.async) ring runs for any D; pad columns are computed
+ * and never stored, and do not interact with the first D.  A plan is used exactly where tfgk_spmm_bf16 uses it.  h and
+ * out_bf16 must be 2-byte aligned and out 4-byte aligned.  Algorithmic bytes: E*(2*D + 4 [+4 weighted]) + N*(4*D + 8)
+ * with both outputs, N*(2*D + 8) for the output side of a bf16-only store. */
+int tfgk_spmm_bf16_dual(const int64_t *rowptr, const int32_t *col, const float *w,
+                        const uint16_t *h, int64_t ldh, int32_t n_dst, int32_t D, int reduce,
+                        float alpha, const float *addend, int64_t ld_addend, float beta,
+                        const float *bias, int act,
+                        float *out, int64_t ldo, uint16_t *out_bf16, int64_t ldob,
+                        const tfgk_plan *plan, void *stream);
 
 /* ---- K3: edge softmax and fused GAT ------------------------------------------------------------------------- */
 

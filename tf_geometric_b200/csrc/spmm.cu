@@ -11,6 +11,7 @@
 //
 // Algorithmic bytes per launch (DESIGN.md): E*(4*D + 4 [+4 weighted]) + N*(4*D + 8).
 #include "common.cuh"
+#include <cuda_bf16.h>
 #include <stdlib.h>
 
 namespace tfgk {
@@ -61,8 +62,15 @@ struct SpmmParams {
     float beta;
     const float *bias;
     int act;
-    float *out;
+    float *out;            // may be nullptr in tfgk_spmm_bf16_dual (bf16 output only)
     int64_t ldo;
+    // tfgk_spmm_bf16_dual only (the kernels instantiated with DUAL): a bf16 copy of the output, the number of columns
+    // stored (D may include pad columns that are computed and never stored) and whether addend / bias / out / outb may
+    // be accessed four columns at a time
+    uint16_t *outb;
+    int64_t ldob;
+    int32_t d_store;
+    bool io4;
     // optional work plan (tfgk_plan): tasks + hub slices; task_row == nullptr -> implicit blocks of consecutive rows
     int32_t n_tasks;
     const int32_t *task_row, *task_nrows;
@@ -78,10 +86,60 @@ template <typename T> __device__ __forceinline__ const T *rows_of(const SpmmPara
 template <> __device__ __forceinline__ const float *rows_of<float>(const SpmmParams &p) { return p.h; }
 template <> __device__ __forceinline__ const uint16_t *rows_of<uint16_t>(const SpmmParams &p) { return p.hb; }
 
+// The epilogue of tfgk_spmm_bf16_dual for N consecutive columns c .. c+N-1 of row r: the arithmetic of every other
+// epilogue in this file (mean, axpby, bias, activation, in that order and rounding), then the value is stored in fp32
+// and/or rounded to nearest even into the bf16 copy.  Columns from p.d_store on are pad columns: never stored.
+template <int N>
+__device__ __forceinline__ void epilogue_dual(const SpmmParams &p, int64_t r, int c, const float (&acc)[N], float cnt) {
+    if (c >= p.d_store) return;
+    float ad[N], bs[N], o[N];
+    if constexpr (N == 4) {
+        if (p.io4) {                             // io4 implies d_store % 4 == 0: all four columns are stored
+            if (p.addend) load_vec<4>(p.addend + r * p.ld_addend + c, ad);
+            if (p.bias) load_vec<4>(p.bias + c, bs);
+        }
+    }
+    if (N != 4 || !p.io4) {
+#pragma unroll
+        for (int x = 0; x < N; ++x) {
+            if (c + x >= p.d_store) break;
+            if (p.addend) ad[x] = p.addend[r * p.ld_addend + c + x];
+            if (p.bias) bs[x] = p.bias[c + x];
+        }
+    }
+#pragma unroll
+    for (int x = 0; x < N; ++x) {
+        float a = acc[x];
+        if (p.reduce == TFGK_REDUCE_MEAN) a = __fdiv_rn(a, cnt);
+        if (p.addend) a = __fadd_rn(__fmul_rn(a, p.alpha), __fmul_rn(ad[x], p.beta));
+        else if (p.alpha != 1.0f) a = __fmul_rn(a, p.alpha);
+        if (p.bias) a = __fadd_rn(a, bs[x]);
+        o[x] = apply_act(a, p.act);
+    }
+    if constexpr (N == 4) {
+        if (p.io4) {
+            if (p.out) store_vec<4>(p.out + r * p.ldo + c, o);
+            if (p.outb) {
+                uint32_t b[4];
+#pragma unroll
+                for (int x = 0; x < 4; ++x) b[x] = __bfloat16_as_ushort(__float2bfloat16_rn(o[x]));
+                *reinterpret_cast<uint2 *>(p.outb + r * p.ldob + c) = make_uint2(b[0] | (b[1] << 16), b[2] | (b[3] << 16));
+            }
+            return;
+        }
+    }
+#pragma unroll
+    for (int x = 0; x < N; ++x) {
+        if (c + x >= p.d_store) break;
+        if (p.out) p.out[r * p.ldo + c + x] = o[x];
+        if (p.outb) p.outb[r * p.ldob + c + x] = __bfloat16_as_ushort(__float2bfloat16_rn(o[x]));
+    }
+}
+
 constexpr int kSpmmThreads = 256;
 
 // G: lanes per row (power of two), NC: vectors per lane, IS_MAX: max-reduce instead of sum/mean, U: rows in flight
-template <int VEC, int G, int NC, bool IS_MAX, int U, typename T>
+template <int VEC, int G, int NC, bool IS_MAX, int U, typename T, bool DUAL = false>
 __global__ void __launch_bounds__(kSpmmThreads) spmm_kernel(const SpmmParams p) {
     constexpr int RPW = 32 / G;   // rows per warp
     const int lane = threadIdx.x & 31;
@@ -170,6 +228,10 @@ __global__ void __launch_bounds__(kSpmmThreads) spmm_kernel(const SpmmParams p) 
 #pragma unroll
     for (int k = 0; k < NC; ++k) {
         if (!cok[k]) continue;
+        if constexpr (DUAL) {
+            epilogue_dual<VEC>(p, r, coff[k], acc[k], cnt);
+            continue;
+        }
         float o[VEC];
         float ad[VEC];
         float bs[VEC];
@@ -507,7 +569,7 @@ __device__ __forceinline__ void cp_async_slice(uint32_t dst, const uint16_t *src
     asm volatile("cp.async.ca.shared.global [%0], [%1], 8;" ::"r"(dst), "l"(src) : "memory");
 }
 
-template <int NC, bool IS_MAX, int U, int S, typename T>
+template <int NC, bool IS_MAX, int U, int S, typename T, bool DUAL = false>
 __global__ void __launch_bounds__(kAsyncWarps * 32) spmm_async_kernel(const SpmmParams p, uint32_t row_bytes) {
     static_assert(32 % U == 0, "a round must not straddle an index chunk");
     constexpr int RPC = 32 / U;
@@ -560,7 +622,11 @@ __global__ void __launch_bounds__(kAsyncWarps * 32) spmm_async_kernel(const Spmm
         const float cnt = (float)max(deg, 1);
 #pragma unroll
         for (int k = 0; k < NC; ++k) {
-            if (cok[k]) {
+            if (DUAL && cok[k]) {
+                epilogue_dual<4>(p, r, coff[k], acc[k], cnt);
+#pragma unroll
+                for (int x = 0; x < 4; ++x) acc[k][x] = IS_MAX ? -FLT_MAX : 0.0f;
+            } else if (cok[k]) {
                 float ad[4], bs[4], o[4];
                 if (p.addend) load_vec<4>(p.addend + r * p.ld_addend + coff[k], ad);
                 if (p.bias) load_vec<4>(p.bias + coff[k], bs);
@@ -683,7 +749,7 @@ __device__ __forceinline__ void tma_row(uint32_t dst, const void *src, uint32_t 
                  ::"r"(dst), "l"(src), "r"(bytes), "r"(bar) : "memory");
 }
 
-template <bool IS_MAX, int S, typename T>
+template <bool IS_MAX, int S, typename T, bool DUAL = false>
 __global__ void __launch_bounds__(kAsyncWarps * 32) spmm_tma4_kernel(const SpmmParams p, uint32_t row_bytes) {
     constexpr int U = 4, RPC = 32 / U;
     static_assert(S <= 2 * RPC, "weight look-ahead registers would be overwritten before they are consumed");
@@ -743,7 +809,11 @@ __global__ void __launch_bounds__(kAsyncWarps * 32) spmm_tma4_kernel(const SpmmP
         const float cnt = (float)max(deg, 1);
 #pragma unroll
         for (int k = 0; k < NCX; ++k) {
-            if (cok[k]) {
+            if (DUAL && cok[k]) {
+                epilogue_dual<4>(p, r, coff[k], acc[k], cnt);
+#pragma unroll
+                for (int x = 0; x < 4; ++x) acc[k][x] = IS_MAX ? -FLT_MAX : 0.0f;
+            } else if (cok[k]) {
                 float ad[4], bs[4], o[4];
                 if (p.addend) load_vec<4>(p.addend + r * p.ld_addend + coff[k], ad);
                 if (p.bias) load_vec<4>(p.bias + coff[k], bs);
@@ -844,7 +914,7 @@ __global__ void __launch_bounds__(kAsyncWarps * 32) spmm_tma4_kernel(const SpmmP
 }
 
 // merges the slices of every hub row in slice order (deterministic) and applies the epilogue; one warp per hub row
-template <bool IS_MAX>
+template <bool IS_MAX, bool DUAL = false>
 __global__ void __launch_bounds__(256) spmm_hub_fixup_kernel(const SpmmParams p) {
     const int lane = threadIdx.x & 31;
     const int h = blockIdx.x * 8 + (threadIdx.x >> 5);
@@ -859,6 +929,10 @@ __global__ void __launch_bounds__(256) spmm_hub_fixup_kernel(const SpmmParams p)
             load_vec<4>(p.scratch + (int64_t)(s0 + s) * p.D + c, v);
 #pragma unroll
             for (int x = 0; x < 4; ++x) acc[x] = IS_MAX ? fmaxf(acc[x], v[x]) : __fadd_rn(acc[x], v[x]);
+        }
+        if constexpr (DUAL) {
+            epilogue_dual<4>(p, r, c, acc, cnt);
+            continue;
         }
         float ad[4], bs[4], o[4];
         if (p.addend) load_vec<4>(p.addend + r * p.ld_addend + c, ad);
@@ -876,7 +950,7 @@ __global__ void __launch_bounds__(256) spmm_hub_fixup_kernel(const SpmmParams p)
     }
 }
 
-template <int NC, int U, int S, typename T = float>
+template <int NC, int U, int S, typename T = float, bool DUAL = false>
 static int launch_spmm_async(const SpmmParams &p, cudaStream_t st) {
     const uint32_t row_bytes = (uint32_t)(p.D * sizeof(T));
     const size_t smem = (size_t)kAsyncWarps * S * U * row_bytes;
@@ -884,23 +958,23 @@ static int launch_spmm_async(const SpmmParams &p, cudaStream_t st) {
     const int64_t n_tasks = p.task_row ? p.n_tasks : ceil_div64(p.n_dst, kAsyncRows);
     const unsigned blocks = (unsigned)ceil_div64(n_tasks, kAsyncWarps);
     if (p.reduce == TFGK_REDUCE_MAX) {
-        TFGK_CUDA(ensure_dynamic_smem(spmm_async_kernel<NC, true, U, S, T>, smem));
-        spmm_async_kernel<NC, true, U, S, T><<<blocks, kAsyncWarps * 32, smem, st>>>(p, row_bytes);
+        TFGK_CUDA(ensure_dynamic_smem(spmm_async_kernel<NC, true, U, S, T, DUAL>, smem));
+        spmm_async_kernel<NC, true, U, S, T, DUAL><<<blocks, kAsyncWarps * 32, smem, st>>>(p, row_bytes);
     } else {
-        TFGK_CUDA(ensure_dynamic_smem(spmm_async_kernel<NC, false, U, S, T>, smem));
-        spmm_async_kernel<NC, false, U, S, T><<<blocks, kAsyncWarps * 32, smem, st>>>(p, row_bytes);
+        TFGK_CUDA(ensure_dynamic_smem(spmm_async_kernel<NC, false, U, S, T, DUAL>, smem));
+        spmm_async_kernel<NC, false, U, S, T, DUAL><<<blocks, kAsyncWarps * 32, smem, st>>>(p, row_bytes);
     }
     TFGK_LAUNCH_CHECK();
     if (p.task_row && p.n_hubs > 0) {
         const unsigned fb = (unsigned)ceil_div64(p.n_hubs, 8);
-        if (p.reduce == TFGK_REDUCE_MAX) spmm_hub_fixup_kernel<true><<<fb, 256, 0, st>>>(p);
-        else spmm_hub_fixup_kernel<false><<<fb, 256, 0, st>>>(p);
+        if (p.reduce == TFGK_REDUCE_MAX) spmm_hub_fixup_kernel<true, DUAL><<<fb, 256, 0, st>>>(p);
+        else spmm_hub_fixup_kernel<false, DUAL><<<fb, 256, 0, st>>>(p);
         TFGK_LAUNCH_CHECK();
     }
     return TFGK_OK;
 }
 
-template <int S, typename T = float>
+template <int S, typename T = float, bool DUAL = false>
 static int launch_spmm_tma4(const SpmmParams &p, cudaStream_t st) {
     // cp.async.bulk wants 16-byte aligned rows: D, ldh multiples of 16 bytes' worth of elements and an aligned base
     constexpr int kPer16 = 16 / (int)sizeof(T);
@@ -913,17 +987,17 @@ static int launch_spmm_tma4(const SpmmParams &p, cudaStream_t st) {
     const int64_t n_tasks = p.task_row ? p.n_tasks : ceil_div64(p.n_dst, kAsyncRows);
     const unsigned blocks = (unsigned)ceil_div64(n_tasks, kAsyncWarps);
     if (p.reduce == TFGK_REDUCE_MAX) {
-        TFGK_CUDA(ensure_dynamic_smem(spmm_tma4_kernel<true, S, T>, smem));
-        spmm_tma4_kernel<true, S, T><<<blocks, kAsyncWarps * 32, smem, st>>>(p, row_bytes);
+        TFGK_CUDA(ensure_dynamic_smem(spmm_tma4_kernel<true, S, T, DUAL>, smem));
+        spmm_tma4_kernel<true, S, T, DUAL><<<blocks, kAsyncWarps * 32, smem, st>>>(p, row_bytes);
     } else {
-        TFGK_CUDA(ensure_dynamic_smem(spmm_tma4_kernel<false, S, T>, smem));
-        spmm_tma4_kernel<false, S, T><<<blocks, kAsyncWarps * 32, smem, st>>>(p, row_bytes);
+        TFGK_CUDA(ensure_dynamic_smem(spmm_tma4_kernel<false, S, T, DUAL>, smem));
+        spmm_tma4_kernel<false, S, T, DUAL><<<blocks, kAsyncWarps * 32, smem, st>>>(p, row_bytes);
     }
     TFGK_LAUNCH_CHECK();
     if (p.task_row && p.n_hubs > 0) {
         const unsigned fb = (unsigned)ceil_div64(p.n_hubs, 8);
-        if (p.reduce == TFGK_REDUCE_MAX) spmm_hub_fixup_kernel<true><<<fb, 256, 0, st>>>(p);
-        else spmm_hub_fixup_kernel<false><<<fb, 256, 0, st>>>(p);
+        if (p.reduce == TFGK_REDUCE_MAX) spmm_hub_fixup_kernel<true, DUAL><<<fb, 256, 0, st>>>(p);
+        else spmm_hub_fixup_kernel<false, DUAL><<<fb, 256, 0, st>>>(p);
         TFGK_LAUNCH_CHECK();
     }
     return TFGK_OK;
@@ -992,36 +1066,36 @@ static int dispatch_spmm_bulk(const SpmmParams &p, cudaStream_t st) {
     return launch_spmm_bulk<4>(p, st);
 }
 
-template <int VEC, int G, int NC, int U, typename T>
+template <int VEC, int G, int NC, int U, typename T, bool DUAL>
 static int launch_spmm(const SpmmParams &p, cudaStream_t st) {
     constexpr int rows_per_block = (kSpmmThreads / 32) * (32 / G);
     const int64_t blocks = ceil_div64(p.n_dst, rows_per_block);
     if (p.reduce == TFGK_REDUCE_MAX)
-        spmm_kernel<VEC, G, NC, true, U, T><<<(unsigned)blocks, kSpmmThreads, 0, st>>>(p);
+        spmm_kernel<VEC, G, NC, true, U, T, DUAL><<<(unsigned)blocks, kSpmmThreads, 0, st>>>(p);
     else
-        spmm_kernel<VEC, G, NC, false, U, T><<<(unsigned)blocks, kSpmmThreads, 0, st>>>(p);
+        spmm_kernel<VEC, G, NC, false, U, T, DUAL><<<(unsigned)blocks, kSpmmThreads, 0, st>>>(p);
     TFGK_LAUNCH_CHECK();
     return TFGK_OK;
 }
 
-template <int VEC, typename T = float>
+template <int VEC, typename T = float, bool DUAL = false>
 static int dispatch_spmm(const SpmmParams &p, int lanes, cudaStream_t st) {
     // lanes = number of VEC-wide vectors in a row (<= 128)
-    if (lanes <= 1) return launch_spmm<VEC, 1, 1, 8, T>(p, st);
-    if (lanes <= 2) return launch_spmm<VEC, 2, 1, 8, T>(p, st);
-    if (lanes <= 4) return launch_spmm<VEC, 4, 1, 8, T>(p, st);
-    if (lanes <= 8) return launch_spmm<VEC, 8, 1, 8, T>(p, st);
-    if (lanes <= 16) return launch_spmm<VEC, 16, 1, 8, T>(p, st);
-    if (lanes <= 32) return launch_spmm<VEC, 32, 1, 8, T>(p, st);
-    if (lanes <= 64) return launch_spmm<VEC, 32, 2, 4, T>(p, st);
-    if (lanes <= 96) return launch_spmm<VEC, 32, 3, 2, T>(p, st);
-    return launch_spmm<VEC, 32, 4, 2, T>(p, st);
+    if (lanes <= 1) return launch_spmm<VEC, 1, 1, 8, T, DUAL>(p, st);
+    if (lanes <= 2) return launch_spmm<VEC, 2, 1, 8, T, DUAL>(p, st);
+    if (lanes <= 4) return launch_spmm<VEC, 4, 1, 8, T, DUAL>(p, st);
+    if (lanes <= 8) return launch_spmm<VEC, 8, 1, 8, T, DUAL>(p, st);
+    if (lanes <= 16) return launch_spmm<VEC, 16, 1, 8, T, DUAL>(p, st);
+    if (lanes <= 32) return launch_spmm<VEC, 32, 1, 8, T, DUAL>(p, st);
+    if (lanes <= 64) return launch_spmm<VEC, 32, 2, 4, T, DUAL>(p, st);
+    if (lanes <= 96) return launch_spmm<VEC, 32, 3, 2, T, DUAL>(p, st);
+    return launch_spmm<VEC, 32, 4, 2, T, DUAL>(p, st);
 }
 
 // argument checks shared by the fp32 and bf16 entry points: TFGK_OK to go on (with *nothing_to_do set for an empty
 // launch), or the error status
 static int spmm_validate(const int64_t *rowptr, const void *h, int64_t ldh, int32_t n_dst, int32_t D, int reduce,
-                         const float *addend, int64_t ld_addend, int act, const float *out, int64_t ldo,
+                         const float *addend, int64_t ld_addend, int act, const void *out, int64_t ldo,
                          const tfgk_plan *plan, bool *nothing_to_do) {
     *nothing_to_do = true;
     TFGK_CHECK_ARG(n_dst >= 0 && D >= 0, "spmm: negative size (n_dst=%d, D=%d)", n_dst, D);
@@ -1047,7 +1121,8 @@ static SpmmParams spmm_params(const int64_t *rowptr, const int32_t *col, const f
     p.reduce = reduce; p.alpha = alpha;
     p.addend = addend ? addend + c0 : nullptr; p.ld_addend = ld_addend; p.beta = beta;
     p.bias = bias ? bias + c0 : nullptr; p.act = act;
-    p.out = out + c0; p.ldo = ldo;
+    p.out = out ? out + c0 : nullptr; p.ldo = ldo;
+    p.outb = nullptr; p.ldob = 0; p.d_store = width; p.io4 = false;
     p.n_tasks = 0; p.task_row = nullptr; p.task_nrows = nullptr; p.task_e0 = nullptr; p.task_e1 = nullptr;
     p.task_slot = nullptr; p.n_hubs = 0; p.hub_row = nullptr; p.hub_slot0 = nullptr; p.hub_nslots = nullptr;
     p.scratch = nullptr;
@@ -1154,6 +1229,67 @@ extern "C" int tfgk_spmm_bf16(const int64_t *rowptr, const int32_t *col, const f
                                    c0, D - c0 < 128 ? D - c0 : 128);
         p.hb = h + c0;
         const int rc = dispatch_spmm<1, uint16_t>(p, p.D, st);
+        if (rc != TFGK_OK) return rc;
+    }
+    return TFGK_OK;
+}
+
+// bf16 rows, fp32 and/or bf16 output.  The kernels are tfgk_spmm_bf16's, instantiated with the dual-store epilogue
+// (epilogue_dual), and take the plan exactly where tfgk_spmm_bf16 takes it for the same h, addend, bias and fp32 out (a
+// dense fp32 out when only the bf16 copy is written): `out` is then bit-identical to tfgk_spmm_bf16's, and out_bf16 is
+// its rounding.  Rows without the plan are summed strictly in CSR order by every kernel, so the ring kernels may also run
+// where tfgk_spmm_bf16 takes the scalar path: a table whose rows are 16-byte (8-byte) aligned with ldh >= D rounded up to
+// 8 (4) is read with its pad columns, which makes the TMA (cp.async) ring available to any D.  Pad columns never interact
+// with the first D and are never stored.
+extern "C" int tfgk_spmm_bf16_dual(const int64_t *rowptr, const int32_t *col, const float *w,
+                                   const uint16_t *h, int64_t ldh, int32_t n_dst, int32_t D, int reduce,
+                                   float alpha, const float *addend, int64_t ld_addend, float beta,
+                                   const float *bias, int act,
+                                   float *out, int64_t ldo, uint16_t *out_bf16, int64_t ldob,
+                                   const tfgk_plan *plan, void *stream) {
+    TFGK_CHECK_ARG(out != nullptr || out_bf16 != nullptr, "spmm_bf16_dual: both outputs are null");
+    bool nothing_to_do = true;
+    const int vrc = spmm_validate(rowptr, h, ldh, n_dst, D, reduce, addend, ld_addend, act,
+                                  out ? (const void *)out : (const void *)out_bf16, out ? ldo : ldob, plan, &nothing_to_do);
+    if (vrc != TFGK_OK || nothing_to_do) return vrc;
+    TFGK_CHECK_ARG(!out_bf16 || ldob >= D, "spmm_bf16_dual: leading dimension < D (ldob=%lld)", (long long)ldob);
+    TFGK_CHECK_ARG((reinterpret_cast<uintptr_t>(h) & 1u) == 0 && (reinterpret_cast<uintptr_t>(out_bf16) & 1u) == 0 &&
+                   (reinterpret_cast<uintptr_t>(out) & 3u) == 0, "spmm_bf16_dual: misaligned h, out or out_bf16");
+
+    const bool in_aligned = (!addend || ((ld_addend % 4 == 0) && aligned16(addend))) && (!bias || aligned16(bias));
+    const bool out4 = !out || ((ldo % 4 == 0) && aligned16(out));
+    const bool outb4 = !out_bf16 || ((ldob % 4 == 0) && aligned8(out_bf16));
+    // tfgk_spmm_bf16's ring condition (its rows4), with the fp32 out it would write
+    const bool rows4 = (D % 4 == 0) && (ldh % 4 == 0) && aligned8(h) && out4 && in_aligned;
+    const bool use_plan = rows4 && D >= 32 && D <= 512 && plan != nullptr && plan->n_tasks > 0 && spmm_impl_choice() >= 3;
+    // width read per row: D, or D with its pad columns where that lets a ring run (the plan's scratch must hold them)
+    const int32_t d8 = (D + 7) / 8 * 8, d4 = (D + 3) / 4 * 4;
+    const bool scratch8 = !use_plan || plan->n_hubs == 0 || plan->scratch_bytes >= (size_t)plan->n_slots * d8 * sizeof(float);
+    int32_t width = 0;                                   // 0: the scalar path
+    if (ldh % 8 == 0 && ldh >= d8 && aligned16(h) && d8 >= 32 && d8 <= 256 && scratch8) width = d8;   // TMA ring
+    else if (ldh % 4 == 0 && ldh >= d4 && aligned8(h) && d4 >= 32 && d4 <= 512) width = d4;            // cp.async ring
+    cudaStream_t st = as_stream(stream);
+    if (width > 0) {
+        SpmmParams p = spmm_params(rowptr, col, w, ldh, n_dst, reduce, alpha, addend, ld_addend, beta, bias, act, out, ldo,
+                                   0, width);
+        p.hb = h;
+        p.outb = out_bf16; p.ldob = ldob; p.d_store = D;
+        p.io4 = D % 4 == 0 && out4 && outb4 && in_aligned;
+        if (use_plan) spmm_use_plan(p, plan);
+        const int rc = launch_spmm_tma4<6, uint16_t, true>(p, st);   // TFGK_ERR_UNSUPPORTED unless 16-byte rows, width <= 256
+        if (rc != TFGK_ERR_UNSUPPORTED) return rc;
+        const int lanes = width / 4;
+        return lanes <= 32 ? launch_spmm_async<1, 4, 3, uint16_t, true>(p, st)
+             : lanes <= 64 ? launch_spmm_async<2, 4, 4, uint16_t, true>(p, st)
+             : lanes <= 96 ? launch_spmm_async<3, 4, 3, uint16_t, true>(p, st)
+                           : launch_spmm_async<4, 2, 4, uint16_t, true>(p, st);
+    }
+    for (int c0 = 0; c0 < D; c0 += 128) {               // scalar path: 32 lanes x 4 single columns per launch
+        SpmmParams p = spmm_params(rowptr, col, w, ldh, n_dst, reduce, alpha, addend, ld_addend, beta, bias, act, out, ldo,
+                                   c0, D - c0 < 128 ? D - c0 : 128);
+        p.hb = h + c0;
+        p.outb = out_bf16 ? out_bf16 + c0 : nullptr; p.ldob = ldob;
+        const int rc = dispatch_spmm<1, uint16_t, true>(p, p.D, st);
         if (rc != TFGK_OK) return rc;
     }
     return TFGK_OK;

@@ -12,8 +12,11 @@ class APPNP(Layer):
 
     def __init__(self, units_list, dense_activation=ops.relu, activation=None, k=10, alpha=0.1,
                  dense_drop_rate=0.0, last_dense_drop_rate=0.0, edge_drop_rate=0.0,
-                 kernel_regularizer=None, bias_regularizer=None, *args, **kwargs):
+                 kernel_regularizer=None, bias_regularizer=None, *args, message_dtype=None, **kwargs):
+        """message_dtype: None / torch.float32, or torch.bfloat16 for inference with bf16 message rows (nn.appnp)."""
         super().__init__(*args, **kwargs)
+        ops.message_dtype(message_dtype)          # ValueError for anything but fp32 / bf16
+        self.message_dtype = message_dtype
         self.units_list = units_list
         self.dense_activation = dense_activation
         self.activation = activation
@@ -54,4 +57,5 @@ class APPNP(Layer):
         return appnp(x, edge_index, edge_weight, self.kernels, self.biases,
                      dense_activation=self.dense_activation, activation=self.activation, k=self.k, alpha=self.alpha,
                      dense_drop_rate=self.dense_drop_rate, last_dense_drop_rate=self.last_dense_drop_rate,
-                     edge_drop_rate=self.edge_drop_rate, cache=cache, training=bool(training))
+                     edge_drop_rate=self.edge_drop_rate, cache=cache, training=bool(training),
+                     message_dtype=self.message_dtype)

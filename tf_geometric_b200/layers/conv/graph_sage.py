@@ -21,8 +21,11 @@ class _PairSage(Layer):
     _fn = None
 
     def __init__(self, units, activation=ops.relu, use_bias=True, concat=True, normalize=False,
-                 kernel_regularizer=None, bias_regularizer=None, *args, **kwargs):
+                 kernel_regularizer=None, bias_regularizer=None, *args, message_dtype=None, **kwargs):
+        """message_dtype: None / torch.float32, or torch.bfloat16 for inference with bf16 message rows (nn.mean_graph_sage / sum_graph_sage)."""
         super().__init__(*args, **kwargs)
+        ops.message_dtype(message_dtype)          # ValueError for anything but fp32 / bf16
+        self.message_dtype = message_dtype
         self.units = units
         self.activation = activation
         self.use_bias = use_bias
@@ -47,7 +50,8 @@ class _PairSage(Layer):
     def call(self, inputs, cache=None, training=None, mask=None):
         x, edge_index, edge_weight = _unpack(inputs)
         return type(self)._fn(x, edge_index, edge_weight, self.self_kernel, self.neighbor_kernel, bias=self.bias,
-                              activation=self.activation, concat=self.concat, normalize=self.normalize)
+                              activation=self.activation, concat=self.concat, normalize=self.normalize,
+                              message_dtype=self.message_dtype)
 
 
 class MeanGraphSage(_PairSage):
@@ -61,8 +65,11 @@ class SumGraphSage(_PairSage):
 class GCNGraphSage(Layer):
 
     def __init__(self, units, activation=ops.relu, use_bias=True, normalize=False,
-                 kernel_regularizer=None, bias_regularizer=None, *args, **kwargs):
+                 kernel_regularizer=None, bias_regularizer=None, *args, message_dtype=None, **kwargs):
+        """message_dtype: None / torch.float32, or torch.bfloat16 for inference with bf16 message rows (nn.gcn_graph_sage)."""
         super().__init__(*args, **kwargs)
+        ops.message_dtype(message_dtype)          # ValueError for anything but fp32 / bf16
+        self.message_dtype = message_dtype
         self.units = units
         self.activation = activation
         self.use_bias = use_bias
@@ -81,7 +88,7 @@ class GCNGraphSage(Layer):
     def call(self, inputs, cache=None, training=None, mask=None):
         x, edge_index, edge_weight = _unpack(inputs)
         return gcn_graph_sage(x, edge_index, edge_weight, self.kernel, self.bias, self.activation, self.normalize,
-                              cache=cache)
+                              cache=cache, message_dtype=self.message_dtype)
 
 
 class _PoolSage(Layer):
@@ -89,8 +96,11 @@ class _PoolSage(Layer):
     _names = ("neighbor_mlp_kernel", "neighbor_mlp_bias", "neighbor_kernel")
 
     def __init__(self, units, activation=ops.relu, use_bias=True, concat=True, normalize=False,
-                 kernel_regularizer=None, bias_regularizer=None, *args, **kwargs):
+                 kernel_regularizer=None, bias_regularizer=None, *args, message_dtype=None, **kwargs):
+        """message_dtype: None / torch.float32, or torch.bfloat16 for inference with bf16 message rows (nn.mean_pool_graph_sage / max_pool_graph_sage)."""
         super().__init__(*args, **kwargs)
+        ops.message_dtype(message_dtype)          # ValueError for anything but fp32 / bf16
+        self.message_dtype = message_dtype
         self.units = units
         self.activation = activation
         self.use_bias = use_bias
@@ -120,7 +130,8 @@ class _PoolSage(Layer):
         mlp_k, mlp_b, neigh_k = self._names
         return type(self)._fn(x, edge_index, edge_weight, self.self_kernel, getattr(self, mlp_k), getattr(self, neigh_k),
                               neighbor_mlp_bias=getattr(self, mlp_b) if self.use_bias else None, bias=self.bias,
-                              activation=self.activation, concat=self.concat, normalize=self.normalize)
+                              activation=self.activation, concat=self.concat, normalize=self.normalize,
+                              message_dtype=self.message_dtype)
 
 
 class MeanPoolGraphSage(_PoolSage):

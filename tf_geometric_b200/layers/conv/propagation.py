@@ -17,8 +17,11 @@ def _unpack(inputs):
 
 class SGC(Layer):
     def __init__(self, units, k=1, activation=None, use_bias=True, renorm=True, improved=False,
-                 kernel_regularizer=None, bias_regularizer=None, *args, **kwargs):
+                 kernel_regularizer=None, bias_regularizer=None, *args, message_dtype=None, **kwargs):
+        """message_dtype: None / torch.float32, or torch.bfloat16 for inference with bf16 message rows (nn.sgc)."""
         super().__init__(*args, **kwargs)
+        ops.message_dtype(message_dtype)          # ValueError for anything but fp32 / bf16
+        self.message_dtype = message_dtype
         self.units, self.k, self.activation, self.use_bias = units, k, activation, use_bias
         self.renorm, self.improved = renorm, improved
         self.kernel = None
@@ -38,14 +41,17 @@ class SGC(Layer):
     def call(self, inputs, cache=None, training=None, mask=None):
         x, edge_index, edge_weight = _unpack(inputs)
         return sgc(x, edge_index, edge_weight, self.k, self.kernel, self.bias, activation=self.activation,
-                   renorm=self.renorm, improved=self.improved, cache=cache)
+                   renorm=self.renorm, improved=self.improved, cache=cache, message_dtype=self.message_dtype)
 
 
 class SSGC(Layer):
     def __init__(self, units_list=None, k=10, alpha=0.1, dense_activation=ops.relu, activation=None,
                  dense_drop_rate=0.0, last_dense_drop_rate=0.0, edge_drop_rate=0.0,
-                 kernel_regularizer=None, bias_regularizer=None, *args, **kwargs):
+                 kernel_regularizer=None, bias_regularizer=None, *args, message_dtype=None, **kwargs):
+        """message_dtype: None / torch.float32, or torch.bfloat16 for inference with bf16 message rows (nn.ssgc)."""
         super().__init__(*args, **kwargs)
+        ops.message_dtype(message_dtype)          # ValueError for anything but fp32 / bf16
+        self.message_dtype = message_dtype
         self.units_list, self.k, self.alpha = units_list, k, alpha
         self.dense_activation, self.activation = dense_activation, activation
         self.dense_drop_rate, self.last_dense_drop_rate, self.edge_drop_rate = dense_drop_rate, last_dense_drop_rate, edge_drop_rate
@@ -67,13 +73,17 @@ class SSGC(Layer):
                     kernels=self.kernels if self.units_list else None, biases=self.biases if self.units_list else None,
                     k=self.k, alpha=self.alpha, dense_activation=self.dense_activation, activation=self.activation,
                     dense_drop_rate=self.dense_drop_rate, last_dense_drop_rate=self.last_dense_drop_rate,
-                    edge_drop_rate=self.edge_drop_rate, cache=cache, training=bool(training))
+                    edge_drop_rate=self.edge_drop_rate, cache=cache, training=bool(training),
+                    message_dtype=self.message_dtype)
 
 
 class TAGCN(Layer):
     def __init__(self, units, k=3, activation=None, use_bias=True, renorm=False, improved=False,
-                 kernel_regularizer=None, bias_regularizer=None, *args, **kwargs):
+                 kernel_regularizer=None, bias_regularizer=None, *args, message_dtype=None, **kwargs):
+        """message_dtype: None / torch.float32, or torch.bfloat16 for inference with bf16 message rows (nn.tagcn)."""
         super().__init__(*args, **kwargs)
+        ops.message_dtype(message_dtype)          # ValueError for anything but fp32 / bf16
+        self.message_dtype = message_dtype
         self.units, self.k, self.activation, self.use_bias = units, k, activation, use_bias
         self.renorm, self.improved = renorm, improved
         self.kernel = None
@@ -90,12 +100,15 @@ class TAGCN(Layer):
     def call(self, inputs, cache=None, training=None, mask=None):
         x, edge_index, edge_weight = _unpack(inputs)
         return tagcn(x, edge_index, edge_weight, self.k, self.kernel, self.bias, activation=self.activation,
-                     renorm=self.renorm, improved=self.improved, cache=cache)
+                     renorm=self.renorm, improved=self.improved, cache=cache, message_dtype=self.message_dtype)
 
 
 class GIN(Layer):
-    def __init__(self, mlp_model, eps=0, train_eps=False, *args, **kwargs):
+    def __init__(self, mlp_model, eps=0, train_eps=False, *args, message_dtype=None, **kwargs):
+        """message_dtype: None / torch.float32, or torch.bfloat16 for inference with bf16 message rows (nn.gin)."""
         super().__init__(*args, **kwargs)
+        ops.message_dtype(message_dtype)          # ValueError for anything but fp32 / bf16
+        self.message_dtype = message_dtype
         self.mlp_model = mlp_model
         self.eps = eps
         if train_eps:
@@ -106,13 +119,16 @@ class GIN(Layer):
 
     def call(self, inputs, cache=None, training=None, mask=None):
         x, edge_index = inputs[0], inputs[1]
-        return gin(x, edge_index, self.mlp_model, self.eps, training=training)
+        return gin(x, edge_index, self.mlp_model, self.eps, training=training, message_dtype=self.message_dtype)
 
 
 class LEConv(Layer):
     def __init__(self, units, activation=None, self_use_bias=True, aggr_self_use_bias=True, aggr_neighbor_use_bias=False,
-                 kernel_regularizer=None, bias_regularizer=None, *args, **kwargs):
+                 kernel_regularizer=None, bias_regularizer=None, *args, message_dtype=None, **kwargs):
+        """message_dtype: None / torch.float32, or torch.bfloat16 for inference with bf16 message rows (nn.le_conv)."""
         super().__init__(*args, **kwargs)
+        ops.message_dtype(message_dtype)          # ValueError for anything but fp32 / bf16
+        self.message_dtype = message_dtype
         self.units, self.activation = units, activation
         self.self_use_bias, self.aggr_self_use_bias, self.aggr_neighbor_use_bias = \
             self_use_bias, aggr_self_use_bias, aggr_neighbor_use_bias
@@ -134,15 +150,19 @@ class LEConv(Layer):
     def call(self, inputs, training=None, mask=None, cache=None):
         x, edge_index, edge_weight = _unpack(inputs)
         return le_conv(x, edge_index, edge_weight, self.self_kernel, self.self_bias, self.aggr_self_kernel,
-                       self.aggr_self_bias, self.aggr_neighbor_kernel, self.aggr_neighbor_bias, activation=self.activation)
+                       self.aggr_self_bias, self.aggr_neighbor_kernel, self.aggr_neighbor_bias, activation=self.activation,
+                       message_dtype=self.message_dtype)
 
 
 class ChebyNet(Layer):
     """tfg.layers.ChebyNet (reference layers/conv/chebynet.py): weights kernel0..kernel{k-1}, bias."""
 
     def __init__(self, units, k, activation=None, use_bias=True, normalization_type="sym", use_dynamic_lambda_max=False,
-                 kernel_regularizer=None, bias_regularizer=None, *args, **kwargs):
+                 kernel_regularizer=None, bias_regularizer=None, *args, message_dtype=None, **kwargs):
+        """message_dtype: None / torch.float32, or torch.bfloat16 for inference with bf16 message rows (nn.chebynet)."""
         super().__init__(*args, **kwargs)
+        ops.message_dtype(message_dtype)          # ValueError for anything but fp32 / bf16
+        self.message_dtype = message_dtype
         self.units, self.k, self.activation, self.use_bias = units, k, activation, use_bias
         self.normalization_type, self.use_dynamic_lambda_max = normalization_type, use_dynamic_lambda_max
         self.kernels = []
@@ -164,4 +184,5 @@ class ChebyNet(Layer):
     def call(self, inputs, cache=None, training=None, mask=None):
         x, edge_index, edge_weight = _unpack(inputs)
         return chebynet(x, edge_index, edge_weight, self.k, self.kernels, self.bias, self.activation,
-                        self.normalization_type, use_dynamic_lambda_max=self.use_dynamic_lambda_max, cache=cache)
+                        self.normalization_type, use_dynamic_lambda_max=self.use_dynamic_lambda_max, cache=cache,
+                        message_dtype=self.message_dtype)

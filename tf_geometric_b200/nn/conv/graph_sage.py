@@ -10,6 +10,8 @@ is replaced by ones in the gcn / pool variants (graph_sage.py:139-140,190-191,25
 import torch
 
 from ... import ops, _structure, autograd
+from . import _bf16
+from .gat import project
 from .gcn import gcn_norm_edge
 from ...sparse import SparseMatrix
 
@@ -64,7 +66,11 @@ def _project_pair_autograd(x, agg, ws, wn, bias, activation, concat, normalize):
     return h
 
 
-def _plain_sage(reduce, x, edge_index, edge_weight, self_kernel, neighbor_kernel, bias, activation, concat, normalize):
+def _plain_sage(reduce, x, edge_index, edge_weight, self_kernel, neighbor_kernel, bias, activation, concat, normalize,
+                message_dtype=None):
+    bf16 = _bf16.enabled(message_dtype)
+    if bf16:
+        _bf16.refuse_unsupported(x, (self_kernel, neighbor_kernel, bias, edge_weight))
     edge_index = ops.as_device(edge_index, torch.int32)
     dev = edge_index.device
     x = ops.as_device(x, torch.float32, device=dev)
@@ -79,26 +85,34 @@ def _plain_sage(reduce, x, edge_index, edge_weight, self_kernel, neighbor_kernel
     w_csr = None
     if edge_weight is not None:
         w_csr = _structure.weights_in_csr_order(ops.as_device(edge_weight, torch.float32, device=dev), csr)
-    agg = ops.spmm(csr, w_csr, x, reduce=reduce)
+    # bf16: the gathered copy of x is rounded, the self term x Ws reads the fp32 x
+    agg = ops.spmm(csr, w_csr, ops.round_bf16_table(x) if bf16 else x, reduce=reduce)
     return _project_pair(x, agg, self_kernel, neighbor_kernel, bias, activation, concat, normalize)
 
 
 def mean_graph_sage(x, edge_index, edge_weight, self_kernel, neighbor_kernel, bias=None, activation=None,
-                    concat=True, normalize=False):
-    """h = act([x Ws || mean_{j in N(i)} (w_ij x_j) Wn] + b)  (reference graph_sage.py:9-60)."""
+                    concat=True, normalize=False, message_dtype=None):
+    """h = act([x Ws || mean_{j in N(i)} (w_ij x_j) Wn] + b)  (reference graph_sage.py:9-60).
+    message_dtype=torch.bfloat16: inference with the gathered x stored in bf16 (an extension of the reference API)."""
     return _plain_sage("mean", x, edge_index, edge_weight, self_kernel, neighbor_kernel, bias, activation, concat,
-                       normalize)
+                       normalize, message_dtype)
 
 
 def sum_graph_sage(x, edge_index, edge_weight, self_kernel, neighbor_kernel, bias=None, activation=None,
-                   concat=True, normalize=False):
-    """Sum aggregator (reference graph_sage.py:64-115)."""
+                   concat=True, normalize=False, message_dtype=None):
+    """Sum aggregator (reference graph_sage.py:64-115).
+    message_dtype=torch.bfloat16: inference with the gathered x stored in bf16 (an extension of the reference API)."""
     return _plain_sage("sum", x, edge_index, edge_weight, self_kernel, neighbor_kernel, bias, activation, concat,
-                       normalize)
+                       normalize, message_dtype)
 
 
-def gcn_graph_sage(x, edge_index, edge_weight, kernel, bias=None, activation=None, normalize=False, cache=None):
-    """GCN aggregator (reference graph_sage.py:118-161): act((norm(A) x) W + b)."""
+def gcn_graph_sage(x, edge_index, edge_weight, kernel, bias=None, activation=None, normalize=False, cache=None,
+                   message_dtype=None):
+    """GCN aggregator (reference graph_sage.py:118-161): act((norm(A) x) W + b).  message_dtype=torch.bfloat16:
+    inference with the gathered x stored in bf16 (an extension of the reference API)."""
+    bf16 = _bf16.enabled(message_dtype)
+    if bf16:
+        _bf16.refuse_unsupported(x, (kernel, bias))
     edge_index = ops.as_device(edge_index, torch.int32)
     dev = edge_index.device
     x = ops.as_device(x, torch.float32, device=dev)
@@ -113,7 +127,7 @@ def gcn_graph_sage(x, edge_index, edge_weight, kernel, bias=None, activation=Non
         if normalize:
             h = h * torch.rsqrt(torch.clamp((h * h).sum(dim=-1, keepdim=True), min=1e-12))
         return h
-    reduced = normed.matmul(x)
+    reduced = normed.matmul(ops.round_bf16_table(x) if bf16 else x)
     act_code, leftover = ops.activation_code(activation)
     h = ops.gemm(reduced, ops.as_device(kernel, torch.float32, device=dev),
                  bias=None if bias is None else ops.as_device(bias, torch.float32, device=dev), act=act_code)
@@ -130,7 +144,10 @@ def _norm_edge_as_matrix(edge_index, num_nodes, edge_weight, renorm):
 
 
 def _pool_sage(reduce, x, edge_index, edge_weight, self_kernel, neighbor_mlp_kernel, neighbor_kernel,
-               neighbor_mlp_bias, bias, activation, concat, normalize):
+               neighbor_mlp_bias, bias, activation, concat, normalize, message_dtype=None):
+    bf16 = _bf16.enabled(message_dtype)
+    if bf16:
+        _bf16.refuse_unsupported(x, (self_kernel, neighbor_mlp_kernel, neighbor_kernel, neighbor_mlp_bias, bias))
     if edge_weight is None:
         # the reference multiplies by `edge_weight` unconditionally (gcn_mapper) and fails on None
         raise TypeError("edge_weight must not be None for the pooling GraphSAGE variants (reference behaviour)")
@@ -152,6 +169,9 @@ def _pool_sage(reduce, x, edge_index, edge_weight, self_kernel, neighbor_mlp_ker
                                       normalize)
     csr, _ = _structure.csr_for_edge_index(edge_index, num_nodes)
     act_code, leftover = ops.activation_code(activation)
+    if bf16:
+        reduced = ops.spmm(csr, None, _pool_mlp_bf16(x, neighbor_mlp_kernel, neighbor_mlp_bias, activation), reduce=reduce)
+        return _project_pair(x, reduced, self_kernel, neighbor_kernel, bias, activation, concat, normalize)
     # per-node neighbour MLP (weights are all ones, so x[col] * w == x[col])
     h_node = ops.gemm(x, ops.as_device(neighbor_mlp_kernel, torch.float32, device=dev),
                       bias=None if neighbor_mlp_bias is None else ops.as_device(neighbor_mlp_bias, torch.float32, device=dev),
@@ -162,18 +182,38 @@ def _pool_sage(reduce, x, edge_index, edge_weight, self_kernel, neighbor_mlp_ker
     return _project_pair(x, reduced, self_kernel, neighbor_kernel, bias, activation, concat, normalize)
 
 
+def _pool_mlp_bf16(x, kernel, bias, activation):
+    """bf16(act(x W + b)) in a padded table: rounded by the projection's epilogue (K4) for relu / no activation, by
+    tfgk_round_bf16 after any other activation."""
+    dev = x.device
+    kernel = ops.as_device(kernel, torch.float32, device=dev)
+    bias = None if bias is None else ops.as_device(bias, torch.float32, device=dev)
+    act_code, leftover = ops.activation_code(activation)
+    if leftover is not None:
+        return ops.round_bf16_table(leftover(ops.gemm(x, kernel, bias=bias, act=act_code)))
+    h = ops.bf16_table(x.shape[0], kernel.shape[1], dev)
+    project(x, [(kernel, bias, act_code, h)])
+    return h
+
+
 def mean_pool_graph_sage(x, edge_index, edge_weight, self_kernel, neighbor_mlp_kernel, neighbor_kernel,
-                         neighbor_mlp_bias=None, bias=None, activation=None, concat=True, normalize=False):
-    """Mean-pooling aggregator (reference graph_sage.py:164-225)."""
+                         neighbor_mlp_bias=None, bias=None, activation=None, concat=True, normalize=False,
+                         message_dtype=None):
+    """Mean-pooling aggregator (reference graph_sage.py:164-225).
+    message_dtype=torch.bfloat16: inference with the neighbour MLP's output stored in bf16 (an extension of the
+    reference API)."""
     return _pool_sage("mean", x, edge_index, edge_weight, self_kernel, neighbor_mlp_kernel, neighbor_kernel,
-                      neighbor_mlp_bias, bias, activation, concat, normalize)
+                      neighbor_mlp_bias, bias, activation, concat, normalize, message_dtype)
 
 
 def max_pool_graph_sage(x, edge_index, edge_weight, self_kernel, neighbor_mlp_kernel, neighbor_kernel,
-                        neighbor_mlp_bias=None, bias=None, activation=None, concat=True, normalize=False):
-    """Max-pooling aggregator (reference graph_sage.py:228-287); nodes without in-edges get float32 lowest."""
+                        neighbor_mlp_bias=None, bias=None, activation=None, concat=True, normalize=False,
+                        message_dtype=None):
+    """Max-pooling aggregator (reference graph_sage.py:228-287); nodes without in-edges get float32 lowest.
+    message_dtype=torch.bfloat16: inference with the neighbour MLP's output stored in bf16 (an extension of the
+    reference API)."""
     return _pool_sage("max", x, edge_index, edge_weight, self_kernel, neighbor_mlp_kernel, neighbor_kernel,
-                      neighbor_mlp_bias, bias, activation, concat, normalize)
+                      neighbor_mlp_bias, bias, activation, concat, normalize, message_dtype)
 
 
 def _lstm_sage(x, edge_index, reduce_steps, step_major, self_kernel, neighbor_kernel, bias, activation, concat,

@@ -6,6 +6,8 @@ import torch
 
 from ... import ops, _structure, autograd
 from ...sparse import SparseMatrix
+from . import _bf16
+from .gat import project
 from .gcn import gcn_norm_adj
 
 
@@ -13,8 +15,13 @@ def _f32(t, dev):
     return None if t is None else ops.as_device(t, torch.float32, device=dev)
 
 
-def sgc(x, edge_index, edge_weight, k, kernel, bias=None, activation=None, renorm=True, improved=False, cache=None):
-    """Simple Graph Convolution: act(norm(A)^k (x W) + b)   (reference sgc.py:10-61)."""
+def sgc(x, edge_index, edge_weight, k, kernel, bias=None, activation=None, renorm=True, improved=False, cache=None,
+        message_dtype=None):
+    """Simple Graph Convolution: act(norm(A)^k (x W) + b)   (reference sgc.py:10-61).  message_dtype=torch.bfloat16:
+    inference with x W and the hops 1 .. k-1 stored in bf16 (an extension of the reference API)."""
+    bf16 = _bf16.enabled(message_dtype)
+    if bf16:
+        _bf16.refuse_unsupported(x, (kernel, bias, edge_weight))
     edge_index = ops.as_device(edge_index, torch.int32)
     dev = edge_index.device
     x = _f32(x, dev)
@@ -23,6 +30,15 @@ def sgc(x, edge_index, edge_weight, k, kernel, bias=None, activation=None, renor
     act_code, leftover = ops.activation_code(activation)
     b = _f32(bias, dev)
     with_grad = autograd.needs_grad(x, kernel, bias, normed.value)     # training: the same kernels behind autograd
+    if bf16 and k > 0:
+        kernel = _f32(kernel, dev)
+        h = ops.bf16_table(n, kernel.shape[1], dev)
+        project(x, [(kernel, None, ops.ACT_NONE, h)])                  # x W rounded by the projection's epilogue
+        bufs = [ops.bf16_table(n, kernel.shape[1], dev) for _ in range(min(k - 1, 2))]
+        for i in range(k - 1):
+            h = normed.matmul(h, out_bf16=bufs[i % 2])                   # intermediate hops: bf16 only
+        h = normed.matmul(h, bias=b, act=act_code)
+        return leftover(h) if leftover is not None else h
     h = autograd.dense(x, _f32(kernel, dev)) if with_grad else ops.gemm(x, _f32(kernel, dev))
     for i in range(k):
         last = i == k - 1
@@ -41,8 +57,15 @@ def sgc(x, edge_index, edge_weight, k, kernel, bias=None, activation=None, renor
 
 
 def ssgc(x, edge_index, edge_weight, kernels=None, biases=None, k=10, alpha=0.1, dense_activation=ops.relu,
-         activation=None, dense_drop_rate=0.0, last_dense_drop_rate=0.0, edge_drop_rate=0.0, cache=None, training=False):
-    """Simple Spectral Graph Convolution: alpha * h + (1 - alpha)/k * sum_{i=1..k} norm(A)^i h   (reference ssgc.py:11-99)."""
+         activation=None, dense_drop_rate=0.0, last_dense_drop_rate=0.0, edge_drop_rate=0.0, cache=None, training=False,
+         message_dtype=None):
+    """Simple Spectral Graph Convolution: alpha * h + (1 - alpha)/k * sum_{i=1..k} norm(A)^i h   (reference ssgc.py:11-99).
+    message_dtype=torch.bfloat16: inference with every gathered hop stored in bf16; the hops that are summed stay fp32 (an
+    extension of the reference API)."""
+    bf16 = _bf16.enabled(message_dtype)
+    if bf16:
+        drop = training and max(dense_drop_rate, last_dense_drop_rate, edge_drop_rate) > 0.0
+        _bf16.refuse_unsupported(x, [edge_weight] + list(kernels or []) + list(biases or []), dropout=drop)
     edge_index = ops.as_device(edge_index, torch.int32)
     dev = edge_index.device
     h = _f32(x, dev)
@@ -63,6 +86,16 @@ def ssgc(x, edge_index, edge_weight, kernels=None, biases=None, k=10, alpha=0.1,
                     h = leftover(h)
             h = autograd.dropout(h, dense_drop_rate if i < num_dense - 1 else last_dense_drop_rate, training)  # :84-88
     output = h * alpha                                    # elementwise glue in the reference's rounding order (:91-94)
+    if bf16 and k > 0:
+        # each hop in fp32 (it is summed) and, from the same launch, in bf16 for the next gather
+        cur = ops.round_bf16_table(h)
+        bufs = [ops.bf16_table(n, h.shape[1], dev) for _ in range(min(k - 1, 2))]
+        for i in range(k):
+            nxt = bufs[i % 2] if i < k - 1 else None
+            h = normed.matmul(cur, out=torch.empty((n, h.shape[1]), dtype=torch.float32, device=dev), out_bf16=nxt)
+            output = output + (1 - alpha) * h / k
+            cur = nxt
+        return activation(output) if activation is not None else output
     for _ in range(k):
         h = autograd.propagate(normed, h) if with_grad else normed.matmul(h)
         output = output + (1 - alpha) * h / k
@@ -71,9 +104,14 @@ def ssgc(x, edge_index, edge_weight, kernels=None, biases=None, k=10, alpha=0.1,
     return output
 
 
-def tagcn(x, edge_index, edge_weight, k, kernel, bias=None, activation=None, renorm=False, improved=False, cache=None):
+def tagcn(x, edge_index, edge_weight, k, kernel, bias=None, activation=None, renorm=False, improved=False, cache=None,
+          message_dtype=None):
     """Topology Adaptive GCN: act([x, Ax, ..., A^k x] W + b); the hops are written straight into the column blocks of
-    the concatenated operand (reference tagcn.py:10-51)."""
+    the concatenated operand (reference tagcn.py:10-51).  message_dtype=torch.bfloat16: inference with x and the hops
+    1 .. k-1 gathered from bf16 copies; the concatenated GEMM operand stays fp32 (an extension of the reference API)."""
+    bf16 = _bf16.enabled(message_dtype)
+    if bf16:
+        _bf16.refuse_unsupported(x, (kernel, bias, edge_weight))
     edge_index = ops.as_device(edge_index, torch.int32)
     dev = edge_index.device
     x = _f32(x, dev)
@@ -86,7 +124,15 @@ def tagcn(x, edge_index, edge_weight, k, kernel, bias=None, activation=None, ren
         return autograd.dense(torch.cat(terms, dim=1), _f32(kernel, dev), _f32(bias, dev), activation)
     hops = torch.empty((n, f * (k + 1)), dtype=torch.float32, device=dev)
     hops[:, :f].copy_(x)
-    for i in range(k):
+    if bf16 and k > 0:
+        # each hop fp32 into its column block and, from the same launch, bf16 for the next gather
+        cur = ops.round_bf16_table(x)
+        bufs = [ops.bf16_table(n, f, dev) for _ in range(min(k - 1, 2))]
+        for i in range(k):
+            nxt = bufs[i % 2] if i < k - 1 else None
+            normed.matmul(cur, out=hops[:, (i + 1) * f:(i + 2) * f], out_bf16=nxt)
+            cur = nxt
+    for i in range(0 if bf16 else k):
         normed.matmul(hops[:, i * f:(i + 1) * f], out=hops[:, (i + 1) * f:(i + 2) * f])
     act_code, leftover = ops.activation_code(activation)
     out = ops.gemm(hops, _f32(kernel, dev), bias=_f32(bias, dev), act=act_code)
@@ -97,9 +143,14 @@ def gin_updater(x, reduced_neighbor_msg, eps):
     return x * (1.0 + eps) + reduced_neighbor_msg
 
 
-def gin(x, edge_index, mlp_model, eps=0.0, training=None):
+def gin(x, edge_index, mlp_model, eps=0.0, training=None, message_dtype=None):
     """Graph Isomorphism Network: mlp((1 + eps) x + sum_{j in N(i)} x_j); the update is the aggregation kernel's axpby
-    epilogue (reference gin.py:11-38)."""
+    epilogue (reference gin.py:11-38).  message_dtype=torch.bfloat16: inference with the gathered x stored in bf16; the
+    (1 + eps) x addend reads the fp32 x (an extension of the reference API)."""
+    bf16 = _bf16.enabled(message_dtype)
+    if bf16:
+        params = list(mlp_model.parameters()) if hasattr(mlp_model, "parameters") else []
+        _bf16.refuse_unsupported(x, [eps] + params)
     edge_index = ops.as_device(edge_index, torch.int32)
     dev = edge_index.device
     x = _f32(x, dev)
@@ -108,7 +159,8 @@ def gin(x, edge_index, mlp_model, eps=0.0, training=None):
     else:
         csr, _ = _structure.csr_for_edge_index(edge_index, x.shape[0])
         eps_value = float(eps.detach().item()) if torch.is_tensor(eps) else float(eps)
-        h = ops.spmm(csr, None, x, reduce="sum", alpha=1.0, addend=x, beta=1.0 + eps_value)
+        h = ops.spmm(csr, None, ops.round_bf16_table(x) if bf16 else x, reduce="sum", alpha=1.0, addend=x,
+                     beta=1.0 + eps_value)
     try:
         return mlp_model(h, training=training)
     except TypeError:
@@ -116,9 +168,15 @@ def gin(x, edge_index, mlp_model, eps=0.0, training=None):
 
 
 def le_conv(x, edge_index, edge_weight, self_kernel, self_bias, aggr_self_kernel, aggr_self_bias,
-            aggr_neighbor_kernel, aggr_neighbor_bias, activation=None):
+            aggr_neighbor_kernel, aggr_neighbor_bias, activation=None, message_dtype=None):
     """LEConv (ASAP): act(x Ws + sum_j w_ij (x_j Wa - x_j Wn)).  Note the reference gathers BOTH aggregation terms by the
-    neighbour index `col` (le_conv.py:40-43), so the per-edge difference is a per-node difference gathered once."""
+    neighbour index `col` (le_conv.py:40-43), so the per-edge difference is a per-node difference gathered once.
+    message_dtype=torch.bfloat16: inference with that fp32 difference rounded once to bf16; the self term stays fp32 (an
+    extension of the reference API)."""
+    bf16 = _bf16.enabled(message_dtype)
+    if bf16:
+        _bf16.refuse_unsupported(x, (self_kernel, self_bias, aggr_self_kernel, aggr_self_bias, aggr_neighbor_kernel,
+                                     aggr_neighbor_bias, edge_weight))
     edge_index = ops.as_device(edge_index, torch.int32)
     dev = edge_index.device
     x = _f32(x, dev)
@@ -138,7 +196,8 @@ def le_conv(x, edge_index, edge_weight, self_kernel, self_bias, aggr_self_kernel
     diff = ops.gemm(x, _f32(aggr_self_kernel, dev), bias=_f32(aggr_self_bias, dev)) \
         - ops.gemm(x, _f32(aggr_neighbor_kernel, dev), bias=_f32(aggr_neighbor_bias, dev))
     act_code, leftover = ops.activation_code(activation)
-    h = ops.spmm(csr, w_csr, diff, reduce="sum", alpha=1.0, addend=self_h, beta=1.0, act=act_code)
+    h = ops.spmm(csr, w_csr, ops.round_bf16_table(diff) if bf16 else diff, reduce="sum", alpha=1.0, addend=self_h, beta=1.0,
+                 act=act_code)
     return leftover(h) if leftover is not None else h
 
 
@@ -210,9 +269,14 @@ def chebynet_norm_edge(edge_index, num_nodes, edge_weight=None, normalization_ty
 
 
 def chebynet(x, edge_index, edge_weight, k, kernels, bias=None, activation=None, normalization_type="sym",
-             use_dynamic_lambda_max=False, cache=None):
+             use_dynamic_lambda_max=False, cache=None, message_dtype=None):
     """sum_i T_i(L~) x K_i with T_0 = x, T_1 = L~ x, T_i = 2 L~ T_{i-1} - T_{i-2}: the recurrence is the aggregation kernel's
-    axpby epilogue, the projections accumulate into `out` through the GEMM's beta (reference chebynet.py:63-137)."""
+    axpby epilogue, the projections accumulate into `out` through the GEMM's beta (reference chebynet.py:63-137).
+    message_dtype=torch.bfloat16: inference with T_0 .. T_{k-2} gathered from bf16 copies; every T_i stays fp32 as GEMM
+    operand and recurrence addend (an extension of the reference API)."""
+    bf16 = _bf16.enabled(message_dtype)
+    if bf16:
+        _bf16.refuse_unsupported(x, [bias, edge_weight] + list(kernels))
     edge_index = ops.as_device(edge_index, torch.int32)
     dev = edge_index.device
     x = _f32(x, dev)
@@ -238,12 +302,23 @@ def chebynet(x, edge_index, edge_weight, k, kernels, bias=None, activation=None,
         return activation(out) if activation is not None else out
     t0 = x
     out = ops.gemm(t0, _f32(kernels[0], dev))
+    # bf16: b1 is the bf16 copy of T1 for the next gather, written by the launch that writes T1 (none for T_{k-1})
+    b1 = None
     if k > 1:
-        t1 = adj.matmul(x)
+        if bf16:
+            b1 = ops.bf16_table(n, x.shape[1], dev) if k > 2 else None
+            t1 = adj.matmul(ops.round_bf16_table(x), out=torch.empty_like(x), out_bf16=b1)
+        else:
+            t1 = adj.matmul(x)
         ops.gemm(t1, _f32(kernels[1], dev), beta=1.0, out=out)
     if k > 2:
         for i in range(2, k):
-            t2 = adj.matmul(t1, alpha=2.0, addend=t0, beta=-1.0)          # (L~ @ T1) * 2.0 - T0
+            if bf16:
+                b2 = ops.bf16_table(n, x.shape[1], dev) if i < k - 1 else None
+                t2 = adj.matmul(b1, alpha=2.0, addend=t0, beta=-1.0, out=torch.empty_like(x), out_bf16=b2)
+                b1 = b2
+            else:
+                t2 = adj.matmul(t1, alpha=2.0, addend=t0, beta=-1.0)          # (L~ @ T1) * 2.0 - T0
             ops.gemm(t2, _f32(kernels[i], dev), beta=1.0, out=out)
             t0, t1 = t1, t2
     if bias is not None:

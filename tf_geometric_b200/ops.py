@@ -270,12 +270,16 @@ def scale_edges(row, col, w, dl=None, dr=None):
 # ---- K1 ----------------------------------------------------------------------------------------------------------
 
 def spmm(csr, w_csr, h, reduce="sum", alpha=1.0, addend=None, beta=0.0, bias=None, act=ACT_NONE, out=None, col=None,
-         keep_layout=False):
+         keep_layout=False, out_bf16=None):
     """out = epilogue(REDUCE_{e in row} w[e] * h[col[e]]); see tfgk_spmm_f32.  `col` overrides csr.col (used by the
     generic reducers, which gather message rows through csr.perm).  h may be bfloat16 (tfgk_spmm_bf16): the output is
     fp32 and bit-identical to the product over h.float(), also for strided or unaligned views of h.  With keep_layout=True
     a bf16 view is read in place, and the result is instead that of the fp32 product over a widened view with the same
-    layout (the column chunks of SparseMatrix.matmul)."""
+    layout (the column chunks of SparseMatrix.matmul).
+    out_bf16 (bf16 h only, tfgk_spmm_bf16_dual): a bfloat16 [n, D] tensor or view that receives the same result rounded
+    to nearest even.  The fp32 result is then written only into an `out` passed explicitly: with out=None the call
+    stores 2 bytes per element and returns out_bf16 (the intermediate hops of a propagation chain).  A bf16 h allocated
+    by bf16_table() is read with its pad columns, which keeps every width on the ring kernels."""
     if h.dtype not in (torch.float32, torch.bfloat16) or not h.is_cuda:
         raise TypeError("h must be a float32 or bfloat16 CUDA tensor")
     ldh = _row_major_2d(h, "h")
@@ -288,9 +292,20 @@ def spmm(csr, w_csr, h, reduce="sum", alpha=1.0, addend=None, beta=0.0, bias=Non
         # so that the result stays bit-identical to the product over h.float()
         h = h.clone(memory_format=torch.contiguous_format)
         ldh = _row_major_2d(h, "h")
-    if out is None:
+    # a bf16 table with padded 16-byte rows (bf16_table) goes to the dual entry, which reads it with its pad columns on
+    # the TMA ring: the same bits as tfgk_spmm_bf16, which would take the cp.async ring or the scalar path
+    d8 = -(-D // 8) * 8
+    padded = h.dtype == torch.bfloat16 and D % 8 != 0 and ldh % 8 == 0 and ldh >= d8 and h.data_ptr() % 16 == 0
+    dual = out_bf16 is not None or padded
+    if out_bf16 is not None:
+        if h.dtype != torch.bfloat16:
+            raise TypeError("spmm: out_bf16 needs a bfloat16 h")
+        if not (out_bf16.is_cuda and out_bf16.dtype == torch.bfloat16 and tuple(out_bf16.shape) == (n_dst, D)):
+            raise TypeError("spmm: out_bf16 must be a bfloat16 CUDA tensor of shape {}".format((n_dst, D)))
+    elif out is None:
         out = torch.empty((n_dst, D), dtype=torch.float32, device=h.device)
-    ldo = _row_major_2d(out, "out")
+    ldo = 0 if out is None else _row_major_2d(out, "out")
+    ldob = 0 if out_bf16 is None else _row_major_2d(out_bf16, "out_bf16")
     lda = 0
     if addend is not None:
         lda = _row_major_2d(addend, "addend")
@@ -299,12 +314,34 @@ def spmm(csr, w_csr, h, reduce="sum", alpha=1.0, addend=None, beta=0.0, bias=Non
     if bias is not None:
         _check(bias, torch.float32, "bias")
     code = _REDUCE_CODES[reduce] if isinstance(reduce, str) else reduce
-    plan_struct = plan.struct(D, h.device) if plan is not None else None
+    # the dual entry may read a padded table up to D rounded to 8 columns, hub slices included
+    plan_struct = plan.struct(d8 if dual else D, h.device) if plan is not None else None
+    plan_ref = ctypes.byref(plan_struct) if plan_struct is not None else None
+    if dual:
+        _ffi.call("tfgk_spmm_bf16_dual", _p(csr.rowptr), _p(csr.col if col is None else col), _p(w_csr), _p(h), ldh,
+                  n_dst, D, code, float(alpha), _p(addend), lda, float(beta), _p(bias), act, _p(out), ldo, _p(out_bf16),
+                  ldob, plan_ref, _stream(h))
+        return out if out is not None else out_bf16
     _ffi.call("tfgk_spmm_bf16" if h.dtype == torch.bfloat16 else "tfgk_spmm_f32", _p(csr.rowptr),
               _p(csr.col if col is None else col), _p(w_csr), _p(h), ldh, n_dst, D,
-              code, float(alpha), _p(addend), lda, float(beta), _p(bias), act, _p(out), ldo,
-              ctypes.byref(plan_struct) if plan_struct is not None else None, _stream(h))
+              code, float(alpha), _p(addend), lda, float(beta), _p(bias), act, _p(out), ldo, plan_ref, _stream(h))
     return out
+
+
+def bf16_table(rows, cols, device):
+    """An empty [rows, cols] bfloat16 table for message rows: a view of a row-major buffer whose rows are padded to a
+    multiple of 8 elements (16 bytes), pad columns zeroed, so that tfgk_spmm_bf16_dual reads every width with its ring
+    kernels."""
+    pitch = -(-int(cols) // 8) * 8
+    buf = torch.empty((int(rows), pitch), dtype=torch.bfloat16, device=device)
+    if pitch != cols:
+        buf[:, cols:].zero_()
+    return buf[:, :cols]
+
+
+def round_bf16_table(src):
+    """bf16_table() holding src (2-D float32 CUDA) rounded to nearest even (tfgk_round_bf16)."""
+    return round_bf16(src, out=bf16_table(src.shape[0], src.shape[1], src.device))
 
 
 # ---- K3 ----------------------------------------------------------------------------------------------------------

@@ -120,7 +120,8 @@ class SparseMatrix(object):
         reference's split -> matmul -> concat; the fused kernel has no [E, D] temporary to bound, so the results are the
         same bits with or without it.  A bfloat16 h stays bfloat16 and is gathered as such (tfgk_spmm_bf16) when no operand
         (h, bias, the values) needs a gradient: the float32 result is bit-identical to the product over h.float(), from
-        half the row bytes."""
+        half the row bytes.  With a bfloat16 h, `out_bf16=` (see ops.spmm) also stores the result rounded to bf16, or only
+        that when no `out` is given."""
         from . import autograd
         # the differentiable route below works in fp32 (its backward products take fp32 operands): a bf16 h is widened
         # for it, as it always was
@@ -146,7 +147,8 @@ class SparseMatrix(object):
             if sum(sizes) != d:
                 raise ValueError("split sizes {} do not add up to {} columns".format(sizes, d))
         out = epilogue.pop("out", None)
-        if out is None:
+        out_bf16 = epilogue.pop("out_bf16", None)
+        if out is None and out_bf16 is None:
             out = torch.empty((self._shape[0], d), dtype=torch.float32, device=h.device)
         bias, addend = epilogue.pop("bias", None), epilogue.pop("addend", None)
         if h.dtype == torch.bfloat16:
@@ -156,11 +158,13 @@ class SparseMatrix(object):
         for width in sizes:
             c1 = c0 + width
             if width:
-                ops.spmm(self.csr, self.value_csr, h[:, c0:c1], reduce="sum", out=out[:, c0:c1],
+                if out_bf16 is not None:
+                    epilogue["out_bf16"] = out_bf16[:, c0:c1]
+                ops.spmm(self.csr, self.value_csr, h[:, c0:c1], reduce="sum", out=None if out is None else out[:, c0:c1],
                          bias=None if bias is None else bias[c0:c1].contiguous(),
                          addend=None if addend is None else addend[:, c0:c1], **epilogue)
             c0 = c1
-        return out
+        return out if out is not None else out_bf16
 
     def __matmul__(self, h):
         return self.matmul(h)
