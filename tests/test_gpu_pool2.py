@@ -160,19 +160,21 @@ def test_sag_pool_matches_oracle(k, ratio):
 
 def test_pools_over_few_large_graphs_use_edge_sized_tasks():
     """Average segment length >= 128: the work plan shrinks its tasks from 32 rows to ~512 entries (ops.build_plan);
-    per-graph sums stay sequential, so the results are still bit-exact."""
+    per-graph sums stay sequential, so the results are still bit-exact.  K1 takes the plan from 32 columns on (d = 64);
+    d = 24 runs the per-row kernel."""
     rs = np.random.RandomState(77)
-    n, graphs, d = 12000, 20, 24
+    n, graphs = 12000, 20
     gi = np.sort(rs.randint(0, graphs, n)).astype(np.int32)
     gi[-1] = graphs - 1
-    x = rs.randn(n, d).astype(np.float32)
     from tf_geometric_b200 import _structure
     seg = _structure.csr_for_segment_ids(dev(gi), graphs)
     if seg.rowptr.is_cuda:             # the real kernels (the host-logic tests replay this body on CPU tensors, without a plan)
         assert seg.plan is not None and seg.plan.n_hubs == 0 and seg.plan.n_tasks >= graphs
-    for name in ("mean_pool", "sum_pool", "max_pool", "min_pool"):
-        got = host(getattr(tfg.nn, name)(dev(x), dev(gi), graphs))
-        np.testing.assert_array_equal(got, getattr(o, name)(x, gi, graphs), err_msg=name)
+    for d in (24, 64):
+        x = rs.randn(n, d).astype(np.float32)
+        for name in ("mean_pool", "sum_pool", "max_pool", "min_pool"):
+            got = host(getattr(tfg.nn, name)(dev(x), dev(gi), graphs))
+            np.testing.assert_array_equal(got, getattr(o, name)(x, gi, graphs), err_msg="{} d={}".format(name, d))
 
 
 def test_sort_pool_drop_edge_layer_and_map_reduce_layer():
