@@ -208,6 +208,22 @@ int tfgk_gat_fused_bf16(const int64_t *rowptr, const int32_t *col,
                         int32_t N, int32_t H, int32_t dqk, int32_t dv, float scale, int split_value_heads,
                         const float *bias, int act, float *att, int write_att, float *out, int64_t ldo,
                         const tfgk_plan *plan, void *stream);
+/* Packed keys: a table of one slot of ldt floats per node (ldt a multiple of 16, at least 2A + 4; A = H * dqk <= 128):
+ *     [0, A) V[n] | [A, A + 4) zero mask, bit c set <=> the bits of K[n, c] are not 0x00000000 |
+ *     [A + 4, ...) the entries of K[n] whose bit is set, in column order, zero-padded to a multiple of four floats
+ * and ksize[n] = 16-byte units of the slot a neighbour's copy reads, (A + 4 + padded count) / 4.  The caller writes V into the
+ * slots; tfgk_gat_pack_keys_f32 writes the mask, the packed keys and ksize from K [N, A] (16-byte aligned rows). */
+int tfgk_gat_pack_keys_f32(const float *K, int64_t ldk, int32_t N, int32_t A, float *table, int64_t ldt, uint8_t *ksize,
+                           void *stream);
+/* tfgk_gat_fused_f32 with heads concatenated and dqk == dv over a packed table: the TMA ring copies 16 * ksize[c] bytes per
+ * neighbour c instead of 8A and rebuilds K[c] from the mask.  Only the bit pattern 0x00000000 is left out of the table, so
+ * the output is bit-identical to tfgk_gat_fused_f32 over the same Q, K, V (for the shapes that take its TMA ring) for any
+ * K.  H a power of two <= 32, dqk / 4 a power of two, A <= 128, 16-byte aligned Q, out, bias and table rows; other shapes
+ * return TFGK_ERR_UNSUPPORTED.  The plan's hub scratch takes A + 64 floats per slot, as for tfgk_gat_fused_f32. */
+int tfgk_gat_fused_packed_f32(const int64_t *rowptr, const int32_t *col, const float *Q, int64_t ldq,
+                              const float *table, int64_t ldt, const uint8_t *ksize, int32_t N, int32_t H, int32_t dqk,
+                              float scale, const float *bias, int act, float *out, int64_t ldo,
+                              const tfgk_plan *plan, void *stream);
 
 /* ---- K4: dense projections (gcn.py:272, gat.py:52,61,70, graph_sage.py:43-44, appnp.py:69) ------------------- */
 

@@ -64,6 +64,9 @@ SIGNATURES = {
                            _int, _ptr, _int, _ptr, _i64, _ptr, _ptr],
     "tfgk_gat_fused_bf16": [_ptr, _ptr, _ptr, _i64, _ptr, _i64, _ptr, _i64, _i32, _i32, _i32, _i32, _f32, _int, _ptr,
                             _int, _ptr, _int, _ptr, _i64, _ptr, _ptr],
+    "tfgk_gat_pack_keys_f32": [_ptr, _i64, _i32, _i32, _ptr, _i64, _ptr, _ptr],
+    "tfgk_gat_fused_packed_f32": [_ptr, _ptr, _ptr, _i64, _ptr, _i64, _ptr, _i32, _i32, _i32, _f32, _ptr, _int, _ptr, _i64,
+                                  _ptr, _ptr],
     "tfgk_gemm_workspace_bytes": [_i32, _i32, _i32, ctypes.POINTER(_size)],
     "tfgk_gemm_f32": [_ptr, _i64, _int, _ptr, _i64, _int, _ptr, _int, _f32, _i32, _i32, _i32, _ptr, _i64, _ptr, _size,
                       _ptr],

@@ -51,6 +51,7 @@ struct GatParams {
     const int32_t *hub_row, *hub_slot0, *hub_nslots;
     float *scratch;      // per slot: [A] partial sums | [32] running max per lane | [32] denominators per lane
     float *stats;        // optional [N, 2H]: per (row, head) softmax maximum and denominator (+1e-8), kept for the backward pass
+    const uint8_t *ksize = nullptr;   // packed keys (tfgk_gat_fused_packed_f32): bytes / 16 to copy of each node's slot in K
 };
 
 // ---- fast path: float4 lanes, H | 32, dqk/4 a power of two, heads concatenated ---------------------------------
@@ -739,6 +740,255 @@ static int dispatch_gat_async(const GatParams &p, cudaStream_t st) {
     return launch_gat_async<2, 3>(p, st);
 }
 
+// ---- packed keys: the TMA ring reads only the non-zero entries of K ------------------------------------------------------
+// With a ReLU key activation about half of K's entries are exactly +0.0, and the ring above loads every one of them once per
+// edge.  A packed table keeps, per node n, one slot of ldt floats (a multiple of 16, so that every slot starts on a 64-byte
+// boundary; ops.gat_packed_width takes a multiple of 32, as 128-byte aligned slots are read faster):
+//     [0, A)        V[n]
+//     [A, A + 4)    zero mask, 128 bits: bit c set <=> the bits of K[n, c] are not 0x00000000
+//     [A + 4, ...)  the entries of K[n] whose bit is set, in column order, zero-padded to a multiple of four floats
+// and ksize[n] = (A + 4 + padded count) / 4, the 16-byte units a neighbour's copy takes.  Only the bit pattern 0x00000000 is
+// dropped (-0.0, NaN, inf and denormals are stored), so the reader rebuilds K[n] bit for bit whatever the activation was, and
+// runs the arithmetic of gat_tma4_kernel on the same values: the output is bit-identical.  One warp per node, four columns a lane.
+constexpr int kPackWarps = 8;
+
+__global__ void __launch_bounds__(kPackWarps * 32) gat_pack_keys_kernel(const float *__restrict__ K, int64_t ldk, int32_t N,
+                                                                       int32_t A, float *__restrict__ table, int64_t ldt,
+                                                                       uint8_t *__restrict__ ksize) {
+    const int lane = threadIdx.x & 31;
+    const int64_t n = (int64_t)blockIdx.x * kPackWarps + (threadIdx.x >> 5);
+    if (n >= N) return;
+    const int ccol = lane * 4;
+    const float4 k = ccol < A ? __ldg(reinterpret_cast<const float4 *>(K + n * ldk + ccol)) : make_float4(0.f, 0.f, 0.f, 0.f);
+    const uint32_t nib = (__float_as_uint(k.x) != 0u ? 1u : 0u) | (__float_as_uint(k.y) != 0u ? 2u : 0u) |
+                         (__float_as_uint(k.z) != 0u ? 4u : 0u) | (__float_as_uint(k.w) != 0u ? 8u : 0u);
+    uint32_t word = nib << ((lane & 7) * 4);          // mask word lane / 8 holds columns 32 (lane / 8) ... + 31
+    word |= __shfl_xor_sync(0xffffffffu, word, 1);
+    word |= __shfl_xor_sync(0xffffffffu, word, 2);
+    word |= __shfl_xor_sync(0xffffffffu, word, 4);
+    const int cnt = __popc(nib);
+    int incl = cnt;                                   // inclusive prefix count of set entries over the lanes
+#pragma unroll
+    for (int off = 1; off < 32; off <<= 1) {
+        const int t = __shfl_up_sync(0xffffffffu, incl, off);
+        if (lane >= off) incl += t;
+    }
+    const int total = __shfl_sync(0xffffffffu, incl, 31);
+    const uint32_t m0 = __shfl_sync(0xffffffffu, word, 0), m1 = __shfl_sync(0xffffffffu, word, 8);
+    const uint32_t m2 = __shfl_sync(0xffffffffu, word, 16), m3 = __shfl_sync(0xffffffffu, word, 24);
+    float *slot = table + n * ldt;
+    if (lane == 0) *reinterpret_cast<uint4 *>(slot + A) = make_uint4(m0, m1, m2, m3);
+    float *packed = slot + A + 4;
+    int o = incl - cnt;
+    if (nib & 1u) packed[o++] = k.x;
+    if (nib & 2u) packed[o++] = k.y;
+    if (nib & 4u) packed[o++] = k.z;
+    if (nib & 8u) packed[o] = k.w;
+    const int padded = (total + 3) & ~3;
+    if (lane < padded - total) packed[total + lane] = 0.0f;
+    if (lane == 0) ksize[n] = (uint8_t)((A + 4 + padded) / 4);
+}
+
+// gat_tma4_kernel<S, float> over a packed table (p.K = table, p.ldk = ldt, p.ksize): lanes 0-3 copy 16 * ksize bytes of each
+// neighbour's slot (V, mask, packed keys) into a fixed, 128-byte aligned place of 8A + 16 bytes or more in the ring stage (the
+// copies run measurably slower into places that are only 16-byte aligned), and lane 0 arms the stage with the
+// sum.  Copy sizes travel with the column ids: chunk c + 1's are fetched half-way through issuing chunk c, by when its column
+// ids (fetched one chunk earlier) have arrived.  Each lane rebuilds its four key columns from the mask; the rest is
+// gat_tma4_kernel line for line.
+template <int S>
+__global__ void __launch_bounds__(kGatAsyncWarps * 32) gat_tma4_packed_kernel(const GatParams p) {
+    constexpr int U = 4, RPC = 32 / U;
+    static_assert(S - 1 <= RPC / 2, "the prologue must not reach the round that fetches chunk 1's copy sizes");
+    extern __shared__ __align__(128) uint8_t gat_pk_ring[];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int A = p.H * p.dqk;
+    const uint32_t row_bytes = (uint32_t)A * 4u;
+    const uint32_t slot_bytes = (2u * row_bytes + 16u + 127u) & ~127u;  // the largest copy (no entry of K[n] is zero), 128-byte aligned
+    const uint32_t stage_bytes = (U * slot_bytes + 127u) & ~127u;
+    uint8_t *my_ring = gat_pk_ring + (size_t)warp * S * stage_bytes;
+    const uint32_t ring_addr = (uint32_t)__cvta_generic_to_shared(my_ring);
+    uint64_t *bars = reinterpret_cast<uint64_t *>(gat_pk_ring + (size_t)kGatAsyncWarps * S * stage_bytes) + warp * S;
+    const uint32_t bar0 = (uint32_t)__cvta_generic_to_shared(bars);
+    if (lane == 0) {
+#pragma unroll
+        for (int i = 0; i < S; ++i) asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(bar0 + 8 * i));
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncwarp();
+    const int64_t task = (int64_t)blockIdx.x * kGatAsyncWarps + warp;
+    int64_t r0, r1, e_begin, e_stop;
+    int slot = -1;
+    if (p.task_row != nullptr) {
+        if (task >= p.n_tasks) return;
+        r0 = p.task_row[task];
+        r1 = r0 + p.task_nrows[task];
+        e_begin = p.task_e0[task];
+        e_stop = p.task_e1[task];
+        slot = p.task_slot[task];
+    } else {
+        r0 = task * kGatAsyncRows;
+        if (r0 >= p.N) return;
+        r1 = min((int64_t)p.N, r0 + kGatAsyncRows);
+        e_begin = p.rowptr[r0];
+        e_stop = p.rowptr[r1];
+    }
+    const int64_t rp_hi = p.rowptr[min(r0 + lane + 1, r1)];
+    const int n_edges = (int)(e_stop - e_begin);
+    const int n_rounds = (n_edges + U - 1) / U;
+    const int lanes_per_head = p.dqk >> 2;
+    const int ccol = lane * 4;
+    const bool cok = ccol < A;
+    // the mask bits below column 4 * lane, word by word: their popcount is the lane's offset into the packed keys
+    const int sh = (lane & 7) * 4, wsel = lane >> 3;
+    const uint32_t below_lo = (1u << sh) - 1u;
+    const uint32_t bm0 = wsel > 0 ? ~0u : wsel == 0 ? below_lo : 0u, bm1 = wsel > 1 ? ~0u : wsel == 1 ? below_lo : 0u;
+    const uint32_t bm2 = wsel > 2 ? ~0u : wsel == 2 ? below_lo : 0u, bm3 = wsel == 3 ? below_lo : 0u;
+
+    int64_t r = r0;
+    int row_end = slot >= 0 ? 0x7fffffff : (int)(__shfl_sync(0xffffffffu, rp_hi, 0) - e_begin);
+    float4 q = cok ? ldg4(p.Q + r * p.ldq + ccol) : make_float4(0.f, 0.f, 0.f, 0.f);
+    float4 q_next = (cok && r + 1 < r1) ? ldg4(p.Q + (r + 1) * p.ldq + ccol) : make_float4(0.f, 0.f, 0.f, 0.f);
+    float mx = -FLT_MAX, den = 0.0f, a0 = 0.f, a1 = 0.f, a2 = 0.f, a3 = 0.f;
+    float4 bias = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (p.bias && cok) bias = ldg4(p.bias + ccol);
+
+    auto finalize_row = [&]() {
+        if (cok) {
+            const float inv = 1.0f / (den + 1e-8f);
+            float4 o;
+            o.x = apply_act(a0 * inv + bias.x, p.act);
+            o.y = apply_act(a1 * inv + bias.y, p.act);
+            o.z = apply_act(a2 * inv + bias.z, p.act);
+            o.w = apply_act(a3 * inv + bias.w, p.act);
+            *reinterpret_cast<float4 *>(p.out + r * p.ldo + ccol) = o;
+        }
+        mx = -FLT_MAX; den = 0.0f; a0 = a1 = a2 = a3 = 0.0f;
+        ++r;
+        q = q_next;
+        if (r < r1) {
+            row_end = (int)(__shfl_sync(0xffffffffu, rp_hi, (int)(r - r0)) - e_begin);
+            if (cok && r + 1 < r1) q_next = ldg4(p.Q + (r + 1) * p.ldq + ccol);
+        }
+    };
+    auto load_chunk = [&](int c) {
+        const int e = c * 32 + lane;
+        return e < n_edges ? ld_stream_i32(p.col + e_begin + e) : 0;
+    };
+    auto load_sizes = [&](int ci) { return (int)__ldg(p.ksize + ci); };    // ci = 0 past the last edge: a valid node
+    auto issue = [&](int g, int ci, int si) {
+        if (g < n_rounds) {
+            const int base = (g % RPC) * U;
+            const int valid = min(U, n_edges - g * U);
+            const int src = base + (lane < U ? lane : 0);
+            const int c = __shfl_sync(0xffffffffu, ci, src);
+            const uint32_t bytes = 16u * (uint32_t)__shfl_sync(0xffffffffu, si, src);
+            uint32_t tx = lane < valid ? bytes : 0u;
+            tx += __shfl_xor_sync(0xffffffffu, tx, 1);
+            tx += __shfl_xor_sync(0xffffffffu, tx, 2);                    // lane 0: the sum over lanes 0-3
+            const uint32_t bar = bar0 + 8 * (uint32_t)(g % S);
+            if (lane == 0)
+                asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(tx) : "memory");
+            if (lane < valid)
+                asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+                             ::"r"(ring_addr + (uint32_t)(g % S) * stage_bytes + (uint32_t)lane * slot_bytes),
+                             "l"(p.K + (int64_t)c * p.ldk), "r"(bytes), "r"(bar) : "memory");
+        }
+    };
+
+    int ca = load_chunk(0), cb = load_chunk(1);
+    int sa = load_sizes(ca), sb = 0;
+#pragma unroll
+    for (int g = 0; g < S - 1; ++g) issue(g, ca, sa);
+
+    for (int g = 0; g < n_rounds; ++g) {
+        __syncwarp();                               // every lane has finished reading the stage that is re-armed now
+        {
+            const int gn = g + S - 1;
+            const int k = gn / RPC;
+            if (gn % RPC == RPC / 2) {              // copy sizes of chunk k + 1, whose column ids came one chunk ago
+                if (k & 1) sa = load_sizes(ca); else sb = load_sizes(cb);
+            }
+            issue(gn, (k & 1) ? cb : ca, (k & 1) ? sb : sa);
+        }
+        gat_mbar_wait(bar0 + 8 * (uint32_t)(g % S), (uint32_t)(g / S) & 1u);
+        const uint8_t *sbuf = my_ring + (size_t)(g % S) * stage_bytes;
+        // the four keys of the round are rebuilt before the first edge is consumed: their shared-memory loads and popcounts
+        // overlap instead of lengthening each edge's dependent chain
+        float4 kr[U];
+#pragma unroll
+        for (int u = 0; u < U; ++u) {
+            kr[u] = make_float4(0.f, 0.f, 0.f, 0.f);
+            if (g * U + u < n_edges && cok) {
+                const uint8_t *sl = sbuf + (size_t)u * slot_bytes + row_bytes;
+                const uint4 m = *reinterpret_cast<const uint4 *>(sl);
+                const uint32_t bits = *reinterpret_cast<const uint32_t *>(sl + 4 * wsel) >> sh;
+                int o = __popc(m.x & bm0) + __popc(m.y & bm1) + __popc(m.z & bm2) + __popc(m.w & bm3);
+                const float *pk = reinterpret_cast<const float *>(sl + 16);
+                if (bits & 1u) kr[u].x = pk[o++];
+                if (bits & 2u) kr[u].y = pk[o++];
+                if (bits & 4u) kr[u].z = pk[o++];
+                if (bits & 8u) kr[u].w = pk[o];
+            }
+        }
+#pragma unroll
+        for (int u = 0; u < U; ++u) {
+            const int e = g * U + u;
+            if (e < n_edges) {
+                while (e == row_end) finalize_row();
+                const float4 kk = kr[u];
+                float4 vv = make_float4(0.f, 0.f, 0.f, 0.f);
+                if (cok) vv = *reinterpret_cast<const float4 *>(sbuf + (size_t)u * slot_bytes + ccol * 4);
+                // the contraction gat_tma4_kernel's  q.x*kk.x + q.y*kk.y + q.z*kk.z + q.w*kk.w  compiles to, spelled out:
+                // left to the compiler, keys rebuilt from the mask lead it to fuse the products in another order
+                float d = __fmul_rn(q.x, kk.x);
+                d = fmaf(q.y, kk.y, d);
+                d = fmaf(q.z, kk.z, d);
+                d = fmaf(q.w, kk.w, d);
+                for (int off = 1; off < lanes_per_head; off <<= 1) d += __shfl_xor_sync(0xffffffffu, d, off);
+                const float s = __fdiv_rn(d, p.scale);
+                const bool up = s > mx;
+                const float t = expf(up ? mx - s : s - mx);
+                const float corr = up ? t : 1.0f, pe = up ? 1.0f : t;
+                mx = up ? s : mx;
+                den = fmaf(den, corr, pe);
+                a0 = fmaf(a0, corr, pe * vv.x);
+                a1 = fmaf(a1, corr, pe * vv.y);
+                a2 = fmaf(a2, corr, pe * vv.z);
+                a3 = fmaf(a3, corr, pe * vv.w);
+            }
+        }
+        if ((g + S) % RPC == 0) {
+            const int dead = (g + S) / RPC - 1;
+            if (dead & 1) cb = load_chunk(dead + 2); else ca = load_chunk(dead + 2);
+        }
+    }
+    if (slot >= 0) {
+        float *dst = p.scratch + (int64_t)slot * (A + 64);
+        if (cok) *reinterpret_cast<float4 *>(dst + ccol) = make_float4(a0, a1, a2, a3);
+        dst[A + lane] = mx;
+        dst[A + 32 + lane] = den;
+        return;
+    }
+    while (r < r1) finalize_row();
+}
+
+template <int S>
+static int launch_gat_packed(const GatParams &p, cudaStream_t st) {
+    const size_t slot_bytes = ((size_t)8 * p.H * p.dqk + 16 + 127) & ~(size_t)127;
+    const size_t stage_pitch = (4 * slot_bytes + 127) & ~(size_t)127;
+    const size_t smem = (size_t)kGatAsyncWarps * S * stage_pitch + (size_t)kGatAsyncWarps * S * 8;
+    TFGK_CUDA(ensure_dynamic_smem(gat_tma4_packed_kernel<S>, smem));
+    const int64_t n_tasks = p.task_row ? p.n_tasks : ceil_div64(p.N, kGatAsyncRows);
+    const unsigned blocks = (unsigned)ceil_div64(n_tasks, kGatAsyncWarps);
+    gat_tma4_packed_kernel<S><<<blocks, kGatAsyncWarps * 32, smem, st>>>(p);
+    TFGK_LAUNCH_CHECK();
+    if (p.task_row && p.n_hubs > 0) {
+        gat_hub_fixup_kernel<<<(unsigned)ceil_div64(p.n_hubs, 8), 256, 0, st>>>(p);
+        TFGK_LAUNCH_CHECK();
+    }
+    return TFGK_OK;
+}
+
 // ---- generic path: any H / dqk / dv, split or averaged heads (correctness first) --------------------------------
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
@@ -1055,4 +1305,63 @@ extern "C" int tfgk_gat_fused_bf16(const int64_t *rowptr, const int32_t *col,
     gat_generic_kernel<uint16_t><<<(unsigned)ceil_div64(N, kGatWarps), kGatThreads, smem, st>>>(p);
     TFGK_LAUNCH_CHECK();
     return TFGK_OK;
+}
+
+// packed keys (see gat_pack_keys_kernel): K [N, A] -> the mask and key columns of table's slots, and ksize [N]
+extern "C" int tfgk_gat_pack_keys_f32(const float *K, int64_t ldk, int32_t N, int32_t A, float *table, int64_t ldt,
+                                      uint8_t *ksize, void *stream) {
+    TFGK_CHECK_ARG(N >= 0 && A >= 4 && A <= 128 && A % 4 == 0, "gat_pack_keys: bad size (N=%d A=%d; A must be 4..128, a multiple of 4)",
+                   N, A);
+    TFGK_CHECK_ARG(ldk >= A && ldk % 4 == 0 && ldt >= 2 * A + 4 && ldt % 16 == 0,
+                   "gat_pack_keys: leading dimensions (ldk=%lld, ldt=%lld; ldt a multiple of 16, at least 2A + 4)",
+                   (long long)ldk, (long long)ldt);
+    if (N == 0) return TFGK_OK;
+    TFGK_CHECK_ARG(K && table && ksize, "gat_pack_keys: null pointer");
+    TFGK_CHECK_ARG(aligned16(K) && aligned16(table), "gat_pack_keys: K and table must be 16-byte aligned");
+    gat_pack_keys_kernel<<<(unsigned)ceil_div64(N, kPackWarps), kPackWarps * 32, 0, as_stream(stream)>>>(K, ldk, N, A, table,
+                                                                                                         ldt, ksize);
+    TFGK_LAUNCH_CHECK();
+    return TFGK_OK;
+}
+
+// tfgk_gat_fused_f32 (heads concatenated, dqk == dv) over a packed table: the output bits of the TMA ring over [K | V]
+extern "C" int tfgk_gat_fused_packed_f32(const int64_t *rowptr, const int32_t *col, const float *Q, int64_t ldq,
+                                         const float *table, int64_t ldt, const uint8_t *ksize, int32_t N, int32_t H,
+                                         int32_t dqk, float scale, const float *bias, int act, float *out, int64_t ldo,
+                                         const tfgk_plan *plan, void *stream) {
+    TFGK_CHECK_ARG(N >= 0 && H >= 1 && dqk >= 1, "gat_packed: bad size (N=%d H=%d dqk=%d)", N, H, dqk);
+    TFGK_CHECK_ARG(act == TFGK_ACT_NONE || act == TFGK_ACT_RELU, "gat_packed: unknown activation %d", act);
+    TFGK_CHECK_ARG(scale > 0.0f, "gat_packed: scale must be positive");
+    const int A = H * dqk;
+    if (!(is_pow2(H) && H <= kMaxHeadsFast && dqk % 4 == 0 && is_pow2(dqk / 4) && A <= 128))
+        return set_error(TFGK_ERR_UNSUPPORTED, "gat_packed: H must be a power of two <= 32, dqk / 4 a power of two, H * dqk <= 128");
+    TFGK_CHECK_ARG(ldq >= A && ldo >= A && ldt >= 2 * A + 4, "gat_packed: leading dimension too small");
+    if (N == 0) return TFGK_OK;
+    TFGK_CHECK_ARG(rowptr && col && Q && table && ksize && out, "gat_packed: null pointer");
+    if (ldq % 4 || ldo % 4 || ldt % 16 || !aligned16(Q) || !aligned16(out) || !aligned16(table) || (bias && !aligned16(bias)))
+        return set_error(TFGK_ERR_UNSUPPORTED, "gat_packed: Q, out, bias and table need 16-byte aligned rows, slots of a multiple of 64 bytes");
+
+    GatParams p;
+    p.rowptr = rowptr; p.col = col;
+    p.Q = Q; p.ldq = ldq; p.K = table; p.ldk = ldt; p.V = table; p.ldv = ldt; p.Kb = nullptr; p.Vb = nullptr;
+    p.N = N; p.H = H; p.dqk = dqk; p.dv = dqk; p.scale = scale; p.split = 1;
+    p.bias = bias; p.act = act; p.att = nullptr; p.write_att = 0; p.out = out; p.ldo = ldo;
+    p.n_tasks = 0; p.task_row = nullptr; p.task_nrows = nullptr; p.task_e0 = nullptr; p.task_e1 = nullptr;
+    p.task_slot = nullptr; p.n_hubs = 0; p.hub_row = nullptr; p.hub_slot0 = nullptr; p.hub_nslots = nullptr; p.scratch = nullptr;
+    p.stats = nullptr;
+    p.ksize = ksize;
+    if (plan != nullptr && plan->n_tasks > 0) {
+        if (plan->n_hubs > 0)
+            TFGK_CHECK_ARG(plan->scratch != nullptr && plan->scratch_bytes >= (size_t)plan->n_slots * (A + 64) * sizeof(float),
+                           "gat_packed: plan scratch too small (need %zu bytes)", (size_t)plan->n_slots * (A + 64) * sizeof(float));
+        p.n_tasks = plan->n_tasks; p.task_row = plan->task_row; p.task_nrows = plan->task_nrows;
+        p.task_e0 = plan->task_e0; p.task_e1 = plan->task_e1; p.task_slot = plan->task_slot;
+        p.n_hubs = plan->n_hubs; p.hub_row = plan->hub_row; p.hub_slot0 = plan->hub_slot0;
+        p.hub_nslots = plan->hub_nslots; p.scratch = plan->scratch;
+    }
+    cudaStream_t st = as_stream(stream);
+    // TFGK_GAT_PACKED_STAGES sets the depth of the ring (2, 3 or 4); two stages keep six blocks on an SM and measured fastest
+    const char *env = getenv("TFGK_GAT_PACKED_STAGES");
+    const int stages = env ? atoi(env) : 2;
+    return stages == 3 ? launch_gat_packed<3>(p, st) : stages == 4 ? launch_gat_packed<4>(p, st) : launch_gat_packed<2>(p, st);
 }

@@ -5,6 +5,8 @@ The reference materialises Q[row] and K[col] ([E', A] each), builds a virtual gr
 segment_softmax over H*E' scores and finally a SpMM.  Here: three dense projections, then ONE fused kernel
 (tfgk_gat_fused_f32) that streams K and V rows once per edge.
 """
+import os
+
 import torch
 
 from ... import ops, _structure, _rng, autograd
@@ -92,12 +94,32 @@ def gat(x, edge_index,
 
     q_act, q_left = ops.activation_code(query_activation)
     k_act, k_left = ops.activation_code(key_activation)
-    # Q, K and V come out of ONE launch that reads x once (tfgk_gemm_proj_f32).  K and V land in ONE [N, A + U]
-    # buffer: the fused kernel then fetches a neighbour's key and value from the same DRAM burst
     wq = ops.as_device(query_kernel, torch.float32, device=dev)
     wk = ops.as_device(key_kernel, torch.float32, device=dev)
     wv = ops.as_device(kernel, torch.float32, device=dev)
     a_units = wk.shape[1]
+    act_code, leftover = ops.activation_code(activation)
+    bias = None if bias is None else ops.as_device(bias, torch.float32, device=dev)
+    if not bf16 and not return_attention and k_act == ops.ACT_RELU and k_left is None and x.is_cuda and \
+            _packed_keys_shape(wq, wk, wv, bias, num_heads, split_value_heads) and \
+            os.environ.get("TFGK_GAT_KEYS", "packed") != "dense":
+        # ReLU keys hold many exact zeros: K goes through a scratch buffer into a packed table whose slots hold V, a zero
+        # mask and the non-zero keys, and the fused kernel gathers only those (same output bits as the dense route)
+        Q = torch.empty((num_nodes, a_units), dtype=torch.float32, device=dev)
+        K = torch.empty((num_nodes, a_units), dtype=torch.float32, device=dev)
+        table, sizes = ops.packed_key_table(num_nodes, a_units, dev)
+        project(x, [(wq, ops.as_device(query_bias, torch.float32, device=dev), q_act, Q),
+                    (wk, ops.as_device(key_bias, torch.float32, device=dev), k_act, K),
+                    (wv, None, ops.ACT_NONE, table[:, :a_units])])
+        if q_left is not None:
+            Q = q_left(Q)
+        ops.gat_pack_keys(K, table, sizes)
+        del K
+        h = ops.gat_fused_packed(csr, Q, table, sizes, num_heads, bias=bias, act=act_code)
+        return leftover(h) if leftover is not None else h
+
+    # Q, K and V come out of ONE launch that reads x once (tfgk_gemm_proj_f32).  K and V land in ONE [N, A + U]
+    # buffer: the fused kernel then fetches a neighbour's key and value from the same DRAM burst
     Q = torch.empty((num_nodes, wq.shape[1]), dtype=torch.float32, device=dev)
     # bf16 messages: the projection rounds K | V in its epilogue; Q stays fp32
     kv = torch.empty((num_nodes, a_units + wv.shape[1]), dtype=torch.bfloat16 if bf16 else torch.float32, device=dev)
@@ -115,8 +137,6 @@ def gat(x, edge_index,
         else:
             ops.round_bf16(k_left(K_f32), out=K)
 
-    act_code, leftover = ops.activation_code(activation)
-    bias = None if bias is None else ops.as_device(bias, torch.float32, device=dev)
     res = ops.gat_fused(csr, Q, K, V, num_heads, split_value_heads=split_value_heads, bias=bias, act=act_code,
                         return_attention=return_attention)
     h, att = res if return_attention else (res, None)
@@ -125,6 +145,16 @@ def gat(x, edge_index,
     if return_attention:
         return h, ops.permute(att, csr.perm, inverse=True)     # [E', H] in edge_index-with-self-loops order
     return h
+
+
+def _packed_keys_shape(wq, wk, wv, bias, num_heads, split_value_heads):
+    """The shapes tfgk_gat_fused_packed_f32 takes: the TMA ring's (heads concatenated, Q, K and V of one width A = H * dqk
+    <= 128, H a power of two <= 32, dqk / 4 a power of two) with a 16-byte aligned bias."""
+    H, A = int(num_heads), wk.shape[1]
+    if not split_value_heads or wq.shape[1] != A or wv.shape[1] != A or A > 128 or H < 1 or H > 32 or H & (H - 1) or A % H:
+        return False
+    d4 = (A // H) // 4
+    return (A // H) % 4 == 0 and d4 >= 1 and d4 & (d4 - 1) == 0 and (bias is None or bias.data_ptr() % 16 == 0)
 
 
 def _gat_training(x, csr, edge_index_used, query_kernel, query_bias, query_activation, key_kernel, key_bias,

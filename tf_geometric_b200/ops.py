@@ -408,6 +408,57 @@ def gat_fused(csr, Q, K, V, num_heads, split_value_heads=True, bias=None, act=AC
     return out
 
 
+def gat_packed_width(units):
+    """Floats per slot of a packed key table for A = units (tfgk_gat_pack_keys_f32): V, the 4-float zero mask and at most A
+    keys, rounded up to 32 floats so that every slot starts on a 128-byte boundary (288 = 1,152 bytes at A = 128; the
+    fused kernel reads 128-byte aligned slots measurably faster than 64-byte aligned ones)."""
+    return -(-(2 * int(units) + 4) // 32) * 32
+
+
+def packed_key_table(num_nodes, units, device):
+    """An empty packed key table [num_nodes, gat_packed_width(units)] float32 and its copy sizes [num_nodes] uint8; the
+    V rows go into table[:, :units], then gat_pack_keys fills the rest."""
+    table = torch.empty((int(num_nodes), gat_packed_width(units)), dtype=torch.float32, device=device)
+    sizes = torch.empty((int(num_nodes),), dtype=torch.uint8, device=device)
+    return table, sizes
+
+
+def gat_pack_keys(K, table, sizes):
+    """Writes K [N, A] (float32, A <= 128) into a packed key table: zero mask, non-zero entries in column order, copy size per
+    node (tfgk_gat_pack_keys_f32).  Only the bit pattern 0x00000000 counts as zero."""
+    if not (K.is_cuda and K.dtype == torch.float32 and K.dim() == 2):
+        raise TypeError("gat_pack_keys: K must be a 2-D float32 CUDA tensor")
+    _check(sizes, torch.uint8, "sizes")
+    N, A = K.shape
+    if table.dtype != torch.float32 or table.shape[0] != N or sizes.shape[0] != N:
+        raise ValueError("gat_pack_keys: table and sizes must have {} rows".format(N))
+    _ffi.call("tfgk_gat_pack_keys_f32", _p(K), _row_major_2d(K, "K"), N, A, _p(table), _row_major_2d(table, "table"),
+              _p(sizes), _stream(K))
+    return table, sizes
+
+
+def gat_fused_packed(csr, Q, table, sizes, num_heads, bias=None, act=ACT_NONE, out=None, scale=None):
+    """gat_fused with heads concatenated over a packed key table (tfgk_gat_fused_packed_f32): the same output bits as
+    gat_fused(csr, Q, K, V, ...) for the K that gat_pack_keys packed and V = table[:, :A]."""
+    _check(sizes, torch.uint8, "sizes")
+    if not (Q.is_cuda and Q.dtype == torch.float32 and table.is_cuda and table.dtype == torch.float32):
+        raise TypeError("gat_fused_packed: Q and table must be float32 CUDA tensors")
+    N, H, A = csr.n_rows, int(num_heads), Q.shape[1]
+    if A % H:
+        raise ValueError("attention units ({}) must be divisible by num_heads ({})".format(A, H))
+    if out is None:
+        out = torch.empty((N, A), dtype=torch.float32, device=Q.device)
+    if bias is not None:
+        _check(bias, torch.float32, "bias")
+    scale = float(np.sqrt(np.float32(A // H))) if scale is None else float(scale)
+    plan = getattr(csr, "plan", None)
+    plan_struct = plan.struct(A + 64, Q.device) if plan is not None else None
+    _ffi.call("tfgk_gat_fused_packed_f32", _p(csr.rowptr), _p(csr.col), _p(Q), _row_major_2d(Q, "Q"), _p(table),
+              _row_major_2d(table, "table"), _p(sizes), N, H, A // H, scale, _p(bias), act, _p(out), _row_major_2d(out, "out"),
+              ctypes.byref(plan_struct) if plan_struct is not None else None, _stream(Q))
+    return out
+
+
 def gat_fused_stats(csr, Q, K, V, num_heads, bias=None, act=ACT_NONE, scale=None):
     """Training forward without the [E, H] coefficient table: returns (out, stats[N, 2H]) or None when the shape is not
     taken by the streaming kernel (tfgk_gat_fused_stats_f32)."""
