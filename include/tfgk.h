@@ -26,6 +26,9 @@
 extern "C" {
 #endif
 
+/* Raised when an existing entry point, struct layout or enum value changes meaning.  New symbols, new structs and new
+ * enum values leave a binding written against an earlier header working, so they keep the version (the bf16 and fp8
+ * entries were added under 7). */
 #define TFGK_ABI_VERSION 7
 
 enum tfgk_status {
@@ -44,8 +47,20 @@ enum tfgk_heads_mode { TFGK_HEADS_SPLIT = 0, TFGK_HEADS_BROADCAST = 1, TFGK_HEAD
 enum tfgk_edge_flag { TFGK_FLAG_ALL = 0, TFGK_FLAG_UPPER = 1, TFGK_FLAG_MAPPED = 2 };
 enum tfgk_bernoulli { TFGK_BERNOULLI_NONE = 0, TFGK_BERNOULLI_DROPOUT = 1, TFGK_BERNOULLI_KEEP = 2 };
 enum tfgk_sample_padding { TFGK_SAMPLE_NO_PADDING = 0, TFGK_SAMPLE_PADDING = 1, TFGK_SAMPLE_HEAD = 2 };
-/* element type of a bf16-capable buffer; bf16 data is passed as its 16-bit patterns (uint16_t) */
-enum tfgk_dtype { TFGK_DTYPE_F32 = 0, TFGK_DTYPE_BF16 = 1 };
+/* element type of a bf16-capable buffer; bf16 data is passed as its 16-bit patterns (uint16_t), fp8 data as bytes */
+enum tfgk_dtype { TFGK_DTYPE_F32 = 0, TFGK_DTYPE_BF16 = 1, TFGK_DTYPE_FP8_E4M3 = 2 };
+
+/* fp8 message rows (inference storage of the rows GCN and GAT gather along edges):
+ *   element   OCP e4m3fn bytes (torch.float8_e4m3fn): max 448, no infinities, NaN = 0x7F / 0xFF;
+ *   scale     one int8 exponent k per row and group of 128 columns (group g = columns [128 g, 128 g + 128)), in a separate
+ *             [N, ceil(D / 128)] array (row stride ceil(D / 128) unless stated otherwise);
+ *   exponent  m = max |x| over the group's finite entries; k = the smallest integer with m 2^-k <= 448, clamped to
+ *             [-126, 127]; k = 0 when m = 0 or the group has no finite entry;
+ *   value     q = RNE-to-e4m3fn(x 2^-k) (never saturates); +-inf and NaN are stored as NaN with their sign; -0.0 stays;
+ *   dequant   x^ = float(q) 2^k, exact in fp32 (except that a value rounded up past FLT_MAX, possible only within 2^-4
+ *             of FLT_MAX, becomes inf), so "the fp32 kernel over x^" is a bit-level reference;
+ *   rows      16-byte aligned (ld % 16 == 0) with zeroed pad columns.
+ * |x^ - x| <= max(2^-4 |x|, 2^(k-10)) per element. */
 
 int tfgk_version(void);
 const char *tfgk_last_error(void);
@@ -177,6 +192,22 @@ int tfgk_spmm_bf16_dual(const int64_t *rowptr, const int32_t *col, const float *
                         float *out, int64_t ldo, uint16_t *out_bf16, int64_t ldob,
                         const tfgk_plan *plan, void *stream);
 
+/* The same with fp8 rows h and exponents h_exp ([N, ceil(D / 128)] int8, 2-byte aligned when D > 128); w, addend, bias,
+ * the accumulators and out stay fp32.  Each element is widened and multiplied by 2^k of its row's group, then the fp32
+ * arithmetic runs in the same order; the plan is used exactly where tfgk_spmm_f32 uses it over the dequantised table with
+ * the same leading dimension, and rows without the plan are summed strictly in CSR order, so the output is bit-identical
+ * to tfgk_spmm_f32 over x^ wherever both use the plan or neither does.  Rows 16-byte aligned with ldh % 16 == 0 and
+ * ldh >= D rounded up to 16, up to 256 columns, take the TMA ring (read with their pad columns, which are computed and
+ * never stored; the plan's scratch holds D rounded up to 16 floats per slot); every other shape takes a scalar path
+ * without the plan (a hub row of a table wider than 256 columns is then summed in order, unlike in fp32).
+ * TFGK_SPMM_FP8_STAGES sets the ring depth (6, 8 or 12; default 12).
+ * Algorithmic bytes: E*(D + 1 [+1 for D > 128] + 4 [+4 weighted]) + N*(4*D + 8). */
+int tfgk_spmm_fp8(const int64_t *rowptr, const int32_t *col, const float *w,
+                  const uint8_t *h, int64_t ldh, const int8_t *h_exp, int32_t n_dst, int32_t D, int reduce,
+                  float alpha, const float *addend, int64_t ld_addend, float beta,
+                  const float *bias, int act,
+                  float *out, int64_t ldo, const tfgk_plan *plan, void *stream);
+
 /* ---- K3: edge softmax and fused GAT ------------------------------------------------------------------------- */
 
 /* nn/kernel/segment.py:26-33 segment_softmax over CSR segments, H interleaved score columns:
@@ -208,6 +239,18 @@ int tfgk_gat_fused_bf16(const int64_t *rowptr, const int32_t *col,
                         int32_t N, int32_t H, int32_t dqk, int32_t dv, float scale, int split_value_heads,
                         const float *bias, int act, float *att, int write_att, float *out, int64_t ldo,
                         const tfgk_plan *plan, void *stream);
+/* The same with fp8 K | V in ONE [N, 2A]-byte buffer KV (K in bytes [0, A), V in [A, 2A) of a row; ldkv % 16 == 0,
+ * 16-byte aligned) with kv_exp [N, 2] int8 (K group, V group; 2-byte aligned), inference only: heads concatenated,
+ * dqk == dv, H a power of two, dqk / 4 a power of two, A = H * dqk <= 128.  Q, bias and out are fp32, 16-byte aligned.
+ * The TMA ring copies 2A bytes (rounded up to 16) per neighbour and reads its two exponents; each element is widened
+ * and scaled by 2^k, then the fp32 ring's arithmetic runs with its lane mapping, so the output is bit-identical to
+ * tfgk_gat_fused_f32 over Q, K^, V^ wherever that takes its TMA ring.  Every other shape returns TFGK_ERR_UNSUPPORTED (no
+ * attention coefficients are returned).  The plan's hub scratch takes A + 64 floats per slot.  TFGK_GAT_FP8_STAGES sets
+ * the ring depth (3, 4, 6 or 8; default 6).  Algorithmic bytes: E*(2A + 2 + 4) + N*(8A + 8). */
+int tfgk_gat_fused_fp8(const int64_t *rowptr, const int32_t *col, const float *Q, int64_t ldq,
+                       const uint8_t *KV, int64_t ldkv, const int8_t *kv_exp, int32_t N, int32_t H, int32_t dqk,
+                       float scale, const float *bias, int act, float *out, int64_t ldo,
+                       const tfgk_plan *plan, void *stream);
 /* Packed keys: a table of one slot of ldt floats per node (ldt a multiple of 16, at least 2A + 4; A = H * dqk <= 128):
  *     [0, A) V[n] | [A, A + 4) zero mask, bit c set <=> the bits of K[n, c] are not 0x00000000 |
  *     [A + 4, ...) the entries of K[n] whose bit is set, in column order, zero-padded to a multiple of four floats
@@ -275,6 +318,30 @@ int tfgk_gemm_proj_mixed(const float *const *A_parts, int32_t n_parts, int64_t p
                          int32_t first_part, int32_t max_ctas, void *stream);
 /* dst[r, c] = bf16(src[r, c]) rounded to nearest even, r < rows, c < cols. */
 int tfgk_round_bf16(const float *src, int64_t lds, int32_t rows, int32_t cols, uint16_t *dst, int64_t ldd, void *stream);
+/* tfgk_gemm_proj_mixed with fp8 blocks as well: a TFGK_DTYPE_FP8_E4M3 block stores the fp32 result of its epilogue (bias,
+ * activation) in the fp8 format above, one exponent per row (a block is at most 128 columns: one group) written to
+ * E[row * lde] (e.g. column g of a [N, G] exponent array).  The bytes and exponents are those of tfgk_quantize_fp8 over
+ * tfgk_gemm_proj_f32's output.  In the m64n128 accumulator layout a row's columns sit in the four threads of a quad: two
+ * xor-shuffles give the row maximum, each thread scales its values and packs pairs with cvt.rn.satfinite.e4m3x2.f32.  GAT's
+ * fp32 Q and fp8 K | V thus come from one launch that reads x once.  Only n_parts == 1; other limits as tfgk_gemm_proj_f32. */
+typedef struct tfgk_proj_block_fp8 {
+    const float *B; int64_t ldb;       /* as in tfgk_proj_block */
+    int32_t ncols;
+    int32_t transB;
+    const float *bias;
+    int act;
+    void *C; int64_t ldc;              /* [M, ncols] output of type c_dtype (may be a column slice) */
+    int32_t c_dtype;                   /* tfgk_dtype */
+    int8_t *E; int64_t lde;            /* TFGK_DTYPE_FP8_E4M3 only: the row exponents, E[row * lde] */
+} tfgk_proj_block_fp8;
+int tfgk_gemm_proj_fp8(const float *const *A_parts, int32_t n_parts, int64_t part_rows, int64_t lda,
+                       int32_t M, int32_t K, const tfgk_proj_block_fp8 *blocks, int32_t n_blocks,
+                       int32_t first_part, int32_t max_ctas, void *stream);
+/* dst = the fp8 format above of src [rows, cols] (leading dimension lds), exps[r * lde + g] for group g < ceil(cols / 128):
+ * for tables tfgk_gemm_proj_fp8 refuses (K > 184), the same bytes it would write from the same fp32 values.  Only the
+ * first cols bytes of a row are written. */
+int tfgk_quantize_fp8(const float *src, int64_t lds, int32_t rows, int32_t cols, uint8_t *dst, int64_t ldd,
+                      int8_t *exps, int64_t lde, void *stream);
 
 /* ---- K5: peer memory for the partitioned path (SURVEY.md 8e) ---------------------------------------------------
  * The ONE exception to "the library never allocates": buffers that other ranks on the same node read over NVLink

@@ -25,7 +25,7 @@ BERNOULLI_NONE, BERNOULLI_DROPOUT, BERNOULLI_KEEP = 0, 1, 2
 SAMPLE_NO_PADDING, SAMPLE_PADDING, SAMPLE_HEAD = 0, 1, 2
 NEG_UPPER, NEG_START = 0, 1
 PAD_ROW_MAJOR, PAD_STEP_MAJOR = 0, 1
-DTYPE_F32, DTYPE_BF16 = 0, 1
+DTYPE_F32, DTYPE_BF16, DTYPE_FP8_E4M3 = 0, 1, 2
 
 _i32, _i64, _f32, _int = ctypes.c_int32, ctypes.c_int64, ctypes.c_float, ctypes.c_int
 _ptr, _size = ctypes.c_void_p, ctypes.c_size_t
@@ -59,11 +59,15 @@ SIGNATURES = {
                        _ptr, _ptr],
     "tfgk_spmm_bf16_dual": [_ptr, _ptr, _ptr, _ptr, _i64, _i32, _i32, _int, _f32, _ptr, _i64, _f32, _ptr, _int, _ptr,
                             _i64, _ptr, _i64, _ptr, _ptr],
+    "tfgk_spmm_fp8": [_ptr, _ptr, _ptr, _ptr, _i64, _ptr, _i32, _i32, _int, _f32, _ptr, _i64, _f32, _ptr, _int, _ptr,
+                      _i64, _ptr, _ptr],
     "tfgk_segment_softmax_f32": [_ptr, _ptr, _i32, _i32, _ptr, _ptr],
     "tfgk_gat_fused_f32": [_ptr, _ptr, _ptr, _i64, _ptr, _i64, _ptr, _i64, _i32, _i32, _i32, _i32, _f32, _int, _ptr,
                            _int, _ptr, _int, _ptr, _i64, _ptr, _ptr],
     "tfgk_gat_fused_bf16": [_ptr, _ptr, _ptr, _i64, _ptr, _i64, _ptr, _i64, _i32, _i32, _i32, _i32, _f32, _int, _ptr,
                             _int, _ptr, _int, _ptr, _i64, _ptr, _ptr],
+    "tfgk_gat_fused_fp8": [_ptr, _ptr, _ptr, _i64, _ptr, _i64, _ptr, _i32, _i32, _i32, _f32, _ptr, _int, _ptr, _i64, _ptr,
+                           _ptr],
     "tfgk_gat_pack_keys_f32": [_ptr, _i64, _i32, _i32, _ptr, _i64, _ptr, _ptr],
     "tfgk_gat_fused_packed_f32": [_ptr, _ptr, _ptr, _i64, _ptr, _i64, _ptr, _i32, _i32, _i32, _f32, _ptr, _int, _ptr, _i64,
                                   _ptr, _ptr],
@@ -73,6 +77,8 @@ SIGNATURES = {
     "tfgk_gemm_proj_f32": [_ptr, _i32, _i64, _i64, _i32, _i32, _ptr, _i32, _i32, _i32, _ptr],
     "tfgk_gemm_proj_mixed": [_ptr, _i32, _i64, _i64, _i32, _i32, _ptr, _i32, _i32, _i32, _ptr],
     "tfgk_round_bf16": [_ptr, _i64, _i32, _i32, _ptr, _i64, _ptr],
+    "tfgk_gemm_proj_fp8": [_ptr, _i32, _i64, _i64, _i32, _i32, _ptr, _i32, _i32, _i32, _ptr],
+    "tfgk_quantize_fp8": [_ptr, _i64, _i32, _i32, _ptr, _i64, _ptr, _i64, _ptr],
     "tfgk_peer_alloc": [_size, ctypes.POINTER(_ptr)],
     "tfgk_peer_free": [_ptr],
     "tfgk_peer_export": [_ptr, _ptr],
@@ -144,6 +150,11 @@ class ProjBlock(ctypes.Structure):
 class ProjBlockOut(ctypes.Structure):
     """struct tfgk_proj_block_out of include/tfgk.h."""
     _fields_ = ProjBlock._fields_ + [("c_dtype", _i32)]
+
+
+class ProjBlockFp8(ctypes.Structure):
+    """struct tfgk_proj_block_fp8 of include/tfgk.h."""
+    _fields_ = ProjBlockOut._fields_ + [("E", _ptr), ("lde", _i64)]
 
 
 PEER_HANDLE_BYTES = 64

@@ -124,4 +124,63 @@ template <> __device__ __forceinline__ float4 load_row4<uint16_t>(const uint8_t 
 
 inline bool aligned8(const void *p) { return (reinterpret_cast<uintptr_t>(p) & 7u) == 0; }
 
+// ---- fp8 message rows (OCP e4m3fn with one power-of-two exponent k per row and group of 128 columns, tfgk.h) ----------
+// Dequantised value x^ = float(q) * 2^k: e4m3 -> f16 -> f32 is exact, and so is the product for every k in [-126, 127],
+// so a kernel that widens each element this way and then runs the fp32 arithmetic computes exactly what the fp32 kernel
+// computes over the dequantised table.
+
+// 2^e for e in [-127, 127] (2^-127 is the one subnormal)
+__device__ __forceinline__ float pow2i(int e) {
+    return e >= -126 ? __int_as_float((e + 127) << 23) : __int_as_float(0x00400000);
+}
+__device__ __forceinline__ float f16_bits_to_f32(unsigned short h) {
+    float f;
+    asm("cvt.f32.f16 %0, %1;" : "=f"(f) : "h"(h));
+    return f;
+}
+// two e4m3 bytes (low byte first) -> f16x2 (low half first), exact
+__device__ __forceinline__ uint32_t e4m3x2_to_f16x2(unsigned short b) {
+    uint32_t r;
+    asm("cvt.rn.f16x2.e4m3x2 %0, %1;" : "=r"(r) : "h"(b));
+    return r;
+}
+__device__ __forceinline__ float e4m3_to_f32(uint32_t byte) {
+    return f16_bits_to_f32((unsigned short)(e4m3x2_to_f16x2((unsigned short)(byte & 0xFFu)) & 0xFFFFu));
+}
+// four e4m3 elements from one 4-byte load, widened (not yet scaled by 2^k)
+template <> __device__ __forceinline__ float4 load_row4<uint8_t>(const uint8_t *p) {
+    const uint32_t t = *reinterpret_cast<const uint32_t *>(p);
+    const uint32_t lo = e4m3x2_to_f16x2((unsigned short)(t & 0xFFFFu)), hi = e4m3x2_to_f16x2((unsigned short)(t >> 16));
+    return make_float4(f16_bits_to_f32((unsigned short)(lo & 0xFFFFu)), f16_bits_to_f32((unsigned short)(lo >> 16)),
+                       f16_bits_to_f32((unsigned short)(hi & 0xFFFFu)), f16_bits_to_f32((unsigned short)(hi >> 16)));
+}
+__device__ __forceinline__ float4 scale4(float4 v, float s) {
+    return make_float4(__fmul_rn(v.x, s), __fmul_rn(v.y, s), __fmul_rn(v.z, s), __fmul_rn(v.w, s));
+}
+// running maximum of |v| over the finite entries of a group
+__device__ __forceinline__ float fp8_amax(float m, float v) {
+    const float a = fabsf(v);
+    return a <= FLT_MAX ? fmaxf(m, a) : m;
+}
+// the smallest k with amax * 2^-k <= 448, clamped to [-126, 127]; 0 for amax == 0 (a group without finite entries).
+// amax = f 2^e with f in [1, 2): k = e - 8 when f <= 1.75 (448 = 1.75 2^8), else e - 7; subnormal amax clamps to -126
+__device__ __forceinline__ int fp8_exponent(float amax) {
+    if (amax == 0.0f) return 0;
+    const uint32_t b = __float_as_uint(amax);
+    const int field = (int)(b >> 23);
+    if (field == 0) return -126;
+    const int k = field - 127 - 8 + ((b & 0x7FFFFFu) > 0x600000u ? 1 : 0);
+    return k < -126 ? -126 : (k > 127 ? 127 : k);
+}
+// x0, x1 -> two e4m3 bytes (x0 in the low byte): RNE of x * inv (inv = 2^-k, the product is exact or far below the
+// smallest e4m3 subnormal); +-inf and NaN become NaN with their sign (0x7F / 0xFF), as e4m3fn has no infinities
+__device__ __forceinline__ uint32_t fp8_pack2(float x0, float x1, float inv) {
+    unsigned short r;
+    asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(r) : "f"(__fmul_rn(x1, inv)), "f"(__fmul_rn(x0, inv)));
+    uint32_t b0 = r & 0xFFu, b1 = (uint32_t)r >> 8;
+    if (!(fabsf(x0) <= FLT_MAX)) b0 = 0x7Fu | ((__float_as_uint(x0) >> 24) & 0x80u);
+    if (!(fabsf(x1) <= FLT_MAX)) b1 = 0x7Fu | ((__float_as_uint(x1) >> 24) & 0x80u);
+    return b0 | (b1 << 8);
+}
+
 }  // namespace tfgk

@@ -34,6 +34,8 @@ struct GatParams {
     const float *K; int64_t ldk;
     const float *V; int64_t ldv;
     const uint16_t *Kb, *Vb;   // bf16 K and V (tfgk_gat_fused_bf16), leading dimensions ldk / ldv
+    const uint8_t *KV8 = nullptr;       // fp8 K | V (tfgk_gat_fused_fp8): one [N, 2A]-byte buffer, leading dimension ldk
+    const int8_t *kvexp = nullptr;      // ... and its [N, 2] exponents (K group, V group)
     int32_t N, H, dqk, dv;
     float scale;
     int split;
@@ -499,15 +501,19 @@ __device__ __forceinline__ void gat_mbar_wait(uint32_t bar, uint32_t parity) {
 template <int S, typename T>
 __global__ void __launch_bounds__(kGatAsyncWarps * 32) gat_tma4_kernel(const GatParams p) {
     constexpr int U = 4, RPC = 32 / U;
+    constexpr bool FP8 = sizeof(T) == 1;
     static_assert(S <= RPC, "index chunk refill assumes the prologue stays inside chunk 0");
     extern __shared__ __align__(128) uint8_t gat_g4_ring[];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int A = p.H * p.dqk;
-    const uint32_t edge_bytes = 2u * (uint32_t)A * (uint32_t)sizeof(T);   // [K row | V row] of one neighbour, contiguous
+    // [K row | V row] of one neighbour, contiguous; fp8 spans are copied up to the next 16 bytes (the row's zeroed pad)
+    const uint32_t edge_bytes = FP8 ? (2u * (uint32_t)A + 15u) & ~15u : 2u * (uint32_t)A * (uint32_t)sizeof(T);
     const uint32_t stage_bytes = (U * edge_bytes + 127u) & ~127u;
     uint8_t *my_ring = gat_g4_ring + (size_t)warp * S * stage_bytes;
     const uint32_t ring_addr = (uint32_t)__cvta_generic_to_shared(my_ring);
     uint64_t *bars = reinterpret_cast<uint64_t *>(gat_g4_ring + (size_t)kGatAsyncWarps * S * stage_bytes) + warp * S;
+    // fp8: the (K, V) exponents of every edge in the ring, [S][U] 16-bit entries per warp (K low byte, V high byte)
+    uint16_t *sexp = reinterpret_cast<uint16_t *>(gat_g4_ring + (size_t)kGatAsyncWarps * S * (stage_bytes + 8)) + warp * S * U;
     const uint32_t bar0 = (uint32_t)__cvta_generic_to_shared(bars);
     if (lane == 0) {
 #pragma unroll
@@ -539,7 +545,7 @@ __global__ void __launch_bounds__(kGatAsyncWarps * 32) gat_tma4_kernel(const Gat
     const int ccol = lane * 4;
     const bool cok = ccol < A;
     const uint32_t row_bytes = (uint32_t)A * (uint32_t)sizeof(T);
-    const T *kv = sizeof(T) == 4 ? (const T *)p.K : (const T *)p.Kb;
+    const T *kv = sizeof(T) == 4 ? (const T *)p.K : sizeof(T) == 2 ? (const T *)p.Kb : (const T *)p.KV8;
 
     int64_t r = r0;
     int row_end = slot >= 0 ? 0x7fffffff : (int)(__shfl_sync(0xffffffffu, rp_hi, 0) - e_begin);
@@ -575,7 +581,15 @@ __global__ void __launch_bounds__(kGatAsyncWarps * 32) gat_tma4_kernel(const Gat
         const int e = c * 32 + lane;
         return e < n_edges ? ld_stream_i32(p.col + e_begin + e) : 0;
     };
+    // fp8: lanes 0-3 load the exponents of the neighbour they copy and store them into sexp at the next issue, a round
+    // later (the load has landed by then); the consumer reads them after a __syncwarp
+    uint32_t xpend = 0;
+    int xslot = -1;
     auto issue = [&](int g, int ci) {
+        if constexpr (FP8) {
+            if (xslot >= 0 && lane < U) sexp[xslot * U + lane] = (uint16_t)xpend;
+            xslot = -1;
+        }
         if (g < n_rounds) {
             const int base = (g % RPC) * U;
             const int valid = min(U, n_edges - g * U);
@@ -588,6 +602,10 @@ __global__ void __launch_bounds__(kGatAsyncWarps * 32) gat_tma4_kernel(const Gat
                 asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
                              ::"r"(ring_addr + (uint32_t)(g % S) * stage_bytes + (uint32_t)lane * edge_bytes),
                              "l"(kv + (int64_t)c * p.ldk), "r"(edge_bytes), "r"(bar) : "memory");
+            if constexpr (FP8) {
+                if (lane < valid) xpend = __ldg(reinterpret_cast<const uint16_t *>(p.kvexp) + c);
+                xslot = g % S;
+            }
         }
     };
 
@@ -601,6 +619,7 @@ __global__ void __launch_bounds__(kGatAsyncWarps * 32) gat_tma4_kernel(const Gat
             const int gn = g + S - 1;
             issue(gn, ((gn / RPC) & 1) ? cb : ca);
         }
+        if constexpr (FP8) __syncwarp();            // the exponents stored by issue() are visible to every lane
         gat_mbar_wait(bar0 + 8 * (uint32_t)(g % S), (uint32_t)(g / S) & 1u);
         const uint8_t *sbuf = my_ring + (size_t)(g % S) * stage_bytes;
 #pragma unroll
@@ -612,6 +631,11 @@ __global__ void __launch_bounds__(kGatAsyncWarps * 32) gat_tma4_kernel(const Gat
                 if (cok) {
                     kk = load_row4<T>(sbuf + (size_t)u * edge_bytes + ccol * sizeof(T));
                     vv = load_row4<T>(sbuf + (size_t)u * edge_bytes + row_bytes + ccol * sizeof(T));
+                    if constexpr (FP8) {                // K^ = float(q) 2^kK, V^ = float(q) 2^kV
+                        const uint32_t xe = sexp[(g % S) * U + u];
+                        kk = scale4(kk, pow2i((int8_t)(xe & 0xFFu)));
+                        vv = scale4(vv, pow2i((int8_t)(xe >> 8)));
+                    }
                 }
                 float d = q.x * kk.x + q.y * kk.y + q.z * kk.z + q.w * kk.w;
                 for (int off = 1; off < lanes_per_head; off <<= 1) d += __shfl_xor_sync(0xffffffffu, d, off);
@@ -702,12 +726,16 @@ static int launch_gat_tma4(const GatParams &p, cudaStream_t st) {
     const int A = p.H * p.dqk;
     // one bulk copy per neighbour: the [K | V] span must be 16-byte aligned and a multiple of 16 bytes
     constexpr int kPer16 = 16 / (int)sizeof(T);
-    const bool adjacent = sizeof(T) == 4 ? p.V == p.K + A : p.Vb == p.Kb + A;
-    const void *base = sizeof(T) == 4 ? (const void *)p.K : (const void *)p.Kb;
-    if (!adjacent || p.ldk != p.ldv || 2 * A > 256 || (p.ldk % kPer16) != 0 || (2 * A) % kPer16 != 0 || !aligned16(base))
+    // fp8: K | V are one buffer by construction, and a span is copied up to the next 16 bytes (within the padded row)
+    const bool adjacent = sizeof(T) == 4 ? p.V == p.K + A : sizeof(T) == 2 ? p.Vb == p.Kb + A : true;
+    const void *base = sizeof(T) == 4 ? (const void *)p.K : sizeof(T) == 2 ? (const void *)p.Kb : (const void *)p.KV8;
+    const size_t edge_bytes = sizeof(T) == 1 ? ((size_t)2 * A + 15) / 16 * 16 : (size_t)2 * A * sizeof(T);
+    if (!adjacent || p.ldk != p.ldv || 2 * A > 256 || (p.ldk % kPer16) != 0 || (sizeof(T) > 1 && (2 * A) % kPer16 != 0) ||
+        (sizeof(T) == 1 && (int64_t)edge_bytes > p.ldk) || !aligned16(base))
         return TFGK_ERR_UNSUPPORTED;
-    const size_t stage_pitch = ((size_t)4 * 2 * A * sizeof(T) + 127) & ~(size_t)127;
-    const size_t smem = (size_t)kGatAsyncWarps * S * stage_pitch + (size_t)kGatAsyncWarps * S * 8;
+    const size_t stage_pitch = ((size_t)4 * edge_bytes + 127) & ~(size_t)127;
+    const size_t smem = (size_t)kGatAsyncWarps * S * stage_pitch + (size_t)kGatAsyncWarps * S * 8 +
+                        (sizeof(T) == 1 ? (size_t)kGatAsyncWarps * S * 4 * sizeof(uint16_t) : 0);
     TFGK_CUDA(ensure_dynamic_smem(gat_tma4_kernel<S, T>, smem));
     const int64_t n_tasks = p.task_row ? p.n_tasks : ceil_div64(p.N, kGatAsyncRows);
     const unsigned blocks = (unsigned)ceil_div64(n_tasks, kGatAsyncWarps);
@@ -1364,4 +1392,54 @@ extern "C" int tfgk_gat_fused_packed_f32(const int64_t *rowptr, const int32_t *c
     const char *env = getenv("TFGK_GAT_PACKED_STAGES");
     const int stages = env ? atoi(env) : 2;
     return stages == 3 ? launch_gat_packed<3>(p, st) : stages == 4 ? launch_gat_packed<4>(p, st) : launch_gat_packed<2>(p, st);
+}
+
+// fp8 K | V (inference): the TMA ring only.  Heads concatenated, dqk == dv, dqk / 4 a power of two, A = H * dqk <= 128, K | V
+// in one [N, 2A]-byte buffer whose rows are 16-byte aligned (ldkv % 16 == 0), one bulk copy of 2A bytes (rounded up to 16)
+// per neighbour, the K and V exponents read per edge.  Each element is widened and scaled by 2^k on its way out of shared
+// memory, then gat_tma4_kernel's fp32 arithmetic runs with its lane mapping: the output is bit-identical to
+// tfgk_gat_fused_f32 over Q, K^, V^ wherever that takes its TMA ring.  Every other shape is TFGK_ERR_UNSUPPORTED.
+extern "C" int tfgk_gat_fused_fp8(const int64_t *rowptr, const int32_t *col, const float *Q, int64_t ldq,
+                                  const uint8_t *KV, int64_t ldkv, const int8_t *kv_exp, int32_t N, int32_t H, int32_t dqk,
+                                  float scale, const float *bias, int act, float *out, int64_t ldo,
+                                  const tfgk_plan *plan, void *stream) {
+    TFGK_CHECK_ARG(N >= 0 && H >= 1 && dqk >= 1, "gat_fp8: bad size (N=%d H=%d dqk=%d)", N, H, dqk);
+    TFGK_CHECK_ARG(act == TFGK_ACT_NONE || act == TFGK_ACT_RELU, "gat_fp8: unknown activation %d", act);
+    TFGK_CHECK_ARG(scale > 0.0f, "gat_fp8: scale must be positive");
+    const int A = H * dqk;
+    if (!(is_pow2(H) && H <= kMaxHeadsFast && dqk % 4 == 0 && is_pow2(dqk / 4) && A <= 128))
+        return set_error(TFGK_ERR_UNSUPPORTED, "gat_fused_fp8: only the TMA ring's shapes (H=%d, dqk=%d)", H, dqk);
+    if (N == 0) return TFGK_OK;
+    TFGK_CHECK_ARG(rowptr && col && Q && KV && kv_exp && out, "gat_fp8: null pointer");
+    TFGK_CHECK_ARG(ldq >= A && ldkv >= 2 * A && ldo >= A, "gat_fp8: leading dimension too small");
+    if (!(ldq % 4 == 0 && ldo % 4 == 0 && ldkv % 16 == 0 && aligned16(Q) && aligned16(KV) && aligned16(out) &&
+          (!bias || aligned16(bias)) && (reinterpret_cast<uintptr_t>(kv_exp) & 1u) == 0))
+        return set_error(TFGK_ERR_UNSUPPORTED, "gat_fused_fp8: Q, out, bias and K | V rows must be 16-byte aligned");
+
+    GatParams p;
+    p.rowptr = rowptr; p.col = col;
+    p.Q = Q; p.ldq = ldq; p.K = nullptr; p.ldk = ldkv; p.V = nullptr; p.ldv = ldkv; p.Kb = nullptr; p.Vb = nullptr;
+    p.KV8 = KV; p.kvexp = kv_exp;
+    p.N = N; p.H = H; p.dqk = dqk; p.dv = dqk; p.scale = scale; p.split = 1;
+    p.bias = bias; p.act = act; p.att = nullptr; p.write_att = 0; p.out = out; p.ldo = ldo;
+    p.n_tasks = 0; p.task_row = nullptr; p.task_nrows = nullptr; p.task_e0 = nullptr; p.task_e1 = nullptr;
+    p.task_slot = nullptr; p.n_hubs = 0; p.hub_row = nullptr; p.hub_slot0 = nullptr; p.hub_nslots = nullptr; p.scratch = nullptr;
+    p.stats = nullptr;
+    if (plan != nullptr && plan->n_tasks > 0) {
+        if (plan->n_hubs > 0)
+            TFGK_CHECK_ARG(plan->scratch != nullptr && plan->scratch_bytes >= (size_t)plan->n_slots * (A + 64) * sizeof(float),
+                           "gat_fp8: plan scratch too small (need %zu bytes)", (size_t)plan->n_slots * (A + 64) * sizeof(float));
+        p.n_tasks = plan->n_tasks; p.task_row = plan->task_row; p.task_nrows = plan->task_nrows;
+        p.task_e0 = plan->task_e0; p.task_e1 = plan->task_e1; p.task_slot = plan->task_slot;
+        p.n_hubs = plan->n_hubs; p.hub_row = plan->hub_row; p.hub_slot0 = plan->hub_slot0;
+        p.hub_nslots = plan->hub_nslots; p.scratch = plan->scratch;
+    }
+    cudaStream_t st = as_stream(stream);
+    // 256-byte [K | V] spans at A = 128: six stages keep about as many bytes in flight per warp as three of bf16
+    const char *cfg = getenv("TFGK_GAT_FP8_STAGES");
+    const int stages = cfg ? atoi(cfg) : 6;
+    return stages == 3 ? launch_gat_tma4<3, uint8_t>(p, st)
+         : stages == 4 ? launch_gat_tma4<4, uint8_t>(p, st)
+         : stages == 8 ? launch_gat_tma4<8, uint8_t>(p, st)
+                       : launch_gat_tma4<6, uint8_t>(p, st);
 }

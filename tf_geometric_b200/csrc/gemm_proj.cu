@@ -52,7 +52,9 @@ struct Params {
     int M, K, kpad, nb, tiles_m, n_groups;
     const float *B[kMaxBlocks]; int64_t ldb[kMaxBlocks];
     const float *bias[kMaxBlocks]; int act[kMaxBlocks]; int ncols[kMaxBlocks]; int transb[kMaxBlocks];
-    void *C[kMaxBlocks]; int64_t ldc[kMaxBlocks]; int c_bf16[kMaxBlocks];   // c_bf16: C holds bf16, rounded to nearest even
+    void *C[kMaxBlocks]; int64_t ldc[kMaxBlocks];
+    int c_kind[kMaxBlocks];            // 0: fp32 C; 1: bf16 C, rounded to nearest even; 2: e4m3 C with exponents in E
+    int8_t *E[kMaxBlocks]; int64_t lde[kMaxBlocks];
 };
 
 // shared memory: W hi | W lo | bias | ring of A stages.  With 1024 bytes of W per K (rounded up to 8), 18 432 per A stage
@@ -204,10 +206,12 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_proj_kernel(const Params p) 
     const int act = p.act[cb];
     float *C = static_cast<float *>(p.C[cb]);
     __nv_bfloat16 *Cb = static_cast<__nv_bfloat16 *>(p.C[cb]);
-    const bool c_bf16 = p.c_bf16[cb] != 0;
+    const bool c_bf16 = p.c_kind[cb] == 1;
+    const bool c_fp8 = p.c_kind[cb] == 2;
     const int64_t ldc = p.ldc[cb];
-    // (col, col + 1) as one 8-byte store (fp32) or one 4-byte store (bf16)
-    const bool vec2 = (ldc % 2) == 0 && (reinterpret_cast<uintptr_t>(p.C[cb]) & (c_bf16 ? 3u : 7u)) == 0;
+    // (col, col + 1) as one 8-byte store (fp32), one 4-byte store (bf16) or one 2-byte store (fp8)
+    const bool vec2 = (ldc % 2) == 0 &&
+                      (reinterpret_cast<uintptr_t>(p.C[cb]) & (c_fp8 ? 1u : c_bf16 ? 3u : 7u)) == 0;
     float acc[64];
 #pragma unroll
     for (int i = 0; i < 64; ++i) acc[i] = 0.0f;
@@ -248,6 +252,40 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_proj_kernel(const Params p) 
         if (kb == kb_per_tile - 1) {              // epilogue of the tile: + bias -> act -> C
             wgmma_wait_all();
             const int64_t row0 = (int64_t)tile_index(p, group, j / kb_per_tile) * BM + frag_row;
+            if (c_fp8) {                          // block-uniform: a row's columns sit in the four threads of a quad
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const int64_t row = row0 + 8 * h;
+                    float m = 0.0f;
+#pragma unroll
+                    for (int nb8 = 0; nb8 < kUN / 8; ++nb8) {
+                        const int col = nb8 * 8 + 2 * frag_col;
+                        if (col < ncols) m = fp8_amax(m, apply_act(acc[4 * nb8 + 2 * h] + s_bias[col], act));
+                        if (col + 1 < ncols) m = fp8_amax(m, apply_act(acc[4 * nb8 + 2 * h + 1] + s_bias[col + 1], act));
+                    }
+                    m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 1));
+                    m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 2));
+                    const int k = fp8_exponent(m);
+                    const float inv = pow2i(-k);
+                    if (row < p.M) {
+                        uint8_t *crow = static_cast<uint8_t *>(p.C[cb]) + row * ldc;
+#pragma unroll
+                        for (int nb8 = 0; nb8 < kUN / 8; ++nb8) {
+                            const int col = nb8 * 8 + 2 * frag_col;
+                            const float v0 = apply_act(acc[4 * nb8 + 2 * h] + s_bias[col], act);
+                            const float v1 = apply_act(acc[4 * nb8 + 2 * h + 1] + s_bias[col + 1], act);
+                            const uint32_t q = fp8_pack2(v0, v1, inv);
+                            if (vec2 && col + 1 < ncols) {
+                                *reinterpret_cast<uint16_t *>(crow + col) = (uint16_t)q;
+                            } else {
+                                if (col < ncols) crow[col] = (uint8_t)(q & 0xFFu);
+                                if (col + 1 < ncols) crow[col + 1] = (uint8_t)(q >> 8);
+                            }
+                        }
+                        if (frag_col == 0) p.E[cb][row * p.lde[cb]] = (int8_t)k;
+                    }
+                }
+            } else {
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
                 const int64_t row = row0 + 8 * h;
@@ -281,6 +319,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_proj_kernel(const Params p) 
                     }
                 }
             }
+            }
         }
     };
     for (int j = 0; j < total; j += 2) {
@@ -309,6 +348,38 @@ __global__ void __launch_bounds__(256) round_bf16_kernel(const float *src, int64
     }
 }
 
+// dst = e4m3(src) with one exponent per row and group of 128 columns, for the projections tfgk_gemm_proj_fp8 cannot take;
+// one warp per (row, group), four columns a lane: the same exponent rule and rounding as the K4 epilogue
+__global__ void __launch_bounds__(256) quantize_fp8_kernel(const float *src, int64_t lds, int32_t rows, int32_t cols,
+                                                           uint8_t *dst, int64_t ldd, int8_t *exps, int64_t lde) {
+    const int lane = threadIdx.x & 31;
+    const int n_grp = (cols + 127) / 128;
+    const int64_t n_tasks = (int64_t)rows * n_grp;
+    for (int64_t t = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) / 32; t < n_tasks;
+         t += (int64_t)gridDim.x * blockDim.x / 32) {
+        const int64_t r = t / n_grp;
+        const int g = (int)(t % n_grp);
+        const int c = g * 128 + lane * 4;
+        float v[4];
+        float m = 0.0f;
+#pragma unroll
+        for (int x = 0; x < 4; ++x) {
+            v[x] = c + x < cols ? src[r * lds + c + x] : 0.0f;
+            if (c + x < cols) m = fp8_amax(m, v[x]);
+        }
+#pragma unroll
+        for (int off = 16; off >= 1; off >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, off));
+        const int k = fp8_exponent(m);
+        const float inv = pow2i(-k);
+        const uint32_t q01 = fp8_pack2(v[0], v[1], inv), q23 = fp8_pack2(v[2], v[3], inv);
+        const uint32_t q[4] = {q01 & 0xFFu, q01 >> 8, q23 & 0xFFu, q23 >> 8};
+#pragma unroll
+        for (int x = 0; x < 4; ++x)
+            if (c + x < cols) dst[r * ldd + c + x] = (uint8_t)q[x];
+        if (lane == 0) exps[r * lde + g] = (int8_t)k;
+    }
+}
+
 }  // namespace proj
 }  // namespace tfgk
 
@@ -316,8 +387,8 @@ using namespace tfgk;
 
 // blocks: n_blocks entries (read only when blocks != nullptr); c_bf16[b] != 0 marks a bf16 output block
 static int gemm_proj_impl(const float *const *A_parts, int32_t n_parts, int64_t part_rows, int64_t lda, int32_t M, int32_t K,
-                          const tfgk_proj_block *blocks, const int *c_bf16, int32_t n_blocks, int32_t first_part,
-                          int32_t max_ctas, void *stream) {
+                          const tfgk_proj_block *blocks, const int *c_kind, int8_t *const *E, const int64_t *lde,
+                          int32_t n_blocks, int32_t first_part, int32_t max_ctas, void *stream) {
     TFGK_CHECK_ARG(A_parts != nullptr && blocks != nullptr, "gemm_proj: null argument");
     TFGK_CHECK_ARG(n_parts >= 1 && n_parts <= proj::kMaxParts, "gemm_proj: n_parts=%d not in [1, %d]", n_parts, proj::kMaxParts);
     TFGK_CHECK_ARG(n_blocks >= 1 && n_blocks <= proj::kMaxBlocks, "gemm_proj: n_blocks=%d not in [1, %d]", n_blocks, proj::kMaxBlocks);
@@ -352,7 +423,8 @@ static int gemm_proj_impl(const float *const *A_parts, int32_t n_parts, int64_t 
         }
         p.B[b] = blk.B; p.ldb[b] = blk.ldb; p.bias[b] = blk.bias; p.act[b] = blk.act; p.ncols[b] = blk.ncols;
         p.transb[b] = blk.transB;
-        p.C[b] = blk.C; p.ldc[b] = blk.ldc; p.c_bf16[b] = b < n_blocks ? c_bf16[b] : 0;
+        p.C[b] = blk.C; p.ldc[b] = blk.ldc; p.c_kind[b] = b < n_blocks ? c_kind[b] : 0;
+        p.E[b] = b < n_blocks && E != nullptr ? E[b] : nullptr; p.lde[b] = b < n_blocks && lde != nullptr ? lde[b] : 0;
     }
     const proj::Plan L(K);
     if (L.stages == 0) return TFGK_ERR_UNSUPPORTED;     // W (hi | lo) does not fit next to two A stages
@@ -376,7 +448,8 @@ extern "C" int tfgk_gemm_proj_f32(const float *const *A_parts, int32_t n_parts, 
                                   int32_t M, int32_t K, const tfgk_proj_block *blocks, int32_t n_blocks,
                                   int32_t first_part, int32_t max_ctas, void *stream) {
     const int all_f32[proj::kMaxBlocks] = {0, 0, 0, 0};
-    return gemm_proj_impl(A_parts, n_parts, part_rows, lda, M, K, blocks, all_f32, n_blocks, first_part, max_ctas, stream);
+    return gemm_proj_impl(A_parts, n_parts, part_rows, lda, M, K, blocks, all_f32, nullptr, nullptr, n_blocks, first_part,
+                          max_ctas, stream);
 }
 
 extern "C" int tfgk_gemm_proj_mixed(const float *const *A_parts, int32_t n_parts, int64_t part_rows, int64_t lda,
@@ -397,7 +470,48 @@ extern "C" int tfgk_gemm_proj_mixed(const float *const *A_parts, int32_t n_parts
         c_bf16[b] = o.c_dtype == TFGK_DTYPE_BF16;
     }
     if (n_parts != 1) return set_error(TFGK_ERR_UNSUPPORTED, "gemm_proj_mixed: only a single-part A is supported (n_parts=%d)", n_parts);
-    return gemm_proj_impl(A_parts, n_parts, part_rows, lda, M, K, plain, c_bf16, n_blocks, first_part, max_ctas, stream);
+    return gemm_proj_impl(A_parts, n_parts, part_rows, lda, M, K, plain, c_bf16, nullptr, nullptr, n_blocks, first_part,
+                          max_ctas, stream);
+}
+
+extern "C" int tfgk_gemm_proj_fp8(const float *const *A_parts, int32_t n_parts, int64_t part_rows, int64_t lda,
+                                  int32_t M, int32_t K, const tfgk_proj_block_fp8 *blocks, int32_t n_blocks,
+                                  int32_t first_part, int32_t max_ctas, void *stream) {
+    TFGK_CHECK_ARG(A_parts != nullptr && blocks != nullptr, "gemm_proj: null argument");
+    TFGK_CHECK_ARG(n_blocks >= 1 && n_blocks <= proj::kMaxBlocks, "gemm_proj: n_blocks=%d not in [1, %d]", n_blocks, proj::kMaxBlocks);
+    tfgk_proj_block plain[proj::kMaxBlocks];
+    int kind[proj::kMaxBlocks];
+    int8_t *E[proj::kMaxBlocks];
+    int64_t lde[proj::kMaxBlocks];
+    for (int b = 0; b < n_blocks; ++b) {
+        const tfgk_proj_block_fp8 &o = blocks[b];
+        TFGK_CHECK_ARG(o.c_dtype == TFGK_DTYPE_F32 || o.c_dtype == TFGK_DTYPE_BF16 || o.c_dtype == TFGK_DTYPE_FP8_E4M3,
+                       "gemm_proj: block %d has unknown dtype %d", b, o.c_dtype);
+        if (o.c_dtype == TFGK_DTYPE_BF16)
+            TFGK_CHECK_ARG((reinterpret_cast<uintptr_t>(o.C) & 1u) == 0, "gemm_proj: block %d: bf16 output not 2-byte aligned", b);
+        if (o.c_dtype == TFGK_DTYPE_FP8_E4M3)
+            TFGK_CHECK_ARG(o.E != nullptr && o.lde >= 1, "gemm_proj: block %d: fp8 output without exponents", b);
+        plain[b].B = o.B; plain[b].ldb = o.ldb; plain[b].ncols = o.ncols; plain[b].transB = o.transB;
+        plain[b].bias = o.bias; plain[b].act = o.act; plain[b].C = static_cast<float *>(o.C); plain[b].ldc = o.ldc;
+        kind[b] = o.c_dtype == TFGK_DTYPE_FP8_E4M3 ? 2 : o.c_dtype == TFGK_DTYPE_BF16 ? 1 : 0;
+        E[b] = o.E; lde[b] = o.lde;
+    }
+    if (n_parts != 1) return set_error(TFGK_ERR_UNSUPPORTED, "gemm_proj_fp8: only a single-part A is supported (n_parts=%d)", n_parts);
+    return gemm_proj_impl(A_parts, n_parts, part_rows, lda, M, K, plain, kind, E, lde, n_blocks, first_part, max_ctas, stream);
+}
+
+extern "C" int tfgk_quantize_fp8(const float *src, int64_t lds, int32_t rows, int32_t cols, uint8_t *dst, int64_t ldd,
+                                 int8_t *exps, int64_t lde, void *stream) {
+    TFGK_CHECK_ARG(rows >= 0 && cols >= 0, "quantize_fp8: negative size (rows=%d, cols=%d)", rows, cols);
+    if (rows == 0 || cols == 0) return TFGK_OK;
+    TFGK_CHECK_ARG(src != nullptr && dst != nullptr && exps != nullptr, "quantize_fp8: null pointer");
+    TFGK_CHECK_ARG(lds >= cols && ldd >= cols && lde >= (cols + 127) / 128, "quantize_fp8: leading dimension too small");
+    const int64_t warps = (int64_t)rows * ((cols + 127) / 128);
+    const int64_t blocks = ceil_div64(warps, 8);
+    const unsigned grid = (unsigned)(blocks < 8 * sm_count() ? blocks : 8 * sm_count());
+    proj::quantize_fp8_kernel<<<grid, 256, 0, as_stream(stream)>>>(src, lds, rows, cols, dst, ldd, exps, lde);
+    TFGK_LAUNCH_CHECK();
+    return TFGK_OK;
 }
 
 extern "C" int tfgk_round_bf16(const float *src, int64_t lds, int32_t rows, int32_t cols, uint16_t *dst, int64_t ldd,

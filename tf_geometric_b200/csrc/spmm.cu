@@ -37,6 +37,13 @@ __device__ __forceinline__ void load_vec(const uint16_t *p, float (&v)[VEC]) {
     v[0] = bf16_to_f32(__ldg(p));
 }
 
+// fp8 rows (scalar path only): one widened element, scaled by the caller
+template <int VEC>
+__device__ __forceinline__ void load_vec(const uint8_t *p, float (&v)[VEC]) {
+    static_assert(VEC == 1, "fp8 rows take the scalar path");
+    v[0] = e4m3_to_f32(__ldg(p));
+}
+
 template <int VEC>
 __device__ __forceinline__ void store_vec(float *p, const float (&v)[VEC]) {
     if constexpr (VEC == 4) {
@@ -52,6 +59,11 @@ struct SpmmParams {
     const float *w;
     const float *h;
     const uint16_t *hb;    // bf16 rows (tfgk_spmm_bf16); the kernels instantiated for uint16_t read this one
+    // fp8 rows (tfgk_spmm_fp8, the kernels instantiated for uint8_t): e4m3 bytes and the [N, n_grp] int8 exponents; the
+    // scalar path covers the columns of group grp0 only
+    const uint8_t *h8;
+    const int8_t *hexp;
+    int32_t n_grp, grp0;
     int64_t ldh;
     int32_t n_dst;
     int32_t D;
@@ -85,6 +97,7 @@ struct SpmmParams {
 template <typename T> __device__ __forceinline__ const T *rows_of(const SpmmParams &p);
 template <> __device__ __forceinline__ const float *rows_of<float>(const SpmmParams &p) { return p.h; }
 template <> __device__ __forceinline__ const uint16_t *rows_of<uint16_t>(const SpmmParams &p) { return p.hb; }
+template <> __device__ __forceinline__ const uint8_t *rows_of<uint8_t>(const SpmmParams &p) { return p.h8; }
 
 // The epilogue of tfgk_spmm_bf16_dual for N consecutive columns c .. c+N-1 of row r: the arithmetic of every other
 // epilogue in this file (mean, axpby, bias, activation, in that order and rounding), then the value is stored in fp32
@@ -202,6 +215,13 @@ __global__ void __launch_bounds__(kSpmmThreads) spmm_kernel(const SpmmParams p) 
 #pragma unroll
                 for (int k = 0; k < NC; ++k) {
                     if (ok && cok[k]) load_vec<VEC>(rowp + coff[k], v[u][k]);
+                }
+                if constexpr (sizeof(T) == 1) {             // fp8: x^ = float(q) * 2^k of the source row's group
+                    if (ok) {
+                        const float s = pow2i(__ldg(p.hexp + (int64_t)c * p.n_grp + p.grp0));
+#pragma unroll
+                        for (int k = 0; k < NC; ++k) v[u][k][0] = __fmul_rn(v[u][k][0], s);
+                    }
                 }
             }
 #pragma unroll
@@ -752,6 +772,7 @@ __device__ __forceinline__ void tma_row(uint32_t dst, const void *src, uint32_t 
 template <bool IS_MAX, int S, typename T, bool DUAL = false>
 __global__ void __launch_bounds__(kAsyncWarps * 32) spmm_tma4_kernel(const SpmmParams p, uint32_t row_bytes) {
     constexpr int U = 4, RPC = 32 / U;
+    constexpr bool FP8 = sizeof(T) == 1;
     static_assert(S <= 2 * RPC, "weight look-ahead registers would be overwritten before they are consumed");
     extern __shared__ __align__(128) uint8_t g4_ring[];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -759,6 +780,8 @@ __global__ void __launch_bounds__(kAsyncWarps * 32) spmm_tma4_kernel(const SpmmP
     uint8_t *my_ring = g4_ring + (size_t)warp * S * stage_bytes;
     const uint32_t ring_addr = (uint32_t)__cvta_generic_to_shared(my_ring);
     uint64_t *bars = reinterpret_cast<uint64_t *>(g4_ring + (size_t)kAsyncWarps * S * stage_bytes) + warp * S;
+    // fp8: the exponents of every edge in the ring, [S][U] 16-bit entries per warp (group 0 low byte, group 1 high byte)
+    uint16_t *sexp = reinterpret_cast<uint16_t *>(g4_ring + (size_t)kAsyncWarps * S * (stage_bytes + 8)) + warp * S * U;
     const uint32_t bar0 = (uint32_t)__cvta_generic_to_shared(bars);
     if (lane == 0) {
 #pragma unroll
@@ -842,8 +865,16 @@ __global__ void __launch_bounds__(kAsyncWarps * 32) spmm_tma4_kernel(const SpmmP
             if (weighted) wi = ld_stream_f32(p.w + e_begin + e);
         }
     };
+    // fp8: lanes 0-3 load the exponents of the round they copy into xpend, and store them into sexp at the next issue, a
+    // round later (the load has landed by then and the warp never waits on it); the consumer reads them after a __syncwarp
+    uint32_t xpend = 0;
+    int xslot = -1;
     // round g (edges [4g, 4g+4)) -> ring stage g % S: armed by lane 0, one row copy from each of lanes 0 .. valid-1
     auto issue = [&](int g, int ci) {
+        if constexpr (FP8) {
+            if (xslot >= 0 && lane < U) sexp[xslot * U + lane] = (uint16_t)xpend;
+            xslot = -1;
+        }
         if (g < n_rounds) {
             const int base = (g % RPC) * U;
             const int valid = min(U, n_edges - g * U);
@@ -855,6 +886,12 @@ __global__ void __launch_bounds__(kAsyncWarps * 32) spmm_tma4_kernel(const SpmmP
             if (lane < valid)
                 tma_row(ring_addr + (uint32_t)(g % S) * stage_bytes + (uint32_t)lane * row_bytes,
                         rows_of<T>(p) + (int64_t)c * p.ldh, row_bytes, bar);
+            if constexpr (FP8) {
+                if (lane < valid)
+                    xpend = p.n_grp == 1 ? (uint32_t)(uint8_t)__ldg(p.hexp + c)
+                                         : (uint32_t)__ldg(reinterpret_cast<const uint16_t *>(p.hexp) + c);
+                xslot = g % S;
+            }
         }
     };
 
@@ -872,6 +909,7 @@ __global__ void __launch_bounds__(kAsyncWarps * 32) spmm_tma4_kernel(const SpmmP
             const int gn = g + S - 1;
             issue(gn, ((gn / RPC) & 1) ? cb : ca);
         }
+        if constexpr (FP8) __syncwarp();            // the exponents stored by issue() are visible to every lane
         mbar_wait_parity(bar0 + 8 * (uint32_t)(g % S), (uint32_t)(g / S) & 1u);
         const int cc = g / RPC;
         const float wi = (cc & 1) ? wb : wa;
@@ -883,10 +921,17 @@ __global__ void __launch_bounds__(kAsyncWarps * 32) spmm_tma4_kernel(const SpmmP
             const float we = __shfl_sync(0xffffffffu, wi, base + u);
             if (e < n_edges) {
                 while (e == row_end) finalize_row();
+                float xs[NCX];                          // fp8: 2^k of the source row's groups 0 and 1
+                if constexpr (FP8) {
+                    const uint32_t xe = sexp[(g % S) * U + u];
+                    xs[0] = pow2i((int8_t)(xe & 0xFFu));
+                    xs[1] = pow2i((int8_t)(xe >> 8));
+                }
 #pragma unroll
                 for (int k = 0; k < NCX; ++k) {
                     if (cok[k]) {
-                        const float4 v = load_row4<T>(sbuf + (size_t)u * row_bytes + coff[k] * sizeof(T));
+                        float4 v = load_row4<T>(sbuf + (size_t)u * row_bytes + coff[k] * sizeof(T));
+                        if constexpr (FP8) v = scale4(v, xs[k]);
                         const float m0 = __fmul_rn(v.x, we), m1 = __fmul_rn(v.y, we), m2 = __fmul_rn(v.z, we), m3 = __fmul_rn(v.w, we);
                         acc[k][0] = IS_MAX ? fmaxf(acc[k][0], m0) : __fadd_rn(acc[k][0], m0);
                         acc[k][1] = IS_MAX ? fmaxf(acc[k][1], m1) : __fadd_rn(acc[k][1], m1);
@@ -978,11 +1023,12 @@ template <int S, typename T = float, bool DUAL = false>
 static int launch_spmm_tma4(const SpmmParams &p, cudaStream_t st) {
     // cp.async.bulk wants 16-byte aligned rows: D, ldh multiples of 16 bytes' worth of elements and an aligned base
     constexpr int kPer16 = 16 / (int)sizeof(T);
-    const void *base = sizeof(T) == 4 ? (const void *)p.h : (const void *)p.hb;
+    const void *base = sizeof(T) == 4 ? (const void *)p.h : sizeof(T) == 2 ? (const void *)p.hb : (const void *)p.h8;
     if (p.D > 256 || p.D % kPer16 != 0 || p.ldh % kPer16 != 0 || !aligned16(base)) return TFGK_ERR_UNSUPPORTED;
     const uint32_t row_bytes = (uint32_t)(p.D * sizeof(T));
     const size_t stage_pitch = ((size_t)4 * row_bytes + 127) & ~(size_t)127;
-    const size_t smem = (size_t)kAsyncWarps * S * stage_pitch + (size_t)kAsyncWarps * S * 8;
+    const size_t smem = (size_t)kAsyncWarps * S * stage_pitch + (size_t)kAsyncWarps * S * 8 +
+                        (sizeof(T) == 1 ? (size_t)kAsyncWarps * S * 4 * sizeof(uint16_t) : 0);
     if (smem > 200 * 1024) return TFGK_ERR_UNSUPPORTED;
     const int64_t n_tasks = p.task_row ? p.n_tasks : ceil_div64(p.n_dst, kAsyncRows);
     const unsigned blocks = (unsigned)ceil_div64(n_tasks, kAsyncWarps);
@@ -1117,6 +1163,7 @@ static SpmmParams spmm_params(const int64_t *rowptr, const int32_t *col, const f
     SpmmParams p;
     p.rowptr = rowptr; p.col = col; p.w = w;
     p.h = nullptr; p.hb = nullptr; p.ldh = ldh; p.n_dst = n_dst;
+    p.h8 = nullptr; p.hexp = nullptr; p.n_grp = 0; p.grp0 = 0;
     p.D = width;
     p.reduce = reduce; p.alpha = alpha;
     p.addend = addend ? addend + c0 : nullptr; p.ld_addend = ld_addend; p.beta = beta;
@@ -1290,6 +1337,60 @@ extern "C" int tfgk_spmm_bf16_dual(const int64_t *rowptr, const int32_t *col, co
         p.hb = h + c0;
         p.outb = out_bf16 ? out_bf16 + c0 : nullptr; p.ldob = ldob;
         const int rc = dispatch_spmm<1, uint16_t, true>(p, p.D, st);
+        if (rc != TFGK_OK) return rc;
+    }
+    return TFGK_OK;
+}
+
+// fp8 rows (e4m3 bytes, exponents [N, ceil(D / 128)]).  The kernels are tfgk_spmm_bf16_dual's with a one-byte element:
+// each element is widened to fp32 and scaled by 2^k of its row's group on its way out of shared memory (or global memory
+// on the scalar path), then the fp32 arithmetic runs in the same order.  The plan is taken exactly where tfgk_spmm_f32
+// takes it over the dequantised table with the same leading dimension, and every kernel sums rows without the plan
+// strictly in CSR order, so the output is bit-identical to tfgk_spmm_f32 over x^ wherever both take the plan or neither
+// does.  A table whose rows are 16-byte aligned with ldh >= D rounded up to 16, up to 256 columns, runs on the TMA ring,
+// read with its pad columns (computed, never stored); every other shape takes the scalar path without the plan.
+extern "C" int tfgk_spmm_fp8(const int64_t *rowptr, const int32_t *col, const float *w,
+                             const uint8_t *h, int64_t ldh, const int8_t *h_exp, int32_t n_dst, int32_t D, int reduce,
+                             float alpha, const float *addend, int64_t ld_addend, float beta,
+                             const float *bias, int act,
+                             float *out, int64_t ldo, const tfgk_plan *plan, void *stream) {
+    bool nothing_to_do = true;
+    const int vrc = spmm_validate(rowptr, h, ldh, n_dst, D, reduce, addend, ld_addend, act, out, ldo, plan, &nothing_to_do);
+    if (vrc != TFGK_OK || nothing_to_do) return vrc;
+    TFGK_CHECK_ARG(h_exp != nullptr, "spmm_fp8: null exponent array");
+    const int32_t n_grp = (D + 127) / 128;
+    TFGK_CHECK_ARG(n_grp == 1 || (reinterpret_cast<uintptr_t>(h_exp) & 1u) == 0, "spmm_fp8: exponents not 2-byte aligned");
+    TFGK_CHECK_ARG((reinterpret_cast<uintptr_t>(out) & 3u) == 0, "spmm_fp8: misaligned out");
+
+    const bool in_aligned = (!addend || ((ld_addend % 4 == 0) && aligned16(addend))) && (!bias || aligned16(bias));
+    const bool out4 = (ldo % 4 == 0) && aligned16(out);
+    // tfgk_spmm_f32's plan condition for the dequantised table (16-byte aligned fp32 rows, same ldh in elements)
+    const bool use_plan = D % 4 == 0 && ldh % 4 == 0 && out4 && in_aligned && D >= 32 && D <= 512 && plan != nullptr &&
+                          plan->n_tasks > 0 && spmm_impl_choice() >= 3;
+    const int32_t d16 = (D + 15) / 16 * 16;
+    cudaStream_t st = as_stream(stream);
+    if (ldh % 16 == 0 && ldh >= d16 && aligned16(h) && d16 <= 256) {
+        if (use_plan && plan->n_hubs > 0)
+            TFGK_CHECK_ARG(plan->scratch != nullptr && plan->scratch_bytes >= (size_t)plan->n_slots * d16 * sizeof(float),
+                           "spmm_fp8: plan scratch too small (need %zu bytes)", (size_t)plan->n_slots * d16 * sizeof(float));
+        SpmmParams p = spmm_params(rowptr, col, w, ldh, n_dst, reduce, alpha, addend, ld_addend, beta, bias, act, out, ldo,
+                                   0, d16);
+        p.h8 = h; p.hexp = h_exp; p.n_grp = n_grp;
+        p.d_store = D;
+        p.io4 = D % 4 == 0 && out4 && in_aligned;
+        if (use_plan) spmm_use_plan(p, plan);
+        // 128-byte rows at D = 128: twelve stages keep as many bytes in flight per warp as six stages of bf16 rows
+        const char *cfg = getenv("TFGK_SPMM_FP8_STAGES");
+        const int stages = cfg ? atoi(cfg) : 12;
+        return stages == 6 ? launch_spmm_tma4<6, uint8_t, true>(p, st)
+             : stages == 8 ? launch_spmm_tma4<8, uint8_t, true>(p, st)
+                            : launch_spmm_tma4<12, uint8_t, true>(p, st);
+    }
+    for (int c0 = 0; c0 < D; c0 += 128) {               // scalar path: 32 lanes x 4 single columns = one group per launch
+        SpmmParams p = spmm_params(rowptr, col, w, ldh, n_dst, reduce, alpha, addend, ld_addend, beta, bias, act, out, ldo,
+                                   c0, D - c0 < 128 ? D - c0 : 128);
+        p.h8 = h + c0; p.hexp = h_exp; p.n_grp = n_grp; p.grp0 = c0 / 128;
+        const int rc = dispatch_spmm<1, uint8_t>(p, p.D, st);
         if (rc != TFGK_OK) return rc;
     }
     return TFGK_OK;

@@ -23,10 +23,11 @@ class GAT(Layer):
         :param num_heads: attention heads; split_value_heads=True concatenates per-head slices of the values,
             False lets every head see full-width values and averages the heads
         :param edge_drop_rate: dropout on the attention coefficients while training
-        :param message_dtype: None / torch.float32, or torch.bfloat16 for inference with bf16 keys and values (nn.gat)
+        :param message_dtype: None / torch.float32, or torch.bfloat16 / torch.float8_e4m3fn for inference with bf16 / fp8
+            keys and values (nn.gat)
         """
         super().__init__(*args, **kwargs)
-        ops.message_dtype(message_dtype)          # ValueError for anything but fp32 / bf16
+        ops.conv_message_dtype(message_dtype)     # ValueError for anything but fp32 / bf16 / fp8 e4m3
         self.message_dtype = message_dtype
         for slot in _WEIGHT_SLOTS:                  # declared up front like the reference, created lazily in build()
             setattr(self, slot, None)
@@ -58,8 +59,9 @@ class GAT(Layer):
         several GPUs [x_local, partitioned_graph] (tf_geometric_b200.dist.PartitionedGraph)."""
         if hasattr(inputs[1], "part") and hasattr(inputs[1], "project_all_rows"):
             from ... import dist as tdist
-            if ops.message_dtype(self.message_dtype) is not None:
-                raise NotImplementedError("message_dtype=bfloat16 is not implemented for partitioned graphs")
+            if ops.conv_message_dtype(self.message_dtype) is not None:
+                raise NotImplementedError("message_dtype={} is not implemented for partitioned graphs".format(
+                    str(ops.conv_message_dtype(self.message_dtype)).replace("torch.", "")))
             if not self.split_value_heads:
                 raise NotImplementedError("partitioned GAT concatenates the heads (split_value_heads=True)")
             return tdist.gat_partitioned(inputs[1], inputs[0], self.query_kernel, self.query_bias, self.query_activation,

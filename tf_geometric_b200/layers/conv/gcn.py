@@ -16,9 +16,10 @@ class GCN(Layer):
                  norm="both", add_self_loop=True, sym=True, renorm=True, improved=False,
                  edge_drop_rate=0.0, num_splits=None, num_or_size_splits=None,
                  kernel_regularizer=None, bias_regularizer=None, *args, message_dtype=None, **kwargs):
-        """message_dtype: None / torch.float32, or torch.bfloat16 for inference with bf16 message rows (nn.gcn)."""
+        """message_dtype: None / torch.float32, or torch.bfloat16 / torch.float8_e4m3fn for inference with bf16 / fp8
+        message rows (nn.gcn)."""
         super().__init__(*args, **kwargs)
-        ops.message_dtype(message_dtype)          # ValueError for anything but fp32 / bf16
+        ops.conv_message_dtype(message_dtype)     # ValueError for anything but fp32 / bf16 / fp8 e4m3
         self.message_dtype = message_dtype
         self.units = units
         self.activation = activation
@@ -78,8 +79,9 @@ class GCN(Layer):
         """inputs: [x, sparse_adj], [x, edge_index] or [x, edge_index, edge_weight]; on several GPUs
         [x_local, partitioned_graph] (tf_geometric_b200.dist.PartitionedGraph; x_local may be the result of its share())."""
         if hasattr(inputs[1], "part") and hasattr(inputs[1], "project_all_rows"):
-            if ops.message_dtype(self.message_dtype) is not None:
-                raise NotImplementedError("message_dtype=bfloat16 is not implemented for partitioned graphs")
+            if ops.conv_message_dtype(self.message_dtype) is not None:
+                raise NotImplementedError("message_dtype={} is not implemented for partitioned graphs".format(
+                    str(ops.conv_message_dtype(self.message_dtype)).replace("torch.", "")))
             return self._call_partitioned(inputs[0], inputs[1])
         if isinstance(inputs[1], SparseMatrix):
             x, sparse_adj = inputs

@@ -43,10 +43,17 @@ def gat(x, edge_index,
     :param seed: optional 64-bit key pinning the dropout mask (extension; default: a fresh key per call)
     :param message_dtype: None / torch.float32 (default), or torch.bfloat16: inference with K and V stored in bf16 (rounded
         once, to nearest even, by the projection that also writes the fp32 Q) and read from half the bytes; scores,
-        softmax, accumulation and output stay fp32.  An extension of the reference API
+        softmax, accumulation and output stay fp32.  Or torch.float8_e4m3fn: K | V stored as e4m3 bytes with a power-of-two
+        scale per row (include/tfgk.h), a quarter of fp32's bytes; heads concatenated, units == attention_units = H * dqk
+        <= 128 with dqk / 4 a power of two.  An extension of the reference API
     :return: [num_nodes, units]
     """
-    bf16 = ops.message_dtype(message_dtype) is not None
+    mdt = ops.conv_message_dtype(message_dtype)
+    if mdt is torch.float8_e4m3fn:
+        return _gat_fp8(x, edge_index, query_kernel, query_bias, query_activation, key_kernel, key_bias, key_activation,
+                        kernel, bias, activation, num_heads, split_value_heads, edge_drop_rate, training, cache,
+                        return_attention)
+    bf16 = mdt is not None
     if bf16:
         if as_sparse_features(x) is not None:
             raise NotImplementedError("message_dtype=bfloat16 takes a dense x")
@@ -145,6 +152,52 @@ def gat(x, edge_index,
     if return_attention:
         return h, ops.permute(att, csr.perm, inverse=True)     # [E', H] in edge_index-with-self-loops order
     return h
+
+
+def _gat_fp8(x, edge_index, query_kernel, query_bias, query_activation, key_kernel, key_bias, key_activation, kernel, bias,
+             activation, num_heads, split_value_heads, edge_drop_rate, training, cache, return_attention):
+    """gat() with fp8 K | V: ONE projection launch writes the fp32 Q and the fp8 K | V (bytes and exponents) from one read
+    of x, then tfgk_gat_fused_fp8 gathers 2A bytes per neighbour.  Every refusal comes before any device work."""
+    if as_sparse_features(x) is not None:
+        raise NotImplementedError("message_dtype=float8_e4m3fn takes a dense x")
+    if training and edge_drop_rate > 0.0:
+        raise NotImplementedError("message_dtype=float8_e4m3fn is for inference: attention dropout is not applied in fp8")
+    if return_attention:
+        raise NotImplementedError("message_dtype=float8_e4m3fn does not return attention coefficients; use bfloat16 or "
+                                  "float32")
+    if autograd.needs_grad(x, query_kernel, query_bias, key_kernel, key_bias, kernel, bias):
+        raise NotImplementedError("message_dtype=float8_e4m3fn is for inference: no operand may require grad")
+    H = int(num_heads)
+    A = key_kernel.shape[1]
+    dqk = A // H if H >= 1 and A % H == 0 else 0
+    if not (split_value_heads and query_kernel.shape[1] == A and kernel.shape[1] == A and A <= 128 and 1 <= H <= 32 and
+            not H & (H - 1) and dqk % 4 == 0 and dqk >= 4 and not (dqk // 4) & (dqk // 4 - 1)):
+        raise NotImplementedError(
+            "message_dtype=float8_e4m3fn takes concatenated heads with units == attention_units = num_heads * d <= 128, "
+            "num_heads and d / 4 powers of two (got {} heads, {} attention units, {} units); use bfloat16 or float32".format(
+                H, A, kernel.shape[1]))
+    edge_index = ops.as_device(edge_index, torch.int32)
+    dev = edge_index.device
+    x = ops.as_device(x, torch.float32, device=dev)
+    num_nodes = x.shape[0]
+    csr, _ = _structure.csr_for_edge_index(edge_index, num_nodes, add_self_loop=True, cache=cache)
+    q_act, q_left = ops.activation_code(query_activation)
+    k_act, k_left = ops.activation_code(key_activation)
+    f32 = lambda t: None if t is None else ops.as_device(t, torch.float32, device=dev)     # noqa: E731
+    Q = torch.empty((num_nodes, A), dtype=torch.float32, device=dev)
+    kv = ops.fp8_table(num_nodes, 2 * A, dev, groups=2)
+    K, V = kv.block(0, A, group=0), kv.block(A, 2 * A, group=1)
+    # a key activation the projection cannot fuse is applied in fp32 before the keys are quantised
+    K_f32 = torch.empty((num_nodes, A), dtype=torch.float32, device=dev) if k_left is not None else K
+    ops.gemm_proj(x, [(f32(query_kernel), f32(query_bias), q_act, Q), (f32(key_kernel), f32(key_bias), k_act, K_f32),
+                      (f32(kernel), None, ops.ACT_NONE, V)])
+    if q_left is not None:
+        Q = q_left(Q)
+    if k_left is not None:
+        ops.quantize_fp8(k_left(K_f32), out=K)
+    act_code, leftover = ops.activation_code(activation)
+    h = ops.gat_fused(csr, Q, kv, None, H, bias=f32(bias), act=act_code)
+    return leftover(h) if leftover is not None else h
 
 
 def _packed_keys_shape(wq, wk, wv, bias, num_heads, split_value_heads):

@@ -131,11 +131,16 @@ def gcn(x, sparse_adj, kernel, bias=None, activation=None,
     :param num_or_size_splits: column chunks of the propagation (gcn.py:274-280): one launch per chunk into slices of one
         output, same bits (the fused kernel has no [E, D] temporary to bound, so this is an API-parity feature)
     :param message_dtype: None / torch.float32 (default), or torch.bfloat16: inference with x W stored in bf16 (rounded
-        once, to nearest even, by the projection) and aggregated from half the bytes in fp32; the output is fp32.  An
-        extension of the reference API
+        once, to nearest even, by the projection) and aggregated from half the bytes in fp32; the output is fp32.  Or
+        torch.float8_e4m3fn: x W stored as e4m3 bytes with a power-of-two scale per row (include/tfgk.h), a quarter of
+        the bytes, aggregated in fp32.  An extension of the reference API
     :return: [num_nodes, units]
     """
-    if ops.message_dtype(message_dtype) is not None:
+    mdt = ops.conv_message_dtype(message_dtype)
+    if mdt is torch.float8_e4m3fn:
+        return _gcn_fp8(x, sparse_adj, kernel, bias, activation, norm, add_self_loop, sym, renorm, improved, edge_drop_rate,
+                        training, cache)
+    if mdt is not None:
         return _gcn_bf16(x, sparse_adj, kernel, bias, activation, norm, add_self_loop, sym, renorm, improved, edge_drop_rate,
                          num_or_size_splits, training, cache)
     normed = gcn_norm_adj(sparse_adj, norm=norm, add_self_loop=add_self_loop, sym=sym, renorm=renorm,
@@ -194,4 +199,35 @@ def _gcn_bf16(x, sparse_adj, kernel, bias, activation, norm, add_self_loop, sym,
         h = torch.empty((x.shape[0], kernel.shape[1]), dtype=torch.bfloat16, device=dev)
         project(x, [(kernel, None, ops.ACT_NONE, h)])
     h = normed.matmul(h, num_or_size_splits=num_or_size_splits, bias=bias, act=act_code)
+    return leftover(h) if leftover is not None else h
+
+
+def _gcn_fp8(x, sparse_adj, kernel, bias, activation, norm, add_self_loop, sym, renorm, improved, edge_drop_rate, training,
+             cache):
+    """gcn() with fp8 message rows: act(norm(A) @ dequant(fp8(x W)) + b), the product over the dequantised rows in fp32.
+    The projection writes the bytes and exponents in its epilogue; one aggregation launch reads them (column splits would
+    give the same bits and are not applied)."""
+    if as_sparse_features(x) is not None:
+        raise NotImplementedError("message_dtype=float8_e4m3fn takes a dense x")
+    if training and edge_drop_rate > 0.0:
+        raise NotImplementedError("message_dtype=float8_e4m3fn is for inference: edge dropout is not applied in fp8")
+    if autograd.needs_grad(x, kernel, bias, sparse_adj.value):
+        raise NotImplementedError("message_dtype=float8_e4m3fn is for inference: no operand may require grad")
+    normed = gcn_norm_adj(sparse_adj, norm=norm, add_self_loop=add_self_loop, sym=sym, renorm=renorm,
+                          improved=improved, cache=cache)
+    dev = normed.index.device
+    x = ops.as_device(x, torch.float32, device=dev)
+    act_code, leftover = ops.activation_code(activation)
+    bias = None if bias is None else ops.as_device(bias, torch.float32, device=dev)
+    if kernel is None:
+        h = ops.quantize_fp8(x)
+    else:
+        kernel = ops.as_device(kernel, torch.float32, device=dev)
+        units = kernel.shape[1]
+        h = ops.fp8_table(x.shape[0], units, dev)
+        pieces = [(kernel[:, c0:min(c0 + 128, units)], None, ops.ACT_NONE, h.block(c0, min(c0 + 128, units)))
+                  for c0 in range(0, units, 128)]
+        for i in range(0, len(pieces), 4):
+            ops.gemm_proj(x, pieces[i:i + 4])
+    h = ops.spmm(normed.csr, normed.value_csr, h, reduce="sum", bias=bias, act=act_code)
     return leftover(h) if leftover is not None else h

@@ -280,6 +280,10 @@ def spmm(csr, w_csr, h, reduce="sum", alpha=1.0, addend=None, beta=0.0, bias=Non
     to nearest even.  The fp32 result is then written only into an `out` passed explicitly: with out=None the call
     stores 2 bytes per element and returns out_bf16 (the intermediate hops of a propagation chain).  A bf16 h allocated
     by bf16_table() is read with its pad columns, which keeps every width on the ring kernels."""
+    if isinstance(h, Fp8Table):
+        if out_bf16 is not None:
+            raise TypeError("spmm: an fp8 table takes no out_bf16")
+        return _spmm_fp8(csr, w_csr, h, reduce, alpha, addend, beta, bias, act, out, col)
     if h.dtype not in (torch.float32, torch.bfloat16) or not h.is_cuda:
         raise TypeError("h must be a float32 or bfloat16 CUDA tensor")
     ldh = _row_major_2d(h, "h")
@@ -328,6 +332,123 @@ def spmm(csr, w_csr, h, reduce="sum", alpha=1.0, addend=None, beta=0.0, bias=Non
     return out
 
 
+def _check_fp8_operand(t, name, n_grp, rows=None, device=None):
+    """An Fp8Table the gather kernels can read: CUDA data and exponents on one device, and exponents as a dense
+    [rows, n_grp] array (the kernels index them as row * n_grp + group).  A column block of a wider table (block()) is
+    what gemm_proj and quantize_fp8 write into, but its exponents are strided: it is refused here rather than read with
+    another row's exponents; gather from a table of its own."""
+    if not isinstance(t, Fp8Table):
+        raise TypeError("{} must be an Fp8Table".format(name))
+    e = t.exps
+    if e.shape[1] != n_grp or (n_grp > 1 and e.stride(1) != 1) or (e.shape[0] > 1 and e.stride(0) != n_grp):
+        raise ValueError("{}: the exponents must be a dense [rows, {}] array (got shape {} with strides {}); a column block "
+                         "of a wider table cannot be gathered".format(name, n_grp, tuple(e.shape), tuple(e.stride())))
+    if rows is not None and t.data.shape[0] < rows:
+        raise ValueError("{} has {} rows; the graph references {}".format(name, t.data.shape[0], rows))
+    if not (t.data.is_cuda and e.is_cuda and e.device == t.data.device):
+        raise TypeError("{}: data and exponents must be CUDA tensors on one device".format(name))
+    if device is not None and t.data.device != device:
+        raise ValueError("{} is on {}, the other operands on {}".format(name, t.data.device, device))
+    _row_major_2d(t.data, name)
+
+
+def _spmm_fp8(csr, w_csr, h, reduce, alpha, addend, beta, bias, act, out, col):
+    """spmm over an fp8 table (tfgk_spmm_fp8): bit-identical to the fp32 product over the dequantised table with the same
+    leading dimension wherever both take the work plan or neither does (tables up to 256 columns)."""
+    n_dst, D = csr.n_rows, h.cols
+    _check_fp8_operand(h, "h", max(-(-D // 128), 1), rows=csr.n_cols if col is None else None,
+                       device=None if out is None else out.device)
+    if out is None:
+        out = torch.empty((n_dst, D), dtype=torch.float32, device=h.device)
+    lda = 0 if addend is None else _row_major_2d(addend, "addend")
+    if w_csr is not None:
+        _check(w_csr, torch.float32, "w_csr")
+    if bias is not None:
+        _check(bias, torch.float32, "bias")
+    code = _REDUCE_CODES[reduce] if isinstance(reduce, str) else reduce
+    plan = getattr(csr, "plan", None)
+    # the TMA ring reads the table with its pad columns, hub slices included
+    plan_struct = plan.struct(-(-D // 16) * 16, h.device) if plan is not None else None
+    _ffi.call("tfgk_spmm_fp8", _p(csr.rowptr), _p(csr.col if col is None else col), _p(w_csr), _p(h.data), h.ld, _p(h.exps), n_dst, D, code,
+              float(alpha), _p(addend), lda, float(beta), _p(bias), act, _p(out), _row_major_2d(out, "out"),
+              ctypes.byref(plan_struct) if plan_struct is not None else None, _stream(out))
+    return out
+
+
+class Fp8Table(object):
+    """fp8 message rows in the format of include/tfgk.h: `data` a [rows, cols] uint8 view of e4m3fn bytes whose rows are
+    16-byte aligned (the pad columns of the buffer zeroed), `exps` the int8 exponents, one column per group of 128
+    columns ([rows, ceil(cols / 128)]; a GAT K | V table has two: the K group and the V group) and `cols` the logical
+    width.  fp8_table() allocates one; block() is the view one K4 column block writes."""
+
+    __slots__ = ("data", "exps", "cols")
+
+    def __init__(self, data, exps, cols):
+        if not (torch.is_tensor(data) and data.dtype == torch.uint8 and data.dim() == 2):
+            raise TypeError("Fp8Table: data must be a 2-D uint8 tensor")
+        if not (torch.is_tensor(exps) and exps.dtype == torch.int8 and exps.dim() == 2 and exps.shape[0] == data.shape[0]):
+            raise TypeError("Fp8Table: exps must be a 2-D int8 tensor with one row per data row")
+        if data.shape[1] != cols:
+            raise ValueError("Fp8Table: data has {} columns, expected {}".format(data.shape[1], cols))
+        self.data, self.exps, self.cols = data, exps, int(cols)
+
+    dtype = torch.float8_e4m3fn
+
+    @property
+    def is_cuda(self):
+        return self.data.is_cuda
+
+    @property
+    def device(self):
+        return self.data.device
+
+    @property
+    def shape(self):
+        return self.data.shape
+
+    @property
+    def ld(self):
+        return _row_major_2d(self.data, "fp8 data")
+
+    def block(self, c0, c1, group=None):
+        """Columns [c0, c1) (at most one group of 128) with the exponent column `group` (default c0 // 128)."""
+        g = c0 // 128 if group is None else int(group)
+        if c1 - c0 > 128 or (group is None and c0 % 128):
+            raise ValueError("Fp8Table.block: [{}, {}) is not inside one group of 128 columns".format(c0, c1))
+        return Fp8Table(self.data[:, c0:c1], self.exps[:, g:g + 1], c1 - c0)
+
+
+def fp8_table(rows, cols, device, groups=None):
+    """An empty fp8 table (Fp8Table): rows padded to a multiple of 16 bytes with the pad columns zeroed, exponents
+    [rows, groups] (default ceil(cols / 128))."""
+    pitch = max(-(-int(cols) // 16) * 16, 16)
+    buf = torch.empty((int(rows), pitch), dtype=torch.uint8, device=device)
+    if pitch != cols:
+        buf[:, cols:].zero_()
+    n_grp = max(-(-int(cols) // 128), 1) if groups is None else int(groups)
+    exps = torch.empty((int(rows), n_grp), dtype=torch.int8, device=device)
+    return Fp8Table(buf[:, :cols], exps, cols)
+
+
+def quantize_fp8(src, out=None):
+    """fp8 table of a 2-D float32 CUDA tensor (tfgk_quantize_fp8): the bytes and exponents the K4 epilogue writes from
+    the same values.  `out` may be an Fp8Table (or a block of one) of the same shape."""
+    if not (torch.is_tensor(src) and src.is_cuda and src.dtype == torch.float32 and src.dim() == 2):
+        raise TypeError("quantize_fp8: src must be a 2-D float32 CUDA tensor")
+    if out is None:
+        out = fp8_table(src.shape[0], src.shape[1], src.device)
+    if not isinstance(out, Fp8Table) or tuple(out.shape) != tuple(src.shape):
+        raise TypeError("quantize_fp8: out must be an Fp8Table of shape {}".format(tuple(src.shape)))
+    if out.exps.shape[1] < -(-src.shape[1] // 128) or (out.exps.shape[1] > 1 and out.exps.stride(1) != 1):
+        raise ValueError("quantize_fp8: out has {} exponent columns (column stride {}) for {} columns".format(
+            out.exps.shape[1], out.exps.stride(1), src.shape[1]))
+    if not (out.data.is_cuda and out.exps.is_cuda and out.data.device == src.device and out.exps.device == src.device):
+        raise TypeError("quantize_fp8: out must live on the device of src ({})".format(src.device))
+    _ffi.call("tfgk_quantize_fp8", _p(src), _row_major_2d(src, "src"), src.shape[0], src.shape[1], _p(out.data), out.ld,
+              _p(out.exps), out.exps.stride(0), _stream(src))
+    return out
+
+
 def bf16_table(rows, cols, device):
     """An empty [rows, cols] bfloat16 table for message rows: a view of a row-major buffer whose rows are padded to a
     multiple of 8 elements (16 bytes), pad columns zeroed, so that tfgk_spmm_bf16_dual reads every width with its ring
@@ -358,7 +479,10 @@ def segment_softmax_csr(csr, score_csr):
 def gat_fused(csr, Q, K, V, num_heads, split_value_heads=True, bias=None, act=ACT_NONE, return_attention=False,
               att_buffer=None, out=None, scale=None):
     """Fused GAT attention (tfgk_gat_fused_f32).  K and V may both be bfloat16 (tfgk_gat_fused_bf16, inference only:
-    no return_attention); Q and the output stay float32."""
+    no return_attention); Q and the output stay float32.  K may instead be an Fp8Table holding K | V ([N, 2A] bytes, two
+    exponent columns) with V None (tfgk_gat_fused_fp8, inference only, the TMA ring's shapes)."""
+    if isinstance(K, Fp8Table):
+        return _gat_fused_fp8(csr, Q, K, V, num_heads, split_value_heads, bias, act, return_attention, out, scale)
     bf16 = K.dtype == torch.bfloat16
     for t, n, dt in ((Q, "Q", torch.float32), (K, "K", K.dtype), (V, "V", K.dtype)):
         if not (t.is_cuda and t.dtype == dt and dt in (torch.float32, torch.bfloat16)):
@@ -405,6 +529,35 @@ def gat_fused(csr, Q, K, V, num_heads, split_value_heads=True, bias=None, act=AC
         launch(att)
     if return_attention:
         return out, att[:csr.nnz]
+    return out
+
+
+def _gat_fused_fp8(csr, Q, kv, V, num_heads, split_value_heads, bias, act, return_attention, out, scale):
+    if V is not None:
+        raise TypeError("gat_fused: an fp8 K | V table holds the values as well (pass V=None)")
+    if return_attention or not split_value_heads:
+        raise NotImplementedError("gat_fused: fp8 K | V concatenate the heads and return no attention coefficients")
+    if not (torch.is_tensor(Q) and Q.dtype == torch.float32 and Q.dim() == 2):
+        raise TypeError("Q must be a 2-D float32 CUDA tensor")
+    H, A = int(num_heads), Q.shape[1]
+    if kv.cols != 2 * A or A % H:
+        raise ValueError("gat_fused: an fp8 K | V table has 2A columns, A divisible by num_heads")
+    if Q.shape[0] != csr.n_rows:
+        raise ValueError("gat_fused: Q has {} rows, the graph {}".format(Q.shape[0], csr.n_rows))
+    _check_fp8_operand(kv, "K | V", 2, rows=csr.n_cols)
+    if not (Q.is_cuda and Q.device == kv.device):
+        raise TypeError("Q must be a CUDA tensor on the device of K | V ({})".format(kv.device))
+    dqk = A // H
+    if out is None:
+        out = torch.empty((csr.n_rows, A), dtype=torch.float32, device=Q.device)
+    if bias is not None:
+        _check(bias, torch.float32, "bias")
+    scale = float(np.sqrt(np.float32(dqk))) if scale is None else float(scale)
+    plan = getattr(csr, "plan", None)
+    plan_struct = plan.struct(A + 64, Q.device) if plan is not None else None
+    _ffi.call("tfgk_gat_fused_fp8", _p(csr.rowptr), _p(csr.col), _p(Q), _row_major_2d(Q, "Q"), _p(kv.data), kv.ld,
+              _p(kv.exps), csr.n_rows, H, dqk, scale, _p(bias), act, _p(out), _row_major_2d(out, "out"),
+              ctypes.byref(plan_struct) if plan_struct is not None else None, _stream(Q))
     return out
 
 
@@ -966,15 +1119,31 @@ def gemm_proj(a, blocks, a_parts=None, part_rows=0, first_part=0, max_ctas=0, nu
         n_cols = w.shape[n_dim]
         if out is None:
             out = torch.empty((M, n_cols), dtype=torch.float32, device=a.device)
-        if not (out.is_cuda and out.dtype in (torch.float32, torch.bfloat16)):
+        if isinstance(out, Fp8Table):
+            if out.cols != n_cols or out.data.shape[0] < M or out.exps.shape[1] != 1:
+                raise TypeError("gemm_proj: fp8 out {} must be a block of {} columns with one exponent column".format(
+                    i, n_cols))
+            if not (out.data.is_cuda and out.exps.is_cuda and out.data.device == a.device and out.exps.device == a.device):
+                raise TypeError("gemm_proj: fp8 out {} must live on the device of a ({})".format(i, a.device))
+        elif not (out.is_cuda and out.dtype in (torch.float32, torch.bfloat16)):
             raise TypeError("gemm_proj: out {} must be a float32 or bfloat16 CUDA tensor".format(i))
         if bias is not None:
             _check(bias, torch.float32, "bias")
+        c = out.data if isinstance(out, Fp8Table) else out
         fields.append((w.data_ptr(), _row_major_2d(w, "weight"), n_cols, 1 if trans_b else 0,
-                       None if bias is None else bias.data_ptr(), int(act), out.data_ptr(), _row_major_2d(out, "out")))
+                       None if bias is None else bias.data_ptr(), int(act), c.data_ptr(), _row_major_2d(c, "out")))
         outs.append(out)
     mixed = any(out.dtype == torch.bfloat16 for out in outs)
-    if mixed:
+    fp8 = any(isinstance(out, Fp8Table) for out in outs)
+    if fp8:
+        if a_parts is not None:
+            raise ValueError("gemm_proj: fp8 outputs need a single-part input")
+        structs = (_ffi.ProjBlockFp8 * len(blocks))(*[
+            _ffi.ProjBlockFp8(*(f + ((_ffi.DTYPE_FP8_E4M3, out.exps.data_ptr(), out.exps.stride(0))
+                                     if isinstance(out, Fp8Table) else
+                                     (_ffi.DTYPE_BF16 if out.dtype == torch.bfloat16 else _ffi.DTYPE_F32, None, 0))))
+            for f, out in zip(fields, outs)])
+    elif mixed:
         if a_parts is not None:
             raise ValueError("gemm_proj: bfloat16 outputs need a single-part input")
         structs = (_ffi.ProjBlockOut * len(blocks))(*[
@@ -989,14 +1158,16 @@ def gemm_proj(a, blocks, a_parts=None, part_rows=0, first_part=0, max_ctas=0, nu
         parts = (ctypes.c_void_p * len(a_parts))(*[int(q) for q in a_parts])
         n_parts = len(a_parts)
     try:
-        _ffi.call("tfgk_gemm_proj_mixed" if mixed else "tfgk_gemm_proj_f32", parts, n_parts, int(part_rows), lda, M, K,
+        _ffi.call("tfgk_gemm_proj_fp8" if fp8 else "tfgk_gemm_proj_mixed" if mixed else "tfgk_gemm_proj_f32", parts, n_parts, int(part_rows), lda, M, K,
                   structs, len(blocks), int(first_part), int(max_ctas), _stream(a))
     except _ffi.TfgkError as err:
         if err.code != _ffi.ERR_UNSUPPORTED or n_parts != 1:
             raise
         for blk, out in zip(blocks, outs):
             tb = bool(blk[4]) if len(blk) > 4 else False
-            if out.dtype == torch.bfloat16:     # the fp32 product, then rounded to nearest even
+            if isinstance(out, Fp8Table):       # the fp32 product, then quantised as the epilogue would
+                quantize_fp8(gemm(a[:M], blk[0], bias=blk[1], act=blk[2], trans_b=tb), out=out)
+            elif out.dtype == torch.bfloat16:   # the fp32 product, then rounded to nearest even
                 round_bf16(gemm(a[:M], blk[0], bias=blk[1], act=blk[2], trans_b=tb), out=out)
             else:
                 gemm(a[:M], blk[0], bias=blk[1], act=blk[2], trans_b=tb, out=out)
@@ -1024,6 +1195,19 @@ def message_dtype(value):
     if value is torch.bfloat16 or value == "bfloat16":
         return torch.bfloat16
     raise ValueError("message_dtype must be None, torch.float32 or torch.bfloat16 (got {!r})".format(value))
+
+
+def conv_message_dtype(value):
+    """message_dtype of GCN and GAT, which also take fp8 message rows: None / torch.float32 -> None, torch.bfloat16 /
+    "bfloat16" -> torch.bfloat16, torch.float8_e4m3fn / "float8_e4m3fn" -> torch.float8_e4m3fn; anything else (e5m2
+    included) raises ValueError.  The other convolutions validate with message_dtype(), which refuses fp8."""
+    if value is torch.float8_e4m3fn or value == "float8_e4m3fn":
+        return torch.float8_e4m3fn
+    try:
+        return message_dtype(value)
+    except ValueError:
+        raise ValueError("message_dtype must be None, torch.float32, torch.bfloat16 or torch.float8_e4m3fn (got {!r})".format(
+            value)) from None
 
 
 def colsum(x):
