@@ -609,6 +609,37 @@ int tfgk_spgemm_fill_f32(const int64_t *a_rowptr, const int32_t *a_col, const fl
                          const int64_t *big_ptr, int64_t big_products, const int64_t *c_rowptr, int32_t *c_col,
                          float *c_val, void *workspace, size_t workspace_bytes, void *stream);
 
+/* ---- K11: max aggregation with tie counts, and its backward over the transposed CSR --------------------------------
+ * (max_pool_graph_sage and aggregate_neighbors(max_reducer) training, ASAP's query; graph_sage.py:228-287) */
+
+/* K11a.  out[r,d] = max_{e in row r} w[e] * h[col[e],d]   (w NULL = 1; an empty row gives -FLT_MAX)
+ *        cnt[r,d] = #{e in row r : w[e] * h[col[e],d] == out[r,d]}, int32, IEEE equality: +0 and -0 are ties, NaN never
+ *        counts, and -inf is no tie of an empty row's -FLT_MAX.
+ * out is bit-identical to tfgk_spmm_f32(reduce = MAX, alpha = 1, no epilogue) with the same CSR, weights and plan: fmaxf
+ * in CSR order from -FLT_MAX, products rounded once, and the plan taken exactly where tfgk_spmm_f32 takes it for the same
+ * h and out (16-byte aligned rows, D % 4 == 0, 32 <= D <= 512), its hub slices merged as (max, count) pairs in slice order.
+ * Any D; rows that are not 16-byte aligned or D % 4 != 0 take a scalar path.  The plan's scratch must hold
+ * n_slots * D * 8 bytes.  Counts are exact up to 2^31 - 1 ties.  No atomics.  Asynchronous.
+ * Algorithmic bytes: E*(4*D + 4 [+4 weighted]) + N*(8*D + 8). */
+int tfgk_spmm_max_f32(const int64_t *rowptr, const int32_t *col, const float *w, const float *h, int64_t ldh,
+                      int32_t n_dst, int32_t D, float *out, int64_t ldo, int32_t *cnt, int64_t ldc,
+                      const tfgk_plan *plan, void *stream);
+/* K11b.  The gradient of K11a's out with respect to h, given g = dL/dout, over the TRANSPOSED CSR: row c of rowptr_t lists
+ * the edges leaving source c in stable edge order, dst_t[p] their destination rows and w_t[p] their weights (NULL = 1):
+ *     dh[c,d] = sum_p ((Gn[r,d] * sel) * w_t[p]),   r = dst_t[p],  sel = (w_t[p] * h[c,d] == out[r,d]) ? 1 : 0,
+ *     Gn = g / max(cnt, 1)   (fp32, correctly rounded; written with out into pk = [out | Gn], [n_dst, 2D] contiguous).
+ * Every edge adds its term, selected or not, so an inf or NaN in g reaches every neighbour of its row (0 * inf = NaN),
+ * as the product of the gradient with the 0/1 selection does.  Sums start at 0 and run in edge order with separate
+ * roundings; sources with hub out-degree are summed in the plan's slices (plan taken where tfgk_spmm_f32 takes it for a
+ * dense [E, D] table: D % 4 == 0, 32 <= D <= 512; scratch n_slots * D * 4 bytes) and merged in slice order.  dh is
+ * therefore bit-identical to gathering h, reducing with SegmentReduce(max) and summing the message gradient with K1
+ * (TakeRows).  Every dh row of [0, n_src) is written once; no atomics.  Asynchronous.
+ * Algorithmic bytes: E*(8*D + 4 [+4 weighted]) + N*(8*D + 8), plus 20*D*N for the pass writing pk. */
+int tfgk_spmm_max_bwd_f32(const int64_t *rowptr_t, const int32_t *dst_t, const float *w_t, const float *h, int64_t ldh,
+                          int32_t n_src, int32_t n_dst, int32_t D, const float *out, int64_t ldo, const int32_t *cnt,
+                          int64_t ldc, const float *g, int64_t ldg, float *pk, float *dh, int64_t lddh,
+                          const tfgk_plan *plan, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

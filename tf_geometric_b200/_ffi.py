@@ -131,6 +131,9 @@ SIGNATURES = {
     "tfgk_spgemm_rowptr": [_ptr, _i32, _ptr, ctypes.POINTER(_i64), _ptr, _size, _ptr],
     "tfgk_spgemm_fill_f32": [_ptr, _ptr, _ptr, _ptr, _ptr, _ptr, _i32, _i32, _ptr, _ptr, _i64, _ptr, _ptr, _ptr, _ptr, _size,
                              _ptr],
+    "tfgk_spmm_max_f32": [_ptr, _ptr, _ptr, _ptr, _i64, _i32, _i32, _ptr, _i64, _ptr, _i64, _ptr, _ptr],
+    "tfgk_spmm_max_bwd_f32": [_ptr, _ptr, _ptr, _ptr, _i64, _i32, _i32, _i32, _ptr, _i64, _ptr, _i64, _ptr, _i64, _ptr,
+                              _ptr, _i64, _ptr, _ptr],
 }
 
 

@@ -76,6 +76,61 @@ class NeighborAggregate(torch.autograd.Function):
         return grad_x, None, grad_w, None, None
 
 
+class NeighborMax(torch.autograd.Function):
+    """agg = MAX_{e: row_e = r} w_e x[col_e] (-FLT_MAX for a node without in-edges), differentiable w.r.t. x; edge_weight
+    (None = 1) is a constant.  Forward: K11a, which also counts the ties of every output entry; out, the counts and x are
+    kept ([N, D] each, no per-edge tensor).  Backward: K11b over the transposed CSR (the one NeighborAggregate uses),
+        dx[c] = sum_{e: col_e = c} ((g[row_e] / max(cnt[row_e], 1)) * (w_e x[c] == agg[row_e])) * w_e
+    in edge order, without atomics: the gradient is shared equally among ties, as SegmentReduce's max backward does, and
+    the bits are those of TakeRows + SegmentReduce("max") over the gathered messages."""
+
+    @staticmethod
+    def forward(ctx, x, edge_index, edge_weight, num_nodes):
+        csr, _ = _structure.csr_for_edge_index(edge_index, num_nodes)
+        w_csr = None if edge_weight is None else _structure.weights_in_csr_order(edge_weight.detach(), csr)
+        xd = x.detach()
+        out, cnt = ops.spmm_max(csr, w_csr, xd)
+        ctx.saved = (edge_index, None if edge_weight is None else edge_weight.detach(), int(num_nodes))
+        ctx.save_for_backward(xd, out, cnt)
+        return out
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        edge_index, edge_weight, num_nodes = ctx.saved
+        x, out, cnt = ctx.saved_tensors
+        if not ctx.needs_input_grad[0]:
+            return None, None, None, None
+        csr_t, w_t = _max_transposed(edge_index, num_nodes, edge_weight)
+        return ops.spmm_max_bwd(csr_t, w_t, x, out, cnt, grad_out.contiguous()), None, None, None
+
+
+def _is_device(t):
+    return torch.is_tensor(t) and t.is_cuda
+
+
+def max_aggregate(x, edge_index, num_nodes):
+    """Differentiable MAX_{e: row_e = r} x[col_e]: NeighborMax for device tensors (the operands of every public entry
+    point, which as_device puts on the GPU).  Host tensors take the composition TakeRows + SegmentReduce("max") that
+    NeighborMax replaces bit for bit, whose blocks any host stand-in of the kernel layer provides."""
+    if _is_device(x):
+        return NeighborMax.apply(x, edge_index, None, num_nodes)
+    messages = TakeRows.apply(x, edge_index[1].contiguous())
+    return SegmentReduce.apply(messages, edge_index[0].contiguous(), num_nodes, "max")
+
+
+def _max_transposed(edge_index, num_nodes, edge_weight):
+    """(csr_t, w_t) for NeighborMax's backward: the CSR of the reversed edges (its col = destination rows, stable by
+    source, memoised under the tag _transposed_structure uses) and the weights in its order (None when unweighted)."""
+    tag = ("csc", int(num_nodes))
+    csr_t = _structure._lookup(edge_index, tag)
+    if csr_t is None:
+        row, col = edge_index[0].contiguous(), edge_index[1].contiguous()
+        csr_t = _structure._store(edge_index, tag, ops.csr_build(col, row, num_nodes, num_nodes))
+    if edge_weight is None:
+        return csr_t, None
+    return csr_t, _structure.weights_in_csr_order(edge_weight, csr_t)
+
+
 class Dense(torch.autograd.Function):
     """y = act(x @ W + b) with act in {None, relu}; dX, dW, db through tfgk_gemm_f32."""
 

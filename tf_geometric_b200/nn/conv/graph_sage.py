@@ -161,10 +161,9 @@ def _pool_sage(reduce, x, edge_index, edge_weight, self_kernel, neighbor_mlp_ker
         if reduce == "mean":
             reduced = autograd.NeighborAggregate.apply(h_node, edge_index, None, "mean", num_nodes)
         else:
-            # training only: the per-edge messages are materialised like the reference does (graph_sage.py:262-270), so that
-            # the max can route its gradient to the selected neighbours (ties share it, TF's UnsortedSegmentMax gradient)
-            messages = autograd.TakeRows.apply(h_node, edge_index[1].contiguous())
-            reduced = autograd.SegmentReduce.apply(messages, edge_index[0].contiguous(), num_nodes, "max")
+            # K11: the max keeps a tie count per output entry, and the backward routes the gradient to the selected
+            # neighbours (ties share it, TF's UnsortedSegmentMax gradient) over the transposed CSR: no per-edge messages
+            reduced = autograd.max_aggregate(h_node, edge_index, num_nodes)
         return _project_pair_autograd(x, reduced, f32(self_kernel), f32(neighbor_kernel), f32(bias), activation, concat,
                                       normalize)
     csr, _ = _structure.csr_for_edge_index(edge_index, num_nodes)

@@ -92,13 +92,19 @@ def aggregate_neighbors(x, edge_index, edge_weight=None, mapper=identity_mapper,
     fused = (reducer in _FUSED_REDUCERS and updater in (sum_updater, identity_updater)
              and (mapper is identity_mapper or (mapper is gcn_mapper and edge_weight is not None)))
     if fused and autograd.needs_grad(x, edge_weight):
-        # differentiable route: sum / mean through NeighborAggregate (transposed-CSR backward); max and differentiable
-        # edge weights through the generic route below (gather + SegmentReduce), which torch autograd can follow
-        if _FUSED_REDUCERS[reducer] != "max" and not autograd.needs_grad(edge_weight):
+        # differentiable route: sum / mean through NeighborAggregate, max through NeighborMax (both with a transposed-CSR
+        # backward); differentiable edge weights (and max over host tensors) through the generic route below (gather +
+        # SegmentReduce), which torch autograd can follow
+        is_max = _FUSED_REDUCERS[reducer] == "max"
+        max_ok = autograd._is_device(x) and num_nodes == x.shape[0]       # NeighborMax: device rows, one per node
+        if not autograd.needs_grad(edge_weight) and (not is_max or max_ok):
             w = None
             if mapper is gcn_mapper:
                 w = ops.as_device(edge_weight, torch.float32, device=x.device)
-            agg = autograd.NeighborAggregate.apply(x, edge_index, w, _FUSED_REDUCERS[reducer], num_nodes)
+            if is_max:
+                agg = autograd.NeighborMax.apply(x, edge_index, w, num_nodes)
+            else:
+                agg = autograd.NeighborAggregate.apply(x, edge_index, w, _FUSED_REDUCERS[reducer], num_nodes)
             return x + agg if updater is sum_updater else agg
         fused = False
     if fused:

@@ -77,8 +77,8 @@ def asap(x, edge_index, edge_weight, node_graph_index,
     attention_h = gcn(x, SparseMatrix(ei, weight, [num_nodes, num_nodes]), f32(attention_gcn_kernel),
                       f32(attention_gcn_bias), cache=cache)                                      # adapter 1
 
-    # max aggregate over the self-looped edges, gathered by TakeRows (a deterministic backward)
-    query = autograd.SegmentReduce.apply(autograd.TakeRows.apply(attention_h, col_sl), row_sl, num_nodes, "max")
+    # max aggregate over the self-looped edges (K11: tie counts forward, transposed-CSR backward, no per-edge messages)
+    query = autograd.max_aggregate(attention_h, ei_sl, num_nodes)
     query = autograd.dense(query, f32(attention_query_kernel), f32(attention_query_bias))
 
     w_s = f32(attention_score_kernel)

@@ -332,6 +332,52 @@ def spmm(csr, w_csr, h, reduce="sum", alpha=1.0, addend=None, beta=0.0, bias=Non
     return out
 
 
+def spmm_max(csr, w_csr, h):
+    """(out, cnt): out[r] = max_{e in row r} w[e] * h[col[e]] (-FLT_MAX for an empty row), bit-identical to
+    spmm(reduce="max"), and cnt[r, d] int32 = how many of those products equal out[r, d] (tfgk_spmm_max_f32, K11a)."""
+    if h.dtype != torch.float32 or not h.is_cuda:
+        raise TypeError("spmm_max: h must be a float32 CUDA tensor")
+    ldh = _row_major_2d(h, "h")
+    n, D = csr.n_rows, h.shape[1]
+    if w_csr is not None:
+        _check(w_csr, torch.float32, "w_csr")
+    out = torch.empty((n, D), dtype=torch.float32, device=h.device)
+    cnt = torch.empty((n, D), dtype=torch.int32, device=h.device)
+    plan = getattr(csr, "plan", None)
+    plan_struct = plan.struct(2 * D, h.device) if plan is not None else None
+    _ffi.call("tfgk_spmm_max_f32", _p(csr.rowptr), _p(csr.col), _p(w_csr), _p(h), ldh, n, D, _p(out), max(D, 1), _p(cnt),
+              max(D, 1), ctypes.byref(plan_struct) if plan_struct is not None else None, _stream(h))
+    return out, cnt
+
+
+def spmm_max_bwd(csr_t, w_t, h, out, cnt, g):
+    """dh = d(spmm_max(...)[0]) / dh for upstream g, over the TRANSPOSED CSR csr_t (one row per source node; its `col`
+    holds the destination row of every edge, w_t the weights in its order or None): tfgk_spmm_max_bwd_f32 (K11b).
+    Bit-identical to the gradient of SegmentReduce(max) over the gathered messages summed by TakeRows."""
+    for t, name in ((h, "h"), (out, "out"), (g, "g")):
+        if t.dtype != torch.float32 or not t.is_cuda:
+            raise TypeError("spmm_max_bwd: {} must be a float32 CUDA tensor".format(name))
+    if cnt.dtype != torch.int32:
+        raise TypeError("spmm_max_bwd: cnt must be int32")
+    n_src, D = csr_t.n_rows, h.shape[1]
+    n_dst = out.shape[0]
+    if h.shape[0] != n_src or tuple(out.shape) != (n_dst, D) or tuple(cnt.shape) != (n_dst, D) or \
+            tuple(g.shape) != (n_dst, D):
+        raise ValueError("spmm_max_bwd: shapes h {}, out {}, cnt {}, g {} do not match {} sources".format(
+            tuple(h.shape), tuple(out.shape), tuple(cnt.shape), tuple(g.shape), n_src))
+    if w_t is not None:
+        _check(w_t, torch.float32, "w_t")
+    pk = torch.empty((n_dst, 2 * D), dtype=torch.float32, device=h.device)
+    dh = torch.empty((n_src, D), dtype=torch.float32, device=h.device)
+    plan = getattr(csr_t, "plan", None)
+    plan_struct = plan.struct(D, h.device) if plan is not None else None
+    _ffi.call("tfgk_spmm_max_bwd_f32", _p(csr_t.rowptr), _p(csr_t.col), _p(w_t), _p(h), _row_major_2d(h, "h"), n_src,
+              n_dst, D, _p(out), _row_major_2d(out, "out"), _p(cnt), _row_major_2d(cnt, "cnt"), _p(g),
+              _row_major_2d(g, "g"), _p(pk), _p(dh), max(D, 1), ctypes.byref(plan_struct) if plan_struct is not None else None,
+              _stream(h))
+    return dh
+
+
 def _check_fp8_operand(t, name, n_grp, rows=None, device=None):
     """An Fp8Table the gather kernels can read: CUDA data and exponents on one device, and exponents as a dense
     [rows, n_grp] array (the kernels index them as row * n_grp + group).  A column block of a wider table (block()) is
