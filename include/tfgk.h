@@ -609,6 +609,38 @@ int tfgk_spgemm_fill_f32(const int64_t *a_rowptr, const int32_t *a_col, const fl
                          const int64_t *big_ptr, int64_t big_products, const int64_t *c_rowptr, int32_t *c_col,
                          float *c_val, void *workspace, size_t workspace_bytes, void *stream);
 
+/* ---- K12: the gradient of K10's C = A B with respect to A's and B's values ------------------------------------------
+ * A is [M, K], B [K, N], C [M, N] with ascending, unique columns in every row (K10's output), dC its upstream gradient in
+ * C's value order.  For every CSR entry p of X, one row of Y is walked and dC is looked up in C:
+ *   TFGK_SPGEMM_GRAD_LEFT   X = A, Y = B:    dA[p = (i, k)] = sum_{q in B.row(k)}   B.val[q]  * dC(i, B.col[q])
+ *   TFGK_SPGEMM_GRAD_RIGHT  X = B, Y = A^T:  dB[p = (k, j)] = sum_{q in A^T.row(k)} At.val[q] * dC(At.col[q], j)
+ * dC(r, c) is found by binary search over C's row r; a column the row does not hold contributes 0 (nothing is added).
+ * Summation order, part of the contract: every product Y.val[q] * dC is rounded once (no fused multiply-add); a Y row is
+ * cut into consecutive slices of TFGK_SPGEMM_GRAD_SLICE entries; a slice sums its products from +0 in Y's CSR order and
+ * the entry sums its slice sums from +0 in slice order.  The bits therefore depend only on the inputs (not on the grid
+ * or on which threads take the slices); no atomics; out[x_perm ? x_perm[p] : p] is written exactly once per entry
+ * (x_perm, X's CSR slot -> COO position map, lands the gradient in X's COO order).
+ *   _plan  slice_ptr[nnz_x + 1] = exclusive scan over X's entries of their slice counts, 0 for an entry whose Y row has
+ *          at most TFGK_SPGEMM_GRAD_SLICE entries (one thread takes it whole) and ceil(len / SLICE) otherwise (the slices
+ *          are spread over threads); *n_slices_host = their total.  Decided from row lengths alone.  A column id of X
+ *          outside [0, K) (left) / [0, N) (right), or of Y outside [0, N) / [0, M), returns TFGK_ERR_INDEX_OUT_OF_RANGE.
+ *          Synchronises once.
+ *   _f32   the gradient, given the plan and `partial`, a scratch of n_slices floats.  Asynchronous.
+ * X's rowptr must end at nnz_x.  Nothing per product is stored.  Algorithmic bytes of _f32 (products = sum over X's
+ * entries of their Y row lengths): X (8 per row, 16 per entry: col, slice_ptr, out, [+4 perm]) + Y's row offsets (16 per
+ * entry) + Y's column and value and the matching C column and dC (16 per product) + C's row offsets (16 per entry left,
+ * 16 per product right) + 8 per hub slice. */
+#define TFGK_SPGEMM_GRAD_SLICE 64
+enum tfgk_spgemm_grad_mode { TFGK_SPGEMM_GRAD_LEFT = 0, TFGK_SPGEMM_GRAD_RIGHT = 1 };
+int tfgk_spgemm_grad_workspace_bytes(int64_t nnz_x, size_t *out_bytes);
+int tfgk_spgemm_grad_plan(int mode, const int64_t *x_rowptr, const int32_t *x_col, int64_t nnz_x, const int64_t *y_rowptr,
+                          const int32_t *y_col, int32_t M, int32_t K, int32_t N, int64_t *slice_ptr,
+                          int64_t *n_slices_host, void *workspace, size_t workspace_bytes, void *stream);
+int tfgk_spgemm_grad_f32(int mode, const int64_t *x_rowptr, const int32_t *x_col, const int32_t *x_perm, int64_t nnz_x,
+                         const int64_t *y_rowptr, const int32_t *y_col, const float *y_val, int32_t M, int32_t K, int32_t N,
+                         const int64_t *c_rowptr, const int32_t *c_col, const float *dC, const int64_t *slice_ptr,
+                         int64_t n_slices, float *partial, float *out, void *stream);
+
 /* ---- K11: max aggregation with tie counts, and its backward over the transposed CSR --------------------------------
  * (max_pool_graph_sage and aggregate_neighbors(max_reducer) training, ASAP's query; graph_sage.py:228-287) */
 

@@ -25,6 +25,7 @@ BERNOULLI_NONE, BERNOULLI_DROPOUT, BERNOULLI_KEEP = 0, 1, 2
 SAMPLE_NO_PADDING, SAMPLE_PADDING, SAMPLE_HEAD = 0, 1, 2
 NEG_UPPER, NEG_START = 0, 1
 PAD_ROW_MAJOR, PAD_STEP_MAJOR = 0, 1
+SPGEMM_GRAD_LEFT, SPGEMM_GRAD_RIGHT = 0, 1
 DTYPE_F32, DTYPE_BF16, DTYPE_FP8_E4M3 = 0, 1, 2
 
 _i32, _i64, _f32, _int = ctypes.c_int32, ctypes.c_int64, ctypes.c_float, ctypes.c_int
@@ -131,7 +132,12 @@ SIGNATURES = {
     "tfgk_spgemm_rowptr": [_ptr, _i32, _ptr, ctypes.POINTER(_i64), _ptr, _size, _ptr],
     "tfgk_spgemm_fill_f32": [_ptr, _ptr, _ptr, _ptr, _ptr, _ptr, _i32, _i32, _ptr, _ptr, _i64, _ptr, _ptr, _ptr, _ptr, _size,
                              _ptr],
-    "tfgk_spmm_max_f32": [_ptr, _ptr, _ptr, _ptr, _i64, _i32, _i32, _ptr, _i64, _ptr, _i64, _ptr, _ptr],
+    "tfgk_spgemm_grad_workspace_bytes": [_i64, ctypes.POINTER(_size)],
+    "tfgk_spgemm_grad_plan": [_int, _ptr, _ptr, _i64, _ptr, _ptr, _i32, _i32, _i32, _ptr, ctypes.POINTER(_i64), _ptr, _size,
+                              _ptr],
+    "tfgk_spgemm_grad_f32": [_int, _ptr, _ptr, _ptr, _i64, _ptr, _ptr, _ptr, _i32, _i32, _i32, _ptr, _ptr, _ptr, _ptr, _i64,
+                             _ptr, _ptr, _ptr],
+    "tfgk_spmm_max_f32":[_ptr, _ptr, _ptr, _ptr, _i64, _i32, _i32, _ptr, _i64, _ptr, _i64, _ptr, _ptr],
     "tfgk_spmm_max_bwd_f32": [_ptr, _ptr, _ptr, _ptr, _i64, _i32, _i32, _i32, _ptr, _i64, _ptr, _i64, _ptr, _i64, _ptr,
                               _ptr, _i64, _ptr, _ptr],
 }

@@ -701,6 +701,44 @@ class AssignGram(torch.autograd.Function):
         return ops.graph_rmm(s, g, lay.node_graph, lay.num_clusters, trans=True, beta=1.0, out=out), None
 
 
+class SparseProduct(torch.autograd.Function):
+    """C = A B for two SparseMatrix operands, differentiable in both operands' values (COO order), as tf_sparse's
+    product is under tf.GradientTape.  Forward: K10 over the operands' CSRs with the values permuted into CSR order,
+    detached, so the bits are the same whatever requires grad; returns C's (values, rowptr, columns), ascending unique
+    columns per row.  Backward, with g = dL/dC in C's value order (K12, written in each operand's COO order through its
+    CSR perm):
+        dA[(i, k)] = sum_{q in B.row(k)} B.val[q] g(i, B.col[q])           (left mode, over A's CSR and B's CSR)
+        dB[(k, j)] = sum_{q in A^T.row(k)} A.val[q] g(A^T.col[q], j)       (right mode, over B's CSR and A's transposed CSR)
+    Only the gradients asked for are computed."""
+
+    @staticmethod
+    def forward(ctx, a_value, b_value, a, b):
+        a_coo = a_value.detach().contiguous()
+        b_val = ops.permute(b_value.detach().contiguous(), b.csr.perm)
+        a_val = ops.permute(a_coo, a.csr.perm)
+        c_rowptr, c_col, c_val = ops.spgemm(a.csr.rowptr, a.csr.col, a_val, b.csr.rowptr, b.csr.col, b_val, b.shape[1])
+        ctx.a, ctx.b = a, b
+        ctx.save_for_backward(a_coo, b_val, c_rowptr, c_col)
+        ctx.mark_non_differentiable(c_rowptr, c_col)
+        return c_val, c_rowptr, c_col
+
+    @staticmethod
+    def backward(ctx, grad_c, grad_rowptr, grad_col):
+        a, b = ctx.a, ctx.b
+        a_coo, b_val, c_rowptr, c_col = ctx.saved_tensors
+        g = grad_c.contiguous()
+        m, k, n = a.shape[0], a.shape[1], b.shape[1]
+        grad_a = grad_b = None
+        if ctx.needs_input_grad[0]:
+            grad_a = ops.spgemm_grad("left", a.csr.rowptr, a.csr.col, b.csr.rowptr, b.csr.col, b_val, c_rowptr, c_col, g,
+                                     m, k, n, perm=a.csr.perm)
+        if ctx.needs_input_grad[1]:
+            at = a._transposed_csr()
+            grad_b = ops.spgemm_grad("right", b.csr.rowptr, b.csr.col, at.rowptr, at.col, ops.permute(a_coo, at.perm),
+                                     c_rowptr, c_col, g, m, k, n, perm=b.csr.perm)
+        return grad_a, grad_b, None, None
+
+
 class RefusedPooledWeights(torch.autograd.Function):
     """The pooled edge weights of cluster_pool (the entries of S^T A S) as a function of A's and S's values.  The forward
     returns the weights K10 computed; their backward is not built, so it raises instead of returning no gradient."""

@@ -153,6 +153,169 @@ __global__ void __launch_bounds__(kRowThreads) spgemm_rows_kernel(
     if (!FILL && threadIdx.x == 0) c_count[i] = carry;
 }
 
+// ---- K12: the gradient of C = A B with respect to A's and B's values ----
+//
+// Both modes walk, for every CSR entry p of X, one row of Y and look the values of dC up in C:
+//   left  (X = A, Y = B):   dA[p = (i, k)] = sum_{q in B.row(k)}  B.val[q]  * dC(i, B.col[q])
+//   right (X = B, Y = A^T): dB[p = (k, j)] = sum_{q in At.row(k)} At.val[q] * dC(At.col[q], j)
+// A Y row is cut into slices of kSlice entries; a slice sums its products (each rounded once) from +0 in Y's order, and
+// the entry sums its slices from +0 in slice order.  Entries with one slice are computed by one thread in one pass; the
+// slices of longer rows ("hub" entries, listed by the plan from row lengths alone) are spread over threads, write their
+// partial sums to the caller's scratch, and the entry pass adds them in order.  Same bits either way; no atomics.
+
+constexpr int kSlice = TFGK_SPGEMM_GRAD_SLICE;
+constexpr int kLookups = 4;                              // binary searches of C in flight per thread
+
+// largest r in [0, n) with ptr[r] <= v, given ptr[0] <= v < ptr[n] (the row, or the entry, that holds v)
+__device__ __forceinline__ int64_t last_le(const int64_t *__restrict__ ptr, int64_t n, int64_t v) {
+    int64_t lo = 0, len = n;
+    while (len > 1) {
+        const int64_t half = len >> 1;
+        if (ptr[lo + half] <= v) {
+            lo += half;
+            len -= half;
+        } else {
+            len = half;
+        }
+    }
+    return lo;
+}
+
+// sum of the products of Y's entries [q0, q1) with dC.  LEFT: C's row is [c0, c1) and the column is y_col[q]; right: C's
+// row is y_col[q] and the column is j.  A column C's row does not hold contributes 0.
+template <bool LEFT>
+__device__ float grad_slice_sum(const int32_t *__restrict__ y_col, const float *__restrict__ y_val, int64_t q0, int64_t q1,
+                                const int64_t *__restrict__ c_rowptr, const int32_t *__restrict__ c_col,
+                                const float *__restrict__ dC, int64_t c0, int64_t c1, int32_t j) {
+    float acc = 0.0f;
+    for (int64_t q = q0; q < q1; q += kLookups) {
+        int64_t lo[kLookups], len[kLookups];
+        int32_t want[kLookups];
+#pragma unroll
+        for (int u = 0; u < kLookups; ++u) {
+            lo[u] = 0;
+            len[u] = 0;
+            want[u] = 0;
+            if (q + u < q1) {
+                const int32_t yc = y_col[q + u];
+                if (LEFT) {
+                    lo[u] = c0;
+                    len[u] = c1 - c0;
+                    want[u] = yc;
+                } else {
+                    lo[u] = c_rowptr[yc];
+                    len[u] = c_rowptr[yc + 1] - lo[u];
+                    want[u] = j;
+                }
+            }
+        }
+        // the searches advance in lock step so that their loads overlap: last position with c_col <= want
+        bool more = true;
+        while (more) {
+            more = false;
+#pragma unroll
+            for (int u = 0; u < kLookups; ++u) {
+                if (len[u] > 1) {
+                    const int64_t half = len[u] >> 1;
+                    if (c_col[lo[u] + half] <= want[u]) lo[u] += half;
+                    len[u] -= half;
+                    more |= len[u] > 1;
+                }
+            }
+        }
+#pragma unroll
+        for (int u = 0; u < kLookups; ++u)
+            if (len[u] == 1 && c_col[lo[u]] == want[u]) acc = __fadd_rn(acc, __fmul_rn(y_val[q + u], dC[lo[u]]));
+    }
+    return acc;
+}
+
+// slices per X entry (0 when one thread takes the whole Y row) and the validation of X's column ids
+template <bool LEFT>
+__global__ void grad_plan_kernel(const int64_t *__restrict__ x_rowptr, const int32_t *__restrict__ x_col, int32_t n_x_rows,
+                                 int64_t nnz_x, int32_t x_ncols, const int64_t *__restrict__ y_rowptr,
+                                 int64_t *__restrict__ cnt, int32_t *__restrict__ flag) {
+    for (int64_t p = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; p < nnz_x; p += (int64_t)gridDim.x * blockDim.x) {
+        const int32_t k = x_col[p];
+        if (k < 0 || k >= x_ncols) {
+            flag[0] = 1;
+            cnt[p] = 0;
+            continue;
+        }
+        const int64_t yr = LEFT ? (int64_t)k : last_le(x_rowptr, n_x_rows, p);
+        const int64_t len = y_rowptr[yr + 1] - y_rowptr[yr];
+        cnt[p] = len > kSlice ? (len + kSlice - 1) / kSlice : 0;
+    }
+}
+
+template <bool LEFT>
+__device__ __forceinline__ float grad_range(const int64_t *__restrict__ x_rowptr, const int32_t *__restrict__ x_col,
+                                            int32_t n_x_rows, int64_t p, int64_t t, const int64_t *__restrict__ y_rowptr,
+                                            const int32_t *__restrict__ y_col, const float *__restrict__ y_val,
+                                            const int64_t *__restrict__ c_rowptr, const int32_t *__restrict__ c_col,
+                                            const float *__restrict__ dC, bool whole) {
+    const int64_t r = last_le(x_rowptr, n_x_rows, p);
+    const int32_t k = x_col[p];
+    const int64_t yr = LEFT ? (int64_t)k : r;
+    const int64_t y_end = y_rowptr[yr + 1];
+    const int64_t q0 = y_rowptr[yr] + (whole ? 0 : t * kSlice);
+    const int64_t q1 = whole ? y_end : min(q0 + kSlice, y_end);
+    if (LEFT) return grad_slice_sum<true>(y_col, y_val, q0, q1, c_rowptr, c_col, dC, c_rowptr[r], c_rowptr[r + 1], 0);
+    return grad_slice_sum<false>(y_col, y_val, q0, q1, c_rowptr, c_col, dC, 0, 0, k);
+}
+
+// one thread per slice of the hub entries: partial[s]
+template <bool LEFT>
+__global__ void __launch_bounds__(256) grad_slices_kernel(
+    const int64_t *__restrict__ x_rowptr, const int32_t *__restrict__ x_col, int32_t n_x_rows, int64_t nnz_x,
+    const int64_t *__restrict__ y_rowptr, const int32_t *__restrict__ y_col, const float *__restrict__ y_val,
+    const int64_t *__restrict__ c_rowptr, const int32_t *__restrict__ c_col, const float *__restrict__ dC,
+    const int64_t *__restrict__ slice_ptr, int64_t n_slices, float *__restrict__ partial) {
+    for (int64_t s = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; s < n_slices; s += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t p = last_le(slice_ptr, nnz_x, s);
+        partial[s] = grad_range<LEFT>(x_rowptr, x_col, n_x_rows, p, s - slice_ptr[p], y_rowptr, y_col, y_val, c_rowptr,
+                                      c_col, dC, false);
+    }
+}
+
+// one thread per X entry: the whole Y row, or the sum of the entry's slices in order
+template <bool LEFT>
+__global__ void __launch_bounds__(256) grad_entries_kernel(
+    const int64_t *__restrict__ x_rowptr, const int32_t *__restrict__ x_col, const int32_t *__restrict__ x_perm,
+    int32_t n_x_rows, int64_t nnz_x, const int64_t *__restrict__ y_rowptr, const int32_t *__restrict__ y_col,
+    const float *__restrict__ y_val, const int64_t *__restrict__ c_rowptr, const int32_t *__restrict__ c_col,
+    const float *__restrict__ dC, const int64_t *__restrict__ slice_ptr, const float *__restrict__ partial,
+    float *__restrict__ out) {
+    for (int64_t p = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; p < nnz_x; p += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t s0 = slice_ptr[p], s1 = slice_ptr[p + 1];
+        float acc = 0.0f;
+        if (s1 > s0) {
+            for (int64_t s = s0; s < s1; ++s) acc = __fadd_rn(acc, partial[s]);
+        } else {
+            acc = grad_range<LEFT>(x_rowptr, x_col, n_x_rows, p, 0, y_rowptr, y_col, y_val, c_rowptr, c_col, dC, true);
+        }
+        out[x_perm ? (int64_t)x_perm[p] : p] = acc;
+    }
+}
+
+struct GradWorkspace {
+    size_t off_flag, off_cnt, off_sums, total;
+    explicit GradWorkspace(int64_t nnz_x) {
+        off_flag = 0;
+        off_cnt = align_up(8);
+        off_sums = off_cnt + align_up((size_t)nnz_x * 8 + 8);
+        total = off_sums + scan_scratch_bytes(nnz_x + 1);
+    }
+};
+
+// X's rows, X's column bound and Y's column bound of a mode (A is [M, K], B [K, N])
+struct GradShape {
+    int32_t x_rows, x_ncols, y_ncols;
+    GradShape(int mode, int32_t M, int32_t K, int32_t N)
+        : x_rows(mode == TFGK_SPGEMM_GRAD_LEFT ? M : K), x_ncols(mode == TFGK_SPGEMM_GRAD_LEFT ? K : N),
+          y_ncols(mode == TFGK_SPGEMM_GRAD_LEFT ? N : M) {}
+};
+
 struct PlanWorkspace {
     size_t off_flag, off_prod, off_big, off_sums, total;
     explicit PlanWorkspace(int32_t M) {
@@ -286,6 +449,91 @@ int tfgk_spgemm_fill_f32(const int64_t *a_rowptr, const int32_t *a_col, const fl
     spgemm_rows_kernel<true><<<(unsigned)(row1 - row0), kRowThreads, 0, as_stream(stream)>>>(
         a_rowptr, a_col, a_val, b_rowptr, b_col, b_val, row0, prod_ptr, big_ptr, nullptr, c_rowptr, c_col, c_val, keys,
         vals);
+    TFGK_LAUNCH_CHECK();
+    return TFGK_OK;
+}
+
+int tfgk_spgemm_grad_workspace_bytes(int64_t nnz_x, size_t *out_bytes) {
+    TFGK_CHECK_ARG(nnz_x >= 0 && out_bytes, "spgemm_grad_workspace_bytes: bad nnz_x or null output");
+    *out_bytes = GradWorkspace(nnz_x).total;
+    return TFGK_OK;
+}
+
+int tfgk_spgemm_grad_plan(int mode, const int64_t *x_rowptr, const int32_t *x_col, int64_t nnz_x, const int64_t *y_rowptr,
+                          const int32_t *y_col, int32_t M, int32_t K, int32_t N, int64_t *slice_ptr,
+                          int64_t *n_slices_host, void *workspace, size_t workspace_bytes, void *stream) {
+    TFGK_CHECK_ARG(mode == TFGK_SPGEMM_GRAD_LEFT || mode == TFGK_SPGEMM_GRAD_RIGHT, "spgemm_grad_plan: bad mode %d", mode);
+    TFGK_CHECK_ARG(M >= 0 && K >= 0 && N >= 0 && nnz_x >= 0, "spgemm_grad_plan: negative M, K, N or nnz_x");
+    TFGK_CHECK_ARG(x_rowptr && y_rowptr && slice_ptr && n_slices_host && (nnz_x == 0 || x_col),
+                   "spgemm_grad_plan: null pointer");
+    const GradWorkspace L(nnz_x);
+    if (workspace == nullptr || workspace_bytes < L.total)
+        return set_error(TFGK_ERR_WORKSPACE, "spgemm_grad_plan: workspace too small (%zu < %zu bytes)", workspace_bytes,
+                         L.total);
+    const GradShape S(mode, M, K, N);
+    cudaStream_t st = as_stream(stream);
+    char *ws = static_cast<char *>(workspace);
+    int32_t *flag = reinterpret_cast<int32_t *>(ws + L.off_flag);
+    int64_t *cnt = reinterpret_cast<int64_t *>(ws + L.off_cnt);
+    int64_t *sums = reinterpret_cast<int64_t *>(ws + L.off_sums);
+    TFGK_CUDA(cudaMemsetAsync(flag, 0, 8, st));
+    if (nnz_x > 0) {
+        if (mode == TFGK_SPGEMM_GRAD_LEFT)
+            grad_plan_kernel<true><<<grid_for(nnz_x), 256, 0, st>>>(x_rowptr, x_col, S.x_rows, nnz_x, S.x_ncols, y_rowptr,
+                                                                     cnt, flag);
+        else
+            grad_plan_kernel<false><<<grid_for(nnz_x), 256, 0, st>>>(x_rowptr, x_col, S.x_rows, nnz_x, S.x_ncols, y_rowptr,
+                                                                      cnt, flag);
+        TFGK_LAUNCH_CHECK();
+    }
+    if (K > 0) {
+        // Y has K rows in both modes; nnz(Y) is only known on the device
+        spgemm_check_cols_kernel<<<(unsigned)sm_count() * 4, 256, 0, st>>>(y_rowptr, K, y_col, S.y_ncols, flag);
+        TFGK_LAUNCH_CHECK();
+    }
+    const int rc = exclusive_scan<int64_t, int64_t>(cnt, nnz_x, nnz_x + 1, slice_ptr, sums, st);
+    if (rc != TFGK_OK) return rc;
+    int32_t bad[2] = {0, 0};
+    TFGK_CUDA(cudaMemcpyAsync(bad, flag, 8, cudaMemcpyDeviceToHost, st));
+    TFGK_CUDA(cudaMemcpyAsync(n_slices_host, slice_ptr + nnz_x, 8, cudaMemcpyDeviceToHost, st));
+    TFGK_CUDA(cudaStreamSynchronize(st));
+    if (bad[0])
+        return set_error(TFGK_ERR_INDEX_OUT_OF_RANGE, "spgemm_grad_plan: a column id of X is outside [0, %d) or of Y outside "
+                         "[0, %d)", S.x_ncols, S.y_ncols);
+    return TFGK_OK;
+}
+
+int tfgk_spgemm_grad_f32(int mode, const int64_t *x_rowptr, const int32_t *x_col, const int32_t *x_perm, int64_t nnz_x,
+                         const int64_t *y_rowptr, const int32_t *y_col, const float *y_val, int32_t M, int32_t K, int32_t N,
+                         const int64_t *c_rowptr, const int32_t *c_col, const float *dC, const int64_t *slice_ptr,
+                         int64_t n_slices, float *partial, float *out, void *stream) {
+    TFGK_CHECK_ARG(mode == TFGK_SPGEMM_GRAD_LEFT || mode == TFGK_SPGEMM_GRAD_RIGHT, "spgemm_grad: bad mode %d", mode);
+    TFGK_CHECK_ARG(M >= 0 && K >= 0 && N >= 0 && nnz_x >= 0 && n_slices >= 0, "spgemm_grad: negative size");
+    if (nnz_x == 0) return TFGK_OK;
+    // y_col, y_val, c_col and dC may be null when Y or C have no entries: no slot outside the row ranges is read
+    TFGK_CHECK_ARG(x_rowptr && x_col && y_rowptr && c_rowptr && slice_ptr && out && (n_slices == 0 || partial),
+                   "spgemm_grad: null pointer");
+    const GradShape S(mode, M, K, N);
+    cudaStream_t st = as_stream(stream);
+    const bool left = mode == TFGK_SPGEMM_GRAD_LEFT;
+    if (n_slices > 0) {
+        if (left)
+            grad_slices_kernel<true><<<grid_for(n_slices), 256, 0, st>>>(x_rowptr, x_col, S.x_rows, nnz_x, y_rowptr, y_col,
+                                                                          y_val, c_rowptr, c_col, dC, slice_ptr, n_slices,
+                                                                          partial);
+        else
+            grad_slices_kernel<false><<<grid_for(n_slices), 256, 0, st>>>(x_rowptr, x_col, S.x_rows, nnz_x, y_rowptr, y_col,
+                                                                           y_val, c_rowptr, c_col, dC, slice_ptr, n_slices,
+                                                                           partial);
+        TFGK_LAUNCH_CHECK();
+    }
+    if (left)
+        grad_entries_kernel<true><<<grid_for(nnz_x), 256, 0, st>>>(x_rowptr, x_col, x_perm, S.x_rows, nnz_x, y_rowptr, y_col,
+                                                                    y_val, c_rowptr, c_col, dC, slice_ptr, partial, out);
+    else
+        grad_entries_kernel<false><<<grid_for(nnz_x), 256, 0, st>>>(x_rowptr, x_col, x_perm, S.x_rows, nnz_x, y_rowptr,
+                                                                     y_col, y_val, c_rowptr, c_col, dC, slice_ptr, partial,
+                                                                     out);
     TFGK_LAUNCH_CHECK();
     return TFGK_OK;
 }

@@ -13,7 +13,7 @@ from . import _ffi
 from ._ffi import (REDUCE_SUM, REDUCE_MEAN, REDUCE_MAX, ACT_NONE, ACT_RELU, POW_INV_SQRT, POW_INV,  # noqa: F401
                    HEADS_SPLIT, HEADS_BROADCAST, HEADS_REDUCE, FLAG_ALL, FLAG_UPPER, FLAG_MAPPED,
                    BERNOULLI_NONE, BERNOULLI_DROPOUT, BERNOULLI_KEEP, SAMPLE_NO_PADDING, SAMPLE_PADDING, SAMPLE_HEAD,
-                   NEG_UPPER, NEG_START, PAD_ROW_MAJOR, PAD_STEP_MAJOR)
+                   NEG_UPPER, NEG_START, PAD_ROW_MAJOR, PAD_STEP_MAJOR, SPGEMM_GRAD_LEFT, SPGEMM_GRAD_RIGHT)
 
 _REDUCE_CODES = {"sum": REDUCE_SUM, "mean": REDUCE_MEAN, "max": REDUCE_MAX}
 
@@ -1109,6 +1109,50 @@ def spgemm(a_rowptr, a_col, a_val, b_rowptr, b_col, b_val, n_cols, budget=SPGEMM
             _ffi.call("tfgk_spgemm_fill_f32", _p(a_rowptr), _p(a_col), _p(a_val), _p(b_rowptr), _p(b_col), _p(b_val), r0,
                       r1, _p(prod_ptr), _p(big_ptr), nb, _p(c_rowptr), _p(c_col), _p(c_val), _p(rws), rows_ws.value, st)
     return c_rowptr, c_col, c_val
+
+
+_SPGEMM_GRAD_MODES = {"left": SPGEMM_GRAD_LEFT, "right": SPGEMM_GRAD_RIGHT}
+
+
+def spgemm_grad(mode, x_rowptr, x_col, y_rowptr, y_col, y_val, c_rowptr, c_col, grad_c, m, k, n, perm=None):
+    """The gradient of K10's C = A B (A [m, k], B [k, n]) with respect to the values of one operand (K12,
+    tfgk_spgemm_grad_*), given C's (rowptr, col) and grad_c = dL/dC in C's value order:
+      mode "left":  X = A's CSR, Y = B's CSR (with values):    dA[(i, kk)] = sum_q B.val[q] * dC(i, B.col[q]) over B.row(kk)
+      mode "right": X = B's CSR, Y = A^T's CSR (with values):  dB[(kk, j)] = sum_q At.val[q] * dC(At.col[q], j) over At.row(kk)
+    Returns one float32 per entry of X, in X's CSR order, or at perm[p] (X's CSR slot -> COO position) when perm is given.
+    A C entry that is missing contributes 0.  The bits depend only on the inputs (summation order in include/tfgk.h)."""
+    if mode not in _SPGEMM_GRAD_MODES:
+        raise ValueError("spgemm_grad: mode must be 'left' or 'right' (got {!r})".format(mode))
+    for t, name, dt in ((x_rowptr, "x_rowptr", torch.int64), (x_col, "x_col", torch.int32), (y_rowptr, "y_rowptr", torch.int64),
+                        (y_col, "y_col", torch.int32), (y_val, "y_val", torch.float32), (c_rowptr, "c_rowptr", torch.int64),
+                        (c_col, "c_col", torch.int32), (grad_c, "grad_c", torch.float32)):
+        _check(t, dt, name)
+    if y_col.numel() != y_val.numel() or c_col.numel() != grad_c.numel():
+        raise ValueError("spgemm_grad: column and value arrays differ in length")
+    m, k, n = int(m), int(k), int(n)
+    x_rows = m if mode == "left" else k
+    for t, rows, name in ((x_rowptr, x_rows, "x_rowptr"), (y_rowptr, k, "y_rowptr"), (c_rowptr, m, "c_rowptr")):
+        if t.numel() != rows + 1:
+            raise ValueError("spgemm_grad: {} has {} entries, {} expected".format(name, t.numel(), rows + 1))
+    nnz_x = x_col.numel()
+    if perm is not None:
+        _check(perm, torch.int32, "perm")
+        if perm.numel() != nnz_x:
+            raise ValueError("spgemm_grad: perm has {} entries for {} entries of X".format(perm.numel(), nnz_x))
+    code = _SPGEMM_GRAD_MODES[mode]
+    dev, st = x_rowptr.device, _stream(x_rowptr)
+    need = ctypes.c_size_t()
+    _ffi.call("tfgk_spgemm_grad_workspace_bytes", nnz_x, ctypes.byref(need))
+    ws = torch.empty((need.value,), dtype=torch.uint8, device=dev)
+    slice_ptr = torch.empty((nnz_x + 1,), dtype=torch.int64, device=dev)
+    n_slices = ctypes.c_int64()
+    _ffi.call("tfgk_spgemm_grad_plan", code, _p(x_rowptr), _p(x_col), nnz_x, _p(y_rowptr), _p(y_col), m, k, n,
+              _p(slice_ptr), ctypes.byref(n_slices), _p(ws), need.value, st)
+    partial = torch.empty((max(n_slices.value, 1),), dtype=torch.float32, device=dev)
+    out = torch.empty((nnz_x,), dtype=torch.float32, device=dev)
+    _ffi.call("tfgk_spgemm_grad_f32", code, _p(x_rowptr), _p(x_col), _p(perm), nnz_x, _p(y_rowptr), _p(y_col), _p(y_val),
+              m, k, n, _p(c_rowptr), _p(c_col), _p(grad_c), _p(slice_ptr), n_slices.value, _p(partial), _p(out), st)
+    return out
 
 
 # ---- K4 ----------------------------------------------------------------------------------------------------------

@@ -115,7 +115,8 @@ class SparseMatrix(object):
         return out
 
     def matmul(self, h, num_or_size_splits=None, **epilogue):
-        """A @ h (gcn.py:280).  `num_or_size_splits` (tf.split semantics: a count of equal column chunks or a list of
+        """A @ h (gcn.py:280).  With a SparseMatrix h, the sparse x sparse product A @ B (see `_sparse_product`), which
+        takes neither `num_or_size_splits` nor epilogue keywords.  `num_or_size_splits` (tf.split semantics: a count of equal column chunks or a list of
         chunk widths, utils/tf_sparse_utils.py:71-90) runs one launch per column chunk into slices of one output, like the
         reference's split -> matmul -> concat; the fused kernel has no [E, D] temporary to bound, so the results are the
         same bits with or without it.  A bfloat16 h stays bfloat16 and is gathered as such (tfgk_spmm_bf16) when no operand
@@ -123,6 +124,11 @@ class SparseMatrix(object):
         half the row bytes.  With a bfloat16 h, `out_bf16=` (see ops.spmm) also stores the result rounded to bf16, or only
         that when no `out` is given."""
         from . import autograd
+        if isinstance(h, SparseMatrix):
+            if num_or_size_splits is not None or epilogue:
+                raise TypeError("SparseMatrix.matmul: a sparse right operand takes no num_or_size_splits or epilogue "
+                                "keywords")
+            return self._sparse_product(h)
         # the differentiable route below works in fp32 (its backward products take fp32 operands): a bf16 h is widened
         # for it, as it always was
         keep_bf16 = torch.is_tensor(h) and h.dtype == torch.bfloat16 and \
@@ -166,6 +172,35 @@ class SparseMatrix(object):
             c0 = c1
         return out if out is not None else out_bf16
 
+    def _sparse_product(self, other):
+        """C = A @ B for two SparseMatrix operands (tf_sparse's sparse x sparse product, as in gcn.py:83-94's
+        diags(d) @ A @ diags(d) and cluster_pool.py:32-36's S^T A S): K10 on the device, differentiable in both operands'
+        values (autograd.SparseProduct, K12).
+        The result has shape [A.shape[0], B.shape[1]] and an int32 index in row-major order: ascending, unique columns
+        in every row, duplicates of the operands merged (their products summed in Gustavson order: A's row left to right,
+        then B's row left to right), exact zeros kept.  tf_sparse's own order for this product cannot be checked (tf_sparse
+        is not available to compare against), so row-major is the order here.  The CSR is prebuilt with the identity
+        permutation and its work plan, so a following C @ h does no sort."""
+        from . import autograd
+        if self._shape[1] != other._shape[0]:
+            raise ValueError("SparseMatrix @ SparseMatrix: inner dimensions differ ({} x {} @ {} x {})".format(
+                self._shape[0], self._shape[1], other._shape[0], other._shape[1]))
+        if self.index.device != other.index.device:
+            raise ValueError("SparseMatrix @ SparseMatrix: operands on {} and {}".format(self.index.device,
+                                                                                        other.index.device))
+        value, rowptr, col = autograd.SparseProduct.apply(self.value, other.value, self, other)
+        nnz = col.shape[0]
+        if nnz >= 2 ** 31:
+            raise ValueError("SparseMatrix @ SparseMatrix: the product has {} entries, more than an int32 index "
+                             "addresses".format(nnz))
+        m, n = self._shape[0], other._shape[1]
+        dev = rowptr.device
+        row = torch.repeat_interleave(torch.arange(m, dtype=torch.int32, device=dev), rowptr[1:] - rowptr[:-1],
+                                      output_size=nnz)
+        csr = ops.CSR(rowptr, col, torch.arange(nnz, dtype=torch.int32, device=dev), m, n)
+        csr.plan = ops.build_plan(csr)
+        return SparseMatrix(torch.stack([row, col]), value, [m, n], _csr=csr, _value_csr=value.detach())
+
     def __matmul__(self, h):
         return self.matmul(h)
 
@@ -182,6 +217,17 @@ class SparseMatrix(object):
 
     def __repr__(self):
         return "SparseMatrix(shape={}, nnz={})".format(self._shape, self.nnz)
+
+
+def diags(values):
+    """tf_sparse's diags: the n x n diagonal SparseMatrix whose values are `values` (a 1-D tensor; gradients flow through
+    them), so the reference's normalisation diags(d) @ A @ diags(d) (gcn.py:83-94) can be written as it is there."""
+    values = ops.as_device(values, torch.float32)
+    if values.dim() != 1:
+        raise ValueError("diags: values must be 1-D (got shape {})".format(tuple(values.shape)))
+    n = values.shape[0]
+    ids = torch.arange(n, dtype=torch.int32, device=values.device)
+    return SparseMatrix(torch.stack([ids, ids]), values, [n, n])
 
 
 def as_sparse_features(x):
