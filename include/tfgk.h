@@ -200,7 +200,6 @@ int tfgk_spmm_bf16_dual(const int64_t *rowptr, const int32_t *col, const float *
  * ldh >= D rounded up to 16, up to 256 columns, take the TMA ring (read with their pad columns, which are computed and
  * never stored; the plan's scratch holds D rounded up to 16 floats per slot); every other shape takes a scalar path
  * without the plan (a hub row of a table wider than 256 columns is then summed in order, unlike in fp32).
- * TFGK_SPMM_FP8_STAGES sets the ring depth (6, 8 or 12; default 12).
  * Algorithmic bytes: E*(D + 1 [+1 for D > 128] + 4 [+4 weighted]) + N*(4*D + 8). */
 int tfgk_spmm_fp8(const int64_t *rowptr, const int32_t *col, const float *w,
                   const uint8_t *h, int64_t ldh, const int8_t *h_exp, int32_t n_dst, int32_t D, int reduce,
@@ -245,8 +244,8 @@ int tfgk_gat_fused_bf16(const int64_t *rowptr, const int32_t *col,
  * The TMA ring copies 2A bytes (rounded up to 16) per neighbour and reads its two exponents; each element is widened
  * and scaled by 2^k, then the fp32 ring's arithmetic runs with its lane mapping, so the output is bit-identical to
  * tfgk_gat_fused_f32 over Q, K^, V^ wherever that takes its TMA ring.  Every other shape returns TFGK_ERR_UNSUPPORTED (no
- * attention coefficients are returned).  The plan's hub scratch takes A + 64 floats per slot.  TFGK_GAT_FP8_STAGES sets
- * the ring depth (3, 4, 6 or 8; default 6).  Algorithmic bytes: E*(2A + 2 + 4) + N*(8A + 8). */
+ * attention coefficients are returned).  The plan's hub scratch takes A + 64 floats per slot.
+ * Algorithmic bytes: E*(2A + 2 + 4) + N*(8A + 8). */
 int tfgk_gat_fused_fp8(const int64_t *rowptr, const int32_t *col, const float *Q, int64_t ldq,
                        const uint8_t *KV, int64_t ldkv, const int8_t *kv_exp, int32_t N, int32_t H, int32_t dqk,
                        float scale, const float *bias, int act, float *out, int64_t ldo,

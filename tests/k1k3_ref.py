@@ -22,9 +22,6 @@ from oracle import c_oracle
 U = 2.0 ** -24                               # unit roundoff of fp32
 FLT_MAX = float(np.finfo(np.float32).max)
 
-# TFGK_SPMM_IMPL -> spmm_impl_choice() of spmm.cu (None: unset, the default by row shape)
-IMPL_CHOICE = {"ldg": 0, "bulk": 1, "stream": 2, "async": 3, "tma": 4, None: 5}
-
 # ops.build_plan's production parameters and its short-task rule (average degree >= DENSE_ROW_DEGREE)
 HUB_THRESHOLD, HUB_CHUNK, ROWS_PER_TASK = 2048, 2048, 32
 DENSE_ROW_DEGREE, TASK_EDGE_TARGET = 128, 512
@@ -148,11 +145,10 @@ def plan_degree_cases():
 
 # ---- K1 -------------------------------------------------------------------------------------------------------------
 
-def k1_takes_plan(D, aligned, impl):
+def k1_takes_plan(D, aligned):
     """spmm.cu tfgk_spmm_f32: the plan is used when the whole width runs in one launch of a ring kernel, i.e. float4 rows
-    (`aligned`: D % 4 == 0, ldh / ldo / ld_addend multiples of 4, 16-byte aligned pointers), 32 <= D <= 512, and
-    TFGK_SPMM_IMPL is unset, "async" or "tma" (ldg / stream / bulk never take it)."""
-    return aligned and 32 <= D <= 512 and IMPL_CHOICE[impl] >= 3
+    (`aligned`: D % 4 == 0, ldh / ldo / ld_addend multiples of 4, 16-byte aligned pointers) and 32 <= D <= 512."""
+    return aligned and 32 <= D <= 512
 
 
 def csr_rows(rowptr):

@@ -129,22 +129,19 @@ def test_gat_hub_rows_sliced_softmax_merge():
     assert_close(host(got_att), want, rtol=2e-5, atol_scale=2e-6, what="gat with hub rows (attention path)")
 
 
-@pytest.mark.parametrize("stages", ["2", "3", "4"])
-def test_gat_tma_gather4_variant_is_bit_identical(stages, monkeypatch):
+@pytest.mark.parametrize("heads", [1, 4, 8])
+def test_gat_tma_gather4_variant_is_bit_identical(heads):
     """K3 with the K|V rows of four neighbours fetched by four TMA bulk copies per round: same bits as the cp.async ring,
-    ragged rows, a hub row cut into slices, with and without the training statistics."""
+    which separate K and V buffers take, ragged rows and a hub row cut into slices."""
     rs = np.random.RandomState(5)
-    n, heads, a = 3000, 8, 128
+    n, a = 3000, 128
     ei = random_graph(n, 40000, seed=6, isolated=5, hub=(17, 9000))
     from tf_geometric_b200 import _structure
     csr, _ = _structure.csr_for_edge_index(dev(ei, torch.int32), n, add_self_loop=True)
     q = dev(rs.randn(n, a).astype(np.float32))
     kv = dev(rs.randn(n, 2 * a).astype(np.float32))
     bias = dev(rs.randn(a).astype(np.float32))
-    monkeypatch.setenv("TFGK_GAT_IMPL", "async")
-    want = ops.gat_fused(csr, q, kv[:, :a], kv[:, a:], heads, bias=bias, act=ops.ACT_RELU)
-    monkeypatch.setenv("TFGK_GAT_IMPL", "tma:" + stages)
+    sep_k, sep_v = kv[:, :a].contiguous(), kv[:, a:].contiguous()          # separate buffers: the cp.async ring
+    want = ops.gat_fused(csr, q, sep_k, sep_v, heads, bias=bias, act=ops.ACT_RELU)
     got = ops.gat_fused(csr, q, kv[:, :a], kv[:, a:], heads, bias=bias, act=ops.ACT_RELU)
     assert torch.equal(got, want)
-    sep_k, sep_v = kv[:, :a].contiguous(), kv[:, a:].contiguous()          # separate buffers: falls back to the cp.async ring
-    assert torch.equal(ops.gat_fused(csr, q, sep_k, sep_v, heads, bias=bias, act=ops.ACT_RELU), want)

@@ -263,10 +263,9 @@ def _stats_forward(csr, Q, K, V, H, bias, act):
 
 @pytest.mark.parametrize("graph", ["main", "hub"])
 @pytest.mark.parametrize("H,dqk", [(8, 16), (8, 8), (4, 32), (1, 128), (1, 4)])
-def test_rings_give_identical_out_and_stats(graph, H, dqk, monkeypatch):
-    """K|V in one [N, 2A] buffer takes the TMA ring (TFGK_GAT_IMPL unset = tma:2, tma:3, tma:4); separate K and V buffers,
-    which is what the training layer hands over, and TFGK_GAT_IMPL=async take the cp.async ring.  Same edge order, same
-    online softmax: the same bits."""
+def test_rings_give_identical_out_and_stats(graph, H, dqk):
+    """K|V in one [N, 2A] buffer takes the TMA ring; separate K and V buffers, which is what the training layer hands over,
+    take the cp.async ring.  Same edge order, same online softmax: the same bits."""
     row, col, n, _ = _main() if graph == "main" else _hub_graph()
     A = H * dqk
     rs = np.random.RandomState(H + dqk)
@@ -275,18 +274,28 @@ def test_rings_give_identical_out_and_stats(graph, H, dqk, monkeypatch):
     kv = torch.from_numpy(rs.randn(n, 2 * A).astype(np.float32)).cuda()
     K, V = kv[:, :A], kv[:, A:]
     bias = torch.from_numpy(rs.randn(A).astype(np.float32)).cuda()
-    monkeypatch.delenv("TFGK_GAT_IMPL", raising=False)
     want = _stats_forward(csr, Q, K.contiguous(), V.contiguous(), H, bias, ops.ACT_RELU)      # cp.async ring
-    runs = {"separate K and V": want, "tma:2": _stats_forward(csr, Q, K, V, H, bias, ops.ACT_RELU)}
-    for impl in ("tma:3", "tma:4", "async"):
-        monkeypatch.setenv("TFGK_GAT_IMPL", impl)
-        runs[impl] = _stats_forward(csr, Q, K, V, H, bias, ops.ACT_RELU)
-    for name, (out, stats) in runs.items():
-        assert torch.equal(out, want[0]), "out differs: " + name
-        assert torch.equal(stats, want[1]), "stats differ: " + name
+    out, stats = _stats_forward(csr, Q, K, V, H, bias, ops.ACT_RELU)                           # TMA ring
+    assert torch.equal(out, want[0]), "out differs"
+    assert torch.equal(stats, want[1]), "stats differ"
 
 
-def test_rings_are_the_kernels_named():
+def _kernel_names(fn):
+    """The tfgk kernels fn launches, as recorded by torch.profiler.  A session opened after another one in the same process
+    can come back without any kernel record (only the runtime calls); such a session says nothing about the kernels, so
+    up to three sessions are opened and the first that recorded a kernel is used."""
+    for _ in range(3):
+        torch.cuda.synchronize()
+        with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
+            fn()
+            torch.cuda.synchronize()
+        names = [e.name for e in prof.events() if "tfgk::" in e.name]
+        if names:
+            return " ".join(names)
+    raise AssertionError("three profiler sessions recorded no tfgk kernel")
+
+
+def test_joint_and_separate_buffers_reach_the_named_rings():
     """The ring test above is only worth something if the joint buffer really reaches the TMA kernel and the separate
     buffers the cp.async kernel."""
     row, col, n, _ = _main()
@@ -297,11 +306,7 @@ def test_rings_are_the_kernels_named():
     names = {}
     for label, K, V in (("joint", kv[:, :A], kv[:, A:]), ("separate", kv[:, :A].contiguous(), kv[:, A:].contiguous())):
         ops.gat_fused_stats(csr, Q, K, V, 8)
-        torch.cuda.synchronize()
-        with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
-            ops.gat_fused_stats(csr, Q, K, V, 8)
-            torch.cuda.synchronize()
-        names[label] = " ".join(e.name for e in prof.events())
+        names[label] = _kernel_names(lambda: ops.gat_fused_stats(csr, Q, K, V, 8))
     assert "gat_tma4_kernel" in names["joint"] and "gat_async_kernel" not in names["joint"], names["joint"]
     assert "gat_async_kernel" in names["separate"] and "gat_tma4_kernel" not in names["separate"], names["separate"]
 

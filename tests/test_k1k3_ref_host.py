@@ -142,12 +142,11 @@ def test_k1_epilogue_order():
     assert got[0, 0] == np.maximum(want0, np.float32(0)) and got[0, 1] == 0.0
 
 
-@pytest.mark.parametrize("D,aligned,impl,want", [
-    (31, True, None, False), (32, True, None, True), (512, True, "tma", True), (516, True, None, False),
-    (128, False, None, False), (128, True, "ldg", False), (128, True, "stream", False), (128, True, "bulk", False),
-    (128, True, "async", True), (256, True, "tma", True)])
-def test_k1_takes_plan(D, aligned, impl, want):
-    assert ref.k1_takes_plan(D, aligned, impl) == want
+@pytest.mark.parametrize("D,aligned,want", [
+    (4, True, False), (31, True, False), (32, True, True), (128, True, True), (256, True, True), (512, True, True),
+    (516, True, False), (1024, True, False), (128, False, False), (512, False, False)])
+def test_k1_takes_plan(D, aligned, want):
+    assert ref.k1_takes_plan(D, aligned) == want
 
 
 # ---- K3 bound -----------------------------------------------------------------------------------------------------

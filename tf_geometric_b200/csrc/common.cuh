@@ -36,6 +36,15 @@ inline cudaStream_t as_stream(void *s) { return reinterpret_cast<cudaStream_t>(s
 
 inline int64_t ceil_div64(int64_t a, int64_t b) { return (a + b - 1) / b; }
 
+// copies a work plan's tasks, hub slices and scratch into a kernel parameter struct (SpmmParams, GatParams, MaxParams)
+template <typename Params>
+inline void use_plan(Params &p, const tfgk_plan *plan) {
+    p.n_tasks = plan->n_tasks; p.task_row = plan->task_row; p.task_nrows = plan->task_nrows;
+    p.task_e0 = plan->task_e0; p.task_e1 = plan->task_e1; p.task_slot = plan->task_slot;
+    p.n_hubs = plan->n_hubs; p.hub_row = plan->hub_row; p.hub_slot0 = plan->hub_slot0; p.hub_nslots = plan->hub_nslots;
+    p.scratch = plan->scratch;
+}
+
 // cudaFuncAttributeMaxDynamicSharedMemorySize once per (kernel, device) instead of on every launch (the attribute call costs
 // microseconds - invisible next to a 10 ms aggregation, visible on Cora-sized graphs where a forward is a few launches).
 // Only ever raises the limit; safe from several host threads (a repeated set is harmless).

@@ -10,8 +10,6 @@
 // roofline of the reference's 5-pass segment_softmax + two [E,A] gathers + SpMM pipeline (SURVEY.md 8d).
 // No tensor cores: the per-edge dot products are 16-wide and the kernel is bound by the gathers.
 #include "common.cuh"
-#include <stdlib.h>
-#include <string.h>
 
 namespace tfgk {
 
@@ -749,22 +747,10 @@ static int launch_gat_tma4(const GatParams &p, cudaStream_t st) {
 }
 
 static int dispatch_gat_async(const GatParams &p, cudaStream_t st) {
-    // default: the TMA ring with two stages whenever K and V sit side by side in one buffer (the layers project them that way).
-    // TFGK_GAT_IMPL=async selects the cp.async ring; "tma:S" sets the depth S of the TMA ring (2, 3 or 4).
-    const char *g4 = getenv("TFGK_GAT_IMPL");
-    if (!(g4 && g4[0] == 'a')) {
-        const char *colon = g4 ? strchr(g4, ':') : nullptr;
-        const int stages = colon ? atoi(colon + 1) : 2;
-        const int rc = stages == 2 ? launch_gat_tma4<2>(p, st) : stages == 4 ? launch_gat_tma4<4>(p, st)
-                                                                           : launch_gat_tma4<3>(p, st);
-        if (rc != TFGK_ERR_UNSUPPORTED) return rc;
-    }
-    const char *cfg = getenv("TFGK_GAT_ASYNC_CFG");        // "UxS"; default 2x3
-    if (cfg && cfg[0] == '4' && cfg[2] == '2') return launch_gat_async<4, 2>(p, st);
-    if (cfg && cfg[0] == '4' && cfg[2] == '3') return launch_gat_async<4, 3>(p, st);
-    if (cfg && cfg[0] == '2' && cfg[2] == '4') return launch_gat_async<2, 4>(p, st);
-    if (cfg && cfg[0] == '2' && cfg[2] == '2') return launch_gat_async<2, 2>(p, st);
-    if (cfg && cfg[0] == '1' && cfg[2] == '4') return launch_gat_async<1, 4>(p, st);
+    // the TMA ring with two stages whenever K and V sit side by side in one buffer (the layers project them that way),
+    // the cp.async ring otherwise
+    const int rc = launch_gat_tma4<2>(p, st);
+    if (rc != TFGK_ERR_UNSUPPORTED) return rc;
     return launch_gat_async<2, 3>(p, st);
 }
 
@@ -1166,6 +1152,21 @@ static int dispatch_gat_v(const GatParams &p, int ncv, cudaStream_t st) {
     }
 }
 
+// the fields every fused GAT entry point sets alike: no K / V rows, attention buffer, plan or statistics yet
+static GatParams gat_params(const int64_t *rowptr, const int32_t *col, const float *Q, int64_t ldq, int64_t ldk,
+                            int64_t ldv, int32_t N, int32_t H, int32_t dqk, int32_t dv, float scale, int split,
+                            const float *bias, int act, float *out, int64_t ldo) {
+    GatParams p;
+    p.rowptr = rowptr; p.col = col;
+    p.Q = Q; p.ldq = ldq; p.K = nullptr; p.ldk = ldk; p.V = nullptr; p.ldv = ldv; p.Kb = nullptr; p.Vb = nullptr;
+    p.N = N; p.H = H; p.dqk = dqk; p.dv = dv; p.scale = scale; p.split = split;
+    p.bias = bias; p.act = act; p.att = nullptr; p.write_att = 0; p.out = out; p.ldo = ldo;
+    p.n_tasks = 0; p.task_row = nullptr; p.task_nrows = nullptr; p.task_e0 = nullptr; p.task_e1 = nullptr;
+    p.task_slot = nullptr; p.n_hubs = 0; p.hub_row = nullptr; p.hub_slot0 = nullptr; p.hub_nslots = nullptr; p.scratch = nullptr;
+    p.stats = nullptr;
+    return p;
+}
+
 }  // namespace tfgk
 
 using namespace tfgk;
@@ -1198,22 +1199,15 @@ static int gat_fused_impl(const int64_t *rowptr, const int32_t *col,
     const int out_w = split_value_heads ? VW : dv;
     TFGK_CHECK_ARG(ldq >= A && ldk >= A && ldv >= VW && ldo >= out_w, "gat: leading dimension too small");
 
-    GatParams p;
-    p.rowptr = rowptr; p.col = col;
-    p.Q = Q; p.ldq = ldq; p.K = K; p.ldk = ldk; p.V = V; p.ldv = ldv; p.Kb = nullptr; p.Vb = nullptr;
-    p.N = N; p.H = H; p.dqk = dqk; p.dv = dv; p.scale = scale; p.split = split_value_heads;
-    p.bias = bias; p.act = act; p.att = att; p.write_att = write_att; p.out = out; p.ldo = ldo;
-    p.n_tasks = 0; p.task_row = nullptr; p.task_nrows = nullptr; p.task_e0 = nullptr; p.task_e1 = nullptr;
-    p.task_slot = nullptr; p.n_hubs = 0; p.hub_row = nullptr; p.hub_slot0 = nullptr; p.hub_nslots = nullptr; p.scratch = nullptr;
+    GatParams p = gat_params(rowptr, col, Q, ldq, ldk, ldv, N, H, dqk, dv, scale, split_value_heads, bias, act, out, ldo);
+    p.K = K; p.V = V;
+    p.att = att; p.write_att = write_att;
     p.stats = stats;
     if (plan != nullptr && plan->n_tasks > 0) {
         if (plan->n_hubs > 0)
             TFGK_CHECK_ARG(plan->scratch != nullptr && plan->scratch_bytes >= (size_t)plan->n_slots * (H * dv + 64) * sizeof(float),
                            "gat: plan scratch too small (need %zu bytes)", (size_t)plan->n_slots * (H * dv + 64) * sizeof(float));
-        p.n_tasks = plan->n_tasks; p.task_row = plan->task_row; p.task_nrows = plan->task_nrows;
-        p.task_e0 = plan->task_e0; p.task_e1 = plan->task_e1; p.task_slot = plan->task_slot;
-        p.n_hubs = plan->n_hubs; p.hub_row = plan->hub_row; p.hub_slot0 = plan->hub_slot0;
-        p.hub_nslots = plan->hub_nslots; p.scratch = plan->scratch;
+        use_plan(p, plan);
     }
     cudaStream_t st = as_stream(stream);
 
@@ -1221,12 +1215,9 @@ static int gat_fused_impl(const int64_t *rowptr, const int32_t *col,
                       dqk <= 128 && dv % 4 == 0 && A <= 512 && VW <= 512 && ldq % 4 == 0 && ldk % 4 == 0 &&
                       ldv % 4 == 0 && ldo % 4 == 0 && aligned16(Q) && aligned16(K) && aligned16(V) && aligned16(out) &&
                       (!bias || aligned16(bias));
-    const char *impl = getenv("TFGK_GAT_IMPL");          // "twopass" forces the reference-order kernel
-    const bool twopass = impl && strncmp(impl, "twopass", 7) == 0, online = impl && strncmp(impl, "online", 6) == 0;
-    if (fast && dqk == dv && A <= 128 && !write_att && (stats != nullptr || !(twopass || online)))
-        return dispatch_gat_async(p, st);                    // "online" forces the register-staged single-pass kernel
+    if (fast && dqk == dv && A <= 128 && !write_att) return dispatch_gat_async(p, st);
     if (stats != nullptr) return TFGK_ERR_UNSUPPORTED;      // only the streaming kernel keeps (max, denominator)
-    if (fast && dqk == dv && !twopass) {
+    if (fast && dqk == dv) {
         switch ((A + 127) / 128) {
             case 1: return launch_gat_online<1>(p, st);
             case 2: return launch_gat_online<2>(p, st);
@@ -1291,22 +1282,14 @@ extern "C" int tfgk_gat_fused_bf16(const int64_t *rowptr, const int32_t *col,
     const int out_w = split_value_heads ? VW : dv;
     TFGK_CHECK_ARG(ldq >= A && ldk >= A && ldv >= VW && ldo >= out_w, "gat: leading dimension too small");
 
-    GatParams p;
-    p.rowptr = rowptr; p.col = col;
-    p.Q = Q; p.ldq = ldq; p.K = nullptr; p.ldk = ldk; p.V = nullptr; p.ldv = ldv; p.Kb = K; p.Vb = V;
-    p.N = N; p.H = H; p.dqk = dqk; p.dv = dv; p.scale = scale; p.split = split_value_heads;
-    p.bias = bias; p.act = act; p.att = att; p.write_att = 0; p.out = out; p.ldo = ldo;
-    p.n_tasks = 0; p.task_row = nullptr; p.task_nrows = nullptr; p.task_e0 = nullptr; p.task_e1 = nullptr;
-    p.task_slot = nullptr; p.n_hubs = 0; p.hub_row = nullptr; p.hub_slot0 = nullptr; p.hub_nslots = nullptr; p.scratch = nullptr;
-    p.stats = nullptr;
+    GatParams p = gat_params(rowptr, col, Q, ldq, ldk, ldv, N, H, dqk, dv, scale, split_value_heads, bias, act, out, ldo);
+    p.Kb = K; p.Vb = V;
+    p.att = att;
     if (plan != nullptr && plan->n_tasks > 0) {
         if (plan->n_hubs > 0)
             TFGK_CHECK_ARG(plan->scratch != nullptr && plan->scratch_bytes >= (size_t)plan->n_slots * (VW + 64) * sizeof(float),
                            "gat: plan scratch too small (need %zu bytes)", (size_t)plan->n_slots * (VW + 64) * sizeof(float));
-        p.n_tasks = plan->n_tasks; p.task_row = plan->task_row; p.task_nrows = plan->task_nrows;
-        p.task_e0 = plan->task_e0; p.task_e1 = plan->task_e1; p.task_slot = plan->task_slot;
-        p.n_hubs = plan->n_hubs; p.hub_row = plan->hub_row; p.hub_slot0 = plan->hub_slot0;
-        p.hub_nslots = plan->hub_nslots; p.scratch = plan->scratch;
+        use_plan(p, plan);
     }
     cudaStream_t st = as_stream(stream);
     // the shapes of the fp32 single-pass kernels (four consecutive columns per lane), with 8-byte aligned bf16 rows
@@ -1369,29 +1352,18 @@ extern "C" int tfgk_gat_fused_packed_f32(const int64_t *rowptr, const int32_t *c
     if (ldq % 4 || ldo % 4 || ldt % 16 || !aligned16(Q) || !aligned16(out) || !aligned16(table) || (bias && !aligned16(bias)))
         return set_error(TFGK_ERR_UNSUPPORTED, "gat_packed: Q, out, bias and table need 16-byte aligned rows, slots of a multiple of 64 bytes");
 
-    GatParams p;
-    p.rowptr = rowptr; p.col = col;
-    p.Q = Q; p.ldq = ldq; p.K = table; p.ldk = ldt; p.V = table; p.ldv = ldt; p.Kb = nullptr; p.Vb = nullptr;
-    p.N = N; p.H = H; p.dqk = dqk; p.dv = dqk; p.scale = scale; p.split = 1;
-    p.bias = bias; p.act = act; p.att = nullptr; p.write_att = 0; p.out = out; p.ldo = ldo;
-    p.n_tasks = 0; p.task_row = nullptr; p.task_nrows = nullptr; p.task_e0 = nullptr; p.task_e1 = nullptr;
-    p.task_slot = nullptr; p.n_hubs = 0; p.hub_row = nullptr; p.hub_slot0 = nullptr; p.hub_nslots = nullptr; p.scratch = nullptr;
-    p.stats = nullptr;
+    GatParams p = gat_params(rowptr, col, Q, ldq, ldt, ldt, N, H, dqk, dqk, scale, 1, bias, act, out, ldo);
+    p.K = table; p.V = table;
     p.ksize = ksize;
     if (plan != nullptr && plan->n_tasks > 0) {
         if (plan->n_hubs > 0)
             TFGK_CHECK_ARG(plan->scratch != nullptr && plan->scratch_bytes >= (size_t)plan->n_slots * (A + 64) * sizeof(float),
                            "gat_packed: plan scratch too small (need %zu bytes)", (size_t)plan->n_slots * (A + 64) * sizeof(float));
-        p.n_tasks = plan->n_tasks; p.task_row = plan->task_row; p.task_nrows = plan->task_nrows;
-        p.task_e0 = plan->task_e0; p.task_e1 = plan->task_e1; p.task_slot = plan->task_slot;
-        p.n_hubs = plan->n_hubs; p.hub_row = plan->hub_row; p.hub_slot0 = plan->hub_slot0;
-        p.hub_nslots = plan->hub_nslots; p.scratch = plan->scratch;
+        use_plan(p, plan);
     }
     cudaStream_t st = as_stream(stream);
-    // TFGK_GAT_PACKED_STAGES sets the depth of the ring (2, 3 or 4); two stages keep six blocks on an SM and measured fastest
-    const char *env = getenv("TFGK_GAT_PACKED_STAGES");
-    const int stages = env ? atoi(env) : 2;
-    return stages == 3 ? launch_gat_packed<3>(p, st) : stages == 4 ? launch_gat_packed<4>(p, st) : launch_gat_packed<2>(p, st);
+    // two ring stages keep six blocks on an SM and measured fastest
+    return launch_gat_packed<2>(p, st);
 }
 
 // fp8 K | V (inference): the TMA ring only.  Heads concatenated, dqk == dv, dqk / 4 a power of two, A = H * dqk <= 128, K | V
@@ -1416,30 +1388,15 @@ extern "C" int tfgk_gat_fused_fp8(const int64_t *rowptr, const int32_t *col, con
           (!bias || aligned16(bias)) && (reinterpret_cast<uintptr_t>(kv_exp) & 1u) == 0))
         return set_error(TFGK_ERR_UNSUPPORTED, "gat_fused_fp8: Q, out, bias and K | V rows must be 16-byte aligned");
 
-    GatParams p;
-    p.rowptr = rowptr; p.col = col;
-    p.Q = Q; p.ldq = ldq; p.K = nullptr; p.ldk = ldkv; p.V = nullptr; p.ldv = ldkv; p.Kb = nullptr; p.Vb = nullptr;
+    GatParams p = gat_params(rowptr, col, Q, ldq, ldkv, ldkv, N, H, dqk, dqk, scale, 1, bias, act, out, ldo);
     p.KV8 = KV; p.kvexp = kv_exp;
-    p.N = N; p.H = H; p.dqk = dqk; p.dv = dqk; p.scale = scale; p.split = 1;
-    p.bias = bias; p.act = act; p.att = nullptr; p.write_att = 0; p.out = out; p.ldo = ldo;
-    p.n_tasks = 0; p.task_row = nullptr; p.task_nrows = nullptr; p.task_e0 = nullptr; p.task_e1 = nullptr;
-    p.task_slot = nullptr; p.n_hubs = 0; p.hub_row = nullptr; p.hub_slot0 = nullptr; p.hub_nslots = nullptr; p.scratch = nullptr;
-    p.stats = nullptr;
     if (plan != nullptr && plan->n_tasks > 0) {
         if (plan->n_hubs > 0)
             TFGK_CHECK_ARG(plan->scratch != nullptr && plan->scratch_bytes >= (size_t)plan->n_slots * (A + 64) * sizeof(float),
                            "gat_fp8: plan scratch too small (need %zu bytes)", (size_t)plan->n_slots * (A + 64) * sizeof(float));
-        p.n_tasks = plan->n_tasks; p.task_row = plan->task_row; p.task_nrows = plan->task_nrows;
-        p.task_e0 = plan->task_e0; p.task_e1 = plan->task_e1; p.task_slot = plan->task_slot;
-        p.n_hubs = plan->n_hubs; p.hub_row = plan->hub_row; p.hub_slot0 = plan->hub_slot0;
-        p.hub_nslots = plan->hub_nslots; p.scratch = plan->scratch;
+        use_plan(p, plan);
     }
     cudaStream_t st = as_stream(stream);
     // 256-byte [K | V] spans at A = 128: six stages keep about as many bytes in flight per warp as three of bf16
-    const char *cfg = getenv("TFGK_GAT_FP8_STAGES");
-    const int stages = cfg ? atoi(cfg) : 6;
-    return stages == 3 ? launch_gat_tma4<3, uint8_t>(p, st)
-         : stages == 4 ? launch_gat_tma4<4, uint8_t>(p, st)
-         : stages == 8 ? launch_gat_tma4<8, uint8_t>(p, st)
-                       : launch_gat_tma4<6, uint8_t>(p, st);
+    return launch_gat_tma4<6, uint8_t>(p, st);
 }

@@ -25,7 +25,6 @@
 // Algorithmic bytes (unweighted; +4 per edge with weights):
 //   K11a  E*(4*D + 4) + N*(8*D + 8)          K11b  E*(8*D + 4) + N*(8*D + 8)   (+ the pass writing [out | Gn]: 20*D*N)
 #include "common.cuh"
-#include <stdlib.h>
 
 namespace tfgk {
 namespace {
@@ -368,12 +367,6 @@ int dispatch_max(const MaxParams &p, cudaStream_t st) {
     return launch_max<BWD, VEC, 32, 4, BWD ? 1 : 2>(p, st);
 }
 
-// tfgk_spmm_f32 takes its plan unless TFGK_SPMM_IMPL selects the register ("ldg"), streaming or bulk kernel
-bool k1_plan_enabled() {
-    const char *e = getenv("TFGK_SPMM_IMPL");
-    return !(e && (e[0] == 'b' || e[0] == 's' || e[0] == 'l'));
-}
-
 MaxParams max_params(const int64_t *rowptr, const int32_t *col, const float *w, const float *h, int64_t ldh, int32_t n,
                      float *out, int64_t ldo) {
     MaxParams p;
@@ -384,13 +377,6 @@ MaxParams max_params(const int64_t *rowptr, const int32_t *col, const float *w, 
     p.task_slot = nullptr; p.n_hubs = 0; p.hub_row = nullptr; p.hub_slot0 = nullptr; p.hub_nslots = nullptr;
     p.scratch = nullptr; p.n_slots = 0;
     return p;
-}
-
-void use_plan(MaxParams &p, const tfgk_plan *plan) {
-    p.n_tasks = plan->n_tasks; p.task_row = plan->task_row; p.task_nrows = plan->task_nrows;
-    p.task_e0 = plan->task_e0; p.task_e1 = plan->task_e1; p.task_slot = plan->task_slot;
-    p.n_hubs = plan->n_hubs; p.hub_row = plan->hub_row; p.hub_slot0 = plan->hub_slot0; p.hub_nslots = plan->hub_nslots;
-    p.scratch = plan->scratch; p.n_slots = plan->n_slots;
 }
 
 }  // namespace
@@ -408,7 +394,7 @@ extern "C" int tfgk_spmm_max_f32(const int64_t *rowptr, const int32_t *col, cons
     const bool vec4 = D % 4 == 0 && ldh % 4 == 0 && ldo % 4 == 0 && ldc % 4 == 0 && aligned16(h) && aligned16(out) &&
                       aligned16(cnt);
     // tfgk_spmm_f32's plan condition for the same h and out (one launch of the float4 ring kernels)
-    const bool plan_on = plan != nullptr && plan->n_tasks > 0 && vec4 && D >= 32 && D <= 512 && k1_plan_enabled();
+    const bool plan_on = plan != nullptr && plan->n_tasks > 0 && vec4 && D >= 32 && D <= 512;
     if (plan_on && plan->n_hubs > 0)
         TFGK_CHECK_ARG(plan->scratch != nullptr && plan->scratch_bytes >= (size_t)plan->n_slots * D * 8,
                        "spmm_max: plan scratch too small (need %zu bytes)", (size_t)plan->n_slots * D * 8);
@@ -419,7 +405,10 @@ extern "C" int tfgk_spmm_max_f32(const int64_t *rowptr, const int32_t *col, cons
         MaxParams p = max_params(rowptr, col, w, h + c0, ldh, n_dst, out + c0, ldo);
         p.D = D - c0 < per_launch ? D - c0 : per_launch;
         p.cnt = cnt + c0; p.ldc = ldc;
-        if (plan_on) use_plan(p, plan);
+        if (plan_on) {
+            use_plan(p, plan);
+            p.n_slots = plan->n_slots;
+        }
         const int rc = vec4 ? dispatch_max<false, 4>(p, st) : dispatch_max<false, 1>(p, st);
         if (rc != TFGK_OK) return rc;
     }
@@ -436,7 +425,7 @@ extern "C" int tfgk_spmm_max_bwd_f32(const int64_t *rowptr_t, const int32_t *dst
     TFGK_CHECK_ARG(rowptr_t && dst_t && h && dh && (n_dst == 0 || (out && cnt && g && pk)), "spmm_max_bwd: null pointer");
     TFGK_CHECK_ARG(ldh >= D && lddh >= D && ldo >= D && ldc >= D && ldg >= D, "spmm_max_bwd: leading dimension < D");
     // the per-edge gradient of the composition is a dense [E, D] table: K1 sums it with the plan for 32 <= D <= 512, D % 4 == 0
-    const bool plan_on = plan != nullptr && plan->n_tasks > 0 && D % 4 == 0 && D >= 32 && D <= 512 && k1_plan_enabled();
+    const bool plan_on = plan != nullptr && plan->n_tasks > 0 && D % 4 == 0 && D >= 32 && D <= 512;
     if (plan_on && plan->n_hubs > 0)
         TFGK_CHECK_ARG(plan->scratch != nullptr && plan->scratch_bytes >= (size_t)plan->n_slots * D * 4,
                        "spmm_max_bwd: plan scratch too small (need %zu bytes)", (size_t)plan->n_slots * D * 4);
@@ -454,7 +443,10 @@ extern "C" int tfgk_spmm_max_bwd_f32(const int64_t *rowptr_t, const int32_t *dst
         MaxParams p = max_params(rowptr_t, dst_t, w_t, h + c0, ldh, n_src, dh + c0, lddh);
         p.D = D - c0 < per_launch ? D - c0 : per_launch;
         p.pk = pk + c0; p.ldpk = 2 * (int64_t)D; p.gn_off = D;
-        if (plan_on) use_plan(p, plan);
+        if (plan_on) {
+            use_plan(p, plan);
+            p.n_slots = plan->n_slots;
+        }
         const int rc = vec4 ? dispatch_max<true, 4>(p, st) : dispatch_max<true, 1>(p, st);
         if (rc != TFGK_OK) return rc;
     }

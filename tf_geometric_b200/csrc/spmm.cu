@@ -12,7 +12,6 @@
 // Algorithmic bytes per launch (DESIGN.md): E*(4*D + 4 [+4 weighted]) + N*(4*D + 8).
 #include "common.cuh"
 #include <cuda_bf16.h>
-#include <stdlib.h>
 
 namespace tfgk {
 
@@ -272,307 +271,14 @@ __global__ void __launch_bounds__(kSpmmThreads) spmm_kernel(const SpmmParams p) 
 
 
 // ------------------------------------------------------------------------------------------------------------
-// TMA variant (D % 4 == 0): the neighbour rows are pulled by the bulk-copy engine (cp.async.bulk, SASS UBLKCP)
-// straight into a per-warp shared-memory ring, 32 rows per stage, completion tracked by an mbarrier transaction
-// count.  A warp owns a block of consecutive destination rows, i.e. a CONTIGUOUS range of CSR edges, and streams
-// that range in 32-edge chunks regardless of row boundaries: chunk j+1 is in flight while chunk j is reduced, so
-// the memory pipe never drains at a row change and no registers are spent on in-flight data.
-// Accumulation order and rounding are identical to spmm_kernel (CSR order, separate mul/add) => same bits.
-// ------------------------------------------------------------------------------------------------------------
-constexpr int kBulkChunk = 32;        // edges (= bulk copies) per stage, one per lane
-constexpr int kBulkRowsPerWarp = 32;  // destination rows per warp
-
-__device__ __forceinline__ uint32_t smem_addr(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
-__device__ __forceinline__ void mbar_wait_parity(uint32_t bar, uint32_t parity) {
-    uint32_t done = 0;
-    for (uint32_t spin = 0; !done; ++spin) {
-        asm volatile(
-            "{\n\t.reg .pred p;\n\t"
-            "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-            "selp.u32 %0, 1, 0, p;\n\t}"
-            : "=r"(done) : "r"(bar), "r"(parity) : "memory");
-        if (spin > (1u << 28)) __trap();     // a lost transaction becomes a launch failure, never a hang
-    }
-}
-
-template <int NC, bool IS_MAX>
-__global__ void __launch_bounds__(256) spmm_bulk_kernel(const SpmmParams p, int warps_per_cta, uint32_t row_bytes) {
-    extern __shared__ __align__(128) uint8_t smem_raw[];
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    // layout: [warps][2 stages][32 rows][row_bytes] then [warps][2] mbarriers
-    const uint32_t stage_bytes = kBulkChunk * row_bytes;
-    uint8_t *my_buf = smem_raw + (size_t)warp * 2 * stage_bytes;
-    uint64_t *bars = reinterpret_cast<uint64_t *>(smem_raw + (size_t)warps_per_cta * 2 * stage_bytes) + warp * 2;
-    const uint32_t bar0 = smem_addr(bars);
-    if (lane == 0) {
-        asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(bar0));
-        asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(bar0 + 8));
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    __syncwarp();
-
-    const int64_t r0 = ((int64_t)blockIdx.x * warps_per_cta + warp) * kBulkRowsPerWarp;
-    if (r0 >= p.n_dst) return;
-    const int64_t r1 = min((int64_t)p.n_dst, r0 + kBulkRowsPerWarp);
-    // lane l keeps rowptr[r0+l] and rowptr[r0+l+1] (clamped): ends of the warp's rows, broadcast by shuffle
-    const int64_t rp_lo = p.rowptr[min(r0 + lane, r1)];
-    const int64_t rp_hi = p.rowptr[min(r0 + lane + 1, r1)];
-    const int64_t e_begin = __shfl_sync(0xffffffffu, rp_lo, 0);
-    const int64_t e_end = p.rowptr[r1];
-    const int n_edges = (int)(e_end - e_begin);
-    const int n_chunks = (n_edges + kBulkChunk - 1) / kBulkChunk;
-    const bool weighted = p.w != nullptr;
-    const uint32_t buf_addr = smem_addr(my_buf);
-
-    float wreg[2] = {1.0f, 1.0f};
-    auto issue = [&](int j) {
-        const int stage = j & 1;
-        const int e = j * kBulkChunk + lane;
-        const int nb = min(kBulkChunk, n_edges - j * kBulkChunk);
-        const uint32_t bar = bar0 + 8 * stage;
-        if (lane == 0)
-            asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"((uint32_t)nb * row_bytes) : "memory");
-        float wv = 1.0f;
-        if (e < n_edges) {
-            const int c = ld_stream_i32(p.col + e_begin + e);
-            if (weighted) wv = ld_stream_f32(p.w + e_begin + e);
-            const float *src = p.h + (int64_t)c * p.ldh;
-            const uint32_t dst = buf_addr + stage * stage_bytes + lane * row_bytes;
-            asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                         ::"r"(dst), "l"(src), "r"(row_bytes), "r"(bar) : "memory");
-        }
-        wreg[stage] = wv;
-    };
-
-    int coff[NC];
-    bool cok[NC];
-    float acc[NC][4];
-#pragma unroll
-    for (int k = 0; k < NC; ++k) {
-        coff[k] = (lane + 32 * k) * 4;
-        cok[k] = coff[k] < p.D;
-#pragma unroll
-        for (int x = 0; x < 4; ++x) acc[k][x] = IS_MAX ? -FLT_MAX : 0.0f;
-    }
-
-    int64_t r = r0;
-    int64_t row_end = __shfl_sync(0xffffffffu, rp_hi, 0) - e_begin;   // end of row r, relative to e_begin
-    const bool is_mean = p.reduce == TFGK_REDUCE_MEAN;
-
-    auto finalize_row = [&]() {
-        const int64_t row_start = __shfl_sync(0xffffffffu, rp_lo, (int)(r - r0));
-        const int deg = (int)(row_end + e_begin - row_start);
-        const float cnt = (float)max(deg, 1);
-#pragma unroll
-        for (int k = 0; k < NC; ++k) {
-            if (cok[k]) {
-                float ad[4], bs[4], o[4];
-                if (p.addend) load_vec<4>(p.addend + r * p.ld_addend + coff[k], ad);
-                if (p.bias) load_vec<4>(p.bias + coff[k], bs);
-#pragma unroll
-                for (int x = 0; x < 4; ++x) {
-                    float a = acc[k][x];
-                    if (is_mean) a = __fdiv_rn(a, cnt);
-                    if (p.addend) a = __fadd_rn(__fmul_rn(a, p.alpha), __fmul_rn(ad[x], p.beta));
-                    else if (p.alpha != 1.0f) a = __fmul_rn(a, p.alpha);
-                    if (p.bias) a = __fadd_rn(a, bs[x]);
-                    o[x] = apply_act(a, p.act);
-                    acc[k][x] = IS_MAX ? -FLT_MAX : 0.0f;
-                }
-                store_vec<4>(p.out + r * p.ldo + coff[k], o);
-            }
-        }
-        ++r;
-        if (r < r1) row_end = __shfl_sync(0xffffffffu, rp_hi, (int)(r - r0)) - e_begin;
-    };
-
-    if (n_chunks > 0) issue(0);
-    for (int j = 0; j < n_chunks; ++j) {
-        __syncwarp();                                   // every lane is done reading the stage issue(j+1) overwrites
-        if (j + 1 < n_chunks) issue(j + 1);
-        const int stage = j & 1;
-        mbar_wait_parity(bar0 + 8 * stage, (uint32_t)(j >> 1) & 1u);
-        const int nb = min(kBulkChunk, n_edges - j * kBulkChunk);
-        const uint8_t *sbuf = my_buf + stage * stage_bytes;
-        const float wmine = wreg[stage];
-        for (int i = 0; i < nb; ++i) {
-            const int64_t e = (int64_t)j * kBulkChunk + i;
-            while (e == row_end) finalize_row();        // also steps over empty rows
-            const float we = __shfl_sync(0xffffffffu, wmine, i);
-#pragma unroll
-            for (int k = 0; k < NC; ++k) {
-                if (cok[k]) {
-                    const float4 v = *reinterpret_cast<const float4 *>(sbuf + (size_t)i * row_bytes + coff[k] * 4);
-                    const float m0 = __fmul_rn(v.x, we), m1 = __fmul_rn(v.y, we), m2 = __fmul_rn(v.z, we), m3 = __fmul_rn(v.w, we);
-                    acc[k][0] = IS_MAX ? fmaxf(acc[k][0], m0) : __fadd_rn(acc[k][0], m0);
-                    acc[k][1] = IS_MAX ? fmaxf(acc[k][1], m1) : __fadd_rn(acc[k][1], m1);
-                    acc[k][2] = IS_MAX ? fmaxf(acc[k][2], m2) : __fadd_rn(acc[k][2], m2);
-                    acc[k][3] = IS_MAX ? fmaxf(acc[k][3], m3) : __fadd_rn(acc[k][3], m3);
-                }
-            }
-        }
-    }
-    while (r < r1) finalize_row();                      // last row and trailing empty rows
-}
-
-// ------------------------------------------------------------------------------------------------------------
-// Streaming variant (float4 rows): a warp owns kStreamRows consecutive destination rows = one CONTIGUOUS range of CSR
-// edges, and walks that range in rounds of U edges with two register buffers: the gathers of round g+1 are issued
-// before round g is reduced, and the (col, w) of the next 32-edge chunk are fetched one chunk ahead.  The memory
-// pipe therefore never drains at a row boundary or while indices are being fetched - by Little's law the achieved
-// bandwidth is (bytes in flight) / (loaded latency), and this keeps 8-16 rows in flight per warp all the time instead
-// of 8 for a fraction of it.  Rounding and order are unchanged (CSR order, separate mul/add) => same bits.
-// ------------------------------------------------------------------------------------------------------------
-constexpr int kStreamRows = 16;        // destination rows per warp (their finished sums wait in shared memory)
-constexpr int kStreamThreads = 128;
-constexpr int kStreamWarps = kStreamThreads / 32;
-
-template <bool IS_MAX, int U, int MINB>
-__global__ void __launch_bounds__(kStreamThreads, MINB) spmm_stream_kernel(const SpmmParams p) {
-    static_assert(32 % U == 0, "a round must not straddle an index chunk");
-    constexpr int RPC = 32 / U;                 // rounds per 32-edge index chunk
-    __shared__ float4 stash[kStreamWarps][kStreamRows][32];      // finished row sums, one float4 per lane
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const int64_t r0 = ((int64_t)blockIdx.x * kStreamWarps + warp) * kStreamRows;
-    if (r0 >= p.n_dst) return;
-    const int n_rows = (int)min((int64_t)kStreamRows, (int64_t)p.n_dst - r0);
-    // lane l < n_rows describes row r0 + l
-    const int64_t rp_lo = p.rowptr[r0 + min(lane, n_rows)];
-    const int64_t rp_hi = p.rowptr[r0 + min(lane + 1, n_rows)];
-    const int64_t e_begin = __shfl_sync(0xffffffffu, rp_lo, 0);
-    const int n_edges = (int)(__shfl_sync(0xffffffffu, rp_hi, n_rows - 1) - e_begin);
-    const int my_end = (int)(rp_hi - e_begin);                   // end of row `lane`, relative
-    const int my_deg = (int)(rp_hi - rp_lo);
-    const uint32_t nonempty = __ballot_sync(0xffffffffu, lane < n_rows && my_deg > 0);
-    const bool weighted = p.w != nullptr;
-    const float *__restrict__ h = p.h;
-    const int coff = lane * 4;
-    const bool cok = coff < p.D;
-    const float init = IS_MAX ? -FLT_MAX : 0.0f;
-
-#pragma unroll
-    for (int i = 0; i < kStreamRows; ++i) stash[warp][i][lane] = make_float4(init, init, init, init);
-
-    float a0 = init, a1 = init, a2 = init, a3 = init;
-    int rel = nonempty ? __ffs(nonempty) - 1 : n_rows;           // current (non-empty) row
-    int row_end = rel < n_rows ? __shfl_sync(0xffffffffu, my_end, rel & 31) : -1;
-
-    auto load_chunk = [&](int c, int &ci, float &wi) {
-        const int e = c * 32 + lane;
-        ci = 0;
-        wi = 1.0f;
-        if (e < n_edges) {
-            ci = ld_stream_i32(p.col + e_begin + e);
-            if (weighted) wi = ld_stream_f32(p.w + e_begin + e);
-        }
-    };
-    auto issue = [&](int g, int ci, float4 (&buf)[U]) {
-        const int base = (g % RPC) * U;
-#pragma unroll
-        for (int u = 0; u < U; ++u) {
-            const int c = __shfl_sync(0xffffffffu, ci, base + u);
-            if (g * U + u < n_edges && cok) buf[u] = __ldg(reinterpret_cast<const float4 *>(h + (int64_t)c * p.ldh + coff));
-        }
-    };
-    auto consume = [&](int g, float wi, const float4 (&buf)[U]) {
-        const int base = (g % RPC) * U;
-#pragma unroll
-        for (int u = 0; u < U; ++u) {
-            const int e = g * U + u;
-            const float we = __shfl_sync(0xffffffffu, wi, base + u);
-            if (e < n_edges) {
-                const float m0 = __fmul_rn(buf[u].x, we), m1 = __fmul_rn(buf[u].y, we);
-                const float m2 = __fmul_rn(buf[u].z, we), m3 = __fmul_rn(buf[u].w, we);
-                a0 = IS_MAX ? fmaxf(a0, m0) : __fadd_rn(a0, m0);
-                a1 = IS_MAX ? fmaxf(a1, m1) : __fadd_rn(a1, m1);
-                a2 = IS_MAX ? fmaxf(a2, m2) : __fadd_rn(a2, m2);
-                a3 = IS_MAX ? fmaxf(a3, m3) : __fadd_rn(a3, m3);
-                if (e + 1 == row_end) {          // last edge of the row: park the sum, move to the next non-empty row
-                    stash[warp][rel][lane] = make_float4(a0, a1, a2, a3);
-                    a0 = a1 = a2 = a3 = init;
-                    const uint32_t rest = rel < 31 ? (nonempty >> (rel + 1)) : 0u;
-                    rel = rest ? rel + __ffs(rest) : n_rows;
-                    row_end = rel < n_rows ? __shfl_sync(0xffffffffu, my_end, rel & 31) : -1;
-                }
-            }
-        }
-    };
-
-    float4 buf0[U], buf1[U];
-    int ca, cb;
-    float wa, wb;
-    load_chunk(0, ca, wa);
-    load_chunk(1, cb, wb);
-    issue(0, ca, buf0);
-    const int n_rounds = (n_edges + U - 1) / U;
-    // two rounds per iteration (buf0 <-> buf1); the chunk registers are picked with selects, not by unrolling
-    for (int g = 0; g < n_rounds; g += 2) {
-        {
-            const int cn = (g + 1) / RPC, cc = g / RPC;
-            issue(g + 1, (cn & 1) ? cb : ca, buf1);
-            consume(g, (cc & 1) ? wb : wa, buf0);
-            if ((g + 1) % RPC == 0) { if (cc & 1) load_chunk(cc + 2, cb, wb); else load_chunk(cc + 2, ca, wa); }
-        }
-        {
-            const int cn = (g + 2) / RPC, cc = (g + 1) / RPC;
-            issue(g + 2, (cn & 1) ? cb : ca, buf0);
-            consume(g + 1, (cc & 1) ? wb : wa, buf1);
-            if ((g + 2) % RPC == 0) { if (cc & 1) load_chunk(cc + 2, cb, wb); else load_chunk(cc + 2, ca, wa); }
-        }
-    }
-
-    // epilogue for the warp's rows: uniform loop, coalesced 512-byte stores
-    const bool is_mean = p.reduce == TFGK_REDUCE_MEAN;
-    float bs[4] = {0.f, 0.f, 0.f, 0.f};
-    if (p.bias && cok) load_vec<4>(p.bias + coff, bs);
-    for (int i = 0; i < n_rows; ++i) {
-        const float cnt = (float)max(__shfl_sync(0xffffffffu, my_deg, i), 1);     // every lane takes part in the shuffle
-        if (!cok) continue;
-        const float4 v = stash[warp][i][lane];
-        float a[4] = {v.x, v.y, v.z, v.w}, ad[4], o[4];
-        const int64_t r = r0 + i;
-        if (p.addend) load_vec<4>(p.addend + r * p.ld_addend + coff, ad);
-#pragma unroll
-        for (int x = 0; x < 4; ++x) {
-            float t = a[x];
-            if (is_mean) t = __fdiv_rn(t, cnt);
-            if (p.addend) t = __fadd_rn(__fmul_rn(t, p.alpha), __fmul_rn(ad[x], p.beta));
-            else if (p.alpha != 1.0f) t = __fmul_rn(t, p.alpha);
-            if (p.bias) t = __fadd_rn(t, bs[x]);
-            o[x] = apply_act(t, p.act);
-        }
-        store_vec<4>(p.out + r * p.ldo + coff, o);
-    }
-}
-
-template <int U, int MINB>
-static int launch_spmm_stream(const SpmmParams &p, cudaStream_t st) {
-    const int64_t rows_per_cta = (int64_t)kStreamWarps * kStreamRows;
-    const unsigned blocks = (unsigned)ceil_div64(p.n_dst, rows_per_cta);
-    if (p.reduce == TFGK_REDUCE_MAX) spmm_stream_kernel<true, U, MINB><<<blocks, kStreamThreads, 0, st>>>(p);
-    else spmm_stream_kernel<false, U, MINB><<<blocks, kStreamThreads, 0, st>>>(p);
-    TFGK_LAUNCH_CHECK();
-    return TFGK_OK;
-}
-
-static int dispatch_spmm_stream(const SpmmParams &p, cudaStream_t st) {
-    if (p.D > 128) return TFGK_ERR_UNSUPPORTED;            // wider rows: the per-row kernel (register budget)
-    const char *cfg = getenv("TFGK_SPMM_STREAM_CFG");     // tuning knob: "8x4" (default), "8x5", "4x8", "16x2"
-    if (cfg && cfg[0] == '4') return launch_spmm_stream<4, 8>(p, st);
-    if (cfg && cfg[0] == '1') return launch_spmm_stream<16, 2>(p, st);
-    if (cfg && cfg[0] == '8' && cfg[2] == '5') return launch_spmm_stream<8, 5>(p, st);
-    return launch_spmm_stream<8, 4>(p, st);
-}
-
-// ------------------------------------------------------------------------------------------------------------
 // cp.async variant.  Register double-buffering cannot overlap two gather rounds: a warp has six counting scoreboard
 // slots, ptxas puts the loads of both rounds on the same slots, and the first use of round g then also waits for
 // round g+1 (visible in the SASS).  LDGSTS copies are tracked by commit groups instead, so a
 // per-warp shared-memory ring of S stages x U rows keeps (S-1)*U rows in flight per warp with no register cost.
 // Each lane copies - and later reads back - only its own 16-byte slices: shared memory is used as an asynchronous
-// extension of the register file, no cross-lane traffic, no barriers.  Edge streaming as above: a warp owns
-// kAsyncRows consecutive rows = a contiguous CSR range.  Same rounding and order => same bits.
+// extension of the register file, no cross-lane traffic, no barriers.  Edge streaming: a warp owns kAsyncRows
+// consecutive rows = a contiguous CSR range, walked in rounds of U edges regardless of row boundaries, so the memory
+// pipe never drains at a row change.  Same rounding and order as spmm_kernel => same bits.
 // ------------------------------------------------------------------------------------------------------------
 constexpr int kAsyncRows = 32;
 constexpr int kAsyncWarps = 4;
@@ -767,6 +473,18 @@ __global__ void __launch_bounds__(kAsyncWarps * 32) spmm_async_kernel(const Spmm
 __device__ __forceinline__ void tma_row(uint32_t dst, const void *src, uint32_t bytes, uint32_t bar) {
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
                  ::"r"(dst), "l"(src), "r"(bytes), "r"(bar) : "memory");
+}
+
+__device__ __forceinline__ void mbar_wait_parity(uint32_t bar, uint32_t parity) {
+    uint32_t done = 0;
+    for (uint32_t spin = 0; !done; ++spin) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\t"
+            "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
+            "selp.u32 %0, 1, 0, p;\n\t}"
+            : "=r"(done) : "r"(bar), "r"(parity) : "memory");
+        if (spin > (1u << 28)) __trap();     // a lost transaction becomes a launch failure, never a hang
+    }
 }
 
 template <bool IS_MAX, int S, typename T, bool DUAL = false>
@@ -1049,67 +767,14 @@ static int launch_spmm_tma4(const SpmmParams &p, cudaStream_t st) {
     return TFGK_OK;
 }
 
+// the cp.async ring by width: four float4 slices of a row per lane at most, 512 columns
+template <typename T, bool DUAL = false>
 static int dispatch_spmm_async(const SpmmParams &p, cudaStream_t st) {
     const int lanes = (p.D + 3) / 4;
-    const char *cfg = getenv("TFGK_SPMM_ASYNC_CFG");      // tuning knob for NC == 1, "UxS"; default 4x3
-    if (lanes <= 32) {
-        if (cfg && cfg[0] == '8' && cfg[2] == '4') return launch_spmm_async<1, 8, 4>(p, st);
-        if (cfg && cfg[0] == '8' && cfg[2] == '2') return launch_spmm_async<1, 8, 2>(p, st);
-        if (cfg && cfg[0] == '8' && cfg[2] == '6') return launch_spmm_async<1, 8, 6>(p, st);
-        if (cfg && cfg[0] == '8' && cfg[2] == '3') return launch_spmm_async<1, 8, 3>(p, st);
-        if (cfg && cfg[0] == '4' && cfg[2] == '4') return launch_spmm_async<1, 4, 4>(p, st);
-        if (cfg && cfg[0] == '4' && cfg[2] == '6') return launch_spmm_async<1, 4, 6>(p, st);
-        if (cfg && cfg[0] == '2' && cfg[2] == '6') return launch_spmm_async<1, 2, 6>(p, st);
-        if (cfg && cfg[0] == '2' && cfg[2] == '4') return launch_spmm_async<1, 2, 4>(p, st);
-        return launch_spmm_async<1, 4, 3>(p, st);      // default: four rows per round, three stages
-    }
-    if (lanes <= 64) return launch_spmm_async<2, 4, 4>(p, st);
-    if (lanes <= 96) return launch_spmm_async<3, 4, 3>(p, st);
-    return launch_spmm_async<4, 2, 4>(p, st);
-}
-
-// Default kernel: the TMA row-copy ring with three stages for every float4-aligned width up to 256 columns.
-// TFGK_SPMM_IMPL=async selects the cp.async ring; TFGK_SPMM_TMA_STAGES sets the depth of the TMA ring (2, 3, 4, 6 or 8).
-static bool spmm_prefers_tma4(int D) { return D >= 32 && D <= 256; }
-
-static int spmm_impl_choice() {
-    // 0 = register-staged LDG gather, 1 = TMA bulk gather.  TFGK_SPMM_IMPL overrides (read per call: cheap).
-    const char *e = getenv("TFGK_SPMM_IMPL");
-    if (e && e[0] == 'b') return 1;
-    if (e && e[0] == 's') return 2;
-    if (e && e[0] == 't') return 4;      // "tma": TMA row-copy ring
-    if (e && e[0] == 'l') return 0;
-    if (e && e[0] == 'a') return 3;      // "async": the cp.async ring for every shape
-    return 5;                            // default: by row shape (spmm_prefers_tma4); "ldg" / "stream" / "bulk" are the alternatives
-}
-
-template <int NC>
-static int launch_spmm_bulk(const SpmmParams &p, cudaStream_t st) {
-    const uint32_t row_bytes = (uint32_t)p.D * 4u;
-    const size_t per_warp = 2u * kBulkChunk * row_bytes + 16;
-    int warps = (int)((220 * 1024) / per_warp);
-    if (warps > 8) warps = 8;
-    if (warps < 1) return TFGK_ERR_UNSUPPORTED;
-    const size_t smem = (size_t)warps * per_warp;
-    const int64_t rows_per_cta = (int64_t)warps * kBulkRowsPerWarp;
-    const unsigned blocks = (unsigned)ceil_div64(p.n_dst, rows_per_cta);
-    if (p.reduce == TFGK_REDUCE_MAX) {
-        TFGK_CUDA(ensure_dynamic_smem(spmm_bulk_kernel<NC, true>, smem));
-        spmm_bulk_kernel<NC, true><<<blocks, warps * 32, smem, st>>>(p, warps, row_bytes);
-    } else {
-        TFGK_CUDA(ensure_dynamic_smem(spmm_bulk_kernel<NC, false>, smem));
-        spmm_bulk_kernel<NC, false><<<blocks, warps * 32, smem, st>>>(p, warps, row_bytes);
-    }
-    TFGK_LAUNCH_CHECK();
-    return TFGK_OK;
-}
-
-static int dispatch_spmm_bulk(const SpmmParams &p, cudaStream_t st) {
-    const int lanes = (p.D + 3) / 4;
-    if (lanes <= 32) return launch_spmm_bulk<1>(p, st);
-    if (lanes <= 64) return launch_spmm_bulk<2>(p, st);
-    if (lanes <= 96) return launch_spmm_bulk<3>(p, st);
-    return launch_spmm_bulk<4>(p, st);
+    return lanes <= 32 ? launch_spmm_async<1, 4, 3, T, DUAL>(p, st)
+         : lanes <= 64 ? launch_spmm_async<2, 4, 4, T, DUAL>(p, st)
+         : lanes <= 96 ? launch_spmm_async<3, 4, 3, T, DUAL>(p, st)
+                       : launch_spmm_async<4, 2, 4, T, DUAL>(p, st);
 }
 
 template <int VEC, int G, int NC, int U, typename T, bool DUAL>
@@ -1176,13 +841,6 @@ static SpmmParams spmm_params(const int64_t *rowptr, const int32_t *col, const f
     return p;
 }
 
-static void spmm_use_plan(SpmmParams &p, const tfgk_plan *plan) {
-    p.n_tasks = plan->n_tasks; p.task_row = plan->task_row; p.task_nrows = plan->task_nrows;
-    p.task_e0 = plan->task_e0; p.task_e1 = plan->task_e1; p.task_slot = plan->task_slot;
-    p.n_hubs = plan->n_hubs; p.hub_row = plan->hub_row; p.hub_slot0 = plan->hub_slot0;
-    p.hub_nslots = plan->hub_nslots; p.scratch = plan->scratch;
-}
-
 }  // namespace tfgk
 
 using namespace tfgk;
@@ -1204,34 +862,15 @@ extern "C" int tfgk_spmm_f32(const int64_t *rowptr, const int32_t *col, const fl
         SpmmParams p = spmm_params(rowptr, col, w, ldh, n_dst, reduce, alpha, addend, ld_addend, beta, bias, act, out, ldo,
                                    c0, (D - c0 < cols_per_launch) ? D - c0 : cols_per_launch);
         p.h = h + c0;
-        // the plan applies when the whole width runs in one launch of the streaming kernel (scratch rows are D wide)
-        const bool use_plan = plan != nullptr && plan->n_tasks > 0 && vec4 && D >= 32 && D <= cols_per_launch &&
-                              (spmm_impl_choice() >= 3);
-        if (use_plan) spmm_use_plan(p, plan);
+        // the plan applies when the whole width runs in one launch of a ring kernel (scratch rows are D wide)
+        if (plan != nullptr && plan->n_tasks > 0 && vec4 && D >= 32 && D <= cols_per_launch) use_plan(p, plan);
+        if (vec4 && p.D >= 32) {
+            // the TMA row-copy ring with three stages up to 256 columns, the cp.async ring above
+            int rcr = launch_spmm_tma4<3>(p, as_stream(stream));
+            if (rcr == TFGK_ERR_UNSUPPORTED) rcr = dispatch_spmm_async<float>(p, as_stream(stream));
+            if (rcr != TFGK_ERR_UNSUPPORTED) { if (rcr != TFGK_OK) return rcr; continue; }
+        }
         const int lanes = (p.D + vec - 1) / vec;
-        const int choice = spmm_impl_choice() == 5 ? (spmm_prefers_tma4(p.D) ? 4 : 3) : spmm_impl_choice();
-        if (vec4 && p.D >= 32 && choice == 4) {
-            const char *cfg = getenv("TFGK_SPMM_TMA_STAGES");
-            const int st = cfg ? atoi(cfg) : 3;
-            const int rcg = st == 2 ? launch_spmm_tma4<2>(p, as_stream(stream))
-                          : st == 3 ? launch_spmm_tma4<3>(p, as_stream(stream))
-                          : st == 6 ? launch_spmm_tma4<6>(p, as_stream(stream))
-                          : st == 8 ? launch_spmm_tma4<8>(p, as_stream(stream))
-                                    : launch_spmm_tma4<4>(p, as_stream(stream));
-            if (rcg != TFGK_ERR_UNSUPPORTED) { if (rcg != TFGK_OK) return rcg; continue; }
-        }
-        if (vec4 && p.D >= 32 && (choice == 3 || choice == 4)) {
-            const int rca = dispatch_spmm_async(p, as_stream(stream));
-            if (rca != TFGK_ERR_UNSUPPORTED) { if (rca != TFGK_OK) return rca; continue; }
-        }
-        if (vec4 && p.D >= 32 && choice == 2) {
-            const int rcs = dispatch_spmm_stream(p, as_stream(stream));
-            if (rcs != TFGK_ERR_UNSUPPORTED) { if (rcs != TFGK_OK) return rcs; continue; }
-        }
-        if (vec4 && p.D >= 32 && choice == 1) {
-            const int rcb = dispatch_spmm_bulk(p, as_stream(stream));
-            if (rcb != TFGK_ERR_UNSUPPORTED) { if (rcb != TFGK_OK) return rcb; continue; }
-        }
         const int rc = vec4 ? dispatch_spmm<4>(p, lanes, as_stream(stream)) : dispatch_spmm<1>(p, lanes, as_stream(stream));
         if (rc != TFGK_OK) return rc;
     }
@@ -1260,16 +899,12 @@ extern "C" int tfgk_spmm_bf16(const int64_t *rowptr, const int32_t *col, const f
         SpmmParams p = spmm_params(rowptr, col, w, ldh, n_dst, reduce, alpha, addend, ld_addend, beta, bias, act, out, ldo,
                                    0, D);
         p.hb = h;
-        // the plan is taken exactly when the fp32 entry point takes it for the same shape (TFGK_SPMM_IMPL included)
-        if (plan != nullptr && plan->n_tasks > 0 && spmm_impl_choice() >= 3) spmm_use_plan(p, plan);
+        // the plan is taken exactly when the fp32 entry point takes it for the same shape
+        if (plan != nullptr && plan->n_tasks > 0) use_plan(p, plan);
         // 256-byte rows at D = 128: six ring stages keep as many bytes in flight per warp as three stages of fp32 rows
         const int rc = launch_spmm_tma4<6, uint16_t>(p, st);        // TFGK_ERR_UNSUPPORTED unless 16-byte rows, D <= 256
         if (rc != TFGK_ERR_UNSUPPORTED) return rc;
-        const int lanes = (D + 3) / 4;
-        return lanes <= 32 ? launch_spmm_async<1, 4, 3, uint16_t>(p, st)
-             : lanes <= 64 ? launch_spmm_async<2, 4, 4, uint16_t>(p, st)
-             : lanes <= 96 ? launch_spmm_async<3, 4, 3, uint16_t>(p, st)
-                           : launch_spmm_async<4, 2, 4, uint16_t>(p, st);
+        return dispatch_spmm_async<uint16_t>(p, st);
     }
     for (int c0 = 0; c0 < D; c0 += 128) {               // scalar path: 32 lanes x 4 single columns per launch
         SpmmParams p = spmm_params(rowptr, col, w, ldh, n_dst, reduce, alpha, addend, ld_addend, beta, bias, act, out, ldo,
@@ -1308,10 +943,10 @@ extern "C" int tfgk_spmm_bf16_dual(const int64_t *rowptr, const int32_t *col, co
     const bool outb4 = !out_bf16 || ((ldob % 4 == 0) && aligned8(out_bf16));
     // tfgk_spmm_bf16's ring condition (its rows4), with the fp32 out it would write
     const bool rows4 = (D % 4 == 0) && (ldh % 4 == 0) && aligned8(h) && out4 && in_aligned;
-    const bool use_plan = rows4 && D >= 32 && D <= 512 && plan != nullptr && plan->n_tasks > 0 && spmm_impl_choice() >= 3;
+    const bool plan_on = rows4 && D >= 32 && D <= 512 && plan != nullptr && plan->n_tasks > 0;
     // width read per row: D, or D with its pad columns where that lets a ring run (the plan's scratch must hold them)
     const int32_t d8 = (D + 7) / 8 * 8, d4 = (D + 3) / 4 * 4;
-    const bool scratch8 = !use_plan || plan->n_hubs == 0 || plan->scratch_bytes >= (size_t)plan->n_slots * d8 * sizeof(float);
+    const bool scratch8 = !plan_on || plan->n_hubs == 0 || plan->scratch_bytes >= (size_t)plan->n_slots * d8 * sizeof(float);
     int32_t width = 0;                                   // 0: the scalar path
     if (ldh % 8 == 0 && ldh >= d8 && aligned16(h) && d8 >= 32 && d8 <= 256 && scratch8) width = d8;   // TMA ring
     else if (ldh % 4 == 0 && ldh >= d4 && aligned8(h) && d4 >= 32 && d4 <= 512) width = d4;            // cp.async ring
@@ -1322,14 +957,10 @@ extern "C" int tfgk_spmm_bf16_dual(const int64_t *rowptr, const int32_t *col, co
         p.hb = h;
         p.outb = out_bf16; p.ldob = ldob; p.d_store = D;
         p.io4 = D % 4 == 0 && out4 && outb4 && in_aligned;
-        if (use_plan) spmm_use_plan(p, plan);
+        if (plan_on) use_plan(p, plan);
         const int rc = launch_spmm_tma4<6, uint16_t, true>(p, st);   // TFGK_ERR_UNSUPPORTED unless 16-byte rows, width <= 256
         if (rc != TFGK_ERR_UNSUPPORTED) return rc;
-        const int lanes = width / 4;
-        return lanes <= 32 ? launch_spmm_async<1, 4, 3, uint16_t, true>(p, st)
-             : lanes <= 64 ? launch_spmm_async<2, 4, 4, uint16_t, true>(p, st)
-             : lanes <= 96 ? launch_spmm_async<3, 4, 3, uint16_t, true>(p, st)
-                           : launch_spmm_async<4, 2, 4, uint16_t, true>(p, st);
+        return dispatch_spmm_async<uint16_t, true>(p, st);
     }
     for (int c0 = 0; c0 < D; c0 += 128) {               // scalar path: 32 lanes x 4 single columns per launch
         SpmmParams p = spmm_params(rowptr, col, w, ldh, n_dst, reduce, alpha, addend, ld_addend, beta, bias, act, out, ldo,
@@ -1365,12 +996,12 @@ extern "C" int tfgk_spmm_fp8(const int64_t *rowptr, const int32_t *col, const fl
     const bool in_aligned = (!addend || ((ld_addend % 4 == 0) && aligned16(addend))) && (!bias || aligned16(bias));
     const bool out4 = (ldo % 4 == 0) && aligned16(out);
     // tfgk_spmm_f32's plan condition for the dequantised table (16-byte aligned fp32 rows, same ldh in elements)
-    const bool use_plan = D % 4 == 0 && ldh % 4 == 0 && out4 && in_aligned && D >= 32 && D <= 512 && plan != nullptr &&
-                          plan->n_tasks > 0 && spmm_impl_choice() >= 3;
+    const bool plan_on = D % 4 == 0 && ldh % 4 == 0 && out4 && in_aligned && D >= 32 && D <= 512 && plan != nullptr &&
+                         plan->n_tasks > 0;
     const int32_t d16 = (D + 15) / 16 * 16;
     cudaStream_t st = as_stream(stream);
     if (ldh % 16 == 0 && ldh >= d16 && aligned16(h) && d16 <= 256) {
-        if (use_plan && plan->n_hubs > 0)
+        if (plan_on && plan->n_hubs > 0)
             TFGK_CHECK_ARG(plan->scratch != nullptr && plan->scratch_bytes >= (size_t)plan->n_slots * d16 * sizeof(float),
                            "spmm_fp8: plan scratch too small (need %zu bytes)", (size_t)plan->n_slots * d16 * sizeof(float));
         SpmmParams p = spmm_params(rowptr, col, w, ldh, n_dst, reduce, alpha, addend, ld_addend, beta, bias, act, out, ldo,
@@ -1378,13 +1009,9 @@ extern "C" int tfgk_spmm_fp8(const int64_t *rowptr, const int32_t *col, const fl
         p.h8 = h; p.hexp = h_exp; p.n_grp = n_grp;
         p.d_store = D;
         p.io4 = D % 4 == 0 && out4 && in_aligned;
-        if (use_plan) spmm_use_plan(p, plan);
+        if (plan_on) use_plan(p, plan);
         // 128-byte rows at D = 128: twelve stages keep as many bytes in flight per warp as six stages of bf16 rows
-        const char *cfg = getenv("TFGK_SPMM_FP8_STAGES");
-        const int stages = cfg ? atoi(cfg) : 12;
-        return stages == 6 ? launch_spmm_tma4<6, uint8_t, true>(p, st)
-             : stages == 8 ? launch_spmm_tma4<8, uint8_t, true>(p, st)
-                            : launch_spmm_tma4<12, uint8_t, true>(p, st);
+        return launch_spmm_tma4<12, uint8_t, true>(p, st);
     }
     for (int c0 = 0; c0 < D; c0 += 128) {               // scalar path: 32 lanes x 4 single columns = one group per launch
         SpmmParams p = spmm_params(rowptr, col, w, ldh, n_dst, reduce, alpha, addend, ld_addend, beta, bias, act, out, ldo,

@@ -2,7 +2,7 @@
 """fp8 message rows against bf16 and fp32 at the ogbn-products shape (2 449 029 nodes, 123.7M directed edges + self loops,
 100 features): CUDA-event times of K4 (the GCN projection, and the GAT projection Q | K | V with K | V in each mode), K1
 (weighted, D = 128), K3 (8 heads, A = 128) and the whole GCN(128, relu) + GAT(128, 8 heads, relu) forward, the three
-modes alternating in one run; then the fp8 ring depths of K1 and K3.  Every fp8 output is checked against its contract
+modes alternating in one run.  Every fp8 output is checked against its contract
 first (K4 against the quantised fp32 projection, K1 and K3 bit for bit against the fp32 kernels over the dequantised
 rows).  Bytes over each kernel's byte floor are reported as a share of the 3.35 TB/s data-sheet bandwidth, with the card's
 name and power limit.
@@ -181,21 +181,6 @@ def main():
         row["fp8_over_bf16_speedup"] = round(row["bf16_ms"] / row["fp8_ms"], 4)
         res[k] = row
 
-    # ---- ring depths of the fp8 kernels (medians of `steps` calls each) -------------------------------------------------
-    sweep = {}
-    for var, values, fn in (("TFGK_SPMM_FP8_STAGES", ("6", "8", "12"), fns["K1"]["fp8"]),
-                            ("TFGK_GAT_FP8_STAGES", ("3", "4", "6", "8"), fns["K3"]["fp8"])):
-        prev = os.environ.get(var)
-        for v in values:
-            os.environ[var] = v
-            for _ in range(args.warmup):
-                fn()
-            sweep["{}={}".format(var, v)] = round(float(np.median(timed(fn, args.steps))), 4)
-        if prev is None:
-            del os.environ[var]
-        else:
-            os.environ[var] = prev
-    res["fp8_stage_sweep_ms"] = sweep
     print(json.dumps(res))
 
 

@@ -1,7 +1,7 @@
 # coding=utf-8
 """Packed keys against the dense K | V table for the fused GAT aggregation (K3) at the ogbn-products shape (2 449 029 nodes,
 123.7M directed edges + self loops, 100 features, 8 heads, A = 128): CUDA-event times of K3 dense (gat_tma4_kernel<2>), K3
-packed at ring depths 2, 3 and 4 (gat_tma4_packed_kernel<S>) and the pack kernel, alternating in one run, first with the
+packed (gat_tma4_packed_kernel<2>) and the pack kernel, alternating in one run, first with the
 layer's own keys (ReLU of x W_k, glorot W_k, zero bias) and then with a worst case without zeros (ReLU of x W_k + 10).
 Every packed output is checked bit for bit against the dense one first.  Prints the zero fraction of K, each kernel's byte
 floor (the packed one from the actual copy sizes) and its share of the 3.35 TB/s data-sheet bandwidth, with the card's name
@@ -26,7 +26,6 @@ from tf_geometric_b200 import ops, _structure        # noqa: E402
 from tf_geometric_b200.nn.conv.gat import project    # noqa: E402
 
 HBM = 3.35e12
-STAGES = ("2", "3", "4")
 
 
 def card():
@@ -46,18 +45,16 @@ def timed_once(fn):
 
 
 def run_alternating(variants, steps, warmup):
-    """variants: {name: (setup, fn)}; one launch of each per round, rounds alternate the order; returns {name: [ms]}."""
+    """variants: {name: fn}; one launch of each per round, rounds alternate the order; returns {name: [ms]}."""
     names = list(variants)
     for _ in range(warmup):
         for name in names:
-            variants[name][0]()
-            variants[name][1]()
+            variants[name]()
     torch.cuda.synchronize()
     events = {name: [] for name in names}
     for i in range(steps):
         for name in (names if i % 2 == 0 else names[::-1]):
-            variants[name][0]()
-            events[name].append(timed_once(variants[name][1]))
+            events[name].append(timed_once(variants[name]))
     torch.cuda.synchronize()
     return {name: [a.elapsed_time(b) for a, b in ev] for name, ev in events.items()}
 
@@ -105,12 +102,10 @@ def main():
 
         pack()
         dense()
-        for s in STAGES:
-            os.environ["TFGK_GAT_PACKED_STAGES"] = s
-            out_p.zero_()
-            packed()
-            if not torch.equal(out_p.view(torch.int32), out_d.view(torch.int32)):
-                raise SystemExit("{}: packed K3 (ring depth {}) is not bit-identical to dense K3".format(case, s))
+        out_p.zero_()
+        packed()
+        if not torch.equal(out_p.view(torch.int32), out_d.view(torch.int32)):
+            raise SystemExit("{}: packed K3 is not bit-identical to dense K3".format(case))
         zero_frac = float((K.contiguous().view(torch.int32) == 0).double().mean())
         copy_bytes = float((sizes.long()[col] * 16).sum())
         node_bytes = n * (4 * a + 4 * a + 8)                       # Q and the output once per node, rowptr
@@ -118,12 +113,7 @@ def main():
         floor_packed = copy_bytes + E * (4 + 1) + node_bytes       # the slot bytes copied, col and ksize per edge
         floor_pack = n * 4 * a + float((sizes.long() * 16 - 4 * a).sum()) + n   # read K, write mask + keys, ksize
 
-        def stage(s):
-            return lambda: os.environ.__setitem__("TFGK_GAT_PACKED_STAGES", s)
-        variants = {"k3_dense": (lambda: None, dense), "pack": (lambda: None, pack)}
-        variants.update({"k3_packed_S" + s: (stage(s), packed) for s in STAGES})
-        ms = run_alternating(variants, args.steps, args.warmup)
-        os.environ.pop("TFGK_GAT_PACKED_STAGES", None)
+        ms = run_alternating({"k3_dense": dense, "pack": pack, "k3_packed": packed}, args.steps, args.warmup)
         res = {"case": case, "key_zero_fraction": zero_frac, "avg_packed_copy_bytes_per_edge": copy_bytes / E,
                "floor_bytes": {"k3_dense": floor_dense, "k3_packed": floor_packed, "pack": floor_pack}, "ms": {}}
         for name, v in ms.items():
