@@ -405,6 +405,36 @@ int tfgk_gat_softmax_bwd_f32(const int64_t *rowptr, const int32_t *col, const fl
                              int32_t n_dst, int32_t H, int32_t dv, int split_value_heads,
                              float drop_rate, uint64_t seed, uint32_t rng_stream, float *ds, void *stream);
 
+/* ---- device keys: the three entries above for CUDA-graph capture ------------------------------------------------
+ * A captured graph replays its launches with the arguments they were captured with, so a key passed by value would draw
+ * the same mask on every replay.  The _devkey entries take (key_base, slot) in place of `seed`: key_base points at one
+ * uint64 in device memory, the base, and the kernel uses
+ *     key = splitmix64(*key_base + 0x9E3779B97F4A7C15 * (slot + 1))
+ * with splitmix64(z) = z ^= z >> 30, z *= 0xBF58476D1CE4E5B9, z ^= z >> 27, z *= 0x94D049BB133111EB, z ^ (z >> 31)
+ * (the output function only; the Weyl step is the + above).  That is the host key sequence of tf_geometric_b200/_rng.py:
+ * its (slot + 1)-th key after set_seed(base) is the key of `slot` here, so a captured run can be repeated eagerly.
+ * Every other argument, and the mask as a function of (key, rng_stream, element), is that of the entry with a seed.
+ * Epochs: tfgk_rng_advance replaces the base by splitmix64(base) on `stream` and, when `epoch` is not NULL, copies the new
+ * base into *epoch.  The host enqueues it once per captured region, before its first keyed launch (slot 0), with an
+ * epoch word of that region's own, and the region's launches take that word as key_base.  Every replay then draws new
+ * masks, and a backward that regenerates a forward's masks reads the value its forward read, even when other graphs that
+ * draw keys replay in between (make_graphed_callables over several modules replays every forward before any backward).
+ * A graph that draws no key (a backward captured on its own) neither advances the base nor owns a word.
+ * tfgk_capture_id: *id = the capture sequence id of `stream` (cudaStreamGetCaptureInfo), 0 when it is not capturing. */
+int tfgk_dropout_devkey_f32(const float *x, int64_t n, float rate, const uint64_t *key_base, uint64_t slot,
+                            uint32_t rng_stream, float *out, void *stream);
+int tfgk_spmm_heads_devkey_f32(const int64_t *rowptr, const int32_t *col, const int32_t *emap, const float *w,
+                               const float *src, int64_t lds, int32_t n_dst, int32_t H, int32_t dh, int mode,
+                               float drop_rate, const uint64_t *key_base, uint64_t slot, uint32_t rng_stream, float alpha,
+                               const float *bias, int act, float *out, int64_t ldo, void *stream);
+int tfgk_gat_softmax_bwd_devkey_f32(const int64_t *rowptr, const int32_t *col, const float *att,
+                                    const float *G, int64_t ldg, const float *V, int64_t ldv,
+                                    int32_t n_dst, int32_t H, int32_t dv, int split_value_heads,
+                                    float drop_rate, const uint64_t *key_base, uint64_t slot, uint32_t rng_stream,
+                                    float *ds, void *stream);
+int tfgk_rng_advance(uint64_t *key_base, uint64_t *epoch, void *stream);
+int tfgk_capture_id(void *stream, uint64_t *id);
+
 /* Training without the [E, H] coefficient table (round 2).  The forward pass is the same streaming kernel as
  * tfgk_gat_fused_f32 (heads concatenated, dqk == dv, H * dqk <= 128) and additionally keeps stats[N, 2H]: per (row, head)
  * the softmax maximum and the denominator (+1e-8).  The backward pass recomputes every coefficient from Q, K and stats:

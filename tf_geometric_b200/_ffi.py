@@ -95,6 +95,13 @@ SIGNATURES = {
                             _int, _ptr, _i64, _ptr],
     "tfgk_gat_softmax_bwd_f32": [_ptr, _ptr, _ptr, _ptr, _i64, _ptr, _i64, _i32, _i32, _i32, _int, _f32, _u64, _u32,
                                  _ptr, _ptr],
+    "tfgk_dropout_devkey_f32": [_ptr, _i64, _f32, _ptr, _u64, _u32, _ptr, _ptr],
+    "tfgk_spmm_heads_devkey_f32": [_ptr, _ptr, _ptr, _ptr, _ptr, _i64, _i32, _i32, _i32, _int, _f32, _ptr, _u64, _u32, _f32,
+                                   _ptr, _int, _ptr, _i64, _ptr],
+    "tfgk_gat_softmax_bwd_devkey_f32": [_ptr, _ptr, _ptr, _ptr, _i64, _ptr, _i64, _i32, _i32, _i32, _int, _f32, _ptr, _u64,
+                                        _u32, _ptr, _ptr],
+    "tfgk_rng_advance": [_ptr, _ptr, _ptr],
+    "tfgk_capture_id": [_ptr, ctypes.POINTER(_u64)],
     "tfgk_gat_fused_stats_f32": [_ptr, _ptr, _ptr, _i64, _ptr, _i64, _ptr, _i64, _i32, _i32, _i32, _i32, _f32, _ptr, _int,
                                  _ptr, _i64, _ptr, _ptr, _ptr],
     "tfgk_gat_bwd_prepare_f32": [_ptr, _i64, _ptr, _i64, _ptr, _int, _ptr, _i32, _i32, _i32, _ptr, _i64, _ptr],
@@ -230,7 +237,46 @@ def set_trace(trace):
     return prev
 
 
+# Entries that cannot be recorded in a CUDA graph, with the op that reaches them and why: they read a result back on the
+# host (a size, a count, an id check), or they take a host-side random key that a graph would replay unchanged.
+NOT_CAPTURABLE = {
+    "tfgk_csr_build": ("the CSR build of an edge list without a cached structure", "it checks the node ids on the host"),
+    "tfgk_plan_build": ("the work-plan build of a CSR", "it returns the task counts to the host"),
+    "tfgk_edge_unique": ("the edge merge", "it returns the number of unique edges to the host"),
+    "tfgk_directed_edges": ("the undirected-to-directed edge conversion", "it returns the edge count to the host"),
+    "tfgk_edge_flags_i32": ("edge filtering (drop_edge, the edge samplers, convert_edge_to_upper)", "its flags are "
+                            "compacted by select_flagged, which returns the number of kept edges to the host"),
+    "tfgk_select_flagged_i32": ("select_flagged", "it returns the number of selected entries to the host"),
+    "tfgk_neighbor_sample_count": ("the neighbour sampler", "it returns the number of sampled edges to the host"),
+    "tfgk_neighbor_sample_fill": ("the neighbour sampler", "it takes a host-side key"),
+    "tfgk_neg_offsets": ("negative sampling", "it returns the number of candidate pairs to the host"),
+    "tfgk_neg_draw": ("negative sampling", "it takes a host-side key"),
+    "tfgk_neg_sample_start": ("negative sampling", "it takes a host-side key"),
+    "tfgk_random_pairs_i32": ("negative sampling", "it takes a host-side key"),
+    "tfgk_spgemm_plan": ("SparseMatrix @ SparseMatrix (K10's plan)", "it returns the product counts to the host"),
+    "tfgk_spgemm_rowptr": ("SparseMatrix @ SparseMatrix (K10's row pointers)", "it returns the number of entries to the host"),
+    "tfgk_spgemm_grad_plan": ("the SparseMatrix @ SparseMatrix gradient (K12's plan)", "it returns the slice count to the "
+                              "host"),
+}
+
+
+def capturing():
+    """Whether the current CUDA stream is recording a graph (torch.cuda.graph, make_graphed_callables)."""
+    import torch
+    return torch.cuda.is_initialized() and torch.cuda.is_current_stream_capturing()
+
+
+def refuse_capture(op, reason):
+    """Raise before any device work when `op` is called while the current stream records a CUDA graph."""
+    if capturing():
+        raise RuntimeError("{} cannot be captured in a CUDA graph: {}. Run it eagerly, outside the capture (a warm-up "
+                           "step builds and caches the structures a captured step needs).".format(op, reason))
+
+
 def call(name, *args):
+    refusal = NOT_CAPTURABLE.get(name)
+    if refusal is not None:
+        refuse_capture(*refusal)
     handle = lib()
     trace = _trace
     if trace is None:

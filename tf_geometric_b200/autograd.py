@@ -281,7 +281,8 @@ class GatAttention(torch.autograd.Function):
       backward: G = dy * act'(y);  ds = tfgk_gat_softmax_bwd_f32(att, G, V);
                 dQ = sum_e ds K[col] / scale                       forward CSR
                 dK = sum_e ds Q[row] / scale,  dV = sum_e a' G[row] transposed CSR
-    The mask is regenerated from (seed, edge, head) in every kernel, never stored."""
+    The mask is regenerated from (seed, edge, head) in every kernel, never stored; `seed` is a host key or an
+    _rng.DeviceKey, which the backward reuses as it is, so under CUDA-graph capture it reads the base its forward read."""
 
     @staticmethod
     def forward(ctx, Q, K, V, bias, csr, edge_index_used, num_heads, split, act_code, drop_rate, seed, scale=None):
@@ -354,7 +355,7 @@ class Dropout(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, x, rate, seed):
-        ctx.rate, ctx.seed = float(rate), int(seed)
+        ctx.rate, ctx.seed = float(rate), seed          # a host key or an _rng.DeviceKey
         return ops.dropout(x.detach().contiguous(), ctx.rate, ctx.seed)
 
     @staticmethod
@@ -367,7 +368,7 @@ def dropout(x, rate, training, seed=None):
     if not training or rate <= 0.0:
         return x
     from . import _rng
-    return Dropout.apply(x, float(rate), _rng.resolve(seed))
+    return Dropout.apply(x, float(rate), _rng.resolve(seed, x.device))
 
 
 def dense(x, weight, bias=None, activation=None):

@@ -66,4 +66,17 @@ __host__ __device__ __forceinline__ uint64_t random_below64(uint64_t seed, uint3
 #endif
 }
 
+// splitmix64's output function (Steele, Lea and Flood, "Fast splittable pseudorandom number generators", OOPSLA'14):
+// the same mix as tf_geometric_b200/_rng.py applies to its keys
+__host__ __device__ __forceinline__ uint64_t splitmix64(uint64_t z) {
+    z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
+    z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
+    return z ^ (z >> 31);
+}
+
+// key of draw `slot` of a captured region whose device-resident base is `base` (include/tfgk.h, "device keys")
+__host__ __device__ __forceinline__ uint64_t device_key(uint64_t base, uint64_t slot) {
+    return splitmix64(base + 0x9E3779B97F4A7C15ull * (slot + 1));
+}
+
 }  // namespace tfgk

@@ -23,10 +23,20 @@ __device__ __forceinline__ float keep_scale(float rate, float scale, uint64_t se
     return random_uniform(seed, stream, idx) >= rate ? scale : 0.0f;
 }
 
-__global__ void dropout_kernel(const float *__restrict__ x, int64_t n, float rate, float scale, uint64_t seed,
-                               uint32_t stream, float *__restrict__ out) {
+// The key of a launch: `seed` itself, or (DEVKEY, CUDA-graph capture) the device key of draw `slot` whose base is read
+// from device memory when the kernel runs.  A template flag, so that the kernels taking a host key compile as they did.
+template <bool DEVKEY>
+__device__ __forceinline__ uint64_t launch_key(uint64_t seed, const uint64_t *key_base, uint64_t slot) {
+    return DEVKEY ? device_key(*key_base, slot) : seed;
+}
+
+template <bool DEVKEY>
+__global__ void dropout_kernel(const float *__restrict__ x, int64_t n, float rate, float scale, uint64_t seed_,
+                               uint32_t stream, float *__restrict__ out, const uint64_t *__restrict__ key_base,
+                               uint64_t slot) {
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
+    const uint64_t seed = launch_key<DEVKEY>(seed_, key_base, slot);
     const float v = x ? x[i] : 1.0f;
     const float k = keep_scale(rate, scale, seed, stream, (uint64_t)i);
     out[i] = k == 0.0f ? 0.0f : __fmul_rn(v, k);
@@ -49,31 +59,35 @@ struct HeadsParams {
     int act;
     float *out;
     int64_t ldo;
+    const uint64_t *key_base;    // the DEVKEY instantiations: the key is device_key(*key_base, slot), not seed
+    uint64_t slot;
 };
 
 template <bool DROP = true>
-__device__ __forceinline__ float head_weight(const HeadsParams &p, int64_t e, int h) {
+__device__ __forceinline__ float head_weight(const HeadsParams &p, uint64_t seed, int64_t e, int h) {
     const int64_t pos = p.emap ? (int64_t)p.emap[e] : e;
     const float w = p.w[pos * p.H + h];
     if (!DROP) return w;                             // compiled without the generator: fewer registers, more warps
-    const float k = keep_scale(p.rate, p.scale, p.seed, p.stream, (uint64_t)(pos * p.H + h));
+    const float k = keep_scale(p.rate, p.scale, seed, p.stream, (uint64_t)(pos * p.H + h));
     return k == 0.0f ? 0.0f : (p.rate > 0.0f ? __fmul_rn(w, k) : w);
 }
 
 // generic shape: one warp per destination row, lanes over output columns
+template <bool DEVKEY>
 __global__ void __launch_bounds__(kTrainThreads) spmm_heads_kernel(const HeadsParams p) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int64_t r = (int64_t)blockIdx.x * kTrainWarps + warp;
     if (r >= p.N) return;
     const int64_t e0 = p.rowptr[r], e1 = p.rowptr[r + 1];
     const int H = p.H, dh = p.dh;
+    const uint64_t seed = launch_key<DEVKEY>(p.seed, p.key_base, p.slot);
     if (p.mode == TFGK_HEADS_REDUCE) {
         for (int u = lane; u < dh; u += 32) {
             float tot = 0.0f;
             for (int h = 0; h < H; ++h) {
                 float acc = 0.0f;
                 for (int64_t e = e0; e < e1; ++e)
-                    acc = __fadd_rn(acc, __fmul_rn(p.src[(int64_t)p.col[e] * p.lds + (int64_t)h * dh + u], head_weight(p, e, h)));
+                    acc = __fadd_rn(acc, __fmul_rn(p.src[(int64_t)p.col[e] * p.lds + (int64_t)h * dh + u], head_weight(p, seed, e, h)));
                 tot = h == 0 ? acc : __fadd_rn(tot, acc);
             }
             float v = __fmul_rn(tot, p.alpha);
@@ -88,7 +102,7 @@ __global__ void __launch_bounds__(kTrainThreads) spmm_heads_kernel(const HeadsPa
         const int sc = p.mode == TFGK_HEADS_BROADCAST ? c - h * dh : c;
         float acc = 0.0f;
         for (int64_t e = e0; e < e1; ++e)
-            acc = __fadd_rn(acc, __fmul_rn(p.src[(int64_t)p.col[e] * p.lds + sc], head_weight(p, e, h)));
+            acc = __fadd_rn(acc, __fmul_rn(p.src[(int64_t)p.col[e] * p.lds + sc], head_weight(p, seed, e, h)));
         float v = __fmul_rn(acc, p.alpha);
         if (p.bias) v += p.bias[c];
         p.out[r * p.ldo + c] = apply_act(v, p.act);
@@ -97,13 +111,14 @@ __global__ void __launch_bounds__(kTrainThreads) spmm_heads_kernel(const HeadsPa
 
 // H*dh == 128, split layout, 16-byte aligned rows: every lane owns one float4 of the output row and the head it
 // belongs to; U edges in flight per iteration
-template <int U, bool DROP>
+template <int U, bool DROP, bool DEVKEY>
 __global__ void __launch_bounds__(kTrainThreads) spmm_heads128_kernel(const HeadsParams p) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int64_t r = (int64_t)blockIdx.x * kTrainWarps + warp;
     if (r >= p.N) return;
     const int64_t e0 = p.rowptr[r], e1 = p.rowptr[r + 1];
     const int h = (lane * 4) / p.dh;
+    const uint64_t seed = DROP ? launch_key<DEVKEY>(p.seed, p.key_base, p.slot) : 0;
     float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
     int64_t e = e0;
     for (; e + U <= e1; e += U) {
@@ -112,7 +127,7 @@ __global__ void __launch_bounds__(kTrainThreads) spmm_heads128_kernel(const Head
 #pragma unroll
         for (int i = 0; i < U; ++i) {
             v[i] = *reinterpret_cast<const float4 *>(p.src + (int64_t)p.col[e + i] * p.lds + lane * 4);
-            w[i] = head_weight<DROP>(p, e + i, h);
+            w[i] = head_weight<DROP>(p, seed, e + i, h);
         }
 #pragma unroll
         for (int i = 0; i < U; ++i) {
@@ -124,7 +139,7 @@ __global__ void __launch_bounds__(kTrainThreads) spmm_heads128_kernel(const Head
     }
     for (; e < e1; ++e) {
         const float4 v = *reinterpret_cast<const float4 *>(p.src + (int64_t)p.col[e] * p.lds + lane * 4);
-        const float w = head_weight<DROP>(p, e, h);
+        const float w = head_weight<DROP>(p, seed, e, h);
         acc.x = __fadd_rn(acc.x, __fmul_rn(v.x, w));
         acc.y = __fadd_rn(acc.y, __fmul_rn(v.y, w));
         acc.z = __fadd_rn(acc.z, __fmul_rn(v.z, w));
@@ -155,9 +170,12 @@ struct GatBwdParams {
     uint64_t seed;
     uint32_t stream;
     float *ds;               // [E, H] out: gradient w.r.t. the raw (already scaled) scores
+    const uint64_t *key_base;    // the DEVKEY instantiations: the key is device_key(*key_base, slot), not seed
+    uint64_t slot;
 };
 
 // one warp per destination row; sweep 1: da = <G_r, V_col> per edge and head, delta = sum a*da; sweep 2: ds = a (da - delta)
+template <bool DEVKEY>
 __global__ void __launch_bounds__(kTrainThreads) gat_softmax_bwd_kernel(const GatBwdParams p) {
     extern __shared__ float smem[];   // [warps][H]
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -172,6 +190,7 @@ __global__ void __launch_bounds__(kTrainThreads) gat_softmax_bwd_kernel(const Ga
     const int32_t *col = p.col + start;
     const float *grow = p.G + r * p.ldg;
     const float inv_h = 1.0f / (float)H;
+    const uint64_t seed = launch_key<DEVKEY>(p.seed, p.key_base, p.slot);
 
     for (int h = lane; h < H; h += 32) delta[h] = 0.0f;
     __syncwarp();
@@ -188,7 +207,7 @@ __global__ void __launch_bounds__(kTrainThreads) gat_softmax_bwd_kernel(const Ga
             if (lane == 0) {
                 if (!p.split) d *= inv_h;
                 const int64_t idx = (int64_t)e * H + h;
-                d *= keep_scale(p.rate, p.scale, p.seed, p.stream, (uint64_t)((start + e) * H + h));
+                d *= keep_scale(p.rate, p.scale, seed, p.stream, (uint64_t)((start + e) * H + h));
                 ds[idx] = d;
                 delta[h] += att[idx] * d;
             }
@@ -200,7 +219,7 @@ __global__ void __launch_bounds__(kTrainThreads) gat_softmax_bwd_kernel(const Ga
 
 // split layout with H*dv == 128 (dv a multiple of 4 dividing 128): lane owns one float4; the dot products of all heads
 // are reduced at once inside groups of dv/4 lanes
-template <int U, int MINB, bool DROP>
+template <int U, int MINB, bool DROP, bool DEVKEY>
 __global__ void __launch_bounds__(kTrainThreads, MINB) gat_softmax_bwd128_kernel(const GatBwdParams p) {
     extern __shared__ float smem[];   // [warps][H]
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -217,12 +236,13 @@ __global__ void __launch_bounds__(kTrainThreads, MINB) gat_softmax_bwd128_kernel
     float *ds = p.ds + start * H;
     const int32_t *col = p.col + start;
     const float4 g = *reinterpret_cast<const float4 *>(p.G + r * p.ldg + lane * 4);
+    const uint64_t seed = DROP ? launch_key<DEVKEY>(p.seed, p.key_base, p.slot) : 0;
     float dacc = 0.0f;
     auto finish = [&](float d, int e) {
         for (int off = group >> 1; off > 0; off >>= 1) d += __shfl_xor_sync(0xffffffffu, d, off);
         if (leader) {
             const int64_t idx = (int64_t)e * H + h;
-            if (DROP) d *= keep_scale(p.rate, p.scale, p.seed, p.stream, (uint64_t)((start + e) * H + h));
+            if (DROP) d *= keep_scale(p.rate, p.scale, seed, p.stream, (uint64_t)((start + e) * H + h));
             ds[idx] = d;
             dacc += att[idx] * d;
         }
@@ -246,28 +266,26 @@ __global__ void __launch_bounds__(kTrainThreads, MINB) gat_softmax_bwd128_kernel
 
 inline bool pow2(int x) { return x > 0 && (x & (x - 1)) == 0; }
 
-}  // namespace
-}  // namespace tfgk
 
-using namespace tfgk;
 
-extern "C" {
-
-int tfgk_dropout_f32(const float *x, int64_t n, float rate, uint64_t seed, uint32_t rng_stream, float *out, void *stream) {
+int dropout_f32(const float *x, int64_t n, float rate, uint64_t seed, const uint64_t *key_base, uint64_t slot,
+                uint32_t rng_stream, float *out, void *stream) {
     TFGK_CHECK_ARG(n >= 0, "dropout: negative size");
     TFGK_CHECK_ARG(rate >= 0.0f && rate < 1.0f, "dropout: rate %g outside [0, 1)", (double)rate);
     if (n == 0) return TFGK_OK;
     TFGK_CHECK_ARG(out != nullptr, "dropout: null output");
     const float scale = 1.0f / (1.0f - rate);
-    dropout_kernel<<<(unsigned)ceil_div64(n, 256), 256, 0, as_stream(stream)>>>(x, n, rate, scale, seed, rng_stream, out);
+    const unsigned blocks = (unsigned)ceil_div64(n, 256);
+    if (key_base) dropout_kernel<true><<<blocks, 256, 0, as_stream(stream)>>>(x, n, rate, scale, seed, rng_stream, out, key_base, slot);
+    else dropout_kernel<false><<<blocks, 256, 0, as_stream(stream)>>>(x, n, rate, scale, seed, rng_stream, out, key_base, slot);
     TFGK_LAUNCH_CHECK();
     return TFGK_OK;
 }
 
-int tfgk_spmm_heads_f32(const int64_t *rowptr, const int32_t *col, const int32_t *emap, const float *w,
-                        const float *src, int64_t lds, int32_t n_dst, int32_t H, int32_t dh, int mode,
-                        float drop_rate, uint64_t seed, uint32_t rng_stream, float alpha,
-                        const float *bias, int act, float *out, int64_t ldo, void *stream) {
+int spmm_heads_f32(const int64_t *rowptr, const int32_t *col, const int32_t *emap, const float *w,
+                   const float *src, int64_t lds, int32_t n_dst, int32_t H, int32_t dh, int mode,
+                   float drop_rate, uint64_t seed, const uint64_t *key_base, uint64_t slot, uint32_t rng_stream,
+                   float alpha, const float *bias, int act, float *out, int64_t ldo, void *stream) {
     TFGK_CHECK_ARG(n_dst >= 0 && H >= 1 && dh >= 1, "spmm_heads: bad size (n_dst=%d H=%d dh=%d)", n_dst, H, dh);
     TFGK_CHECK_ARG(mode == TFGK_HEADS_SPLIT || mode == TFGK_HEADS_BROADCAST || mode == TFGK_HEADS_REDUCE,
                    "spmm_heads: unknown mode %d", mode);
@@ -281,24 +299,26 @@ int tfgk_spmm_heads_f32(const int64_t *rowptr, const int32_t *col, const int32_t
     HeadsParams p;
     p.rowptr = rowptr; p.col = col; p.emap = emap; p.w = w; p.src = src; p.lds = lds;
     p.N = n_dst; p.H = H; p.dh = dh; p.mode = mode;
-    p.rate = drop_rate; p.scale = 1.0f / (1.0f - drop_rate); p.seed = seed; p.stream = rng_stream;
-    p.alpha = alpha; p.bias = bias; p.act = act; p.out = out; p.ldo = ldo;
+    p.rate = drop_rate; p.scale = 1.0f / (1.0f - drop_rate); p.seed = seed; p.key_base = key_base; p.slot = slot;
+    p.stream = rng_stream; p.alpha = alpha; p.bias = bias; p.act = act; p.out = out; p.ldo = ldo;
     const unsigned blocks = (unsigned)ceil_div64(n_dst, kTrainWarps);
     const bool fast = mode == TFGK_HEADS_SPLIT && (int64_t)H * dh == 128 && dh % 4 == 0 && aligned16(src) && aligned16(out) &&
                       lds % 4 == 0 && ldo % 4 == 0 && (!bias || aligned16(bias));
-    if (fast) {
-        if (drop_rate > 0.0f) spmm_heads128_kernel<4, true><<<blocks, kTrainThreads, 0, as_stream(stream)>>>(p);
-        else spmm_heads128_kernel<4, false><<<blocks, kTrainThreads, 0, as_stream(stream)>>>(p);
-    } else
-        spmm_heads_kernel<<<blocks, kTrainThreads, 0, as_stream(stream)>>>(p);
+    const cudaStream_t st = as_stream(stream);
+    if (fast && drop_rate > 0.0f && key_base) spmm_heads128_kernel<4, true, true><<<blocks, kTrainThreads, 0, st>>>(p);
+    else if (fast && drop_rate > 0.0f) spmm_heads128_kernel<4, true, false><<<blocks, kTrainThreads, 0, st>>>(p);
+    else if (fast) spmm_heads128_kernel<4, false, false><<<blocks, kTrainThreads, 0, st>>>(p);
+    else if (key_base) spmm_heads_kernel<true><<<blocks, kTrainThreads, 0, st>>>(p);
+    else spmm_heads_kernel<false><<<blocks, kTrainThreads, 0, st>>>(p);
     TFGK_LAUNCH_CHECK();
     return TFGK_OK;
 }
 
-int tfgk_gat_softmax_bwd_f32(const int64_t *rowptr, const int32_t *col, const float *att,
-                             const float *G, int64_t ldg, const float *V, int64_t ldv,
-                             int32_t n_dst, int32_t H, int32_t dv, int split_value_heads,
-                             float drop_rate, uint64_t seed, uint32_t rng_stream, float *ds, void *stream) {
+int gat_softmax_bwd_f32(const int64_t *rowptr, const int32_t *col, const float *att,
+                        const float *G, int64_t ldg, const float *V, int64_t ldv,
+                        int32_t n_dst, int32_t H, int32_t dv, int split_value_heads,
+                        float drop_rate, uint64_t seed, const uint64_t *key_base, uint64_t slot, uint32_t rng_stream,
+                        float *ds, void *stream) {
     TFGK_CHECK_ARG(n_dst >= 0 && H >= 1 && dv >= 1, "gat_softmax_bwd: bad size (n_dst=%d H=%d dv=%d)", n_dst, H, dv);
     TFGK_CHECK_ARG(drop_rate >= 0.0f && drop_rate < 1.0f, "gat_softmax_bwd: drop rate %g outside [0, 1)", (double)drop_rate);
     if (n_dst == 0) return TFGK_OK;
@@ -308,18 +328,95 @@ int tfgk_gat_softmax_bwd_f32(const int64_t *rowptr, const int32_t *col, const fl
     GatBwdParams p;
     p.rowptr = rowptr; p.col = col; p.att = att; p.G = G; p.ldg = ldg; p.V = V; p.ldv = ldv;
     p.N = n_dst; p.H = H; p.dv = dv; p.split = split_value_heads ? 1 : 0;
-    p.rate = drop_rate; p.scale = 1.0f / (1.0f - drop_rate); p.seed = seed; p.stream = rng_stream; p.ds = ds;
+    p.rate = drop_rate; p.scale = 1.0f / (1.0f - drop_rate); p.seed = seed; p.key_base = key_base; p.slot = slot;
+    p.stream = rng_stream; p.ds = ds;
     const unsigned blocks = (unsigned)ceil_div64(n_dst, kTrainWarps);
     const size_t smem = (size_t)kTrainWarps * H * sizeof(float);
     TFGK_CHECK_ARG(smem <= 48 * 1024, "gat_softmax_bwd: too many heads (%d)", H);
     const bool fast = p.split && (int64_t)H * dv == 128 && dv % 4 == 0 && pow2(dv >> 2) && aligned16(G) && aligned16(V) &&
                       ldg % 4 == 0 && ldv % 4 == 0;
-    if (fast) {
-        if (drop_rate > 0.0f) gat_softmax_bwd128_kernel<4, 4, true><<<blocks, kTrainThreads, smem, as_stream(stream)>>>(p);
-        else gat_softmax_bwd128_kernel<4, 4, false><<<blocks, kTrainThreads, smem, as_stream(stream)>>>(p);
-    } else
-        gat_softmax_bwd_kernel<<<blocks, kTrainThreads, smem, as_stream(stream)>>>(p);
+    const cudaStream_t st = as_stream(stream);
+    if (fast && drop_rate > 0.0f && key_base) gat_softmax_bwd128_kernel<4, 4, true, true><<<blocks, kTrainThreads, smem, st>>>(p);
+    else if (fast && drop_rate > 0.0f) gat_softmax_bwd128_kernel<4, 4, true, false><<<blocks, kTrainThreads, smem, st>>>(p);
+    else if (fast) gat_softmax_bwd128_kernel<4, 4, false, false><<<blocks, kTrainThreads, smem, st>>>(p);
+    else if (key_base) gat_softmax_bwd_kernel<true><<<blocks, kTrainThreads, smem, st>>>(p);
+    else gat_softmax_bwd_kernel<false><<<blocks, kTrainThreads, smem, st>>>(p);
     TFGK_LAUNCH_CHECK();
+    return TFGK_OK;
+}
+
+__global__ void rng_advance_kernel(uint64_t *key_base, uint64_t *epoch) {
+    const uint64_t b = splitmix64(*key_base);
+    *key_base = b;
+    if (epoch) *epoch = b;
+}
+
+}  // namespace
+}  // namespace tfgk
+
+using namespace tfgk;
+
+extern "C" {
+
+int tfgk_dropout_f32(const float *x, int64_t n, float rate, uint64_t seed, uint32_t rng_stream, float *out, void *stream) {
+    return dropout_f32(x, n, rate, seed, nullptr, 0, rng_stream, out, stream);
+}
+
+int tfgk_dropout_devkey_f32(const float *x, int64_t n, float rate, const uint64_t *key_base, uint64_t slot,
+                            uint32_t rng_stream, float *out, void *stream) {
+    TFGK_CHECK_ARG(key_base != nullptr, "dropout_devkey: null key_base");
+    return dropout_f32(x, n, rate, 0, key_base, slot, rng_stream, out, stream);
+}
+
+int tfgk_spmm_heads_f32(const int64_t *rowptr, const int32_t *col, const int32_t *emap, const float *w,
+                        const float *src, int64_t lds, int32_t n_dst, int32_t H, int32_t dh, int mode,
+                        float drop_rate, uint64_t seed, uint32_t rng_stream, float alpha,
+                        const float *bias, int act, float *out, int64_t ldo, void *stream) {
+    return spmm_heads_f32(rowptr, col, emap, w, src, lds, n_dst, H, dh, mode, drop_rate, seed, nullptr, 0, rng_stream,
+                          alpha, bias, act, out, ldo, stream);
+}
+
+int tfgk_spmm_heads_devkey_f32(const int64_t *rowptr, const int32_t *col, const int32_t *emap, const float *w,
+                               const float *src, int64_t lds, int32_t n_dst, int32_t H, int32_t dh, int mode,
+                               float drop_rate, const uint64_t *key_base, uint64_t slot, uint32_t rng_stream, float alpha,
+                               const float *bias, int act, float *out, int64_t ldo, void *stream) {
+    TFGK_CHECK_ARG(key_base != nullptr, "spmm_heads_devkey: null key_base");
+    return spmm_heads_f32(rowptr, col, emap, w, src, lds, n_dst, H, dh, mode, drop_rate, 0, key_base, slot, rng_stream,
+                          alpha, bias, act, out, ldo, stream);
+}
+
+int tfgk_gat_softmax_bwd_f32(const int64_t *rowptr, const int32_t *col, const float *att,
+                             const float *G, int64_t ldg, const float *V, int64_t ldv,
+                             int32_t n_dst, int32_t H, int32_t dv, int split_value_heads,
+                             float drop_rate, uint64_t seed, uint32_t rng_stream, float *ds, void *stream) {
+    return gat_softmax_bwd_f32(rowptr, col, att, G, ldg, V, ldv, n_dst, H, dv, split_value_heads, drop_rate, seed, nullptr,
+                               0, rng_stream, ds, stream);
+}
+
+int tfgk_gat_softmax_bwd_devkey_f32(const int64_t *rowptr, const int32_t *col, const float *att,
+                                    const float *G, int64_t ldg, const float *V, int64_t ldv,
+                                    int32_t n_dst, int32_t H, int32_t dv, int split_value_heads,
+                                    float drop_rate, const uint64_t *key_base, uint64_t slot, uint32_t rng_stream,
+                                    float *ds, void *stream) {
+    TFGK_CHECK_ARG(key_base != nullptr, "gat_softmax_bwd_devkey: null key_base");
+    return gat_softmax_bwd_f32(rowptr, col, att, G, ldg, V, ldv, n_dst, H, dv, split_value_heads, drop_rate, 0, key_base,
+                               slot, rng_stream, ds, stream);
+}
+
+int tfgk_rng_advance(uint64_t *key_base, uint64_t *epoch, void *stream) {
+    TFGK_CHECK_ARG(key_base != nullptr, "rng_advance: null key_base");
+    rng_advance_kernel<<<1, 1, 0, as_stream(stream)>>>(key_base, epoch);
+    TFGK_LAUNCH_CHECK();
+    return TFGK_OK;
+}
+
+int tfgk_capture_id(void *stream, uint64_t *id) {
+    TFGK_CHECK_ARG(id != nullptr, "capture_id: null output");
+    *id = 0;
+    cudaStreamCaptureStatus status = cudaStreamCaptureStatusNone;
+    unsigned long long cid = 0;
+    TFGK_CUDA(cudaStreamGetCaptureInfo(as_stream(stream), &status, &cid));
+    if (status == cudaStreamCaptureStatusActive) *id = (uint64_t)cid;
     return TFGK_OK;
 }
 

@@ -75,7 +75,7 @@ def gat(x, edge_index,
                 raise NotImplementedError("return_attention is an inference-path extension")
             return _gat_training(x_sparse, csr, edge_index_used, query_kernel, query_bias, query_activation, key_kernel,
                                  key_bias, key_activation, kernel, bias, activation, num_heads, split_value_heads, drop_rate,
-                                 _rng.resolve(seed) if drop_rate > 0.0 else 0)
+                                 _rng.resolve(seed, dev) if drop_rate > 0.0 else 0)
         q_act, q_left = ops.activation_code(query_activation)
         k_act, k_left = ops.activation_code(key_activation)
         f32 = lambda t: None if t is None else ops.as_device(t, torch.float32, device=dev)     # noqa: E731
@@ -97,7 +97,7 @@ def gat(x, edge_index,
             raise NotImplementedError("return_attention is an inference-path extension")
         return _gat_training(x, csr, edge_index_used, query_kernel, query_bias, query_activation, key_kernel, key_bias,
                              key_activation, kernel, bias, activation, num_heads, split_value_heads, drop_rate,
-                             _rng.resolve(seed) if drop_rate > 0.0 else 0)
+                             _rng.resolve(seed, dev) if drop_rate > 0.0 else 0)
 
     q_act, q_left = ops.activation_code(query_activation)
     k_act, k_left = ops.activation_code(key_activation)

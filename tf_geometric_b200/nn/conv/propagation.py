@@ -4,7 +4,7 @@ Each one is the K1 kernel (tfgk_spmm_f32) in a loop with the per-layer arithmeti
 reference's rounding order allows it; signatures follow tf_geometric/nn/conv/{sgc,ssgc,tagcn,gin,le_conv}.py."""
 import torch
 
-from ... import ops, _structure, autograd
+from ... import ops, _structure, autograd, _ffi
 from ...sparse import SparseMatrix
 from . import _bf16
 from .gat import project
@@ -233,6 +233,7 @@ def get_laplacian(edge_index, num_nodes, edge_weight, normalization_type, fill_w
 def laplacian_max_eigenvalue(edge_index, num_nodes, edge_weight, normalization_type='sym', is_undirected=True):
     """LaplacianMaxEigenvalue(...)(normalization_type): host-side scipy eigs/eigsh, as in the reference (:884-911, including
     its quirk of building the operator from the edges WITH self loops while the weights had them removed)."""
+    _ffi.refuse_capture("the dynamic lambda_max of ChebyNet", "scipy computes it on the host")
     import numpy as np
     import scipy.sparse
     from scipy.sparse.linalg import eigs, eigsh

@@ -7,7 +7,7 @@ order inside every source), then the deterministic "first node_k entries of each
 Ties keep their input order (the reference's tf.argsort leaves the order of equal scores unspecified)."""
 import torch
 
-from ... import ops
+from ... import ops, _ffi
 
 
 def topk_pool(source_index, score, k=None, ratio=None):
@@ -18,6 +18,7 @@ def topk_pool(source_index, score, k=None, ratio=None):
     :param ratio: keep ceil(num_targets * ratio) targets of every source
     :return: int32 [num_selected] indices into the inputs, grouped by ascending source, best score first
     """
+    _ffi.refuse_capture("topk_pool", "it reads the number of sources and the selection size on the host")
     if k is None and ratio is None:
         raise Exception("you should provide either k or ratio for topk_pool")
     elif k is not None and ratio is not None:

@@ -40,7 +40,7 @@ def drop_edge(inputs, rate=0.5, force_undirected=False, training=None, seed=None
     dev = ei.device
     row, col = ei[0].contiguous(), ei[1].contiguous()
     flag = ops.edge_flags(row, col, row.numel(), mode=ops.FLAG_UPPER if force_undirected else ops.FLAG_ALL,
-                          bernoulli=ops.BERNOULLI_DROPOUT, prob=float(rate), seed=_rng.resolve(seed))
+                          bernoulli=ops.BERNOULLI_DROPOUT, prob=float(rate), seed=_rng.resolve_host(seed))
     index = ops.select_flagged(flag)
     dropped = torch.stack([ops.gather_i32(row, index), ops.gather_i32(col, index)])
     if force_undirected:

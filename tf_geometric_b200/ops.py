@@ -9,7 +9,7 @@ import ctypes
 import numpy as np
 import torch
 
-from . import _ffi
+from . import _ffi, _rng
 from ._ffi import (REDUCE_SUM, REDUCE_MEAN, REDUCE_MAX, ACT_NONE, ACT_RELU, POW_INV_SQRT, POW_INV,  # noqa: F401
                    HEADS_SPLIT, HEADS_BROADCAST, HEADS_REDUCE, FLAG_ALL, FLAG_UPPER, FLAG_MAPPED,
                    BERNOULLI_NONE, BERNOULLI_DROPOUT, BERNOULLI_KEEP, SAMPLE_NO_PADDING, SAMPLE_PADDING, SAMPLE_HEAD,
@@ -713,19 +713,29 @@ def gat_backward_recompute(csr, csr_t, Q, K, V, G, Y, bias, act, stats, num_head
 RNG_STREAM_DROPOUT, RNG_STREAM_SAMPLER, RNG_STREAM_LINK = 0, 1, 2
 
 
+def _keyed(entry, seed):
+    """The entry and key arguments for `seed`: a host key, or an _rng.DeviceKey (CUDA-graph capture), which goes to the
+    _devkey twin of the entry as (base pointer, slot)."""
+    if isinstance(seed, _rng.DeviceKey):
+        return entry[:-len("_f32")] + "_devkey_f32", (_p(seed.base), int(seed.slot))
+    return entry, (int(seed),)
+
+
 def dropout(x, rate, seed, rng_stream=RNG_STREAM_DROPOUT, out=None):
-    """tf.nn.dropout with a counter-based mask: element i is kept iff u(seed, i) >= rate, kept values * 1/(1-rate)."""
+    """tf.nn.dropout with a counter-based mask: element i is kept iff u(seed, i) >= rate, kept values * 1/(1-rate).
+    `seed` is a host key or an _rng.DeviceKey."""
     _check(x, torch.float32, "x")
     if out is None:
         out = torch.empty_like(x)
-    _ffi.call("tfgk_dropout_f32", _p(x), x.numel(), float(rate), int(seed), int(rng_stream), _p(out), _stream(x))
+    entry, key = _keyed("tfgk_dropout_f32", seed)
+    _ffi.call(entry, _p(x), x.numel(), float(rate), *key, int(rng_stream), _p(out), _stream(x))
     return out
 
 
 def spmm_heads(csr, w, src, num_heads, mode=HEADS_SPLIT, emap=None, drop_rate=0.0, seed=0,
                rng_stream=RNG_STREAM_DROPOUT, alpha=1.0, bias=None, act=ACT_NONE, out=None):
     """Per-(edge, head) weighted aggregation over `csr`; see tfgk_spmm_heads_f32.  w: [E, H] (looked up through `emap`
-    when the CSR is a transposed view of the structure w was computed on)."""
+    when the CSR is a transposed view of the structure w was computed on).  `seed` is a host key or an _rng.DeviceKey."""
     _check(w, torch.float32, "w")
     if not (src.is_cuda and src.dtype == torch.float32):
         raise TypeError("src must be a float32 CUDA tensor")
@@ -745,22 +755,25 @@ def spmm_heads(csr, w, src, num_heads, mode=HEADS_SPLIT, emap=None, drop_rate=0.
         out = torch.empty((csr.n_rows, out_w), dtype=torch.float32, device=src.device)
     if bias is not None:
         _check(bias, torch.float32, "bias")
-    _ffi.call("tfgk_spmm_heads_f32", _p(csr.rowptr), _p(csr.col), _p(emap), _p(w), _p(src), lds, csr.n_rows, H, dh,
-              int(mode), float(drop_rate), int(seed), int(rng_stream), float(alpha), _p(bias), act, _p(out),
-              _row_major_2d(out, "out"), _stream(src))
+    entry, key = _keyed("tfgk_spmm_heads_f32", seed)
+    _ffi.call(entry, _p(csr.rowptr), _p(csr.col), _p(emap), _p(w), _p(src), lds, csr.n_rows, H, dh, int(mode),
+              float(drop_rate), *key, int(rng_stream), float(alpha), _p(bias), act, _p(out), _row_major_2d(out, "out"),
+              _stream(src))
     return out
 
 
 def gat_softmax_bwd(csr, att, G, V, num_heads, split_value_heads=True, drop_rate=0.0, seed=0,
                     rng_stream=RNG_STREAM_DROPOUT):
-    """d loss / d scaled scores [E, H] (CSR order) from G = d loss / d aggregated rows; see tfgk_gat_softmax_bwd_f32."""
+    """d loss / d scaled scores [E, H] (CSR order) from G = d loss / d aggregated rows; see tfgk_gat_softmax_bwd_f32.
+    `seed` is a host key or an _rng.DeviceKey."""
     _check(att, torch.float32, "att")
     H = int(num_heads)
     dv = V.shape[1] // H
     ds = torch.empty((csr.nnz, H), dtype=torch.float32, device=att.device)
-    _ffi.call("tfgk_gat_softmax_bwd_f32", _p(csr.rowptr), _p(csr.col), _p(att), _p(G), _row_major_2d(G, "G"), _p(V),
-              _row_major_2d(V, "V"), csr.n_rows, H, dv, 1 if split_value_heads else 0, float(drop_rate), int(seed),
-              int(rng_stream), _p(ds), _stream(att))
+    entry, key = _keyed("tfgk_gat_softmax_bwd_f32", seed)
+    _ffi.call(entry, _p(csr.rowptr), _p(csr.col), _p(att), _p(G), _row_major_2d(G, "G"), _p(V), _row_major_2d(V, "V"),
+              csr.n_rows, H, dv, 1 if split_value_heads else 0, float(drop_rate), *key, int(rng_stream), _p(ds),
+              _stream(att))
     return ds
 
 

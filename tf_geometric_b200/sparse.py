@@ -106,7 +106,7 @@ class SparseMatrix(object):
         if not training or rate <= 0.0:
             return self
         from . import autograd
-        seed = _rng.resolve(seed)
+        seed = _rng.resolve(seed, self.value.device)
         # differentiable values (learnable edge weights) take the gradient through the same regenerated mask
         value = autograd.Dropout.apply(self.value, rate, seed) if autograd.needs_grad(self.value) else \
             ops.dropout(self.value, rate, seed)

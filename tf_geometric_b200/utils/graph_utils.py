@@ -403,7 +403,7 @@ def negative_sampling(num_samples, num_nodes, edge_index=None, replace=True, mod
     :param seed: optional 64-bit key pinning the draws
     :return: device tensors for device (and for absent) edge_index, numpy arrays for numpy edge_index
     """
-    seed = _rng.resolve(seed)
+    seed = _rng.resolve_host(seed)
     num_samples, num_nodes = int(num_samples), int(num_nodes)
     n_batches = 1 if batch_size is None else int(batch_size)
     if num_samples < 0 or num_nodes < 0:
@@ -438,7 +438,7 @@ def negative_sampling_with_start_node(start_node_index, num_nodes, edge_index=No
     uniform over the candidates.  A start node adjacent to every other node raises ValueError (the reference loops
     forever).  Without edge_index b is uniform in [0, num_nodes).  Returns int32 [2, S] in the container of
     start_node_index."""
-    seed = _rng.resolve(seed)
+    seed = _rng.resolve_host(seed)
     num_nodes = int(num_nodes)
     on_device = _is_device(start_node_index)
     dev = edge_index.device if _is_device(edge_index) else None
@@ -472,7 +472,7 @@ def edge_train_test_split(edge_index, test_size, edge_weight=None, mode="undirec
         warnings.warn("argument \"num_nodes\" is deprecated for the method \"edge_train_test_split\", you can remove it")
     if mode != "undirected":
         raise NotImplementedError()
-    seed = _rng.resolve(seed)
+    seed = _rng.resolve_host(seed)
     ei = ops.as_device(edge_index, torch.int32)
     w = None if edge_weight is None else ops.as_device(edge_weight, torch.float32, device=ei.device).reshape(-1)
     upper, props = convert_edge_to_upper(ei, None if w is None else [w], None if w is None else ["max"])

@@ -98,7 +98,7 @@ class RandomNeighborSampler(_SamplerBase):
             w_csr = ops.permute(w, csr.perm)
         if csr.nnz == 0:
             return None, None
-        out_row, out_pos, _ = ops.neighbor_sample(csr, k=k, ratio=ratio, padding=padding, seed=_rng.resolve(seed))
+        out_row, out_pos, _ = ops.neighbor_sample(csr, k=k, ratio=ratio, padding=padding, seed=_rng.resolve_host(seed))
         if out_row.numel() == 0:
             return None, None
         return torch.stack([out_row, ops.gather_i32(csr.col, out_pos)]), ops.permute(w_csr, out_pos)
@@ -108,7 +108,7 @@ class UniformNeighborSampler(_SamplerBase):
     """Independent Bernoulli(prob) edge sampling (graph_utils.py:775-846)."""
 
     def sample(self, prob, sampled_node_index=None, seed=None):
-        seed = _rng.resolve(seed)
+        seed = _rng.resolve_host(seed)
         if sampled_node_index is None:
             flag = ops.edge_flags(None, None, self.num_edges, bernoulli=ops.BERNOULLI_KEEP, prob=float(prob), seed=seed,
                                   device=self.edge_index.device)
