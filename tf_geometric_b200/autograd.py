@@ -162,7 +162,8 @@ class SparseMatmul(torch.autograd.Function):
     """y = act(A @ h + b) for a cached SparseMatrix A (gcn.py:280-288), differentiable w.r.t. h, b and, when they are
     passed as the trailing input, the values of A (COO order; tf_sparse products are differentiable in their values).
     dz = dy * (y > 0) for relu; dh = A^T dz runs the same kernel on the transposed structure of A (built once per
-    matrix, values permuted into it); d value_e = <dz[row_e], h[col_e]> is K7 over A's CSR, written in COO order."""
+    matrix, values permuted into it again after an in-place update, SparseMatrix.value_csc); d value_e =
+    <dz[row_e], h[col_e]> is K7 over A's CSR, written in COO order."""
 
     @staticmethod
     def forward(ctx, h, bias, adj, act_code, value=None):
@@ -184,10 +185,7 @@ class SparseMatmul(torch.autograd.Function):
         adj = ctx.adj
         grad_h = grad_b = grad_value = None
         if ctx.needs_input_grad[0]:
-            csr_t = adj._transposed_csr()
-            if getattr(adj, "_value_csc", None) is None:
-                adj._value_csc = ops.permute(adj.value.detach(), csr_t.perm)
-            grad_h = ops.spmm(csr_t, adj._value_csc, g, reduce="sum")
+            grad_h = ops.spmm(adj._transposed_csr(), adj.value_csc, g, reduce="sum")
         if ctx.has_bias and ctx.needs_input_grad[1]:
             grad_b = ops.colsum(g)
         if len(ctx.needs_input_grad) > 4 and ctx.needs_input_grad[4]:        # four-argument calls pass no values

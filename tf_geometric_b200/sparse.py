@@ -4,9 +4,13 @@
 destination-sorted CSR + sm_90a kernels instead of tf.gather / tf.math.unsorted_segment_sum.
 
 COO semantics are kept on the outside: `index` int32 [2, nnz] (row = aggregation target), `value` float32 [nnz]
-in the caller's edge order, no sorting or merging is visible.  The CSR (stable sort by row) and the CSR-ordered
-values are built lazily, once per object, and reused by every product - this is what `graph.cache` memoises.
+in the caller's edge order, no sorting or merging is visible.  The CSR (stable sort by row) is built lazily, once per
+object, and reused by every product - this is what `graph.cache` memoises.  The values permuted into the CSR (and into
+the transposed CSR) are kept too, for as long as `value` is the same tensor with the same version and storage: an
+in-place update of learnable values (optimizer.step()) makes the next product permute them again.
 """
+import weakref
+
 import torch
 
 from . import ops, _rng
@@ -30,8 +34,10 @@ class SparseMatrix(object):
         self._shape = [int(shape[0]), int(shape[1])]
         self._csr = _csr
         self._value_csr = _value_csr
+        self._value_csr_of = None if _value_csr is None else self._value_stamp()    # derived from the value as given
         self._csc = None
         self._value_csc = None
+        self._value_csc_of = None
         self._pattern_of = None           # matrix with the same pattern whose transposed CSR is shared (dropout)
 
     # ---- structure ----
@@ -58,11 +64,31 @@ class SparseMatrix(object):
                                       self._shape[1])
         return self._csr
 
+    def _value_stamp(self):
+        """What a permuted copy of `value` is valid for: the same tensor (held by weak reference, as _structure._lookup
+        holds its keys), unmodified in place (its version counter) and over the same storage.  An inference tensor
+        (made under torch.inference_mode()) has no version counter: it can only be modified in place inside inference
+        mode, where nothing is learned, so identity and storage are its whole stamp."""
+        v = self.value
+        return weakref.ref(v), None if v.is_inference() else v._version, v.data_ptr()
+
+    def _stamp_current(self, stamp):
+        return stamp is not None and stamp[0]() is self.value and stamp[1:] == self._value_stamp()[1:]
+
     @property
     def value_csr(self):
-        if self._value_csr is None:
+        if self._value_csr is None or not self._stamp_current(self._value_csr_of):
             self._value_csr = ops.permute(self.value, self.csr.perm)
+            self._value_csr_of = self._value_stamp()
         return self._value_csr
+
+    @property
+    def value_csc(self):
+        """`value` (detached) in the order of the transposed CSR, rebuilt under value_csr's rule."""
+        if self._value_csc is None or not self._stamp_current(self._value_csc_of):
+            self._value_csc = ops.permute(self.value.detach(), self._transposed_csr().perm)
+            self._value_csc_of = self._value_stamp()
+        return self._value_csc
 
     def _transposed_csr(self):
         if self._csc is None and self._pattern_of is not None:
