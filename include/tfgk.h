@@ -162,6 +162,16 @@ int tfgk_spmm_f32(const int64_t *rowptr, const int32_t *col, const float *w,
                   float alpha, const float *addend, int64_t ld_addend, float beta,
                   const float *bias, int act,
                   float *out, int64_t ldo, const tfgk_plan *plan, void *stream);
+/* Aggregate, then project (GCN inference when the input is narrower than the layer):
+ *   out[r, :] = act( (SUM_{e in row r} w[e] * x[col[e], :]) . W + bias )          r in [0, n_dst)
+ * x [n, F] fp32 with 16-byte aligned rows and ldx % 4 == 0, W [F, U] row-major, bias [U] or NULL, act NONE or RELU;
+ * 4 <= F < U <= 128 and F % 4 == 0, anything else returns TFGK_ERR_UNSUPPORTED.  The aggregate of each row (never
+ * stored) is bit-identical to tfgk_spmm_f32's SUM over x with the same plan, which it takes where tfgk_spmm_f32 does
+ * (F >= 32; the plan's hub scratch takes F floats per slot).  Each output is then an fmaf chain over k = 0 .. F-1 from
+ * +0, then + bias[c] (rounded), then the activation.  Algorithmic bytes: E*(4*F + 4 [+4 weighted]) + N*(4*U + 8). */
+int tfgk_spmm_proj_f32(const int64_t *rowptr, const int32_t *col, const float *w,
+                       const float *x, int64_t ldx, int32_t n_dst, int32_t F, const float *W, int32_t U,
+                       const float *bias, int act, float *out, int64_t ldo, const tfgk_plan *plan, void *stream);
 /* The same with bf16 rows h (w, addend, bias, the accumulators and out stay fp32).  Bf16 -> fp32 widening is exact, and
  * the kernels widen each element and run the fp32 arithmetic in the same order with the same plan, so the output is
  * bit-identical to tfgk_spmm_f32 over the widened table with the same leading dimension and alignment in elements.  Rows

@@ -56,6 +56,7 @@ SIGNATURES = {
     "tfgk_scale_edges_f32": [_ptr, _ptr, _ptr, _i64, _ptr, _ptr, _ptr, _ptr],
     "tfgk_spmm_f32": [_ptr, _ptr, _ptr, _ptr, _i64, _i32, _i32, _int, _f32, _ptr, _i64, _f32, _ptr, _int, _ptr, _i64,
                       _ptr, _ptr],
+    "tfgk_spmm_proj_f32": [_ptr, _ptr, _ptr, _ptr, _i64, _i32, _i32, _ptr, _i32, _ptr, _int, _ptr, _i64, _ptr, _ptr],
     "tfgk_spmm_bf16": [_ptr, _ptr, _ptr, _ptr, _i64, _i32, _i32, _int, _f32, _ptr, _i64, _f32, _ptr, _int, _ptr, _i64,
                        _ptr, _ptr],
     "tfgk_spmm_bf16_dual": [_ptr, _ptr, _ptr, _ptr, _i64, _i32, _i32, _int, _f32, _ptr, _i64, _f32, _ptr, _int, _ptr,

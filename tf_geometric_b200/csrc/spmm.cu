@@ -90,6 +90,10 @@ struct SpmmParams {
     int32_t n_hubs;
     const int32_t *hub_row, *hub_slot0, *hub_nslots;
     float *scratch;
+    // tfgk_spmm_proj_f32 only (the kernels instantiated with PROJ): out = act(agg . pw + bias), pw [D, pu] row-major
+    const float *pw;
+    int32_t pu;
+    bool pio4;             // bias and out may be accessed four columns at a time
 };
 
 // the message rows of a kernel instantiated for element type T (float or bf16 bits)
@@ -462,6 +466,66 @@ __global__ void __launch_bounds__(kAsyncWarps * 32) spmm_async_kernel(const Spmm
     while (r < r1) finalize_row();
 }
 
+// The epilogue of tfgk_spmm_proj_f32 for NB finished rows row0 .. row0+nrows-1 whose F-wide aggregates sit at agg
+// (ldagg floats apart): out[r, c] = act(fmaf chain over k = 0 .. F-1 of agg[r, k] * W[k, c] from +0, + bias[c]).  Lane j
+// computes columns 4j .. 4j+3, so one W row serves all NB rows; a row's bits depend on nothing but its own aggregate.
+// W rows are ldw floats apart: PADDED = ldw is a multiple of 4 with zero columns from pu on (the shared-memory copy);
+// otherwise W is read column by column with bounds checks (the hub fix-up reads it from global memory).
+template <int NB, bool PADDED>
+__device__ __forceinline__ void project_rows(const SpmmParams &p, const float *__restrict__ Wm, int ldw,
+                                             const float *agg, int ldagg, int nrows, int F, int64_t row0, int lane) {
+    const int c = lane * 4;
+    if (c >= p.pu) return;
+    float o[NB][4];
+#pragma unroll
+    for (int b = 0; b < NB; ++b)
+#pragma unroll
+        for (int x = 0; x < 4; ++x) o[b][x] = 0.0f;
+    for (int k = 0; k < F; k += 4) {
+        float wk[4][4];
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            if constexpr (PADDED) {
+                const float4 t = *reinterpret_cast<const float4 *>(Wm + (k + i) * ldw + c);
+                wk[i][0] = t.x; wk[i][1] = t.y; wk[i][2] = t.z; wk[i][3] = t.w;
+            } else {
+#pragma unroll
+                for (int x = 0; x < 4; ++x) wk[i][x] = c + x < p.pu ? __ldg(Wm + (int64_t)(k + i) * ldw + c + x) : 0.0f;
+            }
+        }
+#pragma unroll
+        for (int b = 0; b < NB; ++b) {
+            const float4 a = *reinterpret_cast<const float4 *>(agg + b * ldagg + k);
+#pragma unroll
+            for (int x = 0; x < 4; ++x) {
+                o[b][x] = fmaf(a.x, wk[0][x], o[b][x]);
+                o[b][x] = fmaf(a.y, wk[1][x], o[b][x]);
+                o[b][x] = fmaf(a.z, wk[2][x], o[b][x]);
+                o[b][x] = fmaf(a.w, wk[3][x], o[b][x]);
+            }
+        }
+    }
+    float bs[4] = {0.f, 0.f, 0.f, 0.f};
+    if (p.bias) {
+        if (p.pio4) load_vec<4>(p.bias + c, bs);
+        else
+#pragma unroll
+            for (int x = 0; x < 4; ++x) if (c + x < p.pu) bs[x] = p.bias[c + x];
+    }
+#pragma unroll
+    for (int b = 0; b < NB; ++b) {
+        if (b >= nrows) break;
+        float v[4];
+#pragma unroll
+        for (int x = 0; x < 4; ++x) v[x] = apply_act(p.bias ? __fadd_rn(o[b][x], bs[x]) : o[b][x], p.act);
+        float *dst = p.out + (row0 + b) * p.ldo + c;
+        if (p.pio4) store_vec<4>(dst, v);
+        else
+#pragma unroll
+            for (int x = 0; x < 4; ++x) if (c + x < p.pu) dst[x] = v[x];
+    }
+}
+
 // ------------------------------------------------------------------------------------------------------------
 // TMA ring variant (north_star: "staged through TMA into shared memory").  Same edge streaming, ring and arithmetic as
 // spmm_async_kernel, but the neighbour rows of a round of U = 4 edges are fetched by the TMA unit: lane 0 arms the
@@ -487,27 +551,56 @@ __device__ __forceinline__ void mbar_wait_parity(uint32_t bar, uint32_t parity) 
     }
 }
 
-template <bool IS_MAX, int S, typename T, bool DUAL = false>
-__global__ void __launch_bounds__(kAsyncWarps * 32) spmm_tma4_kernel(const SpmmParams p, uint32_t row_bytes) {
+// PROJ (tfgk_spmm_proj_f32, fp32 SUM only): the finished rows of a warp are projected through W in batches of kProjRows
+// (project_rows), with W copied into shared memory once per CTA of WARPS warps, behind the ring and its mbarriers.
+constexpr int kProjRows = 4;
+constexpr int kProjWarps = 8;
+
+// shared memory of spmm_tma4_kernel: the ring, the mbarriers, fp8 exponents or (PROJ) W padded to pu rounded up to 4
+// columns and kProjRows aggregate rows per warp
+template <bool PROJ, typename T>
+__host__ __device__ inline size_t tma4_smem_bytes(int warps, int S, uint32_t row_bytes, int D, int pu) {
+    const size_t stage_pitch = ((size_t)4 * row_bytes + 127) & ~(size_t)127;
+    size_t bytes = (size_t)warps * S * stage_pitch + (size_t)warps * S * 8 +
+                   (sizeof(T) == 1 ? (size_t)warps * S * 4 * sizeof(uint16_t) : 0);
+    if (PROJ) bytes = (bytes + 15) / 16 * 16 + ((size_t)D * ((pu + 3) / 4 * 4) + (size_t)warps * kProjRows * D) * 4;
+    return bytes;
+}
+
+template <bool IS_MAX, int S, typename T, bool DUAL, bool PROJ, int WARPS>
+__device__ __forceinline__ void spmm_tma4_body(const SpmmParams &p, uint32_t row_bytes) {
     constexpr int U = 4, RPC = 32 / U;
     constexpr bool FP8 = sizeof(T) == 1;
     static_assert(S <= 2 * RPC, "weight look-ahead registers would be overwritten before they are consumed");
+    static_assert(!PROJ || (!IS_MAX && !DUAL && sizeof(T) == 4), "the projection epilogue follows an fp32 sum");
     extern __shared__ __align__(128) uint8_t g4_ring[];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const uint32_t stage_bytes = (U * row_bytes + 127u) & ~127u;
     uint8_t *my_ring = g4_ring + (size_t)warp * S * stage_bytes;
     const uint32_t ring_addr = (uint32_t)__cvta_generic_to_shared(my_ring);
-    uint64_t *bars = reinterpret_cast<uint64_t *>(g4_ring + (size_t)kAsyncWarps * S * stage_bytes) + warp * S;
+    uint64_t *bars = reinterpret_cast<uint64_t *>(g4_ring + (size_t)WARPS * S * stage_bytes) + warp * S;
     // fp8: the exponents of every edge in the ring, [S][U] 16-bit entries per warp (group 0 low byte, group 1 high byte)
-    uint16_t *sexp = reinterpret_cast<uint16_t *>(g4_ring + (size_t)kAsyncWarps * S * (stage_bytes + 8)) + warp * S * U;
+    uint16_t *sexp = reinterpret_cast<uint16_t *>(g4_ring + (size_t)WARPS * S * (stage_bytes + 8)) + warp * S * U;
     const uint32_t bar0 = (uint32_t)__cvta_generic_to_shared(bars);
+    // PROJ: W [D][ldw] and this warp's kProjRows aggregate rows; every thread helps copy W before any warp can leave
+    float *w_s = nullptr, *agg_s = nullptr;
+    const int ldw = (p.pu + 3) & ~3;
+    if constexpr (PROJ) {
+        w_s = reinterpret_cast<float *>(g4_ring + ((size_t)WARPS * S * (stage_bytes + 8) + 15) / 16 * 16);
+        agg_s = w_s + (size_t)p.D * ldw + (size_t)warp * kProjRows * p.D;
+        for (int i = threadIdx.x; i < p.D * ldw; i += WARPS * 32) {
+            const int k = i / ldw, c = i - k * ldw;
+            w_s[i] = c < p.pu ? __ldg(p.pw + (int64_t)k * p.pu + c) : 0.0f;
+        }
+        __syncthreads();
+    }
     if (lane == 0) {
 #pragma unroll
         for (int i = 0; i < S; ++i) asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(bar0 + 8 * i));
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     __syncwarp();
-    const int64_t task = (int64_t)blockIdx.x * kAsyncWarps + warp;
+    const int64_t task = (int64_t)blockIdx.x * WARPS + warp;
     int64_t r0, r1, e_begin, e_stop;
     int slot = -1;
     if (p.task_row != nullptr) {
@@ -544,13 +637,25 @@ __global__ void __launch_bounds__(kAsyncWarps * 32) spmm_tma4_kernel(const SpmmP
     int row_end = slot >= 0 ? 0x7fffffff : (int)(__shfl_sync(0xffffffffu, rp_hi, 0) - e_begin);
     const bool is_mean = p.reduce == TFGK_REDUCE_MEAN;
 
+    int n_done = 0;                                 // PROJ: finished rows r - n_done .. r-1 waiting in agg_s
+    auto project_done = [&]() {
+        __syncwarp();
+        project_rows<kProjRows, true>(p, w_s, ldw, agg_s, p.D, n_done, p.D, r - n_done, lane);
+        __syncwarp();
+        n_done = 0;
+    };
     auto finalize_row = [&]() {
         const int64_t row_start = __shfl_sync(0xffffffffu, rp_lo, (int)(r - r0));
         const int deg = (int)(row_end + e_begin - row_start);
         const float cnt = (float)max(deg, 1);
 #pragma unroll
         for (int k = 0; k < NCX; ++k) {
-            if (DUAL && cok[k]) {
+            if (PROJ) {                             // D <= 128: the row is acc[0] of lanes 0 .. D/4-1
+                if (k == 0 && cok[0])
+                    *reinterpret_cast<float4 *>(agg_s + n_done * p.D + coff[0]) = make_float4(acc[0][0], acc[0][1], acc[0][2], acc[0][3]);
+#pragma unroll
+                for (int x = 0; x < 4; ++x) acc[k][x] = 0.0f;
+            } else if (DUAL && cok[k]) {
                 epilogue_dual<4>(p, r, coff[k], acc[k], cnt);
 #pragma unroll
                 for (int x = 0; x < 4; ++x) acc[k][x] = IS_MAX ? -FLT_MAX : 0.0f;
@@ -572,6 +677,9 @@ __global__ void __launch_bounds__(kAsyncWarps * 32) spmm_tma4_kernel(const SpmmP
             }
         }
         ++r;
+        if constexpr (PROJ) {
+            if (++n_done == kProjRows) project_done();
+        }
         if (r < r1) row_end = (int)(__shfl_sync(0xffffffffu, rp_hi, (int)(r - r0)) - e_begin);
     };
     auto load_chunk = [&](int c, int &ci, float &wi) {
@@ -674,11 +782,26 @@ __global__ void __launch_bounds__(kAsyncWarps * 32) spmm_tma4_kernel(const SpmmP
         return;
     }
     while (r < r1) finalize_row();
+    if constexpr (PROJ) {
+        if (n_done > 0) project_done();
+    }
+}
+
+template <bool IS_MAX, int S, typename T, bool DUAL = false>
+__global__ void __launch_bounds__(kAsyncWarps * 32) spmm_tma4_kernel(const SpmmParams p, uint32_t row_bytes) {
+    spmm_tma4_body<IS_MAX, S, T, DUAL, false, kAsyncWarps>(p, row_bytes);
+}
+
+// tfgk_spmm_proj_f32: the fp32 SUM ring with the projection epilogue, WARPS warps sharing one copy of W
+template <int S, int WARPS>
+__global__ void __launch_bounds__(WARPS * 32) spmm_proj_tma4_kernel(const SpmmParams p, uint32_t row_bytes) {
+    spmm_tma4_body<false, S, float, false, true, WARPS>(p, row_bytes);
 }
 
 // merges the slices of every hub row in slice order (deterministic) and applies the epilogue; one warp per hub row
-template <bool IS_MAX, bool DUAL = false>
-__global__ void __launch_bounds__(256) spmm_hub_fixup_kernel(const SpmmParams p) {
+// (PROJ: D <= 128; the merged row goes through project_rows with W read from global memory)
+template <bool IS_MAX, bool DUAL, bool PROJ>
+__device__ __forceinline__ void spmm_hub_fixup_body(const SpmmParams &p, float (*agg_s)[128]) {
     const int lane = threadIdx.x & 31;
     const int h = blockIdx.x * 8 + (threadIdx.x >> 5);
     if (h >= p.n_hubs) return;
@@ -692,6 +815,10 @@ __global__ void __launch_bounds__(256) spmm_hub_fixup_kernel(const SpmmParams p)
             load_vec<4>(p.scratch + (int64_t)(s0 + s) * p.D + c, v);
 #pragma unroll
             for (int x = 0; x < 4; ++x) acc[x] = IS_MAX ? fmaxf(acc[x], v[x]) : __fadd_rn(acc[x], v[x]);
+        }
+        if constexpr (PROJ) {
+            store_vec<4>(&agg_s[threadIdx.x >> 5][c], acc);
+            continue;
         }
         if constexpr (DUAL) {
             epilogue_dual<4>(p, r, c, acc, cnt);
@@ -711,6 +838,20 @@ __global__ void __launch_bounds__(256) spmm_hub_fixup_kernel(const SpmmParams p)
         }
         store_vec<4>(p.out + r * p.ldo + c, o);
     }
+    if constexpr (PROJ) {
+        __syncwarp();
+        project_rows<1, false>(p, p.pw, p.pu, agg_s[threadIdx.x >> 5], 128, 1, p.D, r, lane);
+    }
+}
+
+template <bool IS_MAX, bool DUAL = false>
+__global__ void __launch_bounds__(256) spmm_hub_fixup_kernel(const SpmmParams p) {
+    spmm_hub_fixup_body<IS_MAX, DUAL, false>(p, nullptr);
+}
+
+__global__ void __launch_bounds__(256) spmm_hub_fixup_proj_kernel(const SpmmParams p) {
+    __shared__ __align__(16) float agg_s[8][128];      // the merged row of each warp
+    spmm_hub_fixup_body<false, false, true>(p, agg_s);
 }
 
 template <int NC, int U, int S, typename T = float, bool DUAL = false>
@@ -737,20 +878,21 @@ static int launch_spmm_async(const SpmmParams &p, cudaStream_t st) {
     return TFGK_OK;
 }
 
-template <int S, typename T = float, bool DUAL = false>
+template <int S, typename T = float, bool DUAL = false, bool PROJ = false, int WARPS = kAsyncWarps>
 static int launch_spmm_tma4(const SpmmParams &p, cudaStream_t st) {
     // cp.async.bulk wants 16-byte aligned rows: D, ldh multiples of 16 bytes' worth of elements and an aligned base
     constexpr int kPer16 = 16 / (int)sizeof(T);
     const void *base = sizeof(T) == 4 ? (const void *)p.h : sizeof(T) == 2 ? (const void *)p.hb : (const void *)p.h8;
     if (p.D > 256 || p.D % kPer16 != 0 || p.ldh % kPer16 != 0 || !aligned16(base)) return TFGK_ERR_UNSUPPORTED;
     const uint32_t row_bytes = (uint32_t)(p.D * sizeof(T));
-    const size_t stage_pitch = ((size_t)4 * row_bytes + 127) & ~(size_t)127;
-    const size_t smem = (size_t)kAsyncWarps * S * stage_pitch + (size_t)kAsyncWarps * S * 8 +
-                        (sizeof(T) == 1 ? (size_t)kAsyncWarps * S * 4 * sizeof(uint16_t) : 0);
+    const size_t smem = tma4_smem_bytes<PROJ, T>(WARPS, S, row_bytes, p.D, PROJ ? p.pu : 0);
     if (smem > 200 * 1024) return TFGK_ERR_UNSUPPORTED;
     const int64_t n_tasks = p.task_row ? p.n_tasks : ceil_div64(p.n_dst, kAsyncRows);
-    const unsigned blocks = (unsigned)ceil_div64(n_tasks, kAsyncWarps);
-    if (p.reduce == TFGK_REDUCE_MAX) {
+    const unsigned blocks = (unsigned)ceil_div64(n_tasks, WARPS);
+    if constexpr (PROJ) {
+        TFGK_CUDA(ensure_dynamic_smem(spmm_proj_tma4_kernel<S, WARPS>, smem));
+        spmm_proj_tma4_kernel<S, WARPS><<<blocks, WARPS * 32, smem, st>>>(p, row_bytes);
+    } else if (p.reduce == TFGK_REDUCE_MAX) {
         TFGK_CUDA(ensure_dynamic_smem(spmm_tma4_kernel<true, S, T, DUAL>, smem));
         spmm_tma4_kernel<true, S, T, DUAL><<<blocks, kAsyncWarps * 32, smem, st>>>(p, row_bytes);
     } else {
@@ -760,7 +902,8 @@ static int launch_spmm_tma4(const SpmmParams &p, cudaStream_t st) {
     TFGK_LAUNCH_CHECK();
     if (p.task_row && p.n_hubs > 0) {
         const unsigned fb = (unsigned)ceil_div64(p.n_hubs, 8);
-        if (p.reduce == TFGK_REDUCE_MAX) spmm_hub_fixup_kernel<true, DUAL><<<fb, 256, 0, st>>>(p);
+        if (PROJ) spmm_hub_fixup_proj_kernel<<<fb, 256, 0, st>>>(p);
+        else if (p.reduce == TFGK_REDUCE_MAX) spmm_hub_fixup_kernel<true, DUAL><<<fb, 256, 0, st>>>(p);
         else spmm_hub_fixup_kernel<false, DUAL><<<fb, 256, 0, st>>>(p);
         TFGK_LAUNCH_CHECK();
     }
@@ -838,6 +981,7 @@ static SpmmParams spmm_params(const int64_t *rowptr, const int32_t *col, const f
     p.n_tasks = 0; p.task_row = nullptr; p.task_nrows = nullptr; p.task_e0 = nullptr; p.task_e1 = nullptr;
     p.task_slot = nullptr; p.n_hubs = 0; p.hub_row = nullptr; p.hub_slot0 = nullptr; p.hub_nslots = nullptr;
     p.scratch = nullptr;
+    p.pw = nullptr; p.pu = 0; p.pio4 = false;
     return p;
 }
 
@@ -875,6 +1019,31 @@ extern "C" int tfgk_spmm_f32(const int64_t *rowptr, const int32_t *col, const fl
         if (rc != TFGK_OK) return rc;
     }
     return TFGK_OK;
+}
+
+// Aggregate, then project: out = act((A x) W + bias) with the aggregate A x never stored.  The aggregation is
+// tfgk_spmm_f32's TMA ring over the F-wide rows of x, with its plan taken where tfgk_spmm_f32 takes it for x (F >= 32; x
+// has 16-byte aligned rows here), so every aggregate is bit-identical to tfgk_spmm_f32's SUM; each finished row is then
+// projected in the ring kernel's epilogue (project_rows), hub rows in the fix-up kernel after their slices are merged.
+extern "C" int tfgk_spmm_proj_f32(const int64_t *rowptr, const int32_t *col, const float *w,
+                                  const float *x, int64_t ldx, int32_t n_dst, int32_t F, const float *W, int32_t U,
+                                  const float *bias, int act, float *out, int64_t ldo, const tfgk_plan *plan, void *stream) {
+    TFGK_CHECK_ARG(n_dst >= 0 && F >= 0 && U >= 0, "spmm_proj: negative size (n_dst=%d, F=%d, U=%d)", n_dst, F, U);
+    TFGK_CHECK_ARG(act == TFGK_ACT_NONE || act == TFGK_ACT_RELU, "spmm_proj: unknown activation %d", act);
+    if (F < 4 || F % 4 != 0 || F >= U || U > 128 || ldx % 4 != 0 || !aligned16(x)) return TFGK_ERR_UNSUPPORTED;
+    TFGK_CHECK_ARG(ldx >= F && ldo >= U, "spmm_proj: leading dimension too small (ldx=%lld, ldo=%lld)", (long long)ldx,
+                   (long long)ldo);
+    if (plan != nullptr && plan->n_hubs > 0 && F >= 32)
+        TFGK_CHECK_ARG(plan->scratch != nullptr && plan->scratch_bytes >= (size_t)plan->n_slots * F * sizeof(float),
+                       "spmm_proj: plan scratch too small (need %zu bytes)", (size_t)plan->n_slots * F * sizeof(float));
+    if (n_dst == 0) return TFGK_OK;
+    TFGK_CHECK_ARG(rowptr && x && W && out, "spmm_proj: null pointer");
+    SpmmParams p = spmm_params(rowptr, col, w, ldx, n_dst, TFGK_REDUCE_SUM, 1.0f, nullptr, 0, 0.0f, bias, act, out, ldo, 0, F);
+    p.h = x;
+    p.pw = W; p.pu = U;
+    p.pio4 = U % 4 == 0 && ldo % 4 == 0 && aligned16(out) && (!bias || aligned16(bias));
+    if (plan != nullptr && plan->n_tasks > 0 && F >= 32) use_plan(p, plan);
+    return launch_spmm_tma4<3, float, false, true, kProjWarps>(p, as_stream(stream));
 }
 
 // bf16 rows.  The kernels are the fp32 ones with each element widened on the way from shared memory (or from global

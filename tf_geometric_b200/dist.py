@@ -399,20 +399,27 @@ def _unwrap(x_local, dev):
 
 
 def gcn_partitioned(pg, x_local, kernel, bias=None, activation=None, renorm=True, improved=False):
-    """tfg.nn.gcn on a PartitionedGraph: returns this rank's rows of act(norm(A) (x W) + b)."""
+    """tfg.nn.gcn on a PartitionedGraph: returns this rank's rows of act(norm(A) (x W) + b), or of act((norm(A) x) W + b)
+    for the widths ops.spmm_proj takes, like the single-GPU layer."""
     dev = pg.edge_index.device
     _forward_only("gcn_partitioned", x_local, kernel, bias)
     x_local, shared = _unwrap(x_local, dev)
     csr, value_csr = pg.gcn_normed(renorm=renorm, improved=improved)
+    act_code, leftover = ops.activation_code(activation)
+    bias = None if bias is None else ops.as_device(bias, torch.float32, device=dev)
+    if kernel is not None and x_local.is_cuda and ops.spmm_proj_shape(x_local.shape[1], kernel.shape[1]):
+        # narrower input than output: gather x's rows and project each aggregate in the kernel's epilogue, as the
+        # single-GPU layer does (same bits)
+        out = ops.spmm_proj(csr, value_csr, pg.all_gather_rows(x_local),
+                            ops.as_device(kernel, torch.float32, device=dev), bias=bias, act=act_code)
+        return leftover(out) if leftover is not None else out
     h_full = shared.find(kernel) if shared is not None and kernel is not None else None
     if h_full is None:
         if kernel is None:
             h_full = pg.all_gather_rows(x_local)
         else:
             h_full = pg.project_all_rows(x_local, [[(ops.as_device(kernel, torch.float32, device=dev), None, ops.ACT_NONE)]])[0]
-    act_code, leftover = ops.activation_code(activation)
-    out = ops.spmm(csr, value_csr, h_full, reduce="sum",
-                   bias=None if bias is None else ops.as_device(bias, torch.float32, device=dev), act=act_code)
+    out = ops.spmm(csr, value_csr, h_full, reduce="sum", bias=bias, act=act_code)
     return leftover(out) if leftover is not None else out
 
 

@@ -65,8 +65,12 @@ class GCN(Layer):
         return self.build_cache_for_graph(graph, override=override)
 
     def partitioned_projections(self):
-        """All-row projections this layer needs on a partitioned graph: [(key, [(weight, bias, act code)])]."""
-        return [((id(self.kernel),), [(self.kernel, None, ops.ACT_NONE)])] if self.use_kernel else []
+        """All-row projections this layer needs on a partitioned graph: [(key, [(weight, bias, act code)])].  None when
+        the input is narrower than the output (ops.spmm_proj_shape) on the GPU: the rows of x are gathered and projected
+        after aggregation instead (dist.gcn_partitioned)."""
+        if not self.use_kernel or (self.kernel.is_cuda and ops.spmm_proj_shape(self.kernel.shape[0], self.kernel.shape[1])):
+            return []
+        return [((id(self.kernel),), [(self.kernel, None, ops.ACT_NONE)])]
 
     def _call_partitioned(self, x_local, pg):
         from ... import dist as tdist

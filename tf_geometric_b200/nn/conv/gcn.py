@@ -6,7 +6,9 @@
 norm(A) is computed once per graph by the integer/fp32 preprocessing kernels and memoised in `cache` (the reference
 stores a numpy triple under the same key, gcn.py:125-128; here the cached object is a device SparseMatrix that also
 carries the destination-sorted CSR, so a warm forward is exactly two launches: the dense projection and tfgk_spmm_f32
-with bias + activation fused into its epilogue).
+with bias + activation fused into its epilogue).  In inference, when the input is narrower than the output (ops.spmm_proj
+takes the shapes), a warm forward is one launch instead: act((norm(A) x) W + b) by tfgk_spmm_proj_f32, which gathers the
+narrower rows of x and projects each aggregate in its epilogue.
 """
 import torch
 
@@ -169,7 +171,13 @@ def gcn(x, sparse_adj, kernel, bias=None, activation=None,
                                                          ops.ACT_NONE)
         h = autograd.propagate(normed, h, bias, act_code)
         return leftover(h) if leftover is not None else h
-    h = x if kernel is None else ops.gemm(x, ops.as_device(kernel, torch.float32, device=dev))
+    if kernel is not None:
+        kernel = ops.as_device(kernel, torch.float32, device=dev)
+        if num_or_size_splits is None and ops.spmm_proj_supported(x, kernel):
+            # narrower input than output: gather the F-wide rows of x and project each aggregate in the kernel's epilogue
+            h = ops.spmm_proj(normed.csr, normed.value_csr, x, kernel, bias=bias, act=act_code)
+            return leftover(h) if leftover is not None else h
+    h = x if kernel is None else ops.gemm(x, kernel)
     h = normed.matmul(h, num_or_size_splits=num_or_size_splits, bias=bias, act=act_code)
     if leftover is not None:
         h = leftover(h)

@@ -332,6 +332,46 @@ def spmm(csr, w_csr, h, reduce="sum", alpha=1.0, addend=None, beta=0.0, bias=Non
     return out
 
 
+def spmm_proj_supported(x, W):
+    """True when tfgk_spmm_proj_f32 takes x [n, F] and W [F, U]: fp32 CUDA tensors, 4 <= F < U <= 128, F % 4 == 0, and
+    rows of x that are contiguous, 16-byte aligned and a multiple of 4 floats apart.  A shape-only condition."""
+    if not (x.is_cuda and x.dtype == torch.float32 and x.dim() == 2 and W.dim() == 2):
+        return False
+    if W.shape[0] != x.shape[1] or not spmm_proj_shape(x.shape[1], W.shape[1]) or x.stride(1) != 1:
+        return False
+    return _row_major_2d(x, "x") % 4 == 0 and x.data_ptr() % 16 == 0
+
+
+def spmm_proj_shape(F, U):
+    """The widths tfgk_spmm_proj_f32 takes: 4 <= F < U <= 128, F % 4 == 0."""
+    return 4 <= F < U <= 128 and F % 4 == 0
+
+
+def spmm_proj(csr, w_csr, x, W, bias=None, act=ACT_NONE, out=None):
+    """out = act((SUM_{e in row} w[e] * x[col[e]]) @ W + bias) with the aggregate never stored (tfgk_spmm_proj_f32, for
+    x and W that spmm_proj_supported accepts): each aggregate is bit-identical to spmm(csr, w_csr, x)'s, and each output is
+    an fmaf chain over the F columns of the aggregate from +0, then + bias, then the activation."""
+    if not spmm_proj_supported(x, W):
+        raise ValueError("spmm_proj: unsupported x {} / W {} (fp32 CUDA, 4 <= F < U <= 128, F % 4 == 0, aligned rows)".format(
+            tuple(x.shape), tuple(W.shape)))
+    W = W.to(torch.float32).contiguous()
+    n_dst, F, U = csr.n_rows, x.shape[1], W.shape[1]
+    if out is None:
+        out = torch.empty((n_dst, U), dtype=torch.float32, device=x.device)
+    elif not (out.is_cuda and out.dtype == torch.float32 and tuple(out.shape) == (n_dst, U)):
+        raise TypeError("spmm_proj: out must be a float32 CUDA tensor of shape {}".format((n_dst, U)))
+    if w_csr is not None:
+        _check(w_csr, torch.float32, "w_csr")
+    if bias is not None:
+        _check(bias, torch.float32, "bias")
+    plan = getattr(csr, "plan", None)
+    plan_struct = plan.struct(F, x.device) if plan is not None else None
+    _ffi.call("tfgk_spmm_proj_f32", _p(csr.rowptr), _p(csr.col), _p(w_csr), _p(x), _row_major_2d(x, "x"), n_dst, F, _p(W),
+              U, _p(bias), act, _p(out), _row_major_2d(out, "out"),
+              ctypes.byref(plan_struct) if plan_struct is not None else None, _stream(x))
+    return out
+
+
 def spmm_max(csr, w_csr, h):
     """(out, cnt): out[r] = max_{e in row r} w[e] * h[col[e]] (-FLT_MAX for an empty row), bit-identical to
     spmm(reduce="max"), and cnt[r, d] int32 = how many of those products equal out[r, d] (tfgk_spmm_max_f32, K11a)."""
