@@ -513,6 +513,35 @@ int tfgk_neighbor_sample_fill(const int64_t *rowptr, int32_t n_rows, int32_t k, 
                               uint64_t seed, uint32_t rng_stream, const int64_t *out_rowptr,
                               int32_t *out_row, int32_t *out_pos, void *stream);
 
+/* K13: the same sampler over a list of n_list rows of an existing CSR (rowptr with n_rows rows, not copied).  Listed row t
+ * is global row rows[t]; its sampled positions are exactly those tfgk_neighbor_sample_fill writes for that global row with
+ * the same k / ratio / padding / seed / rng_stream, in the same order, so a node's sample depends on the node and the key
+ * only.  Rows may repeat.  _count takes the workspace of tfgk_neighbor_sample_workspace_bytes(n_list), writes the
+ * [n_list + 1] offsets and their total (synchronises) and fails with TFGK_ERR_INDEX_OUT_OF_RANGE for a listed row outside
+ * [0, n_rows).  _fill writes out_pos and, unless out_row is null, the LIST position t of every sampled edge's row.
+ * Work is proportional to the listed rows' degrees: rows of degree <= 128 take one thread, longer rows a CTA of 256. */
+int tfgk_neighbor_sample_rows_count(const int64_t *rowptr, int32_t n_rows, const int32_t *rows, int32_t n_list, int32_t k,
+                                    double ratio, int padding, int64_t *out_rowptr, int64_t *total_host, void *workspace,
+                                    size_t workspace_bytes, void *stream);
+int tfgk_neighbor_sample_rows_fill(const int64_t *rowptr, int32_t n_rows, const int32_t *rows, int32_t n_list, int32_t k,
+                                   double ratio, int padding, uint64_t seed, uint32_t rng_stream, const int64_t *out_rowptr,
+                                   int32_t *out_row, int32_t *out_pos, void *stream);
+
+/* Relabelling through an int32 [N] id -> position map that holds -1 everywhere before and after each call (the caller
+ * fills it with -1 once and may keep it; calls that share a map must be ordered on one stream).  Node ids outside
+ * [0, N) fail with TFGK_ERR_INDEX_OUT_OF_RANGE; *n_dup_host counts the node-list entries that repeat an earlier id (the
+ * output is then meaningless and the caller reports the error).  Both synchronise `stream`.
+ * tfgk_reindex_i32: out[e] = position of ids[e] in nodes[0, n_nodes), -1 when absent or outside [0, N).
+ * tfgk_frontier_i32: nodes[0, n_nodes) is the current list and has room for S more ids.  The ids of cols[0, S) that are
+ * not in the list are appended in first-occurrence order (*n_new_host of them) and local_col[e] = the position of
+ * cols[e] in the grown list.  Deterministic: first occurrences are found with atomicMin and placed by a scan. */
+int tfgk_relabel_workspace_bytes(int64_t n_ids, size_t *out_bytes);
+int tfgk_reindex_i32(const int32_t *nodes, int32_t n_nodes, const int32_t *ids, int64_t n_ids, int32_t N, int32_t *map,
+                     int32_t *out, int32_t *n_dup_host, void *workspace, size_t workspace_bytes, void *stream);
+int tfgk_frontier_i32(const int32_t *cols, int64_t S, int32_t N, int32_t *nodes, int32_t n_nodes, int32_t *map,
+                      int32_t *local_col, int32_t *n_new_host, int32_t *n_dup_host, void *workspace, size_t workspace_bytes,
+                      void *stream);
+
 /* ---- link prediction (SURVEY.md 8(f)5, demo/demo_gae.py) -------------------------------------------------------- */
 
 /* K6, predict_edge of demo/demo_gae.py:53-60: out[e] = sum_d h[row_e, d] * h[col_e, d] in fp32, COO order.

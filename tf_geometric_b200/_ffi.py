@@ -119,6 +119,13 @@ SIGNATURES = {
     "tfgk_neighbor_sample_workspace_bytes": [_i32, ctypes.POINTER(_size)],
     "tfgk_neighbor_sample_count": [_ptr, _i32, _i32, _f64, _int, _ptr, ctypes.POINTER(_i64), _ptr, _size, _ptr],
     "tfgk_neighbor_sample_fill": [_ptr, _i32, _i32, _f64, _int, _u64, _u32, _ptr, _ptr, _ptr, _ptr],
+    "tfgk_neighbor_sample_rows_count": [_ptr, _i32, _ptr, _i32, _i32, _f64, _int, _ptr, ctypes.POINTER(_i64), _ptr, _size,
+                                        _ptr],
+    "tfgk_neighbor_sample_rows_fill": [_ptr, _i32, _ptr, _i32, _i32, _f64, _int, _u64, _u32, _ptr, _ptr, _ptr, _ptr],
+    "tfgk_relabel_workspace_bytes": [_i64, ctypes.POINTER(_size)],
+    "tfgk_reindex_i32": [_ptr, _i32, _ptr, _i64, _i32, _ptr, _ptr, ctypes.POINTER(_i32), _ptr, _size, _ptr],
+    "tfgk_frontier_i32": [_ptr, _i64, _i32, _ptr, _i32, _ptr, _ptr, ctypes.POINTER(_i32), ctypes.POINTER(_i32), _ptr, _size,
+                          _ptr],
     "tfgk_edge_dot_f32": [_ptr, _i64, _i32, _ptr, _ptr, _i64, _i32, _ptr, _ptr],
     "tfgk_neg_offsets_workspace_bytes": [_i32, ctypes.POINTER(_size)],
     "tfgk_neg_offsets": [_ptr, _i32, _int, _ptr, ctypes.POINTER(_i64), _ptr, _size, _ptr],
@@ -250,6 +257,11 @@ NOT_CAPTURABLE = {
     "tfgk_select_flagged_i32": ("select_flagged", "it returns the number of selected entries to the host"),
     "tfgk_neighbor_sample_count": ("the neighbour sampler", "it returns the number of sampled edges to the host"),
     "tfgk_neighbor_sample_fill": ("the neighbour sampler", "it takes a host-side key"),
+    "tfgk_neighbor_sample_rows_count": ("the mini-batch neighbourhood sampler", "it returns the number of sampled edges "
+                                        "to the host"),
+    "tfgk_neighbor_sample_rows_fill": ("the mini-batch neighbourhood sampler", "it takes a host-side key"),
+    "tfgk_reindex_i32": ("reindex_sampled_edge_index", "it returns the number of duplicate node ids to the host"),
+    "tfgk_frontier_i32": ("the mini-batch neighbourhood sampler", "it returns the number of new nodes to the host"),
     "tfgk_neg_offsets": ("negative sampling", "it returns the number of candidate pairs to the host"),
     "tfgk_neg_draw": ("negative sampling", "it takes a host-side key"),
     "tfgk_neg_sample_start": ("negative sampling", "it takes a host-side key"),

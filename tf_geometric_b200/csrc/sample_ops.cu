@@ -85,6 +85,160 @@ __global__ void sample_fill_kernel(const int64_t *__restrict__ rowptr, int32_t N
     }
 }
 
+// ---- K13: fan-out sampling from a list of rows ------------------------------------------------------------------
+// Row t of the list is global row rows[t]; its draws use the keys of that global row, so every listed row gets exactly
+// the positions sample_fill_kernel writes for it.  Algorithm R parallelises: with slot j initialised to start + j, the
+// sequential loop leaves slot j at start + max{i >= num : draw_i = j} (later draws overwrite earlier ones, and every
+// i >= num exceeds j), so an atomicMax per draw gives the same bits in any order.
+constexpr int kRowsPerCta = 256;
+constexpr int kThreadRowMax = 128;     // rows up to this degree are sampled by one thread, longer ones by the whole CTA
+
+__global__ void sample_rows_count_kernel(const int64_t *__restrict__ rowptr, int32_t n_rows,
+                                         const int32_t *__restrict__ rows, int32_t n_list, int k, double ratio,
+                                         int padding, int32_t *__restrict__ cnt, int32_t *__restrict__ n_bad) {
+    const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= n_list) return;
+    const int32_t r = rows[t];
+    int num = 0;
+    if (r < 0 || r >= n_rows) atomicAdd(n_bad, 1);
+    else sample_rule((int)(rowptr[r + 1] - rowptr[r]), k, ratio, padding, num);
+    cnt[t] = num;
+}
+
+__global__ void __launch_bounds__(kRowsPerCta)
+sample_rows_fill_kernel(const int64_t *__restrict__ rowptr, int32_t n_rows, const int32_t *__restrict__ rows,
+                        int32_t n_list, int k, double ratio, int padding, uint64_t seed, uint32_t stream,
+                        const int64_t *__restrict__ out_rowptr, int32_t *__restrict__ out_row,
+                        int32_t *__restrict__ out_pos) {
+    __shared__ int32_t long_rows[kRowsPerCta];
+    __shared__ int n_long;
+    if (threadIdx.x == 0) n_long = 0;
+    __syncthreads();
+    const int64_t t = (int64_t)blockIdx.x * kRowsPerCta + threadIdx.x;
+    if (t < n_list) {
+        const int32_t r = rows[t];
+        if (r >= 0 && r < n_rows) {
+            const int64_t start = rowptr[r];
+            const int deg = (int)(rowptr[r + 1] - start);
+            if (deg > kThreadRowMax) {
+                long_rows[atomicAdd(&n_long, 1)] = threadIdx.x;      // slot order is irrelevant: rows write disjoint ranges
+            } else {
+                int num;
+                const int rule = sample_rule(deg, k, ratio, padding, num);
+                const int64_t o = out_rowptr[t];
+                const uint64_t base = (uint64_t)r << 32;
+                if (out_row)
+                    for (int i = 0; i < num; ++i) out_row[o + i] = (int32_t)t;
+                if (rule == kSampleReplace) {
+                    for (int i = 0; i < num; ++i)
+                        out_pos[o + i] = (int32_t)(start + random_below(seed, stream, base + (uint64_t)i, (uint32_t)deg));
+                } else {
+                    for (int i = 0; i < num; ++i) out_pos[o + i] = (int32_t)(start + i);
+                    if (rule == kSampleReservoir)
+                        for (int i = num; i < deg; ++i) {
+                            const uint32_t j = random_below(seed, stream, base + (uint64_t)i, (uint32_t)(i + 1));
+                            if (j < (uint32_t)num) out_pos[o + j] = (int32_t)(start + i);
+                        }
+                }
+            }
+        }
+    }
+    __syncthreads();
+    const int nl = n_long;
+    // pass 1: row ids, kept and drawn-with-replacement positions, and the initial reservoir slots
+    for (int q = 0; q < nl; ++q) {
+        const int64_t tl = (int64_t)blockIdx.x * kRowsPerCta + long_rows[q];
+        const int32_t r = rows[tl];
+        const int64_t start = rowptr[r];
+        const int deg = (int)(rowptr[r + 1] - start);
+        int num;
+        const int rule = sample_rule(deg, k, ratio, padding, num);
+        const int64_t o = out_rowptr[tl];
+        const uint64_t base = (uint64_t)r << 32;
+        for (int i = threadIdx.x; i < num; i += kRowsPerCta) {
+            if (out_row) out_row[o + i] = (int32_t)tl;
+            out_pos[o + i] = (int32_t)(start + (rule == kSampleReplace
+                                                    ? random_below(seed, stream, base + (uint64_t)i, (uint32_t)deg) : i));
+        }
+    }
+    __syncthreads();                   // every slot holds start + j before any draw competes for it
+    // pass 2: the reservoir draws
+    for (int q = 0; q < nl; ++q) {
+        const int64_t tl = (int64_t)blockIdx.x * kRowsPerCta + long_rows[q];
+        const int32_t r = rows[tl];
+        const int64_t start = rowptr[r];
+        const int deg = (int)(rowptr[r + 1] - start);
+        int num;
+        if (sample_rule(deg, k, ratio, padding, num) != kSampleReservoir) continue;
+        const int64_t o = out_rowptr[tl];
+        const uint64_t base = (uint64_t)r << 32;
+        for (int i = num + threadIdx.x; i < deg; i += kRowsPerCta) {
+            const uint32_t j = random_below(seed, stream, base + (uint64_t)i, (uint32_t)(i + 1));
+            if (j < (uint32_t)num) atomicMax(out_pos + o + j, (int32_t)(start + i));
+        }
+    }
+}
+
+// ---- relabelling: an [N] id -> position map that is -1 everywhere outside a call --------------------------------
+enum { kBadIds = 0, kDupIds = 1, kNewIds = 2 };
+
+__global__ void node_scatter_kernel(const int32_t *__restrict__ nodes, int32_t n, int32_t N, int32_t *__restrict__ map,
+                                    int32_t *__restrict__ counters) {
+    for (int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; p < n; p += (int64_t)gridDim.x * blockDim.x) {
+        const int32_t id = nodes[p];
+        if (id < 0 || id >= N) atomicAdd(counters + kBadIds, 1);
+        else if (atomicCAS(map + id, -1, (int32_t)p) != -1) atomicAdd(counters + kDupIds, 1);
+    }
+}
+
+// reset the map entries of nodes[0, n + *extra)
+__global__ void node_reset_kernel(const int32_t *__restrict__ nodes, int64_t n, const int32_t *__restrict__ extra,
+                                  int32_t N, int32_t *__restrict__ map) {
+    const int64_t total = n + (extra ? *extra : 0);
+    for (int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; p < total; p += (int64_t)gridDim.x * blockDim.x) {
+        const int32_t id = nodes[p];
+        if (id >= 0 && id < N) map[id] = -1;
+    }
+}
+
+__global__ void reindex_gather_kernel(const int32_t *__restrict__ ids, int64_t n, int32_t N,
+                                      const int32_t *__restrict__ map, int32_t *__restrict__ out) {
+    for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < n; e += (int64_t)gridDim.x * blockDim.x) {
+        const int32_t id = ids[e];
+        out[e] = (id >= 0 && id < N) ? map[id] : -1;
+    }
+}
+
+// ids not yet in the map: map[id] = INT32_MIN + (first e holding id).  atomicMin keeps the smallest e whatever the
+// order, and INT32_MIN + e <= -2 stays below the -1 of an absent id and below every position.
+__global__ void frontier_first_kernel(const int32_t *__restrict__ cols, int64_t S, int32_t N, int32_t *__restrict__ map,
+                                      int32_t *__restrict__ counters) {
+    for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < S; e += (int64_t)gridDim.x * blockDim.x) {
+        const int32_t c = cols[e];
+        if (c < 0 || c >= N) atomicAdd(counters + kBadIds, 1);
+        else if (map[c] < 0) atomicMin(map + c, INT32_MIN + (int32_t)e);
+    }
+}
+
+__global__ void frontier_flag_kernel(const int32_t *__restrict__ cols, int64_t S, int32_t N,
+                                     const int32_t *__restrict__ map, int32_t *__restrict__ flag) {
+    for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < S; e += (int64_t)gridDim.x * blockDim.x) {
+        const int32_t c = cols[e];
+        flag[e] = (c >= 0 && c < N && map[c] == INT32_MIN + (int32_t)e) ? 1 : 0;
+    }
+}
+
+__global__ void frontier_emit_kernel(const int32_t *__restrict__ cols, int64_t S, const int32_t *__restrict__ flag,
+                                     const int32_t *__restrict__ off, int32_t n_nodes, int32_t *__restrict__ nodes,
+                                     int32_t *__restrict__ map) {
+    for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < S; e += (int64_t)gridDim.x * blockDim.x)
+        if (flag[e]) {
+            const int32_t pos = n_nodes + off[e];
+            nodes[pos] = cols[e];
+            map[cols[e]] = pos;
+        }
+}
+
 }  // namespace
 }  // namespace tfgk
 
@@ -202,6 +356,159 @@ int tfgk_neighbor_sample_fill(const int64_t *rowptr, int32_t n_rows, int32_t k, 
     sample_fill_kernel<<<(unsigned)ceil_div64(n_rows, 128), 128, 0, as_stream(stream)>>>(rowptr, n_rows, k, ratio, padding, seed,
                                                                                        rng_stream, out_rowptr, out_row, out_pos);
     TFGK_LAUNCH_CHECK();
+    return TFGK_OK;
+}
+
+int tfgk_neighbor_sample_rows_count(const int64_t *rowptr, int32_t n_rows, const int32_t *rows, int32_t n_list, int32_t k,
+                                    double ratio, int padding, int64_t *out_rowptr, int64_t *total_host, void *workspace,
+                                    size_t workspace_bytes, void *stream) {
+    int rc = check_sample_args("neighbor_sample_rows_count", n_list, k, ratio);
+    if (rc != TFGK_OK) return rc;
+    if ((rc = check_sample_mode("neighbor_sample_rows_count", k, ratio, padding)) != TFGK_OK) return rc;
+    TFGK_CHECK_ARG(n_rows >= 0, "neighbor_sample_rows_count: negative CSR row count");
+    TFGK_CHECK_ARG(total_host != nullptr && out_rowptr != nullptr, "neighbor_sample_rows_count: null pointer");
+    *total_host = 0;
+    cudaStream_t st = as_stream(stream);
+    if (n_list == 0) {
+        TFGK_CUDA(cudaMemsetAsync(out_rowptr, 0, 8, st));
+        return TFGK_OK;
+    }
+    TFGK_CHECK_ARG(rowptr != nullptr && rows != nullptr, "neighbor_sample_rows_count: null rowptr or row list");
+    size_t need = 0;
+    tfgk_neighbor_sample_workspace_bytes(n_list, &need);
+    if (workspace == nullptr || workspace_bytes < need)
+        return set_error(TFGK_ERR_WORKSPACE, "neighbor_sample_rows_count: workspace too small (%zu < %zu bytes)",
+                         workspace_bytes, need);
+    char *ws = static_cast<char *>(workspace);
+    int32_t *cnt = reinterpret_cast<int32_t *>(ws);
+    int64_t *sums = reinterpret_cast<int64_t *>(ws + align_up(((size_t)n_list + 1) * 4));
+    int32_t *n_bad = reinterpret_cast<int32_t *>(ws + need - 256);      // the workspace's last 256 bytes
+    TFGK_CUDA(cudaMemsetAsync(n_bad, 0, 4, st));
+    sample_rows_count_kernel<<<(unsigned)ceil_div64(n_list, 256), 256, 0, st>>>(rowptr, n_rows, rows, n_list, k, ratio,
+                                                                                padding, cnt, n_bad);
+    TFGK_LAUNCH_CHECK();
+    rc = exclusive_scan<int32_t, int64_t>(cnt, n_list, (int64_t)n_list + 1, out_rowptr, sums, st);
+    if (rc != TFGK_OK) return rc;
+    int32_t bad = 0;
+    TFGK_CUDA(cudaMemcpyAsync(total_host, out_rowptr + n_list, 8, cudaMemcpyDeviceToHost, st));
+    TFGK_CUDA(cudaMemcpyAsync(&bad, n_bad, 4, cudaMemcpyDeviceToHost, st));
+    TFGK_CUDA(cudaStreamSynchronize(st));
+    if (bad) {
+        *total_host = 0;
+        return set_error(TFGK_ERR_INDEX_OUT_OF_RANGE, "neighbor_sample_rows_count: %d listed rows outside [0, %d)", bad,
+                         n_rows);
+    }
+    TFGK_CHECK_ARG(*total_host < (1ll << 31) - 1, "neighbor_sample_rows_count: %lld sampled edges exceed int32 positions",
+                   (long long)*total_host);
+    return TFGK_OK;
+}
+
+int tfgk_neighbor_sample_rows_fill(const int64_t *rowptr, int32_t n_rows, const int32_t *rows, int32_t n_list, int32_t k,
+                                   double ratio, int padding, uint64_t seed, uint32_t rng_stream, const int64_t *out_rowptr,
+                                   int32_t *out_row, int32_t *out_pos, void *stream) {
+    int rc = check_sample_args("neighbor_sample_rows_fill", n_list, k, ratio);
+    if (rc != TFGK_OK) return rc;
+    if ((rc = check_sample_mode("neighbor_sample_rows_fill", k, ratio, padding)) != TFGK_OK) return rc;
+    if (n_list == 0) return TFGK_OK;
+    TFGK_CHECK_ARG(rowptr && rows && out_rowptr && out_pos, "neighbor_sample_rows_fill: null pointer");
+    sample_rows_fill_kernel<<<(unsigned)ceil_div64(n_list, kRowsPerCta), kRowsPerCta, 0, as_stream(stream)>>>(
+        rowptr, n_rows, rows, n_list, k, ratio, padding, seed, rng_stream, out_rowptr, out_row, out_pos);
+    TFGK_LAUNCH_CHECK();
+    return TFGK_OK;
+}
+
+int tfgk_relabel_workspace_bytes(int64_t n_ids, size_t *out_bytes) {
+    TFGK_CHECK_ARG(out_bytes != nullptr && n_ids >= 0 && n_ids < (1ll << 31) - 1, "relabel_workspace_bytes: bad argument");
+    *out_bytes = 2 * align_up((size_t)(n_ids + 1) * 4) + scan_scratch_bytes(n_ids + 1) + 256;
+    return TFGK_OK;
+}
+
+// the three counters live in the workspace's last 256 bytes
+static int read_counters(const int32_t *counters, int32_t *host, cudaStream_t st) {
+    TFGK_CUDA(cudaMemcpyAsync(host, counters, 3 * 4, cudaMemcpyDeviceToHost, st));
+    TFGK_CUDA(cudaStreamSynchronize(st));
+    return TFGK_OK;
+}
+
+int tfgk_reindex_i32(const int32_t *nodes, int32_t n_nodes, const int32_t *ids, int64_t n_ids, int32_t N, int32_t *map,
+                     int32_t *out, int32_t *n_dup_host, void *workspace, size_t workspace_bytes, void *stream) {
+    TFGK_CHECK_ARG(n_nodes >= 0 && n_ids >= 0 && N >= 0 && n_dup_host != nullptr, "reindex: bad argument");
+    *n_dup_host = 0;
+    if (n_nodes == 0 && n_ids == 0) return TFGK_OK;
+    TFGK_CHECK_ARG(map != nullptr && (n_nodes == 0 || nodes) && (n_ids == 0 || (ids && out)), "reindex: null pointer");
+    size_t need = 0;
+    tfgk_relabel_workspace_bytes(0, &need);
+    if (workspace == nullptr || workspace_bytes < need)
+        return set_error(TFGK_ERR_WORKSPACE, "reindex: workspace too small (%zu < %zu bytes)", workspace_bytes, need);
+    cudaStream_t st = as_stream(stream);
+    int32_t *counters = reinterpret_cast<int32_t *>(static_cast<char *>(workspace) + need - 256);
+    TFGK_CUDA(cudaMemsetAsync(counters, 0, 3 * 4, st));
+    if (n_nodes) {
+        node_scatter_kernel<<<grid_for(n_nodes), 256, 0, st>>>(nodes, n_nodes, N, map, counters);
+        TFGK_LAUNCH_CHECK();
+    }
+    if (n_ids) {
+        reindex_gather_kernel<<<grid_for(n_ids), 256, 0, st>>>(ids, n_ids, N, map, out);
+        TFGK_LAUNCH_CHECK();
+    }
+    if (n_nodes) {
+        node_reset_kernel<<<grid_for(n_nodes), 256, 0, st>>>(nodes, n_nodes, nullptr, N, map);
+        TFGK_LAUNCH_CHECK();
+    }
+    int32_t c[3];
+    int rc = read_counters(counters, c, st);
+    if (rc != TFGK_OK) return rc;
+    if (c[kBadIds]) return set_error(TFGK_ERR_INDEX_OUT_OF_RANGE, "reindex: %d node ids outside [0, %d)", c[kBadIds], N);
+    *n_dup_host = c[kDupIds];
+    return TFGK_OK;
+}
+
+int tfgk_frontier_i32(const int32_t *cols, int64_t S, int32_t N, int32_t *nodes, int32_t n_nodes, int32_t *map,
+                      int32_t *local_col, int32_t *n_new_host, int32_t *n_dup_host, void *workspace, size_t workspace_bytes,
+                      void *stream) {
+    TFGK_CHECK_ARG(S >= 0 && S < (1ll << 31) - 1 && n_nodes >= 0 && N >= 0 && (int64_t)n_nodes + S < (1ll << 31) - 1,
+                   "frontier: bad size");
+    TFGK_CHECK_ARG(n_new_host != nullptr && n_dup_host != nullptr, "frontier: null count");
+    *n_new_host = 0;
+    *n_dup_host = 0;
+    if (n_nodes == 0 && S == 0) return TFGK_OK;
+    TFGK_CHECK_ARG(map && nodes && (S == 0 || (cols && local_col)), "frontier: null pointer");
+    size_t need = 0;
+    tfgk_relabel_workspace_bytes(S, &need);
+    if (workspace == nullptr || workspace_bytes < need)
+        return set_error(TFGK_ERR_WORKSPACE, "frontier: workspace too small (%zu < %zu bytes)", workspace_bytes, need);
+    cudaStream_t st = as_stream(stream);
+    char *ws = static_cast<char *>(workspace);
+    int32_t *flag = reinterpret_cast<int32_t *>(ws);
+    int32_t *off = reinterpret_cast<int32_t *>(ws + align_up((size_t)(S + 1) * 4));
+    int32_t *sums = reinterpret_cast<int32_t *>(ws + 2 * align_up((size_t)(S + 1) * 4));
+    int32_t *counters = reinterpret_cast<int32_t *>(ws + need - 256);
+    TFGK_CUDA(cudaMemsetAsync(counters, 0, 3 * 4, st));
+    if (n_nodes) {
+        node_scatter_kernel<<<grid_for(n_nodes), 256, 0, st>>>(nodes, n_nodes, N, map, counters);
+        TFGK_LAUNCH_CHECK();
+    }
+    if (S) {
+        frontier_first_kernel<<<grid_for(S), 256, 0, st>>>(cols, S, N, map, counters);
+        TFGK_LAUNCH_CHECK();
+        frontier_flag_kernel<<<grid_for(S), 256, 0, st>>>(cols, S, N, map, flag);
+        TFGK_LAUNCH_CHECK();
+        int rc = exclusive_scan<int32_t, int32_t>(flag, S, S + 1, off, sums, st);
+        if (rc != TFGK_OK) return rc;
+        frontier_emit_kernel<<<grid_for(S), 256, 0, st>>>(cols, S, flag, off, n_nodes, nodes, map);
+        TFGK_LAUNCH_CHECK();
+        reindex_gather_kernel<<<grid_for(S), 256, 0, st>>>(cols, S, N, map, local_col);
+        TFGK_LAUNCH_CHECK();
+        TFGK_CUDA(cudaMemcpyAsync(counters + kNewIds, off + S, 4, cudaMemcpyDeviceToDevice, st));
+    }
+    node_reset_kernel<<<grid_for((int64_t)n_nodes + S), 256, 0, st>>>(nodes, n_nodes, S ? off + S : nullptr, N, map);
+    TFGK_LAUNCH_CHECK();
+    int32_t c[3];
+    int rc = read_counters(counters, c, st);
+    if (rc != TFGK_OK) return rc;
+    if (c[kBadIds]) return set_error(TFGK_ERR_INDEX_OUT_OF_RANGE, "frontier: %d node ids outside [0, %d)", c[kBadIds], N);
+    *n_dup_host = c[kDupIds];
+    *n_new_host = c[kNewIds];
     return TFGK_OK;
 }
 

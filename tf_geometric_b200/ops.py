@@ -871,6 +871,12 @@ def stable_argsort(keys, key_bits=32):
     return perm
 
 
+def _padding_code(padding):
+    if padding == "head" or (not isinstance(padding, bool) and padding == SAMPLE_HEAD):
+        return SAMPLE_HEAD
+    return SAMPLE_PADDING if padding else SAMPLE_NO_PADDING
+
+
 def neighbor_sample(csr, k=None, ratio=None, padding=False, seed=0, rng_stream=RNG_STREAM_SAMPLER):
     """Fan-out sampling over the rows of `csr` (tfgk_neighbor_sample_*).  Returns (row int32 [S], pos int32 [S],
     out_rowptr int64 [n_rows+1]): the row of every sampled edge and the CSR position it was drawn from.
@@ -878,10 +884,7 @@ def neighbor_sample(csr, k=None, ratio=None, padding=False, seed=0, rng_stream=R
     dev = csr.rowptr.device
     kk = -1 if k is None else int(k)
     rr = -1.0 if ratio is None else float(ratio)
-    if padding == "head" or (not isinstance(padding, bool) and padding == SAMPLE_HEAD):
-        padding = SAMPLE_HEAD
-    else:
-        padding = SAMPLE_PADDING if padding else SAMPLE_NO_PADDING
+    padding = _padding_code(padding)
     need = ctypes.c_size_t()
     _ffi.call("tfgk_neighbor_sample_workspace_bytes", csr.n_rows, ctypes.byref(need))
     ws = torch.empty((max(need.value, 1),), dtype=torch.uint8, device=dev)
@@ -896,6 +899,70 @@ def neighbor_sample(csr, k=None, ratio=None, padding=False, seed=0, rng_stream=R
         _ffi.call("tfgk_neighbor_sample_fill", _p(csr.rowptr), csr.n_rows, kk, rr, padding, int(seed),
                   int(rng_stream), _p(out_rowptr), _p(out_row), _p(out_pos), _stream(out_rowptr))
     return out_row, out_pos, out_rowptr
+
+
+def neighbor_sample_rows(rowptr, rows, k=None, ratio=None, padding=False, seed=0, rng_stream=RNG_STREAM_SAMPLER):
+    """K13: fan-out sampling of the listed rows of a CSR (tfgk_neighbor_sample_rows_*).  rowptr int64 [n_rows+1] is read in
+    place; rows int32 [R] are global row ids (repeats allowed).  Returns (list position of each sampled edge's row int32 [S],
+    CSR position int32 [S], out_rowptr int64 [R+1]); row t's positions are the ones neighbor_sample draws for row rows[t]."""
+    _check(rowptr, torch.int64, "rowptr")
+    _check(rows, torch.int32, "rows")
+    dev = rowptr.device
+    n_rows, R = rowptr.numel() - 1, rows.numel()
+    kk = -1 if k is None else int(k)
+    rr = -1.0 if ratio is None else float(ratio)
+    padding = _padding_code(padding)
+    need = ctypes.c_size_t()
+    _ffi.call("tfgk_neighbor_sample_workspace_bytes", R, ctypes.byref(need))
+    ws = torch.empty((max(need.value, 1),), dtype=torch.uint8, device=dev)
+    out_rowptr = torch.empty((R + 1,), dtype=torch.int64, device=dev)
+    total = ctypes.c_int64()
+    _ffi.call("tfgk_neighbor_sample_rows_count", _p(rowptr), n_rows, _p(rows), R, kk, rr, padding, _p(out_rowptr),
+              ctypes.byref(total), _p(ws), need.value, _stream(rowptr))
+    S = total.value
+    out_row = torch.empty((S,), dtype=torch.int32, device=dev)
+    out_pos = torch.empty((S,), dtype=torch.int32, device=dev)
+    if S:
+        _ffi.call("tfgk_neighbor_sample_rows_fill", _p(rowptr), n_rows, _p(rows), R, kk, rr, padding, int(seed),
+                  int(rng_stream), _p(out_rowptr), _p(out_row), _p(out_pos), _stream(rowptr))
+    return out_row, out_pos, out_rowptr
+
+
+def _relabel_workspace(n, device):
+    need = ctypes.c_size_t()
+    _ffi.call("tfgk_relabel_workspace_bytes", n, ctypes.byref(need))
+    return torch.empty((need.value,), dtype=torch.uint8, device=device), need.value
+
+
+def reindex(nodes, ids, node_map):
+    """Position of every id of `ids` in the list `nodes` (-1 when absent), through `node_map` (int32 [N], all -1 before
+    and after).  Returns (positions int32 [n_ids], number of repeated entries in `nodes`)."""
+    _check(nodes, torch.int32, "nodes")
+    _check(ids, torch.int32, "ids")
+    _check(node_map, torch.int32, "node_map")
+    out = torch.empty((ids.numel(),), dtype=torch.int32, device=ids.device)
+    ws, nbytes = _relabel_workspace(0, ids.device)
+    n_dup = ctypes.c_int32()
+    _ffi.call("tfgk_reindex_i32", _p(nodes), nodes.numel(), _p(ids), ids.numel(), node_map.numel(), _p(node_map), _p(out),
+              ctypes.byref(n_dup), _p(ws), nbytes, _stream(ids))
+    return out, n_dup.value
+
+
+def frontier(nodes, n_nodes, cols, node_map):
+    """Grow the node list nodes[:n_nodes] (int32, room for cols.numel() more) by the ids of `cols` it lacks, in
+    first-occurrence order, and relabel `cols` into it.  Returns (local cols int32 [S], new ids, repeated list entries)."""
+    _check(nodes, torch.int32, "nodes")
+    _check(cols, torch.int32, "cols")
+    _check(node_map, torch.int32, "node_map")
+    S = cols.numel()
+    if nodes.numel() < n_nodes + S:
+        raise ValueError("frontier: the node buffer holds {} ids, {} needed".format(nodes.numel(), n_nodes + S))
+    local = torch.empty((S,), dtype=torch.int32, device=cols.device)
+    ws, nbytes = _relabel_workspace(S, cols.device)
+    n_new, n_dup = ctypes.c_int32(), ctypes.c_int32()
+    _ffi.call("tfgk_frontier_i32", _p(cols), S, node_map.numel(), _p(nodes), int(n_nodes), _p(node_map), _p(local),
+              ctypes.byref(n_new), ctypes.byref(n_dup), _p(ws), nbytes, _stream(cols))
+    return local, n_new.value, n_dup.value
 
 
 # ---- link prediction: K6 edge scoring, negative sampling ----------------------------------------------------------

@@ -527,5 +527,89 @@ def convert_x_to_3d(x, source_index, k=None, pad=True):
     return autograd.PadRows.apply(x, csr, int(k), False, None)
 
 
+# ---- sampled-subgraph helpers (reference :455-485, :538-551, :946-975) --------------------------------------------
+
+def reindex_sampled_edge_index(sampled_edge_index, sampled_node_index):
+    """Every id of sampled_edge_index replaced by its position in sampled_node_index, -1 for ids not in it (the
+    reference's StaticHashTable with default_value=-1).  Duplicate ids in sampled_node_index raise ValueError, as TF's
+    table refuses duplicate keys.  Device tensors run tfgk_reindex_i32; the int32 result is in the container of
+    sampled_edge_index."""
+    if _is_device(sampled_edge_index):
+        ei = sampled_edge_index.to(torch.int32).contiguous()
+        nodes = ops.as_device(sampled_node_index, torch.int32, device=ei.device).reshape(-1).contiguous()
+        if nodes.numel() and int(nodes.min()) < 0:
+            raise ValueError("sampled_node_index holds negative ids")
+        top = torch.cat([ei.reshape(-1), nodes]).max() if ei.numel() + nodes.numel() else None
+        N = 0 if top is None else max(int(top) + 1, 0)
+        node_map = torch.full((N,), -1, dtype=torch.int32, device=ei.device)
+        out, n_dup = ops.reindex(nodes, ei.reshape(-1), node_map)
+        if n_dup:
+            raise ValueError("sampled_node_index holds {} duplicate ids".format(n_dup))
+        return out.reshape(ei.shape)
+    ei = np.asarray(_to_numpy(sampled_edge_index)).astype(np.int64)
+    nodes = np.asarray(_to_numpy(sampled_node_index)).astype(np.int64).reshape(-1)
+    order = np.argsort(nodes, kind="stable")
+    ordered = nodes[order]
+    if len(ordered) > 1 and np.any(ordered[1:] == ordered[:-1]):
+        raise ValueError("sampled_node_index holds duplicate ids")
+    at = np.clip(np.searchsorted(ordered, ei), 0, max(len(ordered) - 1, 0))
+    found = (ordered[at] == ei) if len(ordered) else np.zeros(ei.shape, bool)
+    out = np.where(found, order[at] if len(ordered) else -1, -1).astype(np.int32)
+    return _like(out, sampled_edge_index, torch.int32)
+
+
+def compute_edge_mask_by_node_index(edge_index, node_index):
+    """bool [E]: both ends of the edge are in node_index (reference :538-551).  Device tensors: the node set becomes an
+    [N] map and tfgk_edge_flags_i32 tests both ends."""
+    if _is_device(edge_index):
+        ei = edge_index.to(torch.int32).contiguous()
+        nodes = ops.as_device(node_index, torch.int32, device=ei.device).reshape(-1)
+        E = ei.shape[1]
+        N = int(torch.cat([ei.reshape(-1), nodes]).max()) + 1 if E + nodes.numel() else 0
+        node_map, _ = _sampling._virtual_mapping(nodes, N, ei.device)
+        flag = ops.edge_flags(ei[0].contiguous(), ei[1].contiguous(), E, mode=ops.FLAG_MAPPED, row_map=node_map,
+                              col_map=node_map)
+        return flag.to(torch.bool)
+    ei = np.asarray(_to_numpy(edge_index)).astype(np.int64)
+    nodes = np.asarray(_to_numpy(node_index)).astype(np.int64).reshape(-1)
+    n = int(max(ei.max(initial=-1), nodes.max(initial=-1))) + 1
+    node_mask = np.zeros(n, bool)
+    node_mask[nodes] = True
+    return node_mask[ei[0]] & node_mask[ei[1]]
+
+
+def extract_unique_edge(edge_index, edge_weight=None, mode="undirected"):
+    """The first occurrence of every edge, in edge order, with its weight (reference :455-485); mode "undirected"
+    compares the ends as a sorted pair, any other mode as an ordered one.  Kept edges keep their orientation.  Device
+    tensors: tfgk_edge_unique over the (sorted) pairs; each container follows its input."""
+    if _is_device(edge_index):
+        ei = edge_index.to(torch.int32).contiguous()
+        row, col = ei[0].contiguous(), ei[1].contiguous()
+        E = row.numel()
+        keep = torch.empty((0,), dtype=torch.int32, device=ei.device)
+        if E:
+            if mode == "undirected":
+                row, col = torch.minimum(row, col).contiguous(), torch.maximum(row, col).contiguous()
+            uniq, of_edge = ops.edge_unique(row, col, int(ei.max()) + 1)
+            first = torch.full((uniq.shape[1],), E, dtype=torch.int64, device=ei.device)
+            first.scatter_reduce_(0, of_edge.long(), torch.arange(E, device=ei.device), reduce="amin")
+            keep = first.to(torch.int32)
+        out_index = torch.stack([ops.gather_i32(ei[0].contiguous(), keep), ops.gather_i32(ei[1].contiguous(), keep)])
+    else:
+        ei = np.asarray(_to_numpy(edge_index)).astype(np.int32).reshape(2, -1)
+        pairs = np.sort(ei, axis=0) if mode == "undirected" else ei
+        h = pairs[0].astype(np.int64) * (int(ei.max(initial=0)) + 1) + pairs[1]
+        _, keep = np.unique(h, return_index=True)
+        keep = np.sort(keep)
+        out_index = _like(ei[:, keep], edge_index, torch.int32)
+    if edge_weight is None:
+        return out_index, None
+    if _is_device(edge_index):
+        out_w = ops.permute(ops.as_device(edge_weight, torch.float32, device=keep.device).reshape(-1), keep)
+        return out_index, (out_w if _is_device(edge_weight) else out_w.cpu().numpy())
+    return out_index, _like(np.asarray(_to_numpy(edge_weight), np.float32).reshape(-1)[keep], edge_weight, torch.float32)
+
+
 # samplers live in utils/sampling.py; re-exported here because the reference defines them in this module (:630-846)
-from .sampling import RandomNeighborSampler, UniformNeighborSampler  # noqa: E402,F401
+from . import sampling as _sampling  # noqa: E402
+from .sampling import RandomNeighborSampler, UniformNeighborSampler, SampledNeighborhood  # noqa: E402,F401

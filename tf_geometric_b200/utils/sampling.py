@@ -4,7 +4,11 @@
 RandomNeighborSampler: the reference keeps a Python dict of neighbour arrays and loops over every node calling
 np.random.choice (the bottleneck of demo/demo_graph_sage.py:53-55); here the dict is the stable row-sorted CSR and the
 loop is one thread per row (tfgk_neighbor_sample_*).  UniformNeighborSampler: a Bernoulli flag per edge + compaction.
-Randomness is counter-based (csrc/rng.cuh); pass `seed=` for reproducible draws."""
+Randomness is counter-based (csrc/rng.cuh); pass `seed=` for reproducible draws.
+
+RandomNeighborSampler.sample_neighborhood (an extension of the reference API) grows a seed-node mini-batch hop by hop
+on the device: K13 samples the listed rows of the cached CSR and tfgk_frontier_i32 appends and relabels the new nodes, so
+the work follows the batch, not the graph."""
 import torch
 
 from .. import ops, _rng
@@ -64,6 +68,23 @@ class _SamplerBase(object):
         return v_row, v_col, ops.permute(self.edge_weight, index), n_vr, n_vc
 
 
+class SampledNeighborhood(object):
+    """A seed-node mini-batch (RandomNeighborSampler.sample_neighborhood).
+
+    node_index: int32 [n] global ids; the seeds first, then every node reached, in first-occurrence order.
+    edge_index_list / edge_weight_list: one edge list per layer, layer 0 nearest the input; rows and columns are positions
+        in node_index.  Layer i's rows lie in node_index[:hop_sizes[-2 - i]] (the nodes whose neighbours it drew).
+    hop_sizes: [number of seeds, list length after hop 1, ..., after the last hop] (the last one is n)."""
+
+    __slots__ = ("node_index", "edge_index_list", "edge_weight_list", "hop_sizes")
+
+    def __init__(self, node_index, edge_index_list, edge_weight_list, hop_sizes):
+        self.node_index = node_index
+        self.edge_index_list = edge_index_list
+        self.edge_weight_list = edge_weight_list
+        self.hop_sizes = hop_sizes
+
+
 class RandomNeighborSampler(_SamplerBase):
     """Per-node fan-out sampling (graph_utils.py:630-776)."""
 
@@ -71,6 +92,8 @@ class RandomNeighborSampler(_SamplerBase):
         super().__init__(edge_index, edge_weight)
         self._csr = None
         self._w_csr = None
+        self._rowptr_all = None
+        self._node_map = None
 
     def _structure(self):
         if self._csr is None:
@@ -102,6 +125,64 @@ class RandomNeighborSampler(_SamplerBase):
         if out_row.numel() == 0:
             return None, None
         return torch.stack([out_row, ops.gather_i32(csr.col, out_pos)]), ops.permute(w_csr, out_pos)
+
+    def _neighborhood_structure(self):
+        """The cached CSR with one row per node id (ids past the last source row have no neighbours), and the [N] id ->
+        position map of the relabelling kernels, which is -1 everywhere between calls."""
+        csr, w_csr = self._structure()
+        if self._node_map is None:
+            n = max(self.num_row_nodes, self.num_col_nodes)
+            rowptr = csr.rowptr
+            if n > csr.n_rows:
+                rowptr = torch.cat([rowptr, rowptr[-1:].expand(n - csr.n_rows)])
+            self._rowptr_all = rowptr
+            self._node_map = torch.full((n,), -1, dtype=torch.int32, device=rowptr.device)
+        return csr, w_csr, self._rowptr_all, self._node_map
+
+    def sample_neighborhood(self, seed_node_index, fanouts, padding=False, seed=None):
+        """Seed-node mini-batch sampling (an extension of the reference API).
+
+        Hop h draws fanouts[-1 - h] neighbours (by sample()'s k rule and `padding`) for EVERY node already in the list, so
+        one index space serves all layers; a node's draw depends only on the node and the hop's key, which is derived
+        from `seed` and h.  The new nodes are appended in the order the sampled edges first reach them.
+        Calls on one sampler must be ordered on one CUDA stream (they share the relabelling map).
+
+        :param seed_node_index: distinct node ids (numpy, list or tensor); duplicates raise ValueError
+        :param fanouts: neighbours per node for each layer, layer 0 nearest the input: sampling starts with fanouts[-1]
+        :return: SampledNeighborhood, on the device
+        """
+        from .graph_utils import _batch_seed         # graph_utils imports this module
+        seed = _rng.resolve_host(seed)
+        csr, w_csr, rowptr, node_map = self._neighborhood_structure()
+        dev = rowptr.device
+        N = node_map.numel()
+        nodes = ops.as_device(seed_node_index, torch.int32, device=dev).reshape(-1).contiguous()
+        if nodes.numel():
+            lo, hi = torch.aminmax(nodes)
+            if int(lo) < 0 or int(hi) >= N:
+                raise ValueError("seed_node_index holds node ids outside [0, {})".format(N))
+        _, n_dup = ops.reindex(nodes, nodes[:0], node_map)
+        if n_dup:
+            raise ValueError("seed_node_index holds {} duplicate node ids".format(n_dup))
+        n = nodes.numel()
+        hop_sizes, hop_edges, hop_weights = [n], [], []
+        for h, k in enumerate(reversed(list(fanouts))):
+            out_row, out_pos, _ = ops.neighbor_sample_rows(rowptr, nodes[:n], k=None if k is None else int(k),
+                                                           padding=padding, seed=_batch_seed(seed, h))
+            S = out_pos.numel()
+            grown = torch.empty((n + S,), dtype=torch.int32, device=dev)
+            grown[:n].copy_(nodes[:n])
+            if S:
+                local, n_new, _ = ops.frontier(grown, n, ops.gather_i32(csr.col, out_pos), node_map)
+                weight = ops.permute(w_csr, out_pos)
+            else:
+                local, n_new = out_pos, 0
+                weight = torch.empty((0,), dtype=torch.float32, device=dev)
+            hop_edges.append(torch.stack([out_row, local]))
+            hop_weights.append(weight)
+            nodes, n = grown, n + n_new
+            hop_sizes.append(n)
+        return SampledNeighborhood(nodes[:n], hop_edges[::-1], hop_weights[::-1], hop_sizes)
 
 
 class UniformNeighborSampler(_SamplerBase):
