@@ -86,6 +86,11 @@ int tfgk_csr_workspace_bytes(int64_t E, int32_t N, size_t *out_bytes);
 int tfgk_csr_build(const int32_t *row, const int32_t *col, int64_t E, int32_t N_rows, int32_t N_cols,
                    int64_t *rowptr, int32_t *col_sorted, int32_t *perm,
                    void *workspace, size_t workspace_bytes, void *stream);
+/* The same CSR without the id check, so without its synchronisation: for edge lists whose ids are in range by
+ * construction (a sampled block's transposed structure).  An id outside the range is undefined behaviour. */
+int tfgk_csr_build_in_range(const int32_t *row, const int32_t *col, int64_t E, int32_t N_rows, int32_t N_cols,
+                            int64_t *rowptr, int32_t *col_sorted, int32_t *perm,
+                            void *workspace, size_t workspace_bytes, void *stream);
 
 /* utils/graph_utils.py:67-125 merge_duplicated_edge, index half: duplicates of (row, col) collapse onto their FIRST occurrence
  * (tf.unique order on the hash num_nodes*row + col, num_nodes = N).  unique_index is [2, E] row-major with the first
@@ -541,6 +546,41 @@ int tfgk_reindex_i32(const int32_t *nodes, int32_t n_nodes, const int32_t *ids, 
 int tfgk_frontier_i32(const int32_t *cols, int64_t S, int32_t N, int32_t *nodes, int32_t n_nodes, int32_t *map,
                       int32_t *local_col, int32_t *n_new_host, int32_t *n_dup_host, void *workspace, size_t workspace_bytes,
                       void *stream);
+
+/* Block sampler: the mini-batch neighbourhood of tfgk_neighbor_sample_rows_* + tfgk_frontier_i32, with every size kept on
+ * the device so that a batch synchronises once, at its end.  Bit for bit, the node list and every hop's edges are those
+ * of the K13 + frontier route with the same keys (hop h samples every listed row, new ids are appended in first-occurrence
+ * order).  state is int32 [4 + 2 L] for L hops: [0] seeds outside [0, N), [1] repeated seeds, [2] unused,
+ * [3 + h] list length after hop h (h = 0: the seeds), [4 + L + h] edges of hop h.  map is the relabelling map of
+ * tfgk_frontier_i32 (-1 everywhere before begin and after end); it stays populated across the hops of a batch.  Calls
+ * of one batch must be ordered on one stream.
+ * _begin: nodes[0, n_seeds) = seeds, map[seed] = position, the seed counters; reads nothing back.
+ * _count: K13's count and scan for hop `hop` (< n_hops, the L of state) over cap_list >= the list length (read from
+ *   state): out_rowptr int64 [cap_list + 1], zero-count rows past the list, so out_rowptr[cap_list] is the hop's edge
+ *   total.  Asynchronous.
+ * A batch that fails between _begin and _end leaves the map populated: the caller resets it (ops.block_sample does).
+ * _read_total: the list length and out_rowptr[cap_list] to the host (synchronises); the fallback for hops whose edge
+ *   capacity is unknown (every neighbour) or not below 2^31.
+ * _fill: K13's fill (out_row = list position, out_gcol = col[pos], out_w = w_csr[pos]; cap_edges >= the edge total),
+ *   then the frontier: new ids appended to nodes (room for them is the caller's), out_local = position of out_gcol in
+ *   the grown list, and state's sizes for the hop.  Asynchronous.  The workspace is that of
+ *   tfgk_block_sample_workspace_bytes(cap_list, cap_edges), shared with _count.
+ * _end: resets map over the final list (cap_nodes >= its length), then copies state to state_host and synchronises. */
+int tfgk_block_sample_workspace_bytes(int32_t cap_list, int64_t cap_edges, size_t *out_bytes);
+int tfgk_block_sample_begin(const int32_t *seeds, int32_t n_seeds, int32_t N, int32_t *nodes, int32_t *map,
+                            int32_t *state, int32_t n_hops, void *stream);
+int tfgk_block_sample_count(const int64_t *rowptr, int32_t n_rows, const int32_t *nodes, const int32_t *state,
+                            int32_t hop, int32_t n_hops, int32_t cap_list, int32_t k, int padding, int64_t *out_rowptr,
+                            void *workspace, size_t workspace_bytes, void *stream);
+int tfgk_block_sample_read_total(const int32_t *state, int32_t hop, const int64_t *out_rowptr, int32_t cap_list,
+                                 int32_t *n_list_host, int64_t *total_host, void *stream);
+int tfgk_block_sample_fill(const int64_t *rowptr, int32_t n_rows, const int32_t *col, const float *w_csr, int32_t N,
+                           int32_t *nodes, int32_t *map, int32_t *state, int32_t hop, int32_t n_hops, int32_t cap_list,
+                           int64_t cap_edges, int32_t k, int padding, uint64_t seed, uint32_t rng_stream,
+                           const int64_t *out_rowptr, int32_t *out_row, int32_t *out_local, int32_t *out_gcol,
+                           float *out_w, void *workspace, size_t workspace_bytes, void *stream);
+int tfgk_block_sample_end(const int32_t *nodes, int32_t cap_nodes, int32_t N, int32_t *map, const int32_t *state,
+                          int32_t n_hops, int32_t *state_host, void *stream);
 
 /* ---- link prediction (SURVEY.md 8(f)5, demo/demo_gae.py) -------------------------------------------------------- */
 

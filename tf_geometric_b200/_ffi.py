@@ -41,6 +41,7 @@ SIGNATURES = {
     "tfgk_segment_count_i32": [_ptr, _i64, _i32, _ptr, _ptr],
     "tfgk_csr_workspace_bytes": [_i64, _i32, ctypes.POINTER(_size)],
     "tfgk_csr_build": [_ptr, _ptr, _i64, _i32, _i32, _ptr, _ptr, _ptr, _ptr, _size, _ptr],
+    "tfgk_csr_build_in_range": [_ptr, _ptr, _i64, _i32, _i32, _ptr, _ptr, _ptr, _ptr, _size, _ptr],
     "tfgk_edge_unique_workspace_bytes": [_i64, _i32, ctypes.POINTER(_size)],
     "tfgk_edge_unique": [_ptr, _ptr, _i64, _i32, _ptr, _ptr, ctypes.POINTER(_i32), _ptr, _size, _ptr],
     "tfgk_directed_workspace_bytes": [_i64, ctypes.POINTER(_size)],
@@ -126,6 +127,13 @@ SIGNATURES = {
     "tfgk_reindex_i32": [_ptr, _i32, _ptr, _i64, _i32, _ptr, _ptr, ctypes.POINTER(_i32), _ptr, _size, _ptr],
     "tfgk_frontier_i32": [_ptr, _i64, _i32, _ptr, _i32, _ptr, _ptr, ctypes.POINTER(_i32), ctypes.POINTER(_i32), _ptr, _size,
                           _ptr],
+    "tfgk_block_sample_workspace_bytes": [_i32, _i64, ctypes.POINTER(_size)],
+    "tfgk_block_sample_begin": [_ptr, _i32, _i32, _ptr, _ptr, _ptr, _i32, _ptr],
+    "tfgk_block_sample_count": [_ptr, _i32, _ptr, _ptr, _i32, _i32, _i32, _i32, _int, _ptr, _ptr, _size, _ptr],
+    "tfgk_block_sample_read_total": [_ptr, _i32, _ptr, _i32, ctypes.POINTER(_i32), ctypes.POINTER(_i64), _ptr],
+    "tfgk_block_sample_fill": [_ptr, _i32, _ptr, _ptr, _i32, _ptr, _ptr, _ptr, _i32, _i32, _i32, _i64, _i32, _int, _u64,
+                               _u32, _ptr, _ptr, _ptr, _ptr, _ptr, _ptr, _size, _ptr],
+    "tfgk_block_sample_end": [_ptr, _i32, _i32, _ptr, _ptr, _i32, _ptr, _ptr],
     "tfgk_edge_dot_f32": [_ptr, _i64, _i32, _ptr, _ptr, _i64, _i32, _ptr, _ptr],
     "tfgk_neg_offsets_workspace_bytes": [_i32, ctypes.POINTER(_size)],
     "tfgk_neg_offsets": [_ptr, _i32, _int, _ptr, ctypes.POINTER(_i64), _ptr, _size, _ptr],
@@ -262,6 +270,9 @@ NOT_CAPTURABLE = {
     "tfgk_neighbor_sample_rows_fill": ("the mini-batch neighbourhood sampler", "it takes a host-side key"),
     "tfgk_reindex_i32": ("reindex_sampled_edge_index", "it returns the number of duplicate node ids to the host"),
     "tfgk_frontier_i32": ("the mini-batch neighbourhood sampler", "it returns the number of new nodes to the host"),
+    "tfgk_block_sample_read_total": ("the block sampler", "it returns a hop's edge total to the host"),
+    "tfgk_block_sample_fill": ("the block sampler", "it takes a host-side key"),
+    "tfgk_block_sample_end": ("the block sampler", "it returns the batch's sizes to the host"),
     "tfgk_neg_offsets": ("negative sampling", "it returns the number of candidate pairs to the host"),
     "tfgk_neg_draw": ("negative sampling", "it takes a host-side key"),
     "tfgk_neg_sample_start": ("negative sampling", "it takes a host-side key"),

@@ -549,6 +549,19 @@ def run_lstm_fp32(module, inputs):
         return module(inputs)[0]
 
 
+def _pair_project(x, agg, ws, wn, b, act_code, concat):
+    """act([x Ws || agg Wn] + b) or act(x Ws + agg Wn + b), both products written straight into the output."""
+    u = ws.shape[1]
+    if concat:
+        out = torch.empty((x.shape[0], u + wn.shape[1]), dtype=torch.float32, device=x.device)
+        ops.gemm(x, ws, bias=None if b is None else b[:u].contiguous(), act=act_code, out=out[:, :u])
+        ops.gemm(agg, wn, bias=None if b is None else b[u:].contiguous(), act=act_code, out=out[:, u:])
+    else:
+        out = ops.gemm(x, ws)
+        ops.gemm(agg, wn, bias=b, act=act_code, beta=1.0, out=out)
+    return out
+
+
 class SagePair(torch.autograd.Function):
     """mean / sum GraphSAGE (nn/conv/graph_sage.py:9-115) as ONE differentiable op:
         out = act([x Ws || agg Wn] + b)   (or x Ws + agg Wn + b),   agg = REDUCE_{e: row_e = r} w_e x[col_e].
@@ -565,14 +578,7 @@ class SagePair(torch.autograd.Function):
         xd, wsd, wnd = x.detach(), ws.detach(), wn.detach()
         b = None if bias is None else bias.detach()
         agg = ops.spmm(csr, w_csr, xd, reduce=reduce)
-        u = wsd.shape[1]
-        if concat:
-            out = torch.empty((n, u + wnd.shape[1]), dtype=torch.float32, device=xd.device)
-            ops.gemm(xd, wsd, bias=None if b is None else b[:u].contiguous(), act=act_code, out=out[:, :u])
-            ops.gemm(agg, wnd, bias=None if b is None else b[u:].contiguous(), act=act_code, out=out[:, u:])
-        else:
-            out = ops.gemm(xd, wsd)
-            ops.gemm(agg, wnd, bias=b, act=act_code, beta=1.0, out=out)
+        out = _pair_project(xd, agg, wsd, wnd, b, act_code, concat)
         ctx.save_for_backward(x, ws, wn, agg, out if act_code == ops.ACT_RELU else None)
         ctx.meta = (edge_index, edge_weight, reduce, act_code, concat, csr, bias is not None)
         return out
@@ -600,6 +606,94 @@ class SagePair(torch.autograd.Function):
         if has_bias and ctx.needs_input_grad[3]:
             grad_b = ops.colsum(gm)
         return grad_x, grad_ws, grad_wn, grad_b, None, None, None, None, None
+
+
+class BlockSagePair(torch.autograd.Function):
+    """SagePair over a sampled block (utils.sampling.Block): out = act([x_self Ws || agg Wn] + b) with num_dst rows, agg
+    = REDUCE over block.csr of the block's weighted rows of x.  Without `self_index`, x is the block's [num_src, F] input
+    and x_self its first num_dst rows (a view).  With `self_index` (the SourceRows route), x is the global feature table,
+    the aggregate reads it through block.global_col, x_self = x[self_index] is gathered, and x gets no gradient.
+    Backward: dX_src = K1 over the block's transposed CSR into num_src rows, plus dX_self added into the first num_dst
+    rows by the GEMM's beta = 1 epilogue."""
+
+    @staticmethod
+    def forward(ctx, x, ws, wn, bias, block, reduce, act_code, concat, self_index):
+        xd, wsd, wnd = x.detach(), ws.detach(), wn.detach()
+        b = None if bias is None else bias.detach()
+        if self_index is None:
+            agg = ops.spmm(block.csr, block.edge_weight, xd, reduce=reduce)
+            x_self = xd[:block.num_dst]
+        else:
+            agg = ops.spmm(block.csr, block.edge_weight, xd, reduce=reduce, col=block.global_col)
+            x_self = ops.permute(xd, self_index)
+        out = _pair_project(x_self, agg, wsd, wnd, b, act_code, concat)
+        ctx.save_for_backward(x_self, ws, wn, agg, out if act_code == ops.ACT_RELU else None)
+        ctx.meta = (block, reduce, act_code, concat, bias is not None)
+        return out
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        x_self, ws, wn, agg, out = ctx.saved_tensors
+        block, reduce, act_code, concat, has_bias = ctx.meta
+        gm = grad_out.contiguous()
+        if act_code == ops.ACT_RELU:
+            gm = _relu_grad(gm, out)
+        u = ws.shape[1]
+        gs, gn = (gm[:, :u], gm[:, u:]) if concat else (gm, gm)
+        wsd, wnd = ws.detach(), wn.detach()
+        grad_x = grad_ws = grad_wn = grad_b = None
+        if ctx.needs_input_grad[0]:
+            csr_t, w_t = block.transposed(reduce)
+            grad_x = ops.spmm(csr_t, w_t, ops.gemm(gn, wnd, trans_b=True), reduce="sum")
+            ops.gemm(gs, wsd, trans_b=True, beta=1.0, out=grad_x[:block.num_dst])
+        if ctx.needs_input_grad[1]:
+            grad_ws = ops.gemm(x_self, gs, trans_a=True)
+        if ctx.needs_input_grad[2]:
+            grad_wn = ops.gemm(agg, gn, trans_a=True)
+        if has_bias and ctx.needs_input_grad[3]:
+            grad_b = ops.colsum(gm)
+        return grad_x, grad_ws, grad_wn, grad_b, None, None, None, None, None
+
+
+class BlockAggregate(torch.autograd.Function):
+    """NeighborAggregate over a sampled block: agg [num_dst, D] = REDUCE over block.csr (sum | mean) of x's rows, weighted
+    by the block's edge weights or, with weighted=False, by ones; `col` overrides the block's local columns (the
+    SourceRows route reads the global table through block.global_col and takes no gradient).  Backward: K1 over the
+    block's transposed CSR into x's num_src rows."""
+
+    @staticmethod
+    def forward(ctx, x, block, reduce, weighted, col):
+        ctx.meta = (block, reduce, weighted)
+        return ops.spmm(block.csr, block.edge_weight if weighted else None, x.detach(), reduce=reduce, col=col)
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        block, reduce, weighted = ctx.meta
+        if not ctx.needs_input_grad[0]:
+            return None, None, None, None, None
+        csr_t, w_t = block.transposed(reduce, weighted)
+        return ops.spmm(csr_t, w_t, grad_out.contiguous(), reduce="sum"), None, None, None, None
+
+
+class BlockMax(torch.autograd.Function):
+    """NeighborMax over a sampled block, unweighted: K11a over block.csr into num_dst rows; K11b over the block's
+    transposed CSR into x's num_src rows."""
+
+    @staticmethod
+    def forward(ctx, x, block):
+        xd = x.detach()
+        out, cnt = ops.spmm_max(block.csr, None, xd)
+        ctx.block = block
+        ctx.save_for_backward(xd, out, cnt)
+        return out
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        x, out, cnt = ctx.saved_tensors
+        if not ctx.needs_input_grad[0]:
+            return None, None
+        csr_t, _ = ctx.block.transposed(None)
+        return ops.spmm_max_bwd(csr_t, None, x, out, cnt, grad_out.contiguous()), None
 
 
 def _half_edge_csr(edge_index, num_nodes):

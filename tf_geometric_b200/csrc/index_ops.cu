@@ -426,13 +426,12 @@ int tfgk_csr_workspace_bytes(int64_t E, int32_t N, size_t *out_bytes) {
     return TFGK_OK;
 }
 
-int tfgk_csr_build(const int32_t *row, const int32_t *col, int64_t E, int32_t N_rows, int32_t N_cols,
-                   int64_t *rowptr, int32_t *col_sorted, int32_t *perm,
-                   void *workspace, size_t workspace_bytes, void *stream) {
+static int csr_build(const int32_t *row, const int32_t *col, int64_t E, int32_t N_rows, int32_t N_cols,
+                     int64_t *rowptr, int32_t *col_sorted, int32_t *perm, void *workspace, size_t workspace_bytes,
+                     bool check_ids, cudaStream_t st) {
     TFGK_CHECK_ARG(E >= 0 && E < (1ll << 31), "csr_build: need 0 <= E < 2^31 (got %lld)", (long long)E);
     TFGK_CHECK_ARG(N_rows >= 0 && N_cols >= 0, "csr_build: negative node count");
     TFGK_CHECK_ARG(rowptr != nullptr, "csr_build: null rowptr");
-    cudaStream_t st = as_stream(stream);
     if (E == 0) {
         TFGK_CUDA(cudaMemsetAsync(rowptr, 0, ((size_t)N_rows + 1) * 8, st));
         return TFGK_OK;
@@ -451,15 +450,17 @@ int tfgk_csr_build(const int32_t *row, const int32_t *col, int64_t E, int32_t N_
     int32_t *counts = reinterpret_cast<int32_t *>(ws + L.off_counts);
 
     // 1. validate ids (TF-CPU's gather / segment ops raise on out-of-range ids)
-    TFGK_CUDA(cudaMemsetAsync(flag, 0, 4, st));
-    validate_kernel<<<grid_for(E), 256, 0, st>>>(row, E, N_rows, flag);
-    TFGK_LAUNCH_CHECK();
-    validate_kernel<<<grid_for(E), 256, 0, st>>>(col, E, N_cols, flag);
-    TFGK_LAUNCH_CHECK();
-    int32_t bad = 0;
-    TFGK_CUDA(cudaMemcpyAsync(&bad, flag, 4, cudaMemcpyDeviceToHost, st));
-    TFGK_CUDA(cudaStreamSynchronize(st));
-    if (bad) return set_error(TFGK_ERR_INDEX_OUT_OF_RANGE, "csr_build: edge_index holds node ids outside [0, N)");
+    if (check_ids) {
+        TFGK_CUDA(cudaMemsetAsync(flag, 0, 4, st));
+        validate_kernel<<<grid_for(E), 256, 0, st>>>(row, E, N_rows, flag);
+        TFGK_LAUNCH_CHECK();
+        validate_kernel<<<grid_for(E), 256, 0, st>>>(col, E, N_cols, flag);
+        TFGK_LAUNCH_CHECK();
+        int32_t bad = 0;
+        TFGK_CUDA(cudaMemcpyAsync(&bad, flag, 4, cudaMemcpyDeviceToHost, st));
+        TFGK_CUDA(cudaStreamSynchronize(st));
+        if (bad) return set_error(TFGK_ERR_INDEX_OUT_OF_RANGE, "csr_build: edge_index holds node ids outside [0, N)");
+    }
 
     // 2. rowptr = exclusive scan of the per-row edge counts
     TFGK_CUDA(cudaMemsetAsync(counts, 0, ((size_t)N_rows + 1) * 4, st));
@@ -476,6 +477,20 @@ int tfgk_csr_build(const int32_t *row, const int32_t *col, int64_t E, int32_t N_
     gather_i32_kernel<<<grid_for(E), 256, 0, st>>>(col, perm, E, col_sorted);
     TFGK_LAUNCH_CHECK();
     return TFGK_OK;
+}
+
+int tfgk_csr_build(const int32_t *row, const int32_t *col, int64_t E, int32_t N_rows, int32_t N_cols,
+                   int64_t *rowptr, int32_t *col_sorted, int32_t *perm,
+                   void *workspace, size_t workspace_bytes, void *stream) {
+    return csr_build(row, col, E, N_rows, N_cols, rowptr, col_sorted, perm, workspace, workspace_bytes, true,
+                     as_stream(stream));
+}
+
+int tfgk_csr_build_in_range(const int32_t *row, const int32_t *col, int64_t E, int32_t N_rows, int32_t N_cols,
+                            int64_t *rowptr, int32_t *col_sorted, int32_t *perm,
+                            void *workspace, size_t workspace_bytes, void *stream) {
+    return csr_build(row, col, E, N_rows, N_cols, rowptr, col_sorted, perm, workspace, workspace_bytes, false,
+                     as_stream(stream));
 }
 
 int tfgk_sort_keys_f32(const float *score, int64_t n, int descending, int32_t *keys, void *stream) {

@@ -105,11 +105,16 @@ __global__ void sample_rows_count_kernel(const int64_t *__restrict__ rowptr, int
     cnt[t] = num;
 }
 
-__global__ void __launch_bounds__(kRowsPerCta)
-sample_rows_fill_kernel(const int64_t *__restrict__ rowptr, int32_t n_rows, const int32_t *__restrict__ rows,
-                        int32_t n_list, int k, double ratio, int padding, uint64_t seed, uint32_t stream,
-                        const int64_t *__restrict__ out_rowptr, int32_t *__restrict__ out_row,
-                        int32_t *__restrict__ out_pos) {
+// The fill of K13.  kBlock (the block sampler) also writes every sampled edge's global column col[pos] and weight
+// w_csr[pos], once its position is final; the plain instantiation leaves that to the caller's gathers.
+template <bool kBlock>
+__device__ __forceinline__ void sample_rows_fill_body(const int64_t *__restrict__ rowptr, int32_t n_rows,
+                                                      const int32_t *__restrict__ rows, int32_t n_list, int k,
+                                                      double ratio, int padding, uint64_t seed, uint32_t stream,
+                                                      const int64_t *__restrict__ out_rowptr, int32_t *__restrict__ out_row,
+                                                      int32_t *__restrict__ out_pos, const int32_t *__restrict__ csr_col,
+                                                      const float *__restrict__ w_csr, int32_t *__restrict__ out_gcol,
+                                                      float *__restrict__ out_w) {
     __shared__ int32_t long_rows[kRowsPerCta];
     __shared__ int n_long;
     if (threadIdx.x == 0) n_long = 0;
@@ -140,6 +145,12 @@ sample_rows_fill_kernel(const int64_t *__restrict__ rowptr, int32_t n_rows, cons
                             if (j < (uint32_t)num) out_pos[o + j] = (int32_t)(start + i);
                         }
                 }
+                if constexpr (kBlock)
+                    for (int i = 0; i < num; ++i) {
+                        const int32_t p = out_pos[o + i];
+                        out_gcol[o + i] = csr_col[p];
+                        out_w[o + i] = w_csr[p];
+                    }
             }
         }
     }
@@ -177,18 +188,45 @@ sample_rows_fill_kernel(const int64_t *__restrict__ rowptr, int32_t n_rows, cons
             if (j < (uint32_t)num) atomicMax(out_pos + o + j, (int32_t)(start + i));
         }
     }
+    if constexpr (kBlock) {
+        __syncthreads();               // the reservoir's atomics are final
+        for (int q = 0; q < nl; ++q) {
+            const int64_t tl = (int64_t)blockIdx.x * kRowsPerCta + long_rows[q];
+            const int32_t r = rows[tl];
+            int num;
+            sample_rule((int)(rowptr[r + 1] - rowptr[r]), k, ratio, padding, num);
+            const int64_t o = out_rowptr[tl];
+            for (int i = threadIdx.x; i < num; i += kRowsPerCta) {
+                const int32_t p = out_pos[o + i];
+                out_gcol[o + i] = csr_col[p];
+                out_w[o + i] = w_csr[p];
+            }
+        }
+    }
+}
+
+__global__ void __launch_bounds__(kRowsPerCta)
+sample_rows_fill_kernel(const int64_t *__restrict__ rowptr, int32_t n_rows, const int32_t *__restrict__ rows,
+                        int32_t n_list, int k, double ratio, int padding, uint64_t seed, uint32_t stream,
+                        const int64_t *__restrict__ out_rowptr, int32_t *__restrict__ out_row,
+                        int32_t *__restrict__ out_pos) {
+    sample_rows_fill_body<false>(rowptr, n_rows, rows, n_list, k, ratio, padding, seed, stream, out_rowptr, out_row,
+                                 out_pos, nullptr, nullptr, nullptr, nullptr);
 }
 
 // ---- relabelling: an [N] id -> position map that is -1 everywhere outside a call --------------------------------
 enum { kBadIds = 0, kDupIds = 1, kNewIds = 2 };
 
+__device__ __forceinline__ void scatter_one(int32_t id, int64_t p, int32_t N, int32_t *__restrict__ map,
+                                            int32_t *__restrict__ counters) {
+    if (id < 0 || id >= N) atomicAdd(counters + kBadIds, 1);
+    else if (atomicCAS(map + id, -1, (int32_t)p) != -1) atomicAdd(counters + kDupIds, 1);
+}
+
 __global__ void node_scatter_kernel(const int32_t *__restrict__ nodes, int32_t n, int32_t N, int32_t *__restrict__ map,
                                     int32_t *__restrict__ counters) {
-    for (int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; p < n; p += (int64_t)gridDim.x * blockDim.x) {
-        const int32_t id = nodes[p];
-        if (id < 0 || id >= N) atomicAdd(counters + kBadIds, 1);
-        else if (atomicCAS(map + id, -1, (int32_t)p) != -1) atomicAdd(counters + kDupIds, 1);
-    }
+    for (int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; p < n; p += (int64_t)gridDim.x * blockDim.x)
+        scatter_one(nodes[p], p, N, map, counters);
 }
 
 // reset the map entries of nodes[0, n + *extra)
@@ -201,42 +239,134 @@ __global__ void node_reset_kernel(const int32_t *__restrict__ nodes, int64_t n, 
     }
 }
 
+__device__ __forceinline__ void gather_one(const int32_t *__restrict__ ids, int64_t e, int32_t N,
+                                           const int32_t *__restrict__ map, int32_t *__restrict__ out) {
+    const int32_t id = ids[e];
+    out[e] = (id >= 0 && id < N) ? map[id] : -1;
+}
+
 __global__ void reindex_gather_kernel(const int32_t *__restrict__ ids, int64_t n, int32_t N,
                                       const int32_t *__restrict__ map, int32_t *__restrict__ out) {
-    for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < n; e += (int64_t)gridDim.x * blockDim.x) {
-        const int32_t id = ids[e];
-        out[e] = (id >= 0 && id < N) ? map[id] : -1;
-    }
+    for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < n; e += (int64_t)gridDim.x * blockDim.x)
+        gather_one(ids, e, N, map, out);
 }
 
 // ids not yet in the map: map[id] = INT32_MIN + (first e holding id).  atomicMin keeps the smallest e whatever the
 // order, and INT32_MIN + e <= -2 stays below the -1 of an absent id and below every position.
+__device__ __forceinline__ void first_one(const int32_t *__restrict__ cols, int64_t e, int32_t N,
+                                          int32_t *__restrict__ map, int32_t *__restrict__ counters) {
+    const int32_t c = cols[e];
+    if (c < 0 || c >= N) atomicAdd(counters + kBadIds, 1);
+    else if (map[c] < 0) atomicMin(map + c, INT32_MIN + (int32_t)e);
+}
+
 __global__ void frontier_first_kernel(const int32_t *__restrict__ cols, int64_t S, int32_t N, int32_t *__restrict__ map,
                                       int32_t *__restrict__ counters) {
-    for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < S; e += (int64_t)gridDim.x * blockDim.x) {
-        const int32_t c = cols[e];
-        if (c < 0 || c >= N) atomicAdd(counters + kBadIds, 1);
-        else if (map[c] < 0) atomicMin(map + c, INT32_MIN + (int32_t)e);
-    }
+    for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < S; e += (int64_t)gridDim.x * blockDim.x)
+        first_one(cols, e, N, map, counters);
+}
+
+__device__ __forceinline__ int32_t flag_one(const int32_t *__restrict__ cols, int64_t e, int32_t N,
+                                            const int32_t *__restrict__ map) {
+    const int32_t c = cols[e];
+    return (c >= 0 && c < N && map[c] == INT32_MIN + (int32_t)e) ? 1 : 0;
 }
 
 __global__ void frontier_flag_kernel(const int32_t *__restrict__ cols, int64_t S, int32_t N,
                                      const int32_t *__restrict__ map, int32_t *__restrict__ flag) {
-    for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < S; e += (int64_t)gridDim.x * blockDim.x) {
-        const int32_t c = cols[e];
-        flag[e] = (c >= 0 && c < N && map[c] == INT32_MIN + (int32_t)e) ? 1 : 0;
-    }
+    for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < S; e += (int64_t)gridDim.x * blockDim.x)
+        flag[e] = flag_one(cols, e, N, map);
+}
+
+__device__ __forceinline__ void emit_one(const int32_t *__restrict__ cols, int64_t e, const int32_t *__restrict__ off,
+                                         int32_t n_nodes, int32_t *__restrict__ nodes, int32_t *__restrict__ map) {
+    const int32_t pos = n_nodes + off[e];
+    nodes[pos] = cols[e];
+    map[cols[e]] = pos;
 }
 
 __global__ void frontier_emit_kernel(const int32_t *__restrict__ cols, int64_t S, const int32_t *__restrict__ flag,
                                      const int32_t *__restrict__ off, int32_t n_nodes, int32_t *__restrict__ nodes,
                                      int32_t *__restrict__ map) {
     for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < S; e += (int64_t)gridDim.x * blockDim.x)
-        if (flag[e]) {
-            const int32_t pos = n_nodes + off[e];
-            nodes[pos] = cols[e];
-            map[cols[e]] = pos;
-        }
+        if (flag[e]) emit_one(cols, e, off, n_nodes, nodes, map);
+}
+
+// ---- the block sampler: the same steps with every size kept on the device --------------------------------------
+// state (include/tfgk.h): [bad seeds, duplicate seeds, -, list length after hop 0..L, edges of hop 0..L-1].  Grids are
+// sized by host-known capacities and threads past the device count exit, so a batch reads nothing back until its end.
+constexpr int kStateSizes = 3;
+
+__global__ void block_begin_kernel(const int32_t *__restrict__ seeds, int32_t n, int32_t N, int32_t *__restrict__ nodes,
+                                   int32_t *__restrict__ map, int32_t *__restrict__ state) {
+    if (blockIdx.x == 0 && threadIdx.x == 0) state[kStateSizes] = n;
+    for (int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; p < n; p += (int64_t)gridDim.x * blockDim.x) {
+        const int32_t id = seeds[p];
+        nodes[p] = id;
+        scatter_one(id, p, N, map, state);
+    }
+}
+
+// listed rows past the device count contribute 0, so the scan over the capacity ends in the hop's edge total
+__global__ void block_count_kernel(const int64_t *__restrict__ rowptr, int32_t n_rows, const int32_t *__restrict__ rows,
+                                   const int32_t *__restrict__ n_list, int32_t cap, int k, int padding,
+                                   int32_t *__restrict__ cnt) {
+    const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= cap) return;
+    int num = 0;
+    if (t < *n_list) {
+        const int32_t r = rows[t];
+        if (r >= 0 && r < n_rows) sample_rule((int)(rowptr[r + 1] - rowptr[r]), k, -1.0, padding, num);
+    }
+    cnt[t] = num;
+}
+
+__global__ void __launch_bounds__(kRowsPerCta)
+block_fill_kernel(const int64_t *__restrict__ rowptr, int32_t n_rows, const int32_t *__restrict__ rows,
+                  const int32_t *__restrict__ n_list, int k, int padding, uint64_t seed, uint32_t stream,
+                  const int64_t *__restrict__ out_rowptr, int32_t *__restrict__ out_row, int32_t *__restrict__ out_pos,
+                  const int32_t *__restrict__ csr_col, const float *__restrict__ w_csr, int32_t *__restrict__ out_gcol,
+                  float *__restrict__ out_w) {
+    sample_rows_fill_body<true>(rowptr, n_rows, rows, *n_list, k, -1.0, padding, seed, stream, out_rowptr, out_row,
+                                out_pos, csr_col, w_csr, out_gcol, out_w);
+}
+
+__global__ void block_first_kernel(const int32_t *__restrict__ cols, const int64_t *__restrict__ S, int32_t N,
+                                   int32_t *__restrict__ map, int32_t *__restrict__ counters) {
+    const int64_t n = *S;
+    for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < n; e += (int64_t)gridDim.x * blockDim.x)
+        first_one(cols, e, N, map, counters);
+}
+
+__global__ void block_flag_kernel(const int32_t *__restrict__ cols, const int64_t *__restrict__ S, int64_t cap,
+                                  int32_t N, const int32_t *__restrict__ map, int32_t *__restrict__ flag) {
+    const int64_t n = *S;
+    for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < cap; e += (int64_t)gridDim.x * blockDim.x)
+        flag[e] = e < n ? flag_one(cols, e, N, map) : 0;
+}
+
+__global__ void block_emit_kernel(const int32_t *__restrict__ cols, const int64_t *__restrict__ S,
+                                  const int32_t *__restrict__ flag, const int32_t *__restrict__ off,
+                                  const int32_t *__restrict__ n_nodes, int32_t *__restrict__ nodes,
+                                  int32_t *__restrict__ map) {
+    const int64_t n = *S;
+    const int32_t base = *n_nodes;
+    for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < n; e += (int64_t)gridDim.x * blockDim.x)
+        if (flag[e]) emit_one(cols, e, off, base, nodes, map);
+}
+
+__global__ void block_gather_kernel(const int32_t *__restrict__ ids, const int64_t *__restrict__ S, int32_t N,
+                                    const int32_t *__restrict__ map, int32_t *__restrict__ out) {
+    const int64_t n = *S;
+    for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < n; e += (int64_t)gridDim.x * blockDim.x)
+        gather_one(ids, e, N, map, out);
+}
+
+// list length after hop h + 1 and the edges of hop h
+__global__ void block_sizes_kernel(const int64_t *__restrict__ S, const int32_t *__restrict__ n_new, int32_t hop,
+                                   int32_t n_hops, int32_t *__restrict__ state) {
+    state[kStateSizes + hop + 1] = state[kStateSizes + hop] + *n_new;
+    state[kStateSizes + n_hops + 1 + hop] = (int32_t)*S;
 }
 
 }  // namespace
@@ -509,6 +639,146 @@ int tfgk_frontier_i32(const int32_t *cols, int64_t S, int32_t N, int32_t *nodes,
     if (c[kBadIds]) return set_error(TFGK_ERR_INDEX_OUT_OF_RANGE, "frontier: %d node ids outside [0, %d)", c[kBadIds], N);
     *n_dup_host = c[kDupIds];
     *n_new_host = c[kNewIds];
+    return TFGK_OK;
+}
+
+// ---- block sampler (include/tfgk.h) -----------------------------------------------------------------------------
+namespace {
+struct BlockWorkspace {
+    size_t off_sums, off_pos, off_flag, off_off, total;
+    BlockWorkspace(int32_t cap_list, int64_t cap_edges) {
+        size_t sums = scan_scratch_bytes((int64_t)cap_list + 1);
+        if (scan_scratch_bytes(cap_edges + 1) > sums) sums = scan_scratch_bytes(cap_edges + 1);
+        off_sums = align_up(((size_t)cap_list + 1) * 4);                   // per-row counts first
+        off_pos = off_sums + sums;
+        off_flag = off_pos + align_up((size_t)(cap_edges > 0 ? cap_edges : 1) * 4);
+        off_off = off_flag + align_up((size_t)(cap_edges + 1) * 4);
+        total = off_off + align_up((size_t)(cap_edges + 1) * 4);
+    }
+};
+}  // namespace
+
+static int block_workspace_check(const char *fn, int32_t cap_list, int64_t cap_edges, void *workspace,
+                                 size_t workspace_bytes) {
+    const size_t need = BlockWorkspace(cap_list, cap_edges).total;
+    if (workspace == nullptr || workspace_bytes < need)
+        return set_error(TFGK_ERR_WORKSPACE, "%s: workspace too small (%zu < %zu bytes)", fn, workspace_bytes, need);
+    return TFGK_OK;
+}
+
+int tfgk_block_sample_workspace_bytes(int32_t cap_list, int64_t cap_edges, size_t *out_bytes) {
+    TFGK_CHECK_ARG(out_bytes != nullptr && cap_list >= 0 && cap_edges >= 0 && cap_edges < (1ll << 31) - 1,
+                   "block_sample_workspace_bytes: bad argument");
+    *out_bytes = BlockWorkspace(cap_list, cap_edges).total;
+    return TFGK_OK;
+}
+
+int tfgk_block_sample_begin(const int32_t *seeds, int32_t n_seeds, int32_t N, int32_t *nodes, int32_t *map,
+                            int32_t *state, int32_t n_hops, void *stream) {
+    TFGK_CHECK_ARG(n_seeds >= 0 && N >= 0 && n_hops >= 0, "block_sample_begin: bad size");
+    TFGK_CHECK_ARG(state != nullptr && (n_seeds == 0 || (seeds && nodes && map)), "block_sample_begin: null pointer");
+    cudaStream_t st = as_stream(stream);
+    TFGK_CUDA(cudaMemsetAsync(state, 0, (size_t)(4 + 2 * n_hops) * 4, st));
+    block_begin_kernel<<<grid_for(n_seeds), 256, 0, st>>>(seeds, n_seeds, N, nodes, map, state);
+    TFGK_LAUNCH_CHECK();
+    return TFGK_OK;
+}
+
+int tfgk_block_sample_count(const int64_t *rowptr, int32_t n_rows, const int32_t *nodes, const int32_t *state,
+                            int32_t hop, int32_t n_hops, int32_t cap_list, int32_t k, int padding, int64_t *out_rowptr,
+                            void *workspace, size_t workspace_bytes, void *stream) {
+    int rc = check_sample_mode("block_sample_count", k, -1.0, padding);
+    if (rc != TFGK_OK) return rc;
+    TFGK_CHECK_ARG(n_rows >= 0 && hop >= 0 && hop < n_hops && cap_list >= 0, "block_sample_count: bad size");
+    TFGK_CHECK_ARG(state != nullptr && out_rowptr != nullptr, "block_sample_count: null pointer");
+    cudaStream_t st = as_stream(stream);
+    if (cap_list == 0) {
+        TFGK_CUDA(cudaMemsetAsync(out_rowptr, 0, 8, st));
+        return TFGK_OK;
+    }
+    TFGK_CHECK_ARG(rowptr != nullptr && nodes != nullptr, "block_sample_count: null rowptr or node list");
+    if ((rc = block_workspace_check("block_sample_count", cap_list, 0, workspace, workspace_bytes)) != TFGK_OK) return rc;
+    char *ws = static_cast<char *>(workspace);
+    const BlockWorkspace L(cap_list, 0);
+    int32_t *cnt = reinterpret_cast<int32_t *>(ws);
+    block_count_kernel<<<(unsigned)ceil_div64(cap_list, 256), 256, 0, st>>>(rowptr, n_rows, nodes,
+                                                                            state + kStateSizes + hop, cap_list, k,
+                                                                            padding, cnt);
+    TFGK_LAUNCH_CHECK();
+    return exclusive_scan<int32_t, int64_t>(cnt, cap_list, (int64_t)cap_list + 1, out_rowptr,
+                                            reinterpret_cast<int64_t *>(ws + L.off_sums), st);
+}
+
+int tfgk_block_sample_read_total(const int32_t *state, int32_t hop, const int64_t *out_rowptr, int32_t cap_list,
+                                 int32_t *n_list_host, int64_t *total_host, void *stream) {
+    TFGK_CHECK_ARG(state && out_rowptr && n_list_host && total_host && hop >= 0 && cap_list >= 0,
+                   "block_sample_read_total: bad argument");
+    cudaStream_t st = as_stream(stream);
+    TFGK_CUDA(cudaMemcpyAsync(n_list_host, state + kStateSizes + hop, 4, cudaMemcpyDeviceToHost, st));
+    TFGK_CUDA(cudaMemcpyAsync(total_host, out_rowptr + cap_list, 8, cudaMemcpyDeviceToHost, st));
+    TFGK_CUDA(cudaStreamSynchronize(st));
+    TFGK_CHECK_ARG(*total_host < (1ll << 31) - 1, "block_sample_read_total: %lld sampled edges exceed int32 positions",
+                   (long long)*total_host);
+    return TFGK_OK;
+}
+
+int tfgk_block_sample_fill(const int64_t *rowptr, int32_t n_rows, const int32_t *col, const float *w_csr, int32_t N,
+                           int32_t *nodes, int32_t *map, int32_t *state, int32_t hop, int32_t n_hops, int32_t cap_list,
+                           int64_t cap_edges, int32_t k, int padding, uint64_t seed, uint32_t rng_stream,
+                           const int64_t *out_rowptr, int32_t *out_row, int32_t *out_local, int32_t *out_gcol,
+                           float *out_w, void *workspace, size_t workspace_bytes, void *stream) {
+    int rc = check_sample_mode("block_sample_fill", k, -1.0, padding);
+    if (rc != TFGK_OK) return rc;
+    TFGK_CHECK_ARG(n_rows >= 0 && N >= 0 && hop >= 0 && hop < n_hops && cap_list >= 0 && cap_edges >= 0 &&
+                   cap_edges < (1ll << 31) - 1, "block_sample_fill: bad size");
+    TFGK_CHECK_ARG(state && out_rowptr, "block_sample_fill: null pointer");
+    if ((rc = block_workspace_check("block_sample_fill", cap_list, cap_edges, workspace, workspace_bytes)) != TFGK_OK)
+        return rc;
+    cudaStream_t st = as_stream(stream);
+    char *ws = static_cast<char *>(workspace);
+    const BlockWorkspace L(cap_list, cap_edges);
+    int32_t *pos = reinterpret_cast<int32_t *>(ws + L.off_pos);
+    int32_t *flag = reinterpret_cast<int32_t *>(ws + L.off_flag);
+    int32_t *off = reinterpret_cast<int32_t *>(ws + L.off_off);
+    const int32_t *n_list = state + kStateSizes + hop;
+    const int64_t *S = out_rowptr + cap_list;               // listed rows past the count add no edges
+    if (cap_list > 0 && cap_edges > 0) {
+        TFGK_CHECK_ARG(rowptr && col && w_csr && nodes && map && out_row && out_local && out_gcol && out_w,
+                       "block_sample_fill: null pointer");
+        block_fill_kernel<<<(unsigned)ceil_div64(cap_list, kRowsPerCta), kRowsPerCta, 0, st>>>(
+            rowptr, n_rows, nodes, n_list, k, padding, seed, rng_stream, out_rowptr, out_row, pos, col, w_csr, out_gcol,
+            out_w);
+        TFGK_LAUNCH_CHECK();
+        block_first_kernel<<<grid_for(cap_edges), 256, 0, st>>>(out_gcol, S, N, map, state);
+        TFGK_LAUNCH_CHECK();
+        block_flag_kernel<<<grid_for(cap_edges), 256, 0, st>>>(out_gcol, S, cap_edges, N, map, flag);
+        TFGK_LAUNCH_CHECK();
+        rc = exclusive_scan<int32_t, int32_t>(flag, cap_edges, cap_edges + 1, off, reinterpret_cast<int32_t *>(ws + L.off_sums),
+                                              st);
+        if (rc != TFGK_OK) return rc;
+        block_emit_kernel<<<grid_for(cap_edges), 256, 0, st>>>(out_gcol, S, flag, off, n_list, nodes, map);
+        TFGK_LAUNCH_CHECK();
+        block_gather_kernel<<<grid_for(cap_edges), 256, 0, st>>>(out_gcol, S, N, map, out_local);
+        TFGK_LAUNCH_CHECK();
+    } else {
+        TFGK_CUDA(cudaMemsetAsync(off, 0, 4, st));          // no edges, no new nodes
+    }
+    block_sizes_kernel<<<1, 1, 0, st>>>(S, off + cap_edges, hop, n_hops, state);
+    TFGK_LAUNCH_CHECK();
+    return TFGK_OK;
+}
+
+int tfgk_block_sample_end(const int32_t *nodes, int32_t cap_nodes, int32_t N, int32_t *map, const int32_t *state,
+                          int32_t n_hops, int32_t *state_host, void *stream) {
+    TFGK_CHECK_ARG(cap_nodes >= 0 && N >= 0 && n_hops >= 0, "block_sample_end: bad size");
+    TFGK_CHECK_ARG(state && state_host && (cap_nodes == 0 || (nodes && map)), "block_sample_end: null pointer");
+    cudaStream_t st = as_stream(stream);
+    if (cap_nodes > 0) {
+        node_reset_kernel<<<grid_for(cap_nodes), 256, 0, st>>>(nodes, 0, state + kStateSizes + n_hops, N, map);
+        TFGK_LAUNCH_CHECK();
+    }
+    TFGK_CUDA(cudaMemcpyAsync(state_host, state, (size_t)(4 + 2 * n_hops) * 4, cudaMemcpyDeviceToHost, st));
+    TFGK_CUDA(cudaStreamSynchronize(st));
     return TFGK_OK;
 }
 

@@ -14,6 +14,7 @@ from . import _bf16
 from .gat import project
 from .gcn import gcn_norm_edge
 from ...sparse import SparseMatrix
+from ...utils.sampling import Block, SourceRows
 
 
 def _project_pair(x, agg, self_kernel, neighbor_kernel, bias, activation, concat, normalize):
@@ -66,8 +67,54 @@ def _project_pair_autograd(x, agg, ws, wn, bias, activation, concat, normalize):
     return h
 
 
+def _block_input(x, block, edge_weight, message_dtype, gather_all):
+    """(table, self_index) for a layer over a sampled block: the block's [num_src, F] input and None, or, for a SourceRows
+    input that mean / sum can read in place, the global table and the node ids of the self rows.  Refuses what blocks do
+    not support before any device work."""
+    if _bf16.enabled(message_dtype):
+        raise NotImplementedError("GraphSAGE on a sampled block takes fp32 messages only (message_dtype=None)")
+    if edge_weight is not None:
+        if torch.is_tensor(edge_weight) and edge_weight.requires_grad:
+            raise NotImplementedError("GraphSAGE on a sampled block has no edge-weight gradient")
+        raise ValueError("a sampled block carries its edge weights: pass [x, block]")
+    if isinstance(x, SourceRows):
+        if x.shape[0] != block.num_src:
+            raise ValueError("the source rows ({}) are not this block's {} input rows".format(x.shape[0], block.num_src))
+        if gather_all or (x.x.requires_grad and torch.is_grad_enabled()):
+            return x.gather(), None
+        return x.x, x.node_index[:block.num_dst]
+    x = ops.as_device(x, torch.float32, device=block.edge_index.device)
+    if x.dim() != 2 or x.shape[0] != block.num_src:
+        raise ValueError("x has {} rows, the block has {} input rows".format(tuple(x.shape)[:1], block.num_src))
+    return x, None
+
+
+def _block_sage(reduce, x, block, edge_weight, self_kernel, neighbor_kernel, bias, activation, concat, normalize,
+                message_dtype):
+    """mean / sum GraphSAGE over a sampled block: num_dst output rows; the self term is the input's first num_dst rows."""
+    table, self_index = _block_input(x, block, edge_weight, message_dtype, False)
+    dev = table.device
+    col = None if self_index is None else block.global_col
+    if autograd.needs_grad(table, self_kernel, neighbor_kernel, bias):
+        f32 = lambda t: None if t is None else ops.as_device(t, torch.float32, device=dev)   # noqa: E731
+        act_code, leftover = ops.activation_code(activation)
+        if leftover is None and not normalize:
+            return autograd.BlockSagePair.apply(table, f32(self_kernel), f32(neighbor_kernel), f32(bias), block, reduce,
+                                                act_code, bool(concat), self_index)
+        agg = autograd.BlockAggregate.apply(table, block, reduce, True, col)
+        x_self = table[:block.num_dst] if self_index is None else ops.permute(table, self_index)
+        return _project_pair_autograd(x_self, agg, f32(self_kernel), f32(neighbor_kernel), f32(bias), activation, concat,
+                                      normalize)
+    agg = ops.spmm(block.csr, block.edge_weight, table, reduce=reduce, col=col)
+    x_self = table[:block.num_dst] if self_index is None else ops.permute(table, self_index)
+    return _project_pair(x_self, agg, self_kernel, neighbor_kernel, bias, activation, concat, normalize)
+
+
 def _plain_sage(reduce, x, edge_index, edge_weight, self_kernel, neighbor_kernel, bias, activation, concat, normalize,
                 message_dtype=None):
+    if isinstance(edge_index, Block):
+        return _block_sage(reduce, x, edge_index, edge_weight, self_kernel, neighbor_kernel, bias, activation, concat,
+                           normalize, message_dtype)
     bf16 = _bf16.enabled(message_dtype)
     if bf16:
         _bf16.refuse_unsupported(x, (self_kernel, neighbor_kernel, bias, edge_weight))
@@ -143,8 +190,34 @@ def _norm_edge_as_matrix(edge_index, num_nodes, edge_weight, renorm):
     return index, value, [num_nodes, num_nodes]
 
 
+def _block_pool_sage(reduce, x, block, edge_weight, self_kernel, neighbor_mlp_kernel, neighbor_kernel, neighbor_mlp_bias,
+                     bias, activation, concat, normalize, message_dtype):
+    """mean-pool / max-pool GraphSAGE over a sampled block: the neighbour MLP runs on every source row (so a SourceRows
+    input is gathered), the reduction over the block's edges with unit weights (the reference's quirk), num_dst rows out."""
+    x, _ = _block_input(x, block, edge_weight, message_dtype, True)
+    dev = x.device
+    f32 = lambda t: None if t is None else ops.as_device(t, torch.float32, device=dev)   # noqa: E731
+    if autograd.needs_grad(x, self_kernel, neighbor_mlp_kernel, neighbor_kernel, neighbor_mlp_bias, bias):
+        h_node = autograd.dense(x, f32(neighbor_mlp_kernel), f32(neighbor_mlp_bias), activation)
+        if reduce == "mean":
+            reduced = autograd.BlockAggregate.apply(h_node, block, "mean", False, None)
+        else:
+            reduced = autograd.BlockMax.apply(h_node, block)
+        return _project_pair_autograd(x[:block.num_dst], reduced, f32(self_kernel), f32(neighbor_kernel), f32(bias),
+                                      activation, concat, normalize)
+    act_code, leftover = ops.activation_code(activation)
+    h_node = ops.gemm(x, f32(neighbor_mlp_kernel), bias=f32(neighbor_mlp_bias), act=act_code)
+    if leftover is not None:
+        h_node = leftover(h_node)
+    reduced = ops.spmm(block.csr, None, h_node, reduce=reduce)
+    return _project_pair(x[:block.num_dst], reduced, self_kernel, neighbor_kernel, bias, activation, concat, normalize)
+
+
 def _pool_sage(reduce, x, edge_index, edge_weight, self_kernel, neighbor_mlp_kernel, neighbor_kernel,
                neighbor_mlp_bias, bias, activation, concat, normalize, message_dtype=None):
+    if isinstance(edge_index, Block):
+        return _block_pool_sage(reduce, x, edge_index, edge_weight, self_kernel, neighbor_mlp_kernel, neighbor_kernel,
+                                neighbor_mlp_bias, bias, activation, concat, normalize, message_dtype)
     bf16 = _bf16.enabled(message_dtype)
     if bf16:
         _bf16.refuse_unsupported(x, (self_kernel, neighbor_mlp_kernel, neighbor_kernel, neighbor_mlp_bias, bias))

@@ -28,6 +28,21 @@ def default_device():
     return torch.device("cuda", torch.cuda.current_device())
 
 
+class SampledInput(object):
+    """Base of the sampled-batch inputs (utils.sampling.Block, SourceRows) that only the block-aware GraphSAGE
+    aggregators take; as_device refuses them, so every other operator rejects them before any device work."""
+
+    __slots__ = ()
+
+
+def refuse_sampled(x):
+    """TypeError for a SampledInput (the check as_device applies to every non-tensor input)."""
+    if isinstance(x, SampledInput):
+        raise TypeError("a {} is taken only by mean_graph_sage, sum_graph_sage, mean_pool_graph_sage and "
+                        "max_pool_graph_sage (and their layers); other operators need a normalisation, self loops or "
+                        "padding that is not defined for a sampled block".format(type(x).__name__))
+
+
 def as_device(x, dtype=None, device=None):
     """numpy / list / torch (any device) -> contiguous CUDA tensor of `dtype` (reference casting rules are applied
     by the callers: int32 edge_index, float32 weights/features; data/graph.py:58-86).
@@ -37,6 +52,7 @@ def as_device(x, dtype=None, device=None):
     if x is None:
         return None
     if not torch.is_tensor(x):
+        refuse_sampled(x)
         x = torch.from_numpy(np.ascontiguousarray(x))
     if device is None:
         device = x.device if x.is_cuda else default_device()
@@ -142,7 +158,9 @@ def segment_count(ids, num_segments):
     return out
 
 
-def csr_build(row, col, n_rows, n_cols=None):
+def csr_build(row, col, n_rows, n_cols=None, ids_in_range=False):
+    """ids_in_range=True: the ids are known to lie in [0, n_rows) x [0, n_cols) (tfgk_csr_build_in_range, which skips the
+    check and its synchronisation; the work plan is still built)."""
     _check(row, torch.int32, "row")
     _check(col, torch.int32, "col")
     n_cols = n_rows if n_cols is None else n_cols
@@ -154,7 +172,8 @@ def csr_build(row, col, n_rows, n_cols=None):
     rowptr = torch.empty((n_rows + 1,), dtype=torch.int64, device=dev)
     col_sorted = torch.empty((E,), dtype=torch.int32, device=dev)
     perm = torch.empty((E,), dtype=torch.int32, device=dev)
-    _ffi.call("tfgk_csr_build", _p(row), _p(col), E, n_rows, n_cols, _p(rowptr), _p(col_sorted), _p(perm),
+    _ffi.call("tfgk_csr_build_in_range" if ids_in_range else "tfgk_csr_build", _p(row), _p(col), E, n_rows, n_cols,
+              _p(rowptr), _p(col_sorted), _p(perm),
               _p(ws), need.value, _stream(row))
     csr = CSR(rowptr, col_sorted, perm, n_rows, n_cols)
     csr.plan = build_plan(csr)
@@ -963,6 +982,90 @@ def frontier(nodes, n_nodes, cols, node_map):
     _ffi.call("tfgk_frontier_i32", _p(cols), S, node_map.numel(), _p(nodes), int(n_nodes), _p(node_map), _p(local),
               ctypes.byref(n_new), ctypes.byref(n_dup), _p(ws), nbytes, _stream(cols))
     return local, n_new.value, n_dup.value
+
+
+def block_capacities(n_listed, k, limit):
+    """(edges, listed rows after the hop) that a hop of fan-out k over at most n_listed rows can produce, with at most
+    `limit` rows in any list, or (None, None) when that is not known in advance (k None: every neighbour) or the edges
+    reach 2^31."""
+    if k is None or n_listed * k >= (1 << 31) - 1:
+        return None, None
+    return n_listed * k, min(limit, n_listed * (1 + k))
+
+
+def _block_workspace(cap_list, cap_edges, device):
+    need = ctypes.c_size_t()
+    _ffi.call("tfgk_block_sample_workspace_bytes", cap_list, cap_edges, ctypes.byref(need))
+    return torch.empty((need.value,), dtype=torch.uint8, device=device), need.value
+
+
+def block_sample(rowptr, col, w_csr, seeds, fanouts, keys, node_map, padding=False, rng_stream=RNG_STREAM_SAMPLER):
+    """The block sampler (tfgk_block_sample_*): the hops of neighbor_sample_rows + frontier for every listed row, with the
+    sizes kept on the device.  A hop whose capacity block_capacities cannot bound reads its edge total back; otherwise
+    the batch synchronises once, in tfgk_block_sample_end, which also leaves node_map clean.
+    rowptr int64 [N + 1], col int32, w_csr float32: the CSR (one row per node id) and its weights; seeds int32 [n];
+    fanouts: one k (or None) per hop, in hop order; keys: the hop keys.
+    Returns (nodes, hop_sizes, hops, n_bad, n_dup): nodes int32 [hop_sizes[-1]]; hops[h] = (out_rowptr int64 [>= n_h + 1],
+    list position of each edge's row, its local column, its global column (int32 [S_h]), its weight float32 [S_h]);
+    n_bad / n_dup count seeds outside [0, N) and repeated seeds (the lists are then meaningless).
+    Every argument the entries would refuse is refused before the map is touched, and a failure between the first and
+    the last entry (an allocation, a hop past 2^31 edges) resets the map before it propagates."""
+    # the fan-out rules of check_sample_mode, here so that no entry refuses a hop once the map holds the seeds
+    padding = _padding_code(padding)
+    if any(k is not None and int(k) < 0 for k in fanouts):
+        raise ValueError("block_sample: fan-outs must be >= 0 or None")
+    if padding == SAMPLE_HEAD and any(k is None for k in fanouts):
+        raise ValueError("block_sample: the head rule needs an integer fan-out for every hop")
+    _check(rowptr, torch.int64, "rowptr")
+    _check(col, torch.int32, "col")
+    _check(w_csr, torch.float32, "w_csr")
+    _check(seeds, torch.int32, "seeds")
+    _check(node_map, torch.int32, "node_map")
+    dev = rowptr.device
+    n_rows, N, L = rowptr.numel() - 1, node_map.numel(), len(fanouts)
+    ks = [-1 if k is None else int(k) for k in fanouts]
+    # a list holds each id once, plus the repeated or invalid seeds of a batch that will be refused
+    limit = N + seeds.numel()
+    cap_nodes = seeds.numel()
+    for k in fanouts:
+        cap_nodes = block_capacities(cap_nodes, k, limit)[1]
+        if cap_nodes is None:
+            cap_nodes = limit
+            break
+    nodes = torch.empty((max(cap_nodes, 1),), dtype=torch.int32, device=dev)
+    state = torch.empty((4 + 2 * L,), dtype=torch.int32, device=dev)
+    st = _stream(rowptr)
+    _ffi.call("tfgk_block_sample_begin", _p(seeds), seeds.numel(), N, _p(nodes), _p(node_map), _p(state), L, st)
+    try:
+        cap_list, hops = seeds.numel(), []
+        for h, k in enumerate(ks):
+            cap_edges, cap_next = block_capacities(cap_list, fanouts[h], limit)
+            ws, nbytes = _block_workspace(cap_list, 0 if cap_edges is None else cap_edges, dev)
+            out_rowptr = torch.empty((cap_list + 1,), dtype=torch.int64, device=dev)
+            _ffi.call("tfgk_block_sample_count", _p(rowptr), n_rows, _p(nodes), _p(state), h, L, cap_list, k, padding,
+                      _p(out_rowptr), _p(ws), nbytes, st)
+            if cap_edges is None:
+                n_list, total = ctypes.c_int32(), ctypes.c_int64()
+                _ffi.call("tfgk_block_sample_read_total", _p(state), h, _p(out_rowptr), cap_list, ctypes.byref(n_list),
+                          ctypes.byref(total), st)
+                cap_edges, cap_next = total.value, min(limit, n_list.value + total.value)
+                ws, nbytes = _block_workspace(cap_list, cap_edges, dev)
+            out = [torch.empty((max(cap_edges, 1),), dtype=torch.int32, device=dev) for _ in range(3)]
+            out_w = torch.empty((max(cap_edges, 1),), dtype=torch.float32, device=dev)
+            _ffi.call("tfgk_block_sample_fill", _p(rowptr), n_rows, _p(col), _p(w_csr), N, _p(nodes), _p(node_map),
+                      _p(state), h, L, cap_list, cap_edges, k, padding, int(keys[h]), int(rng_stream), _p(out_rowptr),
+                      _p(out[0]), _p(out[1]), _p(out[2]), _p(out_w), _p(ws), nbytes, st)
+            hops.append((out_rowptr, out[0], out[1], out[2], out_w))
+            cap_list = cap_next
+        host = (ctypes.c_int32 * (4 + 2 * L))()
+        _ffi.call("tfgk_block_sample_end", _p(nodes), cap_nodes, N, _p(node_map), _p(state), L, host, st)
+    except BaseException:
+        node_map.fill_(-1)            # the map is shared by every call on this sampler: leave it clean
+        raise
+    sizes = [int(v) for v in host[3:4 + L]]
+    edges = [int(v) for v in host[4 + L:4 + 2 * L]]
+    hops = [(rp, row[:S], local[:S], gcol[:S], w[:S]) for (rp, row, local, gcol, w), S in zip(hops, edges)]
+    return nodes[:sizes[-1]], sizes, hops, int(host[0]), int(host[1])
 
 
 # ---- link prediction: K6 edge scoring, negative sampling ----------------------------------------------------------

@@ -6,4 +6,5 @@ from .graph_utils import (add_self_loop_edge, remove_self_loop_edge, convert_edg
                           negative_sampling_with_start_node, edge_train_test_split, convert_dense_adj_to_edge,
                           convert_dense_assign_to_edge, convert_x_to_3d, reindex_sampled_edge_index,
                           compute_edge_mask_by_node_index, extract_unique_edge)
-from .sampling import RandomNeighborSampler, UniformNeighborSampler, SampledNeighborhood
+from .sampling import (RandomNeighborSampler, UniformNeighborSampler, SampledNeighborhood, SampledBlocks, Block,
+                       SourceRows)

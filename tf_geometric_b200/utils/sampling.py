@@ -8,7 +8,12 @@ Randomness is counter-based (csrc/rng.cuh); pass `seed=` for reproducible draws.
 
 RandomNeighborSampler.sample_neighborhood (an extension of the reference API) grows a seed-node mini-batch hop by hop
 on the device: K13 samples the listed rows of the cached CSR and tfgk_frontier_i32 appends and relabels the new nodes, so
-the work follows the batch, not the graph."""
+the work follows the batch, not the graph.
+
+RandomNeighborSampler.sample_blocks (also an extension) samples the same neighbourhood as layer-wise bipartite blocks:
+block i maps the hop_sizes[L - i] nodes of its input onto the hop_sizes[L - 1 - i] nodes the next layer reads, so every
+layer computes only the rows it must.  The sizes stay on the device until the batch ends, which costs one host
+synchronisation per batch."""
 import torch
 
 from .. import ops, _rng
@@ -83,6 +88,83 @@ class SampledNeighborhood(object):
         self.edge_index_list = edge_index_list
         self.edge_weight_list = edge_weight_list
         self.hop_sizes = hop_sizes
+
+
+class Block(ops.SampledInput):
+    """One layer of a SampledBlocks batch: a bipartite graph from num_src input rows to num_dst output rows, where the
+    output rows are the first num_dst input rows (the same nodes).
+
+    edge_index: int32 [2, S] local (row < num_dst, col < num_src), rows ascending and in draw order within a row.
+    edge_weight: float32 [S].  global_col: int32 [S], the node id of every edge's column.
+    csr: ops.CSR with n_rows = num_dst, n_cols = num_src; its perm is the identity (the edges are already in CSR order).
+    The transposed CSR that the backward needs is built on first use and kept on the block."""
+
+    __slots__ = ("num_src", "num_dst", "edge_index", "edge_weight", "global_col", "csr", "_csr_t", "_w_t")
+
+    def __init__(self, num_src, num_dst, edge_index, edge_weight, global_col, csr):
+        self.num_src, self.num_dst = int(num_src), int(num_dst)
+        self.edge_index, self.edge_weight, self.global_col, self.csr = edge_index, edge_weight, global_col, csr
+        self._csr_t, self._w_t = None, {}
+
+    def transposed(self, reduce=None, weighted=True):
+        """(csr_t, w_t): the stable CSR of the edges keyed by local source (n_rows = num_src, n_cols = num_dst) and the
+        edge weights (ones when not `weighted`) in its order, divided by their destination row's edge count for
+        reduce="mean".  w_t is None for reduce=None and for an unweighted sum."""
+        if self._csr_t is None:
+            row, col = self.edge_index[0], self.edge_index[1]
+            self._csr_t = ops.csr_build(col, row, self.num_src, self.num_dst, ids_in_range=True)
+        if reduce is None or (reduce == "sum" and not weighted):
+            return self._csr_t, None
+        w_t = self._w_t.get((reduce, weighted))
+        if w_t is None:
+            w = self.edge_weight if weighted else torch.ones_like(self.edge_weight)
+            if reduce == "mean":
+                cnt = self.csr.degree_i64().clamp(min=1).to(torch.float32)
+                w = ops.scale_edges(self.edge_index[0], None, w, dl=torch.reciprocal(cnt))
+            w_t = self._w_t[(reduce, weighted)] = ops.permute(w, self._csr_t.perm)
+        return self._csr_t, w_t
+
+
+class SourceRows(ops.SampledInput):
+    """Layer 0's input of a SampledBlocks batch taken from the global [N, F] feature table x without gathering it:
+    mean and sum GraphSAGE aggregate straight from x through the block's global columns and gather only the self rows.
+    shape is (num_src, F), the shape of the gathered table."""
+
+    __slots__ = ("x", "node_index")
+
+    def __init__(self, x, node_index):
+        self.x, self.node_index = x, node_index
+
+    @property
+    def shape(self):
+        return (self.node_index.numel(), self.x.shape[1])
+
+    def gather(self, rows=None):
+        """x[node_index[:rows]] (all source rows by default); differentiable when x requires grad."""
+        from .. import autograd
+        index = self.node_index if rows is None else self.node_index[:rows]
+        if self.x.requires_grad and torch.is_grad_enabled():
+            return autograd.TakeRows.apply(self.x, index)
+        return ops.permute(self.x.detach(), index)
+
+
+class SampledBlocks(object):
+    """A seed-node mini-batch as layer-wise blocks (RandomNeighborSampler.sample_blocks).
+
+    node_index, hop_sizes: those of sample_neighborhood with the same arguments.
+    blocks: one Block per layer, layer 0 nearest the input; block i has num_src = hop_sizes[L - i] and num_dst =
+        hop_sizes[L - 1 - i], and its edge_index / edge_weight are sample_neighborhood's edge_index_list[i] /
+        edge_weight_list[i]."""
+
+    __slots__ = ("node_index", "hop_sizes", "blocks")
+
+    def __init__(self, node_index, hop_sizes, blocks):
+        self.node_index, self.hop_sizes, self.blocks = node_index, hop_sizes, blocks
+
+    def source_rows(self, x):
+        """Layer 0's input for the global feature table x [N, F] (a float32 CUDA tensor)."""
+        x = ops.as_device(x, torch.float32, device=self.node_index.device)
+        return SourceRows(x, self.node_index)
 
 
 class RandomNeighborSampler(_SamplerBase):
@@ -183,6 +265,35 @@ class RandomNeighborSampler(_SamplerBase):
             nodes, n = grown, n + n_new
             hop_sizes.append(n)
         return SampledNeighborhood(nodes[:n], hop_edges[::-1], hop_weights[::-1], hop_sizes)
+
+    def sample_blocks(self, seed_node_index, fanouts, padding=False, seed=None):
+        """sample_neighborhood's batch as layer-wise bipartite blocks (an extension of the reference API); same arguments
+        and the same node list and edges for the same key.  Integer fan-outs and device-resident seeds synchronise the
+        host once per batch; a fan-out of None (every neighbour) adds one read-back for its hop.
+
+        :return: SampledBlocks, on the device"""
+        from .graph_utils import _batch_seed         # graph_utils imports this module
+        seed = _rng.resolve_host(seed)
+        csr, w_csr, rowptr, node_map = self._neighborhood_structure()
+        dev = rowptr.device
+        nodes = ops.as_device(seed_node_index, torch.int32, device=dev).reshape(-1).contiguous()
+        hop_fanouts = [None if k is None else int(k) for k in reversed(list(fanouts))]
+        keys = [_batch_seed(seed, h) for h in range(len(hop_fanouts))]
+        node_index, sizes, hops, n_bad, n_dup = ops.block_sample(rowptr, csr.col, w_csr, nodes, hop_fanouts, keys, node_map,
+                                                                 padding=padding)
+        if n_bad:
+            raise ValueError("seed_node_index holds node ids outside [0, {})".format(node_map.numel()))
+        if n_dup:
+            raise ValueError("seed_node_index holds {} duplicate node ids".format(n_dup))
+        blocks = []
+        for h, (k, (out_rowptr, row, local, gcol, w)) in enumerate(zip(hop_fanouts, hops)):
+            n_dst, n_src = sizes[h], sizes[h + 1]
+            S = row.numel()
+            block_csr = ops.CSR(out_rowptr[:n_dst + 1], local, torch.arange(S, dtype=torch.int32, device=dev), n_dst, n_src)
+            if k is None or k >= ops.DENSE_ROW_DEGREE:      # below it every row is short and build_plan returns None
+                block_csr.plan = ops.build_plan(block_csr)
+            blocks.append(Block(n_src, n_dst, torch.stack([row, local]), w, gcol, block_csr))
+        return SampledBlocks(node_index, sizes, blocks[::-1])
 
 
 class UniformNeighborSampler(_SamplerBase):
