@@ -140,6 +140,22 @@ int tfgk_plan_build(const int64_t *rowptr, int32_t N, int32_t hub_threshold, int
 int tfgk_permute_f32(const float *src, const int32_t *perm, int64_t E, int32_t width, float *dst, void *stream);
 int tfgk_unpermute_f32(const float *src, const int32_t *perm, int64_t E, int32_t width, float *dst, void *stream);
 
+/* ---- feature tables in host memory (utils.HostFeatureTable) --------------------------------------------------------
+ * _register   page-locks [ptr, ptr + bytes) in place (cudaHostRegister, portable | mapped) and returns the address the
+ *             device reads it through.  A range that overlaps a registered one fails (one registration per range).
+ * _unregister waits for the current device's work (so no gather in flight reads the range), then releases a
+ *             registration made by _register (ptr is the same host address).
+ * Both return TFGK_ERR_CUDA with CUDA's message on failure and leave no CUDA error pending. */
+int tfgk_host_register(void *ptr, size_t bytes, void **dev_ptr);
+int tfgk_host_unregister(void *ptr);
+/* out[i*ldo + j] = table[index[i]*ld + j] for j < F, where `table` is host memory the device reads over the host link
+ * (a mapped pointer from tfgk_host_register, or pinned memory under unified addressing).  An id outside [0, n_rows)
+ * writes a row of NaN and reads nothing, so a bad id never touches memory past the registered range.  One warp per
+ * output row, grid-strided over 16 warps per SM; 16-byte accesses when F, ld, ldo and both base pointers allow them,
+ * 4-byte accesses otherwise.  Asynchronous.  Bytes over the link: n * F * 4. */
+int tfgk_gather_rows_mapped_f32(const float *table, int64_t ld, int64_t n_rows, int32_t F, const int32_t *index,
+                                int64_t n, float *out, int64_t ldo, void *stream);
+
 /* ---- GCN normalisation (nn/conv/gcn.py:32-130, utils/graph_utils.py:914-943) -------------------------------- */
 
 /* SparseMatrix.segment_sum(axis=-1) on CSR-ordered values: out[r] = sum of w[rowptr[r]..rowptr[r+1]) in order. */

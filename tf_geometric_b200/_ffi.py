@@ -52,6 +52,9 @@ SIGNATURES = {
                         ctypes.POINTER(_i32), _ptr, _size, _ptr],
     "tfgk_permute_f32": [_ptr, _ptr, _i64, _i32, _ptr, _ptr],
     "tfgk_unpermute_f32": [_ptr, _ptr, _i64, _i32, _ptr, _ptr],
+    "tfgk_host_register": [_ptr, _size, ctypes.POINTER(_ptr)],
+    "tfgk_host_unregister": [_ptr],
+    "tfgk_gather_rows_mapped_f32": [_ptr, _i64, _i64, _i32, _ptr, _i64, _ptr, _i64, _ptr],
     "tfgk_csr_rowsum_f32": [_ptr, _ptr, _i32, _ptr, _ptr],
     "tfgk_deg_inv_f32": [_ptr, _i32, _int, _ptr, _ptr],
     "tfgk_scale_edges_f32": [_ptr, _ptr, _ptr, _i64, _ptr, _ptr, _ptr, _ptr],
@@ -273,6 +276,7 @@ NOT_CAPTURABLE = {
     "tfgk_block_sample_read_total": ("the block sampler", "it returns a hop's edge total to the host"),
     "tfgk_block_sample_fill": ("the block sampler", "it takes a host-side key"),
     "tfgk_block_sample_end": ("the block sampler", "it returns the batch's sizes to the host"),
+    "tfgk_host_register": ("HostFeatureTable", "it page-locks host memory, which a graph cannot record"),
     "tfgk_neg_offsets": ("negative sampling", "it returns the number of candidate pairs to the host"),
     "tfgk_neg_draw": ("negative sampling", "it takes a host-side key"),
     "tfgk_neg_sample_start": ("negative sampling", "it takes a host-side key"),

@@ -4,6 +4,7 @@
 #include "common.cuh"
 #include "scan.cuh"
 #include <string.h>
+#include <algorithm>
 
 namespace tfgk {
 
@@ -73,6 +74,64 @@ __global__ void permute_f32_kernel(const float *__restrict__ src, const int32_t 
         if (inverse) dst[p * width + j] = src[i];
         else         dst[i] = src[p * width + j];
     }
+}
+
+// ---- row gather from a feature table in host memory (tfgk_gather_rows_mapped_f32) -----------------------------------
+// One warp per output row, grid-strided.  A read crosses the host link (microseconds, not HBM's hundreds of
+// nanoseconds), so every SM holds gather warps and each lane issues up to kGatherUnroll loads before it stores.  On an
+// H100 the rate of 400-byte rows was the same with 1, 2 and 8 blocks of 8 warps per SM, so the grid stops at 2 per SM and
+// leaves the rest of each SM to kernels on other streams.  An id outside [0, n_rows) gives a NaN row and no read.
+constexpr int kGatherThreads = 256;
+constexpr int kGatherBlocksPerSm = 2;
+constexpr int kGatherUnroll = 4;
+
+template <typename V>
+__device__ __forceinline__ V nan_vec();
+template <> __device__ __forceinline__ float nan_vec<float>() { return __int_as_float(0x7fc00000); }
+template <> __device__ __forceinline__ float4 nan_vec<float4>() {
+    const float q = __int_as_float(0x7fc00000);
+    return make_float4(q, q, q, q);
+}
+
+// V = float4: F, ld and ldo counted in floats are multiples of 4 and both bases are 16-byte aligned
+template <typename V>
+__device__ __forceinline__ void gather_rows_mapped_body(const float *__restrict__ table, int64_t ld, int64_t n_rows,
+                                                        int32_t F, const int32_t *__restrict__ index, int64_t n,
+                                                        float *__restrict__ out, int64_t ldo) {
+    constexpr int kW = sizeof(V) / sizeof(float);
+    const int lane = threadIdx.x & 31;
+    const int32_t nv = F / kW;                                   // vectors per row
+    const int64_t warps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+    for (int64_t i = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; i < n; i += warps) {
+        const int32_t r = index[i];
+        V *dst = reinterpret_cast<V *>(out + i * ldo);
+        if (r < 0 || (int64_t)r >= n_rows) {
+            for (int32_t c = lane; c < nv; c += 32) dst[c] = nan_vec<V>();
+            continue;
+        }
+        const V *src = reinterpret_cast<const V *>(table + (int64_t)r * ld);
+        for (int32_t c0 = lane; c0 < nv; c0 += 32 * kGatherUnroll) {
+            V v[kGatherUnroll];
+#pragma unroll
+            for (int u = 0; u < kGatherUnroll; ++u)
+                if (c0 + 32 * u < nv) v[u] = src[c0 + 32 * u];
+#pragma unroll
+            for (int u = 0; u < kGatherUnroll; ++u)
+                if (c0 + 32 * u < nv) dst[c0 + 32 * u] = v[u];
+        }
+    }
+}
+
+__global__ void __launch_bounds__(kGatherThreads) gather_rows_mapped_vec4_kernel(
+        const float *__restrict__ table, int64_t ld, int64_t n_rows, int32_t F, const int32_t *__restrict__ index,
+        int64_t n, float *__restrict__ out, int64_t ldo) {
+    gather_rows_mapped_body<float4>(table, ld, n_rows, F, index, n, out, ldo);
+}
+
+__global__ void __launch_bounds__(kGatherThreads) gather_rows_mapped_f32_kernel(
+        const float *__restrict__ table, int64_t ld, int64_t n_rows, int32_t F, const int32_t *__restrict__ index,
+        int64_t n, float *__restrict__ out, int64_t ldo) {
+    gather_rows_mapped_body<float>(table, ld, n_rows, F, index, n, out, ldo);
 }
 
 __global__ void csr_rowsum_kernel(const int64_t *__restrict__ rowptr, const float *__restrict__ w, int32_t N,
@@ -711,6 +770,61 @@ int tfgk_unpermute_f32(const float *src, const int32_t *perm, int64_t E, int32_t
     if (E == 0) return TFGK_OK;
     TFGK_CHECK_ARG(src && perm && dst, "unpermute: null pointer");
     permute_f32_kernel<<<grid_for(E * width), 256, 0, as_stream(stream)>>>(src, perm, E, width, dst, true);
+    TFGK_LAUNCH_CHECK();
+    return TFGK_OK;
+}
+
+// a failed registration call leaves its error as the runtime's last error, which the next launch check would report:
+// clear it and return it with the call's name
+static int host_error(cudaError_t err, const char *what) {
+    cudaGetLastError();
+    return set_error(TFGK_ERR_CUDA, "%s failed: %s", what, cudaGetErrorString(err));
+}
+
+int tfgk_host_register(void *ptr, size_t bytes, void **dev_ptr) {
+    TFGK_CHECK_ARG(ptr != nullptr && dev_ptr != nullptr, "host_register: null pointer");
+    TFGK_CHECK_ARG(bytes > 0, "host_register: empty range");
+    *dev_ptr = nullptr;
+    cudaError_t err = cudaHostRegister(ptr, bytes, cudaHostRegisterPortable | cudaHostRegisterMapped);
+    if (err != cudaSuccess) return host_error(err, "cudaHostRegister");
+    void *dev = nullptr;
+    err = cudaHostGetDevicePointer(&dev, ptr, 0);
+    if (err != cudaSuccess) {
+        cudaHostUnregister(ptr);
+        return host_error(err, "cudaHostGetDevicePointer");
+    }
+    *dev_ptr = dev;
+    return TFGK_OK;
+}
+
+int tfgk_host_unregister(void *ptr) {
+    TFGK_CHECK_ARG(ptr != nullptr, "host_unregister: null pointer");
+    // a gather still in flight on any stream would read the range after it is released
+    cudaError_t err = cudaDeviceSynchronize();
+    if (err != cudaSuccess) return host_error(err, "cudaDeviceSynchronize");
+    err = cudaHostUnregister(ptr);
+    if (err != cudaSuccess) return host_error(err, "cudaHostUnregister");
+    return TFGK_OK;
+}
+
+int tfgk_gather_rows_mapped_f32(const float *table, int64_t ld, int64_t n_rows, int32_t F, const int32_t *index,
+                                int64_t n, float *out, int64_t ldo, void *stream) {
+    TFGK_CHECK_ARG(n >= 0 && n_rows >= 0 && F >= 1, "gather_rows_mapped: bad size (n=%lld, n_rows=%lld, F=%d)",
+                   (long long)n, (long long)n_rows, F);
+    TFGK_CHECK_ARG(ld >= F && ldo >= F, "gather_rows_mapped: need ld >= F and ldo >= F (ld=%lld, ldo=%lld, F=%d)",
+                   (long long)ld, (long long)ldo, F);
+    if (n == 0) return TFGK_OK;
+    TFGK_CHECK_ARG(index && out && (table || n_rows == 0), "gather_rows_mapped: null pointer");
+    const int64_t warps_per_block = kGatherThreads / 32;
+    const unsigned blocks = (unsigned)std::min<int64_t>(ceil_div64(n, warps_per_block),
+                                                        (int64_t)sm_count() * kGatherBlocksPerSm);
+    const bool vec = F % 4 == 0 && ld % 4 == 0 && ldo % 4 == 0 && aligned16(table) && aligned16(out);
+    if (vec)
+        gather_rows_mapped_vec4_kernel<<<blocks, kGatherThreads, 0, as_stream(stream)>>>(table, ld, n_rows, F, index, n,
+                                                                                        out, ldo);
+    else
+        gather_rows_mapped_f32_kernel<<<blocks, kGatherThreads, 0, as_stream(stream)>>>(table, ld, n_rows, F, index, n,
+                                                                                       out, ldo);
     TFGK_LAUNCH_CHECK();
     return TFGK_OK;
 }

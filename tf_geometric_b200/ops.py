@@ -265,6 +265,37 @@ def permute(src, perm, inverse=False):
     return dst
 
 
+# ---- feature tables in host memory (utils.HostFeatureTable) -------------------------------------------------------
+
+def host_register(ptr, nbytes):
+    """Page-lock the host range [ptr, ptr + nbytes) in place; returns the address the device reads it through."""
+    dev = ctypes.c_void_p()
+    _ffi.call("tfgk_host_register", ctypes.c_void_p(ptr), nbytes, ctypes.byref(dev))
+    return dev.value
+
+
+def host_unregister(ptr):
+    """Release a registration made by host_register (ptr is the same host address)."""
+    _ffi.call("tfgk_host_unregister", ctypes.c_void_p(ptr))
+
+
+def gather_rows_mapped(table_ptr, ld, n_rows, num_features, index, out=None):
+    """out[i] = table[index[i], :num_features] for a float32 table in mapped host memory at device address table_ptr
+    (row stride ld floats, n_rows rows); ids outside [0, n_rows) give NaN rows.  index: int32 CUDA vector.  Returns out,
+    a new [n, num_features] tensor on index's device unless given (rows contiguous, any row stride)."""
+    _check(index, torch.int32, "index")
+    n = index.numel()
+    if out is None:
+        out = torch.empty((n, num_features), dtype=torch.float32, device=index.device)
+    elif not (torch.is_tensor(out) and out.is_cuda and out.dtype == torch.float32 and tuple(out.shape) == (n, num_features)):
+        raise TypeError("out must be a float32 CUDA tensor of shape {}".format((n, num_features)))
+    if n:
+        ldo = _row_major_2d(out, "out")
+        _ffi.call("tfgk_gather_rows_mapped_f32", ctypes.c_void_p(table_ptr), ld, n_rows, num_features, _p(index), n,
+                  _p(out), ldo, _stream(out))
+    return out
+
+
 def csr_rowsum(csr, w_csr):
     _check(w_csr, torch.float32, "w_csr")
     out = torch.empty((csr.n_rows,), dtype=torch.float32, device=w_csr.device)

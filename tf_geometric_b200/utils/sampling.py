@@ -13,7 +13,13 @@ the work follows the batch, not the graph.
 RandomNeighborSampler.sample_blocks (also an extension) samples the same neighbourhood as layer-wise bipartite blocks:
 block i maps the hop_sizes[L - i] nodes of its input onto the hop_sizes[L - 1 - i] nodes the next layer reads, so every
 layer computes only the rows it must.  The sizes stay on the device until the batch ends, which costs one host
-synchronisation per batch."""
+synchronisation per batch.
+
+HostFeatureTable keeps an [N, F] float32 feature table in host memory (page-locked in place) and gathers the rows a batch
+reads over the host link (tfgk_gather_rows_mapped_f32), so the table need not fit on the device."""
+import threading
+
+import numpy as np
 import torch
 
 from .. import ops, _rng
@@ -154,17 +160,166 @@ class SampledBlocks(object):
     node_index, hop_sizes: those of sample_neighborhood with the same arguments.
     blocks: one Block per layer, layer 0 nearest the input; block i has num_src = hop_sizes[L - i] and num_dst =
         hop_sizes[L - 1 - i], and its edge_index / edge_weight are sample_neighborhood's edge_index_list[i] /
-        edge_weight_list[i]."""
+        edge_weight_list[i].
+    num_nodes: the node count the sampler checked every id against (None for a batch built by hand)."""
 
-    __slots__ = ("node_index", "hop_sizes", "blocks")
+    __slots__ = ("node_index", "hop_sizes", "blocks", "num_nodes")
 
-    def __init__(self, node_index, hop_sizes, blocks):
+    def __init__(self, node_index, hop_sizes, blocks, num_nodes=None):
         self.node_index, self.hop_sizes, self.blocks = node_index, hop_sizes, blocks
+        self.num_nodes = None if num_nodes is None else int(num_nodes)
 
     def source_rows(self, x):
-        """Layer 0's input for the global feature table x [N, F] (a float32 CUDA tensor)."""
+        """Layer 0's input for the global feature table x [N, F]: a float32 tensor (moved to the device when it is not
+        there), or a HostFeatureTable, whose rows node_index are gathered over the host link into a new [num_src, F]
+        device tensor on the current stream.  For a batch from sample_blocks the ids were checked by the sampler, so the
+        table only needs num_nodes rows and the gather makes no host synchronisation; a batch built by hand takes the
+        checked HostFeatureTable.gather."""
+        if isinstance(x, HostFeatureTable):
+            if self.num_nodes is None:
+                return x.gather(self.node_index)
+            if x.num_rows < self.num_nodes:
+                raise ValueError("the feature table has {} rows; the sampler's graph has {} nodes".format(
+                    x.num_rows, self.num_nodes))
+            return x._gather(self.node_index)
         x = ops.as_device(x, torch.float32, device=self.node_index.device)
         return SourceRows(x, self.node_index)
+
+
+# one registration per host buffer: base address -> [number of open tables over it, bytes, device address of the base]
+_host_lock = threading.RLock()
+_host_registered = {}
+
+
+def _host_range(x, array):
+    """(address, bytes) of the whole host buffer under x: its storage, or for a numpy view the array that owns the
+    memory, so that tables over different views of one buffer share one registration."""
+    st = x.untyped_storage()
+    lo, size = st.data_ptr(), st.nbytes()
+    if isinstance(array, np.ndarray):
+        root = array
+        while isinstance(root.base, np.ndarray):
+            root = root.base
+        if (root.flags.c_contiguous or root.flags.f_contiguous) and root.ctypes.data <= lo and \
+                lo + size <= root.ctypes.data + root.nbytes:
+            lo, size = root.ctypes.data, root.nbytes
+    return lo, size
+
+
+class HostFeatureTable(object):
+    """A float32 feature table [N, F] kept in host memory, whose rows the device gathers over the host link.
+
+    x: a CPU float32 2-D tensor or numpy array with unit column stride (numpy is wrapped without a copy).  A pinned
+    tensor is read as it is; otherwise the whole buffer under x (its storage, or the numpy array that owns the memory)
+    is page-locked in place (no copy, so host memory is not doubled), once however many tables share it, and released
+    when the last of them closes.  The
+    table keeps a reference to x.  A host table is a constant: x must not require grad.
+
+    gather(index) and SampledBlocks.source_rows(table) return new float32 device tensors, bit-identical to x[index].
+    close() (or leaving a `with` block) releases the registration after the current device's pending work; a table
+    that is dropped without close() releases it when it is collected."""
+
+    def __init__(self, x):
+        self._closed = True                 # until registration succeeds: nothing for close() / __del__ to release
+        self._key = None
+        array = x
+        if isinstance(x, np.ndarray):
+            x = torch.from_numpy(x)
+        if not torch.is_tensor(x):
+            raise TypeError("HostFeatureTable takes a CPU tensor or a numpy array (got {})".format(type(x).__name__))
+        if x.is_cuda:
+            raise TypeError("HostFeatureTable takes a table in host memory; a CUDA tensor goes to source_rows directly")
+        if x.dim() != 2:
+            raise TypeError("HostFeatureTable takes a 2-D [N, F] table (got {} dimensions)".format(x.dim()))
+        if x.dtype != torch.float32:
+            raise TypeError("HostFeatureTable takes float32 features (got {})".format(x.dtype))
+        if x.requires_grad:
+            raise ValueError("a host feature table is a constant: x must not require grad")
+        n, F = x.shape
+        if F > 1 and x.stride(1) != 1:
+            raise ValueError("HostFeatureTable needs unit column stride (got strides {})".format(tuple(x.stride())))
+        if n > 1 and x.stride(0) < F:
+            raise ValueError("HostFeatureTable needs rows that do not overlap (got strides {})".format(tuple(x.stride())))
+        self.x = x
+        self._ld = max(F, x.stride(0))
+        base, nbytes = _host_range(x, array)
+        dev_base = 0
+        if x.numel():
+            with _host_lock:
+                owner = next((b for b, (_, size, _) in _host_registered.items()
+                              if b <= base and base + nbytes <= b + size), None)
+                if owner is not None:       # inside a buffer an open table registered: count one more user
+                    entry = _host_registered[owner]
+                    entry[0] += 1
+                    self._key, dev_base = owner, entry[2] + (base - owner)
+                elif x.is_pinned():         # pinned memory is mapped at its host address under unified addressing
+                    dev_base = base
+                else:
+                    dev_base = ops.host_register(base, nbytes)
+                    _host_registered[base] = [1, nbytes, dev_base]
+                    self._key = base
+        self._ptr = dev_base + (x.data_ptr() - base)
+        self._closed = False
+
+    @property
+    def num_rows(self):
+        return self.x.shape[0]
+
+    @property
+    def num_features(self):
+        return self.x.shape[1]
+
+    def _check_open(self):
+        if self._closed:
+            raise RuntimeError("this HostFeatureTable is closed")
+
+    def _gather(self, index, out=None):
+        """gather without the id check: index is an int32 device vector of ids in [0, num_rows)."""
+        self._check_open()
+        if index.numel() == 0 and out is None:
+            return torch.empty((0, self.num_features), dtype=torch.float32, device=index.device)
+        return ops.gather_rows_mapped(self._ptr, self._ld, self.num_rows, self.num_features, index.contiguous(), out)
+
+    def gather(self, index, out=None):
+        """x[index] as a new contiguous float32 device tensor [len(index), F] (or into `out`, a float32 CUDA tensor of
+        that shape), on the current stream.  Ids: an integer vector (int32 on the device is used as it is); ids
+        outside [0, num_rows) raise IndexError after one read-back of their range."""
+        self._check_open()
+        idx = ops.as_device(index).reshape(-1)
+        if idx.dtype.is_floating_point or idx.dtype.is_complex or idx.dtype == torch.bool:
+            raise TypeError("gather takes integer ids (got {})".format(idx.dtype))
+        if idx.numel():
+            lo, hi = torch.stack(torch.aminmax(idx)).tolist()
+            if lo < 0 or hi >= self.num_rows:
+                raise IndexError("index holds ids outside [0, {})".format(self.num_rows))
+        return self._gather(idx.to(torch.int32), out)
+
+    def close(self):
+        """Release the registration this table holds (the last table over a storage unregisters it).  Idempotent."""
+        if self._closed:
+            return
+        self._closed = True
+        key, self._key = self._key, None
+        if key is None:
+            return
+        with _host_lock:
+            entry = _host_registered[key]
+            entry[0] -= 1
+            if entry[0] == 0:
+                del _host_registered[key]
+                ops.host_unregister(key)
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
 
 
 class RandomNeighborSampler(_SamplerBase):
@@ -293,7 +448,7 @@ class RandomNeighborSampler(_SamplerBase):
             if k is None or k >= ops.DENSE_ROW_DEGREE:      # below it every row is short and build_plan returns None
                 block_csr.plan = ops.build_plan(block_csr)
             blocks.append(Block(n_src, n_dst, torch.stack([row, local]), w, gcol, block_csr))
-        return SampledBlocks(node_index, sizes, blocks[::-1])
+        return SampledBlocks(node_index, sizes, blocks[::-1], num_nodes=node_map.numel())
 
 
 class UniformNeighborSampler(_SamplerBase):
