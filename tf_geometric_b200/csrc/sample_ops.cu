@@ -414,7 +414,8 @@ int tfgk_select_flagged_i32(const int32_t *flag, int64_t n, int32_t *out_index, 
     char *ws = static_cast<char *>(workspace);
     int32_t *off = reinterpret_cast<int32_t *>(ws);
     int32_t *sums = reinterpret_cast<int32_t *>(ws + align_up((size_t)(n + 1) * 4));
-    const int rc = exclusive_scan<int32_t, int32_t>(flag, n, n + 1, off, sums, st);
+    // offsets count the non-zero flags, not their values: a flag of 2 or -1 selects its position once, like a 1
+    const int rc = exclusive_scan<int32_t, int32_t, true>(flag, n, n + 1, off, sums, st);
     if (rc != TFGK_OK) return rc;
     int32_t total = 0;
     TFGK_CUDA(cudaMemcpyAsync(&total, off + n, 4, cudaMemcpyDeviceToHost, st));

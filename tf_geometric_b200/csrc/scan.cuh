@@ -13,7 +13,8 @@ constexpr int kScanThreads = 256;
 constexpr int kScanItems = 16;
 constexpr int kScanTile = kScanThreads * kScanItems;
 
-template <typename TIn, typename TOut>
+// kCountNonZero: scan (in[i] != 0) instead of in[i], so that a flag of any non-zero value counts once
+template <typename TIn, typename TOut, bool kCountNonZero = false>
 __global__ void __launch_bounds__(kScanThreads) scan_tile_kernel(const TIn *in, int64_t n_in, int64_t n_out,
                                                                  TOut *out, TOut *__restrict__ tile_sums) {
     // thread t owns items [t*kScanItems, (t+1)*kScanItems) of the tile (blocked arrangement)
@@ -24,7 +25,7 @@ __global__ void __launch_bounds__(kScanThreads) scan_tile_kernel(const TIn *in, 
 #pragma unroll
     for (int i = 0; i < kScanItems; ++i) {
         const int64_t idx = base + i;
-        const TOut x = idx < n_in ? (TOut)in[idx] : (TOut)0;
+        const TOut x = idx < n_in ? (kCountNonZero ? (TOut)(in[idx] != 0) : (TOut)in[idx]) : (TOut)0;
         v[i] = sum;      // exclusive within the thread
         sum += x;
     }
@@ -89,12 +90,13 @@ __global__ void __launch_bounds__(kScanThreads) scan_add_kernel(TOut *__restrict
     }
 }
 
-// out[0..n_out) = exclusive scan of in[0..n_in) (elements beyond n_in count as 0; n_out may be n_in + 1)
-template <typename TIn, typename TOut>
+// out[0..n_out) = exclusive scan of in[0..n_in) (elements beyond n_in count as 0; n_out may be n_in + 1);
+// with kCountNonZero, of (in[i] != 0): out[i] is then the number of non-zero entries before i
+template <typename TIn, typename TOut, bool kCountNonZero = false>
 static int exclusive_scan(const TIn *in, int64_t n_in, int64_t n_out, TOut *out, TOut *tile_sums, cudaStream_t st) {
     const int64_t n_tiles = ceil_div64(n_out, kScanTile);
     if (n_tiles == 0) return TFGK_OK;
-    scan_tile_kernel<TIn, TOut><<<(unsigned)n_tiles, kScanThreads, 0, st>>>(in, n_in, n_out, out, tile_sums);
+    scan_tile_kernel<TIn, TOut, kCountNonZero><<<(unsigned)n_tiles, kScanThreads, 0, st>>>(in, n_in, n_out, out, tile_sums);
     TFGK_LAUNCH_CHECK();
     if (n_tiles > 1) {
         scan_sums_kernel<TOut><<<1, 1024, 0, st>>>(tile_sums, n_tiles);
