@@ -156,6 +156,29 @@ int tfgk_host_unregister(void *ptr);
 int tfgk_gather_rows_mapped_f32(const float *table, int64_t ld, int64_t n_rows, int32_t F, const int32_t *index,
                                 int64_t n, float *out, int64_t ldo, void *stream);
 
+/* ---- a CSR built from an edge list in host memory (utils.HostNeighborSampler) -----------------------------------------
+ * row, col [E] int32 (and w [E] float32) are device-readable pointers to page-locked host memory (tfgk_host_register);
+ * E may be 2^31 or more.  Every entry streams them in edge order, 16 bytes per load where the array is 16-byte aligned.
+ * _id_range   range_host[4] = {min row, max row, min col, max col}, from one pass over both arrays (E > 0).  The
+ *             workspace is at least 16 bytes of device memory.  Synchronises `stream`.
+ * _rowptr     rowptr int64 [n_rows + 1] = exclusive scan of the per-row edge counts; rows outside [0, n_rows) are not
+ *             counted.  Equal to tfgk_csr_build's rowptr of the same edges.  Counts are int64, so a row of 2^31 edges
+ *             or more is counted exactly (the caller refuses it).  Asynchronous.
+ * _select_rows the edges with r0 <= row < r1, in edge order: out_row = row - r0, out_col = col, out_w = w (w may be NULL:
+ *             out_w is then untouched), at most cap < 2^31 of them (the caller knows the count from rowptr).  A stable
+ *             compaction in tiles of 1024 edges: int offsets within a tile, int64 tile offsets.  Sorting its output with
+ *             tfgk_csr_build_in_range(out_row, out_col, count, r1 - r0, ...) gives rows [r0, r1) of the CSR of the whole
+ *             edge list (the selection keeps edge order and the sort is stable).  Asynchronous. */
+int tfgk_mapped_id_range_i32(const int32_t *row, const int32_t *col, int64_t E, int32_t *range_host, void *workspace,
+                             size_t workspace_bytes, void *stream);
+int tfgk_mapped_rowptr_workspace_bytes(int32_t n_rows, size_t *out_bytes);
+int tfgk_mapped_rowptr_i32(const int32_t *row, int64_t E, int32_t n_rows, int64_t *rowptr, void *workspace,
+                           size_t workspace_bytes, void *stream);
+int tfgk_mapped_select_rows_workspace_bytes(int64_t E, size_t *out_bytes);
+int tfgk_mapped_select_rows_i32(const int32_t *row, const int32_t *col, const float *w, int64_t E, int32_t r0,
+                                int32_t r1, int32_t *out_row, int32_t *out_col, float *out_w, int64_t cap,
+                                void *workspace, size_t workspace_bytes, void *stream);
+
 /* ---- GCN normalisation (nn/conv/gcn.py:32-130, utils/graph_utils.py:914-943) -------------------------------- */
 
 /* SparseMatrix.segment_sum(axis=-1) on CSR-ordered values: out[r] = sum of w[rowptr[r]..rowptr[r+1]) in order. */
@@ -597,6 +620,19 @@ int tfgk_block_sample_fill(const int64_t *rowptr, int32_t n_rows, const int32_t 
                            float *out_w, void *workspace, size_t workspace_bytes, void *stream);
 int tfgk_block_sample_end(const int32_t *nodes, int32_t cap_nodes, int32_t N, int32_t *map, const int32_t *state,
                           int32_t n_hops, int32_t *state_host, void *stream);
+/* _fill over a CSR in host memory: col (and w_csr) are device-readable pointers to page-locked host memory, and w_csr may
+ * be NULL (every weight is then 1.0f and nothing is read).  CSR positions are int64, so the CSR may hold 2^31 edges or
+ * more; rowptr stays on the device.  Same rule, same draws and same outputs as tfgk_block_sample_fill over the same CSR.
+ * Each sampled edge reads one 4-byte column (and one 4-byte weight) over the host link.  The workspace is that of
+ * tfgk_block_sample_mapped_workspace_bytes(cap_list, cap_edges), which also serves _count; _begin, _count, _read_total
+ * and _end are shared with the device CSR. */
+int tfgk_block_sample_mapped_workspace_bytes(int32_t cap_list, int64_t cap_edges, size_t *out_bytes);
+int tfgk_block_sample_fill_mapped(const int64_t *rowptr, int32_t n_rows, const int32_t *col, const float *w_csr,
+                                  int32_t N, int32_t *nodes, int32_t *map, int32_t *state, int32_t hop, int32_t n_hops,
+                                  int32_t cap_list, int64_t cap_edges, int32_t k, int padding, uint64_t seed,
+                                  uint32_t rng_stream, const int64_t *out_rowptr, int32_t *out_row, int32_t *out_local,
+                                  int32_t *out_gcol, float *out_w, void *workspace, size_t workspace_bytes,
+                                  void *stream);
 
 /* ---- link prediction (SURVEY.md 8(f)5, demo/demo_gae.py) -------------------------------------------------------- */
 

@@ -55,6 +55,11 @@ SIGNATURES = {
     "tfgk_host_register": [_ptr, _size, ctypes.POINTER(_ptr)],
     "tfgk_host_unregister": [_ptr],
     "tfgk_gather_rows_mapped_f32": [_ptr, _i64, _i64, _i32, _ptr, _i64, _ptr, _i64, _ptr],
+    "tfgk_mapped_id_range_i32": [_ptr, _ptr, _i64, _ptr, _ptr, _size, _ptr],
+    "tfgk_mapped_rowptr_workspace_bytes": [_i32, ctypes.POINTER(_size)],
+    "tfgk_mapped_rowptr_i32": [_ptr, _i64, _i32, _ptr, _ptr, _size, _ptr],
+    "tfgk_mapped_select_rows_workspace_bytes": [_i64, ctypes.POINTER(_size)],
+    "tfgk_mapped_select_rows_i32": [_ptr, _ptr, _ptr, _i64, _i32, _i32, _ptr, _ptr, _ptr, _i64, _ptr, _size, _ptr],
     "tfgk_csr_rowsum_f32": [_ptr, _ptr, _i32, _ptr, _ptr],
     "tfgk_deg_inv_f32": [_ptr, _i32, _int, _ptr, _ptr],
     "tfgk_scale_edges_f32": [_ptr, _ptr, _ptr, _i64, _ptr, _ptr, _ptr, _ptr],
@@ -137,6 +142,9 @@ SIGNATURES = {
     "tfgk_block_sample_fill": [_ptr, _i32, _ptr, _ptr, _i32, _ptr, _ptr, _ptr, _i32, _i32, _i32, _i64, _i32, _int, _u64,
                                _u32, _ptr, _ptr, _ptr, _ptr, _ptr, _ptr, _size, _ptr],
     "tfgk_block_sample_end": [_ptr, _i32, _i32, _ptr, _ptr, _i32, _ptr, _ptr],
+    "tfgk_block_sample_mapped_workspace_bytes": [_i32, _i64, ctypes.POINTER(_size)],
+    "tfgk_block_sample_fill_mapped": [_ptr, _i32, _ptr, _ptr, _i32, _ptr, _ptr, _ptr, _i32, _i32, _i32, _i64, _i32, _int,
+                                      _u64, _u32, _ptr, _ptr, _ptr, _ptr, _ptr, _ptr, _size, _ptr],
     "tfgk_edge_dot_f32": [_ptr, _i64, _i32, _ptr, _ptr, _i64, _i32, _ptr, _ptr],
     "tfgk_neg_offsets_workspace_bytes": [_i32, ctypes.POINTER(_size)],
     "tfgk_neg_offsets": [_ptr, _i32, _int, _ptr, ctypes.POINTER(_i64), _ptr, _size, _ptr],
@@ -276,7 +284,9 @@ NOT_CAPTURABLE = {
     "tfgk_block_sample_read_total": ("the block sampler", "it returns a hop's edge total to the host"),
     "tfgk_block_sample_fill": ("the block sampler", "it takes a host-side key"),
     "tfgk_block_sample_end": ("the block sampler", "it returns the batch's sizes to the host"),
+    "tfgk_block_sample_fill_mapped": ("the host-memory block sampler", "it takes a host-side key"),
     "tfgk_host_register": ("HostFeatureTable", "it page-locks host memory, which a graph cannot record"),
+    "tfgk_mapped_id_range_i32": ("the CSR build of HostNeighborSampler", "it returns the id range to the host"),
     "tfgk_neg_offsets": ("negative sampling", "it returns the number of candidate pairs to the host"),
     "tfgk_neg_draw": ("negative sampling", "it takes a host-side key"),
     "tfgk_neg_sample_start": ("negative sampling", "it takes a host-side key"),

@@ -407,6 +407,132 @@ __global__ void plan_fill_kernel(const int64_t *__restrict__ rowptr, int32_t N, 
     }
 }
 
+// ---- building a CSR from an edge list in host memory (utils.HostNeighborSampler) -----------------------------------
+// Every kernel here streams the mapped edge list in order: thread t of a block reads the 4 consecutive ids at
+// 4 (g * blockDim + t), one 16-byte load when the array is 16-byte aligned, so a warp reads 512 contiguous bytes.
+constexpr int kMapThreads = 256;
+constexpr int kMapTile = 4 * kMapThreads;            // edges per tile of the row selection
+
+// ids[e0 .. e0 + 4) into v; ids past n read as -1.  vec: ids is 16-byte aligned (e0 is a multiple of 4).
+__device__ __forceinline__ void load_ids4(const int32_t *__restrict__ ids, int64_t e0, int64_t n, bool vec, int32_t v[4]) {
+    if (vec && e0 + 4 <= n) {
+        const int4 q = *reinterpret_cast<const int4 *>(ids + e0);
+        v[0] = q.x; v[1] = q.y; v[2] = q.z; v[3] = q.w;
+        return;
+    }
+#pragma unroll
+    for (int j = 0; j < 4; ++j) v[j] = e0 + j < n ? ids[e0 + j] : -1;
+}
+
+// range[0..4) = {min row, max row, min col, max col}, folded with atomics into INT32_MAX / INT32_MIN seeds
+__global__ void mapped_range_init_kernel(int32_t *range) {
+    range[0] = range[2] = INT32_MAX;
+    range[1] = range[3] = INT32_MIN;
+}
+
+__global__ void __launch_bounds__(kMapThreads) mapped_id_range_kernel(const int32_t *__restrict__ row,
+                                                                      const int32_t *__restrict__ col, int64_t E,
+                                                                      bool vec_row, bool vec_col, int32_t *range) {
+    int32_t lo[2] = {INT32_MAX, INT32_MAX}, hi[2] = {INT32_MIN, INT32_MIN};
+    const int64_t n4 = (E + 3) / 4;
+    for (int64_t g = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; g < n4; g += (int64_t)gridDim.x * blockDim.x) {
+        int32_t v[4];
+#pragma unroll
+        for (int a = 0; a < 2; ++a) {
+            load_ids4(a ? col : row, 4 * g, E, a ? vec_col : vec_row, v);
+#pragma unroll
+            for (int j = 0; j < 4; ++j)
+                if (4 * g + j < E) { lo[a] = min(lo[a], v[j]); hi[a] = max(hi[a], v[j]); }
+        }
+    }
+#pragma unroll
+    for (int a = 0; a < 2; ++a) {
+#pragma unroll
+        for (int off = 16; off > 0; off >>= 1) {
+            lo[a] = min(lo[a], __shfl_xor_sync(0xffffffffu, lo[a], off));
+            hi[a] = max(hi[a], __shfl_xor_sync(0xffffffffu, hi[a], off));
+        }
+        if ((threadIdx.x & 31) == 0) {
+            atomicMin(range + 2 * a, lo[a]);
+            atomicMax(range + 2 * a + 1, hi[a]);
+        }
+    }
+}
+
+// counts[r] += 1 per edge of row r (int64 counts, so a row of 2^31 edges or more is counted, then refused by the caller)
+__global__ void __launch_bounds__(kMapThreads) mapped_row_count_kernel(const int32_t *__restrict__ row, int64_t E,
+                                                                       bool vec, int32_t n_rows,
+                                                                       unsigned long long *__restrict__ counts) {
+    const int64_t n4 = (E + 3) / 4;
+    for (int64_t g = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; g < n4; g += (int64_t)gridDim.x * blockDim.x) {
+        int32_t v[4];
+        load_ids4(row, 4 * g, E, vec, v);
+#pragma unroll
+        for (int j = 0; j < 4; ++j)
+            if (v[j] >= 0 && v[j] < n_rows) atomicAdd(counts + v[j], 1ull);
+    }
+}
+
+// the edges of tile blockIdx.x with r0 <= row < r1
+__global__ void __launch_bounds__(kMapThreads) mapped_select_count_kernel(const int32_t *__restrict__ row, int64_t E,
+                                                                          bool vec, int32_t r0, int32_t r1,
+                                                                          int64_t *__restrict__ tile_count) {
+    __shared__ int warp_sum[kMapThreads / 32];
+    int32_t v[4];
+    load_ids4(row, (int64_t)blockIdx.x * kMapTile + 4 * threadIdx.x, E, vec, v);
+    int c = 0;
+#pragma unroll
+    for (int j = 0; j < 4; ++j) c += (v[j] >= r0 && v[j] < r1);
+#pragma unroll
+    for (int off = 16; off > 0; off >>= 1) c += __shfl_xor_sync(0xffffffffu, c, off);
+    if ((threadIdx.x & 31) == 0) warp_sum[threadIdx.x >> 5] = c;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        int total = 0;
+        for (int w = 0; w < kMapThreads / 32; ++w) total += warp_sum[w];
+        tile_count[blockIdx.x] = total;
+    }
+}
+
+// Stable compaction of the tile's selected edges to tile_off[tile] + (selected edges before them in the tile): the
+// offset within a tile is an int, the tile's offset an int64.  Writes row - r0, col and w (when w is not null); nothing
+// at or past cap.
+__global__ void __launch_bounds__(kMapThreads) mapped_select_emit_kernel(
+        const int32_t *__restrict__ row, const int32_t *__restrict__ col, const float *__restrict__ w, int64_t E,
+        bool vec, int32_t r0, int32_t r1, const int64_t *__restrict__ tile_off, int64_t cap,
+        int32_t *__restrict__ out_row, int32_t *__restrict__ out_col, float *__restrict__ out_w) {
+    __shared__ int warp_sum[kMapThreads / 32];
+    const int64_t e0 = (int64_t)blockIdx.x * kMapTile + 4 * threadIdx.x;
+    int32_t v[4];
+    load_ids4(row, e0, E, vec, v);
+    int c = 0;
+#pragma unroll
+    for (int j = 0; j < 4; ++j) c += (v[j] >= r0 && v[j] < r1);
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    int incl = c;
+#pragma unroll
+    for (int off = 1; off < 32; off <<= 1) {
+        const int y = __shfl_up_sync(0xffffffffu, incl, off);
+        if (lane >= off) incl += y;
+    }
+    if (lane == 31) warp_sum[warp] = incl;
+    __syncthreads();
+    int before = incl - c;
+    for (int q = 0; q < warp; ++q) before += warp_sum[q];
+    int64_t p = tile_off[blockIdx.x] + before;
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+        if (v[j] >= r0 && v[j] < r1) {
+            if (p < cap) {
+                out_row[p] = v[j] - r0;
+                out_col[p] = col[e0 + j];
+                if (w) out_w[p] = w[e0 + j];
+            }
+            ++p;
+        }
+    }
+}
+
 struct CsrWorkspace {
     size_t off_flag, off_keys_a, off_keys_b, off_vals_b, off_hist, off_sums, off_counts, total;
     int nblk;
@@ -825,6 +951,90 @@ int tfgk_gather_rows_mapped_f32(const float *table, int64_t ld, int64_t n_rows, 
     else
         gather_rows_mapped_f32_kernel<<<blocks, kGatherThreads, 0, as_stream(stream)>>>(table, ld, n_rows, F, index, n,
                                                                                        out, ldo);
+    TFGK_LAUNCH_CHECK();
+    return TFGK_OK;
+}
+
+static unsigned mapped_grid(int64_t E) {
+    return (unsigned)std::max<int64_t>(1, std::min<int64_t>(ceil_div64(ceil_div64(E, 4), kMapThreads),
+                                                            (int64_t)sm_count() * 8));
+}
+
+int tfgk_mapped_id_range_i32(const int32_t *row, const int32_t *col, int64_t E, int32_t *range_host, void *workspace,
+                             size_t workspace_bytes, void *stream) {
+    TFGK_CHECK_ARG(E > 0 && range_host != nullptr, "mapped_id_range: bad argument (E=%lld)", (long long)E);
+    TFGK_CHECK_ARG(row && col, "mapped_id_range: null edge list");
+    if (workspace == nullptr || workspace_bytes < 16)
+        return set_error(TFGK_ERR_WORKSPACE, "mapped_id_range: workspace too small (%zu < 16 bytes)", workspace_bytes);
+    cudaStream_t st = as_stream(stream);
+    int32_t *range = static_cast<int32_t *>(workspace);
+    mapped_range_init_kernel<<<1, 1, 0, st>>>(range);
+    TFGK_LAUNCH_CHECK();
+    mapped_id_range_kernel<<<mapped_grid(E), kMapThreads, 0, st>>>(row, col, E, aligned16(row), aligned16(col), range);
+    TFGK_LAUNCH_CHECK();
+    TFGK_CUDA(cudaMemcpyAsync(range_host, range, 16, cudaMemcpyDeviceToHost, st));
+    TFGK_CUDA(cudaStreamSynchronize(st));
+    return TFGK_OK;
+}
+
+int tfgk_mapped_rowptr_workspace_bytes(int32_t n_rows, size_t *out_bytes) {
+    TFGK_CHECK_ARG(out_bytes != nullptr && n_rows >= 0, "mapped_rowptr_workspace_bytes: bad argument");
+    *out_bytes = scan_scratch_bytes((int64_t)n_rows + 1);
+    return TFGK_OK;
+}
+
+int tfgk_mapped_rowptr_i32(const int32_t *row, int64_t E, int32_t n_rows, int64_t *rowptr, void *workspace,
+                           size_t workspace_bytes, void *stream) {
+    TFGK_CHECK_ARG(E >= 0 && n_rows >= 0, "mapped_rowptr: bad size (E=%lld, n_rows=%d)", (long long)E, n_rows);
+    TFGK_CHECK_ARG(rowptr != nullptr && (E == 0 || row != nullptr), "mapped_rowptr: null pointer");
+    size_t need = 0;
+    tfgk_mapped_rowptr_workspace_bytes(n_rows, &need);
+    if (workspace == nullptr || workspace_bytes < need)
+        return set_error(TFGK_ERR_WORKSPACE, "mapped_rowptr: workspace too small (%zu < %zu bytes)", workspace_bytes, need);
+    cudaStream_t st = as_stream(stream);
+    TFGK_CUDA(cudaMemsetAsync(rowptr, 0, ((size_t)n_rows + 1) * 8, st));
+    if (E > 0 && n_rows > 0) {
+        mapped_row_count_kernel<<<mapped_grid(E), kMapThreads, 0, st>>>(row, E, aligned16(row), n_rows,
+                                                                       reinterpret_cast<unsigned long long *>(rowptr));
+        TFGK_LAUNCH_CHECK();
+    }
+    // in place: each scan thread reads its counts before it writes their offsets
+    return exclusive_scan<int64_t, int64_t>(rowptr, n_rows, (int64_t)n_rows + 1, rowptr,
+                                            static_cast<int64_t *>(workspace), st);
+}
+
+int tfgk_mapped_select_rows_workspace_bytes(int64_t E, size_t *out_bytes) {
+    TFGK_CHECK_ARG(out_bytes != nullptr && E >= 0, "mapped_select_rows_workspace_bytes: bad argument");
+    const int64_t tiles = ceil_div64(E, kMapTile);
+    *out_bytes = align_up((size_t)(tiles + 1) * 8) + scan_scratch_bytes(tiles + 1);
+    return TFGK_OK;
+}
+
+int tfgk_mapped_select_rows_i32(const int32_t *row, const int32_t *col, const float *w, int64_t E, int32_t r0,
+                                int32_t r1, int32_t *out_row, int32_t *out_col, float *out_w, int64_t cap,
+                                void *workspace, size_t workspace_bytes, void *stream) {
+    TFGK_CHECK_ARG(E >= 0 && r0 >= 0 && r1 >= r0 && cap >= 0 && cap < (1ll << 31),
+                   "mapped_select_rows: bad size (E=%lld, rows [%d, %d), cap=%lld)", (long long)E, r0, r1, (long long)cap);
+    if (E == 0 || cap == 0 || r1 == r0) return TFGK_OK;
+    TFGK_CHECK_ARG(row && col && out_row && out_col && (!w || out_w), "mapped_select_rows: null pointer");
+    size_t need = 0;
+    tfgk_mapped_select_rows_workspace_bytes(E, &need);
+    if (workspace == nullptr || workspace_bytes < need)
+        return set_error(TFGK_ERR_WORKSPACE, "mapped_select_rows: workspace too small (%zu < %zu bytes)", workspace_bytes,
+                         need);
+    const int64_t tiles = ceil_div64(E, kMapTile);
+    TFGK_CHECK_ARG(tiles < (1ll << 31), "mapped_select_rows: %lld edges are too many tiles", (long long)E);
+    cudaStream_t st = as_stream(stream);
+    char *ws = static_cast<char *>(workspace);
+    int64_t *tile_off = reinterpret_cast<int64_t *>(ws);
+    int64_t *sums = reinterpret_cast<int64_t *>(ws + align_up((size_t)(tiles + 1) * 8));
+    const bool vec = aligned16(row);
+    mapped_select_count_kernel<<<(unsigned)tiles, kMapThreads, 0, st>>>(row, E, vec, r0, r1, tile_off);
+    TFGK_LAUNCH_CHECK();
+    int rc = exclusive_scan<int64_t, int64_t>(tile_off, tiles, tiles, tile_off, sums, st);
+    if (rc != TFGK_OK) return rc;
+    mapped_select_emit_kernel<<<(unsigned)tiles, kMapThreads, 0, st>>>(row, col, w, E, vec, r0, r1, tile_off, cap, out_row,
+                                                                       out_col, out_w);
     TFGK_LAUNCH_CHECK();
     return TFGK_OK;
 }

@@ -105,14 +105,22 @@ __global__ void sample_rows_count_kernel(const int64_t *__restrict__ rowptr, int
     cnt[t] = num;
 }
 
+// the reservoir's order-free maximum on a CSR position (positions are >= 0, so the unsigned 64-bit order is theirs)
+__device__ __forceinline__ void atomic_max_pos(int32_t *p, int32_t v) { atomicMax(p, v); }
+__device__ __forceinline__ void atomic_max_pos(int64_t *p, int64_t v) {
+    atomicMax(reinterpret_cast<unsigned long long *>(p), (unsigned long long)v);
+}
+
 // The fill of K13.  kBlock (the block sampler) also writes every sampled edge's global column col[pos] and weight
-// w_csr[pos], once its position is final; the plain instantiation leaves that to the caller's gathers.
-template <bool kBlock>
+// w_csr[pos] (1.0f when w_csr is null), once its position is final; the plain instantiation leaves that to the caller's
+// gathers.  TPos is the type of the CSR positions: int32_t for a CSR on the device, int64_t for one in host memory, which
+// may hold 2^31 edges or more.
+template <bool kBlock, typename TPos>
 __device__ __forceinline__ void sample_rows_fill_body(const int64_t *__restrict__ rowptr, int32_t n_rows,
                                                       const int32_t *__restrict__ rows, int32_t n_list, int k,
                                                       double ratio, int padding, uint64_t seed, uint32_t stream,
                                                       const int64_t *__restrict__ out_rowptr, int32_t *__restrict__ out_row,
-                                                      int32_t *__restrict__ out_pos, const int32_t *__restrict__ csr_col,
+                                                      TPos *__restrict__ out_pos, const int32_t *__restrict__ csr_col,
                                                       const float *__restrict__ w_csr, int32_t *__restrict__ out_gcol,
                                                       float *__restrict__ out_w) {
     __shared__ int32_t long_rows[kRowsPerCta];
@@ -136,20 +144,20 @@ __device__ __forceinline__ void sample_rows_fill_body(const int64_t *__restrict_
                     for (int i = 0; i < num; ++i) out_row[o + i] = (int32_t)t;
                 if (rule == kSampleReplace) {
                     for (int i = 0; i < num; ++i)
-                        out_pos[o + i] = (int32_t)(start + random_below(seed, stream, base + (uint64_t)i, (uint32_t)deg));
+                        out_pos[o + i] = (TPos)(start + random_below(seed, stream, base + (uint64_t)i, (uint32_t)deg));
                 } else {
-                    for (int i = 0; i < num; ++i) out_pos[o + i] = (int32_t)(start + i);
+                    for (int i = 0; i < num; ++i) out_pos[o + i] = (TPos)(start + i);
                     if (rule == kSampleReservoir)
                         for (int i = num; i < deg; ++i) {
                             const uint32_t j = random_below(seed, stream, base + (uint64_t)i, (uint32_t)(i + 1));
-                            if (j < (uint32_t)num) out_pos[o + j] = (int32_t)(start + i);
+                            if (j < (uint32_t)num) out_pos[o + j] = (TPos)(start + i);
                         }
                 }
                 if constexpr (kBlock)
                     for (int i = 0; i < num; ++i) {
-                        const int32_t p = out_pos[o + i];
+                        const TPos p = out_pos[o + i];
                         out_gcol[o + i] = csr_col[p];
-                        out_w[o + i] = w_csr[p];
+                        out_w[o + i] = w_csr ? w_csr[p] : 1.0f;
                     }
             }
         }
@@ -168,7 +176,7 @@ __device__ __forceinline__ void sample_rows_fill_body(const int64_t *__restrict_
         const uint64_t base = (uint64_t)r << 32;
         for (int i = threadIdx.x; i < num; i += kRowsPerCta) {
             if (out_row) out_row[o + i] = (int32_t)tl;
-            out_pos[o + i] = (int32_t)(start + (rule == kSampleReplace
+            out_pos[o + i] = (TPos)(start + (rule == kSampleReplace
                                                     ? random_below(seed, stream, base + (uint64_t)i, (uint32_t)deg) : i));
         }
     }
@@ -185,7 +193,7 @@ __device__ __forceinline__ void sample_rows_fill_body(const int64_t *__restrict_
         const uint64_t base = (uint64_t)r << 32;
         for (int i = num + threadIdx.x; i < deg; i += kRowsPerCta) {
             const uint32_t j = random_below(seed, stream, base + (uint64_t)i, (uint32_t)(i + 1));
-            if (j < (uint32_t)num) atomicMax(out_pos + o + j, (int32_t)(start + i));
+            if (j < (uint32_t)num) atomic_max_pos(out_pos + o + j, (TPos)(start + i));
         }
     }
     if constexpr (kBlock) {
@@ -197,9 +205,9 @@ __device__ __forceinline__ void sample_rows_fill_body(const int64_t *__restrict_
             sample_rule((int)(rowptr[r + 1] - rowptr[r]), k, ratio, padding, num);
             const int64_t o = out_rowptr[tl];
             for (int i = threadIdx.x; i < num; i += kRowsPerCta) {
-                const int32_t p = out_pos[o + i];
+                const TPos p = out_pos[o + i];
                 out_gcol[o + i] = csr_col[p];
-                out_w[o + i] = w_csr[p];
+                out_w[o + i] = w_csr ? w_csr[p] : 1.0f;
             }
         }
     }
@@ -210,7 +218,7 @@ sample_rows_fill_kernel(const int64_t *__restrict__ rowptr, int32_t n_rows, cons
                         int32_t n_list, int k, double ratio, int padding, uint64_t seed, uint32_t stream,
                         const int64_t *__restrict__ out_rowptr, int32_t *__restrict__ out_row,
                         int32_t *__restrict__ out_pos) {
-    sample_rows_fill_body<false>(rowptr, n_rows, rows, n_list, k, ratio, padding, seed, stream, out_rowptr, out_row,
+    sample_rows_fill_body<false, int32_t>(rowptr, n_rows, rows, n_list, k, ratio, padding, seed, stream, out_rowptr, out_row,
                                  out_pos, nullptr, nullptr, nullptr, nullptr);
 }
 
@@ -327,8 +335,21 @@ block_fill_kernel(const int64_t *__restrict__ rowptr, int32_t n_rows, const int3
                   const int64_t *__restrict__ out_rowptr, int32_t *__restrict__ out_row, int32_t *__restrict__ out_pos,
                   const int32_t *__restrict__ csr_col, const float *__restrict__ w_csr, int32_t *__restrict__ out_gcol,
                   float *__restrict__ out_w) {
-    sample_rows_fill_body<true>(rowptr, n_rows, rows, *n_list, k, -1.0, padding, seed, stream, out_rowptr, out_row,
-                                out_pos, csr_col, w_csr, out_gcol, out_w);
+    sample_rows_fill_body<true, int32_t>(rowptr, n_rows, rows, *n_list, k, -1.0, padding, seed, stream, out_rowptr,
+                                         out_row, out_pos, csr_col, w_csr, out_gcol, out_w);
+}
+
+// the same fill over a CSR in host memory: csr_col and w_csr (or null: every weight 1.0f) are read over the host link,
+// one 4-byte column (and weight) per sampled edge, at int64 positions.  The minimum of 4 CTAs per SM leaves ptxas room
+// for the 64-bit positions (left to itself it chose 40 registers and spilled).
+__global__ void __launch_bounds__(kRowsPerCta, 4)
+block_fill_mapped_kernel(const int64_t *__restrict__ rowptr, int32_t n_rows, const int32_t *__restrict__ rows,
+                         const int32_t *__restrict__ n_list, int k, int padding, uint64_t seed, uint32_t stream,
+                         const int64_t *__restrict__ out_rowptr, int32_t *__restrict__ out_row,
+                         int64_t *__restrict__ out_pos, const int32_t *__restrict__ csr_col,
+                         const float *__restrict__ w_csr, int32_t *__restrict__ out_gcol, float *__restrict__ out_w) {
+    sample_rows_fill_body<true, int64_t>(rowptr, n_rows, rows, *n_list, k, -1.0, padding, seed, stream, out_rowptr,
+                                         out_row, out_pos, csr_col, w_csr, out_gcol, out_w);
 }
 
 __global__ void block_first_kernel(const int32_t *__restrict__ cols, const int64_t *__restrict__ S, int32_t N,
@@ -645,14 +666,15 @@ int tfgk_frontier_i32(const int32_t *cols, int64_t S, int32_t N, int32_t *nodes,
 
 // ---- block sampler (include/tfgk.h) -----------------------------------------------------------------------------
 namespace {
+// pos_bytes: the size of a CSR position, 4 on the device, 8 for a CSR in host memory
 struct BlockWorkspace {
     size_t off_sums, off_pos, off_flag, off_off, total;
-    BlockWorkspace(int32_t cap_list, int64_t cap_edges) {
+    BlockWorkspace(int32_t cap_list, int64_t cap_edges, size_t pos_bytes = 4) {
         size_t sums = scan_scratch_bytes((int64_t)cap_list + 1);
         if (scan_scratch_bytes(cap_edges + 1) > sums) sums = scan_scratch_bytes(cap_edges + 1);
         off_sums = align_up(((size_t)cap_list + 1) * 4);                   // per-row counts first
         off_pos = off_sums + sums;
-        off_flag = off_pos + align_up((size_t)(cap_edges > 0 ? cap_edges : 1) * 4);
+        off_flag = off_pos + align_up((size_t)(cap_edges > 0 ? cap_edges : 1) * pos_bytes);
         off_off = off_flag + align_up((size_t)(cap_edges + 1) * 4);
         total = off_off + align_up((size_t)(cap_edges + 1) * 4);
     }
@@ -660,8 +682,8 @@ struct BlockWorkspace {
 }  // namespace
 
 static int block_workspace_check(const char *fn, int32_t cap_list, int64_t cap_edges, void *workspace,
-                                 size_t workspace_bytes) {
-    const size_t need = BlockWorkspace(cap_list, cap_edges).total;
+                                 size_t workspace_bytes, size_t pos_bytes = 4) {
+    const size_t need = BlockWorkspace(cap_list, cap_edges, pos_bytes).total;
     if (workspace == nullptr || workspace_bytes < need)
         return set_error(TFGK_ERR_WORKSPACE, "%s: workspace too small (%zu < %zu bytes)", fn, workspace_bytes, need);
     return TFGK_OK;
@@ -671,6 +693,13 @@ int tfgk_block_sample_workspace_bytes(int32_t cap_list, int64_t cap_edges, size_
     TFGK_CHECK_ARG(out_bytes != nullptr && cap_list >= 0 && cap_edges >= 0 && cap_edges < (1ll << 31) - 1,
                    "block_sample_workspace_bytes: bad argument");
     *out_bytes = BlockWorkspace(cap_list, cap_edges).total;
+    return TFGK_OK;
+}
+
+int tfgk_block_sample_mapped_workspace_bytes(int32_t cap_list, int64_t cap_edges, size_t *out_bytes) {
+    TFGK_CHECK_ARG(out_bytes != nullptr && cap_list >= 0 && cap_edges >= 0 && cap_edges < (1ll << 31) - 1,
+                   "block_sample_mapped_workspace_bytes: bad argument");
+    *out_bytes = BlockWorkspace(cap_list, cap_edges, 8).total;
     return TFGK_OK;
 }
 
@@ -723,32 +752,42 @@ int tfgk_block_sample_read_total(const int32_t *state, int32_t hop, const int64_
     return TFGK_OK;
 }
 
-int tfgk_block_sample_fill(const int64_t *rowptr, int32_t n_rows, const int32_t *col, const float *w_csr, int32_t N,
-                           int32_t *nodes, int32_t *map, int32_t *state, int32_t hop, int32_t n_hops, int32_t cap_list,
-                           int64_t cap_edges, int32_t k, int padding, uint64_t seed, uint32_t rng_stream,
-                           const int64_t *out_rowptr, int32_t *out_row, int32_t *out_local, int32_t *out_gcol,
-                           float *out_w, void *workspace, size_t workspace_bytes, void *stream) {
-    int rc = check_sample_mode("block_sample_fill", k, -1.0, padding);
+}  // extern "C"
+
+// tfgk_block_sample_fill and _fill_mapped: K13's fill at positions of type TPos, then the frontier
+template <typename TPos>
+static int block_sample_fill(const char *fn, const int64_t *rowptr, int32_t n_rows, const int32_t *col,
+                             const float *w_csr, int32_t N, int32_t *nodes, int32_t *map, int32_t *state, int32_t hop,
+                             int32_t n_hops, int32_t cap_list, int64_t cap_edges, int32_t k, int padding, uint64_t seed,
+                             uint32_t rng_stream, const int64_t *out_rowptr, int32_t *out_row, int32_t *out_local,
+                             int32_t *out_gcol, float *out_w, void *workspace, size_t workspace_bytes, void *stream) {
+    constexpr bool kMapped = sizeof(TPos) == 8;
+    int rc = check_sample_mode(fn, k, -1.0, padding);
     if (rc != TFGK_OK) return rc;
     TFGK_CHECK_ARG(n_rows >= 0 && N >= 0 && hop >= 0 && hop < n_hops && cap_list >= 0 && cap_edges >= 0 &&
-                   cap_edges < (1ll << 31) - 1, "block_sample_fill: bad size");
-    TFGK_CHECK_ARG(state && out_rowptr, "block_sample_fill: null pointer");
-    if ((rc = block_workspace_check("block_sample_fill", cap_list, cap_edges, workspace, workspace_bytes)) != TFGK_OK)
+                   cap_edges < (1ll << 31) - 1, "%s: bad size", fn);
+    TFGK_CHECK_ARG(state && out_rowptr, "%s: null pointer", fn);
+    if ((rc = block_workspace_check(fn, cap_list, cap_edges, workspace, workspace_bytes, sizeof(TPos))) != TFGK_OK)
         return rc;
     cudaStream_t st = as_stream(stream);
     char *ws = static_cast<char *>(workspace);
-    const BlockWorkspace L(cap_list, cap_edges);
-    int32_t *pos = reinterpret_cast<int32_t *>(ws + L.off_pos);
+    const BlockWorkspace L(cap_list, cap_edges, sizeof(TPos));
+    TPos *pos = reinterpret_cast<TPos *>(ws + L.off_pos);
     int32_t *flag = reinterpret_cast<int32_t *>(ws + L.off_flag);
     int32_t *off = reinterpret_cast<int32_t *>(ws + L.off_off);
     const int32_t *n_list = state + kStateSizes + hop;
     const int64_t *S = out_rowptr + cap_list;               // listed rows past the count add no edges
     if (cap_list > 0 && cap_edges > 0) {
-        TFGK_CHECK_ARG(rowptr && col && w_csr && nodes && map && out_row && out_local && out_gcol && out_w,
-                       "block_sample_fill: null pointer");
-        block_fill_kernel<<<(unsigned)ceil_div64(cap_list, kRowsPerCta), kRowsPerCta, 0, st>>>(
-            rowptr, n_rows, nodes, n_list, k, padding, seed, rng_stream, out_rowptr, out_row, pos, col, w_csr, out_gcol,
-            out_w);
+        TFGK_CHECK_ARG(rowptr && col && (w_csr || kMapped) && nodes && map && out_row && out_local && out_gcol && out_w,
+                       "%s: null pointer", fn);
+        const unsigned grid = (unsigned)ceil_div64(cap_list, kRowsPerCta);
+        if constexpr (kMapped)
+            block_fill_mapped_kernel<<<grid, kRowsPerCta, 0, st>>>(rowptr, n_rows, nodes, n_list, k, padding, seed,
+                                                                  rng_stream, out_rowptr, out_row, pos, col, w_csr,
+                                                                  out_gcol, out_w);
+        else
+            block_fill_kernel<<<grid, kRowsPerCta, 0, st>>>(rowptr, n_rows, nodes, n_list, k, padding, seed, rng_stream,
+                                                           out_rowptr, out_row, pos, col, w_csr, out_gcol, out_w);
         TFGK_LAUNCH_CHECK();
         block_first_kernel<<<grid_for(cap_edges), 256, 0, st>>>(out_gcol, S, N, map, state);
         TFGK_LAUNCH_CHECK();
@@ -767,6 +806,29 @@ int tfgk_block_sample_fill(const int64_t *rowptr, int32_t n_rows, const int32_t 
     block_sizes_kernel<<<1, 1, 0, st>>>(S, off + cap_edges, hop, n_hops, state);
     TFGK_LAUNCH_CHECK();
     return TFGK_OK;
+}
+
+extern "C" {
+
+int tfgk_block_sample_fill(const int64_t *rowptr, int32_t n_rows, const int32_t *col, const float *w_csr, int32_t N,
+                           int32_t *nodes, int32_t *map, int32_t *state, int32_t hop, int32_t n_hops, int32_t cap_list,
+                           int64_t cap_edges, int32_t k, int padding, uint64_t seed, uint32_t rng_stream,
+                           const int64_t *out_rowptr, int32_t *out_row, int32_t *out_local, int32_t *out_gcol,
+                           float *out_w, void *workspace, size_t workspace_bytes, void *stream) {
+    return block_sample_fill<int32_t>("block_sample_fill", rowptr, n_rows, col, w_csr, N, nodes, map, state, hop, n_hops,
+                                      cap_list, cap_edges, k, padding, seed, rng_stream, out_rowptr, out_row, out_local,
+                                      out_gcol, out_w, workspace, workspace_bytes, stream);
+}
+
+int tfgk_block_sample_fill_mapped(const int64_t *rowptr, int32_t n_rows, const int32_t *col, const float *w_csr,
+                                  int32_t N, int32_t *nodes, int32_t *map, int32_t *state, int32_t hop, int32_t n_hops,
+                                  int32_t cap_list, int64_t cap_edges, int32_t k, int padding, uint64_t seed,
+                                  uint32_t rng_stream, const int64_t *out_rowptr, int32_t *out_row, int32_t *out_local,
+                                  int32_t *out_gcol, float *out_w, void *workspace, size_t workspace_bytes,
+                                  void *stream) {
+    return block_sample_fill<int64_t>("block_sample_fill_mapped", rowptr, n_rows, col, w_csr, N, nodes, map, state, hop,
+                                      n_hops, cap_list, cap_edges, k, padding, seed, rng_stream, out_rowptr, out_row,
+                                      out_local, out_gcol, out_w, workspace, workspace_bytes, stream);
 }
 
 int tfgk_block_sample_end(const int32_t *nodes, int32_t cap_nodes, int32_t N, int32_t *map, const int32_t *state,

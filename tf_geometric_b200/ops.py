@@ -296,6 +296,54 @@ def gather_rows_mapped(table_ptr, ld, n_rows, num_features, index, out=None):
     return out
 
 
+# ---- a CSR built from an edge list in host memory (utils.HostNeighborSampler) -------------------------------------
+# row_ptr, col_ptr, w_ptr: device addresses of page-locked host arrays (host_register), int32 / int32 / float32 [E]
+
+def mapped_id_range(row_ptr, col_ptr, num_edges, device):
+    """(min row, max row, min col, max col) of an edge list in host memory with num_edges > 0 edges (synchronises)."""
+    ws = torch.empty((16,), dtype=torch.uint8, device=device)
+    out = (ctypes.c_int32 * 4)()
+    _ffi.call("tfgk_mapped_id_range_i32", ctypes.c_void_p(row_ptr), ctypes.c_void_p(col_ptr), num_edges, out, _p(ws), 16,
+              _stream(ws))
+    return tuple(int(v) for v in out)
+
+
+def mapped_rowptr(row_ptr, num_edges, n_rows, device):
+    """int64 [n_rows + 1] device rowptr of the edge list in host memory (rows outside [0, n_rows) are not counted)."""
+    need = ctypes.c_size_t()
+    _ffi.call("tfgk_mapped_rowptr_workspace_bytes", n_rows, ctypes.byref(need))
+    ws = torch.empty((need.value,), dtype=torch.uint8, device=device)
+    rowptr = torch.empty((n_rows + 1,), dtype=torch.int64, device=device)
+    _ffi.call("tfgk_mapped_rowptr_i32", ctypes.c_void_p(row_ptr), num_edges, n_rows, _p(rowptr), _p(ws), need.value,
+              _stream(rowptr))
+    return rowptr
+
+
+def mapped_csr_range(row_ptr, col_ptr, w_ptr, num_edges, r0, r1, n_range, n_cols, device):
+    """Rows [r0, r1) of the stable row-sorted CSR of the edge list in host memory, which hold n_range < 2^31 edges:
+    (col int32 [n_range], weights float32 [n_range] or None when w_ptr is None), on the device.  The edges are selected in
+    edge order (tfgk_mapped_select_rows_i32), sorted by row - r0 with the stable radix sort of csr_build and permuted."""
+    need = ctypes.c_size_t()
+    _ffi.call("tfgk_mapped_select_rows_workspace_bytes", num_edges, ctypes.byref(need))
+    ws = torch.empty((max(need.value, 1),), dtype=torch.uint8, device=device)
+    sel_row = torch.empty((n_range,), dtype=torch.int32, device=device)
+    sel_col = torch.empty((n_range,), dtype=torch.int32, device=device)
+    sel_w = None if w_ptr is None else torch.empty((n_range,), dtype=torch.float32, device=device)
+    _ffi.call("tfgk_mapped_select_rows_i32", ctypes.c_void_p(row_ptr), ctypes.c_void_p(col_ptr),
+              None if w_ptr is None else ctypes.c_void_p(w_ptr), num_edges, r0, r1, _p(sel_row), _p(sel_col), _p(sel_w),
+              n_range, _p(ws), need.value, _stream(ws))
+    del ws
+    _ffi.call("tfgk_csr_workspace_bytes", n_range, r1 - r0, ctypes.byref(need))
+    ws = torch.empty((max(need.value, 1),), dtype=torch.uint8, device=device)
+    rowptr = torch.empty((r1 - r0 + 1,), dtype=torch.int64, device=device)
+    col = torch.empty((n_range,), dtype=torch.int32, device=device)
+    perm = torch.empty((n_range,), dtype=torch.int32, device=device)
+    _ffi.call("tfgk_csr_build_in_range", _p(sel_row), _p(sel_col), n_range, r1 - r0, n_cols, _p(rowptr), _p(col),
+              _p(perm), _p(ws), need.value, _stream(ws))
+    del ws, sel_row, sel_col, rowptr
+    return col, None if sel_w is None else permute(sel_w, perm)
+
+
 def csr_rowsum(csr, w_csr):
     _check(w_csr, torch.float32, "w_csr")
     out = torch.empty((csr.n_rows,), dtype=torch.float32, device=w_csr.device)
@@ -1024,9 +1072,9 @@ def block_capacities(n_listed, k, limit):
     return n_listed * k, min(limit, n_listed * (1 + k))
 
 
-def _block_workspace(cap_list, cap_edges, device):
+def _block_workspace(cap_list, cap_edges, device, entry="tfgk_block_sample_workspace_bytes"):
     need = ctypes.c_size_t()
-    _ffi.call("tfgk_block_sample_workspace_bytes", cap_list, cap_edges, ctypes.byref(need))
+    _ffi.call(entry, cap_list, cap_edges, ctypes.byref(need))
     return torch.empty((need.value,), dtype=torch.uint8, device=device), need.value
 
 
@@ -1041,15 +1089,35 @@ def block_sample(rowptr, col, w_csr, seeds, fanouts, keys, node_map, padding=Fal
     n_bad / n_dup count seeds outside [0, N) and repeated seeds (the lists are then meaningless).
     Every argument the entries would refuse is refused before the map is touched, and a failure between the first and
     the last entry (an allocation, a hop past 2^31 edges) resets the map before it propagates."""
+    padding = _check_block_fanouts(fanouts, padding)
+    _check(col, torch.int32, "col")
+    _check(w_csr, torch.float32, "w_csr")
+    return _block_sample(rowptr, _p(col), _p(w_csr), seeds, fanouts, keys, node_map, padding, rng_stream, False)
+
+
+def block_sample_mapped(rowptr, col_ptr, w_ptr, seeds, fanouts, keys, node_map, padding=False,
+                        rng_stream=RNG_STREAM_SAMPLER):
+    """block_sample over a CSR in host memory (tfgk_block_sample_fill_mapped): col_ptr and w_ptr are the device addresses
+    of its page-locked int32 columns and float32 weights (w_ptr None: every weight 1.0), at int64 positions; rowptr stays
+    on the device.  Same arguments otherwise, and the same outputs as block_sample over the same CSR."""
+    padding = _check_block_fanouts(fanouts, padding)
+    return _block_sample(rowptr, ctypes.c_void_p(col_ptr), None if w_ptr is None else ctypes.c_void_p(w_ptr), seeds,
+                         fanouts, keys, node_map, padding, rng_stream, True)
+
+
+def _check_block_fanouts(fanouts, padding):
     # the fan-out rules of check_sample_mode, here so that no entry refuses a hop once the map holds the seeds
     padding = _padding_code(padding)
     if any(k is not None and int(k) < 0 for k in fanouts):
         raise ValueError("block_sample: fan-outs must be >= 0 or None")
     if padding == SAMPLE_HEAD and any(k is None for k in fanouts):
         raise ValueError("block_sample: the head rule needs an integer fan-out for every hop")
+    return padding
+
+
+def _block_sample(rowptr, col, w_csr, seeds, fanouts, keys, node_map, padding, rng_stream, mapped):
+    """block_sample's hops; col and w_csr are the fill's pointer arguments, to host memory when `mapped`."""
     _check(rowptr, torch.int64, "rowptr")
-    _check(col, torch.int32, "col")
-    _check(w_csr, torch.float32, "w_csr")
     _check(seeds, torch.int32, "seeds")
     _check(node_map, torch.int32, "node_map")
     dev = rowptr.device
@@ -1065,13 +1133,16 @@ def block_sample(rowptr, col, w_csr, seeds, fanouts, keys, node_map, padding=Fal
             break
     nodes = torch.empty((max(cap_nodes, 1),), dtype=torch.int32, device=dev)
     state = torch.empty((4 + 2 * L,), dtype=torch.int32, device=dev)
+    # the device route passes no entry, so that a replacement of _block_workspace with the plain signature still fits
+    ws_entry = ("tfgk_block_sample_mapped_workspace_bytes",) if mapped else ()
+    fill = "tfgk_block_sample_fill_mapped" if mapped else "tfgk_block_sample_fill"
     st = _stream(rowptr)
     _ffi.call("tfgk_block_sample_begin", _p(seeds), seeds.numel(), N, _p(nodes), _p(node_map), _p(state), L, st)
     try:
         cap_list, hops = seeds.numel(), []
         for h, k in enumerate(ks):
             cap_edges, cap_next = block_capacities(cap_list, fanouts[h], limit)
-            ws, nbytes = _block_workspace(cap_list, 0 if cap_edges is None else cap_edges, dev)
+            ws, nbytes = _block_workspace(cap_list, 0 if cap_edges is None else cap_edges, dev, *ws_entry)
             out_rowptr = torch.empty((cap_list + 1,), dtype=torch.int64, device=dev)
             _ffi.call("tfgk_block_sample_count", _p(rowptr), n_rows, _p(nodes), _p(state), h, L, cap_list, k, padding,
                       _p(out_rowptr), _p(ws), nbytes, st)
@@ -1080,10 +1151,10 @@ def block_sample(rowptr, col, w_csr, seeds, fanouts, keys, node_map, padding=Fal
                 _ffi.call("tfgk_block_sample_read_total", _p(state), h, _p(out_rowptr), cap_list, ctypes.byref(n_list),
                           ctypes.byref(total), st)
                 cap_edges, cap_next = total.value, min(limit, n_list.value + total.value)
-                ws, nbytes = _block_workspace(cap_list, cap_edges, dev)
+                ws, nbytes = _block_workspace(cap_list, cap_edges, dev, *ws_entry)
             out = [torch.empty((max(cap_edges, 1),), dtype=torch.int32, device=dev) for _ in range(3)]
             out_w = torch.empty((max(cap_edges, 1),), dtype=torch.float32, device=dev)
-            _ffi.call("tfgk_block_sample_fill", _p(rowptr), n_rows, _p(col), _p(w_csr), N, _p(nodes), _p(node_map),
+            _ffi.call(fill, _p(rowptr), n_rows, col, w_csr, N, _p(nodes), _p(node_map),
                       _p(state), h, L, cap_list, cap_edges, k, padding, int(keys[h]), int(rng_stream), _p(out_rowptr),
                       _p(out[0]), _p(out[1]), _p(out[2]), _p(out_w), _p(ws), nbytes, st)
             hops.append((out_rowptr, out[0], out[1], out[2], out_w))

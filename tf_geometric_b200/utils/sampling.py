@@ -17,6 +17,7 @@ synchronisation per batch.
 
 HostFeatureTable keeps an [N, F] float32 feature table in host memory (page-locked in place) and gathers the rows a batch
 reads over the host link (tfgk_gather_rows_mapped_f32), so the table need not fit on the device."""
+import mmap
 import threading
 
 import numpy as np
@@ -206,6 +207,40 @@ def _host_range(x, array):
     return lo, size
 
 
+def _host_acquire(x, array=None):
+    """Make the host buffer under the CPU tensor x readable by the device: (key, device address of x.data_ptr()).  The
+    whole buffer (see _host_range) is page-locked in place once however many users share it, and counted; key is the
+    registration to hand back to _host_release, or None when nothing was registered (pinned memory, which is mapped at its
+    host address under unified addressing, or an empty x)."""
+    base, nbytes = _host_range(x, array)
+    if not x.numel():
+        return None, x.data_ptr() - base
+    with _host_lock:
+        owner = next((b for b, (_, size, _) in _host_registered.items() if b <= base and base + nbytes <= b + size), None)
+        if owner is not None:           # inside a buffer an open user registered: count one more user
+            entry = _host_registered[owner]
+            entry[0] += 1
+            return owner, entry[2] + (base - owner) + (x.data_ptr() - base)
+        if x.is_pinned():
+            return None, x.data_ptr()
+        dev_base = ops.host_register(base, nbytes)
+        _host_registered[base] = [1, nbytes, dev_base]
+        return base, dev_base + (x.data_ptr() - base)
+
+
+def _host_release(key):
+    """Drop one user of the registration `key` (from _host_acquire; None does nothing); the last one unregisters it,
+    after the device's pending work."""
+    if key is None:
+        return
+    with _host_lock:
+        entry = _host_registered[key]
+        entry[0] -= 1
+        if entry[0] == 0:
+            del _host_registered[key]
+            ops.host_unregister(key)
+
+
 class HostFeatureTable(object):
     """A float32 feature table [N, F] kept in host memory, whose rows the device gathers over the host link.
 
@@ -242,23 +277,7 @@ class HostFeatureTable(object):
             raise ValueError("HostFeatureTable needs rows that do not overlap (got strides {})".format(tuple(x.stride())))
         self.x = x
         self._ld = max(F, x.stride(0))
-        base, nbytes = _host_range(x, array)
-        dev_base = 0
-        if x.numel():
-            with _host_lock:
-                owner = next((b for b, (_, size, _) in _host_registered.items()
-                              if b <= base and base + nbytes <= b + size), None)
-                if owner is not None:       # inside a buffer an open table registered: count one more user
-                    entry = _host_registered[owner]
-                    entry[0] += 1
-                    self._key, dev_base = owner, entry[2] + (base - owner)
-                elif x.is_pinned():         # pinned memory is mapped at its host address under unified addressing
-                    dev_base = base
-                else:
-                    dev_base = ops.host_register(base, nbytes)
-                    _host_registered[base] = [1, nbytes, dev_base]
-                    self._key = base
-        self._ptr = dev_base + (x.data_ptr() - base)
+        self._key, self._ptr = _host_acquire(x, array)
         self._closed = False
 
     @property
@@ -300,14 +319,7 @@ class HostFeatureTable(object):
             return
         self._closed = True
         key, self._key = self._key, None
-        if key is None:
-            return
-        with _host_lock:
-            entry = _host_registered[key]
-            entry[0] -= 1
-            if entry[0] == 0:
-                del _host_registered[key]
-                ops.host_unregister(key)
+        _host_release(key)
 
     def __enter__(self):
         return self
@@ -427,28 +439,35 @@ class RandomNeighborSampler(_SamplerBase):
         host once per batch; a fan-out of None (every neighbour) adds one read-back for its hop.
 
         :return: SampledBlocks, on the device"""
-        from .graph_utils import _batch_seed         # graph_utils imports this module
-        seed = _rng.resolve_host(seed)
         csr, w_csr, rowptr, node_map = self._neighborhood_structure()
-        dev = rowptr.device
-        nodes = ops.as_device(seed_node_index, torch.int32, device=dev).reshape(-1).contiguous()
-        hop_fanouts = [None if k is None else int(k) for k in reversed(list(fanouts))]
-        keys = [_batch_seed(seed, h) for h in range(len(hop_fanouts))]
-        node_index, sizes, hops, n_bad, n_dup = ops.block_sample(rowptr, csr.col, w_csr, nodes, hop_fanouts, keys, node_map,
-                                                                 padding=padding)
-        if n_bad:
-            raise ValueError("seed_node_index holds node ids outside [0, {})".format(node_map.numel()))
-        if n_dup:
-            raise ValueError("seed_node_index holds {} duplicate node ids".format(n_dup))
-        blocks = []
-        for h, (k, (out_rowptr, row, local, gcol, w)) in enumerate(zip(hop_fanouts, hops)):
-            n_dst, n_src = sizes[h], sizes[h + 1]
-            S = row.numel()
-            block_csr = ops.CSR(out_rowptr[:n_dst + 1], local, torch.arange(S, dtype=torch.int32, device=dev), n_dst, n_src)
-            if k is None or k >= ops.DENSE_ROW_DEGREE:      # below it every row is short and build_plan returns None
-                block_csr.plan = ops.build_plan(block_csr)
-            blocks.append(Block(n_src, n_dst, torch.stack([row, local]), w, gcol, block_csr))
-        return SampledBlocks(node_index, sizes, blocks[::-1], num_nodes=node_map.numel())
+        return _sample_blocks(lambda nodes, hop_fanouts, keys: ops.block_sample(
+            rowptr, csr.col, w_csr, nodes, hop_fanouts, keys, node_map, padding=padding),
+            rowptr.device, node_map.numel(), seed_node_index, fanouts, seed)
+
+
+def _sample_blocks(block_sample, dev, num_nodes, seed_node_index, fanouts, seed):
+    """sample_blocks of both samplers around their block sampler: block_sample(seeds int32, per-hop fan-outs in hop order,
+    hop keys) returns ops.block_sample's (nodes, hop_sizes, hops, n_bad, n_dup); this refuses bad seeds and assembles
+    the SampledBlocks."""
+    from .graph_utils import _batch_seed         # graph_utils imports this module
+    seed = _rng.resolve_host(seed)
+    nodes = ops.as_device(seed_node_index, torch.int32, device=dev).reshape(-1).contiguous()
+    hop_fanouts = [None if k is None else int(k) for k in reversed(list(fanouts))]
+    keys = [_batch_seed(seed, h) for h in range(len(hop_fanouts))]
+    node_index, sizes, hops, n_bad, n_dup = block_sample(nodes, hop_fanouts, keys)
+    if n_bad:
+        raise ValueError("seed_node_index holds node ids outside [0, {})".format(num_nodes))
+    if n_dup:
+        raise ValueError("seed_node_index holds {} duplicate node ids".format(n_dup))
+    blocks = []
+    for h, (k, (out_rowptr, row, local, gcol, w)) in enumerate(zip(hop_fanouts, hops)):
+        n_dst, n_src = sizes[h], sizes[h + 1]
+        S = row.numel()
+        block_csr = ops.CSR(out_rowptr[:n_dst + 1], local, torch.arange(S, dtype=torch.int32, device=dev), n_dst, n_src)
+        if k is None or k >= ops.DENSE_ROW_DEGREE:      # below it every row is short and build_plan returns None
+            block_csr.plan = ops.build_plan(block_csr)
+        blocks.append(Block(n_src, n_dst, torch.stack([row, local]), w, gcol, block_csr))
+    return SampledBlocks(node_index, sizes, blocks[::-1], num_nodes=num_nodes)
 
 
 class UniformNeighborSampler(_SamplerBase):
@@ -465,3 +484,236 @@ class UniformNeighborSampler(_SamplerBase):
         v_row, v_col, w, _, _ = self._virtual_edges(sampled_node_index, bernoulli=ops.BERNOULLI_KEEP, prob=float(prob),
                                                     seed=seed)
         return torch.stack([v_row, v_col]), w
+
+
+# Device bytes the host CSR build holds per edge and per row of a range (ops.mapped_csr_range at its peak, in the radix
+# sort): the selected rows, columns and weights (12), csr_build's two key buffers, value buffer and histogram (12.25)
+# and its sorted columns and permutation (8), without the 4 bytes of selected weights for an unweighted graph; per row,
+# the range's counts and rowptr (12).  Besides the ranges the build holds the graph's rowptr and the selection's tile
+# offsets (HOST_CSR_FIXED_BYTES plus 8 bytes per row of the graph and per 1024 edges).
+HOST_CSR_EDGE_BYTES = 33
+HOST_CSR_EDGE_BYTES_UNWEIGHTED = 29
+HOST_CSR_ROW_BYTES = 12
+HOST_CSR_FIXED_BYTES = 1 << 20
+
+
+def _row_ranges(rowptr, budget, edge_bytes, row_bytes=HOST_CSR_ROW_BYTES):
+    """Cut the rows of rowptr (int64 numpy [n + 1]) into consecutive ranges [r0, r1) of fewer than 2^31 edges whose
+    working set edge_bytes * edges + row_bytes * (rows + 1) fits `budget` bytes, each as long as it can be.  Raises
+    ValueError naming the row when one row alone does not fit, or holds 2^31 edges or more (the draws use a 32-bit
+    degree)."""
+    rowptr = np.asarray(rowptr, np.int64)
+    n = rowptr.size - 1
+    deg = np.diff(rowptr)
+    if n and int(deg.max()) >= (1 << 31) - 1:
+        r = int(deg.argmax())
+        raise ValueError("row {} has {} edges; HostNeighborSampler takes rows of fewer than 2^31 - 1 edges".format(
+            r, int(deg[r])))
+    cost = edge_bytes * rowptr + row_bytes * np.arange(n + 1, dtype=np.int64)       # cost of [r0, r1) = cost[r1] - cost[r0] + row_bytes
+    ranges, r0 = [], 0
+    while r0 < n:
+        r1 = int(np.searchsorted(cost, cost[r0] + budget - row_bytes, side="right")) - 1
+        r1 = min(r1, int(np.searchsorted(rowptr, rowptr[r0] + (1 << 31) - 1, side="right")) - 1)
+        if r1 <= r0:
+            raise ValueError("row {} has {} edges, which need {} bytes of device memory to build; device_bytes leaves "
+                             "{} for a range of rows".format(r0, int(deg[r0]), edge_bytes * int(deg[r0]) + 2 * row_bytes,
+                                                             max(int(budget), 0)))
+        ranges.append((r0, r1))
+        r0 = r1
+    return ranges
+
+
+# cudaHostRegister page-locks whole pages, and a page can be in one registration only, so the sampler reads in place only
+# arrays of at least this size: smaller allocations may share a page with other data (malloc serves them from its heap;
+# glibc's threshold for giving an allocation pages of its own is at most 32 MiB).
+HOST_IN_PLACE_BYTES = 32 << 20
+
+
+def _page_array(n, dtype):
+    """An empty numpy vector of n `dtype` entries on pages of its own (page-aligned, nothing else on its last page)."""
+    page = mmap.PAGESIZE
+    pages = -(-max(n * np.dtype(dtype).itemsize, 1) // page)
+    raw = np.empty((pages + 1) * page, np.uint8)
+    off = -raw.ctypes.data % page
+    return raw[off:off + pages * page].view(dtype)[:n]
+
+
+def _host_array(a, what, dtype, ndim):
+    """`a` as a C-contiguous numpy array of `dtype` that can be page-locked on its own: `a` itself when it is one of at
+    least HOST_IN_PLACE_BYTES, else a copy on pages of its own."""
+    if torch.is_tensor(a):
+        if a.is_cuda:
+            raise TypeError("HostNeighborSampler takes {} in host memory; for a CUDA tensor use RandomNeighborSampler"
+                            .format(what))
+        if a.requires_grad:
+            raise ValueError("{} must not require grad: the sampler's graph is a constant".format(what))
+        a = a.detach().numpy()
+    elif not isinstance(a, np.ndarray):
+        raise TypeError("HostNeighborSampler takes {} as a CPU tensor or a numpy array (got {})".format(
+            what, type(a).__name__))
+    kind = np.dtype(dtype).kind
+    if (a.dtype.kind not in "iu" if kind == "i" else a.dtype.kind not in "iuf"):
+        raise TypeError("HostNeighborSampler takes {} of an {} dtype (got {})".format(
+            what, "integer" if kind == "i" else "integer or floating", a.dtype))
+    if a.ndim != ndim:
+        raise ValueError("{} must have {} dimension(s) (got shape {})".format(what, ndim, a.shape))
+    if a.dtype != dtype:
+        if kind == "i" and a.size:
+            lo, hi = int(a.min()), int(a.max())
+            if lo < 0:
+                raise ValueError("{} holds negative node ids".format(what))
+            if hi >= (1 << 31):
+                raise ValueError("{} holds node ids of 2^31 or more".format(what))
+    elif a.flags.c_contiguous and a.nbytes >= HOST_IN_PLACE_BYTES:
+        return a
+    out = _page_array(a.size, dtype).reshape(a.shape)
+    out[...] = a
+    return out
+
+
+class HostNeighborSampler(object):
+    """RandomNeighborSampler.sample_blocks over a graph whose CSR stays in host memory (an extension of the reference
+    API, for graphs whose edges do not fit on the device, such as ogbn-papers100M on one GPU).
+
+    edge_index: int [2, E] as a CPU tensor or a numpy array; E may be 2^31 or more.  A C-contiguous int32 array (of 32 MiB
+        or more) is read in place; any other integer array is converted once on the host, which makes an int32 copy of
+        it.  Ids must be >= 0.  edge_weight: optional float32 [E], read in place or converted the same way (a copy).
+    device_bytes: the most device memory the build may hold at once (default: half of the device's free memory when the
+        build starts).  A row whose edges do not fit in it is refused with ValueError, as is a row of 2^31 - 1 edges or
+        more.
+
+    The constructor builds the stable row-sorted CSR of RandomNeighborSampler, bit for bit: the edge list is page-locked
+    in place, its id range and row counts are found in streaming passes over the host link, and rows are processed in
+    ranges that fit device_bytes (each range's edges selected in edge order, sorted stably by row, permuted and copied
+    to host arrays, page-locked in place; an unweighted graph keeps no weights).  The edge list is released before the
+    constructor returns; the sampler keeps no reference to it.  The device holds the int64 rowptr (one row per node id)
+    and the [N] relabelling map; the int32 columns and float32 weights stay in host memory and each sampled edge reads
+    them over the host link.
+
+    Nodes: CSR rows = max(row) + 1, and the node count N (seeds, relabelling, SampledBlocks.num_nodes) is
+    max(max row, max col) + 1, as RandomNeighborSampler.  sample_blocks has RandomNeighborSampler.sample_blocks'
+    contract and returns the same batch for the same key, on the device.  sample, sample_neighborhood and the ratio rule
+    are not offered: they take every sampled edge into one index space, which does not scale to such graphs.
+
+    close() (or leaving a `with` block, or collection) releases the host CSR after the device's pending work; batches
+    already returned stay valid (they hold device tensors only), and sampling after close() raises RuntimeError."""
+
+    def __init__(self, edge_index, edge_weight=None, device_bytes=None):
+        self._closed = True                 # until the build succeeds: nothing for close() / __del__ to release
+        self._keys = []
+        ei = _host_array(edge_index, "edge_index", np.int32, 2)
+        if ei.shape[0] != 2:
+            raise ValueError("edge_index must have shape [2, E] (got {})".format(ei.shape))
+        E = ei.shape[1]
+        w = None
+        if edge_weight is not None:
+            w = _host_array(edge_weight.reshape(-1) if hasattr(edge_weight, "reshape") else edge_weight, "edge_weight",
+                            np.float32, 1)
+            if w.shape[0] != E:
+                raise ValueError("edge_weight has {} entries for {} edges".format(w.shape[0], E))
+        dev = ops.default_device()
+        if device_bytes is None:
+            device_bytes = torch.cuda.mem_get_info(dev)[0] // 2
+        self.num_edges = E
+        self._device = dev
+        if E == 0:
+            self.num_nodes, self.num_row_nodes = 0, 0
+            self.rowptr = torch.zeros((1,), dtype=torch.int64, device=dev)
+            self._col_ptr, self._w_ptr, self._ranges = 0, None, []
+            self._col = self._w = None
+        else:
+            self._build(ei, w, int(device_bytes))
+        self._node_map = torch.full((self.num_nodes,), -1, dtype=torch.int32, device=dev)
+        self._closed = False
+
+    def _build(self, ei, w, device_bytes):
+        E, dev = ei.shape[1], self._device
+        edge_keys = []
+        try:
+            key, ei_ptr = _host_acquire(torch.from_numpy(ei))
+            edge_keys.append(key)
+            row_ptr, col_ptr = ei_ptr, ei_ptr + 4 * E
+            w_ptr = None
+            if w is not None:
+                key, w_ptr = _host_acquire(torch.from_numpy(w))
+                edge_keys.append(key)
+            lo_r, hi_r, lo_c, hi_c = ops.mapped_id_range(row_ptr, col_ptr, E, dev)
+            if min(lo_r, lo_c) < 0:
+                raise ValueError("edge_index holds negative node ids")
+            self.num_row_nodes = hi_r + 1
+            self.num_nodes = N = max(hi_r, hi_c) + 1
+            edge_bytes = HOST_CSR_EDGE_BYTES if w is not None else HOST_CSR_EDGE_BYTES_UNWEIGHTED
+            budget = device_bytes - 8 * (N + 1) - 8 * (E // 1024 + 1) - HOST_CSR_FIXED_BYTES
+            rowptr = ops.mapped_rowptr(row_ptr, E, N, dev)
+            rp = rowptr.cpu().numpy()
+            ranges = _row_ranges(rp, budget, edge_bytes)
+            # ordinary host memory, page-locked in place (torch's pinned allocator would round each array up to a power
+            # of two bytes); the CSR's registrations are the sampler's from here on
+            col = _page_array(E, np.int32)
+            key, col_dev = _host_acquire(torch.from_numpy(col))
+            self._keys.append(key)
+            cw, w_dev = None, None
+            if w is not None:
+                cw = _page_array(E, np.float32)
+                key, w_dev = _host_acquire(torch.from_numpy(cw))
+                self._keys.append(key)
+            col_t = torch.from_numpy(col)
+            w_t = None if cw is None else torch.from_numpy(cw)
+            for r0, r1 in ranges:
+                e0, e1 = int(rp[r0]), int(rp[r1])
+                if e1 == e0:
+                    continue
+                c, cwr = ops.mapped_csr_range(row_ptr, col_ptr, w_ptr, E, r0, r1, e1 - e0, N, dev)
+                col_t[e0:e1].copy_(c)
+                if w_t is not None:
+                    w_t[e0:e1].copy_(cwr)
+                del c, cwr
+        except BaseException:
+            for key in self._keys:
+                _host_release(key)
+            self._keys = []
+            raise
+        finally:
+            for key in edge_keys:
+                _host_release(key)
+        self.rowptr = rowptr
+        self._ranges = ranges
+        self._col, self._w = col, cw
+        self._col_ptr, self._w_ptr = col_dev, w_dev
+
+    def _check_open(self):
+        if self._closed:
+            raise RuntimeError("this HostNeighborSampler is closed")
+
+    def sample_blocks(self, seed_node_index, fanouts, padding=False, seed=None):
+        """RandomNeighborSampler.sample_blocks over the host CSR: same arguments, same batch for the same key (rows of
+        the CSR are sampled in place over the host link).  A batch synchronises with the host once (plus one read-back
+        per hop of fan-out None).  Calls on one sampler must be ordered on one CUDA stream.
+
+        :return: SampledBlocks, on the device"""
+        self._check_open()
+        return _sample_blocks(lambda nodes, hop_fanouts, keys: ops.block_sample_mapped(
+            self.rowptr, self._col_ptr, self._w_ptr, nodes, hop_fanouts, keys, self._node_map, padding=padding),
+            self._device, self.num_nodes, seed_node_index, fanouts, seed)
+
+    def close(self):
+        """Release the host CSR's registrations (after the device's pending work) and the arrays.  Idempotent."""
+        if self._closed:
+            return
+        self._closed = True
+        keys, self._keys = self._keys, []
+        for key in keys:
+            _host_release(key)
+        self._col = self._w = None
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
