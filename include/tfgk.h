@@ -634,6 +634,16 @@ int tfgk_block_sample_fill_mapped(const int64_t *rowptr, int32_t n_rows, const i
                                   int32_t *out_gcol, float *out_w, void *workspace, size_t workspace_bytes,
                                   void *stream);
 
+/* A block's self loops (GAT on a sampled block, utils.SelfLoopBlock): the block's CSR (rowptr int64 [n_dst + 1], and for
+ * each of its S edges in CSR order the row row[p] < n_dst and column col[p]) with the edge (r, r) appended after the
+ * sampled edges of every row r < n_dst, where a block's output row r is its input row r.
+ * out_rowptr [n_dst + 1]: out_rowptr[r] = rowptr[r] + r.  out_row / out_col [S + n_dst]: edge p of row r moves to p + r,
+ * and row r's self edge goes to rowptr[r + 1] + r.  row must agree with rowptr (rowptr[row[p]] <= p < rowptr[row[p] + 1]).
+ * One launch, grid-strided over S + n_dst + 1 items; no atomics, no host synchronisation.  S + n_dst >= 2^31 returns
+ * TFGK_ERR_UNSUPPORTED. */
+int tfgk_block_self_loops_i32(const int64_t *rowptr, const int32_t *row, const int32_t *col, int64_t S, int32_t n_dst,
+                              int64_t *out_rowptr, int32_t *out_row, int32_t *out_col, void *stream);
+
 /* ---- link prediction (SURVEY.md 8(f)5, demo/demo_gae.py) -------------------------------------------------------- */
 
 /* K6, predict_edge of demo/demo_gae.py:53-60: out[e] = sum_d h[row_e, d] * h[col_e, d] in fp32, COO order.

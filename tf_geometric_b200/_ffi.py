@@ -145,6 +145,7 @@ SIGNATURES = {
     "tfgk_block_sample_mapped_workspace_bytes": [_i32, _i64, ctypes.POINTER(_size)],
     "tfgk_block_sample_fill_mapped": [_ptr, _i32, _ptr, _ptr, _i32, _ptr, _ptr, _ptr, _i32, _i32, _i32, _i64, _i32, _int,
                                       _u64, _u32, _ptr, _ptr, _ptr, _ptr, _ptr, _ptr, _size, _ptr],
+    "tfgk_block_self_loops_i32": [_ptr, _ptr, _ptr, _i64, _i32, _ptr, _ptr, _ptr, _ptr],
     "tfgk_edge_dot_f32": [_ptr, _i64, _i32, _ptr, _ptr, _i64, _i32, _ptr, _ptr],
     "tfgk_neg_offsets_workspace_bytes": [_i32, ctypes.POINTER(_size)],
     "tfgk_neg_offsets": [_ptr, _i32, _int, _ptr, ctypes.POINTER(_i64), _ptr, _size, _ptr],

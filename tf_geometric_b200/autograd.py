@@ -256,7 +256,11 @@ class GcnNormValues(torch.autograd.Function):
 def _transposed_of_csr(csr, edge_index_used):
     """(csr_t, emap) for a forward CSR: csr_t has one row per SOURCE node, its columns are the destination rows, and
     emap[p] is the forward-CSR position of transposed slot p (per-edge tables such as the attention coefficients are
-    stored in forward-CSR order).  Built once per CSR object."""
+    stored in forward-CSR order).  Built once per CSR object; a SelfLoopBlock (edge_index_used) keeps its own, built
+    without re-checking its ids."""
+    if isinstance(edge_index_used, ops.SampledInput):
+        csr_t = edge_index_used.transposed()
+        return csr_t, csr_t.perm
     hit = _structure._lookup(csr.col, ("csr_t",))
     if hit is not None and hit[0]() is csr:
         return hit[1], hit[2]

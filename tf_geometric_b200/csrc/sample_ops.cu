@@ -390,6 +390,30 @@ __global__ void block_sizes_kernel(const int64_t *__restrict__ S, const int32_t 
     state[kStateSizes + n_hops + 1 + hop] = (int32_t)*S;
 }
 
+// items [0, S) move edge p of row r to p + r; items [S, S + n_dst] write out_rowptr[r] and, for r < n_dst, the self edge
+// (r, r) after the row's sampled edges.  Every output slot has exactly one writer.
+__global__ void block_self_loops_kernel(const int64_t *__restrict__ rowptr, const int32_t *__restrict__ row,
+                                        const int32_t *__restrict__ col, int64_t S, int32_t n_dst,
+                                        int64_t *__restrict__ out_rowptr, int32_t *__restrict__ out_row,
+                                        int32_t *__restrict__ out_col) {
+    const int64_t n = S + n_dst + 1;
+    for (int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; t < n; t += (int64_t)gridDim.x * blockDim.x) {
+        if (t < S) {
+            const int32_t r = row[t];
+            out_row[t + r] = r;
+            out_col[t + r] = col[t];
+        } else {
+            const int32_t r = (int32_t)(t - S);
+            out_rowptr[r] = rowptr[r] + r;
+            if (r < n_dst) {
+                const int64_t q = rowptr[r + 1] + r;
+                out_row[q] = r;
+                out_col[q] = r;
+            }
+        }
+    }
+}
+
 }  // namespace
 }  // namespace tfgk
 
@@ -842,6 +866,20 @@ int tfgk_block_sample_end(const int32_t *nodes, int32_t cap_nodes, int32_t N, in
     }
     TFGK_CUDA(cudaMemcpyAsync(state_host, state, (size_t)(4 + 2 * n_hops) * 4, cudaMemcpyDeviceToHost, st));
     TFGK_CUDA(cudaStreamSynchronize(st));
+    return TFGK_OK;
+}
+
+int tfgk_block_self_loops_i32(const int64_t *rowptr, const int32_t *row, const int32_t *col, int64_t S, int32_t n_dst,
+                              int64_t *out_rowptr, int32_t *out_row, int32_t *out_col, void *stream) {
+    TFGK_CHECK_ARG(S >= 0 && n_dst >= 0, "block_self_loops: bad size (S=%lld, n_dst=%d)", (long long)S, n_dst);
+    if (S + n_dst >= (1ll << 31))
+        return set_error(TFGK_ERR_UNSUPPORTED, "block_self_loops: %lld looped edges exceed int32 positions",
+                         (long long)(S + n_dst));
+    TFGK_CHECK_ARG(rowptr && out_rowptr && (S == 0 || (row && col)) && (S + n_dst == 0 || (out_row && out_col)),
+                   "block_self_loops: null pointer");
+    block_self_loops_kernel<<<grid_for(S + n_dst + 1), 256, 0, as_stream(stream)>>>(rowptr, row, col, S, n_dst, out_rowptr,
+                                                                                     out_row, out_col);
+    TFGK_LAUNCH_CHECK();
     return TFGK_OK;
 }
 

@@ -55,8 +55,9 @@ class GAT(Layer):
                  [(self.key_kernel, self.key_bias, k_act), (self.kernel, None, ops.ACT_NONE)])]
 
     def call(self, inputs, training=None, mask=None, cache=None):
-        """inputs = [x, edge_index] (a third entry, edge_weight, is accepted and ignored like in the reference); on
-        several GPUs [x_local, partitioned_graph] (tf_geometric_b200.dist.PartitionedGraph)."""
+        """inputs = [x, edge_index] (a third entry, edge_weight, is accepted and ignored like in the reference); on a
+        sampled block [x_src or batch.source_rows(x), block.with_self_loops()] (nn.gat); on several GPUs
+        [x_local, partitioned_graph] (tf_geometric_b200.dist.PartitionedGraph)."""
         if hasattr(inputs[1], "part") and hasattr(inputs[1], "project_all_rows"):
             from ... import dist as tdist
             if ops.conv_message_dtype(self.message_dtype) is not None:

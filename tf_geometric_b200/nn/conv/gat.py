@@ -11,6 +11,7 @@ import torch
 
 from ... import ops, _structure, _rng, autograd
 from ...sparse import as_sparse_features, project_features
+from ...utils.sampling import SelfLoopBlock, SourceRows
 
 
 def project(x, blocks):
@@ -22,6 +23,16 @@ def project(x, blocks):
             pieces.append((w[:, c0:c1], None if b is None else b[c0:c1], act, out[:, c0:c1]))
     for i in range(0, len(pieces), 4):
         ops.gemm_proj(x, pieces[i:i + 4])
+
+
+def _project_qkv(x, n_q, q_block, kv_blocks):
+    """Q from x[:n_q] and K | V from every row of x: one launch that reads x once when Q takes every row, else Q from the
+    view of the first n_q rows and K | V in a second launch."""
+    if n_q == x.shape[0]:
+        project(x, [q_block] + kv_blocks)
+    else:
+        project(x[:n_q], [q_block])
+        project(x, kv_blocks)
 
 
 def gat(x, edge_index,
@@ -47,7 +58,17 @@ def gat(x, edge_index,
         scale per row (include/tfgk.h), a quarter of fp32's bytes; heads concatenated, units == attention_units = H * dqk
         <= 128 with dqk / 4 a power of two.  An extension of the reference API
     :return: [num_nodes, units]
+
+    On a sampled block (an extension of the reference API): edge_index is the SelfLoopBlock of block.with_self_loops(),
+    whose own self loops are the only ones; x is the block's [num_src, F] input or a SourceRows (gathered: every source
+    row is read as a key and a value); the output has num_dst rows.  fp32 messages only.
     """
+    if isinstance(edge_index, SelfLoopBlock):
+        x = _block_input(x, edge_index, message_dtype, return_attention, training, edge_drop_rate,
+                         (query_kernel, query_bias, key_kernel, key_bias, kernel, bias))
+        return _gat_dense(x, edge_index.csr, edge_index, query_kernel, query_bias, query_activation, key_kernel,
+                          key_bias, key_activation, kernel, bias, activation, num_heads, split_value_heads,
+                          float(edge_drop_rate) if training else 0.0, False, return_attention, seed)
     mdt = ops.conv_message_dtype(message_dtype)
     if mdt is torch.float8_e4m3fn:
         return _gat_fp8(x, edge_index, query_kernel, query_bias, query_activation, key_kernel, key_bias, key_activation,
@@ -90,6 +111,17 @@ def gat(x, edge_index,
         h, att = res if return_attention else (res, None)
         h = leftover(h) if leftover is not None else h
         return (h, ops.permute(att, csr.perm, inverse=True)) if return_attention else h
+    return _gat_dense(x, csr, edge_index_used, query_kernel, query_bias, query_activation, key_kernel, key_bias,
+                      key_activation, kernel, bias, activation, num_heads, split_value_heads, drop_rate, bf16,
+                      return_attention, seed)
+
+
+def _gat_dense(x, csr, edge_index_used, query_kernel, query_bias, query_activation, key_kernel, key_bias, key_activation,
+               kernel, bias, activation, num_heads, split_value_heads, drop_rate, bf16, return_attention, seed):
+    """gat() over a dense x on the device: csr.n_rows output rows, whose queries come from x[:csr.n_rows], over keys and
+    values from all x.shape[0] rows (the same rows on a full graph; a SelfLoopBlock's num_dst and num_src)."""
+    dev = x.device
+    n_q, num_nodes = csr.n_rows, x.shape[0]
     if drop_rate > 0.0 or autograd.needs_grad(x, query_kernel, query_bias, key_kernel, key_bias, kernel, bias):
         if bf16:
             raise NotImplementedError("message_dtype=bfloat16 is for inference: no operand may require grad")
@@ -112,12 +144,12 @@ def gat(x, edge_index,
             os.environ.get("TFGK_GAT_KEYS", "packed") != "dense":
         # ReLU keys hold many exact zeros: K goes through a scratch buffer into a packed table whose slots hold V, a zero
         # mask and the non-zero keys, and the fused kernel gathers only those (same output bits as the dense route)
-        Q = torch.empty((num_nodes, a_units), dtype=torch.float32, device=dev)
+        Q = torch.empty((n_q, a_units), dtype=torch.float32, device=dev)
         K = torch.empty((num_nodes, a_units), dtype=torch.float32, device=dev)
         table, sizes = ops.packed_key_table(num_nodes, a_units, dev)
-        project(x, [(wq, ops.as_device(query_bias, torch.float32, device=dev), q_act, Q),
-                    (wk, ops.as_device(key_bias, torch.float32, device=dev), k_act, K),
-                    (wv, None, ops.ACT_NONE, table[:, :a_units])])
+        _project_qkv(x, n_q, (wq, ops.as_device(query_bias, torch.float32, device=dev), q_act, Q),
+                     [(wk, ops.as_device(key_bias, torch.float32, device=dev), k_act, K),
+                      (wv, None, ops.ACT_NONE, table[:, :a_units])])
         if q_left is not None:
             Q = q_left(Q)
         ops.gat_pack_keys(K, table, sizes)
@@ -127,15 +159,14 @@ def gat(x, edge_index,
 
     # Q, K and V come out of ONE launch that reads x once (tfgk_gemm_proj_f32).  K and V land in ONE [N, A + U]
     # buffer: the fused kernel then fetches a neighbour's key and value from the same DRAM burst
-    Q = torch.empty((num_nodes, wq.shape[1]), dtype=torch.float32, device=dev)
+    Q = torch.empty((n_q, wq.shape[1]), dtype=torch.float32, device=dev)
     # bf16 messages: the projection rounds K | V in its epilogue; Q stays fp32
     kv = torch.empty((num_nodes, a_units + wv.shape[1]), dtype=torch.bfloat16 if bf16 else torch.float32, device=dev)
     K, V = kv[:, :a_units], kv[:, a_units:]
     # a key activation the projection cannot fuse is applied in fp32 before the keys are rounded
     K_f32 = torch.empty((num_nodes, a_units), dtype=torch.float32, device=dev) if bf16 and k_left is not None else K
-    project(x, [(wq, ops.as_device(query_bias, torch.float32, device=dev), q_act, Q),
-                (wk, ops.as_device(key_bias, torch.float32, device=dev), k_act, K_f32),
-                (wv, None, ops.ACT_NONE, V)])
+    _project_qkv(x, n_q, (wq, ops.as_device(query_bias, torch.float32, device=dev), q_act, Q),
+                 [(wk, ops.as_device(key_bias, torch.float32, device=dev), k_act, K_f32), (wv, None, ops.ACT_NONE, V)])
     if q_left is not None:
         Q = q_left(Q)
     if k_left is not None:
@@ -152,6 +183,22 @@ def gat(x, edge_index,
     if return_attention:
         return h, ops.permute(att, csr.perm, inverse=True)     # [E', H] in edge_index-with-self-loops order
     return h
+
+
+def _block_input(x, block, message_dtype, return_attention, training, edge_drop_rate, weights):
+    """The [num_src, F] device input of GAT over the SelfLoopBlock `block`; refuses what blocks do not support before any
+    device work."""
+    if ops.conv_message_dtype(message_dtype) is not None:
+        raise NotImplementedError("GAT on a sampled block takes fp32 messages only (message_dtype=None)")
+    rows = tuple(x.shape)[:1] if hasattr(x, "shape") and len(x.shape) == 2 else None
+    if rows != (block.num_src,):
+        raise ValueError("x has {} rows, the block has {} input rows".format(rows, block.num_src))
+    if return_attention and ((training and edge_drop_rate > 0.0) or autograd.needs_grad(
+            x.x if isinstance(x, SourceRows) else x, *weights)):
+        raise NotImplementedError("return_attention is an inference-path extension")
+    if isinstance(x, SourceRows):
+        return x.gather()
+    return ops.as_device(x, torch.float32, device=block.edge_index.device)
 
 
 def _gat_fp8(x, edge_index, query_kernel, query_bias, query_activation, key_kernel, key_bias, key_activation, kernel, bias,
@@ -217,16 +264,18 @@ def _gat_training(x, csr, edge_index_used, query_kernel, query_bias, query_activ
     sparse_x = as_sparse_features(x)
     dev = csr.col.device
 
-    def dense(w, b, act):
+    def dense(x, w, b, act):
         code, left = ops.activation_code(act)
         w = ops.as_device(w, torch.float32, device=dev)
         b = None if b is None else ops.as_device(b, torch.float32, device=dev)
         y = autograd.Dense.apply(x, w, b, code) if sparse_x is None else autograd.SparseMatmul.apply(w, b, sparse_x, code)
         return left(y) if left is not None else y
 
-    Q = dense(query_kernel, query_bias, query_activation)
-    K = dense(key_kernel, key_bias, key_activation)
-    V = dense(kernel, None, None)
+    # a block's queries are its output rows, the first csr.n_rows input rows
+    x_q = x if sparse_x is not None or x.shape[0] == csr.n_rows else x[:csr.n_rows]
+    Q = dense(x_q, query_kernel, query_bias, query_activation)
+    K = dense(x, key_kernel, key_bias, key_activation)
+    V = dense(x, kernel, None, None)
     act_code, leftover = ops.activation_code(activation)
     bias = None if bias is None else ops.as_device(bias, torch.float32, device=dev)
     h = autograd.GatAttention.apply(Q, K, V, bias, csr, edge_index_used, int(num_heads), bool(split_value_heads),

@@ -218,6 +218,7 @@ def _pool_sage(reduce, x, edge_index, edge_weight, self_kernel, neighbor_mlp_ker
     if isinstance(edge_index, Block):
         return _block_pool_sage(reduce, x, edge_index, edge_weight, self_kernel, neighbor_mlp_kernel, neighbor_kernel,
                                 neighbor_mlp_bias, bias, activation, concat, normalize, message_dtype)
+    ops.refuse_sampled(edge_index)           # a SelfLoopBlock: the sampled-input refusal, not the edge_weight one
     bf16 = _bf16.enabled(message_dtype)
     if bf16:
         _bf16.refuse_unsupported(x, (self_kernel, neighbor_mlp_kernel, neighbor_kernel, neighbor_mlp_bias, bias))

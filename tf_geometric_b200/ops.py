@@ -29,8 +29,9 @@ def default_device():
 
 
 class SampledInput(object):
-    """Base of the sampled-batch inputs (utils.sampling.Block, SourceRows) that only the block-aware GraphSAGE
-    aggregators take; as_device refuses them, so every other operator rejects them before any device work."""
+    """Base of the sampled-batch inputs (utils.sampling.Block, SelfLoopBlock, SourceRows) that only the block-aware
+    GraphSAGE aggregators and GAT take; as_device refuses them, so every other operator rejects them before any device
+    work."""
 
     __slots__ = ()
 
@@ -39,8 +40,9 @@ def refuse_sampled(x):
     """TypeError for a SampledInput (the check as_device applies to every non-tensor input)."""
     if isinstance(x, SampledInput):
         raise TypeError("a {} is taken only by mean_graph_sage, sum_graph_sage, mean_pool_graph_sage and "
-                        "max_pool_graph_sage (and their layers); other operators need a normalisation, self loops or "
-                        "padding that is not defined for a sampled block".format(type(x).__name__))
+                        "max_pool_graph_sage (and their layers) on a Block, and by gat (and GAT) on the SelfLoopBlock of "
+                        "block.with_self_loops(); other operators need a normalisation, self loops or padding that is not "
+                        "defined for a sampled block".format(type(x).__name__))
 
 
 def as_device(x, dtype=None, device=None):
@@ -1168,6 +1170,22 @@ def _block_sample(rowptr, col, w_csr, seeds, fanouts, keys, node_map, padding, r
     edges = [int(v) for v in host[4 + L:4 + 2 * L]]
     hops = [(rp, row[:S], local[:S], gcol[:S], w[:S]) for (rp, row, local, gcol, w), S in zip(hops, edges)]
     return nodes[:sizes[-1]], sizes, hops, int(host[0]), int(host[1])
+
+
+def block_self_loops(rowptr, edge_index, n_dst):
+    """A block's CSR with the self loop (r, r) appended to every row r < n_dst (tfgk_block_self_loops_i32): rowptr int64
+    [>= n_dst + 1] and edge_index int32 [2, S] in CSR order.  Returns (rowptr int64 [n_dst + 1], edge_index int32
+    [2, S + n_dst]), in CSR order; one launch, no synchronisation."""
+    _check(rowptr, torch.int64, "rowptr")
+    _check(edge_index, torch.int32, "edge_index")
+    S, n_dst = edge_index.shape[1], int(n_dst)
+    if rowptr.numel() < n_dst + 1:
+        raise ValueError("block_self_loops: rowptr has {} entries for {} rows".format(rowptr.numel(), n_dst))
+    out_rowptr = torch.empty((n_dst + 1,), dtype=torch.int64, device=rowptr.device)
+    out = torch.empty((2, S + n_dst), dtype=torch.int32, device=rowptr.device)
+    _ffi.call("tfgk_block_self_loops_i32", _p(rowptr), _p(edge_index[0]), _p(edge_index[1]), S, n_dst, _p(out_rowptr),
+              _p(out[0]), _p(out[1]), _stream(rowptr))
+    return out_rowptr, out
 
 
 # ---- link prediction: K6 edge scoring, negative sampling ----------------------------------------------------------

@@ -104,14 +104,24 @@ class Block(ops.SampledInput):
     edge_index: int32 [2, S] local (row < num_dst, col < num_src), rows ascending and in draw order within a row.
     edge_weight: float32 [S].  global_col: int32 [S], the node id of every edge's column.
     csr: ops.CSR with n_rows = num_dst, n_cols = num_src; its perm is the identity (the edges are already in CSR order).
+    fanout: the fan-out of the hop that drew the block (None: every neighbour, or a block built by hand).
     The transposed CSR that the backward needs is built on first use and kept on the block."""
 
-    __slots__ = ("num_src", "num_dst", "edge_index", "edge_weight", "global_col", "csr", "_csr_t", "_w_t")
+    __slots__ = ("num_src", "num_dst", "edge_index", "edge_weight", "global_col", "csr", "fanout", "_csr_t", "_w_t",
+                 "_looped")
 
-    def __init__(self, num_src, num_dst, edge_index, edge_weight, global_col, csr):
+    def __init__(self, num_src, num_dst, edge_index, edge_weight, global_col, csr, fanout=None):
         self.num_src, self.num_dst = int(num_src), int(num_dst)
         self.edge_index, self.edge_weight, self.global_col, self.csr = edge_index, edge_weight, global_col, csr
-        self._csr_t, self._w_t = None, {}
+        self.fanout = None if fanout is None else int(fanout)
+        self._csr_t, self._w_t, self._looped = None, {}, None
+
+    def with_self_loops(self):
+        """The SelfLoopBlock of this block (GAT's input on a sampled block), made on first use and kept: one launch, and
+        no synchronisation unless its rows are long enough for a work plan."""
+        if self._looped is None:
+            self._looped = SelfLoopBlock(self)
+        return self._looped
 
     def transposed(self, reduce=None, weighted=True):
         """(csr_t, w_t): the stable CSR of the edges keyed by local source (n_rows = num_src, n_cols = num_dst) and the
@@ -130,6 +140,43 @@ class Block(ops.SampledInput):
                 w = ops.scale_edges(self.edge_index[0], None, w, dl=torch.reciprocal(cnt))
             w_t = self._w_t[(reduce, weighted)] = ops.permute(w, self._csr_t.perm)
         return self._csr_t, w_t
+
+
+def _plan_for_fanout(k):
+    """Whether a block CSR whose rows hold at most k edges (None: unbounded) can need a work plan: below
+    DENSE_ROW_DEGREE every row is short and build_plan returns None."""
+    return k is None or k >= ops.DENSE_ROW_DEGREE
+
+
+class SelfLoopBlock(ops.SampledInput):
+    """A Block with GAT's self loops (Block.with_self_loops()): the self loop of output row r is the edge (r, r), since
+    output row r is input row r, appended after the row's sampled edges, where add_self_loop_edge puts self loops in the
+    stable CSR of a full graph.  tfg.nn.gat and tfg.layers.GAT take it in place of an edge_index and add no self loops of
+    their own; every other operator refuses it.
+
+    edge_index: int32 [2, S + num_dst] local, in CSR order.  csr: ops.CSR with n_rows = num_dst, n_cols = num_src and an
+    identity perm; it gets a work plan when its rows may be long (a fan-out of None or of DENSE_ROW_DEGREE - 1 or more).
+    The transposed CSR that the backward needs is built on first use and kept."""
+
+    __slots__ = ("num_src", "num_dst", "edge_index", "csr", "_csr_t")
+
+    def __init__(self, block):
+        self.num_src, self.num_dst = block.num_src, block.num_dst
+        rowptr, self.edge_index = ops.block_self_loops(block.csr.rowptr, block.edge_index, block.num_dst)
+        nnz = self.edge_index.shape[1]
+        self.csr = ops.CSR(rowptr, self.edge_index[1], torch.arange(nnz, dtype=torch.int32, device=rowptr.device),
+                           self.num_dst, self.num_src)
+        if _plan_for_fanout(None if block.fanout is None else block.fanout + 1):
+            self.csr.plan = ops.build_plan(self.csr)
+        self._csr_t = None
+
+    def transposed(self):
+        """The stable CSR of the looped edges keyed by local source (n_rows = num_src, n_cols = num_dst); its perm maps
+        each of its slots to the looped CSR's position."""
+        if self._csr_t is None:
+            self._csr_t = ops.csr_build(self.edge_index[1], self.edge_index[0], self.num_src, self.num_dst,
+                                        ids_in_range=True)
+        return self._csr_t
 
 
 class SourceRows(ops.SampledInput):
@@ -464,9 +511,9 @@ def _sample_blocks(block_sample, dev, num_nodes, seed_node_index, fanouts, seed)
         n_dst, n_src = sizes[h], sizes[h + 1]
         S = row.numel()
         block_csr = ops.CSR(out_rowptr[:n_dst + 1], local, torch.arange(S, dtype=torch.int32, device=dev), n_dst, n_src)
-        if k is None or k >= ops.DENSE_ROW_DEGREE:      # below it every row is short and build_plan returns None
+        if _plan_for_fanout(k):
             block_csr.plan = ops.build_plan(block_csr)
-        blocks.append(Block(n_src, n_dst, torch.stack([row, local]), w, gcol, block_csr))
+        blocks.append(Block(n_src, n_dst, torch.stack([row, local]), w, gcol, block_csr, fanout=k))
     return SampledBlocks(node_index, sizes, blocks[::-1], num_nodes=num_nodes)
 
 
