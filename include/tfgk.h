@@ -47,6 +47,8 @@ enum tfgk_heads_mode { TFGK_HEADS_SPLIT = 0, TFGK_HEADS_BROADCAST = 1, TFGK_HEAD
 enum tfgk_edge_flag { TFGK_FLAG_ALL = 0, TFGK_FLAG_UPPER = 1, TFGK_FLAG_MAPPED = 2 };
 enum tfgk_bernoulli { TFGK_BERNOULLI_NONE = 0, TFGK_BERNOULLI_DROPOUT = 1, TFGK_BERNOULLI_KEEP = 2 };
 enum tfgk_sample_padding { TFGK_SAMPLE_NO_PADDING = 0, TFGK_SAMPLE_PADDING = 1, TFGK_SAMPLE_HEAD = 2 };
+enum tfgk_gcn_norm { TFGK_GCN_NORM_BOTH = 0, TFGK_GCN_NORM_LEFT = 1, TFGK_GCN_NORM_RIGHT = 2 };
+enum tfgk_gcn_loop { TFGK_GCN_LOOP_NONE = 0, TFGK_GCN_LOOP_NORMED = 1, TFGK_GCN_LOOP_FILL = 2 };
 /* element type of a bf16-capable buffer; bf16 data is passed as its 16-bit patterns (uint16_t), fp8 data as bytes */
 enum tfgk_dtype { TFGK_DTYPE_F32 = 0, TFGK_DTYPE_BF16 = 1, TFGK_DTYPE_FP8_E4M3 = 2 };
 
@@ -643,6 +645,28 @@ int tfgk_block_sample_fill_mapped(const int64_t *rowptr, int32_t n_rows, const i
  * TFGK_ERR_UNSUPPORTED. */
 int tfgk_block_self_loops_i32(const int64_t *rowptr, const int32_t *row, const int32_t *col, int64_t S, int32_t n_dst,
                               int64_t *out_rowptr, int32_t *out_row, int32_t *out_col, void *stream);
+
+/* GCN's normalised values on a sampled block (utils.GcnBlock): every row normalised with its FULL-graph degree, and each
+ * output row's sampled edges rescaled so that their sum is an unbiased estimate of the full graph's row.
+ * The block: rowptr int64 [n_dst + 1] (rowptr[0] = 0, rowptr[n_dst] = S), gcol int32 [S] (the global id of every edge's
+ * column), w float32 [S] (NULL: all ones), dst int32 [n_dst] (the global id of every output row).  The full graph:
+ * g_rowptr int64 and g_rowsum float32, indexed by global id: the sampler's CSR rowptr and the sequential fp32 row sums of
+ * its weights (tfgk_csr_rowsum_f32).  For output row r with global id g, k_r = rowptr[r + 1] - rowptr[r] sampled edges
+ * and n_g = g_rowptr[g + 1] - g_rowptr[g] edges in the full graph:
+ *   f(v) = d^-1/2 (norm BOTH) or d^-1 (LEFT, RIGHT) of d = g_rowsum[v] + deg_fill, as tfgk_deg_inv_f32 (inf, nan -> 0)
+ *   edge p of row r:  s_r * (f(g) * w[p] * f(gcol[p]))  BOTH,  s_r * (f(g) * w[p])  LEFT,  s_r * (w[p] * f(gcol[p]))  RIGHT
+ *                     with s_r = (float)n_g / (float)k_r, each product rounded in that order (tfgk_scale_edges_f32's,
+ *                     then s_r; s_r = 1 changes no bit)
+ *   self loop of r:   fill scaled like an edge (g, g) without s_r (loop = TFGK_GCN_LOOP_NORMED), or fill as it is (_FILL)
+ * out: with a loop mode, [S + n_dst] in tfgk_block_self_loops_i32's layout (edge p of row r at p + r, row r's loop at
+ * rowptr[r + 1] + r); with TFGK_GCN_LOOP_NONE, [S] in the block's order.
+ * One launch, grid-strided over S (+ n_dst) items; no atomics, no host synchronisation.  An edge finds its row by binary
+ * search over rowptr.  Algorithmic bytes: 12 per edge (gcol, w, out) plus a 4-byte g_rowsum gather per edge for BOTH and
+ * RIGHT, and 40 per output row (rowptr, dst, g_rowptr, g_rowsum, the loop).  S + n_dst >= 2^31 returns
+ * TFGK_ERR_UNSUPPORTED. */
+int tfgk_block_gcn_values_f32(const int64_t *rowptr, const int32_t *gcol, const float *w, int64_t S, const int32_t *dst,
+                              int32_t n_dst, const int64_t *g_rowptr, const float *g_rowsum, int norm, int loop,
+                              float deg_fill, float fill, float *out, void *stream);
 
 /* ---- link prediction (SURVEY.md 8(f)5, demo/demo_gae.py) -------------------------------------------------------- */
 

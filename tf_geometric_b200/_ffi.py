@@ -23,6 +23,8 @@ HEADS_SPLIT, HEADS_BROADCAST, HEADS_REDUCE = 0, 1, 2
 FLAG_ALL, FLAG_UPPER, FLAG_MAPPED = 0, 1, 2
 BERNOULLI_NONE, BERNOULLI_DROPOUT, BERNOULLI_KEEP = 0, 1, 2
 SAMPLE_NO_PADDING, SAMPLE_PADDING, SAMPLE_HEAD = 0, 1, 2
+GCN_NORM_BOTH, GCN_NORM_LEFT, GCN_NORM_RIGHT = 0, 1, 2
+GCN_LOOP_NONE, GCN_LOOP_NORMED, GCN_LOOP_FILL = 0, 1, 2
 NEG_UPPER, NEG_START = 0, 1
 PAD_ROW_MAJOR, PAD_STEP_MAJOR = 0, 1
 SPGEMM_GRAD_LEFT, SPGEMM_GRAD_RIGHT = 0, 1
@@ -146,6 +148,7 @@ SIGNATURES = {
     "tfgk_block_sample_fill_mapped": [_ptr, _i32, _ptr, _ptr, _i32, _ptr, _ptr, _ptr, _i32, _i32, _i32, _i64, _i32, _int,
                                       _u64, _u32, _ptr, _ptr, _ptr, _ptr, _ptr, _ptr, _size, _ptr],
     "tfgk_block_self_loops_i32": [_ptr, _ptr, _ptr, _i64, _i32, _ptr, _ptr, _ptr, _ptr],
+    "tfgk_block_gcn_values_f32": [_ptr, _ptr, _ptr, _i64, _ptr, _i32, _ptr, _ptr, _int, _int, _f32, _f32, _ptr, _ptr],
     "tfgk_edge_dot_f32": [_ptr, _i64, _i32, _ptr, _ptr, _i64, _i32, _ptr, _ptr],
     "tfgk_neg_offsets_workspace_bytes": [_i32, ctypes.POINTER(_size)],
     "tfgk_neg_offsets": [_ptr, _i32, _int, _ptr, ctypes.POINTER(_i64), _ptr, _size, _ptr],

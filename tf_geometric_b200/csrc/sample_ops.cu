@@ -414,6 +414,55 @@ __global__ void block_self_loops_kernel(const int64_t *__restrict__ rowptr, cons
     }
 }
 
+// f(v) of tfgk_block_gcn_values_f32: deg_inv_kernel's arithmetic on the full graph's degree d = rowsum + deg_fill
+__device__ __forceinline__ float gcn_degree_factor(float rowsum, float deg_fill, int norm) {
+    const float d = __fadd_rn(rowsum, deg_fill);
+    float v = norm == TFGK_GCN_NORM_BOTH ? __frsqrt_rn(d) : __frcp_rn(d);
+    if (isinf(v) || isnan(v)) v = 0.0f;
+    return v;
+}
+
+// v times the factors of its row (fr) and column (fc) in scale_edges_kernel's order: dl on the left, dr on the right
+__device__ __forceinline__ float gcn_scale(float v, int norm, float fr, float fc) {
+    if (norm != TFGK_GCN_NORM_RIGHT) v = __fmul_rn(fr, v);
+    if (norm != TFGK_GCN_NORM_LEFT) v = __fmul_rn(v, fc);
+    return v;
+}
+
+// items [0, S): edge t, whose row is the last r with rowptr[r] <= t; items [S, S + n_dst) (loop modes only): the self
+// loop of row t - S.  Every output slot has exactly one writer.
+__global__ void block_gcn_values_kernel(const int64_t *__restrict__ rowptr, const int32_t *__restrict__ gcol,
+                                        const float *__restrict__ w, int64_t S, const int32_t *__restrict__ dst,
+                                        int32_t n_dst, const int64_t *__restrict__ g_rowptr,
+                                        const float *__restrict__ g_rowsum, int norm, int loop, float deg_fill, float fill,
+                                        float *__restrict__ out) {
+    const int64_t n = S + (loop != TFGK_GCN_LOOP_NONE ? n_dst : 0);
+    for (int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; t < n; t += (int64_t)gridDim.x * blockDim.x) {
+        if (t < S) {
+            int32_t lo = 0, hi = n_dst - 1;
+            while (lo < hi) {
+                const int32_t mid = lo + ((hi - lo + 1) >> 1);
+                if (rowptr[mid] <= t) lo = mid;
+                else hi = mid - 1;
+            }
+            const int32_t g = dst[lo];
+            const float fr = norm != TFGK_GCN_NORM_RIGHT ? gcn_degree_factor(g_rowsum[g], deg_fill, norm) : 0.0f;
+            const float fc = norm != TFGK_GCN_NORM_LEFT ? gcn_degree_factor(g_rowsum[gcol[t]], deg_fill, norm) : 0.0f;
+            const float v = gcn_scale(w ? w[t] : 1.0f, norm, fr, fc);
+            const float s = __fdiv_rn((float)(g_rowptr[g + 1] - g_rowptr[g]), (float)(rowptr[lo + 1] - rowptr[lo]));
+            out[loop != TFGK_GCN_LOOP_NONE ? t + lo : t] = __fmul_rn(s, v);
+        } else {
+            const int32_t r = (int32_t)(t - S);
+            float v = fill;
+            if (loop == TFGK_GCN_LOOP_NORMED) {
+                const float f = gcn_degree_factor(g_rowsum[dst[r]], deg_fill, norm);
+                v = gcn_scale(fill, norm, f, f);
+            }
+            out[rowptr[r + 1] + r] = v;
+        }
+    }
+}
+
 }  // namespace
 }  // namespace tfgk
 
@@ -879,6 +928,27 @@ int tfgk_block_self_loops_i32(const int64_t *rowptr, const int32_t *row, const i
                    "block_self_loops: null pointer");
     block_self_loops_kernel<<<grid_for(S + n_dst + 1), 256, 0, as_stream(stream)>>>(rowptr, row, col, S, n_dst, out_rowptr,
                                                                                      out_row, out_col);
+    TFGK_LAUNCH_CHECK();
+    return TFGK_OK;
+}
+
+int tfgk_block_gcn_values_f32(const int64_t *rowptr, const int32_t *gcol, const float *w, int64_t S, const int32_t *dst,
+                              int32_t n_dst, const int64_t *g_rowptr, const float *g_rowsum, int norm, int loop,
+                              float deg_fill, float fill, float *out, void *stream) {
+    TFGK_CHECK_ARG(S >= 0 && n_dst >= 0, "block_gcn_values: bad size (S=%lld, n_dst=%d)", (long long)S, n_dst);
+    TFGK_CHECK_ARG(norm == TFGK_GCN_NORM_BOTH || norm == TFGK_GCN_NORM_LEFT || norm == TFGK_GCN_NORM_RIGHT,
+                   "block_gcn_values: unknown norm %d", norm);
+    TFGK_CHECK_ARG(loop == TFGK_GCN_LOOP_NONE || loop == TFGK_GCN_LOOP_NORMED || loop == TFGK_GCN_LOOP_FILL,
+                   "block_gcn_values: unknown loop mode %d", loop);
+    TFGK_CHECK_ARG(S == 0 || n_dst > 0, "block_gcn_values: %lld edges and no output rows", (long long)S);
+    if (S + n_dst >= (1ll << 31))
+        return set_error(TFGK_ERR_UNSUPPORTED, "block_gcn_values: %lld looped edges exceed int32 positions",
+                         (long long)(S + n_dst));
+    const int64_t n = S + (loop != TFGK_GCN_LOOP_NONE ? n_dst : 0);
+    if (n == 0) return TFGK_OK;
+    TFGK_CHECK_ARG(rowptr && dst && g_rowptr && g_rowsum && out && (S == 0 || gcol), "block_gcn_values: null pointer");
+    block_gcn_values_kernel<<<grid_for(n), 256, 0, as_stream(stream)>>>(rowptr, gcol, w, S, dst, n_dst, g_rowptr, g_rowsum,
+                                                                         norm, loop, deg_fill, fill, out);
     TFGK_LAUNCH_CHECK();
     return TFGK_OK;
 }

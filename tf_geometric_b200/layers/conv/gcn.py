@@ -2,10 +2,13 @@
 """tfg.layers.GCN (reference layers/conv/gcn.py:12-156)."""
 import warnings
 
+import torch
+
 from ... import ops
 from ...sparse import SparseMatrix
 from ...nn.conv.gcn import gcn, gcn_build_cache_for_graph, gcn_build_cache_by_adj
 from ...utils.graph_utils import compute_num_or_size_splits
+from ...utils.sampling import GcnBlock
 from .._base import Layer
 
 
@@ -80,14 +83,21 @@ class GCN(Layer):
                                      improved=self.improved)
 
     def call(self, inputs, cache=None, split=True, training=None, mask=None):
-        """inputs: [x, sparse_adj], [x, edge_index] or [x, edge_index, edge_weight]; on several GPUs
-        [x_local, partitioned_graph] (tf_geometric_b200.dist.PartitionedGraph; x_local may be the result of its share())."""
+        """inputs: [x, sparse_adj], [x, edge_index] or [x, edge_index, edge_weight]; on a sampled block
+        [x_src or batch.source_rows(x), block.with_gcn_norm()] (nn.gcn); on several GPUs [x_local, partitioned_graph]
+        (tf_geometric_b200.dist.PartitionedGraph; x_local may be the result of its share())."""
         if hasattr(inputs[1], "part") and hasattr(inputs[1], "project_all_rows"):
             if ops.conv_message_dtype(self.message_dtype) is not None:
                 raise NotImplementedError("message_dtype={} is not implemented for partitioned graphs".format(
                     str(ops.conv_message_dtype(self.message_dtype)).replace("torch.", "")))
             return self._call_partitioned(inputs[0], inputs[1])
-        if isinstance(inputs[1], SparseMatrix):
+        if isinstance(inputs[1], GcnBlock):
+            if len(inputs) == 3:
+                if torch.is_tensor(inputs[2]) and inputs[2].requires_grad:
+                    raise NotImplementedError("GCN on a sampled block has no edge-weight gradient")
+                raise ValueError("a sampled block carries its edge weights: pass [x, block.with_gcn_norm()]")
+            x, sparse_adj = inputs
+        elif isinstance(inputs[1], SparseMatrix):
             x, sparse_adj = inputs
         elif len(inputs) == 3:
             x, edge_index, edge_weight = inputs

@@ -14,6 +14,7 @@ import torch
 
 from ... import ops, autograd
 from ...sparse import SparseMatrix, as_sparse_features, project_features
+from ...utils.sampling import GcnBlock, SourceRows, gcn_block_codes
 from ..kernel.map_reduce import gcn_mapper  # noqa: F401  (re-exported like the reference)
 
 CACHE_KEY_GCN_NORMED_ADJ_TEMPLATE = "gcn_normed_adj_{}_{}_{}_{}_{}"
@@ -137,7 +138,16 @@ def gcn(x, sparse_adj, kernel, bias=None, activation=None,
         torch.float8_e4m3fn: x W stored as e4m3 bytes with a power-of-two scale per row (include/tfgk.h), a quarter of
         the bytes, aggregated in fp32.  An extension of the reference API
     :return: [num_nodes, units]
+
+    On a sampled block (an extension of the reference API): sparse_adj is the GcnBlock of block.with_gcn_norm(), whose
+    values for this call's norm / add_self_loop / sym / renorm / improved are the full graph's normalisation with each
+    row's sampled edges rescaled by degree over fan-out (made on first use and kept on the GcnBlock; `cache` is not
+    consulted).  x is the block's dense [num_src, F] input or a SourceRows (gathered: every source row is projected); the
+    output has num_dst rows.  fp32 messages only, and not sym=False with norm="both".
     """
+    if isinstance(sparse_adj, GcnBlock):
+        return _gcn_block(x, sparse_adj, kernel, bias, activation, norm, add_self_loop, sym, renorm, improved,
+                          edge_drop_rate, num_or_size_splits, training, message_dtype)
     mdt = ops.conv_message_dtype(message_dtype)
     if mdt is torch.float8_e4m3fn:
         return _gcn_fp8(x, sparse_adj, kernel, bias, activation, norm, add_self_loop, sym, renorm, improved, edge_drop_rate,
@@ -147,6 +157,30 @@ def gcn(x, sparse_adj, kernel, bias=None, activation=None,
                          num_or_size_splits, training, cache)
     normed = gcn_norm_adj(sparse_adj, norm=norm, add_self_loop=add_self_loop, sym=sym, renorm=renorm,
                           improved=improved, cache=cache)
+    return _gcn_normed(x, normed, kernel, bias, activation, edge_drop_rate, num_or_size_splits, training)
+
+
+def _gcn_block(x, gcn_block, kernel, bias, activation, norm, add_self_loop, sym, renorm, improved, edge_drop_rate,
+               num_or_size_splits, training, message_dtype):
+    """gcn() over a GcnBlock: refuses what blocks do not support before any device work, then runs gcn()'s body over the
+    block's [num_dst, num_src] normalised matrix."""
+    if ops.conv_message_dtype(message_dtype) is not None:
+        raise NotImplementedError("GCN on a sampled block takes fp32 messages only (message_dtype=None)")
+    if not isinstance(x, SourceRows) and as_sparse_features(x) is not None:
+        raise NotImplementedError("GCN on a sampled block takes a dense x")
+    gcn_block_codes(norm, add_self_loop, sym, renorm, improved)
+    rows = tuple(x.shape)[:1] if hasattr(x, "shape") and len(x.shape) == 2 else None
+    if rows != (gcn_block.num_src,):
+        raise ValueError("x has {} rows, the block has {} input rows".format(rows, gcn_block.num_src))
+    if isinstance(x, SourceRows):
+        x = x.gather()
+    normed = gcn_block.normalized(norm, add_self_loop, sym, renorm, improved)
+    return _gcn_normed(x, normed, kernel, bias, activation, edge_drop_rate, num_or_size_splits, training)
+
+
+def _gcn_normed(x, normed, kernel, bias, activation, edge_drop_rate, num_or_size_splits, training):
+    """gcn() after the normalisation: act(normed @ (x W) + b) over the normalised SparseMatrix `normed` (the full graph's
+    square matrix, or a GcnBlock's [num_dst, num_src] one), with edge dropout on its values."""
     normed = normed.dropout(edge_drop_rate, training=training)
     dev = normed.index.device
     act_code, leftover = ops.activation_code(activation)

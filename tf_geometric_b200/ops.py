@@ -13,6 +13,7 @@ from . import _ffi, _rng
 from ._ffi import (REDUCE_SUM, REDUCE_MEAN, REDUCE_MAX, ACT_NONE, ACT_RELU, POW_INV_SQRT, POW_INV,  # noqa: F401
                    HEADS_SPLIT, HEADS_BROADCAST, HEADS_REDUCE, FLAG_ALL, FLAG_UPPER, FLAG_MAPPED,
                    BERNOULLI_NONE, BERNOULLI_DROPOUT, BERNOULLI_KEEP, SAMPLE_NO_PADDING, SAMPLE_PADDING, SAMPLE_HEAD,
+                   GCN_NORM_BOTH, GCN_NORM_LEFT, GCN_NORM_RIGHT, GCN_LOOP_NONE, GCN_LOOP_NORMED, GCN_LOOP_FILL,
                    NEG_UPPER, NEG_START, PAD_ROW_MAJOR, PAD_STEP_MAJOR, SPGEMM_GRAD_LEFT, SPGEMM_GRAD_RIGHT)
 
 _REDUCE_CODES = {"sum": REDUCE_SUM, "mean": REDUCE_MEAN, "max": REDUCE_MAX}
@@ -29,9 +30,9 @@ def default_device():
 
 
 class SampledInput(object):
-    """Base of the sampled-batch inputs (utils.sampling.Block, SelfLoopBlock, SourceRows) that only the block-aware
-    GraphSAGE aggregators and GAT take; as_device refuses them, so every other operator rejects them before any device
-    work."""
+    """Base of the sampled-batch inputs (utils.sampling.Block, SelfLoopBlock, GcnBlock, SourceRows) that only the
+    block-aware GraphSAGE aggregators, GAT and GCN take; as_device refuses them, so every other operator rejects them
+    before any device work."""
 
     __slots__ = ()
 
@@ -40,9 +41,10 @@ def refuse_sampled(x):
     """TypeError for a SampledInput (the check as_device applies to every non-tensor input)."""
     if isinstance(x, SampledInput):
         raise TypeError("a {} is taken only by mean_graph_sage, sum_graph_sage, mean_pool_graph_sage and "
-                        "max_pool_graph_sage (and their layers) on a Block, and by gat (and GAT) on the SelfLoopBlock of "
-                        "block.with_self_loops(); other operators need a normalisation, self loops or padding that is not "
-                        "defined for a sampled block".format(type(x).__name__))
+                        "max_pool_graph_sage (and their layers) on a Block, by gat (and GAT) on the SelfLoopBlock of "
+                        "block.with_self_loops(), and by gcn (and GCN) on the GcnBlock of block.with_gcn_norm(); other "
+                        "operators need a normalisation, self loops or padding that is not defined for a sampled "
+                        "block".format(type(x).__name__))
 
 
 def as_device(x, dtype=None, device=None):
@@ -1186,6 +1188,30 @@ def block_self_loops(rowptr, edge_index, n_dst):
     _ffi.call("tfgk_block_self_loops_i32", _p(rowptr), _p(edge_index[0]), _p(edge_index[1]), S, n_dst, _p(out_rowptr),
               _p(out[0]), _p(out[1]), _stream(rowptr))
     return out_rowptr, out
+
+
+def block_gcn_values(rowptr, gcol, w, dst, g_rowptr, g_rowsum, norm, loop, deg_fill, fill):
+    """GCN's normalised values on a sampled block (tfgk_block_gcn_values_f32): the block's rowptr int64 [>= n_dst + 1],
+    global columns int32 [S] and weights float32 [S] (or None: ones), its output rows' global ids dst int32 [n_dst], and
+    the full graph's rowptr int64 and sequential row sums float32, indexed by global id.  norm: GCN_NORM_*; loop:
+    GCN_LOOP_*; deg_fill is added to every row sum, fill is the self loops' weight.  Returns float32 [S + n_dst] in
+    block_self_loops' layout with a loop mode, else [S] in the block's order; one launch, no synchronisation."""
+    _check(rowptr, torch.int64, "rowptr")
+    _check(gcol, torch.int32, "gcol")
+    _check(dst, torch.int32, "dst")
+    _check(g_rowptr, torch.int64, "g_rowptr")
+    _check(g_rowsum, torch.float32, "g_rowsum")
+    if w is not None:
+        _check(w, torch.float32, "w")
+        if w.numel() != gcol.numel():
+            raise ValueError("block_gcn_values: {} weights for {} edges".format(w.numel(), gcol.numel()))
+    S, n_dst = gcol.numel(), dst.numel()
+    if rowptr.numel() < n_dst + 1:
+        raise ValueError("block_gcn_values: rowptr has {} entries for {} rows".format(rowptr.numel(), n_dst))
+    out = torch.empty((S + (n_dst if loop != GCN_LOOP_NONE else 0),), dtype=torch.float32, device=rowptr.device)
+    _ffi.call("tfgk_block_gcn_values_f32", _p(rowptr), _p(gcol), _p(w), S, _p(dst), n_dst, _p(g_rowptr), _p(g_rowsum),
+              int(norm), int(loop), float(deg_fill), float(fill), _p(out), _stream(rowptr))
+    return out
 
 
 # ---- link prediction: K6 edge scoring, negative sampling ----------------------------------------------------------

@@ -24,6 +24,7 @@ import numpy as np
 import torch
 
 from .. import ops, _rng
+from ..sparse import SparseMatrix
 
 
 def _split_node_index(sampled_node_index):
@@ -105,16 +106,21 @@ class Block(ops.SampledInput):
     edge_weight: float32 [S].  global_col: int32 [S], the node id of every edge's column.
     csr: ops.CSR with n_rows = num_dst, n_cols = num_src; its perm is the identity (the edges are already in CSR order).
     fanout: the fan-out of the hop that drew the block (None: every neighbour, or a block built by hand).
+    dst_ids: int32 [num_dst], the node id of every output row (a view of the batch's node_index; None for a block built
+    by hand).  degrees: the sampler's full-graph degrees for with_gcn_norm(), a callable returning (rowptr int64, row
+    sums float32), both indexed by node id (None for a block built by hand).
     The transposed CSR that the backward needs is built on first use and kept on the block."""
 
-    __slots__ = ("num_src", "num_dst", "edge_index", "edge_weight", "global_col", "csr", "fanout", "_csr_t", "_w_t",
-                 "_looped")
+    __slots__ = ("num_src", "num_dst", "edge_index", "edge_weight", "global_col", "csr", "fanout", "dst_ids", "degrees",
+                 "_csr_t", "_w_t", "_looped", "_gcn")
 
-    def __init__(self, num_src, num_dst, edge_index, edge_weight, global_col, csr, fanout=None):
+    def __init__(self, num_src, num_dst, edge_index, edge_weight, global_col, csr, fanout=None, dst_ids=None,
+                 degrees=None):
         self.num_src, self.num_dst = int(num_src), int(num_dst)
         self.edge_index, self.edge_weight, self.global_col, self.csr = edge_index, edge_weight, global_col, csr
         self.fanout = None if fanout is None else int(fanout)
-        self._csr_t, self._w_t, self._looped = None, {}, None
+        self.dst_ids, self.degrees = dst_ids, degrees
+        self._csr_t, self._w_t, self._looped, self._gcn = None, {}, None, None
 
     def with_self_loops(self):
         """The SelfLoopBlock of this block (GAT's input on a sampled block), made on first use and kept: one launch, and
@@ -122,6 +128,16 @@ class Block(ops.SampledInput):
         if self._looped is None:
             self._looped = SelfLoopBlock(self)
         return self._looped
+
+    def with_gcn_norm(self):
+        """The GcnBlock of this block (GCN's input on a sampled block), made on first use and kept; no device work until
+        a configuration's values are first used.  A block built by hand carries no full-graph degrees: ValueError."""
+        if self._gcn is None:
+            if self.degrees is None or self.dst_ids is None:
+                raise ValueError("with_gcn_norm() needs the full graph's degrees, which only a block from a sampler's "
+                                 "sample_blocks carries")
+            self._gcn = GcnBlock(self)
+        return self._gcn
 
     def transposed(self, reduce=None, weighted=True):
         """(csr_t, w_t): the stable CSR of the edges keyed by local source (n_rows = num_src, n_cols = num_dst) and the
@@ -177,6 +193,80 @@ class SelfLoopBlock(ops.SampledInput):
             self._csr_t = ops.csr_build(self.edge_index[1], self.edge_index[0], self.num_src, self.num_dst,
                                         ids_in_range=True)
         return self._csr_t
+
+
+def gcn_block_codes(norm, add_self_loop, sym, renorm, improved):
+    """(norm code, loop code, deg_fill, fill) of tfgk_block_gcn_values_f32 for a gcn_norm_adj configuration; refuses the
+    ones blocks do not support.  The degree takes the loops' fill when they are added before normalising (renorm, and
+    always for left and right); with norm="both" and renorm=False the loops keep their fill unnormalised."""
+    fill = 2.0 if improved else 1.0
+    codes = {"both": ops.GCN_NORM_BOTH, "left": ops.GCN_NORM_LEFT, "right": ops.GCN_NORM_RIGHT}
+    if norm not in codes:
+        raise Exception("wrong GCN norm type: {}".format(norm))
+    if norm == "both" and not sym:
+        raise NotImplementedError("GCN on a sampled block needs sym=True with norm='both': column sums of the full graph "
+                                  "are not kept by the sampler")
+    if not add_self_loop:
+        return codes[norm], ops.GCN_LOOP_NONE, 0.0, fill
+    if norm == "both" and not renorm:
+        return codes[norm], ops.GCN_LOOP_FILL, 0.0, fill
+    return codes[norm], ops.GCN_LOOP_NORMED, fill, fill
+
+
+class _BlockAdjacency(SparseMatrix):
+    """A GcnBlock's normalised [num_dst, num_src] matrix: index, CSR and values in the block's CSR order (identity perm),
+    and a transposed CSR that is the block's own, built on first use without an id check.  Matrices derived by dropout
+    share it (SparseMatrix._pattern_of)."""
+
+    def __init__(self, index, value, shape, csr, transposed):
+        super().__init__(index, value, shape, _csr=csr, _value_csr=value)
+        self._block_transposed = transposed
+
+    def _transposed_csr(self):
+        if self._csc is None:
+            self._csc = self._block_transposed()
+        return self._csc
+
+
+class GcnBlock(ops.SampledInput):
+    """A Block with GCN's normalisation (Block.with_gcn_norm()): every row, source-only rows included, is normalised with
+    its degree in the sampler's full graph, and the sampled edges of output row r (global id g, k_r sampled of n_g) are
+    scaled by s_r = n_g / k_r, so that each aggregate is an unbiased estimate of the full graph's row.  With every
+    neighbour (fan-out None) s_r = 1 and the values are the full graph's gcn_norm_adj values for the same rows, bit for
+    bit.  tfg.nn.gcn and tfg.layers.GCN take it in place of the adjacency; every other operator refuses it.
+
+    normalized(norm, add_self_loop, sym, renorm, improved) gives the rectangular [num_dst, num_src] SparseMatrix of one
+    configuration, made on first use (one launch of tfgk_block_gcn_values_f32) and kept.  With self loops its structure is
+    block.with_self_loops()'s (CSR, plan and transposed CSR shared with GAT's view of the block), else the block's own."""
+
+    __slots__ = ("num_src", "num_dst", "block", "_normed")
+
+    def __init__(self, block):
+        self.num_src, self.num_dst, self.block = block.num_src, block.num_dst, block
+        self._normed = {}
+
+    def normalized(self, norm="both", add_self_loop=True, sym=True, renorm=True, improved=False):
+        from ..nn.conv.gcn import compute_cache_key         # nn imports this module
+        key = compute_cache_key(norm, add_self_loop, sym, renorm, improved)
+        normed = self._normed.get(key)
+        if normed is None:
+            normed = self._normed[key] = self._make(*gcn_block_codes(norm, add_self_loop, sym, renorm, improved))
+        return normed
+
+    def _make(self, norm, loop, deg_fill, fill):
+        blk = self.block
+        g_rowptr, g_rowsum = blk.degrees()
+        if loop == ops.GCN_LOOP_NONE:
+            index, csr = blk.edge_index, blk.csr
+
+            def transposed():
+                return blk.transposed()[0]
+        else:
+            looped = blk.with_self_loops()
+            index, csr, transposed = looped.edge_index, looped.csr, looped.transposed
+        value = ops.block_gcn_values(blk.csr.rowptr, blk.global_col, blk.edge_weight, blk.dst_ids, g_rowptr, g_rowsum,
+                                     norm, loop, deg_fill, fill)
+        return _BlockAdjacency(index, value, [self.num_dst, self.num_src], csr, transposed)
 
 
 class SourceRows(ops.SampledInput):
@@ -390,6 +480,7 @@ class RandomNeighborSampler(_SamplerBase):
         self._w_csr = None
         self._rowptr_all = None
         self._node_map = None
+        self._rowsum = None
 
     def _structure(self):
         if self._csr is None:
@@ -434,6 +525,19 @@ class RandomNeighborSampler(_SamplerBase):
             self._rowptr_all = rowptr
             self._node_map = torch.full((n,), -1, dtype=torch.int32, device=rowptr.device)
         return csr, w_csr, self._rowptr_all, self._node_map
+
+    def _gcn_degrees(self):
+        """(rowptr int64 [N + 1], row sums float32 [N]) of the cached CSR, one row per node id: the sequential fp32 sums
+        of each row's weights (csr_rowsum, gcn_norm_adj's degrees before any self loop), made on first use and kept."""
+        csr, w_csr, rowptr, node_map = self._neighborhood_structure()
+        if self._rowsum is None:
+            n = node_map.numel()
+            rowsum = ops.csr_rowsum(csr, w_csr) if csr.n_rows else torch.zeros((0,), dtype=torch.float32,
+                                                                              device=rowptr.device)
+            if n > csr.n_rows:
+                rowsum = torch.cat([rowsum, rowsum.new_zeros(n - csr.n_rows)])
+            self._rowsum = rowsum
+        return rowptr, self._rowsum
 
     def sample_neighborhood(self, seed_node_index, fanouts, padding=False, seed=None):
         """Seed-node mini-batch sampling (an extension of the reference API).
@@ -489,13 +593,13 @@ class RandomNeighborSampler(_SamplerBase):
         csr, w_csr, rowptr, node_map = self._neighborhood_structure()
         return _sample_blocks(lambda nodes, hop_fanouts, keys: ops.block_sample(
             rowptr, csr.col, w_csr, nodes, hop_fanouts, keys, node_map, padding=padding),
-            rowptr.device, node_map.numel(), seed_node_index, fanouts, seed)
+            rowptr.device, node_map.numel(), seed_node_index, fanouts, seed, self._gcn_degrees)
 
 
-def _sample_blocks(block_sample, dev, num_nodes, seed_node_index, fanouts, seed):
+def _sample_blocks(block_sample, dev, num_nodes, seed_node_index, fanouts, seed, degrees):
     """sample_blocks of both samplers around their block sampler: block_sample(seeds int32, per-hop fan-outs in hop order,
     hop keys) returns ops.block_sample's (nodes, hop_sizes, hops, n_bad, n_dup); this refuses bad seeds and assembles
-    the SampledBlocks."""
+    the SampledBlocks.  degrees: the sampler's (rowptr, row sums) handle that every Block keeps for with_gcn_norm()."""
     from .graph_utils import _batch_seed         # graph_utils imports this module
     seed = _rng.resolve_host(seed)
     nodes = ops.as_device(seed_node_index, torch.int32, device=dev).reshape(-1).contiguous()
@@ -513,7 +617,8 @@ def _sample_blocks(block_sample, dev, num_nodes, seed_node_index, fanouts, seed)
         block_csr = ops.CSR(out_rowptr[:n_dst + 1], local, torch.arange(S, dtype=torch.int32, device=dev), n_dst, n_src)
         if _plan_for_fanout(k):
             block_csr.plan = ops.build_plan(block_csr)
-        blocks.append(Block(n_src, n_dst, torch.stack([row, local]), w, gcol, block_csr, fanout=k))
+        blocks.append(Block(n_src, n_dst, torch.stack([row, local]), w, gcol, block_csr, fanout=k,
+                            dst_ids=node_index[:n_dst], degrees=degrees))
     return SampledBlocks(node_index, sizes, blocks[::-1], num_nodes=num_nodes)
 
 
@@ -633,8 +738,9 @@ class HostNeighborSampler(object):
     in place, its id range and row counts are found in streaming passes over the host link, and rows are processed in
     ranges that fit device_bytes (each range's edges selected in edge order, sorted stably by row, permuted and copied
     to host arrays, page-locked in place; an unweighted graph keeps no weights).  The edge list is released before the
-    constructor returns; the sampler keeps no reference to it.  The device holds the int64 rowptr (one row per node id)
-    and the [N] relabelling map; the int32 columns and float32 weights stay in host memory and each sampled edge reads
+    constructor returns; the sampler keeps no reference to it.  The device holds the int64 rowptr (one row per node id),
+    the float32 row sums `rowsum` of the weights (GcnBlock's full-graph degrees, summed range by range during the build as
+    csr_rowsum sums RandomNeighborSampler's CSR) and the [N] relabelling map; the int32 columns and float32 weights stay in host memory and each sampled edge reads
     them over the host link.
 
     Nodes: CSR rows = max(row) + 1, and the node count N (seeds, relabelling, SampledBlocks.num_nodes) is
@@ -666,11 +772,14 @@ class HostNeighborSampler(object):
         if E == 0:
             self.num_nodes, self.num_row_nodes = 0, 0
             self.rowptr = torch.zeros((1,), dtype=torch.int64, device=dev)
+            self.rowsum = torch.zeros((0,), dtype=torch.float32, device=dev)
             self._col_ptr, self._w_ptr, self._ranges = 0, None, []
             self._col = self._w = None
         else:
             self._build(ei, w, int(device_bytes))
         self._node_map = torch.full((self.num_nodes,), -1, dtype=torch.int32, device=dev)
+        rowptr, rowsum = self.rowptr, self.rowsum
+        self._degrees = lambda: (rowptr, rowsum)      # the blocks' handle: device tensors only, not the sampler
         self._closed = False
 
     def _build(self, ei, w, device_bytes):
@@ -706,15 +815,20 @@ class HostNeighborSampler(object):
                 self._keys.append(key)
             col_t = torch.from_numpy(col)
             w_t = None if cw is None else torch.from_numpy(cw)
+            # the full graph's row sums (GcnBlock's degrees), from each range's weights while they are on the device
+            rowsum = torch.zeros((N,), dtype=torch.float32, device=dev)
             for r0, r1 in ranges:
                 e0, e1 = int(rp[r0]), int(rp[r1])
                 if e1 == e0:
                     continue
                 c, cwr = ops.mapped_csr_range(row_ptr, col_ptr, w_ptr, E, r0, r1, e1 - e0, N, dev)
+                range_csr = ops.CSR(rowptr[r0:r1 + 1] - e0, c, None, r1 - r0, N)
+                rowsum[r0:r1].copy_(ops.csr_rowsum(range_csr, torch.ones_like(c, dtype=torch.float32) if cwr is None
+                                                   else cwr))
                 col_t[e0:e1].copy_(c)
                 if w_t is not None:
                     w_t[e0:e1].copy_(cwr)
-                del c, cwr
+                del c, cwr, range_csr
         except BaseException:
             for key in self._keys:
                 _host_release(key)
@@ -723,7 +837,7 @@ class HostNeighborSampler(object):
         finally:
             for key in edge_keys:
                 _host_release(key)
-        self.rowptr = rowptr
+        self.rowptr, self.rowsum = rowptr, rowsum
         self._ranges = ranges
         self._col, self._w = col, cw
         self._col_ptr, self._w_ptr = col_dev, w_dev
@@ -741,7 +855,7 @@ class HostNeighborSampler(object):
         self._check_open()
         return _sample_blocks(lambda nodes, hop_fanouts, keys: ops.block_sample_mapped(
             self.rowptr, self._col_ptr, self._w_ptr, nodes, hop_fanouts, keys, self._node_map, padding=padding),
-            self._device, self.num_nodes, seed_node_index, fanouts, seed)
+            self._device, self.num_nodes, seed_node_index, fanouts, seed, self._degrees)
 
     def close(self):
         """Release the host CSR's registrations (after the device's pending work) and the arrays.  Idempotent."""
