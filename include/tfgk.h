@@ -157,6 +157,14 @@ int tfgk_host_unregister(void *ptr);
  * 4-byte accesses otherwise.  Asynchronous.  Bytes over the link: n * F * 4. */
 int tfgk_gather_rows_mapped_f32(const float *table, int64_t ld, int64_t n_rows, int32_t F, const int32_t *index,
                                 int64_t n, float *out, int64_t ldo, void *stream);
+/* The same gather with a device cache of some rows (HostFeatureTable(x, device_rows=...)): slot is an int32 [n_rows]
+ * device map, and slot[r] = s >= 0 means row r is cache[s*ldc + j] for j < F (device memory, ldc >= F), read instead of
+ * the host row; slot[r] = -1 reads the host table.  An id outside [0, n_rows) writes a row of NaN and reads neither the
+ * map nor either table.  One launch serves hits and misses; 16-byte accesses need ldc % 4 == 0 and a 16-byte-aligned
+ * cache as well.  Asynchronous.  Bytes: misses * F * 4 over the host link, hits * F * 4 from device memory. */
+int tfgk_gather_rows_cached_f32(const float *table, int64_t ld, int64_t n_rows, int32_t F, const float *cache,
+                                int64_t ldc, const int32_t *slot, const int32_t *index, int64_t n, float *out,
+                                int64_t ldo, void *stream);
 
 /* ---- a CSR built from an edge list in host memory (utils.HostNeighborSampler) -----------------------------------------
  * row, col [E] int32 (and w [E] float32) are device-readable pointers to page-locked host memory (tfgk_host_register);

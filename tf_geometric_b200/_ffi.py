@@ -57,6 +57,7 @@ SIGNATURES = {
     "tfgk_host_register": [_ptr, _size, ctypes.POINTER(_ptr)],
     "tfgk_host_unregister": [_ptr],
     "tfgk_gather_rows_mapped_f32": [_ptr, _i64, _i64, _i32, _ptr, _i64, _ptr, _i64, _ptr],
+    "tfgk_gather_rows_cached_f32": [_ptr, _i64, _i64, _i32, _ptr, _i64, _ptr, _ptr, _i64, _ptr, _i64, _ptr],
     "tfgk_mapped_id_range_i32": [_ptr, _ptr, _i64, _ptr, _ptr, _size, _ptr],
     "tfgk_mapped_rowptr_workspace_bytes": [_i32, ctypes.POINTER(_size)],
     "tfgk_mapped_rowptr_i32": [_ptr, _i64, _i32, _ptr, _ptr, _size, _ptr],

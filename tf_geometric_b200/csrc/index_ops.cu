@@ -93,10 +93,14 @@ template <> __device__ __forceinline__ float4 nan_vec<float4>() {
     return make_float4(q, q, q, q);
 }
 
-// V = float4: F, ld and ldo counted in floats are multiples of 4 and both bases are 16-byte aligned
-template <typename V>
+// V = float4: F, ld and ldo (and ldc when kCached) counted in floats are multiples of 4 and every base is 16-byte aligned.
+// kCached (tfgk_gather_rows_cached_f32): slot[r] >= 0 says row r is also cache[slot[r], :F] in device memory, which is
+// read instead of the host row; the map is read once per output row, by every lane of its warp from one address.
+template <typename V, bool kCached>
 __device__ __forceinline__ void gather_rows_mapped_body(const float *__restrict__ table, int64_t ld, int64_t n_rows,
-                                                        int32_t F, const int32_t *__restrict__ index, int64_t n,
+                                                        int32_t F, const float *__restrict__ cache, int64_t ldc,
+                                                        const int32_t *__restrict__ slot,
+                                                        const int32_t *__restrict__ index, int64_t n,
                                                         float *__restrict__ out, int64_t ldo) {
     constexpr int kW = sizeof(V) / sizeof(float);
     const int lane = threadIdx.x & 31;
@@ -110,6 +114,10 @@ __device__ __forceinline__ void gather_rows_mapped_body(const float *__restrict_
             continue;
         }
         const V *src = reinterpret_cast<const V *>(table + (int64_t)r * ld);
+        if constexpr (kCached) {
+            const int32_t s = __ldg(slot + r);
+            if (s >= 0) src = reinterpret_cast<const V *>(cache + (int64_t)s * ldc);
+        }
         for (int32_t c0 = lane; c0 < nv; c0 += 32 * kGatherUnroll) {
             V v[kGatherUnroll];
 #pragma unroll
@@ -125,13 +133,27 @@ __device__ __forceinline__ void gather_rows_mapped_body(const float *__restrict_
 __global__ void __launch_bounds__(kGatherThreads) gather_rows_mapped_vec4_kernel(
         const float *__restrict__ table, int64_t ld, int64_t n_rows, int32_t F, const int32_t *__restrict__ index,
         int64_t n, float *__restrict__ out, int64_t ldo) {
-    gather_rows_mapped_body<float4>(table, ld, n_rows, F, index, n, out, ldo);
+    gather_rows_mapped_body<float4, false>(table, ld, n_rows, F, nullptr, 0, nullptr, index, n, out, ldo);
 }
 
 __global__ void __launch_bounds__(kGatherThreads) gather_rows_mapped_f32_kernel(
         const float *__restrict__ table, int64_t ld, int64_t n_rows, int32_t F, const int32_t *__restrict__ index,
         int64_t n, float *__restrict__ out, int64_t ldo) {
-    gather_rows_mapped_body<float>(table, ld, n_rows, F, index, n, out, ldo);
+    gather_rows_mapped_body<float, false>(table, ld, n_rows, F, nullptr, 0, nullptr, index, n, out, ldo);
+}
+
+__global__ void __launch_bounds__(kGatherThreads) gather_rows_cached_vec4_kernel(
+        const float *__restrict__ table, int64_t ld, int64_t n_rows, int32_t F, const float *__restrict__ cache,
+        int64_t ldc, const int32_t *__restrict__ slot, const int32_t *__restrict__ index, int64_t n,
+        float *__restrict__ out, int64_t ldo) {
+    gather_rows_mapped_body<float4, true>(table, ld, n_rows, F, cache, ldc, slot, index, n, out, ldo);
+}
+
+__global__ void __launch_bounds__(kGatherThreads) gather_rows_cached_f32_kernel(
+        const float *__restrict__ table, int64_t ld, int64_t n_rows, int32_t F, const float *__restrict__ cache,
+        int64_t ldc, const int32_t *__restrict__ slot, const int32_t *__restrict__ index, int64_t n,
+        float *__restrict__ out, int64_t ldo) {
+    gather_rows_mapped_body<float, true>(table, ld, n_rows, F, cache, ldc, slot, index, n, out, ldo);
 }
 
 __global__ void csr_rowsum_kernel(const int64_t *__restrict__ rowptr, const float *__restrict__ w, int32_t N,
@@ -951,6 +973,31 @@ int tfgk_gather_rows_mapped_f32(const float *table, int64_t ld, int64_t n_rows, 
     else
         gather_rows_mapped_f32_kernel<<<blocks, kGatherThreads, 0, as_stream(stream)>>>(table, ld, n_rows, F, index, n,
                                                                                        out, ldo);
+    TFGK_LAUNCH_CHECK();
+    return TFGK_OK;
+}
+
+int tfgk_gather_rows_cached_f32(const float *table, int64_t ld, int64_t n_rows, int32_t F, const float *cache,
+                                int64_t ldc, const int32_t *slot, const int32_t *index, int64_t n, float *out,
+                                int64_t ldo, void *stream) {
+    TFGK_CHECK_ARG(n >= 0 && n_rows >= 0 && F >= 1, "gather_rows_cached: bad size (n=%lld, n_rows=%lld, F=%d)",
+                   (long long)n, (long long)n_rows, F);
+    TFGK_CHECK_ARG(ld >= F && ldc >= F && ldo >= F,
+                   "gather_rows_cached: need ld, ldc and ldo >= F (ld=%lld, ldc=%lld, ldo=%lld, F=%d)", (long long)ld,
+                   (long long)ldc, (long long)ldo, F);
+    if (n == 0) return TFGK_OK;
+    TFGK_CHECK_ARG(index && out && cache && slot && (table || n_rows == 0), "gather_rows_cached: null pointer");
+    const int64_t warps_per_block = kGatherThreads / 32;
+    const unsigned blocks = (unsigned)std::min<int64_t>(ceil_div64(n, warps_per_block),
+                                                        (int64_t)sm_count() * kGatherBlocksPerSm);
+    const bool vec = F % 4 == 0 && ld % 4 == 0 && ldc % 4 == 0 && ldo % 4 == 0 && aligned16(table) &&
+                     aligned16(cache) && aligned16(out);
+    if (vec)
+        gather_rows_cached_vec4_kernel<<<blocks, kGatherThreads, 0, as_stream(stream)>>>(table, ld, n_rows, F, cache,
+                                                                                        ldc, slot, index, n, out, ldo);
+    else
+        gather_rows_cached_f32_kernel<<<blocks, kGatherThreads, 0, as_stream(stream)>>>(table, ld, n_rows, F, cache,
+                                                                                       ldc, slot, index, n, out, ldo);
     TFGK_LAUNCH_CHECK();
     return TFGK_OK;
 }

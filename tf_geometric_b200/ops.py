@@ -300,6 +300,37 @@ def gather_rows_mapped(table_ptr, ld, n_rows, num_features, index, out=None):
     return out
 
 
+def gather_rows_cached(table_ptr, ld, n_rows, num_features, cache, slot, index, out=None):
+    """gather_rows_mapped with a device cache of some rows: slot (int32 [n_rows]) maps row r to cache[slot[r]] when
+    slot[r] >= 0, which is read from device memory instead of over the host link; -1 reads the host table.  cache:
+    float32 [C, num_features] CUDA tensor (rows contiguous, any row stride).  cache, slot, index and out share one
+    device.  The cache and the map are recorded on the stream the gather runs on, so dropping them while it is pending
+    is safe."""
+    _check(index, torch.int32, "index")
+    _check(slot, torch.int32, "slot")
+    if not (torch.is_tensor(cache) and cache.is_cuda and cache.dtype == torch.float32 and cache.dim() == 2
+            and cache.shape[1] == num_features):
+        raise TypeError("cache must be a float32 CUDA tensor of shape [C, {}]".format(num_features))
+    if slot.numel() != n_rows:
+        raise ValueError("slot must have one entry per table row ({} != {})".format(slot.numel(), n_rows))
+    n = index.numel()
+    if out is None:
+        out = torch.empty((n, num_features), dtype=torch.float32, device=index.device)
+    elif not (torch.is_tensor(out) and out.is_cuda and out.dtype == torch.float32 and tuple(out.shape) == (n, num_features)):
+        raise TypeError("out must be a float32 CUDA tensor of shape {}".format((n, num_features)))
+    if not (cache.device == slot.device == index.device == out.device):
+        raise ValueError("cache, slot, index and out must be on one device")
+    if n:
+        ldc = _row_major_2d(cache, "cache")
+        ldo = _row_major_2d(out, "out")
+        stream = torch.cuda.current_stream(out.device)
+        _ffi.call("tfgk_gather_rows_cached_f32", ctypes.c_void_p(table_ptr), ld, n_rows, num_features, _p(cache), ldc,
+                  _p(slot), _p(index), n, _p(out), ldo, ctypes.c_void_p(stream.cuda_stream))
+        cache.record_stream(stream)
+        slot.record_stream(stream)
+    return out
+
+
 # ---- a CSR built from an edge list in host memory (utils.HostNeighborSampler) -------------------------------------
 # row_ptr, col_ptr, w_ptr: device addresses of page-locked host arrays (host_register), int32 / int32 / float32 [E]
 

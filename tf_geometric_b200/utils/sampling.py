@@ -16,7 +16,9 @@ layer computes only the rows it must.  The sizes stay on the device until the ba
 synchronisation per batch.
 
 HostFeatureTable keeps an [N, F] float32 feature table in host memory (page-locked in place) and gathers the rows a batch
-reads over the host link (tfgk_gather_rows_mapped_f32), so the table need not fit on the device."""
+reads over the host link (tfgk_gather_rows_mapped_f32), so the table need not fit on the device.  With device_rows it
+also keeps those rows in device memory and reads them from there (tfgk_gather_rows_cached_f32); rank_source_rows
+orders a graph's rows by how many sampled batches read them, to choose which rows to keep."""
 import mmap
 import threading
 
@@ -387,13 +389,23 @@ class HostFeatureTable(object):
     when the last of them closes.  The
     table keeps a reference to x.  A host table is a constant: x must not require grad.
 
-    gather(index) and SampledBlocks.source_rows(table) return new float32 device tensors, bit-identical to x[index].
-    close() (or leaving a `with` block) releases the registration after the current device's pending work; a table
-    that is dropped without close() releases it when it is collected."""
+    device_rows: optional integer id vector (numpy, CPU or CUDA; int32 CUDA is used as it is) of rows to keep in device
+    memory as well, on device_rows' device if it is a CUDA tensor, otherwise on the current device.  Those rows are
+    copied once, by the same host gather, to a [C, F] device buffer, next to an int32 [N] map from row to buffer slot
+    (-1: not cached).  A gather on that device reads cached rows from device memory and the rest over the host link, in
+    one launch; a gather on another device reads every row over the link.  Either way the bits are x[index].  The ids
+    are checked with one read-back: IndexError outside [0, N), ValueError for a repeated id or an array that is not a
+    vector, TypeError for non-integer ids.  The constructor returns once the device rows are in place, so any stream
+    may gather at once.  None or an empty vector keeps no rows on the device.  rank_source_rows chooses the rows.
 
-    def __init__(self, x):
+    gather(index) and SampledBlocks.source_rows(table) return new float32 device tensors, bit-identical to x[index].
+    close() (or leaving a `with` block) drops the device rows and releases the registration after the current device's
+    pending work; a table that is dropped without close() does both when it is collected."""
+
+    def __init__(self, x, device_rows=None):
         self._closed = True                 # until registration succeeds: nothing for close() / __del__ to release
         self._key = None
+        self._cache = self._slot = self._device_rows = None
         array = x
         if isinstance(x, np.ndarray):
             x = torch.from_numpy(x)
@@ -412,10 +424,20 @@ class HostFeatureTable(object):
             raise ValueError("HostFeatureTable needs unit column stride (got strides {})".format(tuple(x.stride())))
         if n > 1 and x.stride(0) < F:
             raise ValueError("HostFeatureTable needs rows that do not overlap (got strides {})".format(tuple(x.stride())))
+        rows = None if device_rows is None else _cached_ids(device_rows, n)
         self.x = x
         self._ld = max(F, x.stride(0))
         self._key, self._ptr = _host_acquire(x, array)
         self._closed = False
+        if rows is not None:
+            self._cache = ops.gather_rows_mapped(self._ptr, self._ld, n, F, rows)
+            slot = torch.full((n,), -1, dtype=torch.int32, device=rows.device)
+            slot[rows.long()] = torch.arange(rows.numel(), dtype=torch.int32, device=rows.device)
+            self._slot, self._device_rows = slot, rows
+            # the cache and the map are private, so no caller can order a gather on another stream after their fill:
+            # the table is ready for any stream when the constructor returns
+            if rows.is_cuda:
+                torch.cuda.current_stream(rows.device).synchronize()
 
     @property
     def num_rows(self):
@@ -424,6 +446,18 @@ class HostFeatureTable(object):
     @property
     def num_features(self):
         return self.x.shape[1]
+
+    @property
+    def device_rows(self):
+        """The ids of the rows kept in device memory (int32 on the device, in cache order), or None."""
+        return self._device_rows
+
+    @property
+    def device_bytes(self):
+        """Device memory this table holds: the cached rows plus the row-to-slot map (0 without device rows)."""
+        if self._cache is None:
+            return 0
+        return self._cache.numel() * 4 + self._slot.numel() * 4
 
     def _check_open(self):
         if self._closed:
@@ -434,6 +468,9 @@ class HostFeatureTable(object):
         self._check_open()
         if index.numel() == 0 and out is None:
             return torch.empty((0, self.num_features), dtype=torch.float32, device=index.device)
+        if self._cache is not None and index.device == self._cache.device:
+            return ops.gather_rows_cached(self._ptr, self._ld, self.num_rows, self.num_features, self._cache, self._slot,
+                                          index.contiguous(), out)
         return ops.gather_rows_mapped(self._ptr, self._ld, self.num_rows, self.num_features, index.contiguous(), out)
 
     def gather(self, index, out=None):
@@ -451,10 +488,12 @@ class HostFeatureTable(object):
         return self._gather(idx.to(torch.int32), out)
 
     def close(self):
-        """Release the registration this table holds (the last table over a storage unregisters it).  Idempotent."""
+        """Drop the device rows and release the registration this table holds (the last table over a storage
+        unregisters it).  Idempotent."""
         if self._closed:
             return
         self._closed = True
+        self._cache = self._slot = self._device_rows = None
         key, self._key = self._key, None
         _host_release(key)
 
@@ -469,6 +508,57 @@ class HostFeatureTable(object):
             self.close()
         except Exception:
             pass
+
+
+def _cached_ids(device_rows, num_rows):
+    """HostFeatureTable's device_rows as an int32 device vector of distinct ids in [0, num_rows), or None when empty;
+    one read-back checks range and repeats."""
+    ids = ops.as_device(device_rows)
+    if ids.dim() != 1:
+        raise ValueError("device_rows takes an id vector (got {} dimensions)".format(ids.dim()))
+    if ids.numel() == 0:
+        return None
+    if ids.dtype.is_floating_point or ids.dtype.is_complex or ids.dtype == torch.bool:
+        raise TypeError("device_rows takes integer ids (got {})".format(ids.dtype))
+    lo, hi = torch.aminmax(ids)
+    # ids clamped into range only so that the count is defined; an id outside the range is refused before it matters
+    count = ops.segment_count(ids.clamp(0, max(num_rows - 1, 0)).to(torch.int32), max(num_rows, 1))
+    lo, hi, most = torch.stack([lo.long(), hi.long(), count.max().long()]).tolist()
+    if lo < 0 or hi >= num_rows:
+        raise IndexError("device_rows holds ids outside [0, {})".format(num_rows))
+    if most > 1:
+        raise ValueError("device_rows holds a repeated id")
+    return ids.to(torch.int32, copy=True)            # the table's own copy: the caller may reuse its buffer
+
+
+def rank_source_rows(batches):
+    """Rank a graph's rows by how often sampled batches read them, to choose HostFeatureTable's device_rows.
+
+    batches: an iterable of SampledBlocks from sample_blocks (RandomNeighborSampler or HostNeighborSampler) over one
+    graph; nothing is sampled here.  Returns (ids, counts), int32 on the batches' device: counts[j] is the number of
+    batches whose node_index (layer 0's source rows) holds j, and ids lists every j with counts[j] > 0, most-read first,
+    ties by smaller id.  One host read-back at the end.  ValueError for a batch built by hand (num_nodes None) or
+    batches over different node counts.  An empty iterable gives two empty vectors."""
+    counts = None
+    num_nodes = None
+    for b in batches:
+        if b.num_nodes is None:
+            raise ValueError("rank_source_rows takes batches from sample_blocks (this one was built by hand)")
+        if counts is None:
+            num_nodes = b.num_nodes
+            counts = ops.segment_count(b.node_index, num_nodes)
+            continue
+        if b.num_nodes != num_nodes:
+            raise ValueError("batches over {} and {} nodes: rank_source_rows takes batches of one graph".format(
+                num_nodes, b.num_nodes))
+        counts += ops.segment_count(b.node_index, num_nodes)
+    if counts is None:
+        empty = torch.empty((0,), dtype=torch.int32, device=ops.default_device())
+        return empty, empty.clone()
+    # radix keys ~count: read as unsigned, a larger count is a smaller key, and the stable sort keeps ties in id order
+    order = ops.stable_argsort(torch.bitwise_not(counts), key_bits=32)
+    read = int(torch.count_nonzero(counts).item())
+    return order[:read], counts
 
 
 class RandomNeighborSampler(_SamplerBase):
