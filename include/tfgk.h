@@ -676,6 +676,69 @@ int tfgk_block_gcn_values_f32(const int64_t *rowptr, const int32_t *gcol, const 
                               int32_t n_dst, const int64_t *g_rowptr, const float *g_rowsum, int norm, int loop,
                               float deg_fill, float fill, float *out, void *stream);
 
+/* Link prediction on sampled blocks (utils.LinkBlocks): a block batch seeded by the endpoints of node pairs, with the
+ * batch's target edges optionally excluded from the CSR rows their endpoints sample.
+ * _begin_pairs: tfgk_block_sample_begin for the endpoint list pair_row[0], pair_col[0], pair_row[1], ... of n_pairs pairs:
+ *   the frontier of an empty list over those 2 n_pairs ids, so nodes[0, n_seeds) holds the distinct endpoints in
+ *   first-occurrence order, map[id] their positions and state[3] = n_seeds (on the device).  Endpoints outside [0, N) are
+ *   counted in state[0] and relabelled -1.  local int32 [2, n_pairs]: the pairs relabelled (sources, then destinations).
+ *   Hop 0's capacity is 2 n_pairs.  Workspace: tfgk_block_pairs_workspace_bytes(n_pairs).  Asynchronous; _count, _fill
+ *   and _end follow as for _begin.
+ * tfgk_link_tail_negatives_i32: out_row[i] = src[i / q], out_col[i] = random_below(seed, rng_stream, i, N) for
+ *   i < n_src * q (tail corruption, uniform over [0, N)).  One launch, asynchronous.
+ * Exclusion lists, for the cap >= n_seeds first rows of the list `nodes`: target_src / target_dst [n_targets] are the
+ *   (local row, global column) pairs to exclude, sorted by (source, destination) (sources outside [0, cap) are
+ *   skipped).  Row t's list is every position p of CSR row nodes[t] whose column col[p] is a target of t, ascending; a
+ *   position is listed once however many targets match it.  col may be device memory or page-locked host memory; each
+ *   targeted row reads its deg columns once per pass.
+ *   _count writes excl_off int64 [cap + 1] (exclusive offsets) and the total to *total_host (synchronises).  _fill
+ *   (int32 positions) and _fill_mapped (int64 positions, a CSR in host memory) then write excl_pos [total], with the
+ *   workspace _count used: tfgk_block_exclusion_workspace_bytes(cap).
+ * _count_excl, _fill_excl, _fill_mapped_excl: _count, _fill and _fill_mapped where list row t < n_excl skips the
+ *   x_t = excl_off[t + 1] - excl_off[t] positions excl_pos[excl_off[t], excl_off[t + 1]) of its CSR row: the rule and
+ *   the draws run over the deg - x_t kept entries in CSR order, so the hop equals that of the same call on the CSR with
+ *   those entries deleted.  Rows without exclusions take the plain path.
+ * tfgk_block_gcn_values_excl_f32: tfgk_block_gcn_values_f32 where output row r < n_excl scales its edges by
+ *   s_r = (n_g - x_r) / k_r. */
+int tfgk_block_pairs_workspace_bytes(int32_t n_pairs, size_t *out_bytes);
+int tfgk_block_sample_begin_pairs(const int32_t *pair_row, const int32_t *pair_col, int32_t n_pairs, int32_t N,
+                                  int32_t *nodes, int32_t *map, int32_t *state, int32_t n_hops, int32_t *local,
+                                  void *workspace, size_t workspace_bytes, void *stream);
+int tfgk_link_tail_negatives_i32(const int32_t *src, int32_t n_src, int32_t q, int32_t N, uint64_t seed,
+                                 uint32_t rng_stream, int32_t *out_row, int32_t *out_col, void *stream);
+int tfgk_block_exclusion_workspace_bytes(int32_t cap, size_t *out_bytes);
+int tfgk_block_exclusion_count(const int64_t *rowptr, int32_t n_rows, const int32_t *col, const int32_t *nodes,
+                               int32_t cap, const int32_t *target_src, const int32_t *target_dst, int64_t n_targets,
+                               int64_t *excl_off, int64_t *total_host, void *workspace, size_t workspace_bytes,
+                               void *stream);
+int tfgk_block_exclusion_fill(const int64_t *rowptr, int32_t n_rows, const int32_t *col, const int32_t *nodes,
+                              int32_t cap, const int32_t *target_dst, const int64_t *excl_off, int32_t *excl_pos,
+                              void *workspace, size_t workspace_bytes, void *stream);
+int tfgk_block_exclusion_fill_mapped(const int64_t *rowptr, int32_t n_rows, const int32_t *col, const int32_t *nodes,
+                                     int32_t cap, const int32_t *target_dst, const int64_t *excl_off, int64_t *excl_pos,
+                                     void *workspace, size_t workspace_bytes, void *stream);
+int tfgk_block_sample_count_excl(const int64_t *rowptr, int32_t n_rows, const int32_t *nodes, const int32_t *state,
+                                 int32_t hop, int32_t n_hops, int32_t cap_list, int32_t k, int padding,
+                                 const int64_t *excl_off, int32_t n_excl, int64_t *out_rowptr, void *workspace,
+                                 size_t workspace_bytes, void *stream);
+int tfgk_block_sample_fill_excl(const int64_t *rowptr, int32_t n_rows, const int32_t *col, const float *w_csr,
+                                int32_t N, int32_t *nodes, int32_t *map, int32_t *state, int32_t hop, int32_t n_hops,
+                                int32_t cap_list, int64_t cap_edges, int32_t k, int padding, uint64_t seed,
+                                uint32_t rng_stream, const int64_t *out_rowptr, int32_t *out_row, int32_t *out_local,
+                                int32_t *out_gcol, float *out_w, const int64_t *excl_off, const int32_t *excl_pos,
+                                int32_t n_excl, void *workspace, size_t workspace_bytes, void *stream);
+int tfgk_block_sample_fill_mapped_excl(const int64_t *rowptr, int32_t n_rows, const int32_t *col, const float *w_csr,
+                                       int32_t N, int32_t *nodes, int32_t *map, int32_t *state, int32_t hop,
+                                       int32_t n_hops, int32_t cap_list, int64_t cap_edges, int32_t k, int padding,
+                                       uint64_t seed, uint32_t rng_stream, const int64_t *out_rowptr, int32_t *out_row,
+                                       int32_t *out_local, int32_t *out_gcol, float *out_w, const int64_t *excl_off,
+                                       const int64_t *excl_pos, int32_t n_excl, void *workspace, size_t workspace_bytes,
+                                       void *stream);
+int tfgk_block_gcn_values_excl_f32(const int64_t *rowptr, const int32_t *gcol, const float *w, int64_t S,
+                                   const int32_t *dst, int32_t n_dst, const int64_t *g_rowptr, const float *g_rowsum,
+                                   int norm, int loop, float deg_fill, float fill, const int64_t *excl_off,
+                                   int32_t n_excl, float *out, void *stream);
+
 /* ---- link prediction (SURVEY.md 8(f)5, demo/demo_gae.py) -------------------------------------------------------- */
 
 /* K6, predict_edge of demo/demo_gae.py:53-60: out[e] = sum_d h[row_e, d] * h[col_e, d] in fp32, COO order.

@@ -700,15 +700,17 @@ class BlockMax(torch.autograd.Function):
         return ops.spmm_max_bwd(csr_t, None, x, out, cnt, grad_out.contiguous()), None
 
 
-def _half_edge_csr(edge_index, num_nodes):
+def _half_edge_csr(edge_index, num_nodes, ids_in_range=False):
     """CSR of the 2E half-edges of a query edge list: keys [row || col], partners [col || row].  Memoised on the edge
-    tensor."""
+    tensor.  ids_in_range=True (ids known to lie in [0, num_nodes)) skips the id check and the work plan, so the build
+    makes no host synchronisation."""
     tag = ("half_edges", int(num_nodes))
     hit = _structure._lookup(edge_index, tag)
     if hit is None:
         row, col = edge_index[0].contiguous(), edge_index[1].contiguous()
-        hit = _structure._store(edge_index, tag, ops.csr_build(torch.cat([row, col]), torch.cat([col, row]), num_nodes,
-                                                               num_nodes))
+        half = (torch.cat([row, col]), torch.cat([col, row]), num_nodes, num_nodes)
+        csr = ops.csr_build(*half, ids_in_range=True, plan=False) if ids_in_range else ops.csr_build(*half)
+        hit = _structure._store(edge_index, tag, csr)
     return hit
 
 

@@ -111,18 +111,41 @@ __device__ __forceinline__ void atomic_max_pos(int64_t *p, int64_t v) {
     atomicMax(reinterpret_cast<unsigned long long *>(p), (unsigned long long)v);
 }
 
+// Excluded CSR entries (the link sampler's target edges): list row t < n_excl skips the x_t ascending CSR positions
+// excl_pos[excl_off[t], excl_off[t + 1]).  Its rule and draws run over the deg - x_t kept entries, so a draw's position is
+// virtual (the v-th kept entry); excl_real maps it to the real one.  The j-th excluded entry has e_j - j kept entries
+// before it, a nondecreasing count, so the v-th kept entry lies past exactly the j with e_j - j <= v.
+__device__ __forceinline__ int excl_count(const int64_t *__restrict__ excl_off, int32_t n_excl, int64_t t) {
+    return t < n_excl ? (int)(excl_off[t + 1] - excl_off[t]) : 0;
+}
+
+template <typename TPos>
+__device__ __forceinline__ TPos excl_real(const TPos *__restrict__ ex, int x, int64_t start, TPos p) {
+    const int64_t v = (int64_t)p - start;
+    int lo = 0, hi = x;
+    while (lo < hi) {
+        const int mid = (lo + hi) >> 1;
+        if ((int64_t)ex[mid] - start - mid <= v) lo = mid + 1;
+        else hi = mid;
+    }
+    return (TPos)(p + lo);
+}
+
 // The fill of K13.  kBlock (the block sampler) also writes every sampled edge's global column col[pos] and weight
 // w_csr[pos] (1.0f when w_csr is null), once its position is final; the plain instantiation leaves that to the caller's
 // gathers.  TPos is the type of the CSR positions: int32_t for a CSR on the device, int64_t for one in host memory, which
-// may hold 2^31 edges or more.
-template <bool kBlock, typename TPos>
+// may hold 2^31 edges or more.  kExcl (with kBlock) skips the excluded entries above: positions stay virtual until the
+// final pass maps them, so the reservoir's atomicMax compares virtual positions, in the same order as the real ones.
+template <bool kBlock, typename TPos, bool kExcl = false>
 __device__ __forceinline__ void sample_rows_fill_body(const int64_t *__restrict__ rowptr, int32_t n_rows,
                                                       const int32_t *__restrict__ rows, int32_t n_list, int k,
                                                       double ratio, int padding, uint64_t seed, uint32_t stream,
                                                       const int64_t *__restrict__ out_rowptr, int32_t *__restrict__ out_row,
                                                       TPos *__restrict__ out_pos, const int32_t *__restrict__ csr_col,
                                                       const float *__restrict__ w_csr, int32_t *__restrict__ out_gcol,
-                                                      float *__restrict__ out_w) {
+                                                      float *__restrict__ out_w,
+                                                      const int64_t *__restrict__ excl_off = nullptr,
+                                                      const TPos *__restrict__ excl_pos = nullptr, int32_t n_excl = 0) {
     __shared__ int32_t long_rows[kRowsPerCta];
     __shared__ int n_long;
     if (threadIdx.x == 0) n_long = 0;
@@ -132,7 +155,8 @@ __device__ __forceinline__ void sample_rows_fill_body(const int64_t *__restrict_
         const int32_t r = rows[t];
         if (r >= 0 && r < n_rows) {
             const int64_t start = rowptr[r];
-            const int deg = (int)(rowptr[r + 1] - start);
+            const int x = kExcl ? excl_count(excl_off, n_excl, t) : 0;
+            const int deg = (int)(rowptr[r + 1] - start) - x;
             if (deg > kThreadRowMax) {
                 long_rows[atomicAdd(&n_long, 1)] = threadIdx.x;      // slot order is irrelevant: rows write disjoint ranges
             } else {
@@ -155,7 +179,9 @@ __device__ __forceinline__ void sample_rows_fill_body(const int64_t *__restrict_
                 }
                 if constexpr (kBlock)
                     for (int i = 0; i < num; ++i) {
-                        const TPos p = out_pos[o + i];
+                        TPos p = out_pos[o + i];
+                        if constexpr (kExcl)
+                            if (x) p = excl_real(excl_pos + excl_off[t], x, start, p);
                         out_gcol[o + i] = csr_col[p];
                         out_w[o + i] = w_csr ? w_csr[p] : 1.0f;
                     }
@@ -169,7 +195,7 @@ __device__ __forceinline__ void sample_rows_fill_body(const int64_t *__restrict_
         const int64_t tl = (int64_t)blockIdx.x * kRowsPerCta + long_rows[q];
         const int32_t r = rows[tl];
         const int64_t start = rowptr[r];
-        const int deg = (int)(rowptr[r + 1] - start);
+        const int deg = (int)(rowptr[r + 1] - start) - (kExcl ? excl_count(excl_off, n_excl, tl) : 0);
         int num;
         const int rule = sample_rule(deg, k, ratio, padding, num);
         const int64_t o = out_rowptr[tl];
@@ -186,7 +212,7 @@ __device__ __forceinline__ void sample_rows_fill_body(const int64_t *__restrict_
         const int64_t tl = (int64_t)blockIdx.x * kRowsPerCta + long_rows[q];
         const int32_t r = rows[tl];
         const int64_t start = rowptr[r];
-        const int deg = (int)(rowptr[r + 1] - start);
+        const int deg = (int)(rowptr[r + 1] - start) - (kExcl ? excl_count(excl_off, n_excl, tl) : 0);
         int num;
         if (sample_rule(deg, k, ratio, padding, num) != kSampleReservoir) continue;
         const int64_t o = out_rowptr[tl];
@@ -201,11 +227,14 @@ __device__ __forceinline__ void sample_rows_fill_body(const int64_t *__restrict_
         for (int q = 0; q < nl; ++q) {
             const int64_t tl = (int64_t)blockIdx.x * kRowsPerCta + long_rows[q];
             const int32_t r = rows[tl];
+            const int x = kExcl ? excl_count(excl_off, n_excl, tl) : 0;
             int num;
-            sample_rule((int)(rowptr[r + 1] - rowptr[r]), k, ratio, padding, num);
+            sample_rule((int)(rowptr[r + 1] - rowptr[r]) - x, k, ratio, padding, num);
             const int64_t o = out_rowptr[tl];
             for (int i = threadIdx.x; i < num; i += kRowsPerCta) {
-                const TPos p = out_pos[o + i];
+                TPos p = out_pos[o + i];
+                if constexpr (kExcl)
+                    if (x) p = excl_real(excl_pos + excl_off[tl], x, rowptr[r], p);
                 out_gcol[o + i] = csr_col[p];
                 out_w[o + i] = w_csr ? w_csr[p] : 1.0f;
             }
@@ -315,18 +344,36 @@ __global__ void block_begin_kernel(const int32_t *__restrict__ seeds, int32_t n,
     }
 }
 
-// listed rows past the device count contribute 0, so the scan over the capacity ends in the hop's edge total
-__global__ void block_count_kernel(const int64_t *__restrict__ rowptr, int32_t n_rows, const int32_t *__restrict__ rows,
-                                   const int32_t *__restrict__ n_list, int32_t cap, int k, int padding,
-                                   int32_t *__restrict__ cnt) {
+// listed rows past the device count contribute 0, so the scan over the capacity ends in the hop's edge total; kExcl
+// counts over the kept entries of rows with exclusions (sample_rows_fill_body)
+template <bool kExcl>
+__device__ __forceinline__ void block_count_body(const int64_t *__restrict__ rowptr, int32_t n_rows,
+                                                 const int32_t *__restrict__ rows, const int32_t *__restrict__ n_list,
+                                                 int32_t cap, int k, int padding, int32_t *__restrict__ cnt,
+                                                 const int64_t *__restrict__ excl_off, int32_t n_excl) {
     const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (t >= cap) return;
     int num = 0;
     if (t < *n_list) {
         const int32_t r = rows[t];
-        if (r >= 0 && r < n_rows) sample_rule((int)(rowptr[r + 1] - rowptr[r]), k, -1.0, padding, num);
+        if (r >= 0 && r < n_rows)
+            sample_rule((int)(rowptr[r + 1] - rowptr[r]) - (kExcl ? excl_count(excl_off, n_excl, t) : 0), k, -1.0,
+                        padding, num);
     }
     cnt[t] = num;
+}
+
+__global__ void block_count_kernel(const int64_t *__restrict__ rowptr, int32_t n_rows, const int32_t *__restrict__ rows,
+                                   const int32_t *__restrict__ n_list, int32_t cap, int k, int padding,
+                                   int32_t *__restrict__ cnt) {
+    block_count_body<false>(rowptr, n_rows, rows, n_list, cap, k, padding, cnt, nullptr, 0);
+}
+
+__global__ void block_count_excl_kernel(const int64_t *__restrict__ rowptr, int32_t n_rows,
+                                        const int32_t *__restrict__ rows, const int32_t *__restrict__ n_list, int32_t cap,
+                                        int k, int padding, int32_t *__restrict__ cnt,
+                                        const int64_t *__restrict__ excl_off, int32_t n_excl) {
+    block_count_body<true>(rowptr, n_rows, rows, n_list, cap, k, padding, cnt, excl_off, n_excl);
 }
 
 __global__ void __launch_bounds__(kRowsPerCta)
@@ -350,6 +397,31 @@ block_fill_mapped_kernel(const int64_t *__restrict__ rowptr, int32_t n_rows, con
                          const float *__restrict__ w_csr, int32_t *__restrict__ out_gcol, float *__restrict__ out_w) {
     sample_rows_fill_body<true, int64_t>(rowptr, n_rows, rows, *n_list, k, -1.0, padding, seed, stream, out_rowptr,
                                          out_row, out_pos, csr_col, w_csr, out_gcol, out_w);
+}
+
+// the minimum of 4 CTAs per SM, as for block_fill_mapped_kernel: left to itself ptxas chose 40 registers and spilled
+__global__ void __launch_bounds__(kRowsPerCta, 4)
+block_fill_excl_kernel(const int64_t *__restrict__ rowptr, int32_t n_rows, const int32_t *__restrict__ rows,
+                       const int32_t *__restrict__ n_list, int k, int padding, uint64_t seed, uint32_t stream,
+                       const int64_t *__restrict__ out_rowptr, int32_t *__restrict__ out_row, int32_t *__restrict__ out_pos,
+                       const int32_t *__restrict__ csr_col, const float *__restrict__ w_csr, int32_t *__restrict__ out_gcol,
+                       float *__restrict__ out_w, const int64_t *__restrict__ excl_off,
+                       const int32_t *__restrict__ excl_pos, int32_t n_excl) {
+    sample_rows_fill_body<true, int32_t, true>(rowptr, n_rows, rows, *n_list, k, -1.0, padding, seed, stream, out_rowptr,
+                                               out_row, out_pos, csr_col, w_csr, out_gcol, out_w, excl_off, excl_pos,
+                                               n_excl);
+}
+
+__global__ void __launch_bounds__(kRowsPerCta, 4)
+block_fill_mapped_excl_kernel(const int64_t *__restrict__ rowptr, int32_t n_rows, const int32_t *__restrict__ rows,
+                              const int32_t *__restrict__ n_list, int k, int padding, uint64_t seed, uint32_t stream,
+                              const int64_t *__restrict__ out_rowptr, int32_t *__restrict__ out_row,
+                              int64_t *__restrict__ out_pos, const int32_t *__restrict__ csr_col,
+                              const float *__restrict__ w_csr, int32_t *__restrict__ out_gcol, float *__restrict__ out_w,
+                              const int64_t *__restrict__ excl_off, const int64_t *__restrict__ excl_pos, int32_t n_excl) {
+    sample_rows_fill_body<true, int64_t, true>(rowptr, n_rows, rows, *n_list, k, -1.0, padding, seed, stream, out_rowptr,
+                                               out_row, out_pos, csr_col, w_csr, out_gcol, out_w, excl_off, excl_pos,
+                                               n_excl);
 }
 
 __global__ void block_first_kernel(const int32_t *__restrict__ cols, const int64_t *__restrict__ S, int32_t N,
@@ -430,12 +502,16 @@ __device__ __forceinline__ float gcn_scale(float v, int norm, float fr, float fc
 }
 
 // items [0, S): edge t, whose row is the last r with rowptr[r] <= t; items [S, S + n_dst) (loop modes only): the self
-// loop of row t - S.  Every output slot has exactly one writer.
-__global__ void block_gcn_values_kernel(const int64_t *__restrict__ rowptr, const int32_t *__restrict__ gcol,
-                                        const float *__restrict__ w, int64_t S, const int32_t *__restrict__ dst,
-                                        int32_t n_dst, const int64_t *__restrict__ g_rowptr,
-                                        const float *__restrict__ g_rowsum, int norm, int loop, float deg_fill, float fill,
-                                        float *__restrict__ out) {
+// loop of row t - S.  Every output slot has exactly one writer.  kExcl: row r < n_excl had x_r of its n_g entries
+// excluded, and its scale is (n_g - x_r) / k_r.
+template <bool kExcl>
+__device__ __forceinline__ void block_gcn_values_body(const int64_t *__restrict__ rowptr, const int32_t *__restrict__ gcol,
+                                                      const float *__restrict__ w, int64_t S,
+                                                      const int32_t *__restrict__ dst, int32_t n_dst,
+                                                      const int64_t *__restrict__ g_rowptr,
+                                                      const float *__restrict__ g_rowsum, int norm, int loop,
+                                                      float deg_fill, float fill, float *__restrict__ out,
+                                                      const int64_t *__restrict__ excl_off, int32_t n_excl) {
     const int64_t n = S + (loop != TFGK_GCN_LOOP_NONE ? n_dst : 0);
     for (int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; t < n; t += (int64_t)gridDim.x * blockDim.x) {
         if (t < S) {
@@ -449,7 +525,8 @@ __global__ void block_gcn_values_kernel(const int64_t *__restrict__ rowptr, cons
             const float fr = norm != TFGK_GCN_NORM_RIGHT ? gcn_degree_factor(g_rowsum[g], deg_fill, norm) : 0.0f;
             const float fc = norm != TFGK_GCN_NORM_LEFT ? gcn_degree_factor(g_rowsum[gcol[t]], deg_fill, norm) : 0.0f;
             const float v = gcn_scale(w ? w[t] : 1.0f, norm, fr, fc);
-            const float s = __fdiv_rn((float)(g_rowptr[g + 1] - g_rowptr[g]), (float)(rowptr[lo + 1] - rowptr[lo]));
+            const float s = __fdiv_rn((float)(g_rowptr[g + 1] - g_rowptr[g] - (kExcl ? excl_count(excl_off, n_excl, lo) : 0)),
+                                      (float)(rowptr[lo + 1] - rowptr[lo]));
             out[loop != TFGK_GCN_LOOP_NONE ? t + lo : t] = __fmul_rn(s, v);
         } else {
             const int32_t r = (int32_t)(t - S);
@@ -461,6 +538,104 @@ __global__ void block_gcn_values_kernel(const int64_t *__restrict__ rowptr, cons
             out[rowptr[r + 1] + r] = v;
         }
     }
+}
+
+__global__ void block_gcn_values_kernel(const int64_t *__restrict__ rowptr, const int32_t *__restrict__ gcol,
+                                        const float *__restrict__ w, int64_t S, const int32_t *__restrict__ dst,
+                                        int32_t n_dst, const int64_t *__restrict__ g_rowptr,
+                                        const float *__restrict__ g_rowsum, int norm, int loop, float deg_fill, float fill,
+                                        float *__restrict__ out) {
+    block_gcn_values_body<false>(rowptr, gcol, w, S, dst, n_dst, g_rowptr, g_rowsum, norm, loop, deg_fill, fill, out,
+                                 nullptr, 0);
+}
+
+__global__ void block_gcn_values_excl_kernel(const int64_t *__restrict__ rowptr, const int32_t *__restrict__ gcol,
+                                             const float *__restrict__ w, int64_t S, const int32_t *__restrict__ dst,
+                                             int32_t n_dst, const int64_t *__restrict__ g_rowptr,
+                                             const float *__restrict__ g_rowsum, int norm, int loop, float deg_fill,
+                                             float fill, const int64_t *__restrict__ excl_off, int32_t n_excl,
+                                             float *__restrict__ out) {
+    block_gcn_values_body<true>(rowptr, gcol, w, S, dst, n_dst, g_rowptr, g_rowsum, norm, loop, deg_fill, fill, out,
+                                excl_off, n_excl);
+}
+
+// ---- link prediction on blocks: pair begin, tail negatives and the exclusion lists ---------------------------------
+// endpoint e of a pair list is pair e >> 1's source (e even) or destination (e odd): the seeds' first-occurrence order
+__global__ void pair_ends_kernel(const int32_t *__restrict__ pair_row, const int32_t *__restrict__ pair_col, int64_t P,
+                                 int32_t *__restrict__ ends) {
+    for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < P; e += (int64_t)gridDim.x * blockDim.x)
+        ends[e] = (e & 1) ? pair_col[e >> 1] : pair_row[e >> 1];
+}
+
+// the pairs relabelled, int32 [2, P / 2]: sources, then destinations
+__global__ void pair_gather_kernel(const int32_t *__restrict__ ends, int64_t P, int32_t N, const int32_t *__restrict__ map,
+                                   int32_t *__restrict__ local) {
+    const int64_t n_pairs = P >> 1;
+    for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < P; e += (int64_t)gridDim.x * blockDim.x) {
+        const int32_t id = ends[e];
+        local[(e & 1) * n_pairs + (e >> 1)] = (id >= 0 && id < N) ? map[id] : -1;
+    }
+}
+
+__global__ void tail_negatives_kernel(const int32_t *__restrict__ src, int64_t n, int32_t q, uint32_t N, uint64_t seed,
+                                      uint32_t stream, int32_t *__restrict__ out_row, int32_t *__restrict__ out_col) {
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+        out_row[i] = src[i / q];
+        out_col[i] = (int32_t)random_below(seed, stream, (uint64_t)i, N);
+    }
+}
+
+// [tbeg[s], tend[s]): the targets of seed s in the list sorted by (source, destination); sources outside [0, cap) (-1:
+// an endpoint outside the graph) are skipped
+__global__ void excl_mark_kernel(const int32_t *__restrict__ ts, int64_t T, int32_t cap, int32_t *__restrict__ tbeg,
+                                 int32_t *__restrict__ tend) {
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < T; i += (int64_t)gridDim.x * blockDim.x) {
+        const int32_t s = ts[i];
+        if (s < 0 || s >= cap) continue;
+        if (i == 0 || ts[i - 1] != s) tbeg[s] = (int32_t)i;
+        if (i == T - 1 || ts[i + 1] != s) tend[s] = (int32_t)(i + 1);
+    }
+}
+
+// one warp per seed row with targets, 32 entries at a time: an entry is excluded when its column is among the row's
+// sorted target destinations (binary search, so a repeated target excludes an entry once).  The count pass writes x_t;
+// the fill pass writes the excluded positions in CSR order from excl_off[t] (ballot and prefix count).
+template <bool kFill, typename TPos>
+__global__ void excl_scan_kernel(const int64_t *__restrict__ rowptr, int32_t n_rows, const int32_t *__restrict__ col,
+                                 const int32_t *__restrict__ nodes, int32_t cap, const int32_t *__restrict__ td,
+                                 const int32_t *__restrict__ tbeg, const int32_t *__restrict__ tend,
+                                 int32_t *__restrict__ cnt, const int64_t *__restrict__ excl_off, TPos *__restrict__ out) {
+    const int64_t t = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const int lane = threadIdx.x & 31;
+    if (t >= cap) return;                       // whole warps
+    const int32_t b = tbeg[t], e = tend[t];
+    int64_t n = kFill ? excl_off[t] : 0;
+    if (e > b) {
+        const int32_t r = nodes[t];
+        if (r >= 0 && r < n_rows) {
+            const int64_t end = rowptr[r + 1];
+            for (int64_t p0 = rowptr[r]; p0 < end; p0 += 32) {
+                const int64_t p = p0 + lane;
+                bool hit = false;
+                if (p < end) {
+                    const int32_t c = col[p];
+                    int32_t lo = b, hi = e;
+                    while (lo < hi) {
+                        const int32_t mid = (lo + hi) >> 1;
+                        if (td[mid] < c) lo = mid + 1;
+                        else hi = mid;
+                    }
+                    hit = lo < e && td[lo] == c;
+                }
+                const unsigned mask = __ballot_sync(0xffffffffu, hit);
+                if constexpr (kFill)
+                    if (hit) out[n + __popc(mask & ((1u << lane) - 1u))] = (TPos)p;
+                n += __popc(mask);
+            }
+        }
+    }
+    if constexpr (!kFill)
+        if (lane == 0) cnt[t] = (int32_t)n;
 }
 
 }  // namespace
@@ -787,29 +962,55 @@ int tfgk_block_sample_begin(const int32_t *seeds, int32_t n_seeds, int32_t N, in
     return TFGK_OK;
 }
 
-int tfgk_block_sample_count(const int64_t *rowptr, int32_t n_rows, const int32_t *nodes, const int32_t *state,
-                            int32_t hop, int32_t n_hops, int32_t cap_list, int32_t k, int padding, int64_t *out_rowptr,
-                            void *workspace, size_t workspace_bytes, void *stream) {
-    int rc = check_sample_mode("block_sample_count", k, -1.0, padding);
+}  // extern "C"
+
+// tfgk_block_sample_count and _count_excl (excl_off null: no exclusions)
+static int block_sample_count(const char *fn, const int64_t *rowptr, int32_t n_rows, const int32_t *nodes,
+                              const int32_t *state, int32_t hop, int32_t n_hops, int32_t cap_list, int32_t k, int padding,
+                              const int64_t *excl_off, int32_t n_excl, int64_t *out_rowptr, void *workspace,
+                              size_t workspace_bytes, void *stream) {
+    int rc = check_sample_mode(fn, k, -1.0, padding);
     if (rc != TFGK_OK) return rc;
-    TFGK_CHECK_ARG(n_rows >= 0 && hop >= 0 && hop < n_hops && cap_list >= 0, "block_sample_count: bad size");
-    TFGK_CHECK_ARG(state != nullptr && out_rowptr != nullptr, "block_sample_count: null pointer");
+    TFGK_CHECK_ARG(n_rows >= 0 && hop >= 0 && hop < n_hops && cap_list >= 0 && n_excl >= 0, "%s: bad size", fn);
+    TFGK_CHECK_ARG(state != nullptr && out_rowptr != nullptr, "%s: null pointer", fn);
     cudaStream_t st = as_stream(stream);
     if (cap_list == 0) {
         TFGK_CUDA(cudaMemsetAsync(out_rowptr, 0, 8, st));
         return TFGK_OK;
     }
-    TFGK_CHECK_ARG(rowptr != nullptr && nodes != nullptr, "block_sample_count: null rowptr or node list");
-    if ((rc = block_workspace_check("block_sample_count", cap_list, 0, workspace, workspace_bytes)) != TFGK_OK) return rc;
+    TFGK_CHECK_ARG(rowptr != nullptr && nodes != nullptr, "%s: null rowptr or node list", fn);
+    if ((rc = block_workspace_check(fn, cap_list, 0, workspace, workspace_bytes)) != TFGK_OK) return rc;
     char *ws = static_cast<char *>(workspace);
     const BlockWorkspace L(cap_list, 0);
     int32_t *cnt = reinterpret_cast<int32_t *>(ws);
-    block_count_kernel<<<(unsigned)ceil_div64(cap_list, 256), 256, 0, st>>>(rowptr, n_rows, nodes,
-                                                                            state + kStateSizes + hop, cap_list, k,
-                                                                            padding, cnt);
+    const unsigned grid = (unsigned)ceil_div64(cap_list, 256);
+    if (excl_off)
+        block_count_excl_kernel<<<grid, 256, 0, st>>>(rowptr, n_rows, nodes, state + kStateSizes + hop, cap_list, k,
+                                                      padding, cnt, excl_off, n_excl);
+    else
+        block_count_kernel<<<grid, 256, 0, st>>>(rowptr, n_rows, nodes, state + kStateSizes + hop, cap_list, k, padding,
+                                                 cnt);
     TFGK_LAUNCH_CHECK();
     return exclusive_scan<int32_t, int64_t>(cnt, cap_list, (int64_t)cap_list + 1, out_rowptr,
                                             reinterpret_cast<int64_t *>(ws + L.off_sums), st);
+}
+
+extern "C" {
+
+int tfgk_block_sample_count(const int64_t *rowptr, int32_t n_rows, const int32_t *nodes, const int32_t *state,
+                            int32_t hop, int32_t n_hops, int32_t cap_list, int32_t k, int padding, int64_t *out_rowptr,
+                            void *workspace, size_t workspace_bytes, void *stream) {
+    return block_sample_count("block_sample_count", rowptr, n_rows, nodes, state, hop, n_hops, cap_list, k, padding,
+                              nullptr, 0, out_rowptr, workspace, workspace_bytes, stream);
+}
+
+int tfgk_block_sample_count_excl(const int64_t *rowptr, int32_t n_rows, const int32_t *nodes, const int32_t *state,
+                                 int32_t hop, int32_t n_hops, int32_t cap_list, int32_t k, int padding,
+                                 const int64_t *excl_off, int32_t n_excl, int64_t *out_rowptr, void *workspace,
+                                 size_t workspace_bytes, void *stream) {
+    TFGK_CHECK_ARG(excl_off != nullptr, "block_sample_count_excl: null exclusion offsets");
+    return block_sample_count("block_sample_count_excl", rowptr, n_rows, nodes, state, hop, n_hops, cap_list, k, padding,
+                              excl_off, n_excl, out_rowptr, workspace, workspace_bytes, stream);
 }
 
 int tfgk_block_sample_read_total(const int32_t *state, int32_t hop, const int64_t *out_rowptr, int32_t cap_list,
@@ -827,18 +1028,20 @@ int tfgk_block_sample_read_total(const int32_t *state, int32_t hop, const int64_
 
 }  // extern "C"
 
-// tfgk_block_sample_fill and _fill_mapped: K13's fill at positions of type TPos, then the frontier
+// tfgk_block_sample_fill, _fill_mapped and their _excl twins (excl_off null: no exclusions): K13's fill at positions of
+// type TPos, then the frontier
 template <typename TPos>
 static int block_sample_fill(const char *fn, const int64_t *rowptr, int32_t n_rows, const int32_t *col,
                              const float *w_csr, int32_t N, int32_t *nodes, int32_t *map, int32_t *state, int32_t hop,
                              int32_t n_hops, int32_t cap_list, int64_t cap_edges, int32_t k, int padding, uint64_t seed,
                              uint32_t rng_stream, const int64_t *out_rowptr, int32_t *out_row, int32_t *out_local,
-                             int32_t *out_gcol, float *out_w, void *workspace, size_t workspace_bytes, void *stream) {
+                             int32_t *out_gcol, float *out_w, const int64_t *excl_off, const TPos *excl_pos,
+                             int32_t n_excl, void *workspace, size_t workspace_bytes, void *stream) {
     constexpr bool kMapped = sizeof(TPos) == 8;
     int rc = check_sample_mode(fn, k, -1.0, padding);
     if (rc != TFGK_OK) return rc;
     TFGK_CHECK_ARG(n_rows >= 0 && N >= 0 && hop >= 0 && hop < n_hops && cap_list >= 0 && cap_edges >= 0 &&
-                   cap_edges < (1ll << 31) - 1, "%s: bad size", fn);
+                   cap_edges < (1ll << 31) - 1 && n_excl >= 0, "%s: bad size", fn);
     TFGK_CHECK_ARG(state && out_rowptr, "%s: null pointer", fn);
     if ((rc = block_workspace_check(fn, cap_list, cap_edges, workspace, workspace_bytes, sizeof(TPos))) != TFGK_OK)
         return rc;
@@ -854,13 +1057,26 @@ static int block_sample_fill(const char *fn, const int64_t *rowptr, int32_t n_ro
         TFGK_CHECK_ARG(rowptr && col && (w_csr || kMapped) && nodes && map && out_row && out_local && out_gcol && out_w,
                        "%s: null pointer", fn);
         const unsigned grid = (unsigned)ceil_div64(cap_list, kRowsPerCta);
-        if constexpr (kMapped)
-            block_fill_mapped_kernel<<<grid, kRowsPerCta, 0, st>>>(rowptr, n_rows, nodes, n_list, k, padding, seed,
-                                                                  rng_stream, out_rowptr, out_row, pos, col, w_csr,
-                                                                  out_gcol, out_w);
-        else
-            block_fill_kernel<<<grid, kRowsPerCta, 0, st>>>(rowptr, n_rows, nodes, n_list, k, padding, seed, rng_stream,
-                                                           out_rowptr, out_row, pos, col, w_csr, out_gcol, out_w);
+        if constexpr (kMapped) {
+            if (excl_off)
+                block_fill_mapped_excl_kernel<<<grid, kRowsPerCta, 0, st>>>(rowptr, n_rows, nodes, n_list, k, padding,
+                                                                           seed, rng_stream, out_rowptr, out_row, pos,
+                                                                           col, w_csr, out_gcol, out_w, excl_off,
+                                                                           excl_pos, n_excl);
+            else
+                block_fill_mapped_kernel<<<grid, kRowsPerCta, 0, st>>>(rowptr, n_rows, nodes, n_list, k, padding, seed,
+                                                                      rng_stream, out_rowptr, out_row, pos, col, w_csr,
+                                                                      out_gcol, out_w);
+        } else {
+            if (excl_off)
+                block_fill_excl_kernel<<<grid, kRowsPerCta, 0, st>>>(rowptr, n_rows, nodes, n_list, k, padding, seed,
+                                                                    rng_stream, out_rowptr, out_row, pos, col, w_csr,
+                                                                    out_gcol, out_w, excl_off, excl_pos, n_excl);
+            else
+                block_fill_kernel<<<grid, kRowsPerCta, 0, st>>>(rowptr, n_rows, nodes, n_list, k, padding, seed,
+                                                               rng_stream, out_rowptr, out_row, pos, col, w_csr, out_gcol,
+                                                               out_w);
+        }
         TFGK_LAUNCH_CHECK();
         block_first_kernel<<<grid_for(cap_edges), 256, 0, st>>>(out_gcol, S, N, map, state);
         TFGK_LAUNCH_CHECK();
@@ -890,7 +1106,20 @@ int tfgk_block_sample_fill(const int64_t *rowptr, int32_t n_rows, const int32_t 
                            float *out_w, void *workspace, size_t workspace_bytes, void *stream) {
     return block_sample_fill<int32_t>("block_sample_fill", rowptr, n_rows, col, w_csr, N, nodes, map, state, hop, n_hops,
                                       cap_list, cap_edges, k, padding, seed, rng_stream, out_rowptr, out_row, out_local,
-                                      out_gcol, out_w, workspace, workspace_bytes, stream);
+                                      out_gcol, out_w, nullptr, nullptr, 0, workspace, workspace_bytes, stream);
+}
+
+int tfgk_block_sample_fill_excl(const int64_t *rowptr, int32_t n_rows, const int32_t *col, const float *w_csr,
+                                int32_t N, int32_t *nodes, int32_t *map, int32_t *state, int32_t hop, int32_t n_hops,
+                                int32_t cap_list, int64_t cap_edges, int32_t k, int padding, uint64_t seed,
+                                uint32_t rng_stream, const int64_t *out_rowptr, int32_t *out_row, int32_t *out_local,
+                                int32_t *out_gcol, float *out_w, const int64_t *excl_off, const int32_t *excl_pos,
+                                int32_t n_excl, void *workspace, size_t workspace_bytes, void *stream) {
+    TFGK_CHECK_ARG(excl_off != nullptr && excl_pos != nullptr, "block_sample_fill_excl: null exclusion lists");
+    return block_sample_fill<int32_t>("block_sample_fill_excl", rowptr, n_rows, col, w_csr, N, nodes, map, state, hop,
+                                      n_hops, cap_list, cap_edges, k, padding, seed, rng_stream, out_rowptr, out_row,
+                                      out_local, out_gcol, out_w, excl_off, excl_pos, n_excl, workspace, workspace_bytes,
+                                      stream);
 }
 
 int tfgk_block_sample_fill_mapped(const int64_t *rowptr, int32_t n_rows, const int32_t *col, const float *w_csr,
@@ -901,7 +1130,21 @@ int tfgk_block_sample_fill_mapped(const int64_t *rowptr, int32_t n_rows, const i
                                   void *stream) {
     return block_sample_fill<int64_t>("block_sample_fill_mapped", rowptr, n_rows, col, w_csr, N, nodes, map, state, hop,
                                       n_hops, cap_list, cap_edges, k, padding, seed, rng_stream, out_rowptr, out_row,
-                                      out_local, out_gcol, out_w, workspace, workspace_bytes, stream);
+                                      out_local, out_gcol, out_w, nullptr, nullptr, 0, workspace, workspace_bytes, stream);
+}
+
+int tfgk_block_sample_fill_mapped_excl(const int64_t *rowptr, int32_t n_rows, const int32_t *col, const float *w_csr,
+                                       int32_t N, int32_t *nodes, int32_t *map, int32_t *state, int32_t hop,
+                                       int32_t n_hops, int32_t cap_list, int64_t cap_edges, int32_t k, int padding,
+                                       uint64_t seed, uint32_t rng_stream, const int64_t *out_rowptr, int32_t *out_row,
+                                       int32_t *out_local, int32_t *out_gcol, float *out_w, const int64_t *excl_off,
+                                       const int64_t *excl_pos, int32_t n_excl, void *workspace, size_t workspace_bytes,
+                                       void *stream) {
+    TFGK_CHECK_ARG(excl_off != nullptr && excl_pos != nullptr, "block_sample_fill_mapped_excl: null exclusion lists");
+    return block_sample_fill<int64_t>("block_sample_fill_mapped_excl", rowptr, n_rows, col, w_csr, N, nodes, map, state,
+                                      hop, n_hops, cap_list, cap_edges, k, padding, seed, rng_stream, out_rowptr, out_row,
+                                      out_local, out_gcol, out_w, excl_off, excl_pos, n_excl, workspace, workspace_bytes,
+                                      stream);
 }
 
 int tfgk_block_sample_end(const int32_t *nodes, int32_t cap_nodes, int32_t N, int32_t *map, const int32_t *state,
@@ -932,10 +1175,15 @@ int tfgk_block_self_loops_i32(const int64_t *rowptr, const int32_t *row, const i
     return TFGK_OK;
 }
 
-int tfgk_block_gcn_values_f32(const int64_t *rowptr, const int32_t *gcol, const float *w, int64_t S, const int32_t *dst,
-                              int32_t n_dst, const int64_t *g_rowptr, const float *g_rowsum, int norm, int loop,
-                              float deg_fill, float fill, float *out, void *stream) {
-    TFGK_CHECK_ARG(S >= 0 && n_dst >= 0, "block_gcn_values: bad size (S=%lld, n_dst=%d)", (long long)S, n_dst);
+}  // extern "C"
+
+// tfgk_block_gcn_values_f32 and _excl_f32 (excl_off null: no exclusions)
+static int block_gcn_values(const int64_t *rowptr, const int32_t *gcol, const float *w, int64_t S, const int32_t *dst,
+                            int32_t n_dst, const int64_t *g_rowptr, const float *g_rowsum, int norm, int loop,
+                            float deg_fill, float fill, const int64_t *excl_off, int32_t n_excl, float *out,
+                            void *stream) {
+    TFGK_CHECK_ARG(S >= 0 && n_dst >= 0 && n_excl >= 0, "block_gcn_values: bad size (S=%lld, n_dst=%d)", (long long)S,
+                   n_dst);
     TFGK_CHECK_ARG(norm == TFGK_GCN_NORM_BOTH || norm == TFGK_GCN_NORM_LEFT || norm == TFGK_GCN_NORM_RIGHT,
                    "block_gcn_values: unknown norm %d", norm);
     TFGK_CHECK_ARG(loop == TFGK_GCN_LOOP_NONE || loop == TFGK_GCN_LOOP_NORMED || loop == TFGK_GCN_LOOP_FILL,
@@ -947,10 +1195,185 @@ int tfgk_block_gcn_values_f32(const int64_t *rowptr, const int32_t *gcol, const 
     const int64_t n = S + (loop != TFGK_GCN_LOOP_NONE ? n_dst : 0);
     if (n == 0) return TFGK_OK;
     TFGK_CHECK_ARG(rowptr && dst && g_rowptr && g_rowsum && out && (S == 0 || gcol), "block_gcn_values: null pointer");
-    block_gcn_values_kernel<<<grid_for(n), 256, 0, as_stream(stream)>>>(rowptr, gcol, w, S, dst, n_dst, g_rowptr, g_rowsum,
-                                                                         norm, loop, deg_fill, fill, out);
+    if (excl_off)
+        block_gcn_values_excl_kernel<<<grid_for(n), 256, 0, as_stream(stream)>>>(rowptr, gcol, w, S, dst, n_dst, g_rowptr,
+                                                                                  g_rowsum, norm, loop, deg_fill, fill,
+                                                                                  excl_off, n_excl, out);
+    else
+        block_gcn_values_kernel<<<grid_for(n), 256, 0, as_stream(stream)>>>(rowptr, gcol, w, S, dst, n_dst, g_rowptr,
+                                                                             g_rowsum, norm, loop, deg_fill, fill, out);
     TFGK_LAUNCH_CHECK();
     return TFGK_OK;
+}
+
+extern "C" {
+
+int tfgk_block_gcn_values_f32(const int64_t *rowptr, const int32_t *gcol, const float *w, int64_t S, const int32_t *dst,
+                              int32_t n_dst, const int64_t *g_rowptr, const float *g_rowsum, int norm, int loop,
+                              float deg_fill, float fill, float *out, void *stream) {
+    return block_gcn_values(rowptr, gcol, w, S, dst, n_dst, g_rowptr, g_rowsum, norm, loop, deg_fill, fill, nullptr, 0,
+                            out, stream);
+}
+
+int tfgk_block_gcn_values_excl_f32(const int64_t *rowptr, const int32_t *gcol, const float *w, int64_t S,
+                                   const int32_t *dst, int32_t n_dst, const int64_t *g_rowptr, const float *g_rowsum,
+                                   int norm, int loop, float deg_fill, float fill, const int64_t *excl_off,
+                                   int32_t n_excl, float *out, void *stream) {
+    TFGK_CHECK_ARG(excl_off != nullptr || n_dst == 0, "block_gcn_values_excl: null exclusion offsets");
+    return block_gcn_values(rowptr, gcol, w, S, dst, n_dst, g_rowptr, g_rowsum, norm, loop, deg_fill, fill, excl_off,
+                            n_excl, out, stream);
+}
+
+// ---- link prediction on blocks ----------------------------------------------------------------------------------
+int tfgk_block_pairs_workspace_bytes(int32_t n_pairs, size_t *out_bytes) {
+    TFGK_CHECK_ARG(out_bytes != nullptr && n_pairs >= 0 && n_pairs < (1 << 30) - 1, "block_pairs_workspace_bytes: bad argument");
+    const int64_t P = 2 * (int64_t)n_pairs;
+    *out_bytes = 3 * align_up((size_t)(P + 1) * 4) + scan_scratch_bytes(P + 1);
+    return TFGK_OK;
+}
+
+int tfgk_block_sample_begin_pairs(const int32_t *pair_row, const int32_t *pair_col, int32_t n_pairs, int32_t N,
+                                  int32_t *nodes, int32_t *map, int32_t *state, int32_t n_hops, int32_t *local,
+                                  void *workspace, size_t workspace_bytes, void *stream) {
+    TFGK_CHECK_ARG(n_pairs >= 0 && n_pairs < (1 << 30) - 1 && N >= 0 && n_hops >= 0, "block_sample_begin_pairs: bad size");
+    TFGK_CHECK_ARG(state != nullptr && (n_pairs == 0 || (pair_row && pair_col && nodes && map && local)),
+                   "block_sample_begin_pairs: null pointer");
+    size_t need = 0;
+    tfgk_block_pairs_workspace_bytes(n_pairs, &need);
+    if (n_pairs > 0 && (workspace == nullptr || workspace_bytes < need))
+        return set_error(TFGK_ERR_WORKSPACE, "block_sample_begin_pairs: workspace too small (%zu < %zu bytes)",
+                         workspace_bytes, need);
+    cudaStream_t st = as_stream(stream);
+    TFGK_CUDA(cudaMemsetAsync(state, 0, (size_t)(4 + 2 * n_hops) * 4, st));
+    if (n_pairs == 0) return TFGK_OK;
+    const int64_t P = 2 * (int64_t)n_pairs;
+    char *ws = static_cast<char *>(workspace);
+    int32_t *ends = reinterpret_cast<int32_t *>(ws);
+    int32_t *flag = reinterpret_cast<int32_t *>(ws + align_up((size_t)(P + 1) * 4));
+    int32_t *off = reinterpret_cast<int32_t *>(ws + 2 * align_up((size_t)(P + 1) * 4));
+    int32_t *sums = reinterpret_cast<int32_t *>(ws + 3 * align_up((size_t)(P + 1) * 4));
+    // the frontier of an empty list: first occurrences (ids outside [0, N) counted in state[0]), flags, scan, emit
+    pair_ends_kernel<<<grid_for(P), 256, 0, st>>>(pair_row, pair_col, P, ends);
+    TFGK_LAUNCH_CHECK();
+    frontier_first_kernel<<<grid_for(P), 256, 0, st>>>(ends, P, N, map, state);
+    TFGK_LAUNCH_CHECK();
+    frontier_flag_kernel<<<grid_for(P), 256, 0, st>>>(ends, P, N, map, flag);
+    TFGK_LAUNCH_CHECK();
+    int rc = exclusive_scan<int32_t, int32_t>(flag, P, P + 1, off, sums, st);
+    if (rc != TFGK_OK) return rc;
+    frontier_emit_kernel<<<grid_for(P), 256, 0, st>>>(ends, P, flag, off, 0, nodes, map);
+    TFGK_LAUNCH_CHECK();
+    pair_gather_kernel<<<grid_for(P), 256, 0, st>>>(ends, P, N, map, local);
+    TFGK_LAUNCH_CHECK();
+    TFGK_CUDA(cudaMemcpyAsync(state + kStateSizes, off + P, 4, cudaMemcpyDeviceToDevice, st));
+    return TFGK_OK;
+}
+
+int tfgk_link_tail_negatives_i32(const int32_t *src, int32_t n_src, int32_t q, int32_t N, uint64_t seed,
+                                 uint32_t rng_stream, int32_t *out_row, int32_t *out_col, void *stream) {
+    TFGK_CHECK_ARG(n_src >= 0 && q >= 0 && (int64_t)n_src * q < (1ll << 31) - 1, "link_tail_negatives: bad size");
+    const int64_t n = (int64_t)n_src * q;
+    if (n == 0) return TFGK_OK;
+    TFGK_CHECK_ARG(N > 0, "link_tail_negatives: no nodes to draw from");
+    TFGK_CHECK_ARG(src && out_row && out_col, "link_tail_negatives: null pointer");
+    tail_negatives_kernel<<<grid_for(n), 256, 0, as_stream(stream)>>>(src, n, q, (uint32_t)N, seed, rng_stream, out_row,
+                                                                       out_col);
+    TFGK_LAUNCH_CHECK();
+    return TFGK_OK;
+}
+
+namespace {
+struct ExclWorkspace {
+    size_t off_tend, off_cnt, off_sums, total;
+    explicit ExclWorkspace(int32_t cap) {
+        const size_t row = align_up(((size_t)cap + 1) * 4);
+        off_tend = row;
+        off_cnt = 2 * row;
+        off_sums = 3 * row;
+        total = off_sums + scan_scratch_bytes((int64_t)cap + 1);
+    }
+};
+}  // namespace
+
+int tfgk_block_exclusion_workspace_bytes(int32_t cap, size_t *out_bytes) {
+    TFGK_CHECK_ARG(out_bytes != nullptr && cap >= 0, "block_exclusion_workspace_bytes: bad argument");
+    *out_bytes = ExclWorkspace(cap).total;
+    return TFGK_OK;
+}
+
+int tfgk_block_exclusion_count(const int64_t *rowptr, int32_t n_rows, const int32_t *col, const int32_t *nodes,
+                               int32_t cap, const int32_t *target_src, const int32_t *target_dst, int64_t n_targets,
+                               int64_t *excl_off, int64_t *total_host, void *workspace, size_t workspace_bytes,
+                               void *stream) {
+    TFGK_CHECK_ARG(n_rows >= 0 && cap >= 0 && n_targets >= 0 && n_targets < (1ll << 31) - 1,
+                   "block_exclusion_count: bad size");
+    TFGK_CHECK_ARG(total_host != nullptr && excl_off != nullptr, "block_exclusion_count: null pointer");
+    *total_host = 0;
+    cudaStream_t st = as_stream(stream);
+    if (cap == 0) {
+        TFGK_CUDA(cudaMemsetAsync(excl_off, 0, 8, st));
+        return TFGK_OK;
+    }
+    TFGK_CHECK_ARG(rowptr && col && nodes && (n_targets == 0 || (target_src && target_dst)),
+                   "block_exclusion_count: null pointer");
+    const ExclWorkspace L(cap);
+    if (workspace == nullptr || workspace_bytes < L.total)
+        return set_error(TFGK_ERR_WORKSPACE, "block_exclusion_count: workspace too small (%zu < %zu bytes)",
+                         workspace_bytes, L.total);
+    char *ws = static_cast<char *>(workspace);
+    int32_t *tbeg = reinterpret_cast<int32_t *>(ws);
+    int32_t *tend = reinterpret_cast<int32_t *>(ws + L.off_tend);
+    int32_t *cnt = reinterpret_cast<int32_t *>(ws + L.off_cnt);
+    TFGK_CUDA(cudaMemsetAsync(ws, 0, L.off_cnt, st));            // tbeg = tend = 0: no targets
+    if (n_targets) {
+        excl_mark_kernel<<<grid_for(n_targets), 256, 0, st>>>(target_src, n_targets, cap, tbeg, tend);
+        TFGK_LAUNCH_CHECK();
+    }
+    excl_scan_kernel<false, int32_t><<<(unsigned)ceil_div64((int64_t)cap * 32, 256), 256, 0, st>>>(
+        rowptr, n_rows, col, nodes, cap, target_dst, tbeg, tend, cnt, nullptr, nullptr);
+    TFGK_LAUNCH_CHECK();
+    int rc = exclusive_scan<int32_t, int64_t>(cnt, cap, (int64_t)cap + 1, excl_off,
+                                              reinterpret_cast<int64_t *>(ws + L.off_sums), st);
+    if (rc != TFGK_OK) return rc;
+    TFGK_CUDA(cudaMemcpyAsync(total_host, excl_off + cap, 8, cudaMemcpyDeviceToHost, st));
+    TFGK_CUDA(cudaStreamSynchronize(st));
+    return TFGK_OK;
+}
+
+}  // extern "C"
+
+template <typename TPos>
+static int block_exclusion_fill(const char *fn, const int64_t *rowptr, int32_t n_rows, const int32_t *col,
+                                const int32_t *nodes, int32_t cap, const int32_t *target_dst, const int64_t *excl_off,
+                                TPos *excl_pos, void *workspace, size_t workspace_bytes, void *stream) {
+    TFGK_CHECK_ARG(n_rows >= 0 && cap >= 0, "%s: bad size", fn);
+    if (cap == 0) return TFGK_OK;
+    TFGK_CHECK_ARG(rowptr && col && nodes && excl_off, "%s: null pointer", fn);
+    const ExclWorkspace L(cap);
+    if (workspace == nullptr || workspace_bytes < L.total)
+        return set_error(TFGK_ERR_WORKSPACE, "%s: workspace too small (%zu < %zu bytes)", fn, workspace_bytes, L.total);
+    char *ws = static_cast<char *>(workspace);
+    excl_scan_kernel<true, TPos><<<(unsigned)ceil_div64((int64_t)cap * 32, 256), 256, 0, as_stream(stream)>>>(
+        rowptr, n_rows, col, nodes, cap, target_dst, reinterpret_cast<const int32_t *>(ws),
+        reinterpret_cast<const int32_t *>(ws + L.off_tend), nullptr, excl_off, excl_pos);
+    TFGK_LAUNCH_CHECK();
+    return TFGK_OK;
+}
+
+extern "C" {
+
+int tfgk_block_exclusion_fill(const int64_t *rowptr, int32_t n_rows, const int32_t *col, const int32_t *nodes,
+                              int32_t cap, const int32_t *target_dst, const int64_t *excl_off, int32_t *excl_pos,
+                              void *workspace, size_t workspace_bytes, void *stream) {
+    return block_exclusion_fill<int32_t>("block_exclusion_fill", rowptr, n_rows, col, nodes, cap, target_dst, excl_off,
+                                         excl_pos, workspace, workspace_bytes, stream);
+}
+
+int tfgk_block_exclusion_fill_mapped(const int64_t *rowptr, int32_t n_rows, const int32_t *col, const int32_t *nodes,
+                                     int32_t cap, const int32_t *target_dst, const int64_t *excl_off, int64_t *excl_pos,
+                                     void *workspace, size_t workspace_bytes, void *stream) {
+    return block_exclusion_fill<int64_t>("block_exclusion_fill_mapped", rowptr, n_rows, col, nodes, cap, target_dst,
+                                         excl_off, excl_pos, workspace, workspace_bytes, stream);
 }
 
 }  // extern "C"

@@ -162,9 +162,10 @@ def segment_count(ids, num_segments):
     return out
 
 
-def csr_build(row, col, n_rows, n_cols=None, ids_in_range=False):
+def csr_build(row, col, n_rows, n_cols=None, ids_in_range=False, plan=True):
     """ids_in_range=True: the ids are known to lie in [0, n_rows) x [0, n_cols) (tfgk_csr_build_in_range, which skips the
-    check and its synchronisation; the work plan is still built)."""
+    check and its synchronisation; the work plan is still built).  plan=False builds no work plan, whose build reads its
+    task counts back: with ids_in_range the build then makes no host synchronisation, and hub rows run unsplit."""
     _check(row, torch.int32, "row")
     _check(col, torch.int32, "col")
     n_cols = n_rows if n_cols is None else n_cols
@@ -180,7 +181,7 @@ def csr_build(row, col, n_rows, n_cols=None, ids_in_range=False):
               _p(rowptr), _p(col_sorted), _p(perm),
               _p(ws), need.value, _stream(row))
     csr = CSR(rowptr, col_sorted, perm, n_rows, n_cols)
-    csr.plan = build_plan(csr)
+    csr.plan = build_plan(csr) if plan else None
     return csr
 
 
@@ -1150,17 +1151,97 @@ def _check_block_fanouts(fanouts, padding):
     return padding
 
 
-def _block_sample(rowptr, col, w_csr, seeds, fanouts, keys, node_map, padding, rng_stream, mapped):
-    """block_sample's hops; col and w_csr are the fill's pointer arguments, to host memory when `mapped`."""
+def link_block_sample(rowptr, col, w_csr, pairs, n_pos, fanouts, keys, node_map, exclude=None, padding=False,
+                      rng_stream=RNG_STREAM_SAMPLER):
+    """block_sample seeded by the endpoints of node pairs (tfgk_block_sample_begin_pairs): pairs int32 [2, P] (contiguous
+    rows), whose distinct endpoints, taken pair by pair (source, then destination) in first-occurrence order, are the
+    seeds.  exclude: None, "self" (every CSR entry (u, v) of the first n_pos pairs leaves u's row, at every hop) or
+    "reverse" (and every entry (v, u)); the exclusion lists take one more host synchronisation (their total).
+    Returns (nodes, hop_sizes, hops, n_bad, local, excluded): block_sample's outputs, with n_bad counting endpoints outside
+    [0, N); local int32 [2, P], the pairs relabelled to positions in nodes; excluded = (excl_off int64, n_excl): row
+    t < n_excl of every list had excl_off[t + 1] - excl_off[t] entries excluded (None without exclusion)."""
+    padding = _check_block_fanouts(fanouts, padding)
+    _check(col, torch.int32, "col")
+    _check(w_csr, torch.float32, "w_csr")
+    return _block_sample(rowptr, _p(col), _p(w_csr), None, fanouts, keys, node_map, padding, rng_stream, False,
+                         pairs=(pairs, int(n_pos), exclude))
+
+
+def link_block_sample_mapped(rowptr, col_ptr, w_ptr, pairs, n_pos, fanouts, keys, node_map, exclude=None, padding=False,
+                             rng_stream=RNG_STREAM_SAMPLER):
+    """link_block_sample over a CSR in host memory (block_sample_mapped's arguments); the exclusion lists read the
+    targeted rows' columns over the host link."""
+    padding = _check_block_fanouts(fanouts, padding)
+    return _block_sample(rowptr, ctypes.c_void_p(col_ptr), None if w_ptr is None else ctypes.c_void_p(w_ptr), None,
+                         fanouts, keys, node_map, padding, rng_stream, True, pairs=(pairs, int(n_pos), exclude))
+
+
+def link_tail_negatives(src, q, num_nodes, seed, out_row, out_col, rng_stream=RNG_STREAM_LINK):
+    """Tail-corrupted negatives (tfgk_link_tail_negatives_i32): pair b * q + j is (src[b], random_below(seed, rng_stream,
+    b * q + j, num_nodes)), written to out_row / out_col int32 [len(src) * q]."""
+    _check(src, torch.int32, "src")
+    _check(out_row, torch.int32, "out_row")
+    _check(out_col, torch.int32, "out_col")
+    n = src.numel() * int(q)
+    if out_row.numel() != n or out_col.numel() != n:
+        raise ValueError("link_tail_negatives: outputs of {} and {} entries for {} pairs".format(
+            out_row.numel(), out_col.numel(), n))
+    _ffi.call("tfgk_link_tail_negatives_i32", _p(src), src.numel(), int(q), int(num_nodes), int(seed), int(rng_stream),
+              _p(out_row), _p(out_col), _stream(src))
+
+
+def _exclusion_lists(rowptr, col, nodes, cap, local, pairs, n_pos, exclude, mapped):
+    """(excl_off int64 [cap + 1], excl_pos): the CSR positions the first n_pos pairs exclude from the rows of the list's
+    first cap entries (tfgk_block_exclusion_*).  The targets (local source, global destination) are sorted by two stable
+    radix passes, destination first."""
+    dev = rowptr.device
+    ts, td = local[0, :n_pos], pairs[1, :n_pos]
+    if exclude == "reverse":
+        ts, td = torch.cat([ts, local[1, :n_pos]]), torch.cat([td, pairs[0, :n_pos]])
+    ts, td = ts.contiguous(), td.contiguous()
+    if ts.numel():
+        order = stable_argsort(td)
+        ts, td = gather_i32(ts, order), gather_i32(td, order)
+        order = stable_argsort(ts)
+        ts, td = gather_i32(ts, order), gather_i32(td, order)
+    need = ctypes.c_size_t()
+    _ffi.call("tfgk_block_exclusion_workspace_bytes", cap, ctypes.byref(need))
+    ws = torch.empty((max(need.value, 1),), dtype=torch.uint8, device=dev)
+    excl_off = torch.empty((cap + 1,), dtype=torch.int64, device=dev)
+    total = ctypes.c_int64()
+    n_rows = rowptr.numel() - 1
+    _ffi.call("tfgk_block_exclusion_count", _p(rowptr), n_rows, col, _p(nodes), cap, _p(ts), _p(td), ts.numel(),
+              _p(excl_off), ctypes.byref(total), _p(ws), need.value, _stream(rowptr))
+    excl_pos = torch.empty((max(total.value, 1),), dtype=torch.int64 if mapped else torch.int32, device=dev)
+    _ffi.call("tfgk_block_exclusion_fill_mapped" if mapped else "tfgk_block_exclusion_fill", _p(rowptr), n_rows, col,
+              _p(nodes), cap, _p(td), _p(excl_off), _p(excl_pos), _p(ws), need.value, _stream(rowptr))
+    return excl_off, excl_pos
+
+
+def _block_sample(rowptr, col, w_csr, seeds, fanouts, keys, node_map, padding, rng_stream, mapped, pairs=None):
+    """block_sample's hops; col and w_csr are the fill's pointer arguments, to host memory when `mapped`.  The batch
+    begins from the seed list `seeds`, or with pairs = (pair tensor, n_pos, exclude) from link_block_sample's pairs."""
     _check(rowptr, torch.int64, "rowptr")
-    _check(seeds, torch.int32, "seeds")
     _check(node_map, torch.int32, "node_map")
+    if pairs is None:
+        _check(seeds, torch.int32, "seeds")
+        n_begin = seeds.numel()
+    else:
+        pair_t, n_pos, exclude = pairs
+        _check(pair_t, torch.int32, "pairs")
+        if pair_t.dim() != 2 or pair_t.shape[0] != 2 or not 0 <= n_pos <= pair_t.shape[1]:
+            raise ValueError("link_block_sample: pairs must be [2, P] with n_pos <= P (got {}, n_pos {})".format(
+                tuple(pair_t.shape), n_pos))
+        if exclude not in (None, "self", "reverse"):
+            raise ValueError("link_block_sample: exclude must be None, 'self' or 'reverse' (got {!r})".format(exclude))
+        n_begin = 2 * pair_t.shape[1]                 # hop 0's capacity: every endpoint
     dev = rowptr.device
     n_rows, N, L = rowptr.numel() - 1, node_map.numel(), len(fanouts)
     ks = [-1 if k is None else int(k) for k in fanouts]
-    # a list holds each id once, plus the repeated or invalid seeds of a batch that will be refused
-    limit = N + seeds.numel()
-    cap_nodes = seeds.numel()
+    # a list holds each id once, plus the repeated or invalid seeds of a batch that will be refused (a pair list holds
+    # its distinct valid endpoints only)
+    limit = N + (n_begin if pairs is None else 0)
+    cap_nodes = n_begin
     for k in fanouts:
         cap_nodes = block_capacities(cap_nodes, k, limit)[1]
         if cap_nodes is None:
@@ -1172,15 +1253,35 @@ def _block_sample(rowptr, col, w_csr, seeds, fanouts, keys, node_map, padding, r
     ws_entry = ("tfgk_block_sample_mapped_workspace_bytes",) if mapped else ()
     fill = "tfgk_block_sample_fill_mapped" if mapped else "tfgk_block_sample_fill"
     st = _stream(rowptr)
-    _ffi.call("tfgk_block_sample_begin", _p(seeds), seeds.numel(), N, _p(nodes), _p(node_map), _p(state), L, st)
+    local = excluded = None
+    if pairs is None:
+        _ffi.call("tfgk_block_sample_begin", _p(seeds), seeds.numel(), N, _p(nodes), _p(node_map), _p(state), L, st)
     try:
-        cap_list, hops = seeds.numel(), []
+        excl_args = ()
+        if pairs is not None:
+            P = pair_t.shape[1]
+            local = torch.empty((2, P), dtype=torch.int32, device=dev)
+            need = ctypes.c_size_t()
+            _ffi.call("tfgk_block_pairs_workspace_bytes", P, ctypes.byref(need))
+            ws = torch.empty((max(need.value, 1),), dtype=torch.uint8, device=dev)
+            _ffi.call("tfgk_block_sample_begin_pairs", _p(pair_t[0]), _p(pair_t[1]), P, N, _p(nodes), _p(node_map),
+                      _p(state), L, _p(local), _p(ws), need.value, st)
+        if pairs is not None and exclude is not None:
+            excl_off, excl_pos = _exclusion_lists(rowptr, col, nodes, n_begin, local, pair_t, n_pos, exclude, mapped)
+            excluded = (excl_off, n_begin)
+            excl_args = (_p(excl_off), _p(excl_pos), n_begin)
+            fill += "_excl"
+        cap_list, hops = n_begin, []
         for h, k in enumerate(ks):
             cap_edges, cap_next = block_capacities(cap_list, fanouts[h], limit)
             ws, nbytes = _block_workspace(cap_list, 0 if cap_edges is None else cap_edges, dev, *ws_entry)
             out_rowptr = torch.empty((cap_list + 1,), dtype=torch.int64, device=dev)
-            _ffi.call("tfgk_block_sample_count", _p(rowptr), n_rows, _p(nodes), _p(state), h, L, cap_list, k, padding,
-                      _p(out_rowptr), _p(ws), nbytes, st)
+            if excl_args:
+                _ffi.call("tfgk_block_sample_count_excl", _p(rowptr), n_rows, _p(nodes), _p(state), h, L, cap_list, k,
+                          padding, excl_args[0], excl_args[2], _p(out_rowptr), _p(ws), nbytes, st)
+            else:
+                _ffi.call("tfgk_block_sample_count", _p(rowptr), n_rows, _p(nodes), _p(state), h, L, cap_list, k,
+                          padding, _p(out_rowptr), _p(ws), nbytes, st)
             if cap_edges is None:
                 n_list, total = ctypes.c_int32(), ctypes.c_int64()
                 _ffi.call("tfgk_block_sample_read_total", _p(state), h, _p(out_rowptr), cap_list, ctypes.byref(n_list),
@@ -1191,7 +1292,7 @@ def _block_sample(rowptr, col, w_csr, seeds, fanouts, keys, node_map, padding, r
             out_w = torch.empty((max(cap_edges, 1),), dtype=torch.float32, device=dev)
             _ffi.call(fill, _p(rowptr), n_rows, col, w_csr, N, _p(nodes), _p(node_map),
                       _p(state), h, L, cap_list, cap_edges, k, padding, int(keys[h]), int(rng_stream), _p(out_rowptr),
-                      _p(out[0]), _p(out[1]), _p(out[2]), _p(out_w), _p(ws), nbytes, st)
+                      _p(out[0]), _p(out[1]), _p(out[2]), _p(out_w), *excl_args, _p(ws), nbytes, st)
             hops.append((out_rowptr, out[0], out[1], out[2], out_w))
             cap_list = cap_next
         host = (ctypes.c_int32 * (4 + 2 * L))()
@@ -1201,7 +1302,9 @@ def _block_sample(rowptr, col, w_csr, seeds, fanouts, keys, node_map, padding, r
         raise
     sizes = [int(v) for v in host[3:4 + L]]
     edges = [int(v) for v in host[4 + L:4 + 2 * L]]
-    hops = [(rp, row[:S], local[:S], gcol[:S], w[:S]) for (rp, row, local, gcol, w), S in zip(hops, edges)]
+    hops = [(rp, row[:S], loc[:S], gcol[:S], w[:S]) for (rp, row, loc, gcol, w), S in zip(hops, edges)]
+    if pairs is not None:
+        return nodes[:sizes[-1]], sizes, hops, int(host[0]), local, excluded
     return nodes[:sizes[-1]], sizes, hops, int(host[0]), int(host[1])
 
 
@@ -1221,12 +1324,14 @@ def block_self_loops(rowptr, edge_index, n_dst):
     return out_rowptr, out
 
 
-def block_gcn_values(rowptr, gcol, w, dst, g_rowptr, g_rowsum, norm, loop, deg_fill, fill):
+def block_gcn_values(rowptr, gcol, w, dst, g_rowptr, g_rowsum, norm, loop, deg_fill, fill, excluded=None):
     """GCN's normalised values on a sampled block (tfgk_block_gcn_values_f32): the block's rowptr int64 [>= n_dst + 1],
     global columns int32 [S] and weights float32 [S] (or None: ones), its output rows' global ids dst int32 [n_dst], and
     the full graph's rowptr int64 and sequential row sums float32, indexed by global id.  norm: GCN_NORM_*; loop:
     GCN_LOOP_*; deg_fill is added to every row sum, fill is the self loops' weight.  Returns float32 [S + n_dst] in
-    block_self_loops' layout with a loop mode, else [S] in the block's order; one launch, no synchronisation."""
+    block_self_loops' layout with a loop mode, else [S] in the block's order; one launch, no synchronisation.
+    excluded: (excl_off int64, n_excl) of a link batch's block (tfgk_block_gcn_values_excl_f32): output row r < n_excl
+    had excl_off[r + 1] - excl_off[r] of its full-graph entries excluded, which its scale leaves out."""
     _check(rowptr, torch.int64, "rowptr")
     _check(gcol, torch.int32, "gcol")
     _check(dst, torch.int32, "dst")
@@ -1240,8 +1345,17 @@ def block_gcn_values(rowptr, gcol, w, dst, g_rowptr, g_rowsum, norm, loop, deg_f
     if rowptr.numel() < n_dst + 1:
         raise ValueError("block_gcn_values: rowptr has {} entries for {} rows".format(rowptr.numel(), n_dst))
     out = torch.empty((S + (n_dst if loop != GCN_LOOP_NONE else 0),), dtype=torch.float32, device=rowptr.device)
-    _ffi.call("tfgk_block_gcn_values_f32", _p(rowptr), _p(gcol), _p(w), S, _p(dst), n_dst, _p(g_rowptr), _p(g_rowsum),
-              int(norm), int(loop), float(deg_fill), float(fill), _p(out), _stream(rowptr))
+    if excluded is None:
+        _ffi.call("tfgk_block_gcn_values_f32", _p(rowptr), _p(gcol), _p(w), S, _p(dst), n_dst, _p(g_rowptr),
+                  _p(g_rowsum), int(norm), int(loop), float(deg_fill), float(fill), _p(out), _stream(rowptr))
+        return out
+    excl_off, n_excl = excluded
+    _check(excl_off, torch.int64, "excl_off")
+    if excl_off.numel() < int(n_excl) + 1:
+        raise ValueError("block_gcn_values: {} exclusion offsets for {} rows".format(excl_off.numel(), n_excl))
+    _ffi.call("tfgk_block_gcn_values_excl_f32", _p(rowptr), _p(gcol), _p(w), S, _p(dst), n_dst, _p(g_rowptr),
+              _p(g_rowsum), int(norm), int(loop), float(deg_fill), float(fill), _p(excl_off), int(n_excl), _p(out),
+              _stream(rowptr))
     return out
 
 

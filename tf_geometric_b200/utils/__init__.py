@@ -7,4 +7,5 @@ from .graph_utils import (add_self_loop_edge, remove_self_loop_edge, convert_edg
                           convert_dense_assign_to_edge, convert_x_to_3d, reindex_sampled_edge_index,
                           compute_edge_mask_by_node_index, extract_unique_edge)
 from .sampling import (RandomNeighborSampler, UniformNeighborSampler, SampledNeighborhood, SampledBlocks, Block,
-                       SelfLoopBlock, GcnBlock, SourceRows, HostFeatureTable, rank_source_rows, HostNeighborSampler)
+                       SelfLoopBlock, GcnBlock, SourceRows, HostFeatureTable, rank_source_rows, HostNeighborSampler,
+                       LinkBlocks)

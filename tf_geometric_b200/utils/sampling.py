@@ -13,7 +13,8 @@ the work follows the batch, not the graph.
 RandomNeighborSampler.sample_blocks (also an extension) samples the same neighbourhood as layer-wise bipartite blocks:
 block i maps the hop_sizes[L - i] nodes of its input onto the hop_sizes[L - 1 - i] nodes the next layer reads, so every
 layer computes only the rows it must.  The sizes stay on the device until the batch ends, which costs one host
-synchronisation per batch.
+synchronisation per batch.  sample_link_blocks seeds such a batch with the endpoints of target pairs and their
+negatives (LinkBlocks), optionally with the targets excluded from the neighbourhoods their endpoints aggregate.
 
 HostFeatureTable keeps an [N, F] float32 feature table in host memory (page-locked in place) and gathers the rows a batch
 reads over the host link (tfgk_gather_rows_mapped_f32), so the table need not fit on the device.  With device_rows it
@@ -110,18 +111,20 @@ class Block(ops.SampledInput):
     fanout: the fan-out of the hop that drew the block (None: every neighbour, or a block built by hand).
     dst_ids: int32 [num_dst], the node id of every output row (a view of the batch's node_index; None for a block built
     by hand).  degrees: the sampler's full-graph degrees for with_gcn_norm(), a callable returning (rowptr int64, row
-    sums float32), both indexed by node id (None for a block built by hand).
+    sums float32), both indexed by node id (None for a block built by hand).  excluded: for a block of a link batch that
+    excluded its target edges, (excl_off int64, n_excl): output row r < n_excl lost excl_off[r + 1] - excl_off[r] of its
+    full-graph entries, which with_gcn_norm() leaves out of its scale (None otherwise, and for a block built by hand).
     The transposed CSR that the backward needs is built on first use and kept on the block."""
 
     __slots__ = ("num_src", "num_dst", "edge_index", "edge_weight", "global_col", "csr", "fanout", "dst_ids", "degrees",
-                 "_csr_t", "_w_t", "_looped", "_gcn")
+                 "excluded", "_csr_t", "_w_t", "_looped", "_gcn")
 
     def __init__(self, num_src, num_dst, edge_index, edge_weight, global_col, csr, fanout=None, dst_ids=None,
-                 degrees=None):
+                 degrees=None, excluded=None):
         self.num_src, self.num_dst = int(num_src), int(num_dst)
         self.edge_index, self.edge_weight, self.global_col, self.csr = edge_index, edge_weight, global_col, csr
         self.fanout = None if fanout is None else int(fanout)
-        self.dst_ids, self.degrees = dst_ids, degrees
+        self.dst_ids, self.degrees, self.excluded = dst_ids, degrees, excluded
         self._csr_t, self._w_t, self._looped, self._gcn = None, {}, None, None
 
     def with_self_loops(self):
@@ -235,7 +238,9 @@ class GcnBlock(ops.SampledInput):
     its degree in the sampler's full graph, and the sampled edges of output row r (global id g, k_r sampled of n_g) are
     scaled by s_r = n_g / k_r, so that each aggregate is an unbiased estimate of the full graph's row.  With every
     neighbour (fan-out None) s_r = 1 and the values are the full graph's gcn_norm_adj values for the same rows, bit for
-    bit.  tfg.nn.gcn and tfg.layers.GCN take it in place of the adjacency; every other operator refuses it.
+    bit.  In a link batch that excluded x_r of row r's entries, s_r = (n_g - x_r) / k_r: the degrees stay the full
+    graph's, and the aggregate estimates the full graph's row without the excluded terms (with fan-out None, exactly
+    those values).  tfg.nn.gcn and tfg.layers.GCN take it in place of the adjacency; every other operator refuses it.
 
     normalized(norm, add_self_loop, sym, renorm, improved) gives the rectangular [num_dst, num_src] SparseMatrix of one
     configuration, made on first use (one launch of tfgk_block_gcn_values_f32) and kept.  With self loops its structure is
@@ -266,8 +271,10 @@ class GcnBlock(ops.SampledInput):
         else:
             looped = blk.with_self_loops()
             index, csr, transposed = looped.edge_index, looped.csr, looped.transposed
-        value = ops.block_gcn_values(blk.csr.rowptr, blk.global_col, blk.edge_weight, blk.dst_ids, g_rowptr, g_rowsum,
-                                     norm, loop, deg_fill, fill)
+        args = (blk.csr.rowptr, blk.global_col, blk.edge_weight, blk.dst_ids, g_rowptr, g_rowsum, norm, loop, deg_fill,
+                fill)
+        value = ops.block_gcn_values(*args) if blk.excluded is None else \
+            ops.block_gcn_values(*args, excluded=blk.excluded)
         return _BlockAdjacency(index, value, [self.num_dst, self.num_src], csr, transposed)
 
 
@@ -561,6 +568,38 @@ def rank_source_rows(batches):
     return order[:read], counts
 
 
+_LINK_DOC = """Link-prediction mini-batch on blocks (an extension of the reference API, as DGL's edge data loaders and
+        PyG's LinkNeighborLoader): the target pairs `edge_index` and their negatives are scored on the final embeddings
+        of their endpoints, whose neighbourhoods are sampled as sample_blocks samples a seed list.
+
+        Seeds: the distinct endpoints of the positive pairs, then of the negative pairs, pair by pair (source, then
+        destination) in first-occurrence order; node_index[:hop_sizes[0]] is that list.  With exclude=None the batch is
+        sample_blocks(that list, fanouts, padding, seed), bit for bit.
+        Negatives: with num_negatives = q, negative pair b * q + j is (u_b, t), u_b the source of positive b and t drawn
+        uniformly from all nodes (random_below(seed, RNG_STREAM_LINK, b * q + j, N), tail corruption).  A negative may
+        coincide with a true edge; for exact non-edges pass negative_edge_index (for example from
+        negative_sampling_with_start_node) with num_negatives=0.  Both at once: ValueError.
+        Exclusion: "self" removes every CSR entry (u, v) of every positive pair (u, v) from u's row (duplicates
+        included), at every hop and before any draw; "reverse" also removes (v, u).  Negatives are never excluded, and a
+        pair that is not an edge excludes nothing.  The batch equals sample_blocks on a sampler built over the edge list
+        with those entries deleted (same order, weights following), for every fan-out rule; with_gcn_norm() keeps the
+        full graph's degrees and rescales by the kept entries.
+        Synchronisation: one host read-back per batch, one more for the exclusion lists' total, and one per hop of
+        fan-out None.  Calls on one sampler must be ordered on one CUDA stream.
+
+        :param edge_index: int [2, B] target pairs (numpy, list or tensor)
+        :param fanouts: as sample_blocks
+        :param num_negatives: negatives drawn per positive pair
+        :param negative_edge_index: int [2, M] negative pairs to use instead
+        :param exclude: None, "self" or "reverse"
+        :return: LinkBlocks, on the device.  Ids outside [0, N) raise ValueError after the batch's read-back."""
+
+
+def _with_link_doc(fn):
+    fn.__doc__ = _LINK_DOC
+    return fn
+
+
 class RandomNeighborSampler(_SamplerBase):
     """Per-node fan-out sampling (graph_utils.py:630-776)."""
 
@@ -685,21 +724,25 @@ class RandomNeighborSampler(_SamplerBase):
             rowptr, csr.col, w_csr, nodes, hop_fanouts, keys, node_map, padding=padding),
             rowptr.device, node_map.numel(), seed_node_index, fanouts, seed, self._gcn_degrees)
 
+    @_with_link_doc
+    def sample_link_blocks(self, edge_index, fanouts, num_negatives=1, negative_edge_index=None, exclude=None,
+                           padding=False, seed=None):
+        csr, w_csr, rowptr, node_map = self._neighborhood_structure()
+        return _sample_link_blocks(lambda pairs, n_pos, hop_fanouts, keys, exclude: ops.link_block_sample(
+            rowptr, csr.col, w_csr, pairs, n_pos, hop_fanouts, keys, node_map, exclude=exclude, padding=padding),
+            rowptr.device, node_map.numel(), edge_index, fanouts, num_negatives, negative_edge_index, exclude, padding,
+            seed, self._gcn_degrees)
 
-def _sample_blocks(block_sample, dev, num_nodes, seed_node_index, fanouts, seed, degrees):
-    """sample_blocks of both samplers around their block sampler: block_sample(seeds int32, per-hop fan-outs in hop order,
-    hop keys) returns ops.block_sample's (nodes, hop_sizes, hops, n_bad, n_dup); this refuses bad seeds and assembles
-    the SampledBlocks.  degrees: the sampler's (rowptr, row sums) handle that every Block keeps for with_gcn_norm()."""
+
+def _hop_keys(fanouts, seed):
+    """(per-hop fan-outs in hop order, hop keys) of a batch with the resolved key `seed`."""
     from .graph_utils import _batch_seed         # graph_utils imports this module
-    seed = _rng.resolve_host(seed)
-    nodes = ops.as_device(seed_node_index, torch.int32, device=dev).reshape(-1).contiguous()
     hop_fanouts = [None if k is None else int(k) for k in reversed(list(fanouts))]
-    keys = [_batch_seed(seed, h) for h in range(len(hop_fanouts))]
-    node_index, sizes, hops, n_bad, n_dup = block_sample(nodes, hop_fanouts, keys)
-    if n_bad:
-        raise ValueError("seed_node_index holds node ids outside [0, {})".format(num_nodes))
-    if n_dup:
-        raise ValueError("seed_node_index holds {} duplicate node ids".format(n_dup))
+    return hop_fanouts, [_batch_seed(seed, h) for h in range(len(hop_fanouts))]
+
+
+def _blocks_of(dev, node_index, sizes, hops, hop_fanouts, degrees, excluded=None):
+    """The Blocks of a batch, layer 0 first, from the block sampler's hops."""
     blocks = []
     for h, (k, (out_rowptr, row, local, gcol, w)) in enumerate(zip(hop_fanouts, hops)):
         n_dst, n_src = sizes[h], sizes[h + 1]
@@ -708,8 +751,102 @@ def _sample_blocks(block_sample, dev, num_nodes, seed_node_index, fanouts, seed,
         if _plan_for_fanout(k):
             block_csr.plan = ops.build_plan(block_csr)
         blocks.append(Block(n_src, n_dst, torch.stack([row, local]), w, gcol, block_csr, fanout=k,
-                            dst_ids=node_index[:n_dst], degrees=degrees))
-    return SampledBlocks(node_index, sizes, blocks[::-1], num_nodes=num_nodes)
+                            dst_ids=node_index[:n_dst], degrees=degrees, excluded=excluded))
+    return blocks[::-1]
+
+
+def _sample_blocks(block_sample, dev, num_nodes, seed_node_index, fanouts, seed, degrees):
+    """sample_blocks of both samplers around their block sampler: block_sample(seeds int32, per-hop fan-outs in hop order,
+    hop keys) returns ops.block_sample's (nodes, hop_sizes, hops, n_bad, n_dup); this refuses bad seeds and assembles
+    the SampledBlocks.  degrees: the sampler's (rowptr, row sums) handle that every Block keeps for with_gcn_norm()."""
+    seed = _rng.resolve_host(seed)
+    nodes = ops.as_device(seed_node_index, torch.int32, device=dev).reshape(-1).contiguous()
+    hop_fanouts, keys = _hop_keys(fanouts, seed)
+    node_index, sizes, hops, n_bad, n_dup = block_sample(nodes, hop_fanouts, keys)
+    if n_bad:
+        raise ValueError("seed_node_index holds node ids outside [0, {})".format(num_nodes))
+    if n_dup:
+        raise ValueError("seed_node_index holds {} duplicate node ids".format(n_dup))
+    return SampledBlocks(node_index, sizes, _blocks_of(dev, node_index, sizes, hops, hop_fanouts, degrees),
+                         num_nodes=num_nodes)
+
+
+class LinkBlocks(SampledBlocks):
+    """A link-prediction mini-batch as layer-wise blocks (sample_link_blocks of RandomNeighborSampler and
+    HostNeighborSampler): a SampledBlocks seeded by the distinct endpoints of its pairs, so source_rows and
+    rank_source_rows take it as they take any batch.
+
+    pos_index: int32 [2, B], the target pairs relabelled to positions in node_index (all < hop_sizes[0]).
+    neg_index: int32 [2, M], the negative pairs, relabelled the same way.
+    predict_edge(h) scores both on the seeds' final embeddings."""
+
+    __slots__ = ("pos_index", "neg_index", "_pairs", "_half_csr")
+
+    def __init__(self, node_index, hop_sizes, blocks, num_nodes, pairs, num_pos):
+        super().__init__(node_index, hop_sizes, blocks, num_nodes=num_nodes)
+        self._pairs = pairs
+        self.pos_index, self.neg_index = pairs[:, :num_pos], pairs[:, num_pos:]
+        self._half_csr = None
+
+    def predict_edge(self, h):
+        """(pos_logits [B], neg_logits [M]): <h[u], h[v]> for every positive and negative pair (u, v), from one EdgeDot
+        over [pos || neg]; h: [hop_sizes[0], D], the last layer's output.  Differentiable in h, with the deterministic
+        backward of tfg.nn.predict_edge; its half-edge CSR is built without an id check (the local ids are in range by
+        construction) and kept on the batch.  No host synchronisation."""
+        from .. import autograd
+        n = self.hop_sizes[0]
+        if h.dim() != 2 or h.shape[0] != n:
+            raise ValueError("predict_edge takes the seeds' embeddings, [{}, D] (got {})".format(n, tuple(h.shape)))
+        if self._half_csr is None and h.requires_grad and torch.is_grad_enabled():
+            self._half_csr = autograd._half_edge_csr(self._pairs, n, ids_in_range=True)
+        logits = autograd.EdgeDot.apply(h, self._pairs)
+        B = self.pos_index.shape[1]
+        return logits[:B], logits[B:]
+
+
+def _pair_tensor(pairs, dev, what):
+    """`pairs` as an int32 [2, P] device tensor: ValueError for another shape, TypeError for non-integer ids."""
+    t = ops.as_device(pairs, device=dev)
+    if t.dim() != 2 or t.shape[0] != 2:
+        raise ValueError("{} must have shape [2, B] (got {})".format(what, tuple(t.shape)))
+    if t.dtype.is_floating_point or t.dtype.is_complex or t.dtype == torch.bool:
+        raise TypeError("{} takes integer node ids (got {})".format(what, t.dtype))
+    return t
+
+
+def _sample_link_blocks(link_block_sample, dev, num_nodes, edge_index, fanouts, num_negatives, negative_edge_index,
+                        exclude, padding, seed, degrees):
+    """sample_link_blocks of both samplers around their link block sampler: link_block_sample(pairs int32 [2, P], n_pos,
+    per-hop fan-outs, hop keys, exclude) returns ops.link_block_sample's outputs.  This checks the arguments, writes the
+    pairs (positives, then negatives), refuses endpoints outside the graph and assembles the LinkBlocks."""
+    pos = _pair_tensor(edge_index, dev, "edge_index")
+    if isinstance(num_negatives, bool) or not isinstance(num_negatives, (int, np.integer)) or num_negatives < 0:
+        raise ValueError("num_negatives must be an integer >= 0 (got {!r})".format(num_negatives))
+    q = int(num_negatives)
+    if negative_edge_index is not None and q > 0:
+        raise ValueError("pass either num_negatives > 0 (negatives drawn here) or negative_edge_index, not both; "
+                         "with negative_edge_index set num_negatives=0")
+    if exclude not in (None, "self", "reverse"):
+        raise ValueError("exclude must be None, 'self' or 'reverse' (got {!r})".format(exclude))
+    neg = None if negative_edge_index is None else _pair_tensor(negative_edge_index, dev, "negative_edge_index")
+    ops._check_block_fanouts(list(fanouts), padding)
+    B = pos.shape[1]
+    M = B * q if neg is None else neg.shape[1]
+    if num_nodes == 0 and B + M:
+        raise ValueError("the pairs hold node ids outside [0, 0): the graph has no nodes")
+    seed = _rng.resolve_host(seed)
+    hop_fanouts, keys = _hop_keys(fanouts, seed)
+    pairs = torch.empty((2, B + M), dtype=torch.int32, device=dev)
+    pairs[:, :B].copy_(pos)
+    if neg is not None:
+        pairs[:, B:].copy_(neg)
+    elif M:
+        ops.link_tail_negatives(pairs[0, :B], q, num_nodes, seed, pairs[0, B:], pairs[1, B:])
+    node_index, sizes, hops, n_bad, local, excluded = link_block_sample(pairs, B, hop_fanouts, keys, exclude)
+    if n_bad:
+        raise ValueError("the pairs hold {} node ids outside [0, {})".format(n_bad, num_nodes))
+    blocks = _blocks_of(dev, node_index, sizes, hops, hop_fanouts, degrees, excluded)
+    return LinkBlocks(node_index, sizes, blocks, num_nodes, local, B)
 
 
 class UniformNeighborSampler(_SamplerBase):
@@ -946,6 +1083,15 @@ class HostNeighborSampler(object):
         return _sample_blocks(lambda nodes, hop_fanouts, keys: ops.block_sample_mapped(
             self.rowptr, self._col_ptr, self._w_ptr, nodes, hop_fanouts, keys, self._node_map, padding=padding),
             self._device, self.num_nodes, seed_node_index, fanouts, seed, self._degrees)
+
+    @_with_link_doc
+    def sample_link_blocks(self, edge_index, fanouts, num_negatives=1, negative_edge_index=None, exclude=None,
+                           padding=False, seed=None):
+        self._check_open()
+        return _sample_link_blocks(lambda pairs, n_pos, hop_fanouts, keys, exclude: ops.link_block_sample_mapped(
+            self.rowptr, self._col_ptr, self._w_ptr, pairs, n_pos, hop_fanouts, keys, self._node_map, exclude=exclude,
+            padding=padding), self._device, self.num_nodes, edge_index, fanouts, num_negatives, negative_edge_index,
+            exclude, padding, seed, self._degrees)
 
     def close(self):
         """Release the host CSR's registrations (after the device's pending work) and the arrays.  Idempotent."""
