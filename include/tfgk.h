@@ -654,6 +654,24 @@ int tfgk_block_sample_fill_mapped(const int64_t *rowptr, int32_t n_rows, const i
 int tfgk_block_self_loops_i32(const int64_t *rowptr, const int32_t *row, const int32_t *col, int64_t S, int32_t n_dst,
                               int64_t *out_rowptr, int32_t *out_row, int32_t *out_col, void *stream);
 
+/* A row block (layer-wise inference, utils.RandomNeighborSampler.row_block / HostNeighborSampler.row_block): the block
+ * sampler's batch for the seeds r0, ..., r1 - 1 and one hop of fan-out None, bit for bit, from the range's columns.
+ * rowptr int64 [N + 1] (device) is the graph's CSR row pointer; cols int32 [S] (device) its columns
+ * [rowptr[r0], rowptr[r1]), staged by the caller, S = rowptr[r1] - rowptr[r0] < 2^31.  map is the int32 [N] relabelling
+ * map of tfgk_frontier_i32 (-1 everywhere before and after).  Writes, with n = r1 - r0:
+ *   nodes [n + S at most]: nodes[i] = r0 + i, then the columns outside the range in first-occurrence order;
+ *   out_rowptr int64 [n + 1] = rowptr[r0 .. r1] - rowptr[r0];  out_row [S]: each edge's output row;
+ *   out_local [S]: each column's position in nodes;  *num_src_host: the length of nodes.
+ * The range's ids are distinct and in range by construction, so the seeds get no duplicate or bad-id pass; the columns
+ * are relabelled by tfgk_frontier_i32's kernels and scan.  Workspace: tfgk_relabel_workspace_bytes(S).  One host read-back
+ * (the list length) when S > 0, none when S == 0.  A column id outside [0, N) fails with TFGK_ERR_INDEX_OUT_OF_RANGE. */
+int tfgk_row_block_i32(const int64_t *rowptr, int32_t N, int32_t r0, int32_t r1, const int32_t *cols, int64_t S,
+                       int32_t *nodes, int32_t *map, int64_t *out_rowptr, int32_t *out_row, int32_t *out_local,
+                       int32_t *num_src_host, void *workspace, size_t workspace_bytes, void *stream);
+/* cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDefault, stream): asynchronous between device memory and page-locked host
+ * memory (tfgk_host_register's ranges, or pinned allocations), whatever a framework knows of the host buffer. */
+int tfgk_copy_async(void *dst, const void *src, size_t bytes, void *stream);
+
 /* GCN's normalised values on a sampled block (utils.GcnBlock): every row normalised with its FULL-graph degree, and each
  * output row's sampled edges rescaled so that their sum is an unbiased estimate of the full graph's row.
  * The block: rowptr int64 [n_dst + 1] (rowptr[0] = 0, rowptr[n_dst] = S), gcol int32 [S] (the global id of every edge's

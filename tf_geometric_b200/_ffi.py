@@ -167,6 +167,9 @@ SIGNATURES = {
                                            _ptr],
     "tfgk_block_gcn_values_excl_f32": [_ptr, _ptr, _ptr, _i64, _ptr, _i32, _ptr, _ptr, _int, _int, _f32, _f32, _ptr, _i32,
                                        _ptr, _ptr],
+    "tfgk_row_block_i32": [_ptr, _i32, _i32, _i32, _ptr, _i64, _ptr, _ptr, _ptr, _ptr, _ptr, ctypes.POINTER(_i32), _ptr,
+                           _size, _ptr],
+    "tfgk_copy_async": [_ptr, _ptr, _size, _ptr],
     "tfgk_edge_dot_f32": [_ptr, _i64, _i32, _ptr, _ptr, _i64, _i32, _ptr, _ptr],
     "tfgk_neg_offsets_workspace_bytes": [_i32, ctypes.POINTER(_size)],
     "tfgk_neg_offsets": [_ptr, _i32, _int, _ptr, ctypes.POINTER(_i64), _ptr, _size, _ptr],
@@ -311,6 +314,7 @@ NOT_CAPTURABLE = {
     "tfgk_block_sample_fill_mapped_excl": ("the host-memory link block sampler", "it takes a host-side key"),
     "tfgk_link_tail_negatives_i32": ("the link block sampler's negatives", "it takes a host-side key"),
     "tfgk_block_exclusion_count": ("the link block sampler's exclusion lists", "it returns their total to the host"),
+    "tfgk_row_block_i32": ("the row blocks of layer-wise inference", "it returns the number of source rows to the host"),
     "tfgk_host_register": ("HostFeatureTable", "it page-locks host memory, which a graph cannot record"),
     "tfgk_mapped_id_range_i32": ("the CSR build of HostNeighborSampler", "it returns the id range to the host"),
     "tfgk_neg_offsets": ("negative sampling", "it returns the number of candidate pairs to the host"),

@@ -863,6 +863,37 @@ int tfgk_reindex_i32(const int32_t *nodes, int32_t n_nodes, const int32_t *ids, 
     return TFGK_OK;
 }
 
+}  // extern "C"
+
+// the frontier's relabelling once the list nodes[0, n_nodes) is in the map and the counters are cleared: the ids of
+// cols[0, S) not in the list are appended in first-occurrence order and local_col written; then the map is reset and
+// the three counters read back into c (one synchronisation).  ws / need: tfgk_relabel_workspace_bytes(S)'s layout.
+static int frontier_relabel(const int32_t *cols, int64_t S, int32_t N, int32_t *nodes, int32_t n_nodes, int32_t *map,
+                            int32_t *local_col, char *ws, size_t need, int32_t *c, cudaStream_t st) {
+    int32_t *flag = reinterpret_cast<int32_t *>(ws);
+    int32_t *off = reinterpret_cast<int32_t *>(ws + align_up((size_t)(S + 1) * 4));
+    int32_t *sums = reinterpret_cast<int32_t *>(ws + 2 * align_up((size_t)(S + 1) * 4));
+    int32_t *counters = reinterpret_cast<int32_t *>(ws + need - 256);
+    if (S) {
+        frontier_first_kernel<<<grid_for(S), 256, 0, st>>>(cols, S, N, map, counters);
+        TFGK_LAUNCH_CHECK();
+        frontier_flag_kernel<<<grid_for(S), 256, 0, st>>>(cols, S, N, map, flag);
+        TFGK_LAUNCH_CHECK();
+        int rc = exclusive_scan<int32_t, int32_t>(flag, S, S + 1, off, sums, st);
+        if (rc != TFGK_OK) return rc;
+        frontier_emit_kernel<<<grid_for(S), 256, 0, st>>>(cols, S, flag, off, n_nodes, nodes, map);
+        TFGK_LAUNCH_CHECK();
+        reindex_gather_kernel<<<grid_for(S), 256, 0, st>>>(cols, S, N, map, local_col);
+        TFGK_LAUNCH_CHECK();
+        TFGK_CUDA(cudaMemcpyAsync(counters + kNewIds, off + S, 4, cudaMemcpyDeviceToDevice, st));
+    }
+    node_reset_kernel<<<grid_for((int64_t)n_nodes + S), 256, 0, st>>>(nodes, n_nodes, S ? off + S : nullptr, N, map);
+    TFGK_LAUNCH_CHECK();
+    return read_counters(counters, c, st);
+}
+
+extern "C" {
+
 int tfgk_frontier_i32(const int32_t *cols, int64_t S, int32_t N, int32_t *nodes, int32_t n_nodes, int32_t *map,
                       int32_t *local_col, int32_t *n_new_host, int32_t *n_dup_host, void *workspace, size_t workspace_bytes,
                       void *stream) {
@@ -879,32 +910,14 @@ int tfgk_frontier_i32(const int32_t *cols, int64_t S, int32_t N, int32_t *nodes,
         return set_error(TFGK_ERR_WORKSPACE, "frontier: workspace too small (%zu < %zu bytes)", workspace_bytes, need);
     cudaStream_t st = as_stream(stream);
     char *ws = static_cast<char *>(workspace);
-    int32_t *flag = reinterpret_cast<int32_t *>(ws);
-    int32_t *off = reinterpret_cast<int32_t *>(ws + align_up((size_t)(S + 1) * 4));
-    int32_t *sums = reinterpret_cast<int32_t *>(ws + 2 * align_up((size_t)(S + 1) * 4));
     int32_t *counters = reinterpret_cast<int32_t *>(ws + need - 256);
     TFGK_CUDA(cudaMemsetAsync(counters, 0, 3 * 4, st));
     if (n_nodes) {
         node_scatter_kernel<<<grid_for(n_nodes), 256, 0, st>>>(nodes, n_nodes, N, map, counters);
         TFGK_LAUNCH_CHECK();
     }
-    if (S) {
-        frontier_first_kernel<<<grid_for(S), 256, 0, st>>>(cols, S, N, map, counters);
-        TFGK_LAUNCH_CHECK();
-        frontier_flag_kernel<<<grid_for(S), 256, 0, st>>>(cols, S, N, map, flag);
-        TFGK_LAUNCH_CHECK();
-        int rc = exclusive_scan<int32_t, int32_t>(flag, S, S + 1, off, sums, st);
-        if (rc != TFGK_OK) return rc;
-        frontier_emit_kernel<<<grid_for(S), 256, 0, st>>>(cols, S, flag, off, n_nodes, nodes, map);
-        TFGK_LAUNCH_CHECK();
-        reindex_gather_kernel<<<grid_for(S), 256, 0, st>>>(cols, S, N, map, local_col);
-        TFGK_LAUNCH_CHECK();
-        TFGK_CUDA(cudaMemcpyAsync(counters + kNewIds, off + S, 4, cudaMemcpyDeviceToDevice, st));
-    }
-    node_reset_kernel<<<grid_for((int64_t)n_nodes + S), 256, 0, st>>>(nodes, n_nodes, S ? off + S : nullptr, N, map);
-    TFGK_LAUNCH_CHECK();
     int32_t c[3];
-    int rc = read_counters(counters, c, st);
+    int rc = frontier_relabel(cols, S, N, nodes, n_nodes, map, local_col, ws, need, c, st);
     if (rc != TFGK_OK) return rc;
     if (c[kBadIds]) return set_error(TFGK_ERR_INDEX_OUT_OF_RANGE, "frontier: %d node ids outside [0, %d)", c[kBadIds], N);
     *n_dup_host = c[kDupIds];
@@ -1374,6 +1387,92 @@ int tfgk_block_exclusion_fill_mapped(const int64_t *rowptr, int32_t n_rows, cons
                                      void *workspace, size_t workspace_bytes, void *stream) {
     return block_exclusion_fill<int64_t>("block_exclusion_fill_mapped", rowptr, n_rows, col, nodes, cap, target_dst,
                                          excl_off, excl_pos, workspace, workspace_bytes, stream);
+}
+
+}  // extern "C"
+
+// ---- row blocks: every in-neighbour of a range of rows (layer-wise inference) --------------------------------------
+namespace tfgk {
+namespace {
+
+// items [0, n): output row i is node r0 + i, at position i of the list and of the map, with its rebased rowptr; item n:
+// the closing rowptr; items n + 1 + e: edge e's output row, the last row i with rowptr[r0 + i] <= rowptr[r0] + e (a
+// binary search, so that no thread walks a row and a hub's edges spread over as many threads as it has edges)
+__global__ void row_block_begin_kernel(const int64_t *__restrict__ rowptr, int32_t r0, int32_t n, int64_t S,
+                                       int32_t *__restrict__ nodes, int32_t *__restrict__ map,
+                                       int64_t *__restrict__ out_rowptr, int32_t *__restrict__ out_row) {
+    const int64_t *__restrict__ rp = rowptr + r0;
+    const int64_t e0 = rp[0];
+    const int64_t total = (int64_t)n + 1 + S;
+    for (int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; t < total; t += (int64_t)gridDim.x * blockDim.x) {
+        if (t <= n) {
+            out_rowptr[t] = rp[t] - e0;
+            if (t < n) {
+                nodes[t] = r0 + (int32_t)t;
+                map[r0 + t] = (int32_t)t;
+            }
+        } else {
+            const int64_t p = e0 + (t - n - 1);
+            int32_t lo = 0, hi = n - 1;
+            while (lo < hi) {
+                const int32_t mid = lo + (hi - lo + 1) / 2;
+                if (rp[mid] <= p) lo = mid;
+                else hi = mid - 1;
+            }
+            out_row[t - n - 1] = lo;
+        }
+    }
+}
+
+}  // namespace
+}  // namespace tfgk
+
+extern "C" {
+
+int tfgk_row_block_i32(const int64_t *rowptr, int32_t N, int32_t r0, int32_t r1, const int32_t *cols, int64_t S,
+                       int32_t *nodes, int32_t *map, int64_t *out_rowptr, int32_t *out_row, int32_t *out_local,
+                       int32_t *num_src_host, void *workspace, size_t workspace_bytes, void *stream) {
+    TFGK_CHECK_ARG(N >= 0 && r0 >= 0 && r0 <= r1 && r1 <= N, "row_block: bad range [%d, %d) of %d rows", r0, r1, N);
+    TFGK_CHECK_ARG(S >= 0 && S < (1ll << 31) - 1, "row_block: %lld edges; a row block takes fewer than 2^31 - 1",
+                   (long long)S);
+    TFGK_CHECK_ARG(S == 0 || r0 < r1, "row_block: %lld edges and no rows", (long long)S);
+    TFGK_CHECK_ARG(num_src_host != nullptr && rowptr != nullptr && out_rowptr != nullptr, "row_block: null pointer");
+    const int32_t n = r1 - r0;
+    *num_src_host = n;
+    TFGK_CHECK_ARG(n == 0 || (nodes && map), "row_block: null node list or map");
+    TFGK_CHECK_ARG(S == 0 || (cols && out_row && out_local), "row_block: null edge array");
+    size_t need = 0;
+    int rc = tfgk_relabel_workspace_bytes(S, &need);
+    if (rc != TFGK_OK) return rc;
+    if (workspace == nullptr || workspace_bytes < need)
+        return set_error(TFGK_ERR_WORKSPACE, "row_block: workspace too small (%zu < %zu bytes)", workspace_bytes, need);
+    cudaStream_t st = as_stream(stream);
+    char *ws = static_cast<char *>(workspace);
+    int32_t *counters = reinterpret_cast<int32_t *>(ws + need - 256);
+    row_block_begin_kernel<<<grid_for((int64_t)n + 1 + S), 256, 0, st>>>(rowptr, r0, n, S, nodes, map, out_rowptr,
+                                                                        out_row);
+    TFGK_LAUNCH_CHECK();
+    if (S == 0) {                       // no columns: the list is the range, and nothing is read back
+        if (n) {
+            node_reset_kernel<<<grid_for(n), 256, 0, st>>>(nodes, n, nullptr, N, map);
+            TFGK_LAUNCH_CHECK();
+        }
+        return TFGK_OK;
+    }
+    // the frontier's relabelling after the range's rows: columns outside the list appended in first-occurrence order
+    TFGK_CUDA(cudaMemsetAsync(counters, 0, 3 * 4, st));
+    int32_t c[3];
+    if ((rc = frontier_relabel(cols, S, N, nodes, n, map, out_local, ws, need, c, st)) != TFGK_OK) return rc;
+    if (c[kBadIds]) return set_error(TFGK_ERR_INDEX_OUT_OF_RANGE, "row_block: %d column ids outside [0, %d)", c[kBadIds], N);
+    *num_src_host = n + c[kNewIds];
+    return TFGK_OK;
+}
+
+int tfgk_copy_async(void *dst, const void *src, size_t bytes, void *stream) {
+    if (bytes == 0) return TFGK_OK;
+    TFGK_CHECK_ARG(dst != nullptr && src != nullptr, "copy_async: null pointer");
+    TFGK_CUDA(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDefault, as_stream(stream)));
+    return TFGK_OK;
 }
 
 }  // extern "C"

@@ -1324,6 +1324,48 @@ def block_self_loops(rowptr, edge_index, n_dst):
     return out_rowptr, out
 
 
+def row_block(rowptr, r0, r1, cols, node_map):
+    """The block sampler's one-hop batch for the seeds r0, ..., r1 - 1 with fan-out None (tfgk_row_block_i32), from the
+    range's columns: rowptr int64 [N + 1] of the graph's CSR on the device, cols int32 [S], the columns
+    [rowptr[r0], rowptr[r1]) staged on the device, node_map the sampler's int32 [N] map (-1 before and after).
+    Returns (nodes int32 [num_src], out_rowptr int64 [n + 1], out_row int32 [S], out_local int32 [S]) with n = r1 - r0.
+    One host read-back when S > 0."""
+    _check(rowptr, torch.int64, "rowptr")
+    _check(cols, torch.int32, "cols")
+    _check(node_map, torch.int32, "node_map")
+    N, S, n = node_map.numel(), cols.numel(), int(r1) - int(r0)
+    if rowptr.numel() != N + 1:
+        raise ValueError("row_block: rowptr has {} entries for {} nodes".format(rowptr.numel(), N))
+    if not 0 <= r0 <= r1 <= N:
+        raise ValueError("row_block: rows [{}, {}) are not a range of [0, {})".format(r0, r1, N))
+    dev = rowptr.device
+    nodes = torch.empty((max(min(N, n + S), 1),), dtype=torch.int32, device=dev)
+    out_rowptr = torch.empty((n + 1,), dtype=torch.int64, device=dev)
+    out_row = torch.empty((S,), dtype=torch.int32, device=dev)
+    out_local = torch.empty((S,), dtype=torch.int32, device=dev)
+    ws, nbytes = _relabel_workspace(S, dev)
+    num_src = ctypes.c_int32()
+    try:
+        _ffi.call("tfgk_row_block_i32", _p(rowptr), N, int(r0), int(r1), _p(cols), S, _p(nodes), _p(node_map),
+                  _p(out_rowptr), _p(out_row), _p(out_local), ctypes.byref(num_src), _p(ws), nbytes, _stream(rowptr))
+    except BaseException:
+        node_map.fill_(-1)            # the map is shared by every call on the sampler: leave it clean
+        raise
+    return nodes[:num_src.value], out_rowptr, out_row, out_local
+
+
+def copy_async(dst, src_address, nbytes):
+    """Copy nbytes from the address src_address (device memory, or page-locked host memory) into the CUDA tensor dst on
+    the current stream, asynchronously (tfgk_copy_async).  dst may also be a CPU tensor over page-locked memory, with a
+    device tensor's address as src_address."""
+    if not dst.is_contiguous() or dst.numel() * dst.element_size() < nbytes:
+        raise ValueError("copy_async: the destination holds {} contiguous bytes, {} needed".format(
+            dst.numel() * dst.element_size() if dst.is_contiguous() else 0, nbytes))
+    st = torch.cuda.current_stream().cuda_stream
+    _ffi.call("tfgk_copy_async", _p(dst) if nbytes else None, ctypes.c_void_p(src_address) if nbytes else None,
+              int(nbytes), ctypes.c_void_p(st))
+
+
 def block_gcn_values(rowptr, gcol, w, dst, g_rowptr, g_rowsum, norm, loop, deg_fill, fill, excluded=None):
     """GCN's normalised values on a sampled block (tfgk_block_gcn_values_f32): the block's rowptr int64 [>= n_dst + 1],
     global columns int32 [S] and weights float32 [S] (or None: ones), its output rows' global ids dst int32 [n_dst], and

@@ -8,4 +8,5 @@ from .graph_utils import (add_self_loop_edge, remove_self_loop_edge, convert_edg
                           compute_edge_mask_by_node_index, extract_unique_edge)
 from .sampling import (RandomNeighborSampler, UniformNeighborSampler, SampledNeighborhood, SampledBlocks, Block,
                        SelfLoopBlock, GcnBlock, SourceRows, HostFeatureTable, rank_source_rows, HostNeighborSampler,
-                       LinkBlocks)
+                       LinkBlocks, layerwise_chunk_bytes)
+from .layerwise import layerwise_inference

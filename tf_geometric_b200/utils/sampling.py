@@ -600,6 +600,46 @@ def _with_link_doc(fn):
     return fn
 
 
+_ROW_BLOCK_DOC = """Every in-neighbour of the rows r0, ..., r1 - 1 as a one-block batch (layer-wise inference, as DGL's
+        full-neighbour loaders and PyG's subgraph_loader): output rows are the nodes r0 .. r1 - 1 and hop_sizes is
+        [r1 - r0, num_src].  The batch is sample_blocks(torch.arange(r0, r1), [None]), bit for bit (node list, edges,
+        weights, CSR and work plan, degrees handle), so with_self_loops() and with_gcn_norm() apply unchanged.
+
+        The range is one contiguous slice of the CSR, so its columns (and weights) are taken whole: in place on
+        RandomNeighborSampler, by one asynchronous bulk copy per array from HostNeighborSampler's host CSR (an unweighted
+        graph's ones are made on the device).  tfgk_row_block_i32 then relabels them.  Synchronisation: one read-back
+        when the range has edges, plus the block's work plan.  Calls on one sampler must be ordered on one CUDA stream.
+
+        :param r0, r1: the rows, 0 <= r0 <= r1 <= N; ValueError otherwise, or for a range of 2^31 - 1 edges or more
+        :return: SampledBlocks with one Block, on the device"""
+
+
+def _row_range(rp, r0, r1):
+    """(r0, r1, e0, e1): the rows [r0, r1) of the host rowptr rp and their CSR positions [e0, e1); ValueError for rows
+    outside [0, N), r0 > r1, or a range of 2^31 - 1 edges or more (tfgk_row_block_i32's int32 positions)."""
+    N = rp.size - 1
+    if not all(isinstance(r, (int, np.integer)) and not isinstance(r, bool) for r in (r0, r1)):
+        raise TypeError("row_block takes integer rows (got {!r}, {!r})".format(r0, r1))
+    r0, r1 = int(r0), int(r1)
+    if r0 < 0 or r1 > N or r0 > r1:
+        raise ValueError("row_block takes rows 0 <= r0 <= r1 <= {} (got r0={}, r1={})".format(N, r0, r1))
+    e0, e1 = int(rp[r0]), int(rp[r1])
+    if e1 - e0 >= (1 << 31) - 1:
+        raise ValueError("rows [{}, {}) hold {} edges; a row block takes fewer than 2^31 - 1".format(r0, r1, e1 - e0))
+    return r0, r1, e0, e1
+
+
+def _row_block(sampler, r0, r1, staged=None):
+    """row_block of either sampler; staged = (cols, w) when the caller staged the range's arrays itself."""
+    r0, r1, e0, e1 = _row_range(sampler._host_rowptr(), r0, r1)
+    cols, w = sampler._stage(e0, e1) if staged is None else staged
+    rowptr, node_map, degrees = sampler._row_block_args()
+    nodes, out_rowptr, row, local = ops.row_block(rowptr, r0, r1, cols, node_map)
+    sizes = [r1 - r0, nodes.numel()]
+    blocks = _blocks_of(rowptr.device, nodes, sizes, [(out_rowptr, row, local, cols, w)], [None], degrees)
+    return SampledBlocks(nodes, sizes, blocks, num_nodes=node_map.numel())
+
+
 class RandomNeighborSampler(_SamplerBase):
     """Per-node fan-out sampling (graph_utils.py:630-776)."""
 
@@ -610,6 +650,7 @@ class RandomNeighborSampler(_SamplerBase):
         self._rowptr_all = None
         self._node_map = None
         self._rowsum = None
+        self._rowptr_host = None
 
     def _structure(self):
         if self._csr is None:
@@ -723,6 +764,26 @@ class RandomNeighborSampler(_SamplerBase):
         return _sample_blocks(lambda nodes, hop_fanouts, keys: ops.block_sample(
             rowptr, csr.col, w_csr, nodes, hop_fanouts, keys, node_map, padding=padding),
             rowptr.device, node_map.numel(), seed_node_index, fanouts, seed, self._gcn_degrees)
+
+    def row_block(self, r0, r1):
+        return _row_block(self, r0, r1)
+
+    row_block.__doc__ = _ROW_BLOCK_DOC
+
+    def _host_rowptr(self):
+        """The CSR's rowptr (one row per node id) as int64 numpy, read back once on first use."""
+        if self._rowptr_host is None:
+            self._rowptr_host = self._neighborhood_structure()[2].cpu().numpy()
+        return self._rowptr_host
+
+    def _stage(self, e0, e1):
+        """The columns and weights of CSR positions [e0, e1): slices of the device CSR, read in place."""
+        csr, w_csr, _, _ = self._neighborhood_structure()
+        return csr.col[e0:e1], w_csr[e0:e1]
+
+    def _row_block_args(self):
+        _, _, rowptr, node_map = self._neighborhood_structure()
+        return rowptr, node_map, self._gcn_degrees
 
     @_with_link_doc
     def sample_link_blocks(self, edge_index, fanouts, num_negatives=1, negative_edge_index=None, exclude=None,
@@ -875,6 +936,55 @@ HOST_CSR_EDGE_BYTES_UNWEIGHTED = 29
 HOST_CSR_ROW_BYTES = 12
 HOST_CSR_FIXED_BYTES = 1 << 20
 
+# Device bytes one chunk of layerwise_inference holds per edge and per output row of its range, as the code allocates
+# them.  Row block, per edge: the staged columns and weights of this range and of the next one, staged while this one is
+# computed (16); the relabelling's flags and offsets (8); the block's output rows and local columns (8), its edge_index
+# (8) and CSR perm (4); the node list (4); the work plan's hub slices (1).  Per row: the rebased rowptr (8), the node list
+# (4), the relabelling's map of row ids is the sampler's (0), the work plan's workspace (24) and task arrays, allocated at
+# capacity and then cloned (2 x 28).  With self loops (GAT, and GCN's block values) the looped edge_index and perm (12
+# per edge; per row one more edge, its rowptr and its own work plan: 12 + 8 + 80).  GCN's values: 4 per edge and per row.
+ROW_BLOCK_EDGE_BYTES = 49
+ROW_BLOCK_ROW_BYTES = 92
+LOOPED_EDGE_BYTES = 12
+LOOPED_ROW_BYTES = 100
+GCN_VALUE_BYTES = 4
+LAYERWISE_FIXED_BYTES = 16 << 20        # scan scratch, counters, per-call buffers and the allocator's rounding
+
+
+def layerwise_chunk_bytes(layer, in_width):
+    """(edge_bytes, row_bytes, out_width): the device bytes layerwise_inference counts per edge and per output row of a
+    chunk of `layer` over an input of in_width features, and the layer's output width.  Every edge counts as a possible
+    new source row, whose input row (in_width floats, gathered) and projections are held; every output row holds its own
+    source row, its aggregates and projections, and two output rows (the chunk's, and the previous chunk's until its copy
+    to host memory ends).  TypeError for a layer layerwise_inference does not take."""
+    from .. import layers as L           # layers import this module
+    F = int(in_width)
+    eb, rb = ROW_BLOCK_EDGE_BYTES, ROW_BLOCK_ROW_BYTES
+    if isinstance(layer, L.GCN):
+        D = layer.units if layer.use_kernel else F
+        src = F + D                                      # gathered row, its projection
+        eb, rb = eb + LOOPED_EDGE_BYTES + GCN_VALUE_BYTES, rb + LOOPED_ROW_BYTES + GCN_VALUE_BYTES
+        dst = src + D                                    # and its aggregate
+    elif isinstance(layer, L.GAT):
+        D = layer.units
+        V = layer.units * (1 if layer.split_value_heads else layer.num_heads)
+        src = F + 2 * layer.attention_units + V          # gathered row, query, key and value
+        eb, rb = eb + LOOPED_EDGE_BYTES, rb + LOOPED_ROW_BYTES
+        dst = src + V
+    elif isinstance(layer, (L.MeanGraphSage, L.SumGraphSage)):
+        D = layer.units
+        src = F                                          # gathered row (a device x is read in place)
+        dst = src + 2 * F + 2 * D                        # aggregate, self row, the two projections
+    elif isinstance(layer, (L.MeanPoolGraphSage, L.MaxPoolGraphSage)):
+        D = layer.units
+        k = layer.units // 2 if layer.concat else layer.units
+        src = F + 4 * k                                  # gathered row, its neighbour-MLP row
+        dst = src + 4 * k + 2 * D                        # reduced row, the two projections
+    else:
+        raise TypeError("layerwise_inference takes tfg.layers.GCN, GAT, MeanGraphSage, SumGraphSage, MeanPoolGraphSage "
+                        "and MaxPoolGraphSage layers (got {})".format(type(layer).__name__))
+    return eb + 4 * src, rb + 4 * (dst + 2 * D), D
+
 
 def _row_ranges(rowptr, budget, edge_bytes, row_bytes=HOST_CSR_ROW_BYTES):
     """Cut the rows of rowptr (int64 numpy [n + 1]) into consecutive ranges [r0, r1) of fewer than 2^31 edges whose
@@ -999,6 +1109,7 @@ class HostNeighborSampler(object):
         if E == 0:
             self.num_nodes, self.num_row_nodes = 0, 0
             self.rowptr = torch.zeros((1,), dtype=torch.int64, device=dev)
+            self._rp = np.zeros((1,), np.int64)
             self.rowsum = torch.zeros((0,), dtype=torch.float32, device=dev)
             self._col_ptr, self._w_ptr, self._ranges = 0, None, []
             self._col = self._w = None
@@ -1065,6 +1176,7 @@ class HostNeighborSampler(object):
             for key in edge_keys:
                 _host_release(key)
         self.rowptr, self.rowsum = rowptr, rowsum
+        self._rp = rp                   # the host copy: each row block's CSR positions, and the chunks cut from them
         self._ranges = ranges
         self._col, self._w = col, cw
         self._col_ptr, self._w_ptr = col_dev, w_dev
@@ -1092,6 +1204,33 @@ class HostNeighborSampler(object):
             self.rowptr, self._col_ptr, self._w_ptr, pairs, n_pos, hop_fanouts, keys, self._node_map, exclude=exclude,
             padding=padding), self._device, self.num_nodes, edge_index, fanouts, num_negatives, negative_edge_index,
             exclude, padding, seed, self._degrees)
+
+    def row_block(self, r0, r1):
+        self._check_open()
+        return _row_block(self, r0, r1)
+
+    row_block.__doc__ = _ROW_BLOCK_DOC
+
+    def _host_rowptr(self):
+        return self._rp
+
+    def _stage(self, e0, e1):
+        """The columns and weights of CSR positions [e0, e1) in new device buffers, copied from the page-locked host CSR
+        by one asynchronous bulk copy per array on the current stream (an unweighted graph's ones made on the device)."""
+        self._check_open()
+        S = e1 - e0
+        cols = torch.empty((S,), dtype=torch.int32, device=self._device)
+        if S:
+            ops.copy_async(cols, self._col.ctypes.data + 4 * e0, 4 * S)
+        if self._w is None:
+            return cols, torch.ones((S,), dtype=torch.float32, device=self._device)
+        w = torch.empty((S,), dtype=torch.float32, device=self._device)
+        if S:
+            ops.copy_async(w, self._w.ctypes.data + 4 * e0, 4 * S)
+        return cols, w
+
+    def _row_block_args(self):
+        return self.rowptr, self._node_map, self._degrees
 
     def close(self):
         """Release the host CSR's registrations (after the device's pending work) and the arrays.  Idempotent."""
