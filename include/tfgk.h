@@ -49,8 +49,9 @@ enum tfgk_bernoulli { TFGK_BERNOULLI_NONE = 0, TFGK_BERNOULLI_DROPOUT = 1, TFGK_
 enum tfgk_sample_padding { TFGK_SAMPLE_NO_PADDING = 0, TFGK_SAMPLE_PADDING = 1, TFGK_SAMPLE_HEAD = 2 };
 enum tfgk_gcn_norm { TFGK_GCN_NORM_BOTH = 0, TFGK_GCN_NORM_LEFT = 1, TFGK_GCN_NORM_RIGHT = 2 };
 enum tfgk_gcn_loop { TFGK_GCN_LOOP_NONE = 0, TFGK_GCN_LOOP_NORMED = 1, TFGK_GCN_LOOP_FILL = 2 };
-/* element type of a bf16-capable buffer; bf16 data is passed as its 16-bit patterns (uint16_t), fp8 data as bytes */
-enum tfgk_dtype { TFGK_DTYPE_F32 = 0, TFGK_DTYPE_BF16 = 1, TFGK_DTYPE_FP8_E4M3 = 2 };
+/* element type of a bf16-capable buffer; bf16 and fp16 data are passed as their 16-bit patterns (uint16_t), fp8 data as
+ * bytes.  TFGK_DTYPE_F16 (IEEE binary16) is taken only by the 16-bit host-table gathers. */
+enum tfgk_dtype { TFGK_DTYPE_F32 = 0, TFGK_DTYPE_BF16 = 1, TFGK_DTYPE_FP8_E4M3 = 2, TFGK_DTYPE_F16 = 3 };
 
 /* fp8 message rows (inference storage of the rows GCN and GAT gather along edges):
  *   element   OCP e4m3fn bytes (torch.float8_e4m3fn): max 448, no infinities, NaN = 0x7F / 0xFF;
@@ -165,6 +166,22 @@ int tfgk_gather_rows_mapped_f32(const float *table, int64_t ld, int64_t n_rows, 
 int tfgk_gather_rows_cached_f32(const float *table, int64_t ld, int64_t n_rows, int32_t F, const float *cache,
                                 int64_t ldc, const int32_t *slot, const int32_t *index, int64_t n, float *out,
                                 int64_t ldo, void *stream);
+/* The two gathers above from a 16-bit table: dtype is TFGK_DTYPE_BF16 or TFGK_DTYPE_F16, and ld, ldc and ldo count
+ * elements.  The rows are those of the float32 entries, each element widened to float32 exactly (bf16 by a 16-bit shift,
+ * fp16 by the hardware conversion), so out is the gather of the widened table bit for bit; an id outside [0, n_rows)
+ * writes a float32 NaN row and reads nothing.  The cache holds rows in the table's dtype.
+ * out_dtype (mapped entry): TFGK_DTYPE_F32, or the table's dtype to copy the 16-bit patterns unchanged (NaN payloads
+ * included; a bad id then writes the 16-bit NaN 0x7FC0 / 0x7E00), which fills a 16-bit device cache without a float32
+ * staging buffer.  Any other dtype or out_dtype: TFGK_ERR_INVALID_ARGUMENT.
+ * Loads carry 8, 4, 2 or 1 elements (16, 8, 4 or 2 bytes): the widest that F, the strides and the base pointers allow
+ * (F = 100 rows at 8-byte alignment take 8 bytes; F = 104 at 16-byte alignment take 16).  Asynchronous, no host
+ * synchronisation.  Bytes over the link: misses * F * 2. */
+int tfgk_gather_rows_mapped_16(const uint16_t *table, int32_t dtype, int64_t ld, int64_t n_rows, int32_t F,
+                               const int32_t *index, int64_t n, void *out, int32_t out_dtype, int64_t ldo,
+                               void *stream);
+int tfgk_gather_rows_cached_16(const uint16_t *table, int32_t dtype, int64_t ld, int64_t n_rows, int32_t F,
+                               const uint16_t *cache, int64_t ldc, const int32_t *slot, const int32_t *index,
+                               int64_t n, float *out, int64_t ldo, void *stream);
 
 /* ---- a CSR built from an edge list in host memory (utils.HostNeighborSampler) -----------------------------------------
  * row, col [E] int32 (and w [E] float32) are device-readable pointers to page-locked host memory (tfgk_host_register);

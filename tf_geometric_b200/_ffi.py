@@ -28,7 +28,7 @@ GCN_LOOP_NONE, GCN_LOOP_NORMED, GCN_LOOP_FILL = 0, 1, 2
 NEG_UPPER, NEG_START = 0, 1
 PAD_ROW_MAJOR, PAD_STEP_MAJOR = 0, 1
 SPGEMM_GRAD_LEFT, SPGEMM_GRAD_RIGHT = 0, 1
-DTYPE_F32, DTYPE_BF16, DTYPE_FP8_E4M3 = 0, 1, 2
+DTYPE_F32, DTYPE_BF16, DTYPE_FP8_E4M3, DTYPE_F16 = 0, 1, 2, 3
 
 _i32, _i64, _f32, _int = ctypes.c_int32, ctypes.c_int64, ctypes.c_float, ctypes.c_int
 _ptr, _size = ctypes.c_void_p, ctypes.c_size_t
@@ -58,6 +58,8 @@ SIGNATURES = {
     "tfgk_host_unregister": [_ptr],
     "tfgk_gather_rows_mapped_f32": [_ptr, _i64, _i64, _i32, _ptr, _i64, _ptr, _i64, _ptr],
     "tfgk_gather_rows_cached_f32": [_ptr, _i64, _i64, _i32, _ptr, _i64, _ptr, _ptr, _i64, _ptr, _i64, _ptr],
+    "tfgk_gather_rows_mapped_16": [_ptr, _i32, _i64, _i64, _i32, _ptr, _i64, _ptr, _i32, _i64, _ptr],
+    "tfgk_gather_rows_cached_16": [_ptr, _i32, _i64, _i64, _i32, _ptr, _i64, _ptr, _ptr, _i64, _ptr, _i64, _ptr],
     "tfgk_mapped_id_range_i32": [_ptr, _ptr, _i64, _ptr, _ptr, _size, _ptr],
     "tfgk_mapped_rowptr_workspace_bytes": [_i32, ctypes.POINTER(_size)],
     "tfgk_mapped_rowptr_i32": [_ptr, _i64, _i32, _ptr, _ptr, _size, _ptr],

@@ -3,6 +3,7 @@
 // radix ranks, no tensor cores.  Results are bit-exact with the numpy oracle (oracle/tfg_oracle.py).
 #include "common.cuh"
 #include "scan.cuh"
+#include <cuda_fp16.h>
 #include <string.h>
 #include <algorithm>
 
@@ -154,6 +155,147 @@ __global__ void __launch_bounds__(kGatherThreads) gather_rows_cached_f32_kernel(
         int64_t ldc, const int32_t *__restrict__ slot, const int32_t *__restrict__ index, int64_t n,
         float *__restrict__ out, int64_t ldo) {
     gather_rows_mapped_body<float, true>(table, ld, n_rows, F, cache, ldc, slot, index, n, out, ldo);
+}
+
+// ---- the same gather from a 16-bit table (tfgk_gather_rows_mapped_16, tfgk_gather_rows_cached_16) ------------------
+// Elements are bf16 or fp16 bit patterns; kVec of them (8, 4, 2 or 1: 16, 8, 4 or 2 bytes) travel in one load, and the
+// launcher takes the widest kVec that F, the strides and the base pointers allow.  Each element is widened to float32
+// exactly (bf16: a 16-bit shift; fp16: the hardware conversion), so out is the float32 table's gather bit for bit.
+// kCopy (mapped entry only) stores the 16-bit patterns unchanged instead, and a 16-bit NaN for a bad id.
+template <int kVec> struct Bits16;
+template <> struct Bits16<8> { using T = uint4; };
+template <> struct Bits16<4> { using T = uint2; };
+template <> struct Bits16<2> { using T = uint32_t; };
+template <> struct Bits16<1> { using T = uint16_t; };
+
+template <bool kHalf>
+__device__ __forceinline__ float widen16(uint32_t h) {
+    if constexpr (kHalf) return __half2float(__ushort_as_half((unsigned short)h));
+    else return __uint_as_float(h << 16);
+}
+
+// element j of a kVec-wide load (little-endian: element 0 is the low half of the first word)
+template <int kVec>
+__device__ __forceinline__ uint32_t elem16(const typename Bits16<kVec>::T &v, int j) {
+    if constexpr (kVec == 1) {
+        return v;
+    } else {
+        const uint32_t *w = reinterpret_cast<const uint32_t *>(&v);
+        return (w[j >> 1] >> (16 * (j & 1))) & 0xffffu;
+    }
+}
+
+template <int kVec>
+__device__ __forceinline__ typename Bits16<kVec>::T splat16(uint32_t h) {
+    using L = typename Bits16<kVec>::T;
+    if constexpr (kVec == 1) {
+        return (L)h;
+    } else {
+        L v;
+        uint32_t *w = reinterpret_cast<uint32_t *>(&v);
+#pragma unroll
+        for (int k = 0; k < kVec / 2; ++k) w[k] = h | (h << 16);
+        return v;
+    }
+}
+
+// kVec float32 values at dst, in float4 / float2 / float stores (dst is aligned to min(16, 4 kVec) bytes)
+template <int kVec>
+__device__ __forceinline__ void store_f32(float *dst, const float (&f)[kVec]) {
+    if constexpr (kVec >= 4) {
+#pragma unroll
+        for (int k = 0; k < kVec / 4; ++k)
+            reinterpret_cast<float4 *>(dst)[k] = make_float4(f[4 * k], f[4 * k + 1], f[4 * k + 2], f[4 * k + 3]);
+    } else if constexpr (kVec == 2) {
+        *reinterpret_cast<float2 *>(dst) = make_float2(f[0], f[1]);
+    } else {
+        dst[0] = f[0];
+    }
+}
+
+template <int kVec, bool kHalf, bool kCached, bool kCopy>
+__global__ void __launch_bounds__(kGatherThreads) gather_rows_16_kernel(
+        const uint16_t *__restrict__ table, int64_t ld, int64_t n_rows, int32_t F, const uint16_t *__restrict__ cache,
+        int64_t ldc, const int32_t *__restrict__ slot, const int32_t *__restrict__ index, int64_t n,
+        void *__restrict__ out, int64_t ldo) {
+    using L = typename Bits16<kVec>::T;
+    const int lane = threadIdx.x & 31;
+    const int32_t nv = F / kVec;                                 // loads per row
+    const int64_t warps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+    for (int64_t i = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; i < n; i += warps) {
+        const int32_t r = index[i];
+        L *dst16 = reinterpret_cast<L *>(static_cast<uint16_t *>(out) + i * ldo);
+        float *dst32 = static_cast<float *>(out) + i * ldo;
+        if (r < 0 || (int64_t)r >= n_rows) {
+            if constexpr (kCopy) {
+                for (int32_t c = lane; c < nv; c += 32) dst16[c] = splat16<kVec>(kHalf ? 0x7e00u : 0x7fc0u);
+            } else {
+                float q[kVec];
+#pragma unroll
+                for (int j = 0; j < kVec; ++j) q[j] = __int_as_float(0x7fc00000);
+                for (int32_t c = lane; c < nv; c += 32) store_f32<kVec>(dst32 + (int64_t)c * kVec, q);
+            }
+            continue;
+        }
+        const L *src = reinterpret_cast<const L *>(table + (int64_t)r * ld);
+        if constexpr (kCached) {
+            const int32_t s = __ldg(slot + r);
+            if (s >= 0) src = reinterpret_cast<const L *>(cache + (int64_t)s * ldc);
+        }
+        for (int32_t c0 = lane; c0 < nv; c0 += 32 * kGatherUnroll) {
+            L v[kGatherUnroll];
+#pragma unroll
+            for (int u = 0; u < kGatherUnroll; ++u)
+                if (c0 + 32 * u < nv) v[u] = src[c0 + 32 * u];
+#pragma unroll
+            for (int u = 0; u < kGatherUnroll; ++u) {
+                const int32_t c = c0 + 32 * u;
+                if (c >= nv) continue;
+                if constexpr (kCopy) {
+                    dst16[c] = v[u];
+                } else {
+                    float f[kVec];
+#pragma unroll
+                    for (int j = 0; j < kVec; ++j) f[j] = widen16<kHalf>(elem16<kVec>(v[u], j));
+                    store_f32<kVec>(dst32 + (int64_t)c * kVec, f);
+                }
+            }
+        }
+    }
+}
+
+// Whether kVec 16-bit elements per load fit: F and every stride a multiple of kVec, the 16-bit bases aligned to 2 kVec
+// bytes, and the output's rows and base aligned to its store width (2 kVec bytes when copying, min(16, 4 kVec) when
+// widening to float32, which is stored in float4 pieces).
+static bool gather16_fits(int kVec, int32_t F, int64_t ld, const void *table, int64_t ldc, const void *cache,
+                          int64_t ldo, const void *out, int out_bytes) {
+    const uintptr_t in_align = 2u * kVec;
+    const uintptr_t out_align = out_bytes == 2 ? in_align : (uintptr_t)std::min(16, 4 * kVec);
+    return F % kVec == 0 && ld % kVec == 0 && (reinterpret_cast<uintptr_t>(table) & (in_align - 1)) == 0 &&
+           (cache == nullptr || (ldc % kVec == 0 && (reinterpret_cast<uintptr_t>(cache) & (in_align - 1)) == 0)) &&
+           ((uint64_t)ldo * out_bytes) % out_align == 0 && (reinterpret_cast<uintptr_t>(out) & (out_align - 1)) == 0;
+}
+
+template <bool kHalf, bool kCached, bool kCopy>
+static void launch_gather16(const uint16_t *table, int64_t ld, int64_t n_rows, int32_t F, const uint16_t *cache,
+                            int64_t ldc, const int32_t *slot, const int32_t *index, int64_t n, void *out, int64_t ldo,
+                            cudaStream_t st) {
+    const int64_t warps_per_block = kGatherThreads / 32;
+    const unsigned blocks = (unsigned)std::min<int64_t>(ceil_div64(n, warps_per_block),
+                                                        (int64_t)sm_count() * kGatherBlocksPerSm);
+    const int out_bytes = kCopy ? 2 : 4;
+    if (gather16_fits(8, F, ld, table, ldc, cache, ldo, out, out_bytes))
+        gather_rows_16_kernel<8, kHalf, kCached, kCopy><<<blocks, kGatherThreads, 0, st>>>(table, ld, n_rows, F, cache,
+                                                                                          ldc, slot, index, n, out, ldo);
+    else if (gather16_fits(4, F, ld, table, ldc, cache, ldo, out, out_bytes))
+        gather_rows_16_kernel<4, kHalf, kCached, kCopy><<<blocks, kGatherThreads, 0, st>>>(table, ld, n_rows, F, cache,
+                                                                                          ldc, slot, index, n, out, ldo);
+    else if (gather16_fits(2, F, ld, table, ldc, cache, ldo, out, out_bytes))
+        gather_rows_16_kernel<2, kHalf, kCached, kCopy><<<blocks, kGatherThreads, 0, st>>>(table, ld, n_rows, F, cache,
+                                                                                          ldc, slot, index, n, out, ldo);
+    else
+        gather_rows_16_kernel<1, kHalf, kCached, kCopy><<<blocks, kGatherThreads, 0, st>>>(table, ld, n_rows, F, cache,
+                                                                                          ldc, slot, index, n, out, ldo);
 }
 
 __global__ void csr_rowsum_kernel(const int64_t *__restrict__ rowptr, const float *__restrict__ w, int32_t N,
@@ -998,6 +1140,55 @@ int tfgk_gather_rows_cached_f32(const float *table, int64_t ld, int64_t n_rows, 
     else
         gather_rows_cached_f32_kernel<<<blocks, kGatherThreads, 0, as_stream(stream)>>>(table, ld, n_rows, F, cache,
                                                                                        ldc, slot, index, n, out, ldo);
+    TFGK_LAUNCH_CHECK();
+    return TFGK_OK;
+}
+
+int tfgk_gather_rows_mapped_16(const uint16_t *table, int32_t dtype, int64_t ld, int64_t n_rows, int32_t F,
+                               const int32_t *index, int64_t n, void *out, int32_t out_dtype, int64_t ldo,
+                               void *stream) {
+    TFGK_CHECK_ARG(dtype == TFGK_DTYPE_BF16 || dtype == TFGK_DTYPE_F16,
+                   "gather_rows_mapped_16: dtype must be TFGK_DTYPE_BF16 or TFGK_DTYPE_F16 (got %d)", dtype);
+    TFGK_CHECK_ARG(out_dtype == TFGK_DTYPE_F32 || out_dtype == dtype,
+                   "gather_rows_mapped_16: out_dtype must be TFGK_DTYPE_F32 or the table's dtype %d (got %d)", dtype,
+                   out_dtype);
+    TFGK_CHECK_ARG(n >= 0 && n_rows >= 0 && F >= 1, "gather_rows_mapped_16: bad size (n=%lld, n_rows=%lld, F=%d)",
+                   (long long)n, (long long)n_rows, F);
+    TFGK_CHECK_ARG(ld >= F && ldo >= F, "gather_rows_mapped_16: need ld >= F and ldo >= F (ld=%lld, ldo=%lld, F=%d)",
+                   (long long)ld, (long long)ldo, F);
+    if (n == 0) return TFGK_OK;
+    TFGK_CHECK_ARG(index && out && (table || n_rows == 0), "gather_rows_mapped_16: null pointer");
+    const bool half = dtype == TFGK_DTYPE_F16, copy = out_dtype == dtype;
+    cudaStream_t st = as_stream(stream);
+    if (half && copy)
+        launch_gather16<true, false, true>(table, ld, n_rows, F, nullptr, 0, nullptr, index, n, out, ldo, st);
+    else if (half)
+        launch_gather16<true, false, false>(table, ld, n_rows, F, nullptr, 0, nullptr, index, n, out, ldo, st);
+    else if (copy)
+        launch_gather16<false, false, true>(table, ld, n_rows, F, nullptr, 0, nullptr, index, n, out, ldo, st);
+    else
+        launch_gather16<false, false, false>(table, ld, n_rows, F, nullptr, 0, nullptr, index, n, out, ldo, st);
+    TFGK_LAUNCH_CHECK();
+    return TFGK_OK;
+}
+
+int tfgk_gather_rows_cached_16(const uint16_t *table, int32_t dtype, int64_t ld, int64_t n_rows, int32_t F,
+                               const uint16_t *cache, int64_t ldc, const int32_t *slot, const int32_t *index,
+                               int64_t n, float *out, int64_t ldo, void *stream) {
+    TFGK_CHECK_ARG(dtype == TFGK_DTYPE_BF16 || dtype == TFGK_DTYPE_F16,
+                   "gather_rows_cached_16: dtype must be TFGK_DTYPE_BF16 or TFGK_DTYPE_F16 (got %d)", dtype);
+    TFGK_CHECK_ARG(n >= 0 && n_rows >= 0 && F >= 1, "gather_rows_cached_16: bad size (n=%lld, n_rows=%lld, F=%d)",
+                   (long long)n, (long long)n_rows, F);
+    TFGK_CHECK_ARG(ld >= F && ldc >= F && ldo >= F,
+                   "gather_rows_cached_16: need ld, ldc and ldo >= F (ld=%lld, ldc=%lld, ldo=%lld, F=%d)",
+                   (long long)ld, (long long)ldc, (long long)ldo, F);
+    if (n == 0) return TFGK_OK;
+    TFGK_CHECK_ARG(index && out && cache && slot && (table || n_rows == 0), "gather_rows_cached_16: null pointer");
+    cudaStream_t st = as_stream(stream);
+    if (dtype == TFGK_DTYPE_F16)
+        launch_gather16<true, true, false>(table, ld, n_rows, F, cache, ldc, slot, index, n, out, ldo, st);
+    else
+        launch_gather16<false, true, false>(table, ld, n_rows, F, cache, ldc, slot, index, n, out, ldo, st);
     TFGK_LAUNCH_CHECK();
     return TFGK_OK;
 }

@@ -332,6 +332,65 @@ def gather_rows_cached(table_ptr, ld, n_rows, num_features, cache, slot, index, 
     return out
 
 
+_DTYPE16_CODES = {torch.bfloat16: _ffi.DTYPE_BF16, torch.float16: _ffi.DTYPE_F16}
+
+
+def _gather_out(out, n, num_features, dtype, device):
+    if out is None:
+        return torch.empty((n, num_features), dtype=dtype, device=device)
+    if not (torch.is_tensor(out) and out.is_cuda and out.dtype == dtype and tuple(out.shape) == (n, num_features)):
+        raise TypeError("out must be a {} CUDA tensor of shape {}".format(dtype, (n, num_features)))
+    return out
+
+
+def gather_rows_mapped_16(table_ptr, dtype, ld, n_rows, num_features, index, out=None, out_dtype=torch.float32):
+    """gather_rows_mapped for a 16-bit table (dtype torch.bfloat16 or torch.float16; ld counted in elements): out[i] =
+    table[index[i], :num_features] widened exactly to float32, bit-identical to the float32 table's gather; ids outside
+    [0, n_rows) give NaN rows.  out_dtype=dtype copies the 16-bit patterns unchanged instead (a bad id then gives a
+    16-bit NaN row), which fills a 16-bit device cache.  Returns out, a new [n, num_features] tensor of out_dtype on
+    index's device unless given (rows contiguous, any row stride)."""
+    if dtype not in _DTYPE16_CODES:
+        raise ValueError("gather_rows_mapped_16 takes a torch.bfloat16 or torch.float16 table (got {})".format(dtype))
+    if out_dtype not in (torch.float32, dtype):
+        raise ValueError("out_dtype must be torch.float32 or the table's {} (got {})".format(dtype, out_dtype))
+    _check(index, torch.int32, "index")
+    n = index.numel()
+    out = _gather_out(out, n, num_features, out_dtype, index.device)
+    if n:
+        ldo = _row_major_2d(out, "out")
+        _ffi.call("tfgk_gather_rows_mapped_16", ctypes.c_void_p(table_ptr), _DTYPE16_CODES[dtype], ld, n_rows,
+                  num_features, _p(index), n, _p(out), _ffi.DTYPE_F32 if out_dtype == torch.float32 else
+                  _DTYPE16_CODES[dtype], ldo, _stream(out))
+    return out
+
+
+def gather_rows_cached_16(table_ptr, ld, n_rows, num_features, cache, slot, index, out=None):
+    """gather_rows_cached for a 16-bit table: the table's dtype is cache's (torch.bfloat16 or torch.float16, [C,
+    num_features], rows contiguous, any row stride), ld counts elements, and out is float32, each element widened
+    exactly.  cache, slot, index and out share one device; the cache and the map are recorded on the gather's stream."""
+    _check(index, torch.int32, "index")
+    _check(slot, torch.int32, "slot")
+    if not (torch.is_tensor(cache) and cache.is_cuda and cache.dtype in _DTYPE16_CODES and cache.dim() == 2
+            and cache.shape[1] == num_features):
+        raise TypeError("cache must be a bfloat16 or float16 CUDA tensor of shape [C, {}]".format(num_features))
+    if slot.numel() != n_rows:
+        raise ValueError("slot must have one entry per table row ({} != {})".format(slot.numel(), n_rows))
+    n = index.numel()
+    out = _gather_out(out, n, num_features, torch.float32, index.device)
+    if not (cache.device == slot.device == index.device == out.device):
+        raise ValueError("cache, slot, index and out must be on one device")
+    if n:
+        ldc = _row_major_2d(cache, "cache")
+        ldo = _row_major_2d(out, "out")
+        stream = torch.cuda.current_stream(out.device)
+        _ffi.call("tfgk_gather_rows_cached_16", ctypes.c_void_p(table_ptr), _DTYPE16_CODES[cache.dtype], ld, n_rows,
+                  num_features, _p(cache), ldc, _p(slot), _p(index), n, _p(out), ldo,
+                  ctypes.c_void_p(stream.cuda_stream))
+        cache.record_stream(stream)
+        slot.record_stream(stream)
+    return out
+
+
 # ---- a CSR built from an edge list in host memory (utils.HostNeighborSampler) -------------------------------------
 # row_ptr, col_ptr, w_ptr: device addresses of page-locked host arrays (host_register), int32 / int32 / float32 [E]
 

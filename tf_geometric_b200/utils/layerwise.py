@@ -106,7 +106,7 @@ def layerwise_inference(sampler, x, layers, device_bytes=None):
     """layers[-1](... layers[0](x) ...) for every node of the sampler's graph, one layer at a time.
 
     sampler: a RandomNeighborSampler or a HostNeighborSampler.  x: a float32 [N, F] device tensor or a HostFeatureTable
-    (at least N rows).  layers: tfg.layers.GCN, GAT, MeanGraphSage, SumGraphSage, MeanPoolGraphSage or
+    of any of its dtypes (at least N rows; a 16-bit table's rows reach the first layer widened exactly to float32).  layers: tfg.layers.GCN, GAT, MeanGraphSage, SumGraphSage, MeanPoolGraphSage or
     MaxPoolGraphSage, already built (trained); anything else raises TypeError before any device work.
 
     Each layer cuts the rows into consecutive ranges (_row_ranges) whose working set, layerwise_chunk_bytes per edge and

@@ -16,10 +16,11 @@ layer computes only the rows it must.  The sizes stay on the device until the ba
 synchronisation per batch.  sample_link_blocks seeds such a batch with the endpoints of target pairs and their
 negatives (LinkBlocks), optionally with the targets excluded from the neighbourhoods their endpoints aggregate.
 
-HostFeatureTable keeps an [N, F] float32 feature table in host memory (page-locked in place) and gathers the rows a batch
-reads over the host link (tfgk_gather_rows_mapped_f32), so the table need not fit on the device.  With device_rows it
-also keeps those rows in device memory and reads them from there (tfgk_gather_rows_cached_f32); rank_source_rows
-orders a graph's rows by how many sampled batches read them, to choose which rows to keep."""
+HostFeatureTable keeps an [N, F] float32, float16 or bfloat16 feature table in host memory (page-locked in place) and
+gathers the rows a batch reads over the host link (tfgk_gather_rows_mapped_f32, or tfgk_gather_rows_mapped_16 for a
+16-bit table, whose rows arrive widened to float32), so the table need not fit on the device.  With device_rows it also
+keeps those rows in device memory, in the table's dtype, and reads them from there (tfgk_gather_rows_cached_f32 /
+_16); rank_source_rows orders a graph's rows by how many sampled batches read them, to choose which rows to keep."""
 import mmap
 import threading
 
@@ -318,10 +319,11 @@ class SampledBlocks(object):
 
     def source_rows(self, x):
         """Layer 0's input for the global feature table x [N, F]: a float32 tensor (moved to the device when it is not
-        there), or a HostFeatureTable, whose rows node_index are gathered over the host link into a new [num_src, F]
-        device tensor on the current stream.  For a batch from sample_blocks the ids were checked by the sampler, so the
-        table only needs num_nodes rows and the gather makes no host synchronisation; a batch built by hand takes the
-        checked HostFeatureTable.gather."""
+        there; any other dtype is converted to a float32 copy first), or a HostFeatureTable, whose rows node_index are
+        gathered over the host link into a new float32 [num_src, F] device tensor on the current stream (a 16-bit
+        table's rows widened exactly, so the rows are x.float()[node_index] bit for bit).  For a batch from
+        sample_blocks the ids were checked by the sampler, so the table only needs num_nodes rows and the gather makes
+        no host synchronisation; a batch built by hand takes the checked HostFeatureTable.gather."""
         if isinstance(x, HostFeatureTable):
             if self.num_nodes is None:
                 return x.gather(self.node_index)
@@ -388,31 +390,39 @@ def _host_release(key):
 
 
 class HostFeatureTable(object):
-    """A float32 feature table [N, F] kept in host memory, whose rows the device gathers over the host link.
+    """A feature table [N, F] kept in host memory, whose rows the device gathers over the host link.
 
-    x: a CPU float32 2-D tensor or numpy array with unit column stride (numpy is wrapped without a copy).  A pinned
-    tensor is read as it is; otherwise the whole buffer under x (its storage, or the numpy array that owns the memory)
-    is page-locked in place (no copy, so host memory is not doubled), once however many tables share it, and released
-    when the last of them closes.  The
-    table keeps a reference to x.  A host table is a constant: x must not require grad.
+    x: a CPU 2-D tensor or numpy array of `dtype` with unit column stride (numpy is wrapped without a copy).
+    dtype: the storage type, torch.float32 (the default), torch.float16 or torch.bfloat16; anything else raises
+    ValueError, and an x of another dtype raises TypeError: the table never converts or copies x, so a float32 table
+    becomes a 16-bit one only by the caller's own copy (x.to(torch.bfloat16)).  numpy has no bfloat16, so a bfloat16
+    table takes a torch tensor.  A 16-bit table moves half the bytes over the link and keeps twice the rows in the same
+    device memory; its gathers still return float32, each element widened exactly.
+    A pinned tensor is read as it is; otherwise the whole buffer under x (its storage, or the numpy array that owns the
+    memory) is page-locked in place (no copy, so host memory is not doubled), once however many tables share it, and
+    released when the last of them closes.  The table keeps a reference to x.  A host table is a constant: x must not require grad.
 
     device_rows: optional integer id vector (numpy, CPU or CUDA; int32 CUDA is used as it is) of rows to keep in device
     memory as well, on device_rows' device if it is a CUDA tensor, otherwise on the current device.  Those rows are
-    copied once, by the same host gather, to a [C, F] device buffer, next to an int32 [N] map from row to buffer slot
-    (-1: not cached).  A gather on that device reads cached rows from device memory and the rest over the host link, in
+    copied once, by the same host gather, to a [C, F] device buffer in the table's dtype (a 16-bit table copies the
+    rows' bit patterns), next to an int32 [N] map from row to buffer slot (-1: not cached).  A gather on that device reads cached rows from device memory and the rest over the host link, in
     one launch; a gather on another device reads every row over the link.  Either way the bits are x[index].  The ids
     are checked with one read-back: IndexError outside [0, N), ValueError for a repeated id or an array that is not a
     vector, TypeError for non-integer ids.  The constructor returns once the device rows are in place, so any stream
     may gather at once.  None or an empty vector keeps no rows on the device.  rank_source_rows chooses the rows.
 
-    gather(index) and SampledBlocks.source_rows(table) return new float32 device tensors, bit-identical to x[index].
+    gather(index) and SampledBlocks.source_rows(table) return new float32 device tensors, bit-identical to
+    x.float()[index] (x[index] for a float32 table).
     close() (or leaving a `with` block) drops the device rows and releases the registration after the current device's
     pending work; a table that is dropped without close() does both when it is collected."""
 
-    def __init__(self, x, device_rows=None):
+    def __init__(self, x, device_rows=None, dtype=torch.float32):
         self._closed = True                 # until registration succeeds: nothing for close() / __del__ to release
         self._key = None
         self._cache = self._slot = self._device_rows = None
+        if dtype not in (torch.float32, torch.float16, torch.bfloat16):
+            raise ValueError("HostFeatureTable stores torch.float32, torch.float16 or torch.bfloat16 (got dtype={})"
+                             .format(dtype))
         array = x
         if isinstance(x, np.ndarray):
             x = torch.from_numpy(x)
@@ -422,8 +432,11 @@ class HostFeatureTable(object):
             raise TypeError("HostFeatureTable takes a table in host memory; a CUDA tensor goes to source_rows directly")
         if x.dim() != 2:
             raise TypeError("HostFeatureTable takes a 2-D [N, F] table (got {} dimensions)".format(x.dim()))
-        if x.dtype != torch.float32:
-            raise TypeError("HostFeatureTable takes float32 features (got {})".format(x.dtype))
+        if x.dtype != dtype:
+            if dtype == torch.float32:
+                raise TypeError("HostFeatureTable takes float32 features (got {})".format(x.dtype))
+            raise TypeError("HostFeatureTable(dtype={}) takes {} features (got {}); the table does not convert "
+                            "x".format(dtype, dtype, x.dtype))
         if x.requires_grad:
             raise ValueError("a host feature table is a constant: x must not require grad")
         n, F = x.shape
@@ -437,7 +450,10 @@ class HostFeatureTable(object):
         self._key, self._ptr = _host_acquire(x, array)
         self._closed = False
         if rows is not None:
-            self._cache = ops.gather_rows_mapped(self._ptr, self._ld, n, F, rows)
+            if dtype == torch.float32:
+                self._cache = ops.gather_rows_mapped(self._ptr, self._ld, n, F, rows)
+            else:                           # the rows' 16-bit patterns as they are
+                self._cache = ops.gather_rows_mapped_16(self._ptr, dtype, self._ld, n, F, rows, out_dtype=dtype)
             slot = torch.full((n,), -1, dtype=torch.int32, device=rows.device)
             slot[rows.long()] = torch.arange(rows.numel(), dtype=torch.int32, device=rows.device)
             self._slot, self._device_rows = slot, rows
@@ -455,16 +471,22 @@ class HostFeatureTable(object):
         return self.x.shape[1]
 
     @property
+    def dtype(self):
+        """The storage type of x: torch.float32, torch.float16 or torch.bfloat16 (gathers return float32)."""
+        return self.x.dtype
+
+    @property
     def device_rows(self):
         """The ids of the rows kept in device memory (int32 on the device, in cache order), or None."""
         return self._device_rows
 
     @property
     def device_bytes(self):
-        """Device memory this table holds: the cached rows plus the row-to-slot map (0 without device rows)."""
+        """Device memory this table holds: the cached rows (C * F * itemsize) plus the row-to-slot map (4 * N), 0
+        without device rows."""
         if self._cache is None:
             return 0
-        return self._cache.numel() * 4 + self._slot.numel() * 4
+        return self._cache.numel() * self._cache.element_size() + self._slot.numel() * 4
 
     def _check_open(self):
         if self._closed:
@@ -475,15 +497,23 @@ class HostFeatureTable(object):
         self._check_open()
         if index.numel() == 0 and out is None:
             return torch.empty((0, self.num_features), dtype=torch.float32, device=index.device)
-        if self._cache is not None and index.device == self._cache.device:
+        cached = self._cache is not None and index.device == self._cache.device
+        if self.x.dtype != torch.float32:
+            if cached:
+                return ops.gather_rows_cached_16(self._ptr, self._ld, self.num_rows, self.num_features, self._cache,
+                                                 self._slot, index.contiguous(), out)
+            return ops.gather_rows_mapped_16(self._ptr, self.x.dtype, self._ld, self.num_rows, self.num_features,
+                                             index.contiguous(), out)
+        if cached:
             return ops.gather_rows_cached(self._ptr, self._ld, self.num_rows, self.num_features, self._cache, self._slot,
                                           index.contiguous(), out)
         return ops.gather_rows_mapped(self._ptr, self._ld, self.num_rows, self.num_features, index.contiguous(), out)
 
     def gather(self, index, out=None):
         """x[index] as a new contiguous float32 device tensor [len(index), F] (or into `out`, a float32 CUDA tensor of
-        that shape), on the current stream.  Ids: an integer vector (int32 on the device is used as it is); ids
-        outside [0, num_rows) raise IndexError after one read-back of their range."""
+        that shape), on the current stream; a 16-bit table's rows are widened exactly (x.float()[index]).  Ids: an
+        integer vector (int32 on the device is used as it is); ids outside [0, num_rows) raise IndexError after one
+        read-back of their range."""
         self._check_open()
         idx = ops.as_device(index).reshape(-1)
         if idx.dtype.is_floating_point or idx.dtype.is_complex or idx.dtype == torch.bool:
