@@ -719,8 +719,8 @@ int tfgk_block_gcn_values_f32(const int64_t *rowptr, const int32_t *gcol, const 
  *   counted in state[0] and relabelled -1.  local int32 [2, n_pairs]: the pairs relabelled (sources, then destinations).
  *   Hop 0's capacity is 2 n_pairs.  Workspace: tfgk_block_pairs_workspace_bytes(n_pairs).  Asynchronous; _count, _fill
  *   and _end follow as for _begin.
- * tfgk_link_tail_negatives_i32: out_row[i] = src[i / q], out_col[i] = random_below(seed, rng_stream, i, N) for
- *   i < n_src * q (tail corruption, uniform over [0, N)).  One launch, asynchronous.
+ * tfgk_link_tail_negatives_i32: out_row[i] = src[i / q], out_col[i] = random_below64(seed, rng_stream, i, N) for
+ *   i < n_src * q (tail corruption, uniform over [0, N) to within N / 2^64).  One launch, asynchronous.
  * Exclusion lists, for the cap >= n_seeds first rows of the list `nodes`: target_src / target_dst [n_targets] are the
  *   (local row, global column) pairs to exclude, sorted by (source, destination) (sources outside [0, cap) are
  *   skipped).  Row t's list is every position p of CSR row nodes[t] whose column col[p] is a target of t, ascending; a
@@ -805,8 +805,9 @@ int tfgk_neg_decode(const int64_t *rowptr, const int32_t *col, const int64_t *of
                     int64_t S, int32_t *out_row, int32_t *out_col, void *stream);
 int tfgk_neg_sample_start(const int64_t *rowptr, const int32_t *col, int32_t N, const int32_t *start, int64_t S,
                           uint64_t seed, uint32_t rng_stream, int32_t *out_col, void *stream);
-/* np.random.randint(0, N, [2, S]) with the counter-based generator: out[0, s] = random_below(seed, rng_stream, 2 s, N),
- * out[1, s] = random_below(seed, rng_stream, 2 s + 1, N)  (negative_sampling without edge_index, graph_utils.py:384-386). */
+/* np.random.randint(0, N, [2, S]) with the counter-based generator: out[0, s] = random_below64(seed, rng_stream, 2 s, N),
+ * out[1, s] = random_below64(seed, rng_stream, 2 s + 1, N), one Philox block per pair and uniform over [0, N) to within
+ * N / 2^64  (negative_sampling without edge_index, graph_utils.py:384-386). */
 int tfgk_random_pairs_i32(int32_t N, int64_t S, uint64_t seed, uint32_t rng_stream, int32_t *out, void *stream);
 
 /* ---- edge-weight gradients ------------------------------------------------------------------------------------ */

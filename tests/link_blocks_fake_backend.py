@@ -8,8 +8,8 @@ no such path.  `calls` counts the fake entries and records the flags of every CS
 import numpy as np
 
 import block_fake_backend
+import link_oracle as lo
 from fake_backend import _np, _t
-from oracle import tfg_oracle as o
 
 
 def pair_begin_np(pairs, N):
@@ -30,7 +30,7 @@ def pair_begin_np(pairs, N):
 def tail_negatives_np(src, q, N, seed, stream=2):
     n = len(src) * q
     return np.stack([np.repeat(np.asarray(src, np.int32), q),
-                     o.random_below(seed, stream, np.arange(n, dtype=np.uint64), N).astype(np.int32)]).reshape(2, n)
+                     lo.random_below64(seed, stream, np.arange(n, dtype=np.uint64), N).astype(np.int32)]).reshape(2, n)
 
 
 def exclusion_lists_np(rowptr, col, nodes, cap, ts, td):

@@ -8,7 +8,6 @@ import numpy as np
 import fake_backend
 import link_oracle as lo
 from fake_backend import _np, _t
-from oracle import tfg_oracle as o
 
 
 def install(monkeypatch):
@@ -56,8 +55,8 @@ def install(monkeypatch):
 
     def random_pairs(num_nodes, num_samples, seed, device, rng_stream=ops.RNG_STREAM_LINK):
         s2 = np.arange(num_samples, dtype=np.uint64) * np.uint64(2)
-        return _t(np.stack([o.random_below(seed, rng_stream, s2, num_nodes),
-                            o.random_below(seed, rng_stream, s2 + np.uint64(1), num_nodes)]).astype(np.int32))
+        return _t(np.stack([lo.random_below64(seed, rng_stream, s2, num_nodes),
+                            lo.random_below64(seed, rng_stream, s2 + np.uint64(1), num_nodes)]).astype(np.int32))
 
     for name, fn in dict(edge_dot=edge_dot, neg_offsets=neg_offsets, neg_draw=neg_draw, neg_dup_flags=neg_dup_flags,
                          neg_decode=neg_decode, neg_sample_start=neg_sample_start, random_pairs=random_pairs).items():

@@ -119,8 +119,8 @@ def negative_sampling(num_samples, num_nodes, edge_index=None, replace=True, bat
         sb = link_batch_seed(seed, b)
         if edge_index is None:
             s2 = np.arange(num_samples, dtype=np.uint64) * np.uint64(2)
-            out.append(np.stack([o.random_below(sb, RNG_STREAM_LINK, s2, num_nodes),
-                                 o.random_below(sb, RNG_STREAM_LINK, s2 + np.uint64(1), num_nodes)]).astype(np.int32))
+            out.append(np.stack([random_below64(sb, RNG_STREAM_LINK, s2, num_nodes),
+                                 random_below64(sb, RNG_STREAM_LINK, s2 + np.uint64(1), num_nodes)]).astype(np.int32))
             continue
         rowptr, col, offsets = negative_structure(edge_index, num_nodes)
         C = int(offsets[-1])
@@ -138,7 +138,7 @@ def negative_sampling_with_start_node(start_node_index, num_nodes, edge_index=No
     start = np.asarray(start_node_index, np.int64).reshape(-1)
     S = len(start)
     if edge_index is None:
-        end = o.random_below(seed, RNG_STREAM_LINK, np.arange(S, dtype=np.uint64) * np.uint64(2) + np.uint64(1), num_nodes)
+        end = random_below64(seed, RNG_STREAM_LINK, np.arange(S, dtype=np.uint64) * np.uint64(2) + np.uint64(1), num_nodes)
         return np.stack([start, end]).astype(np.int32)
     rowptr, col, offsets = negative_structure(edge_index, num_nodes, start=True)
     end = np.empty(S, np.int64)

@@ -145,7 +145,8 @@ def test_negative_sampling_full_candidate_set_and_numpy_container(ref):
     np.testing.assert_array_equal(got, lo.negative_sampling(C, n, ei, replace=False, seed=5))
 
 
-def test_negative_sampling_without_edge_index():
+def test_negative_sampling_without_edge_index_draws_64_bit_ids():
+    """Both ends are random_below64 draws 2 s and 2 s + 1 of each batch's key (uniform on [0, N) to within N / 2^64)."""
     got = tfg.utils.negative_sampling(1000, 37, None, batch_size=2, seed=4)
     want = lo.negative_sampling(1000, 37, None, batch_size=2, seed=4)
     for g, w in zip(got, want):
@@ -197,7 +198,9 @@ def test_negative_sampling_on_a_graph_the_reference_cannot_hold():
 
 # ---- start node ------------------------------------------------------------------------------------------------------------
 
-def test_start_node_sampling(ref):
+def test_start_node_sampling_draws_64_bit_ids(ref):
+    """Partners against the restatement, with edge_index (a candidate index per start node) and without (the
+    random_below64 draw 2 s + 1 of the key)."""
     n, ei, start = int(ref["n"]), ref["ei"], ref["start"]
     got = tfg.utils.negative_sampling_with_start_node(torch.from_numpy(start).to(DEV), n, torch.from_numpy(ei).to(DEV),
                                                       seed=12)

@@ -3,7 +3,7 @@
 exclusion the batch bit for bit against sample_blocks over the first-occurrence endpoint list; with "self" and "reverse"
 exclusion bit for bit against sample_blocks over a sampler built on the edge list with those entries deleted (a
 5 000-edge hub holding targets, rows on both sides of the 128-entry thread limit, duplicate edges, a row emptied
-entirely); the negatives against the oracle's random_below; the host synchronisations; GCN values with exclusion
+entirely); the negatives against link_oracle's random_below64; the host synchronisations; GCN values with exclusion
 against the full graph; the backward against float64; learning evaluated on the full graph; the refusals."""
 import numpy as np
 import pytest
@@ -12,8 +12,8 @@ import torch
 import tf_geometric_b200 as tfg
 from tf_geometric_b200 import ops, _ffi
 from tf_geometric_b200.utils import sampling
-from oracle import tfg_oracle as o
 from conftest import random_graph
+import link_oracle as lo
 import train_bound
 
 pytestmark = pytest.mark.gpu
@@ -134,7 +134,9 @@ def test_exclusion_is_sample_blocks_over_the_deleted_graph(samplers, exclude, fa
         assert np.array_equal(np.diff(host(off))[:seeds.size], want) and want[where[9]] >= 30
 
 
-def test_negatives_against_the_oracle(samplers):
+def test_tail_negatives_are_64_bit_draws(samplers):
+    """Negative b q + j is (u_b, random_below64(seed, RNG_STREAM_LINK, b q + j, N)) on both samplers; given negatives
+    are relabelled."""
     s, ei, _ = samplers
     pos = _targets(ei)[:, :300]
     N = s["device"]._neighborhood_structure()[3].numel()
@@ -142,7 +144,7 @@ def test_negatives_against_the_oracle(samplers):
         b = s[kind].sample_link_blocks(pos, [5], num_negatives=3, seed=1234)
         neg = host(b.node_index)[host(b.neg_index)]
         idx = np.arange(pos.shape[1] * 3, dtype=np.uint64)
-        want = np.stack([np.repeat(pos[0], 3), o.random_below(1234, ops.RNG_STREAM_LINK, idx, N)]).astype(np.int32)
+        want = np.stack([np.repeat(pos[0], 3), lo.random_below64(1234, ops.RNG_STREAM_LINK, idx, N)]).astype(np.int32)
         assert np.array_equal(neg, want)
         given = np.array([[0, 5, 9], [3100, 7, 9]], np.int32)
         b = s[kind].sample_link_blocks(pos, [5], num_negatives=0, negative_edge_index=given, seed=3)

@@ -187,10 +187,12 @@ __global__ void neg_start_kernel(const int64_t *__restrict__ rowptr, const int32
     }
 }
 
+// both ends by 64-bit multiply-shift (draws 2 s and 2 s + 1: one Philox block per pair), uniform to within N / 2^64; a
+// 32-bit multiply-shift over-weights 2^32 mod N of the ids by N / 2^32
 __global__ void random_pairs_kernel(int32_t N, int64_t S, uint64_t seed, uint32_t stream, int32_t *__restrict__ out) {
     for (int64_t s = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; s < S; s += (int64_t)gridDim.x * blockDim.x) {
-        out[s] = (int32_t)random_below(seed, stream, 2 * (uint64_t)s, (uint32_t)N);
-        out[S + s] = (int32_t)random_below(seed, stream, 2 * (uint64_t)s + 1, (uint32_t)N);
+        out[s] = (int32_t)random_below64(seed, stream, 2 * (uint64_t)s, (uint64_t)N);
+        out[S + s] = (int32_t)random_below64(seed, stream, 2 * (uint64_t)s + 1, (uint64_t)N);
     }
 }
 

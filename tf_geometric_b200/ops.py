@@ -1236,8 +1236,8 @@ def link_block_sample_mapped(rowptr, col_ptr, w_ptr, pairs, n_pos, fanouts, keys
 
 
 def link_tail_negatives(src, q, num_nodes, seed, out_row, out_col, rng_stream=RNG_STREAM_LINK):
-    """Tail-corrupted negatives (tfgk_link_tail_negatives_i32): pair b * q + j is (src[b], random_below(seed, rng_stream,
-    b * q + j, num_nodes)), written to out_row / out_col int32 [len(src) * q]."""
+    """Tail-corrupted negatives (tfgk_link_tail_negatives_i32): pair b * q + j is (src[b], random_below64(seed,
+    rng_stream, b * q + j, num_nodes)), written to out_row / out_col int32 [len(src) * q]."""
     _check(src, torch.int32, "src")
     _check(out_row, torch.int32, "out_row")
     _check(out_col, torch.int32, "out_col")

@@ -606,7 +606,7 @@ _LINK_DOC = """Link-prediction mini-batch on blocks (an extension of the referen
         destination) in first-occurrence order; node_index[:hop_sizes[0]] is that list.  With exclude=None the batch is
         sample_blocks(that list, fanouts, padding, seed), bit for bit.
         Negatives: with num_negatives = q, negative pair b * q + j is (u_b, t), u_b the source of positive b and t drawn
-        uniformly from all nodes (random_below(seed, RNG_STREAM_LINK, b * q + j, N), tail corruption).  A negative may
+        uniformly from all nodes (random_below64(seed, RNG_STREAM_LINK, b * q + j, N), tail corruption).  A negative may
         coincide with a true edge; for exact non-edges pass negative_edge_index (for example from
         negative_sampling_with_start_node) with num_negatives=0.  Both at once: ValueError.
         Exclusion: "self" removes every CSR entry (u, v) of every positive pair (u, v) from u's row (duplicates
