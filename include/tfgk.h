@@ -769,6 +769,88 @@ int tfgk_block_sample_fill_mapped_excl(const int64_t *rowptr, int32_t n_rows, co
                                        int32_t *out_local, int32_t *out_gcol, float *out_w, const int64_t *excl_off,
                                        const int64_t *excl_pos, int32_t n_excl, void *workspace, size_t workspace_bytes,
                                        void *stream);
+
+/* Weighted block sampler: fan-outs drawn in proportion to the CSR's float32 weights w_csr (utils.RandomNeighborSampler /
+ * HostNeighborSampler with weighted=True).  The draw rule, for listed row t of global row r under hop key `seed`:
+ *   Candidates: the row's kept entries (all of them, or those the _excl lists leave), numbered by virtual position v as
+ *     the _excl entries number them; only entries of weight > 0 can be drawn, and d+ counts them.
+ *   Key: E(v, j) = -ln(u) / w in double, w the float32 weight widened, u = ((u64 >> 11) + 1) 2^-53 in (0, 1] where u64 is
+ *     lanes 0 | 1 << 32 of one Philox4x32-10 block with counter (v, r, rng_stream, j) and key `seed`.  ln is rng.cuh's
+ *     log_rn (exact exponent extraction, a fixed polynomial in explicitly rounded double operations), not the libm.
+ *   Integer fan-out k, padding 0, or padding 1 with k < d+: the min(k, d+) candidates of smallest (E(v, 0), v), without
+ *     replacement (successive sampling, Efraimidis-Spirakis), written in ascending CSR position.
+ *   Padding 1 with k >= d+ > 0: k draws with replacement, P(entry) = w / W; draw j is the candidate of smallest
+ *     (E(v, j + 1), v) (an exponential race: no prefix sums, so no bit depends on a summation order); draws in order.
+ *   d+ = 0: nothing.  Fan-out None is not a weighted rule (it takes every kept entry, zero weights included: the caller
+ *   uses the unweighted entries), and neither is the head rule; both are refused.
+ * pos_deg int32 [n_rows]: the positive degree of every CSR row, from tfgk_csr_positive_degree_f32.
+ * tfgk_csr_positive_degree_f32: pos_deg[r] = the entries of weight > 0 (and finite) of rows [0, n_rows) of rowptr, whose
+ *   weights are w[p - w_base] (w_base: the CSR position of w[0], so a range of rows staged on the device takes the
+ *   range's slice of rowptr and its first position); adds the count of negative, NaN and infinite weights to *n_invalid
+ *   (device).  One warp per row; asynchronous.
+ * _count_weighted / _count_weighted_excl / _count_weighted_mapped_excl: _count / _count_excl by the rule above (the _excl
+ *   forms read the weights at the excluded positions, int32 or, over a host CSR, int64).
+ * _fill_weighted, _fill_weighted_excl, _fill_weighted_mapped, _fill_weighted_mapped_excl: the _fill entries by the rule
+ *   above, same outputs otherwise (positions, then global columns and weights, then the frontier).  A row of at most 128
+ *   entries is drawn by one warp, which reads its weights once in 128-byte segments; a longer row by the CTA, with a
+ *   radix select of the k smallest keys (8 bits a pass, keys recomputed from the counter each pass, so no workspace grows
+ *   with the degree) or one CTA argmin per draw with replacement.  Over a host CSR every candidate's weight crosses the
+ *   link: once for a warp row, once per pass for a CTA row.
+ * tfgk_neighbor_sample_rows_count_weighted / _fill_weighted: K13's count and fill by the same rule, for
+ *   sample_neighborhood (device CSR, int32 positions). */
+int tfgk_csr_positive_degree_f32(const int64_t *rowptr, int32_t n_rows, const float *w, int64_t w_base,
+                                 int32_t *pos_deg, int32_t *n_invalid, void *stream);
+int tfgk_neighbor_sample_rows_count_weighted(const int64_t *rowptr, int32_t n_rows, const int32_t *rows, int32_t n_list,
+                                             int32_t k, int padding, const int32_t *pos_deg, const float *w_csr,
+                                             int64_t *out_rowptr, int64_t *total_host, void *workspace,
+                                             size_t workspace_bytes, void *stream);
+int tfgk_neighbor_sample_rows_fill_weighted(const int64_t *rowptr, int32_t n_rows, const int32_t *rows, int32_t n_list,
+                                            int32_t k, int padding, const int32_t *pos_deg, const float *w_csr,
+                                            uint64_t seed, uint32_t rng_stream, const int64_t *out_rowptr,
+                                            int32_t *out_row, int32_t *out_pos, void *stream);
+int tfgk_block_sample_count_weighted(const int64_t *rowptr, int32_t n_rows, const int32_t *nodes, const int32_t *state,
+                                     int32_t hop, int32_t n_hops, int32_t cap_list, int32_t k, int padding,
+                                     const int32_t *pos_deg, const float *w_csr, int64_t *out_rowptr, void *workspace,
+                                     size_t workspace_bytes, void *stream);
+int tfgk_block_sample_count_weighted_excl(const int64_t *rowptr, int32_t n_rows, const int32_t *nodes,
+                                          const int32_t *state, int32_t hop, int32_t n_hops, int32_t cap_list, int32_t k,
+                                          int padding, const int32_t *pos_deg, const float *w_csr,
+                                          const int64_t *excl_off, const int32_t *excl_pos, int32_t n_excl,
+                                          int64_t *out_rowptr, void *workspace, size_t workspace_bytes, void *stream);
+int tfgk_block_sample_count_weighted_mapped_excl(const int64_t *rowptr, int32_t n_rows, const int32_t *nodes,
+                                                 const int32_t *state, int32_t hop, int32_t n_hops, int32_t cap_list,
+                                                 int32_t k, int padding, const int32_t *pos_deg, const float *w_csr,
+                                                 const int64_t *excl_off, const int64_t *excl_pos, int32_t n_excl,
+                                                 int64_t *out_rowptr, void *workspace, size_t workspace_bytes,
+                                                 void *stream);
+int tfgk_block_sample_fill_weighted(const int64_t *rowptr, int32_t n_rows, const int32_t *col, const float *w_csr,
+                                    const int32_t *pos_deg, int32_t N, int32_t *nodes, int32_t *map, int32_t *state,
+                                    int32_t hop, int32_t n_hops, int32_t cap_list, int64_t cap_edges, int32_t k,
+                                    int padding, uint64_t seed, uint32_t rng_stream, const int64_t *out_rowptr,
+                                    int32_t *out_row, int32_t *out_local, int32_t *out_gcol, float *out_w,
+                                    void *workspace, size_t workspace_bytes, void *stream);
+int tfgk_block_sample_fill_weighted_excl(const int64_t *rowptr, int32_t n_rows, const int32_t *col, const float *w_csr,
+                                         const int32_t *pos_deg, int32_t N, int32_t *nodes, int32_t *map, int32_t *state,
+                                         int32_t hop, int32_t n_hops, int32_t cap_list, int64_t cap_edges, int32_t k,
+                                         int padding, uint64_t seed, uint32_t rng_stream, const int64_t *out_rowptr,
+                                         int32_t *out_row, int32_t *out_local, int32_t *out_gcol, float *out_w,
+                                         const int64_t *excl_off, const int32_t *excl_pos, int32_t n_excl,
+                                         void *workspace, size_t workspace_bytes, void *stream);
+int tfgk_block_sample_fill_weighted_mapped(const int64_t *rowptr, int32_t n_rows, const int32_t *col,
+                                           const float *w_csr, const int32_t *pos_deg, int32_t N, int32_t *nodes,
+                                           int32_t *map, int32_t *state, int32_t hop, int32_t n_hops, int32_t cap_list,
+                                           int64_t cap_edges, int32_t k, int padding, uint64_t seed, uint32_t rng_stream,
+                                           const int64_t *out_rowptr, int32_t *out_row, int32_t *out_local,
+                                           int32_t *out_gcol, float *out_w, void *workspace, size_t workspace_bytes,
+                                           void *stream);
+int tfgk_block_sample_fill_weighted_mapped_excl(const int64_t *rowptr, int32_t n_rows, const int32_t *col,
+                                                const float *w_csr, const int32_t *pos_deg, int32_t N, int32_t *nodes,
+                                                int32_t *map, int32_t *state, int32_t hop, int32_t n_hops,
+                                                int32_t cap_list, int64_t cap_edges, int32_t k, int padding,
+                                                uint64_t seed, uint32_t rng_stream, const int64_t *out_rowptr,
+                                                int32_t *out_row, int32_t *out_local, int32_t *out_gcol, float *out_w,
+                                                const int64_t *excl_off, const int64_t *excl_pos, int32_t n_excl,
+                                                void *workspace, size_t workspace_bytes, void *stream);
 int tfgk_block_gcn_values_excl_f32(const int64_t *rowptr, const int32_t *gcol, const float *w, int64_t S,
                                    const int32_t *dst, int32_t n_dst, const int64_t *g_rowptr, const float *g_rowsum,
                                    int norm, int loop, float deg_fill, float fill, const int64_t *excl_off,

@@ -169,6 +169,28 @@ SIGNATURES = {
                                            _ptr],
     "tfgk_block_gcn_values_excl_f32": [_ptr, _ptr, _ptr, _i64, _ptr, _i32, _ptr, _ptr, _int, _int, _f32, _f32, _ptr, _i32,
                                        _ptr, _ptr],
+    "tfgk_csr_positive_degree_f32": [_ptr, _i32, _ptr, _i64, _ptr, _ptr, _ptr],
+    "tfgk_neighbor_sample_rows_count_weighted": [_ptr, _i32, _ptr, _i32, _i32, _int, _ptr, _ptr, _ptr,
+                                                 ctypes.POINTER(_i64), _ptr, _size, _ptr],
+    "tfgk_neighbor_sample_rows_fill_weighted": [_ptr, _i32, _ptr, _i32, _i32, _int, _ptr, _ptr, _u64, _u32, _ptr, _ptr,
+                                                _ptr, _ptr],
+    "tfgk_block_sample_count_weighted": [_ptr, _i32, _ptr, _ptr, _i32, _i32, _i32, _i32, _int, _ptr, _ptr, _ptr, _ptr,
+                                         _size, _ptr],
+    "tfgk_block_sample_count_weighted_excl": [_ptr, _i32, _ptr, _ptr, _i32, _i32, _i32, _i32, _int, _ptr, _ptr, _ptr,
+                                              _ptr, _i32, _ptr, _ptr, _size, _ptr],
+    "tfgk_block_sample_count_weighted_mapped_excl": [_ptr, _i32, _ptr, _ptr, _i32, _i32, _i32, _i32, _int, _ptr, _ptr,
+                                                     _ptr, _ptr, _i32, _ptr, _ptr, _size, _ptr],
+    "tfgk_block_sample_fill_weighted": [_ptr, _i32, _ptr, _ptr, _ptr, _i32, _ptr, _ptr, _ptr, _i32, _i32, _i32, _i64,
+                                        _i32, _int, _u64, _u32, _ptr, _ptr, _ptr, _ptr, _ptr, _ptr, _size, _ptr],
+    "tfgk_block_sample_fill_weighted_excl": [_ptr, _i32, _ptr, _ptr, _ptr, _i32, _ptr, _ptr, _ptr, _i32, _i32, _i32,
+                                             _i64, _i32, _int, _u64, _u32, _ptr, _ptr, _ptr, _ptr, _ptr, _ptr, _ptr,
+                                             _i32, _ptr, _size, _ptr],
+    "tfgk_block_sample_fill_weighted_mapped": [_ptr, _i32, _ptr, _ptr, _ptr, _i32, _ptr, _ptr, _ptr, _i32, _i32, _i32,
+                                               _i64, _i32, _int, _u64, _u32, _ptr, _ptr, _ptr, _ptr, _ptr, _ptr, _size,
+                                               _ptr],
+    "tfgk_block_sample_fill_weighted_mapped_excl": [_ptr, _i32, _ptr, _ptr, _ptr, _i32, _ptr, _ptr, _ptr, _i32, _i32,
+                                                    _i32, _i64, _i32, _int, _u64, _u32, _ptr, _ptr, _ptr, _ptr, _ptr,
+                                                    _ptr, _ptr, _i32, _ptr, _size, _ptr],
     "tfgk_row_block_i32": [_ptr, _i32, _i32, _i32, _ptr, _i64, _ptr, _ptr, _ptr, _ptr, _ptr, ctypes.POINTER(_i32), _ptr,
                            _size, _ptr],
     "tfgk_copy_async": [_ptr, _ptr, _size, _ptr],
@@ -315,6 +337,14 @@ NOT_CAPTURABLE = {
     "tfgk_block_sample_fill_excl": ("the link block sampler", "it takes a host-side key"),
     "tfgk_block_sample_fill_mapped_excl": ("the host-memory link block sampler", "it takes a host-side key"),
     "tfgk_link_tail_negatives_i32": ("the link block sampler's negatives", "it takes a host-side key"),
+    "tfgk_neighbor_sample_rows_count_weighted": ("the weighted mini-batch neighbourhood sampler", "it returns the "
+                                                 "number of sampled edges to the host"),
+    "tfgk_neighbor_sample_rows_fill_weighted": ("the weighted mini-batch neighbourhood sampler", "it takes a host-side key"),
+    "tfgk_block_sample_fill_weighted": ("the weighted block sampler", "it takes a host-side key"),
+    "tfgk_block_sample_fill_weighted_excl": ("the weighted link block sampler", "it takes a host-side key"),
+    "tfgk_block_sample_fill_weighted_mapped": ("the weighted host-memory block sampler", "it takes a host-side key"),
+    "tfgk_block_sample_fill_weighted_mapped_excl": ("the weighted host-memory link block sampler",
+                                                    "it takes a host-side key"),
     "tfgk_block_exclusion_count": ("the link block sampler's exclusion lists", "it returns their total to the host"),
     "tfgk_row_block_i32": ("the row blocks of layer-wise inference", "it returns the number of source rows to the host"),
     "tfgk_host_register": ("HostFeatureTable", "it page-locks host memory, which a graph cannot record"),

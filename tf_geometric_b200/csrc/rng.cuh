@@ -66,6 +66,88 @@ __host__ __device__ __forceinline__ uint64_t random_below64(uint64_t seed, uint3
 #endif
 }
 
+// ---- weighted draws (include/tfgk.h, "weighted block sampler") ----------------------------------------------------
+// Every double operation below is rounded on its own (__dmul_rn and friends on the device, plain SSE2 arithmetic on the
+// host), so that no contraction into an FMA can change a bit and numpy float64 restates the routine exactly.
+__host__ __device__ __forceinline__ double rn_add(double a, double b) {
+#ifdef __CUDA_ARCH__
+    return __dadd_rn(a, b);
+#else
+    return a + b;
+#endif
+}
+__host__ __device__ __forceinline__ double rn_sub(double a, double b) {
+#ifdef __CUDA_ARCH__
+    return __dsub_rn(a, b);
+#else
+    return a - b;
+#endif
+}
+__host__ __device__ __forceinline__ double rn_mul(double a, double b) {
+#ifdef __CUDA_ARCH__
+    return __dmul_rn(a, b);
+#else
+    return a * b;
+#endif
+}
+__host__ __device__ __forceinline__ double rn_div(double a, double b) {
+#ifdef __CUDA_ARCH__
+    return __ddiv_rn(a, b);
+#else
+    return a / b;
+#endif
+}
+__host__ __device__ __forceinline__ uint64_t dbits(double x) {
+    union { double d; uint64_t u; } c;
+    c.d = x;
+    return c.u;
+}
+__host__ __device__ __forceinline__ double dfrom(uint64_t u) {
+    union { double d; uint64_t u; } c;
+    c.u = u;
+    return c.d;
+}
+
+// ln(u) for a positive normal double u, not the device libm: u = 2^e m with m in [sqrt(2)/2, sqrt(2)] by exact exponent
+// extraction, f = m - 1 (exact), s = f / (2 + f) and ln(m) = f - f^2/2 + s (f^2/2 + R(s^2)), with the degree-14 minimax
+// polynomial R and the split ln 2 of the classic fdlibm log (Sun Microsystems, 1993).  Within 2 ulp of math.log on (0, 1]
+// (tests/test_weighted_sampling_host.py).
+__host__ __device__ __forceinline__ double log_rn(double u) {
+    const double Lg1 = dfrom(0x3FE5555555555593ull), Lg2 = dfrom(0x3FD999999997FA04ull),
+                 Lg3 = dfrom(0x3FD2492494229359ull), Lg4 = dfrom(0x3FCC71C51D8E78AFull),
+                 Lg5 = dfrom(0x3FC7466496CB03DEull), Lg6 = dfrom(0x3FC39A09D078C69Full),
+                 Lg7 = dfrom(0x3FC2F112DF3E5244ull);
+    const double ln2_hi = dfrom(0x3FE62E42FEE00000ull), ln2_lo = dfrom(0x3DEA39EF35793C76ull);
+    const uint64_t b = dbits(u);
+    int e = (int)(b >> 52) - 1023;
+    uint64_t mb = (b & 0x000FFFFFFFFFFFFFull) | 0x3FF0000000000000ull;
+    if (mb > 0x3FF6A09E667F3BCDull) {                // m > sqrt(2): halve it (exact) and carry the factor into e
+        mb -= 1ull << 52;
+        e += 1;
+    }
+    const double f = rn_sub(dfrom(mb), 1.0);
+    const double s = rn_div(f, rn_add(2.0, f));
+    const double z = rn_mul(s, s), w = rn_mul(z, z);
+    const double t1 = rn_mul(w, rn_add(Lg2, rn_mul(w, rn_add(Lg4, rn_mul(w, Lg6)))));
+    const double t2 = rn_mul(z, rn_add(Lg1, rn_mul(w, rn_add(Lg3, rn_mul(w, rn_add(Lg5, rn_mul(w, Lg7)))))));
+    const double R = rn_add(t2, t1);
+    const double hfsq = rn_mul(0.5, rn_mul(f, f));
+    const double dk = (double)e;
+    return rn_sub(rn_mul(dk, ln2_hi),
+                  rn_sub(rn_sub(hfsq, rn_add(rn_mul(s, rn_add(hfsq, R)), rn_mul(dk, ln2_lo))), f));
+}
+
+// The Efraimidis-Spirakis key of entry v (virtual position) of global row r, draw j, weight w > 0: one Philox block
+// with counter (v, r, stream, j), u = ((lanes 0 | 1 << 32) >> 11) + 1) 2^-53 in (0, 1], E = -ln(u) / w in double.
+// Returned as the bits of E with the sign cleared (E = -0.0 at u = 1): non-negative doubles order as their bits.
+__host__ __device__ __forceinline__ uint64_t weighted_key(uint64_t seed, uint32_t stream, uint32_t v, uint32_t r,
+                                                          uint32_t j, float w) {
+    const Philox4 x = philox4x32_10(v, r, stream, j, (uint32_t)seed, (uint32_t)(seed >> 32));
+    const uint64_t u64 = (uint64_t)x.v[0] | ((uint64_t)x.v[1] << 32);
+    const double u = rn_mul((double)((u64 >> 11) + 1), 1.1102230246251565e-16);      // 2^-53
+    return dbits(rn_div(-log_rn(u), (double)w)) & 0x7FFFFFFFFFFFFFFFull;
+}
+
 // splitmix64's output function (Steele, Lea and Flood, "Fast splittable pseudorandom number generators", OOPSLA'14):
 // the same mix as tf_geometric_b200/_rng.py applies to its keys
 __host__ __device__ __forceinline__ uint64_t splitmix64(uint64_t z) {

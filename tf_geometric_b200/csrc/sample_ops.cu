@@ -424,6 +424,423 @@ block_fill_mapped_excl_kernel(const int64_t *__restrict__ rowptr, int32_t n_rows
                                                n_excl);
 }
 
+// ---- weighted fan-outs (include/tfgk.h, "weighted block sampler") -------------------------------------------------
+// A listed row's candidates are its kept entries with weight > 0, numbered by virtual position v as excl_real numbers
+// them; d+ counts them.  Without replacement the draw is the num = min(k, d+) candidates of smallest (E, v), E the key of
+// weighted_key with j = 0, written in ascending CSR position; with padding and k >= d+, draw j is the candidate of smallest
+// (E_j, v) with j + 1 in the key's counter.  (E, v) and (E, p) order the same way, since v grows with the real position p.
+constexpr int kWeightedRowsPerCta = 64;        // rows per CTA: eight per warp
+constexpr int kWarps = kRowsPerCta / 32;
+constexpr int kWarpSlots = kThreadRowMax / 32;  // a row of up to kThreadRowMax entries is held by one warp, 4 per lane
+constexpr uint64_t kNoKey = ~0ull;              // above every key (keys have no sign bit): entries that cannot be drawn
+enum { kWeightedNone = 0, kWeightedAll = 1, kWeightedReplace = 2, kWeightedSelect = 3 };
+
+// sample_rule on d+ for an integer fan-out k >= 0 and padding 0 / 1
+__device__ __forceinline__ int weighted_rule(int dplus, int k, int padding, int &num) {
+    sample_rule(dplus, k, -1.0, padding, num);
+    if (num == 0) return kWeightedNone;
+    if (padding && k >= dplus) return kWeightedReplace;
+    return num == dplus ? kWeightedAll : kWeightedSelect;
+}
+
+// d+ of list row t (global row r): the row's positive entries less its excluded entries of positive weight
+template <typename TPos, bool kExcl>
+__device__ __forceinline__ int positive_degree(const int32_t *__restrict__ pos_deg, int32_t r,
+                                               const float *__restrict__ w_csr, int64_t t,
+                                               const int64_t *__restrict__ excl_off, const TPos *__restrict__ excl_pos,
+                                               int32_t n_excl) {
+    int d = pos_deg[r];
+    if constexpr (kExcl)
+        if (t < n_excl)
+            for (int64_t j = excl_off[t]; j < excl_off[t + 1]; ++j) d -= w_csr[excl_pos[j]] > 0.0f ? 1 : 0;
+    return d;
+}
+
+template <typename TPos>
+struct WeightedRow {
+    int64_t t, start, end, o;
+    int32_t r;
+    int x, num, rule;
+    const TPos *ex;
+};
+
+template <typename TPos, bool kExcl>
+__device__ __forceinline__ WeightedRow<TPos> weighted_row(int64_t t, int32_t r, const int64_t *__restrict__ rowptr,
+                                                          const int32_t *__restrict__ pos_deg,
+                                                          const float *__restrict__ w_csr, int k, int padding,
+                                                          const int64_t *__restrict__ out_rowptr,
+                                                          const int64_t *__restrict__ excl_off,
+                                                          const TPos *__restrict__ excl_pos, int32_t n_excl) {
+    WeightedRow<TPos> R;
+    R.t = t;
+    R.r = r;
+    R.start = rowptr[r];
+    R.end = rowptr[r + 1];
+    R.o = out_rowptr[t];
+    R.x = kExcl ? excl_count(excl_off, n_excl, t) : 0;
+    R.ex = kExcl && R.x ? excl_pos + excl_off[t] : nullptr;
+    R.rule = weighted_rule(positive_degree<TPos, kExcl>(pos_deg, r, w_csr, t, excl_off, excl_pos, n_excl), k, padding,
+                           R.num);
+    return R;
+}
+
+// the weight of the entry at real position p (0 when it is excluded) and its virtual position v
+template <typename TPos, bool kExcl>
+__device__ __forceinline__ float entry_weight(const WeightedRow<TPos> &R, const float *__restrict__ w_csr, int64_t p,
+                                              uint32_t &v) {
+    int before = 0;
+    bool hit = false;
+    if constexpr (kExcl)
+        if (R.x) {
+            int lo = 0, hi = R.x;
+            while (lo < hi) {
+                const int mid = (lo + hi) >> 1;
+                if ((int64_t)R.ex[mid] < p) lo = mid + 1;
+                else hi = mid;
+            }
+            before = lo;
+            hit = lo < R.x && (int64_t)R.ex[lo] == p;
+        }
+    v = (uint32_t)(p - R.start - before);
+    return hit ? 0.0f : w_csr[p];
+}
+
+template <bool kBlock, typename TPos>
+__device__ __forceinline__ void weighted_emit(const WeightedRow<TPos> &R, int64_t slot, int64_t p, float w,
+                                              int32_t *__restrict__ out_row, TPos *__restrict__ out_pos,
+                                              const int32_t *__restrict__ csr_col, int32_t *__restrict__ out_gcol,
+                                              float *__restrict__ out_w) {
+    const int64_t o = R.o + slot;
+    if (out_row) out_row[o] = (int32_t)R.t;
+    out_pos[o] = (TPos)p;
+    if constexpr (kBlock) {
+        out_gcol[o] = csr_col[p];
+        out_w[o] = w;
+    }
+}
+
+// (a, pa) < (b, pb) lexicographically
+__device__ __forceinline__ bool key_less(uint64_t a, int64_t pa, uint64_t b, int64_t pb) {
+    return a < b || (a == b && pa < pb);
+}
+
+// exclusive count of `flag` over the CTA in thread order; *total gets the CTA's count
+__device__ __forceinline__ int cta_exclusive_count(bool flag, int *s_warp, int &total) {
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const unsigned m = __ballot_sync(0xffffffffu, flag);
+    if (lane == 0) s_warp[warp] = __popc(m);
+    __syncthreads();
+    int before = 0;
+    total = 0;
+#pragma unroll
+    for (int w = 0; w < kWarps; ++w) {
+        const int c = s_warp[w];
+        if (w < warp) before += c;
+        total += c;
+    }
+    __syncthreads();                   // s_warp is reused by the next call
+    return before + __popc(m & ((1u << lane) - 1u));
+}
+
+// a row of at most kThreadRowMax entries on one warp: weights read once, in 128-byte segments, and kept in registers
+template <bool kBlock, typename TPos, bool kExcl>
+__device__ __forceinline__ void weighted_warp_row(const WeightedRow<TPos> &R, const float *__restrict__ w_csr,
+                                                  uint64_t seed, uint32_t stream, int32_t *__restrict__ out_row,
+                                                  TPos *__restrict__ out_pos, const int32_t *__restrict__ csr_col,
+                                                  int32_t *__restrict__ out_gcol, float *__restrict__ out_w) {
+    const int lane = threadIdx.x & 31;
+    const int nchunks = (int)((R.end - R.start + 31) >> 5);
+    float wt[kWarpSlots];
+    uint32_t vv[kWarpSlots];
+#pragma unroll
+    for (int i = 0; i < kWarpSlots; ++i) {
+        const int64_t p = R.start + lane + 32 * i;
+        wt[i] = 0.0f;
+        vv[i] = 0;
+        if (i < nchunks && p < R.end) wt[i] = entry_weight<TPos, kExcl>(R, w_csr, p, vv[i]);
+    }
+    if (R.rule == kWeightedReplace) {
+        for (int j = 0; j < R.num; ++j) {
+            uint64_t best = kNoKey;
+            int64_t bp = INT64_MAX;
+            float bw = 0.0f;
+#pragma unroll
+            for (int i = 0; i < kWarpSlots; ++i)
+                if (wt[i] > 0.0f) {
+                    const uint64_t key = weighted_key(seed, stream, vv[i], (uint32_t)R.r, (uint32_t)j + 1u, wt[i]);
+                    if (key < best) {          // positions grow with i: a tie keeps the earlier one
+                        best = key;
+                        bp = lane + 32 * i;
+                        bw = wt[i];
+                    }
+                }
+#pragma unroll
+            for (int off = 16; off > 0; off >>= 1) {
+                const uint64_t ok = __shfl_xor_sync(0xffffffffu, best, off);
+                const int64_t op = __shfl_xor_sync(0xffffffffu, bp, off);
+                const float ow = __shfl_xor_sync(0xffffffffu, bw, off);
+                if (key_less(ok, op, best, bp)) {
+                    best = ok;
+                    bp = op;
+                    bw = ow;
+                }
+            }
+            if (lane == 0)
+                weighted_emit<kBlock, TPos>(R, j, R.start + bp, bw, out_row, out_pos, csr_col, out_gcol, out_w);
+        }
+        return;
+    }
+    bool sel[kWarpSlots];
+    if (R.rule == kWeightedSelect) {
+        uint64_t key[kWarpSlots];
+        int rank[kWarpSlots];
+#pragma unroll
+        for (int i = 0; i < kWarpSlots; ++i) {
+            key[i] = wt[i] > 0.0f ? weighted_key(seed, stream, vv[i], (uint32_t)R.r, 0u, wt[i]) : kNoKey;
+            rank[i] = 0;
+        }
+        // rank of every entry among the row's: the number of entries of smaller (key, position)
+#pragma unroll
+        for (int i2 = 0; i2 < kWarpSlots; ++i2) {
+            if (i2 >= nchunks) break;
+            for (int s = 0; s < 32; ++s) {
+                const uint64_t kb = __shfl_sync(0xffffffffu, key[i2], s);
+                const int pb = s + 32 * i2;
+#pragma unroll
+                for (int i = 0; i < kWarpSlots; ++i) rank[i] += key_less(kb, pb, key[i], lane + 32 * i) ? 1 : 0;
+            }
+        }
+#pragma unroll
+        for (int i = 0; i < kWarpSlots; ++i) sel[i] = key[i] != kNoKey && rank[i] < R.num;
+    } else {
+#pragma unroll
+        for (int i = 0; i < kWarpSlots; ++i) sel[i] = wt[i] > 0.0f;
+    }
+    int base = 0;
+#pragma unroll
+    for (int i = 0; i < kWarpSlots; ++i) {
+        const unsigned m = __ballot_sync(0xffffffffu, sel[i]);
+        if (sel[i])
+            weighted_emit<kBlock, TPos>(R, base + __popc(m & ((1u << lane) - 1u)), R.start + lane + 32 * i, wt[i],
+                                        out_row, out_pos, csr_col, out_gcol, out_w);
+        base += __popc(m);
+    }
+}
+
+struct WeightedShared {
+    int hist[256];
+    int warp_count[kWarps];
+    uint64_t key[kWarps];
+    int64_t pos[kWarps];
+    float w[kWarps];
+    uint64_t prefix;
+    int need, done;
+};
+
+// a longer row on the whole CTA.  Without replacement: a radix select of the num smallest keys, eight bits a pass from
+// the top, each pass recomputing the keys from their counters (no workspace grows with the row), stopping once the
+// bucket of the num-th key is taken whole; then one ordered pass writes the entries below the found prefix and, of those
+// equal to it (ties after all 64 bits only), the first in position order.  With replacement: one CTA argmin per draw.
+template <bool kBlock, typename TPos, bool kExcl>
+__device__ __forceinline__ void weighted_cta_row(const WeightedRow<TPos> &R, const float *__restrict__ w_csr,
+                                                 uint64_t seed, uint32_t stream, WeightedShared &sh,
+                                                 int32_t *__restrict__ out_row, TPos *__restrict__ out_pos,
+                                                 const int32_t *__restrict__ csr_col, int32_t *__restrict__ out_gcol,
+                                                 float *__restrict__ out_w) {
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    if (R.rule == kWeightedReplace) {
+        for (int j = 0; j < R.num; ++j) {
+            uint64_t best = kNoKey;
+            int64_t bp = INT64_MAX;
+            float bw = 0.0f;
+            for (int64_t p = R.start + threadIdx.x; p < R.end; p += kRowsPerCta) {
+                uint32_t v;
+                const float w = entry_weight<TPos, kExcl>(R, w_csr, p, v);
+                if (w > 0.0f) {
+                    const uint64_t key = weighted_key(seed, stream, v, (uint32_t)R.r, (uint32_t)j + 1u, w);
+                    if (key < best) {
+                        best = key;
+                        bp = p;
+                        bw = w;
+                    }
+                }
+            }
+#pragma unroll
+            for (int off = 16; off > 0; off >>= 1) {
+                const uint64_t ok = __shfl_xor_sync(0xffffffffu, best, off);
+                const int64_t op = __shfl_xor_sync(0xffffffffu, bp, off);
+                const float ow = __shfl_xor_sync(0xffffffffu, bw, off);
+                if (key_less(ok, op, best, bp)) {
+                    best = ok;
+                    bp = op;
+                    bw = ow;
+                }
+            }
+            if (lane == 0) {
+                sh.key[warp] = best;
+                sh.pos[warp] = bp;
+                sh.w[warp] = bw;
+            }
+            __syncthreads();
+            if (threadIdx.x == 0) {
+                for (int w = 1; w < kWarps; ++w)
+                    if (key_less(sh.key[w], sh.pos[w], best, bp)) {
+                        best = sh.key[w];
+                        bp = sh.pos[w];
+                        bw = sh.w[w];
+                    }
+                weighted_emit<kBlock, TPos>(R, j, bp, bw, out_row, out_pos, csr_col, out_gcol, out_w);
+            }
+            __syncthreads();
+        }
+        return;
+    }
+    uint64_t prefix = 0;
+    int shift = 64, need = R.num;
+    if (R.rule == kWeightedSelect) {
+        for (int s = 56; s >= 0; s -= 8) {
+            sh.hist[threadIdx.x] = 0;
+            __syncthreads();
+            for (int64_t p = R.start + threadIdx.x; p < R.end; p += kRowsPerCta) {
+                uint32_t v;
+                const float w = entry_weight<TPos, kExcl>(R, w_csr, p, v);
+                if (w > 0.0f) {
+                    const uint64_t key = weighted_key(seed, stream, v, (uint32_t)R.r, 0u, w);
+                    if (s == 56 || (key >> (s + 8)) == prefix) atomicAdd(&sh.hist[(key >> s) & 255], 1);
+                }
+            }
+            __syncthreads();
+            if (threadIdx.x == 0) {
+                int b = 0, cum = 0;
+                while (cum + sh.hist[b] < need) cum += sh.hist[b++];
+                sh.prefix = (prefix << 8) | (uint64_t)b;
+                sh.need = need - cum;
+                sh.done = sh.hist[b] == need - cum;
+            }
+            __syncthreads();
+            prefix = sh.prefix;
+            need = sh.need;
+            shift = s;
+            const bool done = sh.done;
+            __syncthreads();               // every thread has read the pass's result before the next one writes it
+            if (done) break;
+        }
+    }
+    int64_t base = 0;
+    int eq_base = 0;
+    for (int64_t c = R.start; c < R.end; c += kRowsPerCta) {
+        const int64_t p = c + threadIdx.x;
+        bool lt = false, eq = false;
+        float w = 0.0f;
+        if (p < R.end) {
+            uint32_t v;
+            w = entry_weight<TPos, kExcl>(R, w_csr, p, v);
+            if (w > 0.0f) {
+                if (R.rule == kWeightedAll) {
+                    lt = true;
+                } else {
+                    const uint64_t kp = weighted_key(seed, stream, v, (uint32_t)R.r, 0u, w) >> shift;
+                    lt = kp < prefix;
+                    eq = kp == prefix;
+                }
+            }
+        }
+        int n_eq, n_sel;
+        const int eq_rank = eq_base + cta_exclusive_count(eq, sh.warp_count, n_eq);
+        const bool sel = lt || (eq && eq_rank < need);
+        const int slot = cta_exclusive_count(sel, sh.warp_count, n_sel);
+        if (sel) weighted_emit<kBlock, TPos>(R, base + slot, p, w, out_row, out_pos, csr_col, out_gcol, out_w);
+        eq_base += n_eq;
+        base += n_sel;
+    }
+}
+
+// The weighted fill: kWeightedRowsPerCta listed rows per CTA, a warp per row up to kThreadRowMax entries, then the
+// longer rows one after another on the whole CTA.  n_list_dev (the block sampler's device count) overrides n_list.
+// The explicit minimum of one CTA per SM lets ptxas take the 74-80 registers the keys need: left to itself it chose 64
+// and spilled 4-20 bytes.
+template <bool kBlock, typename TPos, bool kExcl>
+__global__ void __launch_bounds__(kRowsPerCta, 1)
+weighted_fill_kernel(const int64_t *__restrict__ rowptr, int32_t n_rows, const int32_t *__restrict__ rows,
+                     const int32_t *__restrict__ n_list_dev, int32_t n_list, int k, int padding,
+                     const int32_t *__restrict__ pos_deg, const float *__restrict__ w_csr, uint64_t seed, uint32_t stream,
+                     const int64_t *__restrict__ out_rowptr, int32_t *__restrict__ out_row, TPos *__restrict__ out_pos,
+                     const int32_t *__restrict__ csr_col, int32_t *__restrict__ out_gcol, float *__restrict__ out_w,
+                     const int64_t *__restrict__ excl_off, const TPos *__restrict__ excl_pos, int32_t n_excl) {
+    __shared__ int32_t long_rows[kWeightedRowsPerCta];
+    __shared__ int n_long;
+    __shared__ WeightedShared sh;
+    if (n_list_dev) n_list = *n_list_dev;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    if (threadIdx.x == 0) n_long = 0;
+    __syncthreads();
+    for (int q = warp; q < kWeightedRowsPerCta; q += kWarps) {
+        const int64_t t = (int64_t)blockIdx.x * kWeightedRowsPerCta + q;
+        if (t >= n_list) break;
+        const int32_t r = rows[t];
+        if (r < 0 || r >= n_rows) continue;
+        const WeightedRow<TPos> R = weighted_row<TPos, kExcl>(t, r, rowptr, pos_deg, w_csr, k, padding, out_rowptr,
+                                                              excl_off, excl_pos, n_excl);
+        if (R.rule == kWeightedNone) continue;
+        if (R.end - R.start > kThreadRowMax) {
+            if (lane == 0) long_rows[atomicAdd(&n_long, 1)] = q;     // rows write disjoint ranges: any order
+            continue;
+        }
+        weighted_warp_row<kBlock, TPos, kExcl>(R, w_csr, seed, stream, out_row, out_pos, csr_col, out_gcol, out_w);
+    }
+    __syncthreads();
+    const int nl = n_long;
+    for (int i = 0; i < nl; ++i) {
+        const int64_t t = (int64_t)blockIdx.x * kWeightedRowsPerCta + long_rows[i];
+        const WeightedRow<TPos> R = weighted_row<TPos, kExcl>(t, rows[t], rowptr, pos_deg, w_csr, k, padding, out_rowptr,
+                                                              excl_off, excl_pos, n_excl);
+        weighted_cta_row<kBlock, TPos, kExcl>(R, w_csr, seed, stream, sh, out_row, out_pos, csr_col, out_gcol, out_w);
+    }
+}
+
+// per-row counts of the weighted rule; K13's form (n_list on the host, listed rows outside [0, n_rows) counted in n_bad)
+// when n_bad is set, the block sampler's otherwise (rows past the device count contribute 0)
+template <typename TPos, bool kExcl>
+__global__ void weighted_count_kernel(const int64_t *__restrict__ rowptr, int32_t n_rows, const int32_t *__restrict__ rows,
+                                      const int32_t *__restrict__ n_list_dev, int32_t cap, int k, int padding,
+                                      const int32_t *__restrict__ pos_deg, const float *__restrict__ w_csr,
+                                      int32_t *__restrict__ cnt, int32_t *__restrict__ n_bad,
+                                      const int64_t *__restrict__ excl_off, const TPos *__restrict__ excl_pos,
+                                      int32_t n_excl) {
+    const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= cap) return;
+    int num = 0;
+    if (!n_list_dev || t < *n_list_dev) {
+        const int32_t r = rows[t];
+        if (r >= 0 && r < n_rows)
+            weighted_rule(positive_degree<TPos, kExcl>(pos_deg, r, w_csr, t, excl_off, excl_pos, n_excl), k, padding,
+                          num);
+        else if (n_bad)
+            atomicAdd(n_bad, 1);
+    }
+    cnt[t] = num;
+}
+
+// one warp per row: the entries of weight > 0, and (atomically, into n_invalid) those negative, NaN or infinite
+__global__ void positive_degree_kernel(const int64_t *__restrict__ rowptr, int32_t n_rows, const float *__restrict__ w,
+                                       int64_t w_base, int32_t *__restrict__ pos_deg, int32_t *__restrict__ n_invalid) {
+    const int64_t r = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const int lane = threadIdx.x & 31;
+    if (r >= n_rows) return;                    // whole warps
+    int pos = 0, bad = 0;
+    for (int64_t p = rowptr[r] + lane; p < rowptr[r + 1]; p += 32) {
+        const float x = w[p - w_base];
+        pos += x > 0.0f && x <= FLT_MAX ? 1 : 0;
+        bad += !(x >= 0.0f && x <= FLT_MAX) ? 1 : 0;
+    }
+    pos = __reduce_add_sync(0xffffffffu, pos);
+    bad = __reduce_add_sync(0xffffffffu, bad);
+    if (lane == 0) {
+        pos_deg[r] = pos;
+        if (bad) atomicAdd(n_invalid, bad);
+    }
+}
+
 __global__ void block_first_kernel(const int32_t *__restrict__ cols, const int64_t *__restrict__ S, int32_t N,
                                    int32_t *__restrict__ map, int32_t *__restrict__ counters) {
     const int64_t n = *S;
@@ -819,6 +1236,79 @@ int tfgk_neighbor_sample_rows_fill(const int64_t *rowptr, int32_t n_rows, const 
     return TFGK_OK;
 }
 
+int tfgk_neighbor_sample_rows_count_weighted(const int64_t *rowptr, int32_t n_rows, const int32_t *rows, int32_t n_list,
+                                             int32_t k, int padding, const int32_t *pos_deg, const float *w_csr,
+                                             int64_t *out_rowptr, int64_t *total_host, void *workspace,
+                                             size_t workspace_bytes, void *stream) {
+    TFGK_CHECK_ARG(n_rows >= 0 && n_list >= 0, "neighbor_sample_rows_count_weighted: bad size");
+    TFGK_CHECK_ARG(k >= 0 && (padding == 0 || padding == 1), "neighbor_sample_rows_count_weighted: the weighted rule "
+                   "takes an integer fan-out and padding 0 or 1");
+    TFGK_CHECK_ARG(total_host != nullptr && out_rowptr != nullptr, "neighbor_sample_rows_count_weighted: null pointer");
+    *total_host = 0;
+    cudaStream_t st = as_stream(stream);
+    if (n_list == 0) {
+        TFGK_CUDA(cudaMemsetAsync(out_rowptr, 0, 8, st));
+        return TFGK_OK;
+    }
+    TFGK_CHECK_ARG(rowptr && rows && pos_deg && w_csr, "neighbor_sample_rows_count_weighted: null pointer");
+    size_t need = 0;
+    tfgk_neighbor_sample_workspace_bytes(n_list, &need);
+    if (workspace == nullptr || workspace_bytes < need)
+        return set_error(TFGK_ERR_WORKSPACE, "neighbor_sample_rows_count_weighted: workspace too small (%zu < %zu bytes)",
+                         workspace_bytes, need);
+    char *ws = static_cast<char *>(workspace);
+    int32_t *cnt = reinterpret_cast<int32_t *>(ws);
+    int64_t *sums = reinterpret_cast<int64_t *>(ws + align_up(((size_t)n_list + 1) * 4));
+    int32_t *n_bad = reinterpret_cast<int32_t *>(ws + need - 256);
+    TFGK_CUDA(cudaMemsetAsync(n_bad, 0, 4, st));
+    weighted_count_kernel<int32_t, false><<<(unsigned)ceil_div64(n_list, 256), 256, 0, st>>>(
+        rowptr, n_rows, rows, nullptr, n_list, k, padding, pos_deg, w_csr, cnt, n_bad, nullptr, nullptr, 0);
+    TFGK_LAUNCH_CHECK();
+    int rc = exclusive_scan<int32_t, int64_t>(cnt, n_list, (int64_t)n_list + 1, out_rowptr, sums, st);
+    if (rc != TFGK_OK) return rc;
+    int32_t bad = 0;
+    TFGK_CUDA(cudaMemcpyAsync(total_host, out_rowptr + n_list, 8, cudaMemcpyDeviceToHost, st));
+    TFGK_CUDA(cudaMemcpyAsync(&bad, n_bad, 4, cudaMemcpyDeviceToHost, st));
+    TFGK_CUDA(cudaStreamSynchronize(st));
+    if (bad) {
+        *total_host = 0;
+        return set_error(TFGK_ERR_INDEX_OUT_OF_RANGE, "neighbor_sample_rows_count_weighted: %d listed rows outside [0, %d)",
+                         bad, n_rows);
+    }
+    TFGK_CHECK_ARG(*total_host < (1ll << 31) - 1, "neighbor_sample_rows_count_weighted: %lld sampled edges exceed int32 "
+                   "positions", (long long)*total_host);
+    return TFGK_OK;
+}
+
+int tfgk_neighbor_sample_rows_fill_weighted(const int64_t *rowptr, int32_t n_rows, const int32_t *rows, int32_t n_list,
+                                            int32_t k, int padding, const int32_t *pos_deg, const float *w_csr,
+                                            uint64_t seed, uint32_t rng_stream, const int64_t *out_rowptr,
+                                            int32_t *out_row, int32_t *out_pos, void *stream) {
+    TFGK_CHECK_ARG(n_rows >= 0 && n_list >= 0, "neighbor_sample_rows_fill_weighted: bad size");
+    TFGK_CHECK_ARG(k >= 0 && (padding == 0 || padding == 1), "neighbor_sample_rows_fill_weighted: the weighted rule "
+                   "takes an integer fan-out and padding 0 or 1");
+    if (n_list == 0) return TFGK_OK;
+    TFGK_CHECK_ARG(rowptr && rows && pos_deg && w_csr && out_rowptr && out_pos,
+                   "neighbor_sample_rows_fill_weighted: null pointer");
+    weighted_fill_kernel<false, int32_t, false><<<(unsigned)ceil_div64(n_list, kWeightedRowsPerCta), kRowsPerCta, 0,
+                                                  as_stream(stream)>>>(
+        rowptr, n_rows, rows, nullptr, n_list, k, padding, pos_deg, w_csr, seed, rng_stream, out_rowptr, out_row, out_pos,
+        nullptr, nullptr, nullptr, nullptr, nullptr, 0);
+    TFGK_LAUNCH_CHECK();
+    return TFGK_OK;
+}
+
+int tfgk_csr_positive_degree_f32(const int64_t *rowptr, int32_t n_rows, const float *w, int64_t w_base,
+                                 int32_t *pos_deg, int32_t *n_invalid, void *stream) {
+    TFGK_CHECK_ARG(n_rows >= 0 && w_base >= 0, "csr_positive_degree: bad size");
+    if (n_rows == 0) return TFGK_OK;
+    TFGK_CHECK_ARG(rowptr && w && pos_deg && n_invalid, "csr_positive_degree: null pointer");
+    positive_degree_kernel<<<(unsigned)ceil_div64((int64_t)n_rows * 32, 256), 256, 0, as_stream(stream)>>>(
+        rowptr, n_rows, w, w_base, pos_deg, n_invalid);
+    TFGK_LAUNCH_CHECK();
+    return TFGK_OK;
+}
+
 int tfgk_relabel_workspace_bytes(int64_t n_ids, size_t *out_bytes) {
     TFGK_CHECK_ARG(out_bytes != nullptr && n_ids >= 0 && n_ids < (1ll << 31) - 1, "relabel_workspace_bytes: bad argument");
     *out_bytes = 2 * align_up((size_t)(n_ids + 1) * 4) + scan_scratch_bytes(n_ids + 1) + 256;
@@ -979,11 +1469,14 @@ int tfgk_block_sample_begin(const int32_t *seeds, int32_t n_seeds, int32_t N, in
 
 }  // extern "C"
 
-// tfgk_block_sample_count and _count_excl (excl_off null: no exclusions)
+// tfgk_block_sample_count, _count_excl (excl_off null: no exclusions) and their _weighted twins (pos_deg set: the
+// weighted rule over d+, which reads the weights w_csr at the excluded positions excl_pos)
+template <typename TPos = int32_t>
 static int block_sample_count(const char *fn, const int64_t *rowptr, int32_t n_rows, const int32_t *nodes,
                               const int32_t *state, int32_t hop, int32_t n_hops, int32_t cap_list, int32_t k, int padding,
                               const int64_t *excl_off, int32_t n_excl, int64_t *out_rowptr, void *workspace,
-                              size_t workspace_bytes, void *stream) {
+                              size_t workspace_bytes, void *stream, const int32_t *pos_deg = nullptr,
+                              const float *w_csr = nullptr, const TPos *excl_pos = nullptr) {
     int rc = check_sample_mode(fn, k, -1.0, padding);
     if (rc != TFGK_OK) return rc;
     TFGK_CHECK_ARG(n_rows >= 0 && hop >= 0 && hop < n_hops && cap_list >= 0 && n_excl >= 0, "%s: bad size", fn);
@@ -999,7 +1492,19 @@ static int block_sample_count(const char *fn, const int64_t *rowptr, int32_t n_r
     const BlockWorkspace L(cap_list, 0);
     int32_t *cnt = reinterpret_cast<int32_t *>(ws);
     const unsigned grid = (unsigned)ceil_div64(cap_list, 256);
-    if (excl_off)
+    if (pos_deg) {
+        TFGK_CHECK_ARG(k >= 0 && padding != TFGK_SAMPLE_HEAD, "%s: the weighted rule takes an integer fan-out and no "
+                       "head rule", fn);
+        TFGK_CHECK_ARG(!excl_off || (w_csr && excl_pos), "%s: null weights or exclusion list", fn);
+        if (excl_off)
+            weighted_count_kernel<TPos, true><<<grid, 256, 0, st>>>(rowptr, n_rows, nodes, state + kStateSizes + hop,
+                                                                    cap_list, k, padding, pos_deg, w_csr, cnt, nullptr,
+                                                                    excl_off, excl_pos, n_excl);
+        else
+            weighted_count_kernel<TPos, false><<<grid, 256, 0, st>>>(rowptr, n_rows, nodes, state + kStateSizes + hop,
+                                                                     cap_list, k, padding, pos_deg, w_csr, cnt, nullptr,
+                                                                     nullptr, nullptr, 0);
+    } else if (excl_off)
         block_count_excl_kernel<<<grid, 256, 0, st>>>(rowptr, n_rows, nodes, state + kStateSizes + hop, cap_list, k,
                                                       padding, cnt, excl_off, n_excl);
     else
@@ -1028,6 +1533,41 @@ int tfgk_block_sample_count_excl(const int64_t *rowptr, int32_t n_rows, const in
                               excl_off, n_excl, out_rowptr, workspace, workspace_bytes, stream);
 }
 
+int tfgk_block_sample_count_weighted(const int64_t *rowptr, int32_t n_rows, const int32_t *nodes, const int32_t *state,
+                                     int32_t hop, int32_t n_hops, int32_t cap_list, int32_t k, int padding,
+                                     const int32_t *pos_deg, const float *w_csr, int64_t *out_rowptr, void *workspace,
+                                     size_t workspace_bytes, void *stream) {
+    TFGK_CHECK_ARG(pos_deg != nullptr, "block_sample_count_weighted: null positive degrees");
+    return block_sample_count<int32_t>("block_sample_count_weighted", rowptr, n_rows, nodes, state, hop, n_hops,
+                                       cap_list, k, padding, nullptr, 0, out_rowptr, workspace, workspace_bytes, stream,
+                                       pos_deg, w_csr, nullptr);
+}
+
+int tfgk_block_sample_count_weighted_excl(const int64_t *rowptr, int32_t n_rows, const int32_t *nodes,
+                                          const int32_t *state, int32_t hop, int32_t n_hops, int32_t cap_list, int32_t k,
+                                          int padding, const int32_t *pos_deg, const float *w_csr,
+                                          const int64_t *excl_off, const int32_t *excl_pos, int32_t n_excl,
+                                          int64_t *out_rowptr, void *workspace, size_t workspace_bytes, void *stream) {
+    TFGK_CHECK_ARG(pos_deg != nullptr && excl_off != nullptr, "block_sample_count_weighted_excl: null positive degrees "
+                   "or exclusion offsets");
+    return block_sample_count<int32_t>("block_sample_count_weighted_excl", rowptr, n_rows, nodes, state, hop, n_hops,
+                                       cap_list, k, padding, excl_off, n_excl, out_rowptr, workspace, workspace_bytes,
+                                       stream, pos_deg, w_csr, excl_pos);
+}
+
+int tfgk_block_sample_count_weighted_mapped_excl(const int64_t *rowptr, int32_t n_rows, const int32_t *nodes,
+                                                 const int32_t *state, int32_t hop, int32_t n_hops, int32_t cap_list,
+                                                 int32_t k, int padding, const int32_t *pos_deg, const float *w_csr,
+                                                 const int64_t *excl_off, const int64_t *excl_pos, int32_t n_excl,
+                                                 int64_t *out_rowptr, void *workspace, size_t workspace_bytes,
+                                                 void *stream) {
+    TFGK_CHECK_ARG(pos_deg != nullptr && excl_off != nullptr, "block_sample_count_weighted_mapped_excl: null positive "
+                   "degrees or exclusion offsets");
+    return block_sample_count<int64_t>("block_sample_count_weighted_mapped_excl", rowptr, n_rows, nodes, state, hop,
+                                       n_hops, cap_list, k, padding, excl_off, n_excl, out_rowptr, workspace,
+                                       workspace_bytes, stream, pos_deg, w_csr, excl_pos);
+}
+
 int tfgk_block_sample_read_total(const int32_t *state, int32_t hop, const int64_t *out_rowptr, int32_t cap_list,
                                  int32_t *n_list_host, int64_t *total_host, void *stream) {
     TFGK_CHECK_ARG(state && out_rowptr && n_list_host && total_host && hop >= 0 && cap_list >= 0,
@@ -1051,10 +1591,13 @@ static int block_sample_fill(const char *fn, const int64_t *rowptr, int32_t n_ro
                              int32_t n_hops, int32_t cap_list, int64_t cap_edges, int32_t k, int padding, uint64_t seed,
                              uint32_t rng_stream, const int64_t *out_rowptr, int32_t *out_row, int32_t *out_local,
                              int32_t *out_gcol, float *out_w, const int64_t *excl_off, const TPos *excl_pos,
-                             int32_t n_excl, void *workspace, size_t workspace_bytes, void *stream) {
+                             int32_t n_excl, void *workspace, size_t workspace_bytes, void *stream,
+                             const int32_t *pos_deg = nullptr) {
     constexpr bool kMapped = sizeof(TPos) == 8;
     int rc = check_sample_mode(fn, k, -1.0, padding);
     if (rc != TFGK_OK) return rc;
+    TFGK_CHECK_ARG(!pos_deg || (k >= 0 && padding != TFGK_SAMPLE_HEAD),
+                   "%s: the weighted rule takes an integer fan-out and no head rule", fn);
     TFGK_CHECK_ARG(n_rows >= 0 && N >= 0 && hop >= 0 && hop < n_hops && cap_list >= 0 && cap_edges >= 0 &&
                    cap_edges < (1ll << 31) - 1 && n_excl >= 0, "%s: bad size", fn);
     TFGK_CHECK_ARG(state && out_rowptr, "%s: null pointer", fn);
@@ -1069,10 +1612,21 @@ static int block_sample_fill(const char *fn, const int64_t *rowptr, int32_t n_ro
     const int32_t *n_list = state + kStateSizes + hop;
     const int64_t *S = out_rowptr + cap_list;               // listed rows past the count add no edges
     if (cap_list > 0 && cap_edges > 0) {
-        TFGK_CHECK_ARG(rowptr && col && (w_csr || kMapped) && nodes && map && out_row && out_local && out_gcol && out_w,
+        TFGK_CHECK_ARG(rowptr && col && (w_csr || (kMapped && !pos_deg)) && nodes && map && out_row && out_local &&
+                       out_gcol && out_w,
                        "%s: null pointer", fn);
         const unsigned grid = (unsigned)ceil_div64(cap_list, kRowsPerCta);
-        if constexpr (kMapped) {
+        if (pos_deg) {
+            const unsigned wgrid = (unsigned)ceil_div64(cap_list, kWeightedRowsPerCta);
+            if (excl_off)
+                weighted_fill_kernel<true, TPos, true><<<wgrid, kRowsPerCta, 0, st>>>(
+                    rowptr, n_rows, nodes, n_list, 0, k, padding, pos_deg, w_csr, seed, rng_stream, out_rowptr, out_row,
+                    pos, col, out_gcol, out_w, excl_off, excl_pos, n_excl);
+            else
+                weighted_fill_kernel<true, TPos, false><<<wgrid, kRowsPerCta, 0, st>>>(
+                    rowptr, n_rows, nodes, n_list, 0, k, padding, pos_deg, w_csr, seed, rng_stream, out_rowptr, out_row,
+                    pos, col, out_gcol, out_w, nullptr, nullptr, 0);
+        } else if constexpr (kMapped) {
             if (excl_off)
                 block_fill_mapped_excl_kernel<<<grid, kRowsPerCta, 0, st>>>(rowptr, n_rows, nodes, n_list, k, padding,
                                                                            seed, rng_stream, out_rowptr, out_row, pos,
@@ -1160,6 +1714,64 @@ int tfgk_block_sample_fill_mapped_excl(const int64_t *rowptr, int32_t n_rows, co
                                       hop, n_hops, cap_list, cap_edges, k, padding, seed, rng_stream, out_rowptr, out_row,
                                       out_local, out_gcol, out_w, excl_off, excl_pos, n_excl, workspace, workspace_bytes,
                                       stream);
+}
+
+int tfgk_block_sample_fill_weighted(const int64_t *rowptr, int32_t n_rows, const int32_t *col, const float *w_csr,
+                                    const int32_t *pos_deg, int32_t N, int32_t *nodes, int32_t *map, int32_t *state,
+                                    int32_t hop, int32_t n_hops, int32_t cap_list, int64_t cap_edges, int32_t k,
+                                    int padding, uint64_t seed, uint32_t rng_stream, const int64_t *out_rowptr,
+                                    int32_t *out_row, int32_t *out_local, int32_t *out_gcol, float *out_w,
+                                    void *workspace, size_t workspace_bytes, void *stream) {
+    TFGK_CHECK_ARG(pos_deg != nullptr, "block_sample_fill_weighted: null positive degrees");
+    return block_sample_fill<int32_t>("block_sample_fill_weighted", rowptr, n_rows, col, w_csr, N, nodes, map, state, hop,
+                                      n_hops, cap_list, cap_edges, k, padding, seed, rng_stream, out_rowptr, out_row,
+                                      out_local, out_gcol, out_w, nullptr, nullptr, 0, workspace, workspace_bytes, stream,
+                                      pos_deg);
+}
+
+int tfgk_block_sample_fill_weighted_excl(const int64_t *rowptr, int32_t n_rows, const int32_t *col, const float *w_csr,
+                                         const int32_t *pos_deg, int32_t N, int32_t *nodes, int32_t *map, int32_t *state,
+                                         int32_t hop, int32_t n_hops, int32_t cap_list, int64_t cap_edges, int32_t k,
+                                         int padding, uint64_t seed, uint32_t rng_stream, const int64_t *out_rowptr,
+                                         int32_t *out_row, int32_t *out_local, int32_t *out_gcol, float *out_w,
+                                         const int64_t *excl_off, const int32_t *excl_pos, int32_t n_excl,
+                                         void *workspace, size_t workspace_bytes, void *stream) {
+    TFGK_CHECK_ARG(pos_deg != nullptr && excl_off != nullptr && excl_pos != nullptr,
+                   "block_sample_fill_weighted_excl: null positive degrees or exclusion lists");
+    return block_sample_fill<int32_t>("block_sample_fill_weighted_excl", rowptr, n_rows, col, w_csr, N, nodes, map,
+                                      state, hop, n_hops, cap_list, cap_edges, k, padding, seed, rng_stream, out_rowptr,
+                                      out_row, out_local, out_gcol, out_w, excl_off, excl_pos, n_excl, workspace,
+                                      workspace_bytes, stream, pos_deg);
+}
+
+int tfgk_block_sample_fill_weighted_mapped(const int64_t *rowptr, int32_t n_rows, const int32_t *col,
+                                           const float *w_csr, const int32_t *pos_deg, int32_t N, int32_t *nodes,
+                                           int32_t *map, int32_t *state, int32_t hop, int32_t n_hops, int32_t cap_list,
+                                           int64_t cap_edges, int32_t k, int padding, uint64_t seed, uint32_t rng_stream,
+                                           const int64_t *out_rowptr, int32_t *out_row, int32_t *out_local,
+                                           int32_t *out_gcol, float *out_w, void *workspace, size_t workspace_bytes,
+                                           void *stream) {
+    TFGK_CHECK_ARG(pos_deg != nullptr, "block_sample_fill_weighted_mapped: null positive degrees");
+    return block_sample_fill<int64_t>("block_sample_fill_weighted_mapped", rowptr, n_rows, col, w_csr, N, nodes, map,
+                                      state, hop, n_hops, cap_list, cap_edges, k, padding, seed, rng_stream, out_rowptr,
+                                      out_row, out_local, out_gcol, out_w, nullptr, nullptr, 0, workspace,
+                                      workspace_bytes, stream, pos_deg);
+}
+
+int tfgk_block_sample_fill_weighted_mapped_excl(const int64_t *rowptr, int32_t n_rows, const int32_t *col,
+                                                const float *w_csr, const int32_t *pos_deg, int32_t N, int32_t *nodes,
+                                                int32_t *map, int32_t *state, int32_t hop, int32_t n_hops,
+                                                int32_t cap_list, int64_t cap_edges, int32_t k, int padding,
+                                                uint64_t seed, uint32_t rng_stream, const int64_t *out_rowptr,
+                                                int32_t *out_row, int32_t *out_local, int32_t *out_gcol, float *out_w,
+                                                const int64_t *excl_off, const int64_t *excl_pos, int32_t n_excl,
+                                                void *workspace, size_t workspace_bytes, void *stream) {
+    TFGK_CHECK_ARG(pos_deg != nullptr && excl_off != nullptr && excl_pos != nullptr,
+                   "block_sample_fill_weighted_mapped_excl: null positive degrees or exclusion lists");
+    return block_sample_fill<int64_t>("block_sample_fill_weighted_mapped_excl", rowptr, n_rows, col, w_csr, N, nodes,
+                                      map, state, hop, n_hops, cap_list, cap_edges, k, padding, seed, rng_stream,
+                                      out_rowptr, out_row, out_local, out_gcol, out_w, excl_off, excl_pos, n_excl,
+                                      workspace, workspace_bytes, stream, pos_deg);
 }
 
 int tfgk_block_sample_end(const int32_t *nodes, int32_t cap_nodes, int32_t N, int32_t *map, const int32_t *state,

@@ -942,8 +942,9 @@ def gat_backward_recompute(csr, csr_t, Q, K, V, G, Y, bias, act, stats, num_head
 
 # ---- training-mode extras: dropout, per-head aggregation, GAT softmax backward -----------------------------------
 
-# rng_stream ids: independent draws for the same (seed, element); LINK = negative sampling and the edge split
-RNG_STREAM_DROPOUT, RNG_STREAM_SAMPLER, RNG_STREAM_LINK = 0, 1, 2
+# rng_stream ids: independent draws for the same (seed, element); LINK = negative sampling and the edge split, WEIGHTED =
+# the weighted fan-outs' keys (include/tfgk.h, "weighted block sampler")
+RNG_STREAM_DROPOUT, RNG_STREAM_SAMPLER, RNG_STREAM_LINK, RNG_STREAM_WEIGHTED = 0, 1, 2, 3
 
 
 def _keyed(entry, seed):
@@ -1094,10 +1095,13 @@ def neighbor_sample(csr, k=None, ratio=None, padding=False, seed=0, rng_stream=R
     return out_row, out_pos, out_rowptr
 
 
-def neighbor_sample_rows(rowptr, rows, k=None, ratio=None, padding=False, seed=0, rng_stream=RNG_STREAM_SAMPLER):
+def neighbor_sample_rows(rowptr, rows, k=None, ratio=None, padding=False, seed=0, rng_stream=RNG_STREAM_SAMPLER,
+                         weighted=None):
     """K13: fan-out sampling of the listed rows of a CSR (tfgk_neighbor_sample_rows_*).  rowptr int64 [n_rows+1] is read in
     place; rows int32 [R] are global row ids (repeats allowed).  Returns (list position of each sampled edge's row int32 [S],
-    CSR position int32 [S], out_rowptr int64 [R+1]); row t's positions are the ones neighbor_sample draws for row rows[t]."""
+    CSR position int32 [S], out_rowptr int64 [R+1]); row t's positions are the ones neighbor_sample draws for row rows[t].
+    weighted = (pos_deg int32 [n_rows], w_csr float32): an integer k draws by the weighted rule (the _weighted entries);
+    k None takes every entry, as without weights."""
     _check(rowptr, torch.int64, "rowptr")
     _check(rows, torch.int32, "rows")
     dev = rowptr.device
@@ -1105,20 +1109,48 @@ def neighbor_sample_rows(rowptr, rows, k=None, ratio=None, padding=False, seed=0
     kk = -1 if k is None else int(k)
     rr = -1.0 if ratio is None else float(ratio)
     padding = _padding_code(padding)
+    if weighted is not None and k is not None:
+        pos_deg, w_csr = weighted
+        _check(pos_deg, torch.int32, "pos_deg")
+        _check(w_csr, torch.float32, "w_csr")
+        if ratio is not None or padding == SAMPLE_HEAD or kk < 0:
+            raise ValueError("neighbor_sample_rows: the weighted rule takes a fan-out k >= 0, no ratio and no head rule")
     need = ctypes.c_size_t()
     _ffi.call("tfgk_neighbor_sample_workspace_bytes", R, ctypes.byref(need))
     ws = torch.empty((max(need.value, 1),), dtype=torch.uint8, device=dev)
     out_rowptr = torch.empty((R + 1,), dtype=torch.int64, device=dev)
     total = ctypes.c_int64()
-    _ffi.call("tfgk_neighbor_sample_rows_count", _p(rowptr), n_rows, _p(rows), R, kk, rr, padding, _p(out_rowptr),
-              ctypes.byref(total), _p(ws), need.value, _stream(rowptr))
+    if weighted is not None and k is not None:
+        _ffi.call("tfgk_neighbor_sample_rows_count_weighted", _p(rowptr), n_rows, _p(rows), R, kk, padding, _p(pos_deg),
+                  _p(w_csr), _p(out_rowptr), ctypes.byref(total), _p(ws), need.value, _stream(rowptr))
+    else:
+        _ffi.call("tfgk_neighbor_sample_rows_count", _p(rowptr), n_rows, _p(rows), R, kk, rr, padding, _p(out_rowptr),
+                  ctypes.byref(total), _p(ws), need.value, _stream(rowptr))
     S = total.value
     out_row = torch.empty((S,), dtype=torch.int32, device=dev)
     out_pos = torch.empty((S,), dtype=torch.int32, device=dev)
-    if S:
+    if S and weighted is not None and k is not None:
+        _ffi.call("tfgk_neighbor_sample_rows_fill_weighted", _p(rowptr), n_rows, _p(rows), R, kk, padding, _p(pos_deg),
+                  _p(w_csr), int(seed), int(rng_stream), _p(out_rowptr), _p(out_row), _p(out_pos), _stream(rowptr))
+    elif S:
         _ffi.call("tfgk_neighbor_sample_rows_fill", _p(rowptr), n_rows, _p(rows), R, kk, rr, padding, int(seed),
                   int(rng_stream), _p(out_rowptr), _p(out_row), _p(out_pos), _stream(rowptr))
     return out_row, out_pos, out_rowptr
+
+
+def csr_positive_degree(rowptr, w, pos_deg, n_invalid, w_base=0):
+    """tfgk_csr_positive_degree_f32: pos_deg int32 [n] = the entries of weight > 0 of the n rows of rowptr int64 [n + 1],
+    whose weights are w[p - w_base] (float32, device); adds the number of negative, NaN and infinite weights to n_invalid
+    (int32 [1], device).  Asynchronous."""
+    _check(rowptr, torch.int64, "rowptr")
+    _check(w, torch.float32, "w")
+    _check(pos_deg, torch.int32, "pos_deg")
+    _check(n_invalid, torch.int32, "n_invalid")
+    n = rowptr.numel() - 1
+    if pos_deg.numel() != n:
+        raise ValueError("csr_positive_degree: {} outputs for {} rows".format(pos_deg.numel(), n))
+    _ffi.call("tfgk_csr_positive_degree_f32", _p(rowptr), n, _p(w), int(w_base), _p(pos_deg), _p(n_invalid),
+              _stream(rowptr))
 
 
 def _relabel_workspace(n, device):
@@ -1173,7 +1205,8 @@ def _block_workspace(cap_list, cap_edges, device, entry="tfgk_block_sample_works
     return torch.empty((need.value,), dtype=torch.uint8, device=device), need.value
 
 
-def block_sample(rowptr, col, w_csr, seeds, fanouts, keys, node_map, padding=False, rng_stream=RNG_STREAM_SAMPLER):
+def block_sample(rowptr, col, w_csr, seeds, fanouts, keys, node_map, padding=False, rng_stream=RNG_STREAM_SAMPLER,
+                 pos_deg=None):
     """The block sampler (tfgk_block_sample_*): the hops of neighbor_sample_rows + frontier for every listed row, with the
     sizes kept on the device.  A hop whose capacity block_capacities cannot bound reads its edge total back; otherwise
     the batch synchronises once, in tfgk_block_sample_end, which also leaves node_map clean.
@@ -1182,57 +1215,66 @@ def block_sample(rowptr, col, w_csr, seeds, fanouts, keys, node_map, padding=Fal
     Returns (nodes, hop_sizes, hops, n_bad, n_dup): nodes int32 [hop_sizes[-1]]; hops[h] = (out_rowptr int64 [>= n_h + 1],
     list position of each edge's row, its local column, its global column (int32 [S_h]), its weight float32 [S_h]);
     n_bad / n_dup count seeds outside [0, N) and repeated seeds (the lists are then meaningless).
+    pos_deg: int32 [N], the CSR's positive degrees (csr_positive_degree), or None.  Given, every integer fan-out draws by
+    the weighted rule (tfgk_block_sample_*_weighted; pass rng_stream=RNG_STREAM_WEIGHTED) and fan-out None as without it.
     Every argument the entries would refuse is refused before the map is touched, and a failure between the first and
     the last entry (an allocation, a hop past 2^31 edges) resets the map before it propagates."""
-    padding = _check_block_fanouts(fanouts, padding)
+    padding = _check_block_fanouts(fanouts, padding, pos_deg)
     _check(col, torch.int32, "col")
     _check(w_csr, torch.float32, "w_csr")
-    return _block_sample(rowptr, _p(col), _p(w_csr), seeds, fanouts, keys, node_map, padding, rng_stream, False)
+    return _block_sample(rowptr, _p(col), _p(w_csr), seeds, fanouts, keys, node_map, padding, rng_stream, False,
+                         pos_deg=pos_deg)
 
 
 def block_sample_mapped(rowptr, col_ptr, w_ptr, seeds, fanouts, keys, node_map, padding=False,
-                        rng_stream=RNG_STREAM_SAMPLER):
+                        rng_stream=RNG_STREAM_SAMPLER, pos_deg=None):
     """block_sample over a CSR in host memory (tfgk_block_sample_fill_mapped): col_ptr and w_ptr are the device addresses
     of its page-locked int32 columns and float32 weights (w_ptr None: every weight 1.0), at int64 positions; rowptr stays
     on the device.  Same arguments otherwise, and the same outputs as block_sample over the same CSR."""
-    padding = _check_block_fanouts(fanouts, padding)
+    padding = _check_block_fanouts(fanouts, padding, pos_deg)
     return _block_sample(rowptr, ctypes.c_void_p(col_ptr), None if w_ptr is None else ctypes.c_void_p(w_ptr), seeds,
-                         fanouts, keys, node_map, padding, rng_stream, True)
+                         fanouts, keys, node_map, padding, rng_stream, True, pos_deg=pos_deg)
 
 
-def _check_block_fanouts(fanouts, padding):
+def _check_block_fanouts(fanouts, padding, pos_deg=None):
     # the fan-out rules of check_sample_mode, here so that no entry refuses a hop once the map holds the seeds
     padding = _padding_code(padding)
     if any(k is not None and int(k) < 0 for k in fanouts):
         raise ValueError("block_sample: fan-outs must be >= 0 or None")
     if padding == SAMPLE_HEAD and any(k is None for k in fanouts):
         raise ValueError("block_sample: the head rule needs an integer fan-out for every hop")
+    if pos_deg is not None:
+        _check(pos_deg, torch.int32, "pos_deg")
+        if padding == SAMPLE_HEAD:
+            raise ValueError("block_sample: the head rule takes no weights")
     return padding
 
 
 def link_block_sample(rowptr, col, w_csr, pairs, n_pos, fanouts, keys, node_map, exclude=None, padding=False,
-                      rng_stream=RNG_STREAM_SAMPLER):
+                      rng_stream=RNG_STREAM_SAMPLER, pos_deg=None):
     """block_sample seeded by the endpoints of node pairs (tfgk_block_sample_begin_pairs): pairs int32 [2, P] (contiguous
     rows), whose distinct endpoints, taken pair by pair (source, then destination) in first-occurrence order, are the
     seeds.  exclude: None, "self" (every CSR entry (u, v) of the first n_pos pairs leaves u's row, at every hop) or
     "reverse" (and every entry (v, u)); the exclusion lists take one more host synchronisation (their total).
     Returns (nodes, hop_sizes, hops, n_bad, local, excluded): block_sample's outputs, with n_bad counting endpoints outside
     [0, N); local int32 [2, P], the pairs relabelled to positions in nodes; excluded = (excl_off int64, n_excl): row
-    t < n_excl of every list had excl_off[t + 1] - excl_off[t] entries excluded (None without exclusion)."""
-    padding = _check_block_fanouts(fanouts, padding)
+    t < n_excl of every list had excl_off[t + 1] - excl_off[t] entries excluded (None without exclusion).
+    pos_deg: as block_sample's."""
+    padding = _check_block_fanouts(fanouts, padding, pos_deg)
     _check(col, torch.int32, "col")
     _check(w_csr, torch.float32, "w_csr")
     return _block_sample(rowptr, _p(col), _p(w_csr), None, fanouts, keys, node_map, padding, rng_stream, False,
-                         pairs=(pairs, int(n_pos), exclude))
+                         pairs=(pairs, int(n_pos), exclude), pos_deg=pos_deg)
 
 
 def link_block_sample_mapped(rowptr, col_ptr, w_ptr, pairs, n_pos, fanouts, keys, node_map, exclude=None, padding=False,
-                             rng_stream=RNG_STREAM_SAMPLER):
+                             rng_stream=RNG_STREAM_SAMPLER, pos_deg=None):
     """link_block_sample over a CSR in host memory (block_sample_mapped's arguments); the exclusion lists read the
     targeted rows' columns over the host link."""
-    padding = _check_block_fanouts(fanouts, padding)
+    padding = _check_block_fanouts(fanouts, padding, pos_deg)
     return _block_sample(rowptr, ctypes.c_void_p(col_ptr), None if w_ptr is None else ctypes.c_void_p(w_ptr), None,
-                         fanouts, keys, node_map, padding, rng_stream, True, pairs=(pairs, int(n_pos), exclude))
+                         fanouts, keys, node_map, padding, rng_stream, True, pairs=(pairs, int(n_pos), exclude),
+                         pos_deg=pos_deg)
 
 
 def link_tail_negatives(src, q, num_nodes, seed, out_row, out_col, rng_stream=RNG_STREAM_LINK):
@@ -1277,9 +1319,11 @@ def _exclusion_lists(rowptr, col, nodes, cap, local, pairs, n_pos, exclude, mapp
     return excl_off, excl_pos
 
 
-def _block_sample(rowptr, col, w_csr, seeds, fanouts, keys, node_map, padding, rng_stream, mapped, pairs=None):
+def _block_sample(rowptr, col, w_csr, seeds, fanouts, keys, node_map, padding, rng_stream, mapped, pairs=None,
+                  pos_deg=None):
     """block_sample's hops; col and w_csr are the fill's pointer arguments, to host memory when `mapped`.  The batch
-    begins from the seed list `seeds`, or with pairs = (pair tensor, n_pos, exclude) from link_block_sample's pairs."""
+    begins from the seed list `seeds`, or with pairs = (pair tensor, n_pos, exclude) from link_block_sample's pairs.
+    pos_deg (not None): integer fan-outs by the weighted rule."""
     _check(rowptr, torch.int64, "rowptr")
     _check(node_map, torch.int32, "node_map")
     if pairs is None:
@@ -1335,7 +1379,16 @@ def _block_sample(rowptr, col, w_csr, seeds, fanouts, keys, node_map, padding, r
             cap_edges, cap_next = block_capacities(cap_list, fanouts[h], limit)
             ws, nbytes = _block_workspace(cap_list, 0 if cap_edges is None else cap_edges, dev, *ws_entry)
             out_rowptr = torch.empty((cap_list + 1,), dtype=torch.int64, device=dev)
-            if excl_args:
+            weighted = pos_deg is not None and k >= 0
+            if weighted and excl_args:
+                _ffi.call("tfgk_block_sample_count_weighted_mapped_excl" if mapped else
+                          "tfgk_block_sample_count_weighted_excl", _p(rowptr), n_rows, _p(nodes), _p(state), h, L,
+                          cap_list, k, padding, _p(pos_deg), w_csr, excl_args[0], excl_args[1], excl_args[2],
+                          _p(out_rowptr), _p(ws), nbytes, st)
+            elif weighted:
+                _ffi.call("tfgk_block_sample_count_weighted", _p(rowptr), n_rows, _p(nodes), _p(state), h, L, cap_list, k,
+                          padding, _p(pos_deg), w_csr, _p(out_rowptr), _p(ws), nbytes, st)
+            elif excl_args:
                 _ffi.call("tfgk_block_sample_count_excl", _p(rowptr), n_rows, _p(nodes), _p(state), h, L, cap_list, k,
                           padding, excl_args[0], excl_args[2], _p(out_rowptr), _p(ws), nbytes, st)
             else:
@@ -1349,9 +1402,16 @@ def _block_sample(rowptr, col, w_csr, seeds, fanouts, keys, node_map, padding, r
                 ws, nbytes = _block_workspace(cap_list, cap_edges, dev, *ws_entry)
             out = [torch.empty((max(cap_edges, 1),), dtype=torch.int32, device=dev) for _ in range(3)]
             out_w = torch.empty((max(cap_edges, 1),), dtype=torch.float32, device=dev)
-            _ffi.call(fill, _p(rowptr), n_rows, col, w_csr, N, _p(nodes), _p(node_map),
-                      _p(state), h, L, cap_list, cap_edges, k, padding, int(keys[h]), int(rng_stream), _p(out_rowptr),
-                      _p(out[0]), _p(out[1]), _p(out[2]), _p(out_w), *excl_args, _p(ws), nbytes, st)
+            if weighted:
+                wfill = fill.replace("tfgk_block_sample_fill", "tfgk_block_sample_fill_weighted")
+                _ffi.call(wfill, _p(rowptr), n_rows, col, w_csr, _p(pos_deg), N, _p(nodes), _p(node_map),
+                          _p(state), h, L, cap_list, cap_edges, k, padding, int(keys[h]), int(rng_stream),
+                          _p(out_rowptr), _p(out[0]), _p(out[1]), _p(out[2]), _p(out_w), *excl_args, _p(ws), nbytes, st)
+            else:
+                _ffi.call(fill, _p(rowptr), n_rows, col, w_csr, N, _p(nodes), _p(node_map),
+                          _p(state), h, L, cap_list, cap_edges, k, padding, int(keys[h]), int(rng_stream),
+                          _p(out_rowptr), _p(out[0]), _p(out[1]), _p(out[2]), _p(out_w), *excl_args, _p(ws), nbytes,
+                          st)
             hops.append((out_rowptr, out[0], out[1], out[2], out_w))
             cap_list = cap_next
         host = (ctypes.c_int32 * (4 + 2 * L))()

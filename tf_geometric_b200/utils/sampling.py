@@ -63,6 +63,7 @@ class _SamplerBase(object):
         self.num_edges = E
         self.edge_weight = torch.ones((E,), dtype=torch.float32, device=dev) if edge_weight is None \
             else ops.as_device(edge_weight, torch.float32, device=dev).reshape(-1)
+        self._has_weights = edge_weight is not None
         self.row, self.col = self.edge_index[0].contiguous(), self.edge_index[1].contiguous()
         self.num_row_nodes = int(self.row.max().item()) + 1 if E else 0
         self.num_col_nodes = int(self.col.max().item()) + 1 if E else 0
@@ -115,17 +116,19 @@ class Block(ops.SampledInput):
     sums float32), both indexed by node id (None for a block built by hand).  excluded: for a block of a link batch that
     excluded its target edges, (excl_off int64, n_excl): output row r < n_excl lost excl_off[r + 1] - excl_off[r] of its
     full-graph entries, which with_gcn_norm() leaves out of its scale (None otherwise, and for a block built by hand).
+    weighted: whether the hop drew its fan-out in proportion to the edge weights (weighted=True of the samplers).
     The transposed CSR that the backward needs is built on first use and kept on the block."""
 
     __slots__ = ("num_src", "num_dst", "edge_index", "edge_weight", "global_col", "csr", "fanout", "dst_ids", "degrees",
-                 "excluded", "_csr_t", "_w_t", "_looped", "_gcn")
+                 "excluded", "weighted", "_csr_t", "_w_t", "_looped", "_gcn")
 
     def __init__(self, num_src, num_dst, edge_index, edge_weight, global_col, csr, fanout=None, dst_ids=None,
-                 degrees=None, excluded=None):
+                 degrees=None, excluded=None, weighted=False):
         self.num_src, self.num_dst = int(num_src), int(num_dst)
         self.edge_index, self.edge_weight, self.global_col, self.csr = edge_index, edge_weight, global_col, csr
         self.fanout = None if fanout is None else int(fanout)
         self.dst_ids, self.degrees, self.excluded = dst_ids, degrees, excluded
+        self.weighted = bool(weighted)
         self._csr_t, self._w_t, self._looped, self._gcn = None, {}, None, None
 
     def with_self_loops(self):
@@ -137,7 +140,12 @@ class Block(ops.SampledInput):
 
     def with_gcn_norm(self):
         """The GcnBlock of this block (GCN's input on a sampled block), made on first use and kept; no device work until
-        a configuration's values are first used.  A block built by hand carries no full-graph degrees: ValueError."""
+        a configuration's values are first used.  A block built by hand carries no full-graph degrees: ValueError.
+        A weighted block with an integer fan-out: NotImplementedError (the rescale n_g / k_r is the unbiased factor of
+        uniform draws; a weighted sample would need every entry's inclusion probability)."""
+        if self.weighted and self.fanout is not None:
+            raise NotImplementedError("with_gcn_norm() rescales uniform draws; a block drawn with weighted=True would "
+                                      "need inclusion probabilities")
         if self._gcn is None:
             if self.degrees is None or self.dst_ids is None:
                 raise ValueError("with_gcn_norm() needs the full graph's degrees, which only a block from a sampler's "
@@ -622,6 +630,8 @@ _LINK_DOC = """Link-prediction mini-batch on blocks (an extension of the referen
         :param num_negatives: negatives drawn per positive pair
         :param negative_edge_index: int [2, M] negative pairs to use instead
         :param exclude: None, "self" or "reverse"
+        :param weighted: draw every integer fan-out in proportion to edge_weight, as sample_blocks(weighted=True); the
+            excluded entries are not candidates
         :return: LinkBlocks, on the device.  Ids outside [0, N) raise ValueError after the batch's read-back."""
 
 
@@ -681,6 +691,7 @@ class RandomNeighborSampler(_SamplerBase):
         self._node_map = None
         self._rowsum = None
         self._rowptr_host = None
+        self._pos_deg = None
 
     def _structure(self):
         if self._csr is None:
@@ -739,7 +750,22 @@ class RandomNeighborSampler(_SamplerBase):
             self._rowsum = rowsum
         return rowptr, self._rowsum
 
-    def sample_neighborhood(self, seed_node_index, fanouts, padding=False, seed=None):
+    def _positive_degrees(self):
+        """int32 [N]: every row's entries of weight > 0 (the weighted rule's d+), made on the first weighted call and
+        kept.  That call reads the count of invalid weights back once: ValueError for a negative, NaN or infinite weight,
+        and for a sampler built without edge_weight."""
+        if self._pos_deg is None:
+            if not self._has_weights:
+                raise ValueError("weighted=True draws in proportion to edge_weight; this sampler was built without one")
+            csr, w_csr, rowptr, node_map = self._neighborhood_structure()
+            pos_deg = torch.empty((node_map.numel(),), dtype=torch.int32, device=rowptr.device)
+            n_invalid = torch.zeros((1,), dtype=torch.int32, device=rowptr.device)
+            ops.csr_positive_degree(rowptr, w_csr, pos_deg, n_invalid)
+            _check_weights(int(n_invalid.item()))
+            self._pos_deg = pos_deg
+        return self._pos_deg
+
+    def sample_neighborhood(self, seed_node_index, fanouts, padding=False, seed=None, weighted=False):
         """Seed-node mini-batch sampling (an extension of the reference API).
 
         Hop h draws fanouts[-1 - h] neighbours (by sample()'s k rule and `padding`) for EVERY node already in the list, so
@@ -749,11 +775,16 @@ class RandomNeighborSampler(_SamplerBase):
 
         :param seed_node_index: distinct node ids (numpy, list or tensor); duplicates raise ValueError
         :param fanouts: neighbours per node for each layer, layer 0 nearest the input: sampling starts with fanouts[-1]
+        :param weighted: draw every integer fan-out in proportion to edge_weight (sample_blocks' weighted rule)
         :return: SampledNeighborhood, on the device
         """
         from .graph_utils import _batch_seed         # graph_utils imports this module
         seed = _rng.resolve_host(seed)
+        _check_weighted_padding(weighted, padding)
         csr, w_csr, rowptr, node_map = self._neighborhood_structure()
+        wargs = {}
+        if weighted:
+            wargs = dict(weighted=(self._positive_degrees(), w_csr), rng_stream=ops.RNG_STREAM_WEIGHTED)
         dev = rowptr.device
         N = node_map.numel()
         nodes = ops.as_device(seed_node_index, torch.int32, device=dev).reshape(-1).contiguous()
@@ -768,7 +799,7 @@ class RandomNeighborSampler(_SamplerBase):
         hop_sizes, hop_edges, hop_weights = [n], [], []
         for h, k in enumerate(reversed(list(fanouts))):
             out_row, out_pos, _ = ops.neighbor_sample_rows(rowptr, nodes[:n], k=None if k is None else int(k),
-                                                           padding=padding, seed=_batch_seed(seed, h))
+                                                           padding=padding, seed=_batch_seed(seed, h), **wargs)
             S = out_pos.numel()
             grown = torch.empty((n + S,), dtype=torch.int32, device=dev)
             grown[:n].copy_(nodes[:n])
@@ -784,16 +815,24 @@ class RandomNeighborSampler(_SamplerBase):
             hop_sizes.append(n)
         return SampledNeighborhood(nodes[:n], hop_edges[::-1], hop_weights[::-1], hop_sizes)
 
-    def sample_blocks(self, seed_node_index, fanouts, padding=False, seed=None):
+    def sample_blocks(self, seed_node_index, fanouts, padding=False, seed=None, weighted=False):
         """sample_neighborhood's batch as layer-wise bipartite blocks (an extension of the reference API); same arguments
         and the same node list and edges for the same key.  Integer fan-outs and device-resident seeds synchronise the
         host once per batch; a fan-out of None (every neighbour) adds one read-back for its hop.
 
+        weighted=True (DGL's prob=, PyG's weight_attr=): every integer fan-out draws in proportion to the sampler's
+        edge_weight, by the rule of include/tfgk.h ("weighted block sampler"): min(k, d+) entries without replacement by
+        successive sampling, or with padding and k >= d+ k draws with replacement, P = w / W; entries of weight 0 are
+        never drawn, and fan-out None takes every entry as without weights.  A sampler built without edge_weight, and
+        padding="head", raise ValueError; the first weighted call makes the positive degrees and reads back once more.
+
         :return: SampledBlocks, on the device"""
+        _check_weighted_padding(weighted, padding)
         csr, w_csr, rowptr, node_map = self._neighborhood_structure()
+        pos_deg = self._positive_degrees() if weighted else None
         return _sample_blocks(lambda nodes, hop_fanouts, keys: ops.block_sample(
-            rowptr, csr.col, w_csr, nodes, hop_fanouts, keys, node_map, padding=padding),
-            rowptr.device, node_map.numel(), seed_node_index, fanouts, seed, self._gcn_degrees)
+            rowptr, csr.col, w_csr, nodes, hop_fanouts, keys, node_map, padding=padding, **_weighted_args(pos_deg)),
+            rowptr.device, node_map.numel(), seed_node_index, fanouts, seed, self._gcn_degrees, weighted)
 
     def row_block(self, r0, r1):
         return _row_block(self, r0, r1)
@@ -817,12 +856,30 @@ class RandomNeighborSampler(_SamplerBase):
 
     @_with_link_doc
     def sample_link_blocks(self, edge_index, fanouts, num_negatives=1, negative_edge_index=None, exclude=None,
-                           padding=False, seed=None):
+                           padding=False, seed=None, weighted=False):
+        _check_weighted_padding(weighted, padding)
         csr, w_csr, rowptr, node_map = self._neighborhood_structure()
+        pos_deg = self._positive_degrees() if weighted else None
         return _sample_link_blocks(lambda pairs, n_pos, hop_fanouts, keys, exclude: ops.link_block_sample(
-            rowptr, csr.col, w_csr, pairs, n_pos, hop_fanouts, keys, node_map, exclude=exclude, padding=padding),
-            rowptr.device, node_map.numel(), edge_index, fanouts, num_negatives, negative_edge_index, exclude, padding,
-            seed, self._gcn_degrees)
+            rowptr, csr.col, w_csr, pairs, n_pos, hop_fanouts, keys, node_map, exclude=exclude, padding=padding,
+            **_weighted_args(pos_deg)), rowptr.device, node_map.numel(), edge_index, fanouts, num_negatives,
+            negative_edge_index, exclude, padding, seed, self._gcn_degrees, weighted)
+
+
+def _check_weighted_padding(weighted, padding):
+    if weighted and ops._padding_code(padding) == ops.SAMPLE_HEAD:
+        raise ValueError("padding='head' takes the first entries of each row and draws nothing: it cannot be weighted")
+
+
+def _check_weights(n_invalid):
+    if n_invalid:
+        raise ValueError("edge_weight holds {} negative, NaN or infinite weights; weighted=True draws in proportion to "
+                         "weights >= 0".format(n_invalid))
+
+
+def _weighted_args(pos_deg):
+    """The block samplers' keywords for a weighted batch (pos_deg not None) or an unweighted one."""
+    return {} if pos_deg is None else dict(pos_deg=pos_deg, rng_stream=ops.RNG_STREAM_WEIGHTED)
 
 
 def _hop_keys(fanouts, seed):
@@ -832,7 +889,7 @@ def _hop_keys(fanouts, seed):
     return hop_fanouts, [_batch_seed(seed, h) for h in range(len(hop_fanouts))]
 
 
-def _blocks_of(dev, node_index, sizes, hops, hop_fanouts, degrees, excluded=None):
+def _blocks_of(dev, node_index, sizes, hops, hop_fanouts, degrees, excluded=None, weighted=False):
     """The Blocks of a batch, layer 0 first, from the block sampler's hops."""
     blocks = []
     for h, (k, (out_rowptr, row, local, gcol, w)) in enumerate(zip(hop_fanouts, hops)):
@@ -842,11 +899,11 @@ def _blocks_of(dev, node_index, sizes, hops, hop_fanouts, degrees, excluded=None
         if _plan_for_fanout(k):
             block_csr.plan = ops.build_plan(block_csr)
         blocks.append(Block(n_src, n_dst, torch.stack([row, local]), w, gcol, block_csr, fanout=k,
-                            dst_ids=node_index[:n_dst], degrees=degrees, excluded=excluded))
+                            dst_ids=node_index[:n_dst], degrees=degrees, excluded=excluded, weighted=weighted))
     return blocks[::-1]
 
 
-def _sample_blocks(block_sample, dev, num_nodes, seed_node_index, fanouts, seed, degrees):
+def _sample_blocks(block_sample, dev, num_nodes, seed_node_index, fanouts, seed, degrees, weighted=False):
     """sample_blocks of both samplers around their block sampler: block_sample(seeds int32, per-hop fan-outs in hop order,
     hop keys) returns ops.block_sample's (nodes, hop_sizes, hops, n_bad, n_dup); this refuses bad seeds and assembles
     the SampledBlocks.  degrees: the sampler's (rowptr, row sums) handle that every Block keeps for with_gcn_norm()."""
@@ -858,8 +915,8 @@ def _sample_blocks(block_sample, dev, num_nodes, seed_node_index, fanouts, seed,
         raise ValueError("seed_node_index holds node ids outside [0, {})".format(num_nodes))
     if n_dup:
         raise ValueError("seed_node_index holds {} duplicate node ids".format(n_dup))
-    return SampledBlocks(node_index, sizes, _blocks_of(dev, node_index, sizes, hops, hop_fanouts, degrees),
-                         num_nodes=num_nodes)
+    return SampledBlocks(node_index, sizes, _blocks_of(dev, node_index, sizes, hops, hop_fanouts, degrees,
+                                                       weighted=weighted), num_nodes=num_nodes)
 
 
 class LinkBlocks(SampledBlocks):
@@ -906,7 +963,7 @@ def _pair_tensor(pairs, dev, what):
 
 
 def _sample_link_blocks(link_block_sample, dev, num_nodes, edge_index, fanouts, num_negatives, negative_edge_index,
-                        exclude, padding, seed, degrees):
+                        exclude, padding, seed, degrees, weighted=False):
     """sample_link_blocks of both samplers around their link block sampler: link_block_sample(pairs int32 [2, P], n_pos,
     per-hop fan-outs, hop keys, exclude) returns ops.link_block_sample's outputs.  This checks the arguments, writes the
     pairs (positives, then negatives), refuses endpoints outside the graph and assembles the LinkBlocks."""
@@ -936,7 +993,7 @@ def _sample_link_blocks(link_block_sample, dev, num_nodes, edge_index, fanouts, 
     node_index, sizes, hops, n_bad, local, excluded = link_block_sample(pairs, B, hop_fanouts, keys, exclude)
     if n_bad:
         raise ValueError("the pairs hold {} node ids outside [0, {})".format(n_bad, num_nodes))
-    blocks = _blocks_of(dev, node_index, sizes, hops, hop_fanouts, degrees, excluded)
+    blocks = _blocks_of(dev, node_index, sizes, hops, hop_fanouts, degrees, excluded, weighted)
     return LinkBlocks(node_index, sizes, blocks, num_nodes, local, B)
 
 
@@ -1136,6 +1193,7 @@ class HostNeighborSampler(object):
             device_bytes = torch.cuda.mem_get_info(dev)[0] // 2
         self.num_edges = E
         self._device = dev
+        self._has_weights = w is not None
         if E == 0:
             self.num_nodes, self.num_row_nodes = 0, 0
             self.rowptr = torch.zeros((1,), dtype=torch.int64, device=dev)
@@ -1146,6 +1204,7 @@ class HostNeighborSampler(object):
         else:
             self._build(ei, w, int(device_bytes))
         self._node_map = torch.full((self.num_nodes,), -1, dtype=torch.int32, device=dev)
+        self._pos_deg = None
         rowptr, rowsum = self.rowptr, self.rowsum
         self._degrees = lambda: (rowptr, rowsum)      # the blocks' handle: device tensors only, not the sampler
         self._closed = False
@@ -1215,25 +1274,49 @@ class HostNeighborSampler(object):
         if self._closed:
             raise RuntimeError("this HostNeighborSampler is closed")
 
-    def sample_blocks(self, seed_node_index, fanouts, padding=False, seed=None):
+    def _positive_degrees(self):
+        """RandomNeighborSampler._positive_degrees over the host CSR: tfgk_csr_positive_degree_f32 range by range over the
+        build's row ranges, each range's weights (only they) copied to the device by one asynchronous bulk copy."""
+        if self._pos_deg is None:
+            if not self._has_weights:
+                raise ValueError("weighted=True draws in proportion to edge_weight; this sampler was built without one")
+            pos_deg = torch.zeros((self.num_nodes,), dtype=torch.int32, device=self._device)
+            n_invalid = torch.zeros((1,), dtype=torch.int32, device=self._device)
+            for r0, r1 in self._ranges:
+                e0, e1 = int(self._rp[r0]), int(self._rp[r1])
+                if e1 > e0:
+                    w = torch.empty((e1 - e0,), dtype=torch.float32, device=self._device)
+                    ops.copy_async(w, self._w.ctypes.data + 4 * e0, 4 * (e1 - e0))
+                    ops.csr_positive_degree(self.rowptr[r0:r1 + 1], w, pos_deg[r0:r1], n_invalid, w_base=e0)
+            _check_weights(int(n_invalid.item()))
+            self._pos_deg = pos_deg
+        return self._pos_deg
+
+    def sample_blocks(self, seed_node_index, fanouts, padding=False, seed=None, weighted=False):
         """RandomNeighborSampler.sample_blocks over the host CSR: same arguments, same batch for the same key (rows of
         the CSR are sampled in place over the host link).  A batch synchronises with the host once (plus one read-back
-        per hop of fan-out None).  Calls on one sampler must be ordered on one CUDA stream.
+        per hop of fan-out None).  Calls on one sampler must be ordered on one CUDA stream.  weighted=True: as
+        RandomNeighborSampler's; every candidate's weight is read over the host link.
 
         :return: SampledBlocks, on the device"""
         self._check_open()
+        _check_weighted_padding(weighted, padding)
+        pos_deg = self._positive_degrees() if weighted else None
         return _sample_blocks(lambda nodes, hop_fanouts, keys: ops.block_sample_mapped(
-            self.rowptr, self._col_ptr, self._w_ptr, nodes, hop_fanouts, keys, self._node_map, padding=padding),
-            self._device, self.num_nodes, seed_node_index, fanouts, seed, self._degrees)
+            self.rowptr, self._col_ptr, self._w_ptr, nodes, hop_fanouts, keys, self._node_map, padding=padding,
+            **_weighted_args(pos_deg)), self._device, self.num_nodes, seed_node_index, fanouts, seed, self._degrees,
+            weighted)
 
     @_with_link_doc
     def sample_link_blocks(self, edge_index, fanouts, num_negatives=1, negative_edge_index=None, exclude=None,
-                           padding=False, seed=None):
+                           padding=False, seed=None, weighted=False):
         self._check_open()
+        _check_weighted_padding(weighted, padding)
+        pos_deg = self._positive_degrees() if weighted else None
         return _sample_link_blocks(lambda pairs, n_pos, hop_fanouts, keys, exclude: ops.link_block_sample_mapped(
             self.rowptr, self._col_ptr, self._w_ptr, pairs, n_pos, hop_fanouts, keys, self._node_map, exclude=exclude,
-            padding=padding), self._device, self.num_nodes, edge_index, fanouts, num_negatives, negative_edge_index,
-            exclude, padding, seed, self._degrees)
+            padding=padding, **_weighted_args(pos_deg)), self._device, self.num_nodes, edge_index, fanouts,
+            num_negatives, negative_edge_index, exclude, padding, seed, self._degrees, weighted)
 
     def row_block(self, r0, r1):
         self._check_open()
