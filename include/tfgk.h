@@ -851,6 +851,71 @@ int tfgk_block_sample_fill_weighted_mapped_excl(const int64_t *rowptr, int32_t n
                                                 int32_t *out_row, int32_t *out_local, int32_t *out_gcol, float *out_w,
                                                 const int64_t *excl_off, const int64_t *excl_pos, int32_t n_excl,
                                                 void *workspace, size_t workspace_bytes, void *stream);
+
+/* LABOR block sampler: layer-neighbour sampling (LABOR-0; Balin & Catalyurek, NeurIPS 2023), the rule of
+ * utils.RandomNeighborSampler / HostNeighborSampler with labor=True.  For listed row t of global row r under hop key
+ * `seed` (the hop's _batch_seed key, or hop 0's at every hop with layer dependency) and integer fan-out k >= 0:
+ *   Candidates: the row's kept entries (all of them, or those the _excl lists leave); d counts them.
+ *   Variate: u_c = lane 0 of one Philox4x32-10 block with counter (c, 0, rng_stream, 0) and key `seed`, c the entry's
+ *     column (a global node id); rng_stream is RNG_STREAM_LABOR = 4.  u_c depends on c and the key only: not on the row,
+ *     the CSR position or the exclusions.
+ *   Rule: d <= k keeps every candidate (no column is read to count it); otherwise candidate (t, c) is kept iff
+ *     (uint64) u_c * d < (uint64) k << 32, exact integer arithmetic.  k = 0 keeps nothing.  Kept entries are written in
+ *     ascending CSR position, with their global columns and their weights w_csr[p] (1.0f when w_csr is null).
+ *   Properties, with pi(k, d) = ceil(k 2^32 / d) / 2^32 for d > k and 1 otherwise: each candidate is kept with
+ *     probability pi; given its count m, a row's kept set is uniform over the m-subsets of its distinct columns (repeated
+ *     columns are kept or dropped together); two rows of one hop sharing c both keep it with probability min(pi_1, pi_2),
+ *     so c is reached with probability max pi over the listed rows holding it; a row with d > k keeps nothing with
+ *     probability (1 - pi)^(distinct columns).  A row keeps k entries in expectation and up to d, so no capacity bounds a
+ *     LABOR hop: the caller reads its edge total back (tfgk_block_sample_read_total), as for fan-out None.
+ *   Fan-out None and padding are not LABOR rules (refused: the caller uses the uniform entries for None).
+ * _count_labor / _count_labor_excl / _count_labor_mapped_excl: _count / _count_excl by this rule (col: the CSR's int32
+ *   columns, on the device or page-locked in host memory; the _excl forms take int32 or, over a host CSR, int64
+ *   excluded positions).  _fill_labor, _fill_labor_excl, _fill_labor_mapped, _fill_labor_mapped_excl: the _fill entries
+ *   by this rule, same outputs otherwise.  Both passes visit a row of d > k (and the fill every row) with the same
+ *   predicate: one warp for a row of at most 128 entries, its columns read 32 at a time (128-byte segments over the host
+ *   link) and its kept entries placed by a ballot prefix; the whole CTA for a longer row, 256 columns at a time and a
+ *   block-wide prefix count.  Every candidate column of a row of d > k is read twice (count, fill). */
+int tfgk_block_sample_count_labor(const int64_t *rowptr, int32_t n_rows, const int32_t *col, const int32_t *nodes,
+                                  const int32_t *state, int32_t hop, int32_t n_hops, int32_t cap_list, int32_t k,
+                                  uint64_t seed, uint32_t rng_stream, int64_t *out_rowptr, void *workspace,
+                                  size_t workspace_bytes, void *stream);
+int tfgk_block_sample_count_labor_excl(const int64_t *rowptr, int32_t n_rows, const int32_t *col, const int32_t *nodes,
+                                       const int32_t *state, int32_t hop, int32_t n_hops, int32_t cap_list, int32_t k,
+                                       uint64_t seed, uint32_t rng_stream, const int64_t *excl_off,
+                                       const int32_t *excl_pos, int32_t n_excl, int64_t *out_rowptr, void *workspace,
+                                       size_t workspace_bytes, void *stream);
+int tfgk_block_sample_count_labor_mapped_excl(const int64_t *rowptr, int32_t n_rows, const int32_t *col,
+                                              const int32_t *nodes, const int32_t *state, int32_t hop, int32_t n_hops,
+                                              int32_t cap_list, int32_t k, uint64_t seed, uint32_t rng_stream,
+                                              const int64_t *excl_off, const int64_t *excl_pos, int32_t n_excl,
+                                              int64_t *out_rowptr, void *workspace, size_t workspace_bytes,
+                                              void *stream);
+int tfgk_block_sample_fill_labor(const int64_t *rowptr, int32_t n_rows, const int32_t *col, const float *w_csr,
+                                 int32_t N, int32_t *nodes, int32_t *map, int32_t *state, int32_t hop, int32_t n_hops,
+                                 int32_t cap_list, int64_t cap_edges, int32_t k, uint64_t seed, uint32_t rng_stream,
+                                 const int64_t *out_rowptr, int32_t *out_row, int32_t *out_local, int32_t *out_gcol,
+                                 float *out_w, void *workspace, size_t workspace_bytes, void *stream);
+int tfgk_block_sample_fill_labor_excl(const int64_t *rowptr, int32_t n_rows, const int32_t *col, const float *w_csr,
+                                      int32_t N, int32_t *nodes, int32_t *map, int32_t *state, int32_t hop,
+                                      int32_t n_hops, int32_t cap_list, int64_t cap_edges, int32_t k, uint64_t seed,
+                                      uint32_t rng_stream, const int64_t *out_rowptr, int32_t *out_row,
+                                      int32_t *out_local, int32_t *out_gcol, float *out_w, const int64_t *excl_off,
+                                      const int32_t *excl_pos, int32_t n_excl, void *workspace, size_t workspace_bytes,
+                                      void *stream);
+int tfgk_block_sample_fill_labor_mapped(const int64_t *rowptr, int32_t n_rows, const int32_t *col, const float *w_csr,
+                                        int32_t N, int32_t *nodes, int32_t *map, int32_t *state, int32_t hop,
+                                        int32_t n_hops, int32_t cap_list, int64_t cap_edges, int32_t k, uint64_t seed,
+                                        uint32_t rng_stream, const int64_t *out_rowptr, int32_t *out_row,
+                                        int32_t *out_local, int32_t *out_gcol, float *out_w, void *workspace,
+                                        size_t workspace_bytes, void *stream);
+int tfgk_block_sample_fill_labor_mapped_excl(const int64_t *rowptr, int32_t n_rows, const int32_t *col,
+                                             const float *w_csr, int32_t N, int32_t *nodes, int32_t *map, int32_t *state,
+                                             int32_t hop, int32_t n_hops, int32_t cap_list, int64_t cap_edges, int32_t k,
+                                             uint64_t seed, uint32_t rng_stream, const int64_t *out_rowptr,
+                                             int32_t *out_row, int32_t *out_local, int32_t *out_gcol, float *out_w,
+                                             const int64_t *excl_off, const int64_t *excl_pos, int32_t n_excl,
+                                             void *workspace, size_t workspace_bytes, void *stream);
 int tfgk_block_gcn_values_excl_f32(const int64_t *rowptr, const int32_t *gcol, const float *w, int64_t S,
                                    const int32_t *dst, int32_t n_dst, const int64_t *g_rowptr, const float *g_rowsum,
                                    int norm, int loop, float deg_fill, float fill, const int64_t *excl_off,

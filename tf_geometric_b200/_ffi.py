@@ -191,6 +191,21 @@ SIGNATURES = {
     "tfgk_block_sample_fill_weighted_mapped_excl": [_ptr, _i32, _ptr, _ptr, _ptr, _i32, _ptr, _ptr, _ptr, _i32, _i32,
                                                     _i32, _i64, _i32, _int, _u64, _u32, _ptr, _ptr, _ptr, _ptr, _ptr,
                                                     _ptr, _ptr, _i32, _ptr, _size, _ptr],
+    "tfgk_block_sample_count_labor": [_ptr, _i32, _ptr, _ptr, _ptr, _i32, _i32, _i32, _i32, _u64, _u32, _ptr, _ptr, _size,
+                                      _ptr],
+    "tfgk_block_sample_count_labor_excl": [_ptr, _i32, _ptr, _ptr, _ptr, _i32, _i32, _i32, _i32, _u64, _u32, _ptr, _ptr,
+                                           _i32, _ptr, _ptr, _size, _ptr],
+    "tfgk_block_sample_count_labor_mapped_excl": [_ptr, _i32, _ptr, _ptr, _ptr, _i32, _i32, _i32, _i32, _u64, _u32, _ptr,
+                                                  _ptr, _i32, _ptr, _ptr, _size, _ptr],
+    "tfgk_block_sample_fill_labor": [_ptr, _i32, _ptr, _ptr, _i32, _ptr, _ptr, _ptr, _i32, _i32, _i32, _i64, _i32, _u64,
+                                     _u32, _ptr, _ptr, _ptr, _ptr, _ptr, _ptr, _size, _ptr],
+    "tfgk_block_sample_fill_labor_excl": [_ptr, _i32, _ptr, _ptr, _i32, _ptr, _ptr, _ptr, _i32, _i32, _i32, _i64, _i32,
+                                          _u64, _u32, _ptr, _ptr, _ptr, _ptr, _ptr, _ptr, _ptr, _i32, _ptr, _size, _ptr],
+    "tfgk_block_sample_fill_labor_mapped": [_ptr, _i32, _ptr, _ptr, _i32, _ptr, _ptr, _ptr, _i32, _i32, _i32, _i64, _i32,
+                                            _u64, _u32, _ptr, _ptr, _ptr, _ptr, _ptr, _ptr, _size, _ptr],
+    "tfgk_block_sample_fill_labor_mapped_excl": [_ptr, _i32, _ptr, _ptr, _i32, _ptr, _ptr, _ptr, _i32, _i32, _i32, _i64,
+                                                 _i32, _u64, _u32, _ptr, _ptr, _ptr, _ptr, _ptr, _ptr, _ptr, _i32, _ptr,
+                                                 _size, _ptr],
     "tfgk_row_block_i32": [_ptr, _i32, _i32, _i32, _ptr, _i64, _ptr, _ptr, _ptr, _ptr, _ptr, ctypes.POINTER(_i32), _ptr,
                            _size, _ptr],
     "tfgk_copy_async": [_ptr, _ptr, _size, _ptr],
@@ -345,6 +360,13 @@ NOT_CAPTURABLE = {
     "tfgk_block_sample_fill_weighted_mapped": ("the weighted host-memory block sampler", "it takes a host-side key"),
     "tfgk_block_sample_fill_weighted_mapped_excl": ("the weighted host-memory link block sampler",
                                                     "it takes a host-side key"),
+    "tfgk_block_sample_count_labor": ("the LABOR block sampler", "it takes a host-side key"),
+    "tfgk_block_sample_count_labor_excl": ("the LABOR link block sampler", "it takes a host-side key"),
+    "tfgk_block_sample_count_labor_mapped_excl": ("the LABOR host-memory link block sampler", "it takes a host-side key"),
+    "tfgk_block_sample_fill_labor": ("the LABOR block sampler", "it takes a host-side key"),
+    "tfgk_block_sample_fill_labor_excl": ("the LABOR link block sampler", "it takes a host-side key"),
+    "tfgk_block_sample_fill_labor_mapped": ("the LABOR host-memory block sampler", "it takes a host-side key"),
+    "tfgk_block_sample_fill_labor_mapped_excl": ("the LABOR host-memory link block sampler", "it takes a host-side key"),
     "tfgk_block_exclusion_count": ("the link block sampler's exclusion lists", "it returns their total to the host"),
     "tfgk_row_block_i32": ("the row blocks of layer-wise inference", "it returns the number of source rows to the host"),
     "tfgk_host_register": ("HostFeatureTable", "it page-locks host memory, which a graph cannot record"),

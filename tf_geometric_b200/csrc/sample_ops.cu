@@ -841,6 +841,136 @@ __global__ void positive_degree_kernel(const int64_t *__restrict__ rowptr, int32
     }
 }
 
+// ---- layer-neighbour (LABOR-0) fan-outs (include/tfgk.h, "LABOR block sampler") ------------------------------------
+// Row t keeps its candidate (t, c) iff u_c * d < k 2^32, u_c one variate per column node id c under the hop key, so rows
+// that share a neighbour keep it together.  Rows of d <= k keep every candidate; k = 0 keeps none.  The count and the
+// fill visit a row with the same predicate, in CSR order: one warp for a row of up to kThreadRowMax entries (columns
+// read 32 at a time, 128 bytes), the whole CTA for a longer one (kRowsPerCta at a time).
+enum { kLaborNone = 0, kLaborAll = 1, kLaborDraw = 2 };
+
+__device__ __forceinline__ bool labor_keep(int32_t c, uint64_t seed, uint32_t stream, int d, int k) {
+    const uint32_t u = philox4x32_10((uint32_t)c, 0u, stream, 0u, (uint32_t)seed, (uint32_t)(seed >> 32)).v[0];
+    return (uint64_t)u * (uint64_t)d < ((uint64_t)k << 32);
+}
+
+// whether real position p is one of the row's x excluded positions ex[0, x) (ascending)
+template <typename TPos>
+__device__ __forceinline__ bool excl_hit(const TPos *__restrict__ ex, int x, int64_t p) {
+    int lo = 0, hi = x;
+    while (lo < hi) {
+        const int mid = (lo + hi) >> 1;
+        if ((int64_t)ex[mid] < p) lo = mid + 1;
+        else hi = mid;
+    }
+    return lo < x && (int64_t)ex[lo] == p;
+}
+
+// listed row t's rule: WeightedRow with num = d (its candidates) and rule kLabor*
+template <typename TPos, bool kExcl>
+__device__ __forceinline__ WeightedRow<TPos> labor_row(int64_t t, int32_t r, const int64_t *__restrict__ rowptr, int k,
+                                                       const int64_t *__restrict__ excl_off,
+                                                       const TPos *__restrict__ excl_pos, int32_t n_excl) {
+    WeightedRow<TPos> R;
+    R.t = t;
+    R.r = r;
+    R.start = rowptr[r];
+    R.end = rowptr[r + 1];
+    R.o = 0;
+    R.x = kExcl ? excl_count(excl_off, n_excl, t) : 0;
+    R.ex = kExcl && R.x ? excl_pos + excl_off[t] : nullptr;
+    R.num = (int)(R.end - R.start) - R.x;
+    R.rule = (k == 0 || R.num == 0) ? kLaborNone : R.num <= k ? kLaborAll : kLaborDraw;
+    return R;
+}
+
+// Visits row R's entries kWidth at a time (32: the calling warp, kRowsPerCta: the CTA) and returns how many it keeps;
+// kFill writes them at R.o + slot in CSR order, with their list row, global column and weight (w_csr null: 1.0f).
+template <bool kFill, int kWidth, typename TPos, bool kExcl>
+__device__ __forceinline__ int labor_visit(const WeightedRow<TPos> &R, const int32_t *__restrict__ csr_col,
+                                           const float *__restrict__ w_csr, int k, uint64_t seed, uint32_t stream,
+                                           int *s_warp, int32_t *__restrict__ out_row, int32_t *__restrict__ out_gcol,
+                                           float *__restrict__ out_w) {
+    const int i = kWidth == 32 ? (int)(threadIdx.x & 31) : (int)threadIdx.x;
+    int base = 0;
+    for (int64_t c0 = R.start; c0 < R.end; c0 += kWidth) {
+        const int64_t p = c0 + i;
+        bool keep = false;
+        int32_t c = 0;
+        if (p < R.end && !(kExcl && R.x && excl_hit(R.ex, R.x, p))) {
+            c = csr_col[p];
+            keep = R.rule == kLaborAll || labor_keep(c, seed, stream, R.num, k);
+        }
+        int slot, n;
+        if constexpr (kWidth == 32) {
+            const unsigned m = __ballot_sync(0xffffffffu, keep);
+            slot = __popc(m & ((1u << i) - 1u));
+            n = __popc(m);
+        } else {
+            slot = cta_exclusive_count(keep, s_warp, n);
+        }
+        if (kFill && keep) {
+            const int64_t o = R.o + base + slot;
+            out_row[o] = (int32_t)R.t;
+            out_gcol[o] = c;
+            out_w[o] = w_csr ? w_csr[p] : 1.0f;
+        }
+        base += n;
+    }
+    return base;
+}
+
+// The count (kFill false: cnt[t] for every t < cap, 0 past the device count n_list) and the fill of the LABOR rule over
+// kWeightedRowsPerCta listed rows per CTA: a warp per row, then the rows longer than kThreadRowMax one after another on
+// the CTA.  The count skips the column reads of rows that keep every candidate or none.  The minimum of 4 CTAs per SM,
+// as for block_fill_mapped_kernel: left to itself ptxas chose 40-48 registers and spilled 4-8 bytes.
+template <bool kFill, typename TPos, bool kExcl>
+__global__ void __launch_bounds__(kRowsPerCta, 4)
+labor_kernel(const int64_t *__restrict__ rowptr, int32_t n_rows, const int32_t *__restrict__ rows,
+             const int32_t *__restrict__ n_list_dev, int32_t cap, int k, uint64_t seed, uint32_t stream,
+             const int32_t *__restrict__ csr_col, const float *__restrict__ w_csr, int32_t *__restrict__ cnt,
+             const int64_t *__restrict__ out_rowptr, int32_t *__restrict__ out_row, int32_t *__restrict__ out_gcol,
+             float *__restrict__ out_w, const int64_t *__restrict__ excl_off, const TPos *__restrict__ excl_pos,
+             int32_t n_excl) {
+    __shared__ int32_t long_rows[kWeightedRowsPerCta];
+    __shared__ int n_long;
+    __shared__ int s_warp[kWarps];
+    const int n_list = *n_list_dev;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    if (threadIdx.x == 0) n_long = 0;
+    __syncthreads();
+    for (int q = warp; q < kWeightedRowsPerCta; q += kWarps) {
+        const int64_t t = (int64_t)blockIdx.x * kWeightedRowsPerCta + q;
+        if (t >= cap) break;
+        const int32_t r = t < n_list ? rows[t] : -1;
+        int num = 0;
+        if (r >= 0 && r < n_rows) {
+            WeightedRow<TPos> R = labor_row<TPos, kExcl>(t, r, rowptr, k, excl_off, excl_pos, n_excl);
+            if (!kFill && R.rule == kLaborAll) {
+                num = R.num;
+            } else if (R.rule != kLaborNone) {
+                if (R.end - R.start > kThreadRowMax) {
+                    if (lane == 0) long_rows[atomicAdd(&n_long, 1)] = q;     // rows write disjoint ranges: any order
+                    continue;
+                }
+                if constexpr (kFill) R.o = out_rowptr[t];
+                num = labor_visit<kFill, 32, TPos, kExcl>(R, csr_col, w_csr, k, seed, stream, nullptr, out_row,
+                                                          out_gcol, out_w);
+            }
+        }
+        if (!kFill && lane == 0) cnt[t] = num;
+    }
+    __syncthreads();
+    const int nl = n_long;
+    for (int j = 0; j < nl; ++j) {
+        const int64_t t = (int64_t)blockIdx.x * kWeightedRowsPerCta + long_rows[j];
+        WeightedRow<TPos> R = labor_row<TPos, kExcl>(t, rows[t], rowptr, k, excl_off, excl_pos, n_excl);
+        if constexpr (kFill) R.o = out_rowptr[t];
+        const int num = labor_visit<kFill, kRowsPerCta, TPos, kExcl>(R, csr_col, w_csr, k, seed, stream, s_warp,
+                                                                     out_row, out_gcol, out_w);
+        if (!kFill && threadIdx.x == 0) cnt[t] = num;
+    }
+}
+
 __global__ void block_first_kernel(const int32_t *__restrict__ cols, const int64_t *__restrict__ S, int32_t N,
                                    int32_t *__restrict__ map, int32_t *__restrict__ counters) {
     const int64_t n = *S;
@@ -1469,14 +1599,16 @@ int tfgk_block_sample_begin(const int32_t *seeds, int32_t n_seeds, int32_t N, in
 
 }  // extern "C"
 
-// tfgk_block_sample_count, _count_excl (excl_off null: no exclusions) and their _weighted twins (pos_deg set: the
-// weighted rule over d+, which reads the weights w_csr at the excluded positions excl_pos)
+// tfgk_block_sample_count, _count_excl (excl_off null: no exclusions), their _weighted twins (pos_deg set: the
+// weighted rule over d+, which reads the weights w_csr at the excluded positions excl_pos) and their _labor twins
+// (labor_col set: the LABOR rule over the CSR columns labor_col under hop key seed)
 template <typename TPos = int32_t>
 static int block_sample_count(const char *fn, const int64_t *rowptr, int32_t n_rows, const int32_t *nodes,
                               const int32_t *state, int32_t hop, int32_t n_hops, int32_t cap_list, int32_t k, int padding,
                               const int64_t *excl_off, int32_t n_excl, int64_t *out_rowptr, void *workspace,
                               size_t workspace_bytes, void *stream, const int32_t *pos_deg = nullptr,
-                              const float *w_csr = nullptr, const TPos *excl_pos = nullptr) {
+                              const float *w_csr = nullptr, const TPos *excl_pos = nullptr,
+                              const int32_t *labor_col = nullptr, uint64_t seed = 0, uint32_t rng_stream = 0) {
     int rc = check_sample_mode(fn, k, -1.0, padding);
     if (rc != TFGK_OK) return rc;
     TFGK_CHECK_ARG(n_rows >= 0 && hop >= 0 && hop < n_hops && cap_list >= 0 && n_excl >= 0, "%s: bad size", fn);
@@ -1492,7 +1624,19 @@ static int block_sample_count(const char *fn, const int64_t *rowptr, int32_t n_r
     const BlockWorkspace L(cap_list, 0);
     int32_t *cnt = reinterpret_cast<int32_t *>(ws);
     const unsigned grid = (unsigned)ceil_div64(cap_list, 256);
-    if (pos_deg) {
+    if (labor_col) {
+        TFGK_CHECK_ARG(k >= 0 && padding == 0, "%s: the LABOR rule takes an integer fan-out and no padding", fn);
+        TFGK_CHECK_ARG(!excl_off || excl_pos, "%s: null exclusion positions", fn);
+        const unsigned lgrid = (unsigned)ceil_div64(cap_list, kWeightedRowsPerCta);
+        if (excl_off)
+            labor_kernel<false, TPos, true><<<lgrid, kRowsPerCta, 0, st>>>(
+                rowptr, n_rows, nodes, state + kStateSizes + hop, cap_list, k, seed, rng_stream, labor_col, nullptr, cnt,
+                nullptr, nullptr, nullptr, nullptr, excl_off, excl_pos, n_excl);
+        else
+            labor_kernel<false, TPos, false><<<lgrid, kRowsPerCta, 0, st>>>(
+                rowptr, n_rows, nodes, state + kStateSizes + hop, cap_list, k, seed, rng_stream, labor_col, nullptr, cnt,
+                nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, 0);
+    } else if (pos_deg) {
         TFGK_CHECK_ARG(k >= 0 && padding != TFGK_SAMPLE_HEAD, "%s: the weighted rule takes an integer fan-out and no "
                        "head rule", fn);
         TFGK_CHECK_ARG(!excl_off || (w_csr && excl_pos), "%s: null weights or exclusion list", fn);
@@ -1568,6 +1712,41 @@ int tfgk_block_sample_count_weighted_mapped_excl(const int64_t *rowptr, int32_t 
                                        workspace_bytes, stream, pos_deg, w_csr, excl_pos);
 }
 
+int tfgk_block_sample_count_labor(const int64_t *rowptr, int32_t n_rows, const int32_t *col, const int32_t *nodes,
+                                  const int32_t *state, int32_t hop, int32_t n_hops, int32_t cap_list, int32_t k,
+                                  uint64_t seed, uint32_t rng_stream, int64_t *out_rowptr, void *workspace,
+                                  size_t workspace_bytes, void *stream) {
+    TFGK_CHECK_ARG(col != nullptr, "block_sample_count_labor: null columns");
+    return block_sample_count<int32_t>("block_sample_count_labor", rowptr, n_rows, nodes, state, hop, n_hops, cap_list,
+                                       k, 0, nullptr, 0, out_rowptr, workspace, workspace_bytes, stream, nullptr, nullptr,
+                                       nullptr, col, seed, rng_stream);
+}
+
+int tfgk_block_sample_count_labor_excl(const int64_t *rowptr, int32_t n_rows, const int32_t *col, const int32_t *nodes,
+                                       const int32_t *state, int32_t hop, int32_t n_hops, int32_t cap_list, int32_t k,
+                                       uint64_t seed, uint32_t rng_stream, const int64_t *excl_off,
+                                       const int32_t *excl_pos, int32_t n_excl, int64_t *out_rowptr, void *workspace,
+                                       size_t workspace_bytes, void *stream) {
+    TFGK_CHECK_ARG(col != nullptr && excl_off != nullptr, "block_sample_count_labor_excl: null columns or exclusion "
+                   "offsets");
+    return block_sample_count<int32_t>("block_sample_count_labor_excl", rowptr, n_rows, nodes, state, hop, n_hops,
+                                       cap_list, k, 0, excl_off, n_excl, out_rowptr, workspace, workspace_bytes, stream,
+                                       nullptr, nullptr, excl_pos, col, seed, rng_stream);
+}
+
+int tfgk_block_sample_count_labor_mapped_excl(const int64_t *rowptr, int32_t n_rows, const int32_t *col,
+                                              const int32_t *nodes, const int32_t *state, int32_t hop, int32_t n_hops,
+                                              int32_t cap_list, int32_t k, uint64_t seed, uint32_t rng_stream,
+                                              const int64_t *excl_off, const int64_t *excl_pos, int32_t n_excl,
+                                              int64_t *out_rowptr, void *workspace, size_t workspace_bytes,
+                                              void *stream) {
+    TFGK_CHECK_ARG(col != nullptr && excl_off != nullptr, "block_sample_count_labor_mapped_excl: null columns or "
+                   "exclusion offsets");
+    return block_sample_count<int64_t>("block_sample_count_labor_mapped_excl", rowptr, n_rows, nodes, state, hop,
+                                       n_hops, cap_list, k, 0, excl_off, n_excl, out_rowptr, workspace, workspace_bytes,
+                                       stream, nullptr, nullptr, excl_pos, col, seed, rng_stream);
+}
+
 int tfgk_block_sample_read_total(const int32_t *state, int32_t hop, const int64_t *out_rowptr, int32_t cap_list,
                                  int32_t *n_list_host, int64_t *total_host, void *stream) {
     TFGK_CHECK_ARG(state && out_rowptr && n_list_host && total_host && hop >= 0 && cap_list >= 0,
@@ -1592,12 +1771,13 @@ static int block_sample_fill(const char *fn, const int64_t *rowptr, int32_t n_ro
                              uint32_t rng_stream, const int64_t *out_rowptr, int32_t *out_row, int32_t *out_local,
                              int32_t *out_gcol, float *out_w, const int64_t *excl_off, const TPos *excl_pos,
                              int32_t n_excl, void *workspace, size_t workspace_bytes, void *stream,
-                             const int32_t *pos_deg = nullptr) {
+                             const int32_t *pos_deg = nullptr, bool labor = false) {
     constexpr bool kMapped = sizeof(TPos) == 8;
     int rc = check_sample_mode(fn, k, -1.0, padding);
     if (rc != TFGK_OK) return rc;
     TFGK_CHECK_ARG(!pos_deg || (k >= 0 && padding != TFGK_SAMPLE_HEAD),
                    "%s: the weighted rule takes an integer fan-out and no head rule", fn);
+    TFGK_CHECK_ARG(!labor || (k >= 0 && padding == 0), "%s: the LABOR rule takes an integer fan-out and no padding", fn);
     TFGK_CHECK_ARG(n_rows >= 0 && N >= 0 && hop >= 0 && hop < n_hops && cap_list >= 0 && cap_edges >= 0 &&
                    cap_edges < (1ll << 31) - 1 && n_excl >= 0, "%s: bad size", fn);
     TFGK_CHECK_ARG(state && out_rowptr, "%s: null pointer", fn);
@@ -1616,7 +1796,17 @@ static int block_sample_fill(const char *fn, const int64_t *rowptr, int32_t n_ro
                        out_gcol && out_w,
                        "%s: null pointer", fn);
         const unsigned grid = (unsigned)ceil_div64(cap_list, kRowsPerCta);
-        if (pos_deg) {
+        if (labor) {
+            const unsigned lgrid = (unsigned)ceil_div64(cap_list, kWeightedRowsPerCta);
+            if (excl_off)
+                labor_kernel<true, TPos, true><<<lgrid, kRowsPerCta, 0, st>>>(
+                    rowptr, n_rows, nodes, n_list, cap_list, k, seed, rng_stream, col, w_csr, nullptr, out_rowptr,
+                    out_row, out_gcol, out_w, excl_off, excl_pos, n_excl);
+            else
+                labor_kernel<true, TPos, false><<<lgrid, kRowsPerCta, 0, st>>>(
+                    rowptr, n_rows, nodes, n_list, cap_list, k, seed, rng_stream, col, w_csr, nullptr, out_rowptr,
+                    out_row, out_gcol, out_w, nullptr, nullptr, 0);
+        } else if (pos_deg) {
             const unsigned wgrid = (unsigned)ceil_div64(cap_list, kWeightedRowsPerCta);
             if (excl_off)
                 weighted_fill_kernel<true, TPos, true><<<wgrid, kRowsPerCta, 0, st>>>(
@@ -1772,6 +1962,58 @@ int tfgk_block_sample_fill_weighted_mapped_excl(const int64_t *rowptr, int32_t n
                                       map, state, hop, n_hops, cap_list, cap_edges, k, padding, seed, rng_stream,
                                       out_rowptr, out_row, out_local, out_gcol, out_w, excl_off, excl_pos, n_excl,
                                       workspace, workspace_bytes, stream, pos_deg);
+}
+
+int tfgk_block_sample_fill_labor(const int64_t *rowptr, int32_t n_rows, const int32_t *col, const float *w_csr,
+                                 int32_t N, int32_t *nodes, int32_t *map, int32_t *state, int32_t hop, int32_t n_hops,
+                                 int32_t cap_list, int64_t cap_edges, int32_t k, uint64_t seed, uint32_t rng_stream,
+                                 const int64_t *out_rowptr, int32_t *out_row, int32_t *out_local, int32_t *out_gcol,
+                                 float *out_w, void *workspace, size_t workspace_bytes, void *stream) {
+    return block_sample_fill<int32_t>("block_sample_fill_labor", rowptr, n_rows, col, w_csr, N, nodes, map, state, hop,
+                                      n_hops, cap_list, cap_edges, k, 0, seed, rng_stream, out_rowptr, out_row, out_local,
+                                      out_gcol, out_w, nullptr, nullptr, 0, workspace, workspace_bytes, stream, nullptr,
+                                      true);
+}
+
+int tfgk_block_sample_fill_labor_excl(const int64_t *rowptr, int32_t n_rows, const int32_t *col, const float *w_csr,
+                                      int32_t N, int32_t *nodes, int32_t *map, int32_t *state, int32_t hop,
+                                      int32_t n_hops, int32_t cap_list, int64_t cap_edges, int32_t k, uint64_t seed,
+                                      uint32_t rng_stream, const int64_t *out_rowptr, int32_t *out_row,
+                                      int32_t *out_local, int32_t *out_gcol, float *out_w, const int64_t *excl_off,
+                                      const int32_t *excl_pos, int32_t n_excl, void *workspace, size_t workspace_bytes,
+                                      void *stream) {
+    TFGK_CHECK_ARG(excl_off != nullptr && excl_pos != nullptr, "block_sample_fill_labor_excl: null exclusion lists");
+    return block_sample_fill<int32_t>("block_sample_fill_labor_excl", rowptr, n_rows, col, w_csr, N, nodes, map, state,
+                                      hop, n_hops, cap_list, cap_edges, k, 0, seed, rng_stream, out_rowptr, out_row,
+                                      out_local, out_gcol, out_w, excl_off, excl_pos, n_excl, workspace, workspace_bytes,
+                                      stream, nullptr, true);
+}
+
+int tfgk_block_sample_fill_labor_mapped(const int64_t *rowptr, int32_t n_rows, const int32_t *col, const float *w_csr,
+                                        int32_t N, int32_t *nodes, int32_t *map, int32_t *state, int32_t hop,
+                                        int32_t n_hops, int32_t cap_list, int64_t cap_edges, int32_t k, uint64_t seed,
+                                        uint32_t rng_stream, const int64_t *out_rowptr, int32_t *out_row,
+                                        int32_t *out_local, int32_t *out_gcol, float *out_w, void *workspace,
+                                        size_t workspace_bytes, void *stream) {
+    return block_sample_fill<int64_t>("block_sample_fill_labor_mapped", rowptr, n_rows, col, w_csr, N, nodes, map, state,
+                                      hop, n_hops, cap_list, cap_edges, k, 0, seed, rng_stream, out_rowptr, out_row,
+                                      out_local, out_gcol, out_w, nullptr, nullptr, 0, workspace, workspace_bytes, stream,
+                                      nullptr, true);
+}
+
+int tfgk_block_sample_fill_labor_mapped_excl(const int64_t *rowptr, int32_t n_rows, const int32_t *col,
+                                             const float *w_csr, int32_t N, int32_t *nodes, int32_t *map, int32_t *state,
+                                             int32_t hop, int32_t n_hops, int32_t cap_list, int64_t cap_edges, int32_t k,
+                                             uint64_t seed, uint32_t rng_stream, const int64_t *out_rowptr,
+                                             int32_t *out_row, int32_t *out_local, int32_t *out_gcol, float *out_w,
+                                             const int64_t *excl_off, const int64_t *excl_pos, int32_t n_excl,
+                                             void *workspace, size_t workspace_bytes, void *stream) {
+    TFGK_CHECK_ARG(excl_off != nullptr && excl_pos != nullptr, "block_sample_fill_labor_mapped_excl: null exclusion "
+                   "lists");
+    return block_sample_fill<int64_t>("block_sample_fill_labor_mapped_excl", rowptr, n_rows, col, w_csr, N, nodes, map,
+                                      state, hop, n_hops, cap_list, cap_edges, k, 0, seed, rng_stream, out_rowptr,
+                                      out_row, out_local, out_gcol, out_w, excl_off, excl_pos, n_excl, workspace,
+                                      workspace_bytes, stream, nullptr, true);
 }
 
 int tfgk_block_sample_end(const int32_t *nodes, int32_t cap_nodes, int32_t N, int32_t *map, const int32_t *state,

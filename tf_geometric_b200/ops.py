@@ -943,8 +943,9 @@ def gat_backward_recompute(csr, csr_t, Q, K, V, G, Y, bias, act, stats, num_head
 # ---- training-mode extras: dropout, per-head aggregation, GAT softmax backward -----------------------------------
 
 # rng_stream ids: independent draws for the same (seed, element); LINK = negative sampling and the edge split, WEIGHTED =
-# the weighted fan-outs' keys (include/tfgk.h, "weighted block sampler")
-RNG_STREAM_DROPOUT, RNG_STREAM_SAMPLER, RNG_STREAM_LINK, RNG_STREAM_WEIGHTED = 0, 1, 2, 3
+# the weighted fan-outs' keys (include/tfgk.h, "weighted block sampler"), LABOR = the layer-neighbour variates ("LABOR
+# block sampler")
+RNG_STREAM_DROPOUT, RNG_STREAM_SAMPLER, RNG_STREAM_LINK, RNG_STREAM_WEIGHTED, RNG_STREAM_LABOR = 0, 1, 2, 3, 4
 
 
 def _keyed(entry, seed):
@@ -1206,7 +1207,7 @@ def _block_workspace(cap_list, cap_edges, device, entry="tfgk_block_sample_works
 
 
 def block_sample(rowptr, col, w_csr, seeds, fanouts, keys, node_map, padding=False, rng_stream=RNG_STREAM_SAMPLER,
-                 pos_deg=None):
+                 pos_deg=None, labor=False):
     """The block sampler (tfgk_block_sample_*): the hops of neighbor_sample_rows + frontier for every listed row, with the
     sizes kept on the device.  A hop whose capacity block_capacities cannot bound reads its edge total back; otherwise
     the batch synchronises once, in tfgk_block_sample_end, which also leaves node_map clean.
@@ -1217,32 +1218,40 @@ def block_sample(rowptr, col, w_csr, seeds, fanouts, keys, node_map, padding=Fal
     n_bad / n_dup count seeds outside [0, N) and repeated seeds (the lists are then meaningless).
     pos_deg: int32 [N], the CSR's positive degrees (csr_positive_degree), or None.  Given, every integer fan-out draws by
     the weighted rule (tfgk_block_sample_*_weighted; pass rng_stream=RNG_STREAM_WEIGHTED) and fan-out None as without it.
+    labor: every integer fan-out draws by the LABOR rule (tfgk_block_sample_*_labor; pass rng_stream=RNG_STREAM_LABOR,
+    and the same key for every hop for layer dependency), fan-out None as without it; no padding, no pos_deg.  No
+    capacity bounds a LABOR hop, so each one reads its edge total back, as a hop of fan-out None does.
     Every argument the entries would refuse is refused before the map is touched, and a failure between the first and
     the last entry (an allocation, a hop past 2^31 edges) resets the map before it propagates."""
-    padding = _check_block_fanouts(fanouts, padding, pos_deg)
+    padding = _check_block_fanouts(fanouts, padding, pos_deg, labor)
     _check(col, torch.int32, "col")
     _check(w_csr, torch.float32, "w_csr")
     return _block_sample(rowptr, _p(col), _p(w_csr), seeds, fanouts, keys, node_map, padding, rng_stream, False,
-                         pos_deg=pos_deg)
+                         pos_deg=pos_deg, labor=labor)
 
 
 def block_sample_mapped(rowptr, col_ptr, w_ptr, seeds, fanouts, keys, node_map, padding=False,
-                        rng_stream=RNG_STREAM_SAMPLER, pos_deg=None):
+                        rng_stream=RNG_STREAM_SAMPLER, pos_deg=None, labor=False):
     """block_sample over a CSR in host memory (tfgk_block_sample_fill_mapped): col_ptr and w_ptr are the device addresses
     of its page-locked int32 columns and float32 weights (w_ptr None: every weight 1.0), at int64 positions; rowptr stays
     on the device.  Same arguments otherwise, and the same outputs as block_sample over the same CSR."""
-    padding = _check_block_fanouts(fanouts, padding, pos_deg)
+    padding = _check_block_fanouts(fanouts, padding, pos_deg, labor)
     return _block_sample(rowptr, ctypes.c_void_p(col_ptr), None if w_ptr is None else ctypes.c_void_p(w_ptr), seeds,
-                         fanouts, keys, node_map, padding, rng_stream, True, pos_deg=pos_deg)
+                         fanouts, keys, node_map, padding, rng_stream, True, pos_deg=pos_deg, labor=labor)
 
 
-def _check_block_fanouts(fanouts, padding, pos_deg=None):
+def _check_block_fanouts(fanouts, padding, pos_deg=None, labor=False):
     # the fan-out rules of check_sample_mode, here so that no entry refuses a hop once the map holds the seeds
     padding = _padding_code(padding)
     if any(k is not None and int(k) < 0 for k in fanouts):
         raise ValueError("block_sample: fan-outs must be >= 0 or None")
     if padding == SAMPLE_HEAD and any(k is None for k in fanouts):
         raise ValueError("block_sample: the head rule needs an integer fan-out for every hop")
+    if labor:
+        if padding:
+            raise ValueError("block_sample: the LABOR rule draws without replacement and takes no padding")
+        if pos_deg is not None:
+            raise NotImplementedError("block_sample: weighted LABOR is not implemented")
     if pos_deg is not None:
         _check(pos_deg, torch.int32, "pos_deg")
         if padding == SAMPLE_HEAD:
@@ -1251,7 +1260,7 @@ def _check_block_fanouts(fanouts, padding, pos_deg=None):
 
 
 def link_block_sample(rowptr, col, w_csr, pairs, n_pos, fanouts, keys, node_map, exclude=None, padding=False,
-                      rng_stream=RNG_STREAM_SAMPLER, pos_deg=None):
+                      rng_stream=RNG_STREAM_SAMPLER, pos_deg=None, labor=False):
     """block_sample seeded by the endpoints of node pairs (tfgk_block_sample_begin_pairs): pairs int32 [2, P] (contiguous
     rows), whose distinct endpoints, taken pair by pair (source, then destination) in first-occurrence order, are the
     seeds.  exclude: None, "self" (every CSR entry (u, v) of the first n_pos pairs leaves u's row, at every hop) or
@@ -1259,22 +1268,22 @@ def link_block_sample(rowptr, col, w_csr, pairs, n_pos, fanouts, keys, node_map,
     Returns (nodes, hop_sizes, hops, n_bad, local, excluded): block_sample's outputs, with n_bad counting endpoints outside
     [0, N); local int32 [2, P], the pairs relabelled to positions in nodes; excluded = (excl_off int64, n_excl): row
     t < n_excl of every list had excl_off[t + 1] - excl_off[t] entries excluded (None without exclusion).
-    pos_deg: as block_sample's."""
-    padding = _check_block_fanouts(fanouts, padding, pos_deg)
+    pos_deg, labor: as block_sample's; a LABOR row's candidates are its entries less the excluded ones."""
+    padding = _check_block_fanouts(fanouts, padding, pos_deg, labor)
     _check(col, torch.int32, "col")
     _check(w_csr, torch.float32, "w_csr")
     return _block_sample(rowptr, _p(col), _p(w_csr), None, fanouts, keys, node_map, padding, rng_stream, False,
-                         pairs=(pairs, int(n_pos), exclude), pos_deg=pos_deg)
+                         pairs=(pairs, int(n_pos), exclude), pos_deg=pos_deg, labor=labor)
 
 
 def link_block_sample_mapped(rowptr, col_ptr, w_ptr, pairs, n_pos, fanouts, keys, node_map, exclude=None, padding=False,
-                             rng_stream=RNG_STREAM_SAMPLER, pos_deg=None):
+                             rng_stream=RNG_STREAM_SAMPLER, pos_deg=None, labor=False):
     """link_block_sample over a CSR in host memory (block_sample_mapped's arguments); the exclusion lists read the
     targeted rows' columns over the host link."""
-    padding = _check_block_fanouts(fanouts, padding, pos_deg)
+    padding = _check_block_fanouts(fanouts, padding, pos_deg, labor)
     return _block_sample(rowptr, ctypes.c_void_p(col_ptr), None if w_ptr is None else ctypes.c_void_p(w_ptr), None,
                          fanouts, keys, node_map, padding, rng_stream, True, pairs=(pairs, int(n_pos), exclude),
-                         pos_deg=pos_deg)
+                         pos_deg=pos_deg, labor=labor)
 
 
 def link_tail_negatives(src, q, num_nodes, seed, out_row, out_col, rng_stream=RNG_STREAM_LINK):
@@ -1320,10 +1329,10 @@ def _exclusion_lists(rowptr, col, nodes, cap, local, pairs, n_pos, exclude, mapp
 
 
 def _block_sample(rowptr, col, w_csr, seeds, fanouts, keys, node_map, padding, rng_stream, mapped, pairs=None,
-                  pos_deg=None):
+                  pos_deg=None, labor=False):
     """block_sample's hops; col and w_csr are the fill's pointer arguments, to host memory when `mapped`.  The batch
     begins from the seed list `seeds`, or with pairs = (pair tensor, n_pos, exclude) from link_block_sample's pairs.
-    pos_deg (not None): integer fan-outs by the weighted rule."""
+    pos_deg (not None): integer fan-outs by the weighted rule; labor: by the LABOR rule, each read back as a None hop."""
     _check(rowptr, torch.int64, "rowptr")
     _check(node_map, torch.int32, "node_map")
     if pairs is None:
@@ -1341,11 +1350,12 @@ def _block_sample(rowptr, col, w_csr, seeds, fanouts, keys, node_map, padding, r
     dev = rowptr.device
     n_rows, N, L = rowptr.numel() - 1, node_map.numel(), len(fanouts)
     ks = [-1 if k is None else int(k) for k in fanouts]
+    bounds = [None if labor else k for k in fanouts]      # a LABOR row keeps up to all its entries
     # a list holds each id once, plus the repeated or invalid seeds of a batch that will be refused (a pair list holds
     # its distinct valid endpoints only)
     limit = N + (n_begin if pairs is None else 0)
     cap_nodes = n_begin
-    for k in fanouts:
+    for k in bounds:
         cap_nodes = block_capacities(cap_nodes, k, limit)[1]
         if cap_nodes is None:
             cap_nodes = limit
@@ -1376,11 +1386,16 @@ def _block_sample(rowptr, col, w_csr, seeds, fanouts, keys, node_map, padding, r
             fill += "_excl"
         cap_list, hops = n_begin, []
         for h, k in enumerate(ks):
-            cap_edges, cap_next = block_capacities(cap_list, fanouts[h], limit)
+            cap_edges, cap_next = block_capacities(cap_list, bounds[h], limit)
             ws, nbytes = _block_workspace(cap_list, 0 if cap_edges is None else cap_edges, dev, *ws_entry)
             out_rowptr = torch.empty((cap_list + 1,), dtype=torch.int64, device=dev)
             weighted = pos_deg is not None and k >= 0
-            if weighted and excl_args:
+            by_labor = labor and k >= 0
+            if by_labor:
+                _ffi.call("tfgk_block_sample_count_labor" + ("_mapped_excl" if mapped else "_excl") * bool(excl_args),
+                          _p(rowptr), n_rows, col, _p(nodes), _p(state), h, L, cap_list, k, int(keys[h]),
+                          int(rng_stream), *excl_args, _p(out_rowptr), _p(ws), nbytes, st)
+            elif weighted and excl_args:
                 _ffi.call("tfgk_block_sample_count_weighted_mapped_excl" if mapped else
                           "tfgk_block_sample_count_weighted_excl", _p(rowptr), n_rows, _p(nodes), _p(state), h, L,
                           cap_list, k, padding, _p(pos_deg), w_csr, excl_args[0], excl_args[1], excl_args[2],
@@ -1402,7 +1417,12 @@ def _block_sample(rowptr, col, w_csr, seeds, fanouts, keys, node_map, padding, r
                 ws, nbytes = _block_workspace(cap_list, cap_edges, dev, *ws_entry)
             out = [torch.empty((max(cap_edges, 1),), dtype=torch.int32, device=dev) for _ in range(3)]
             out_w = torch.empty((max(cap_edges, 1),), dtype=torch.float32, device=dev)
-            if weighted:
+            if by_labor:
+                _ffi.call(fill.replace("tfgk_block_sample_fill", "tfgk_block_sample_fill_labor"), _p(rowptr), n_rows, col,
+                          w_csr, N, _p(nodes), _p(node_map), _p(state), h, L, cap_list, cap_edges, k, int(keys[h]),
+                          int(rng_stream), _p(out_rowptr), _p(out[0]), _p(out[1]), _p(out[2]), _p(out_w), *excl_args,
+                          _p(ws), nbytes, st)
+            elif weighted:
                 wfill = fill.replace("tfgk_block_sample_fill", "tfgk_block_sample_fill_weighted")
                 _ffi.call(wfill, _p(rowptr), n_rows, col, w_csr, _p(pos_deg), N, _p(nodes), _p(node_map),
                           _p(state), h, L, cap_list, cap_edges, k, padding, int(keys[h]), int(rng_stream),

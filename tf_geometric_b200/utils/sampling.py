@@ -110,25 +110,29 @@ class Block(ops.SampledInput):
     edge_index: int32 [2, S] local (row < num_dst, col < num_src), rows ascending and in draw order within a row.
     edge_weight: float32 [S].  global_col: int32 [S], the node id of every edge's column.
     csr: ops.CSR with n_rows = num_dst, n_cols = num_src; its perm is the identity (the edges are already in CSR order).
-    fanout: the fan-out of the hop that drew the block (None: every neighbour, or a block built by hand).
+    fanout: the fan-out of the hop that drew the block (None: every neighbour, or a block built by hand); for a LABOR
+    block, the k each row keeps in expectation.
     dst_ids: int32 [num_dst], the node id of every output row (a view of the batch's node_index; None for a block built
     by hand).  degrees: the sampler's full-graph degrees for with_gcn_norm(), a callable returning (rowptr int64, row
     sums float32), both indexed by node id (None for a block built by hand).  excluded: for a block of a link batch that
     excluded its target edges, (excl_off int64, n_excl): output row r < n_excl lost excl_off[r + 1] - excl_off[r] of its
     full-graph entries, which with_gcn_norm() leaves out of its scale (None otherwise, and for a block built by hand).
     weighted: whether the hop drew its fan-out in proportion to the edge weights (weighted=True of the samplers).
+    labor: whether the hop drew by the layer-neighbour rule (labor=True of the samplers, integer fan-outs): its fanout is
+    then k in expectation, and a row may hold up to all its neighbours.
     The transposed CSR that the backward needs is built on first use and kept on the block."""
 
     __slots__ = ("num_src", "num_dst", "edge_index", "edge_weight", "global_col", "csr", "fanout", "dst_ids", "degrees",
-                 "excluded", "weighted", "_csr_t", "_w_t", "_looped", "_gcn")
+                 "excluded", "weighted", "labor", "_csr_t", "_w_t", "_looped", "_gcn")
 
     def __init__(self, num_src, num_dst, edge_index, edge_weight, global_col, csr, fanout=None, dst_ids=None,
-                 degrees=None, excluded=None, weighted=False):
+                 degrees=None, excluded=None, weighted=False, labor=False):
         self.num_src, self.num_dst = int(num_src), int(num_dst)
         self.edge_index, self.edge_weight, self.global_col, self.csr = edge_index, edge_weight, global_col, csr
         self.fanout = None if fanout is None else int(fanout)
         self.dst_ids, self.degrees, self.excluded = dst_ids, degrees, excluded
         self.weighted = bool(weighted)
+        self.labor = bool(labor)
         self._csr_t, self._w_t, self._looped, self._gcn = None, {}, None, None
 
     def with_self_loops(self):
@@ -185,7 +189,8 @@ class SelfLoopBlock(ops.SampledInput):
     their own; every other operator refuses it.
 
     edge_index: int32 [2, S + num_dst] local, in CSR order.  csr: ops.CSR with n_rows = num_dst, n_cols = num_src and an
-    identity perm; it gets a work plan when its rows may be long (a fan-out of None or of DENSE_ROW_DEGREE - 1 or more).
+    identity perm; it gets a work plan when its rows may be long (a fan-out of None or of DENSE_ROW_DEGREE - 1 or more,
+    and every LABOR block).
     The transposed CSR that the backward needs is built on first use and kept."""
 
     __slots__ = ("num_src", "num_dst", "edge_index", "csr", "_csr_t")
@@ -196,7 +201,7 @@ class SelfLoopBlock(ops.SampledInput):
         nnz = self.edge_index.shape[1]
         self.csr = ops.CSR(rowptr, self.edge_index[1], torch.arange(nnz, dtype=torch.int32, device=rowptr.device),
                            self.num_dst, self.num_src)
-        if _plan_for_fanout(None if block.fanout is None else block.fanout + 1):
+        if _plan_for_fanout(None if block.fanout is None or block.labor else block.fanout + 1):
             self.csr.plan = ops.build_plan(self.csr)
         self._csr_t = None
 
@@ -623,7 +628,7 @@ _LINK_DOC = """Link-prediction mini-batch on blocks (an extension of the referen
         with those entries deleted (same order, weights following), for every fan-out rule; with_gcn_norm() keeps the
         full graph's degrees and rescales by the kept entries.
         Synchronisation: one host read-back per batch, one more for the exclusion lists' total, and one per hop of
-        fan-out None.  Calls on one sampler must be ordered on one CUDA stream.
+        fan-out None or drawn by LABOR.  Calls on one sampler must be ordered on one CUDA stream.
 
         :param edge_index: int [2, B] target pairs (numpy, list or tensor)
         :param fanouts: as sample_blocks
@@ -632,6 +637,8 @@ _LINK_DOC = """Link-prediction mini-batch on blocks (an extension of the referen
         :param exclude: None, "self" or "reverse"
         :param weighted: draw every integer fan-out in proportion to edge_weight, as sample_blocks(weighted=True); the
             excluded entries are not candidates
+        :param labor, layer_dependency: draw every integer fan-out by the layer-neighbour rule, as
+            sample_blocks(labor=True); the excluded entries are not candidates (d counts the kept entries only)
         :return: LinkBlocks, on the device.  Ids outside [0, N) raise ValueError after the batch's read-back."""
 
 
@@ -815,7 +822,8 @@ class RandomNeighborSampler(_SamplerBase):
             hop_sizes.append(n)
         return SampledNeighborhood(nodes[:n], hop_edges[::-1], hop_weights[::-1], hop_sizes)
 
-    def sample_blocks(self, seed_node_index, fanouts, padding=False, seed=None, weighted=False):
+    def sample_blocks(self, seed_node_index, fanouts, padding=False, seed=None, weighted=False, labor=False,
+                      layer_dependency=False):
         """sample_neighborhood's batch as layer-wise bipartite blocks (an extension of the reference API); same arguments
         and the same node list and edges for the same key.  Integer fan-outs and device-resident seeds synchronise the
         host once per batch; a fan-out of None (every neighbour) adds one read-back for its hop.
@@ -826,13 +834,27 @@ class RandomNeighborSampler(_SamplerBase):
         never drawn, and fan-out None takes every entry as without weights.  A sampler built without edge_weight, and
         padding="head", raise ValueError; the first weighted call makes the positive degrees and reads back once more.
 
+        labor=True (layer-neighbour sampling, LABOR-0: Balin & Catalyurek, NeurIPS 2023; DGL's LaborSampler): every
+        integer fan-out k draws by the rule of include/tfgk.h ("LABOR block sampler").  Each source node c gets one
+        variate u_c per hop, and a row of d > k neighbours keeps its neighbour c iff u_c * d < k 2^32, so each row keeps
+        every neighbour with probability pi = ceil(k 2^32 / d) / 2^32 (k in expectation, up to d), the kept set is uniform
+        given its size, and rows that share a neighbour keep it together: a batch reaches fewer distinct source rows than
+        with independent draws.  A row of d <= k keeps every neighbour; a row of d > k keeps none with probability
+        (1 - pi)^d (over its distinct neighbours).  The mean and with_gcn_norm()'s n_g / k_r rescale stay unbiased given
+        k_r >= 1.  layer_dependency=True uses hop 0's variates at every hop, so a node drawn at one hop is preferred at the
+        next.  Fan-out None takes every neighbour as without LABOR.  padding (True or "head") and layer_dependency
+        without labor raise ValueError, weighted=True raises NotImplementedError, all before any device work.  No
+        capacity bounds a LABOR hop, so each one reads its edge total back and its block is planned as a fan-out None
+        block (a work-plan build, one more read-back): a batch of L integer LABOR hops synchronises 1 + 2 L times.
+
         :return: SampledBlocks, on the device"""
-        _check_weighted_padding(weighted, padding)
+        _check_rule(weighted, labor, layer_dependency, padding)
         csr, w_csr, rowptr, node_map = self._neighborhood_structure()
         pos_deg = self._positive_degrees() if weighted else None
         return _sample_blocks(lambda nodes, hop_fanouts, keys: ops.block_sample(
-            rowptr, csr.col, w_csr, nodes, hop_fanouts, keys, node_map, padding=padding, **_weighted_args(pos_deg)),
-            rowptr.device, node_map.numel(), seed_node_index, fanouts, seed, self._gcn_degrees, weighted)
+            rowptr, csr.col, w_csr, nodes, hop_fanouts, keys, node_map, padding=padding, **_rule_args(pos_deg, labor)),
+            rowptr.device, node_map.numel(), seed_node_index, fanouts, seed, self._gcn_degrees, weighted, labor,
+            layer_dependency)
 
     def row_block(self, r0, r1):
         return _row_block(self, r0, r1)
@@ -856,14 +878,14 @@ class RandomNeighborSampler(_SamplerBase):
 
     @_with_link_doc
     def sample_link_blocks(self, edge_index, fanouts, num_negatives=1, negative_edge_index=None, exclude=None,
-                           padding=False, seed=None, weighted=False):
-        _check_weighted_padding(weighted, padding)
+                           padding=False, seed=None, weighted=False, labor=False, layer_dependency=False):
+        _check_rule(weighted, labor, layer_dependency, padding)
         csr, w_csr, rowptr, node_map = self._neighborhood_structure()
         pos_deg = self._positive_degrees() if weighted else None
         return _sample_link_blocks(lambda pairs, n_pos, hop_fanouts, keys, exclude: ops.link_block_sample(
             rowptr, csr.col, w_csr, pairs, n_pos, hop_fanouts, keys, node_map, exclude=exclude, padding=padding,
-            **_weighted_args(pos_deg)), rowptr.device, node_map.numel(), edge_index, fanouts, num_negatives,
-            negative_edge_index, exclude, padding, seed, self._gcn_degrees, weighted)
+            **_rule_args(pos_deg, labor)), rowptr.device, node_map.numel(), edge_index, fanouts, num_negatives,
+            negative_edge_index, exclude, padding, seed, self._gcn_degrees, weighted, labor, layer_dependency)
 
 
 def _check_weighted_padding(weighted, padding):
@@ -877,46 +899,65 @@ def _check_weights(n_invalid):
                          "weights >= 0".format(n_invalid))
 
 
-def _weighted_args(pos_deg):
-    """The block samplers' keywords for a weighted batch (pos_deg not None) or an unweighted one."""
+def _check_rule(weighted, labor, layer_dependency, padding):
+    """The samplers' refusals of a draw rule, before any device work."""
+    _check_weighted_padding(weighted, padding)
+    if layer_dependency and not labor:
+        raise ValueError("layer_dependency=True reuses LABOR's variates across hops: it needs labor=True")
+    if labor and ops._padding_code(padding):
+        raise ValueError("labor=True draws without replacement: it takes no padding (True or 'head')")
+    if labor and weighted:
+        raise NotImplementedError("weighted LABOR is not implemented: it needs a per-row solve for the inclusion "
+                                  "probabilities")
+
+
+def _rule_args(pos_deg, labor=False):
+    """The block samplers' keywords for a weighted batch (pos_deg not None), a LABOR batch or a uniform one."""
+    if labor:
+        return dict(labor=True, rng_stream=ops.RNG_STREAM_LABOR)
     return {} if pos_deg is None else dict(pos_deg=pos_deg, rng_stream=ops.RNG_STREAM_WEIGHTED)
 
 
-def _hop_keys(fanouts, seed):
-    """(per-hop fan-outs in hop order, hop keys) of a batch with the resolved key `seed`."""
+def _hop_keys(fanouts, seed, layer_dependency=False):
+    """(per-hop fan-outs in hop order, hop keys) of a batch with the resolved key `seed`; with layer_dependency every
+    hop takes hop 0's key."""
     from .graph_utils import _batch_seed         # graph_utils imports this module
     hop_fanouts = [None if k is None else int(k) for k in reversed(list(fanouts))]
-    return hop_fanouts, [_batch_seed(seed, h) for h in range(len(hop_fanouts))]
+    return hop_fanouts, [_batch_seed(seed, 0 if layer_dependency else h) for h in range(len(hop_fanouts))]
 
 
-def _blocks_of(dev, node_index, sizes, hops, hop_fanouts, degrees, excluded=None, weighted=False):
-    """The Blocks of a batch, layer 0 first, from the block sampler's hops."""
+def _blocks_of(dev, node_index, sizes, hops, hop_fanouts, degrees, excluded=None, weighted=False, labor=False):
+    """The Blocks of a batch, layer 0 first, from the block sampler's hops.  A LABOR block's rows are not bounded by its
+    fan-out, so it is planned as a block of fan-out None."""
     blocks = []
     for h, (k, (out_rowptr, row, local, gcol, w)) in enumerate(zip(hop_fanouts, hops)):
         n_dst, n_src = sizes[h], sizes[h + 1]
         S = row.numel()
+        by_labor = labor and k is not None
         block_csr = ops.CSR(out_rowptr[:n_dst + 1], local, torch.arange(S, dtype=torch.int32, device=dev), n_dst, n_src)
-        if _plan_for_fanout(k):
+        if _plan_for_fanout(None if by_labor else k):
             block_csr.plan = ops.build_plan(block_csr)
         blocks.append(Block(n_src, n_dst, torch.stack([row, local]), w, gcol, block_csr, fanout=k,
-                            dst_ids=node_index[:n_dst], degrees=degrees, excluded=excluded, weighted=weighted))
+                            dst_ids=node_index[:n_dst], degrees=degrees, excluded=excluded, weighted=weighted,
+                            labor=by_labor))
     return blocks[::-1]
 
 
-def _sample_blocks(block_sample, dev, num_nodes, seed_node_index, fanouts, seed, degrees, weighted=False):
+def _sample_blocks(block_sample, dev, num_nodes, seed_node_index, fanouts, seed, degrees, weighted=False, labor=False,
+                   layer_dependency=False):
     """sample_blocks of both samplers around their block sampler: block_sample(seeds int32, per-hop fan-outs in hop order,
     hop keys) returns ops.block_sample's (nodes, hop_sizes, hops, n_bad, n_dup); this refuses bad seeds and assembles
     the SampledBlocks.  degrees: the sampler's (rowptr, row sums) handle that every Block keeps for with_gcn_norm()."""
     seed = _rng.resolve_host(seed)
     nodes = ops.as_device(seed_node_index, torch.int32, device=dev).reshape(-1).contiguous()
-    hop_fanouts, keys = _hop_keys(fanouts, seed)
+    hop_fanouts, keys = _hop_keys(fanouts, seed, layer_dependency)
     node_index, sizes, hops, n_bad, n_dup = block_sample(nodes, hop_fanouts, keys)
     if n_bad:
         raise ValueError("seed_node_index holds node ids outside [0, {})".format(num_nodes))
     if n_dup:
         raise ValueError("seed_node_index holds {} duplicate node ids".format(n_dup))
     return SampledBlocks(node_index, sizes, _blocks_of(dev, node_index, sizes, hops, hop_fanouts, degrees,
-                                                       weighted=weighted), num_nodes=num_nodes)
+                                                       weighted=weighted, labor=labor), num_nodes=num_nodes)
 
 
 class LinkBlocks(SampledBlocks):
@@ -963,7 +1004,7 @@ def _pair_tensor(pairs, dev, what):
 
 
 def _sample_link_blocks(link_block_sample, dev, num_nodes, edge_index, fanouts, num_negatives, negative_edge_index,
-                        exclude, padding, seed, degrees, weighted=False):
+                        exclude, padding, seed, degrees, weighted=False, labor=False, layer_dependency=False):
     """sample_link_blocks of both samplers around their link block sampler: link_block_sample(pairs int32 [2, P], n_pos,
     per-hop fan-outs, hop keys, exclude) returns ops.link_block_sample's outputs.  This checks the arguments, writes the
     pairs (positives, then negatives), refuses endpoints outside the graph and assembles the LinkBlocks."""
@@ -983,7 +1024,7 @@ def _sample_link_blocks(link_block_sample, dev, num_nodes, edge_index, fanouts, 
     if num_nodes == 0 and B + M:
         raise ValueError("the pairs hold node ids outside [0, 0): the graph has no nodes")
     seed = _rng.resolve_host(seed)
-    hop_fanouts, keys = _hop_keys(fanouts, seed)
+    hop_fanouts, keys = _hop_keys(fanouts, seed, layer_dependency)
     pairs = torch.empty((2, B + M), dtype=torch.int32, device=dev)
     pairs[:, :B].copy_(pos)
     if neg is not None:
@@ -993,7 +1034,7 @@ def _sample_link_blocks(link_block_sample, dev, num_nodes, edge_index, fanouts, 
     node_index, sizes, hops, n_bad, local, excluded = link_block_sample(pairs, B, hop_fanouts, keys, exclude)
     if n_bad:
         raise ValueError("the pairs hold {} node ids outside [0, {})".format(n_bad, num_nodes))
-    blocks = _blocks_of(dev, node_index, sizes, hops, hop_fanouts, degrees, excluded, weighted)
+    blocks = _blocks_of(dev, node_index, sizes, hops, hop_fanouts, degrees, excluded, weighted, labor)
     return LinkBlocks(node_index, sizes, blocks, num_nodes, local, B)
 
 
@@ -1292,31 +1333,35 @@ class HostNeighborSampler(object):
             self._pos_deg = pos_deg
         return self._pos_deg
 
-    def sample_blocks(self, seed_node_index, fanouts, padding=False, seed=None, weighted=False):
+    def sample_blocks(self, seed_node_index, fanouts, padding=False, seed=None, weighted=False, labor=False,
+                      layer_dependency=False):
         """RandomNeighborSampler.sample_blocks over the host CSR: same arguments, same batch for the same key (rows of
         the CSR are sampled in place over the host link).  A batch synchronises with the host once (plus one read-back
         per hop of fan-out None).  Calls on one sampler must be ordered on one CUDA stream.  weighted=True: as
-        RandomNeighborSampler's; every candidate's weight is read over the host link.
+        RandomNeighborSampler's; every candidate's weight is read over the host link.  labor=True, layer_dependency: as
+        RandomNeighborSampler's (1 + 2 L read-backs for L integer hops); the columns of every row of d > k cross the host
+        link twice, warp-wide, once to count and once to fill.
 
         :return: SampledBlocks, on the device"""
         self._check_open()
-        _check_weighted_padding(weighted, padding)
+        _check_rule(weighted, labor, layer_dependency, padding)
         pos_deg = self._positive_degrees() if weighted else None
         return _sample_blocks(lambda nodes, hop_fanouts, keys: ops.block_sample_mapped(
             self.rowptr, self._col_ptr, self._w_ptr, nodes, hop_fanouts, keys, self._node_map, padding=padding,
-            **_weighted_args(pos_deg)), self._device, self.num_nodes, seed_node_index, fanouts, seed, self._degrees,
-            weighted)
+            **_rule_args(pos_deg, labor)), self._device, self.num_nodes, seed_node_index, fanouts, seed, self._degrees,
+            weighted, labor, layer_dependency)
 
     @_with_link_doc
     def sample_link_blocks(self, edge_index, fanouts, num_negatives=1, negative_edge_index=None, exclude=None,
-                           padding=False, seed=None, weighted=False):
+                           padding=False, seed=None, weighted=False, labor=False, layer_dependency=False):
         self._check_open()
-        _check_weighted_padding(weighted, padding)
+        _check_rule(weighted, labor, layer_dependency, padding)
         pos_deg = self._positive_degrees() if weighted else None
         return _sample_link_blocks(lambda pairs, n_pos, hop_fanouts, keys, exclude: ops.link_block_sample_mapped(
             self.rowptr, self._col_ptr, self._w_ptr, pairs, n_pos, hop_fanouts, keys, self._node_map, exclude=exclude,
-            padding=padding, **_weighted_args(pos_deg)), self._device, self.num_nodes, edge_index, fanouts,
-            num_negatives, negative_edge_index, exclude, padding, seed, self._degrees, weighted)
+            padding=padding, **_rule_args(pos_deg, labor)), self._device, self.num_nodes, edge_index, fanouts,
+            num_negatives, negative_edge_index, exclude, padding, seed, self._degrees, weighted, labor,
+            layer_dependency)
 
     def row_block(self, r0, r1):
         self._check_open()
